@@ -2,7 +2,8 @@
 """bench.py -- headline benchmark: tracked points*frames / second, CoTracker3 offline predictor,
 synthetic 512x512x16 video, grid_size=80 (N=6400 tracks), 6 refinement iterations (BASELINE.json `metric`).
 
-    python bench.py --gpus 1 --steps 5 --warmup 3                 # this repo (libct3_b200.so on the B200)
+    python bench.py --gpus 1 --steps 5 --warmup 3                 # this repo (libct3_b200.so on the H100)
+    python bench.py --gpus 1 --steps 5 --warmup 3 --dump-outputs DIR   # + the last timed step's tracks/visibility as .npy
     python bench.py --impl reference --gpus 1 --steps 2 --warmup 1  # CPU arm: the UNMODIFIED reference on the host cores
     python bench.py --grid 30 | --frames 48 | --online --grid 50    # BASELINE.json configs C2 / C3 / C4
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
@@ -11,7 +12,7 @@ synthetic 512x512x16 video, grid_size=80 (N=6400 tracks), 6 refinement iteration
 One JSON line on stdout (rank 0).  A "step" = one CoTrackerPredictor.forward over one clip.
   value : whole-job points*frames/s with the clip resident in HBM when the timed region starts
   e2e   : same call with the clip in pinned HOST memory (H2D copy + D2H of tracks/visibility inside the region)
-  roofline     : dominant kernel (the tcgen05 split-bf16x3 GEMM) -- algorithmic FLOPs / live CUDA-event time
+  roofline     : dominant kernel (the wgmma split-bf16x3 GEMM) -- algorithmic FLOPs / live CUDA-event time
   roofline_corr: the fused sampling+correlation kernel against the HBM roofline (4.71 GB/iteration, SURVEY 8d)
   cpu_baseline : the reference's own PyTorch-CPU path on a bounded sample of the same workload (rank 0, N=1 only)
 
@@ -50,7 +51,8 @@ def peaks():
         with open(p) as f:
             d = json.load(f)
         return dict(hbm=d["hbm_gbs"], bf16=d["bf16_tflops_sustained"], bf16_burst=d["bf16_tflops"], source="measured")
-    return dict(hbm=6650.0, bf16=1400.0, bf16_burst=1590.0, source="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- upper bounds, not measured here
+    return dict(hbm=3350.0, bf16=989.0, bf16_burst=989.0, source="H100 SXM data sheet")
 
 
 
@@ -92,7 +94,7 @@ def reference_predictor(ref_dir, sd, online=False):
 
 
 def workload_config(T, G, world, online=False):
-    """`config` of the JSON line -- identical for the B200 arm and the CPU reference arm."""
+    """`config` of the JSON line -- identical for the GPU arm and the CPU reference arm."""
     N = G * G
     if online:
         w = (f"cotracker3_online predictor, synthetic {SIZE}x{SIZE} texture stream, window 16 / step 8, "
@@ -101,7 +103,7 @@ def workload_config(T, G, world, online=False):
         w = (f"cotracker3_offline predictor, synthetic {SIZE}x{SIZE}x{T} texture video, grid_size={G} "
              f"({N} tracks), 6 iters, one clip per GPU")
     return {"workload": w, "global_batch": world, "parallelism": f"replicas x{world} (no hot-loop collective)",
-            "l2": "no explicit flush: per-step working set of several GB >> 126 MB L2"}
+            "l2": "no explicit flush: per-step working set of several GB >> 50 MB L2"}
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -160,7 +162,7 @@ class ClockSampler:
 # ---------------------------------------------------------------------------------------------------
 def cpu_run(sd, video, G, online, ref_dir):
     """One timed CPU pass of the workload: the unmodified reference if present, else the oracle port.
-    Offline: one predictor call.  Online: is_first_step + one 16-frame chunk (the unit bench.py's B200 arm times)."""
+    Offline: one predictor call.  Online: is_first_step + one 16-frame chunk (the unit bench.py's GPU arm times)."""
     with torch.no_grad():
         if ref_dir:
             p = reference_predictor(ref_dir, sd, online)
@@ -184,7 +186,7 @@ def cpu_run(sd, video, G, online, ref_dir):
 
 def bench_reference(args, rank):
     """CPU arm: the reference's own PyTorch-CPU implementation on all usable host cores, on the SAME config as the
-    B200 arm (grid/frames as given; default = the headline shape).  One repetition takes 1-2 minutes there, so the
+    GPU arm (grid/frames as given; default = the headline shape).  One repetition takes 1-2 minutes there, so the
     warm-up runs at grid_size=10 and the timed repetitions are capped by a time budget; `steps` is what actually ran."""
     if rank != 0:
         return
@@ -221,6 +223,26 @@ def bench_reference(args, rank):
     print(json.dumps(line), flush=True)
 
 
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, outputs):
+    """The arrays a caller of the timed path receives from its last step (tracks, visibilities) as float32 .npy.
+    Above 64 MB in all, each array is replaced by a fixed seeded sample of its elements (flattened, same share of the
+    budget each): <name>.npy holds the sampled values and <name>_index.npy their flat indices (float64, exact)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {name: t.detach().float().cpu().numpy() for name, t in zip(("tracks", "visibility"), outputs)}
+    total = sum(a.nbytes for a in arrays.values())
+    for i, (name, a) in enumerate(arrays.items()):
+        if total > DUMP_BYTES:
+            k = DUMP_BYTES // (len(arrays) * 12)              # 4 B value + 8 B index per sampled element
+            idx = np.sort(np.random.default_rng(i).choice(a.size, size=min(k, a.size), replace=False))
+            np.save(os.path.join(out_dir, name + "_index.npy"), idx.astype(np.float64))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 # ---------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -234,7 +256,11 @@ def main():
     ap.add_argument("--online", action="store_true", help="BASELINE config C4: cotracker3_online, window 16 / step 8")
     ap.add_argument("--opt", action="append", default=[], metavar="NAME=VALUE",
                     help="library option for A/B runs, e.g. --opt fuse=1 --opt prec.fc1=2 (ct3_set_option)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the tracks and visibilities of the last timed step to DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
     rank = int(os.environ.get("RANK", "0"))
@@ -338,8 +364,10 @@ def main():
         run_resident()
     sampler = ClockSampler(local_rank)
     sampler.start()
-    ms_step, _ = timed(run_resident, args.steps)
+    ms_step, last = timed(run_resident, args.steps)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     for _ in range(1):
         run_e2e()
     ms_e2e, (tr, vis) = timed(run_e2e, args.steps)
@@ -356,14 +384,6 @@ def main():
     engine.profile_enable(False)
     pk = peaks()
     prec = engine.precision_summary()
-    traffic, traffic_src = {}, None
-    for name in ("r2_dram_traffic.json", "r1_dram_traffic.json"):   # ncu-measured DRAM bytes of one headline step
-        tp = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(tp) and T == T_FRAMES and G == GRID and not online:
-            with open(tp) as f:
-                traffic = json.load(f)
-            traffic_src = "profiles/" + name + " (ncu --set full capture of this command; NOT measured in this run)"
-            break
     gemm_tflops = gemm_flops / (cat_ms["gemm"] / 1e3) / 1e12 if cat_ms["gemm"] > 0 else 0.0
     # SURVEY 8d: pyramid read once (16320 texels/frame at the 384x512 model resolution) + support + coords + volume
     # write; the volume is written with `vol_bytes` bytes per element (4 = split bf16 hi|lo, 2 = single fp16 plane)
@@ -387,27 +407,22 @@ def main():
                 "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": tr.numel() * 4 + vis.numel()},
         "gpu_launches": int(sum(cat_n.values())),
         "clocks": clocks,
-        "roofline": {"kernel": "gemm_split3_pair_kernel / gemm_split3_tc_kernel (tcgen05, all linear layers)",
+        "roofline": {"kernel": "gemm_split3_tc_kernel (wgmma, all linear layers)",
                      "bound": "tensor", "achieved": gemm_tflops, "peak": pk["bf16"], "unit": "TFLOP/s",
                      "frac": gemm_tflops / pk["bf16"],
-                     "traffic": traffic.get("gemm", {}).get("dram_bytes_per_step"),
-                     "traffic_source": traffic_src,
                      "note": "algorithmic fp32-equivalent FLOPs (2*M*N*K per linear layer) / live CUDA-event time of "
-                             "the GEMM launches; products per FLOP: " + prec["products"] + "; peak = sustained cuBLAS "
+                             "the GEMM launches; products per FLOP: " + prec["products"] + "; peak = dense "
                              "bf16 (" + pk["source"] + ")",
                      "ms_per_step": cat_ms["gemm"], "launches_per_step": cat_n["gemm"]},
         "roofline_corr": {"kernel": "corr_patch_t_kernel (corr_tc3.cu; fused bilinear sampling + 4-D correlation)",
                           "bound": "hbm", "achieved": corr_gbs, "peak": pk["hbm"],
                           "unit": "GB/s", "frac": corr_gbs / pk["hbm"],
-                          "traffic": traffic.get("corr_sample", {}).get("dram_bytes_per_step"),
-                          "traffic_source": traffic_src,
                           "algorithmic_bytes_per_step": corr_bytes, "volume_bytes_per_element": vol_bytes,
                           "ms_per_step": cat_ms["corr_sample"], "launches_per_step": cat_n["corr_sample"]},
         "roofline_qkv_attention": {"kernel": "gemm_qkv_time_attn_kernel (q|k|v projection + per-track time attention, one "
                                              "kernel)", "bound": "tensor", "achieved": qkva_tflops, "peak": pk["bf16"],
                                    "unit": "TFLOP/s", "frac": qkva_tflops / pk["bf16"],
-                                   "note": "projection FLOPs only (the T x T attention runs as fp32 FMA in the epilogue); "
-                                           "ncu tensor-pipe active 52 % (profiles/r2_ncu_qkv_time_attn.txt)",
+                                   "note": "projection FLOPs only (the T x T attention runs as fp32 FMA in the epilogue)",
                                    "ms_per_step": cat_ms.get("qkv_time_attention", 0.0)},
         "kernel_ms_per_step": cat_ms, "library_ms_per_step": lib_ms,
     }

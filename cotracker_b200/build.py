@@ -12,7 +12,7 @@ from .model import CoTrackerThreeOffline, CoTrackerThreeOnline
 
 def build_cotracker(checkpoint=None, offline=True, window_len=16, v2=False):
     if v2:
-        raise NotImplementedError("CoTracker2 is not part of the B200 hot path (SURVEY.md §2, row 3b)")
+        raise NotImplementedError("CoTracker2 is not part of the H100 hot path (SURVEY.md §2, row 3b)")
     cls = CoTrackerThreeOffline if offline else CoTrackerThreeOnline
     cotracker = cls(stride=4, corr_radius=3, window_len=window_len)
     if checkpoint is not None:

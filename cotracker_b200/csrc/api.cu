@@ -20,13 +20,13 @@ thread_local char g_err[512] = "";
 // another thread's verification switches or profile records.
 struct OptDef { const char* name; int lo, hi; };
 enum { OPT_GEMM = 0, OPT_CORR, OPT_ATTN, OPT_PREC_CORR, OPT_PREC_FC1, OPT_FUSE, OPT_COUNT };
-constexpr int kDefPrecCorr = 2, kDefPrecFc1 = 3;   // chosen by measurement: profiles/r2_precision_sweep.txt
+constexpr int kDefPrecCorr = 2, kDefPrecFc1 = 3;   // DESIGN.md section 2
 constexpr OptDef kOptDefs[OPT_COUNT] = {
-    {"gemm", 0, 1},   // 0 tcgen05, 1 SIMT verification
-    {"corr", 0, 3},   // 0 tcgen05 correlate-then-interpolate (corr_tc3.cu / corr_tc2.cu), 1 exact-fp32 SIMT, 2 corr_tc.cu,
+    {"gemm", 0, 1},   // 0 wgmma, 1 SIMT verification
+    {"corr", 0, 3},   // 0 wgmma correlate-then-interpolate (corr_tc3.cu / corr_tc2.cu), 1 exact-fp32 SIMT, 2 corr_tc.cu,
                       // 3 correlate-then-interpolate with corr_tc2.cu for every precision mode (A/B)
-    {"attn", 0, 2},   // 0 tensor-core kernels (tcgen05 point<-virtual, mma.sync elsewhere), 1 exact-fp32 SIMT verification,
-                      // 2 = mma.sync for point<-virtual too (the kernel attention_p2v.cu replaced; A/B)
+    {"attn", 0, 2},   // 0 tensor-core kernels (wgmma point<-virtual, mma.sync elsewhere), 1 exact-fp32 SIMT verification,
+                      // 2 = mma.sync for point<-virtual too (A/B against attention_p2v.cu)
     // tensor-core products per FLOP of a GEMM group (DESIGN.md section 2): 3 = split x split (hi*hi + lo*hi + hi*lo),
     // 2 = fp16 activation plane x split fp16 weights, 1 = single fp16 product.  Only the correlation branch has the
     // switch: SURVEY 7.3 measured that every transformer GEMM breaks the 1e-3 px budget with fewer than 3 products.
@@ -58,13 +58,13 @@ int fail_cuda(cudaError_t e, const char* where) {
 int num_sms() {   // of the CURRENT device (one process may drive several GPUs)
   static std::atomic<int> cache[64] = {};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   if (dev >= 0 && dev < 64) {
     const int c = cache[dev].load(std::memory_order_relaxed);
     if (c > 0) return c;
   }
   int n = 0;
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   if (dev >= 0 && dev < 64) cache[dev].store(n, std::memory_order_relaxed);
   return n;
 }
@@ -296,7 +296,7 @@ struct Runner {
 
 int run_attention(Runner& R, const Workspace& W, const AttnParams& a, bool per_warp) {
   if (g_opt_attn == 1) return (int)launch_attention(a, R.s);
-  // point <- virtual (64 keys per frame, thousands of queries): tcgen05 kernel with TMA row staging (attention_p2v.cu)
+  // point <- virtual (64 keys per frame, thousands of queries): wgmma kernel with TMA row staging (attention_p2v.cu)
   if (g_opt_attn == 0 && !per_warp && a.Lq > kV && attention_p2v_supported(a)) return (int)launch_attention_p2v(a, R.s);
   return (int)launch_attention_tc(a, per_warp, W.att_part, num_sms(), R.s);
 }

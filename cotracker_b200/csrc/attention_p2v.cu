@@ -1,4 +1,4 @@
-// attention_p2v.cu -- point <- virtual cross attention on the 5th-gen tensor cores (tcgen05):
+// attention_p2v.cu -- point <- virtual cross attention on the Hopper tensor cores (wgmma):
 //     out[n, t, h*48 ..] = softmax( q_h[n,t] . K_h[t]^T * 48^-1/2 ) V_h[t]          over the 64 virtual tokens of frame t
 // (Attention.forward, blocks.py:379-398, called from CrossAttnBlock as space_point2virtual_blocks, cotracker.py:515-517).
 // One CTA = one frame t x 128 consecutive tracks; per head:
@@ -9,14 +9,15 @@
 //      as 128B-swizzled K-major operand tiles (q pre-multiplied by 48^-1/2 log2 e; head dim 48 zero-padded to the
 //      64-element swizzle row); V_h is written TRANSPOSED ([48 dims x 64 keys], K = keys) as the B operand of the
 //      second product
-//   2. S = Q K^T : tcgen05.mma M=128, N=64, 3 k16 steps x 3 split products -> TMEM
-//   3. softmax on the thread's own row (TMEM lane = query row: 64 scores in registers, exp2), P normalised, split,
-//      written over the Q tiles as the K-major A tile of the second product (64 keys = exactly one 128-byte row)
-//   4. O = P V : M=128, N=48, 4 k16 steps x 3 split products -> TMEM -> registers -> split bf16 rows staged in shared
-//      memory -> two 3-D TMA stores (hi plane, lo plane) into the out-projection's operand buffer
+//   2. S = Q K^T : the CTA is one warpgroup; wgmma m64n64k16 on both 64-row halves, 3 k16 steps x 3 split products,
+//      fp32 scores in registers (a query row's 64 scores are spread over the 4 lanes of a quad)
+//   3. softmax per row in registers (max and sum over the quad by two shuffles, exp2), P normalised, split, written
+//      over the Q tiles as the K-major A tile of the second product (64 keys = exactly one 128-byte row)
+//   4. O = P V : wgmma m64n48k16 on both halves, 4 k16 steps x 3 split products -> registers -> split bf16 rows staged
+//      in shared memory -> two 3-D TMA stores (hi plane, lo plane) into the out-projection's operand buffer
 // A first version with one global load / store stream per thread (= per row, rows T*ld*4 bytes apart) was bound by the
 // LSU request rate (252 us per call at N=6400, T=16; long_scoreboard 5.6 per issue); TMA moves whole rows instead.
-// Two CTAs are resident per SM (113 KiB of shared memory each = the 228 KiB of the SM exactly; 128 TMEM columns each).
+// Two CTAs are resident per SM (113 KiB of shared memory each = the 228 KiB of the SM exactly).
 #include "gemm.cuh"
 #include "kernels.cuh"
 
@@ -51,9 +52,6 @@ attn_p2v_tc_kernel(const __grid_constant__ P2vMaps maps, AttnParams p, int tiles
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_align1024(smem_raw);
   uint64_t* bar_ld = reinterpret_cast<uint64_t*>(smem + PV_OFF_BAR);
-  uint64_t* bar_s = bar_ld + 1;
-  uint64_t* bar_o = bar_ld + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_ld + 3);
   const int r = threadIdx.x, warp = r >> 5, lane = r & 31;
   const int t = blockIdx.x / tiles_per_seq, n0 = (blockIdx.x % tiles_per_seq) * 128;
 
@@ -66,19 +64,12 @@ attn_p2v_tc_kernel(const __grid_constant__ P2vMaps maps, AttnParams p, int tiles
     tma_prefetch_desc(&maps.kv);
     tma_prefetch_desc(&maps.out);
     mbar_init(bar_ld, 1);
-    mbar_init(bar_s, 1);
-    mbar_init(bar_o, 1);
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc(tmem_slot, 128);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t t_s = tmem_base + ((uint32_t)(warp * 32) << 16);         // S: columns 0..63
-  const uint32_t t_o = t_s + 64;                                          // O: columns 64..111
   const float qscale = p.scale * 1.44269504088896340736f;
-  constexpr uint32_t idesc_s = umma_idesc_bf16(128, 64), idesc_o = umma_idesc_bf16(128, 48);
+  // wgmma fragment rows of this thread: half hh, rows 64hh + rq and 64hh + rq + 8; columns 8j + cq, 8j + cq + 1
+  const int rq = 16 * warp + (lane >> 2), cq = 2 * (lane & 3);
   const uint32_t sQ = smem_u32(smem + PV_OFF_Q), sK = smem_u32(smem + PV_OFF_K), sV = smem_u32(smem + PV_OFF_V);
   // key / value conversion: this thread's key and the first of its six 4-float chunks (rotated by the lane so that the
   // 192-byte staging rows are read, and the transposed V rows written, without bank conflicts)
@@ -143,83 +134,94 @@ attn_p2v_tc_kernel(const __grid_constant__ P2vMaps maps, AttnParams p, int tiles
     fence_proxy_async_smem();
     __syncthreads();                               // tiles complete; staging consumed
     if (r == 0 && h + 1 < kHeads) issue_loads(h + 1);   // next head's rows arrive while this head computes
-    // ---- 2. S = Q K^T
-    if (warp == 0 && elect_one()) {
-      tc_fence_after_sync();
+    // ---- 2. S = Q K^T (both 64-row halves; q already carries the softmax scale and log2 e)
+    float s0[32], s1[32];
+    wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < kDh / 16; ++kk) {
-        const uint32_t ko = kk * 32;
-        const uint64_t qh = umma_desc_sw128(sQ + ko), ql = umma_desc_sw128(sQ + PV_TILE_Q + ko);
-        const uint64_t kh = umma_desc_sw128(sK + ko), kl = umma_desc_sw128(sK + PV_TILE_K + ko);
-        umma_bf16(tmem_base, ql, kh, idesc_s, kk != 0 ? 1u : 0u);
-        umma_bf16(tmem_base, qh, kl, idesc_s, 1u);
-        umma_bf16(tmem_base, qh, kh, idesc_s, 1u);
-      }
-      umma_commit(bar_s);
+    for (int kk = 0; kk < kDh / 16; ++kk) {
+      const uint32_t ko = kk * 32;
+      const uint64_t kh = gmma_desc_sw128(sK + ko), kl = gmma_desc_sw128(sK + PV_TILE_K + ko);
+      const uint32_t first = kk != 0 ? 1u : 0u;
+      wgmma_tile<64, false>(s0, gmma_desc_sw128(sQ + PV_TILE_Q + ko), kh, first);
+      wgmma_tile<64, false>(s0, gmma_desc_sw128(sQ + ko), kl, 1u);
+      wgmma_tile<64, false>(s0, gmma_desc_sw128(sQ + ko), kh, 1u);
+      wgmma_tile<64, false>(s1, gmma_desc_sw128(sQ + 8192 + PV_TILE_Q + ko), kh, first);
+      wgmma_tile<64, false>(s1, gmma_desc_sw128(sQ + 8192 + ko), kl, 1u);
+      wgmma_tile<64, false>(s1, gmma_desc_sw128(sQ + 8192 + ko), kh, 1u);
     }
-    mbar_wait(bar_s, ph);
-    tc_fence_after_sync();
-    // ---- 3. softmax of this thread's row -> normalised P (split) over the Q tiles = A tile of the second product
-    {
-      float s[64];
-      tmem_ld64(t_s, s);
-      float m = s[0];
+    wgmma_commit();
+    wgmma_wait0(s0);
+    wgmma_wait0(s1);
+    __syncthreads();                               // every warp's MMAs have read the Q tiles: P may overwrite them
+    // ---- 3. softmax of each row (4 lanes of a quad x 16 scores) -> normalised P (split) over the Q tiles
 #pragma unroll
-      for (int i = 1; i < 64; ++i) m = fmaxf(m, s[i]);
-      float l = 0.f;
+    for (int hh = 0; hh < 2; ++hh) {
+      float (&sc)[32] = hh ? s1 : s0;
 #pragma unroll
-      for (int i = 0; i < 64; ++i) { s[i] = exp2f(s[i] - m); l += s[i]; }
-      const float inv = 1.0f / l;
+      for (int rr = 0; rr < 2; ++rr) {             // fragment elements 4j + 2rr + {0,1}: row 64hh + rq + 8rr
+        float m = -INFINITY;
 #pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        uint32_t hh[4], ll[4];
+        for (int j = 0; j < 8; ++j) m = fmaxf(m, fmaxf(sc[4 * j + 2 * rr], sc[4 * j + 2 * rr + 1]));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+        float l = 0.f;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) split2(s[8 * c + 2 * j] * inv, s[8 * c + 2 * j + 1] * inv, hh[j], ll[j]);
-        *reinterpret_cast<uint4*>(smem + PV_OFF_Q + swz(r, c)) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
-        *reinterpret_cast<uint4*>(smem + PV_OFF_Q + PV_TILE_Q + swz(r, c)) = make_uint4(ll[0], ll[1], ll[2], ll[3]);
+        for (int j = 0; j < 8; ++j) {
+          sc[4 * j + 2 * rr] = exp2f(sc[4 * j + 2 * rr] - m);
+          sc[4 * j + 2 * rr + 1] = exp2f(sc[4 * j + 2 * rr + 1] - m);
+          l += sc[4 * j + 2 * rr] + sc[4 * j + 2 * rr + 1];
+        }
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const float inv = 1.0f / l;
+        const int row = 64 * hh + rq + 8 * rr;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          uint32_t ph, pl;
+          split2(sc[4 * j + 2 * rr] * inv, sc[4 * j + 2 * rr + 1] * inv, ph, pl);
+          const uint32_t off = swz(row, j) + (uint32_t)(cq * 2);
+          *reinterpret_cast<uint32_t*>(smem + PV_OFF_Q + off) = ph;
+          *reinterpret_cast<uint32_t*>(smem + PV_OFF_Q + PV_TILE_Q + off) = pl;
+        }
       }
     }
-    tc_fence_before_sync();
     fence_proxy_async_smem();
     __syncthreads();
     // ---- 4. O = P V
-    if (warp == 0 && elect_one()) {
-      tc_fence_after_sync();
+    float o0[24], o1[24];
+    wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        const uint32_t ko = kk * 32;
-        const uint64_t phd = umma_desc_sw128(sQ + ko), pld = umma_desc_sw128(sQ + PV_TILE_Q + ko);
-        const uint64_t vh = umma_desc_sw128(sV + ko), vl = umma_desc_sw128(sV + PV_TILE_K + ko);
-        umma_bf16(tmem_base + 64, pld, vh, idesc_o, kk != 0 ? 1u : 0u);
-        umma_bf16(tmem_base + 64, phd, vl, idesc_o, 1u);
-        umma_bf16(tmem_base + 64, phd, vh, idesc_o, 1u);
-      }
-      umma_commit(bar_o);
+    for (int kk = 0; kk < 4; ++kk) {
+      const uint32_t ko = kk * 32;
+      const uint64_t vh = gmma_desc_sw128(sV + ko), vl = gmma_desc_sw128(sV + PV_TILE_K + ko);
+      const uint32_t first = kk != 0 ? 1u : 0u;
+      wgmma_tile<48, false>(o0, gmma_desc_sw128(sQ + PV_TILE_Q + ko), vh, first);
+      wgmma_tile<48, false>(o0, gmma_desc_sw128(sQ + ko), vl, 1u);
+      wgmma_tile<48, false>(o0, gmma_desc_sw128(sQ + ko), vh, 1u);
+      wgmma_tile<48, false>(o1, gmma_desc_sw128(sQ + 8192 + PV_TILE_Q + ko), vh, first);
+      wgmma_tile<48, false>(o1, gmma_desc_sw128(sQ + 8192 + ko), vl, 1u);
+      wgmma_tile<48, false>(o1, gmma_desc_sw128(sQ + 8192 + ko), vh, 1u);
     }
-    mbar_wait(bar_o, ph);
-    tc_fence_after_sync();
-    {
-      // the P tiles are dead: stage the 128 x 48 output rows there (hi plane | lo plane, dense 96-byte rows)
-      float o[kDh];
+    wgmma_commit();
+    wgmma_wait0(o0);
+    wgmma_wait0(o1);
+    __syncthreads();                               // the P tiles are dead: stage the 128 x 48 output rows there
 #pragma unroll
-      for (int c = 0; c < kDh / 16; ++c) {
-        float v[16];
-        tmem_ld16(t_o + 16 * c, v);
+    for (int hh = 0; hh < 2; ++hh) {
+      const float (&oc)[24] = hh ? o1 : o0;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) o[16 * c + j] = v[j];
-      }
-      uint4* oh = reinterpret_cast<uint4*>(smem + PV_OFF_Q + r * (kDh * 2));
-      uint4* ol = reinterpret_cast<uint4*>(smem + PV_OFF_Q + PV_TILE_Q + r * (kDh * 2));
+      for (int rr = 0; rr < 2; ++rr) {
+        const int row = 64 * hh + rq + 8 * rr;
 #pragma unroll
-      for (int c = 0; c < kDh / 8; ++c) {
-        uint32_t hh[4], ll[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) split2(o[8 * c + 2 * j], o[8 * c + 2 * j + 1], hh[j], ll[j]);
-        oh[c] = make_uint4(hh[0], hh[1], hh[2], hh[3]);
-        ol[c] = make_uint4(ll[0], ll[1], ll[2], ll[3]);
+        for (int j = 0; j < 6; ++j) {
+          uint32_t oh, ol;
+          split2(oc[4 * j + 2 * rr], oc[4 * j + 2 * rr + 1], oh, ol);
+          const int off = row * (kDh * 2) + (8 * j + cq) * 2;   // dense 96-byte rows: hi plane | lo plane
+          *reinterpret_cast<uint32_t*>(smem + PV_OFF_Q + off) = oh;
+          *reinterpret_cast<uint32_t*>(smem + PV_OFF_Q + PV_TILE_Q + off) = ol;
+        }
       }
     }
-    tc_fence_before_sync();
     fence_proxy_async_smem();
     __syncthreads();
     if (r == 0) {
@@ -231,7 +233,6 @@ attn_p2v_tc_kernel(const __grid_constant__ P2vMaps maps, AttnParams p, int tiles
     __syncthreads();
   }
   if (r == 0) bulk_wait0();
-  if (warp == 0) tmem_dealloc(tmem_base, 128);
 }
 
 }  // namespace

@@ -5,9 +5,9 @@
 //
 // Flash-style: one warp owns a 16-query tile; keys stream through shared memory in chunks of KB; scores and
 // P*V run on the tensor cores as m16n8k16 bf16 MMAs with every operand split hi+lo (3 MMAs per product:
-// lo*hi + hi*lo + hi*hi, fp32 accumulate) -- the same 2^-17 product precision as the tcgen05 linear layers;
+// lo*hi + hi*lo + hi*hi, fp32 accumulate) -- the same 2^-17 product precision as the wgmma linear layers;
 // max / exp / sum are fp32 on the accumulator fragments (online softmax).  Attention is ~2 % of a block's
-// FLOPs and its tiles are 16 x 48: warp-level mma.sync is the right granularity here (a 128-row tcgen05 tile
+// FLOPs and its tiles are 16 x 48: warp-level mma.sync is the right granularity here (a 64-row wgmma tile
 // would idle 7/8 of the array for the T=16 time attention), the 128-wide contractions live in gemm.cu.
 //
 // Modes:  PER_WARP  = each warp has its own (sequence, head, q-tile) and its own K/V smem slice (time attention)

@@ -1,4 +1,4 @@
-// corr_tc.cu -- fused bilinear sampling + 4-D correlation on the 5th-gen tensor cores (the production path of
+// corr_tc.cu -- fused bilinear sampling + 4-D correlation on the Hopper tensor cores (the production path of
 // launch_corr_sample; corr.cu keeps the exact-fp32 SIMT version the tests cross-check against).
 //
 //   vol[(n,t,l)][(a*7+b)*49 + (i*7+j)] = < bilinear(F_l[t], cx/2^l + a-3, cy/2^l + b-3) , S_l[n, i*7+j, :] >
@@ -6,17 +6,18 @@
 //
 // Persistent, warp-specialised; work unit = (track n, level l), tile = two frames of that unit:
 //   patches : the 8x8-texel neighbourhood of a (t,n,l) is ONE 4-D TMA box load (128 ch x 8 x 8 x 1 frame = 32 KiB,
-//             origin clamped into the map) from the channels-last pyramid into a 3-slot shared-memory ring; every
+//             origin clamped into the map) from the channels-last pyramid into a 2-slot shared-memory ring; every
 //             texel crosses L2->SM once (64 instead of 112 line reads per frame) and no warp waits on a gather
 //   A tile  [128 x 128] : rows f*49 + a*7 + b (98 used) = the 49 sampled feature vectors of 2 frames, blended from
 //             the staged patch (separable 4-tap, border clamp per sample) and stored split-bf16 in the
 //             128B-swizzled K-major layout
 //   B tile  [ 64 x 128] : the 49 support vectors of (n,l) (rows 49..63 zero), split-bf16, built once per unit
-//   D       [128 x  64] : fp32 in TMEM, 3 tcgen05.mma per k16 step (lo*hi + hi*lo + hi*hi), double buffered
-//   epilogue            : tcgen05.ld -> split-bf16 -> byte image of the complete 9728-byte volume rows
+//   D       [128 x  64] : fp32, 3 wgmma per k16 step (lo*hi + hi*lo + hi*hi) by the epilogue warpgroup, handed to
+//                         its row-per-thread epilogue through shared memory
+//   epilogue            : accumulator row -> split-bf16 -> byte image of the complete 9728-byte volume rows
 //                         ([hi(2432) | lo(2432)], K padding zero) -> fully coalesced 16-byte stores
-// Warps: 0..13 samplers (warp w: frame w/7 of the tile, x-offset a = w%7), 14 MMA issuer (+TMEM alloc), 15 TMA
-// issuer, 16..19 epilogue.  Neither the sampled features (10 GB/iteration in the reference) nor an fp32 volume
+// Warps: 0..13 samplers (warp w: frame w/7 of the tile, x-offset a = w%7), 14 idle, 15 TMA issuer, 16..19 MMA +
+// epilogue warpgroup.  Neither the sampled features (10 GB/iteration in the reference) nor an fp32 volume
 // ever touch HBM.
 #include "gemm.cuh"
 #include "kernels.cuh"
@@ -25,16 +26,15 @@ namespace ct3 {
 namespace {
 
 constexpr int PW = 14;                    // sampler warps
-constexpr int MMA_WARP = 14;
-constexpr int TMA_WARP = 15;
-constexpr int EPI_WARP0 = 16;             // warps 16..19 -> TMEM lane quarters 0..3
+constexpr int TMA_WARP = 15;              // warp 14 idle
+constexpr int EPI_WARP0 = 16;             // warps 16..19: one warpgroup, MMA (wgmma) + epilogue
 constexpr int THREADS = 20 * 32;
 constexpr int A_PART = 2 * 16384;         // one bf16 plane of A: 2 K-atoms x [128 rows x 128 B]
 constexpr int A_BYTES = 2 * A_PART;       // hi + lo = 64 KiB
 constexpr int S_PART = 2 * 8192;          // one plane of S: 2 K-atoms x [64 rows x 128 B]
 constexpr int S_BYTES = 2 * S_PART;       // 32 KiB
 constexpr int PATCH_BYTES = 8 * 8 * kD * 4;  // 32 KiB
-constexpr int NPATCH = 3;
+constexpr int NPATCH = 2;
 constexpr int ROW_BYTES = 2 * kVolPad * 2;   // 9728: one volume row image [hi | lo]
 constexpr int STG_BYTES = 2 * ROW_BYTES;     // two frames per tile
 constexpr int OFF_S = 0;
@@ -42,10 +42,11 @@ constexpr int OFF_A = OFF_S + S_BYTES;
 constexpr int OFF_PATCH = OFF_A + A_BYTES;
 constexpr int OFF_STG = OFF_PATCH + NPATCH * PATCH_BYTES;
 constexpr int OFF_PARAM = OFF_STG + STG_BYTES;      // NPATCH x {cx, cy, box_x, box_y}
-constexpr int OFF_BAR = OFF_PARAM + NPATCH * 16;
+constexpr int ACC_LD = 64 + 4;            // accumulator tile [128 rows][ACC_LD] fp32 (MMA registers -> row per thread)
+constexpr int OFF_ACC = OFF_PARAM + NPATCH * 16;
+constexpr int OFF_BAR = OFF_ACC + 128 * ACC_LD * 4;
 constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
 static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-constexpr uint32_t TMEM_COLS = 128;       // 2 accumulators x 64 columns
 
 struct CorrTcArgs {
   const float* pyr;
@@ -95,14 +96,12 @@ corr_sample_tc_kernel(const __grid_constant__ CorrTcArgs g, const __grid_constan
   uint8_t* smem = smem_align1024(smem_raw);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* a_full = bars;          // samplers -> MMA            (count 14)
-  uint64_t* a_empty = bars + 1;     // MMA -> samplers            (tcgen05.commit)
-  uint64_t* d_full = bars + 2;      // [2] MMA -> epilogue        (tcgen05.commit)
-  uint64_t* d_empty = bars + 4;     // [2] epilogue -> MMA        (count 4)
-  uint64_t* s_full = bars + 6;      // samplers -> MMA, per unit  (count 14)
-  uint64_t* s_empty = bars + 7;     // MMA -> samplers, per unit  (tcgen05.commit)
-  uint64_t* p_full = bars + 8;      // [3] TMA -> samplers        (count 1 + tx bytes)
-  uint64_t* p_empty = bars + 11;    // [3] samplers -> TMA        (count 7)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 14);
+  uint64_t* a_empty = bars + 1;     // MMA -> samplers            (one arrive per MMA warp)
+  uint64_t* s_full = bars + 2;      // samplers -> MMA, per unit  (count 14)
+  uint64_t* s_empty = bars + 3;     // MMA -> samplers, per unit  (one arrive per MMA warp)
+  uint64_t* p_full = bars + 4;      // [NPATCH] TMA -> samplers   (count 1 + tx bytes)
+  uint64_t* p_empty = bars + 4 + NPATCH;   // [NPATCH] samplers -> TMA  (count 7)
+  float* acc_tile = reinterpret_cast<float*>(smem + OFF_ACC);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_per_unit = (g.T + 1) / 2;
@@ -113,19 +112,14 @@ corr_sample_tc_kernel(const __grid_constant__ CorrTcArgs g, const __grid_constan
   fence_proxy_async_smem();
   if (threadIdx.x == 0) {
     mbar_init(a_full, PW);
-    mbar_init(a_empty, 1);
-    for (int i = 0; i < 2; ++i) { mbar_init(&d_full[i], 1); mbar_init(&d_empty[i], 4); }
+    mbar_init(a_empty, 4);
     mbar_init(s_full, PW);
-    mbar_init(s_empty, 1);
+    mbar_init(s_empty, 4);
     for (int i = 0; i < NPATCH; ++i) { mbar_init(&p_full[i], 1); mbar_init(&p_empty[i], 7); }
     fence_barrier_init();
     for (int l = 0; l < kL; ++l) tma_prefetch_desc(&maps.m[l]);
   }
-  if (warp == MMA_WARP) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < PW) {
     // ================================================================== samplers
@@ -265,63 +259,63 @@ corr_sample_tc_kernel(const __grid_constant__ CorrTcArgs g, const __grid_constan
         __syncwarp();
       }
     }
-  } else if (warp == MMA_WARP) {
-    // ================================================================== MMA issuer
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(128, 64);
-      uint32_t it = 0, ui = 0;
-      const uint32_t s_base = smem_u32(smem + OFF_S);
-      const uint32_t a_base = smem_u32(smem + OFF_A);
-      for (int u = blockIdx.x; u < num_units; u += gridDim.x, ++ui) {
-        mbar_wait(s_full, ui & 1u);
-        for (int tp = 0; tp < tiles_per_unit; ++tp, ++it) {
-          const int acc = it & 1;
-          mbar_wait(a_full, it & 1u);
-          mbar_wait(&d_empty[acc], ((it >> 1) & 1u) ^ 1u);
-          tc_fence_after_sync();
-          const uint32_t d_tmem = tmem_base + (uint32_t)(acc * 64);
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks) {
-            const uint32_t ao = (uint32_t)((ks >> 2) * 16384 + (ks & 3) * 32);
-            const uint32_t so = (uint32_t)((ks >> 2) * 8192 + (ks & 3) * 32);
-            const uint64_t dah = umma_desc_sw128(a_base + ao), dal = umma_desc_sw128(a_base + A_PART + ao);
-            const uint64_t dsh = umma_desc_sw128(s_base + so), dsl = umma_desc_sw128(s_base + S_PART + so);
-            umma_bf16(d_tmem, dal, dsh, idesc, ks != 0 ? 1u : 0u);
-            umma_bf16(d_tmem, dah, dsl, idesc, 1u);
-            umma_bf16(d_tmem, dah, dsh, idesc, 1u);
-          }
-          umma_commit(a_empty);
-          umma_commit(&d_full[acc]);
-        }
-        umma_commit(s_empty);
-      }
-    }
-  } else {
-    // ================================================================== epilogue
-    const int q = warp & 3;              // TMEM lane quarter
+  } else if (warp >= EPI_WARP0) {
+    // ================================================================== MMA (wgmma) + epilogue warpgroup
+    const int q = warp & 3;              // row quarter
     const int r = q * 32 + lane;         // D row
     const int f = r >= kP ? 1 : 0;
     const int rho = r - f * kP;          // a*7+b
     const int et = threadIdx.x - EPI_WARP0 * 32;  // 0..127
     uint8_t* stg = smem + OFF_STG;
-    uint32_t it = 0;
-    for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
+    const uint32_t s_base = smem_u32(smem + OFF_S);
+    const uint32_t a_base = smem_u32(smem + OFF_A);
+    uint32_t it = 0, ui = 0;
+    for (int u = blockIdx.x; u < num_units; u += gridDim.x, ++ui) {
       const int n = u / kL, l = u % kL;
+      mbar_wait(s_full, ui & 1u);
       for (int tp = 0; tp < tiles_per_unit; ++tp, ++it) {
-        const int acc = it & 1;
-        mbar_wait(&d_full[acc], (it >> 1) & 1u);
-        tc_fence_after_sync();
+        mbar_wait(a_full, it & 1u);
+        float d0[32], d1[32];   // D rows 0..63 / 64..127 (samples) x 64 columns (support rows)
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks) {
+          const uint32_t ao = (uint32_t)((ks >> 2) * 16384 + (ks & 3) * 32);
+          const uint32_t so = (uint32_t)((ks >> 2) * 8192 + (ks & 3) * 32);
+          const uint64_t dsh = gmma_desc_sw128(s_base + so), dsl = gmma_desc_sw128(s_base + S_PART + so);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t ah = (uint32_t)(h * 8192);   // rows 64..127 of the A atom
+            const uint64_t dah = gmma_desc_sw128(a_base + ao + ah), dal = gmma_desc_sw128(a_base + A_PART + ao + ah);
+            if (h == 0) {
+              wgmma_tile<64, false>(d0, dal, dsh, ks != 0 ? 1u : 0u);
+              wgmma_tile<64, false>(d0, dah, dsl, 1u);
+              wgmma_tile<64, false>(d0, dah, dsh, 1u);
+            } else {
+              wgmma_tile<64, false>(d1, dal, dsh, ks != 0 ? 1u : 0u);
+              wgmma_tile<64, false>(d1, dah, dsl, 1u);
+              wgmma_tile<64, false>(d1, dah, dsh, 1u);
+            }
+          }
+        }
+        wgmma_commit();
+        wgmma_wait0(d0);
+        wgmma_wait0(d1);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(a_empty);     // A may be rewritten by the samplers
+        acc_store<64>(d0, acc_tile, ACC_LD);
+        acc_store<64>(d1, acc_tile + 64 * ACC_LD, ACC_LD);
+        asm volatile("bar.sync 1, 128;" ::: "memory");   // the whole tile is in shared memory
         const bool row_ok = r < 2 * kP && (2 * tp + f) < g.T;
         __nv_bfloat16* dst_hi = reinterpret_cast<__nv_bfloat16*>(stg + f * ROW_BYTES) + rho * kP;
         __nv_bfloat16* dst_lo = dst_hi + kVolPad;
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * 64);
+        const float* arow = acc_tile + r * ACC_LD;
         // 49 bf16 per plane at element offset rho*49 of the row image: one 2-byte edge element (first column
-        // if that offset is odd, else the last) + 24 aligned 4-byte pairs, in two TMEM loads of 32 columns
+        // if that offset is odd, else the last) + 24 aligned 4-byte pairs, in two loads of 32 columns
         const bool odd = (rho & 1) != 0;
         uint32_t* ph = reinterpret_cast<uint32_t*>(dst_hi + (odd ? 1 : 0));
         uint32_t* pl = reinterpret_cast<uint32_t*>(dst_lo + (odd ? 1 : 0));
         float v[32];
-        tmem_ld32(taddr, v);                       // columns 0..31
+        acc_row_ld<32>(arow, v);                   // columns 0..31
         const float carry = v[31];
         if (row_ok) {
           if (odd) {
@@ -343,10 +337,7 @@ corr_sample_tc_kernel(const __grid_constant__ CorrTcArgs g, const __grid_constan
             pl[15] = lo;
           }
         }
-        tmem_ld32(taddr + 32, v);                  // columns 32..63 (32..48 used)
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&d_empty[acc]);  // accumulator drained (registers hold the rest)
+        acc_row_ld<32>(arow + 32, v);              // columns 32..63 (32..48 used)
         if (row_ok) {
           if (odd) {
             uint32_t hi, lo;
@@ -377,14 +368,12 @@ corr_sample_tc_kernel(const __grid_constant__ CorrTcArgs g, const __grid_constan
             grow[w16] = reinterpret_cast<const uint4*>(stg + ff * ROW_BYTES)[w16];
           }
         }
-        asm volatile("bar.sync 1, 128;" ::: "memory");   // image may be overwritten by the next tile
+        asm volatile("bar.sync 1, 128;" ::: "memory");   // image and accumulator tile may be overwritten by the next tile
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(s_empty);       // this warp's MMAs of the unit have all completed
     }
   }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == MMA_WARP) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 }  // namespace

@@ -13,25 +13,22 @@
 //
 //   pyramid : a split-bf16 copy [level][plane hi|lo][T][H][W][128] made once per update-loop call
 //   A tile  [128 x 128] : rows f*64 + y*8 + x = the raw texels of 2 frames; each (frame, plane, K-half) is ONE 4-D
-//             TMA box (64 ch x 8 x 8 x 1) landing directly in the 128B-swizzled K-major operand layout; the ring
-//             holds 4 K-half slots (32 KiB: hi|lo x 2 frames), each freed as soon as its 8 MMAs retire
+//             TMA box (64 ch x 8 x 8 x 1) landing directly in the 128B-swizzled K-major operand layout; the 64 KiB ring
+//             is split between the two groups (each owns the slots of its own tiles), each slot freed as soon as the
+//             MMAs reading it have completed
 //   B tile  [128 x 128] : rows 0..63 hi plane / 64..127 lo plane of the 49 support vectors of (n,l) (rows 49..63
 //             of each plane zero), built once per unit by 2 warps
-//   D       [128 x 128] : fp32 in TMEM, 2 tcgen05.mma per k16 step: A_hi x [S_hi ; S_lo] (N=128, A_hi fetched once
-//             for both products) and A_lo x S_hi (N=64); the epilogue adds columns k and 64+k; 4 accumulators, so
-//             the MMA issuer runs up to 4 tiles ahead of the epilogue
-//   epilogue (2 groups x 4 warps, alternating tiles): tcgen05.ld (accumulator handed back at once) -> x-blend by
-//             warp shuffles inside each 8-texel row -> y-blend: interior tiles entirely in registers (next texel row = 8 lanes up, texel row 4 crosses
-//             the warp boundary through a 3 KiB exchange buffer); tiles with a border clamp through a shared
-//             [row][a][k] buffer and a per-row tap table -> one thread per volume row ->
-//             split-bf16 byte image of the two 9728-byte volume rows (reusing the blend buffer, K padding zero)
-//             -> one bulk shared->global copy (TMA engine) per 9728-byte volume row
-// Warps: 0 TMA issuer, 1 MMA issuer (+TMEM alloc), 2..3 support builders, 4..11 epilogue.
+//   D       [128 x 128] : fp32 wgmma accumulators of the group that owns the tile: A_hi x [S_hi ; S_lo] (N=128, A_hi
+//             fetched once for both products) and A_lo x S_hi (N=64 into columns 0..63); columns k and 64+k are added
+//             in registers and the [128 x 64] sum goes to the group's accumulator tile in shared memory
+//   epilogue (2 groups x 4 warps = 2 warpgroups, alternating tiles; each runs the MMAs of its own tiles) ->
+//             x-blend by warp shuffles inside each 8-texel row -> y-blend: interior tiles entirely in registers (next
+//             texel row = 8 lanes up, texel row 4 crosses the warp boundary through a 3 KiB exchange buffer); tiles
+//             with a border clamp through a shared [row][a][k] buffer and a per-row tap table -> one thread per
+//             volume row -> split-bf16 byte image of the two 9728-byte volume rows (reusing the blend buffer, K
+//             padding zero) -> one bulk shared->global copy (TMA engine) per 9728-byte volume row
+// Warps: 0 TMA issuer, 1 idle, 2..3 support builders, 4..11 the two MMA + epilogue groups.
 // Diagnostics: -DCT3_TRACE records a clock64 timeline of CTA 0 (8 events per tile) and prints it after the 3rd launch.
-// Measured (N=6400, T=16): 1.8-2.0 ms per launch.  Knock-out builds show no single saturated resource: without the
-// epilogue 1.49 ms, with half the TMA bytes or a third of the MMAs -9 % each; the per-warp dependent-instruction
-// latency of the 8 epilogue warps (~800 instructions per tile and warp, 2 such warps per scheduler) is what the
-// producer side ends up waiting for, and registers (168 x 384 threads = the whole file) cap the warp count.
 #include <cstdio>
 #include "gemm.cuh"
 #include "kernels.cuh"
@@ -39,24 +36,33 @@
 namespace ct3 {
 namespace {
 
-constexpr int TMA_WARP = 0;
-constexpr int MMA_WARP = 1;
+constexpr int TMA_WARP = 0;               // warp 1 idle
 constexpr int SB_WARP0 = 2;               // 2 support-builder warps
-constexpr int EPI_WARP0 = 4;              // warps 4..7 group 0, 8..11 group 1; (warp & 3) = TMEM lane quarter
+constexpr int EPI_WARP0 = 4;              // warps 4..7 group 0, 8..11 group 1: each a warpgroup, MMA (wgmma) + epilogue
 constexpr int THREADS = 12 * 32;
 // Precision modes (products per correlation FLOP; DESIGN.md section 2):
 //   MODE 3: texels split bf16 hi|lo, support split bf16: A_hi x [S_hi;S_lo] + A_lo x S_hi      (rel. err ~2^-17)
 //   MODE 2: texels ONE fp16 plane (rounded, 2^-12), support split fp16: A x [S_hi;S_lo] as one N=128 MMA
 //   MODE 1: texels one fp16 plane, support one fp16 plane: A x S_hi (N=64)
 // MODE <= 2 halves the bytes every tile pulls through the L2->SM path (the resource this kernel saturates:
-// 64 KiB per 2-frame tile in MODE 3) and doubles the tiles in flight for the same 128 KiB ring.
+// 64 KiB per 2-frame tile in MODE 3) and doubles the tiles in flight for the same 64 KiB ring.
 constexpr int A_PLANE = 16384;            // one 16-bit plane of a slot: [128 rows x 128 B]
-constexpr int A_RING = 131072;            // ring bytes: 4 slots of hi|lo (MODE 3) or 8 single-plane slots
+constexpr int A_RING = 65536;             // ring bytes: 2 slots of hi|lo (MODE 3) or 4 single-plane slots
 template <int MODE> struct Ring {
   static constexpr int A_SLOT = MODE == 3 ? 2 * A_PLANE : A_PLANE;   // one K-half (64 channels) of a 2-frame tile
   static constexpr int NSLOT = A_RING / A_SLOT;
 };
-constexpr int MAX_NSLOT = 8;
+// Tiles alternate between the two MMA + epilogue groups, and each group owns half of the ring: K-half kh of tile it
+// goes to slot (it & 1) * NSLOT/2 + u % (NSLOT/2), u = (it >> 1) * 2 + kh, in phase u / (NSLOT/2).  A slot is then only
+// ever consumed by one group, in order, so a parity wait can never alias a phase two completions ahead.
+template <int NSLOT>
+__device__ __forceinline__ void ring_slot(uint32_t it, int kh, int& sl, uint32_t& parity) {
+  constexpr uint32_t SPG = NSLOT / 2;
+  const uint32_t u = (it >> 1) * 2u + (uint32_t)kh;
+  sl = (int)((it & 1u) * SPG + u % SPG);
+  parity = (u / SPG) & 1u;
+}
+constexpr int MAX_NSLOT = 4;
 constexpr int S_HALF = 2 * 8192;          // one K-half of S: [hi rows 0..63 | lo rows 64..127] x 128 B = one N=128 operand
 constexpr int S_BYTES = 2 * S_HALF;       // 32 KiB
 constexpr int H_A = 52;                   // floats per (texel row, a): 49 + pad, keeps every vector 16-byte aligned
@@ -66,8 +72,8 @@ constexpr int H_GROUP = 2 * H_FRAME * 4;  // bytes per epilogue group (2 frames)
 constexpr int ROW_BYTES_SPLIT = 2 * kVolPad * 2;   // 9728: one volume row image [hi | lo] (split bf16)
 constexpr int ROW_BYTES_H16 = kVolPad * 2;         // 4864: one volume row image, single fp16 plane
 static_assert(2 * ROW_BYTES_SPLIT <= H_GROUP, "the output image of a tile reuses the blend buffer");
-constexpr int NACC = 4;                   // TMEM accumulators (tile it -> it % NACC): the MMA issuer runs ahead of the epilogue
-constexpr uint32_t TMEM_COLS = NACC * 128;  // each: 64 columns (A_hi+A_lo) S_hi | 64 columns A_hi S_lo
+constexpr int ACC_LD = 64 + 4;            // per group: accumulator tile [128 rows][ACC_LD] fp32 (MMA registers -> row per thread)
+constexpr int ACC_BYTES = 128 * ACC_LD * 4;
 constexpr int NPARAM = 8;                 // parameter ring: a tile's slot may only be rewritten after its epilogue read it
 constexpr int OFF_A = 0;
 constexpr int OFF_S = OFF_A + A_RING;
@@ -76,7 +82,8 @@ constexpr int OFF_TAB = OFF_H + 2 * H_GROUP;     // [group 2][frame 2][b 8] x {w
 constexpr int XCH_GROUP = 2 * 7 * H_A * 4;       // texel row 4 of both frames: [frame][a][k], register y-blend path
 constexpr int OFF_XCH = OFF_TAB + 2 * 2 * 8 * 16;
 constexpr int OFF_PARAM = OFF_XCH + 2 * XCH_GROUP;   // [slot NPARAM][frame 2] x {cx, cy, box_x, box_y}
-constexpr int OFF_BAR = OFF_PARAM + NPARAM * 2 * 16;
+constexpr int OFF_ACC = OFF_PARAM + NPARAM * 2 * 16;
+constexpr int OFF_BAR = OFF_ACC + 2 * ACC_BYTES;
 constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
 static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 
@@ -127,12 +134,9 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
   uint8_t* smem = smem_align1024(smem_raw);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* a_full = bars;                  // [NSLOT] TMA -> MMA         (count 1 + tx bytes)
-  uint64_t* a_empty = bars + MAX_NSLOT;     // [NSLOT] MMA -> TMA         (tcgen05.commit)
-  uint64_t* d_full = bars + 2 * MAX_NSLOT;             // [NACC] MMA -> epilogue group  (tcgen05.commit)
-  uint64_t* d_empty = bars + 2 * MAX_NSLOT + NACC;     // [NACC] epilogue group -> MMA  (count 4)
-  uint64_t* s_full = bars + 2 * MAX_NSLOT + 2 * NACC;      // builders -> MMA, per unit  (count 2)
-  uint64_t* s_empty = bars + 2 * MAX_NSLOT + 2 * NACC + 1; // MMA -> builders, per unit  (tcgen05.commit)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * MAX_NSLOT + 2 * NACC + 2);
+  uint64_t* a_empty = bars + MAX_NSLOT;     // [NSLOT] MMA -> TMA         (one arrive per warp of the consuming group)
+  uint64_t* s_full = bars + 2 * MAX_NSLOT;      // builders -> MMA, per unit  (count 2)
+  uint64_t* s_empty = bars + 2 * MAX_NSLOT + 1; // MMA -> builders, per unit  (one arrive per warp of both groups)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_per_unit = (g.T + 1) / 2;
@@ -143,26 +147,18 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
   if (threadIdx.x == 0) {
     for (int i = 0; i < NSLOT; ++i) {
       mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 1);
-    }
-    for (int i = 0; i < NACC; ++i) {
-      mbar_init(&d_full[i], 1);
-      mbar_init(&d_empty[i], 4);
+      mbar_init(&a_empty[i], 4);
     }
     mbar_init(s_full, 2);
-    mbar_init(s_empty, 1);
+    mbar_init(s_empty, 8);
     fence_barrier_init();
     for (int l = 0; l < kL; ++l) tma_prefetch_desc(&maps.m[l]);
   }
-  if (warp == MMA_WARP) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == TMA_WARP) {
     // ================================================================== TMA issuer (whole warp walks, lane 0 issues)
-    uint32_t it = 0, hc = 0;   // tile / K-half slot counters
+    uint32_t it = 0;   // tile counter
     for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
       const int n = u / kL, l = u % kL;
       const int H = g.lay.h[l], W = g.lay.w[l];
@@ -181,12 +177,14 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
             const int bx0 = box_origin8(cx0, W), by0 = box_origin8(cy0, H);
             const int bx1 = box_origin8(cx1, W), by1 = box_origin8(cy1, H);
 #pragma unroll
-            for (int kh = 0; kh < 2; ++kh, ++hc) {
-              const int sl = hc % NSLOT;
+            for (int kh = 0; kh < 2; ++kh) {
+              int sl;
+              uint32_t par;
+              ring_slot<NSLOT>(it, kh, sl, par);
               if (kh == 0) TRACE(it, 0);
-              mbar_wait_spin(&a_empty[sl], ((hc / NSLOT) & 1u) ^ 1u);
+              mbar_wait_spin(&a_empty[sl], par ^ 1u);
               if (kh == 0) TRACE(it, 1);
-              if (kh == 0) {   // the tile's parameters become visible to the epilogue through a_full -> d_full
+              if (kh == 0) {   // the tile's parameters become visible to the epilogue through a_full
                 float4* prm = reinterpret_cast<float4*>(smem + OFF_PARAM + (it % NPARAM) * 32);
                 prm[0] = make_float4(cx0, cy0, __int_as_float(bx0), __int_as_float(by0));
                 prm[1] = make_float4(cx1, cy1, __int_as_float(bx1), __int_as_float(by1));
@@ -209,44 +207,7 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
         __syncwarp();
       }
     }
-  } else if (warp == MMA_WARP) {
-    // ================================================================== MMA issuer
-    if (elect_one()) {
-      constexpr uint32_t idesc64 = umma_idesc_16(128, 64, F16), idesc128 = umma_idesc_16(128, 128, F16);
-      uint32_t it = 0, ui = 0, hc = 0;
-      const uint32_t s_base = smem_u32(smem + OFF_S);
-      for (int u = blockIdx.x; u < num_units; u += gridDim.x, ++ui) {
-        mbar_wait_spin(s_full, ui & 1u);
-        for (int tp = 0; tp < tiles_per_unit; ++tp, ++it) {
-          const int acc = it % NACC;
-          const uint32_t d_tmem = tmem_base + (uint32_t)(acc * 128);
-#pragma unroll
-          for (int kh = 0; kh < 2; ++kh, ++hc) {
-            const int sl = hc % NSLOT;
-            mbar_wait_spin(&a_full[sl], (hc / NSLOT) & 1u);
-            if (kh == 0) TRACE(it, 2);
-            if (kh == 0) mbar_wait_spin(&d_empty[acc], ((it / NACC) & 1u) ^ 1u);
-            if (kh == 0) TRACE(it, 3);
-            tc_fence_after_sync();
-            const uint32_t a_base = smem_u32(smem + OFF_A + sl * A_SLOT);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              // A_hi x [S_hi ; S_lo] as ONE N=128 MMA (A_hi is fetched once for both products): columns 0..63 += A_hi S_hi,
-              // columns 64..127 += A_hi S_lo; then A_lo x S_hi (N=64) on columns 0..63.  The epilogue adds the halves.
-              const uint64_t dah = umma_desc_sw128(a_base + j * 32);
-              const uint64_t ds = umma_desc_sw128(s_base + (uint32_t)(kh * S_HALF + j * 32));
-              umma_bf16(d_tmem, dah, ds, MODE == 1 ? idesc64 : idesc128, (kh | j) != 0 ? 1u : 0u);
-              if (MODE == 3) umma_bf16(d_tmem, umma_desc_sw128(a_base + A_PLANE + j * 32), ds, idesc64, 1u);
-            }
-            umma_commit(&a_empty[sl]);   // this K-half may be refilled while the other one is still being multiplied
-          }
-          umma_commit(&d_full[acc]);
-          TRACE(it, 4);
-        }
-        umma_commit(s_empty);
-      }
-    }
-  } else if (warp < EPI_WARP0) {
+  } else if (warp >= SB_WARP0 && warp < EPI_WARP0) {
     // ================================================================== support builders (B operand, once per unit)
     const int sb = warp - SB_WARP0;
     const int atom = lane >> 4, chunk = (lane & 15) >> 1, half = lane & 1;  // where this lane's 4 channels live
@@ -285,10 +246,10 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
       __syncwarp();
       if (lane == 0) mbar_arrive(s_full);
     }
-  } else {
-    // ================================================================== epilogue
-    const int grp = (warp - EPI_WARP0) >> 2;   // tiles with (it & 1) == grp, accumulator grp
-    const int q = warp & 3;                    // TMEM lane quarter
+  } else if (warp >= EPI_WARP0) {
+    // ================================================================== MMA + epilogue groups
+    const int grp = (warp - EPI_WARP0) >> 2;   // tiles with (it & 1) == grp
+    const int q = warp & 3;                    // row quarter
     const int r = q * 32 + lane;               // D row = f*64 + y*8 + x; also this thread's index in the group
     const int f = r >> 6, py = (r >> 3) & 7, px = r & 7;
     const int a = min(px, 6);                  // x-offset index this lane blends (lane px == 7 only feeds others)
@@ -297,7 +258,8 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
     float4* tab = reinterpret_cast<float4*>(smem + OFF_TAB + grp * 256);
     float4* xch = reinterpret_cast<float4*>(smem + OFF_XCH + grp * XCH_GROUP);
     float4* hrow = reinterpret_cast<float4*>(hbuf + f * H_FRAME + py * H_ROW + a * H_A);
-    const uint32_t tlane = tmem_base + ((uint32_t)(q * 32) << 16);
+    float* acc_tile = reinterpret_cast<float*>(smem + OFF_ACC + grp * ACC_BYTES);
+    const uint32_t s_base = smem_u32(smem + OFF_S);
     const int bar_id = 1 + grp;
     // volume row owned by this thread when the y-blend runs ...
     //   in registers (interior tiles): lane (texel row b = py < 7, a = px < 7) of frame f -> rho = a*7 + b
@@ -309,17 +271,57 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
     const int yf = r >= kP ? 1 : 0;
     const int rho_gen = r - yf * kP;
     const int ya = rho_gen / 7, yb = rho_gen - ya * 7;
-    uint32_t it = 0;
-    for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
+    uint32_t it = 0, ui = 0;
+    for (int u = blockIdx.x; u < num_units; u += gridDim.x, ++ui) {
       const int n = u / kL, l = u % kL;
       const int H = g.lay.h[l], W = g.lay.w[l];
+      mbar_wait(s_full, ui & 1u);
       for (int tp = 0; tp < tiles_per_unit; ++tp, ++it) {
         if ((int)(it & 1u) != grp) continue;
-        const int acc = it % NACC;
-        const uint32_t taddr = tlane + (uint32_t)(acc * 128);
-        mbar_wait(&d_full[acc], (it / NACC) & 1u);
+        {
+          // D[texel row][k] over both K-halves: A x [S_hi ; S_lo] as ONE N=128 MMA (columns 0..63 += A_hi S_hi,
+          // 64..127 += A_hi S_lo), then A_lo x S_hi (N=64) on columns 0..63 (MODE 3); the halves are added in
+          // registers, so the tile handed to the epilogue is [128 rows][64 columns]
+          constexpr int NN = MODE == 1 ? 64 : 128;
+          float d0[NN / 2], d1[NN / 2];
+#pragma unroll
+          for (int kh = 0; kh < 2; ++kh) {
+            int sl;
+            uint32_t par;
+            ring_slot<NSLOT>(it, kh, sl, par);
+            mbar_wait(&a_full[sl], par);
+            if (kh == 0) TRACE(it, 2);
+            wgmma_fence();
+            const uint32_t a_base = smem_u32(smem + OFF_A + sl * A_SLOT);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const uint64_t ds = gmma_desc_sw128(s_base + (uint32_t)(kh * S_HALF + j * 32));
+              const uint32_t first = (kh | j) != 0 ? 1u : 0u;
+              wgmma_tile<NN, F16>(d0, gmma_desc_sw128(a_base + j * 32), ds, first);
+              wgmma_tile<NN, F16>(d1, gmma_desc_sw128(a_base + 8192 + j * 32), ds, first);
+              if constexpr (MODE == 3) {
+                wgmma_m64n64_bf16_head(d0, gmma_desc_sw128(a_base + A_PLANE + j * 32), ds, 1u);
+                wgmma_m64n64_bf16_head(d1, gmma_desc_sw128(a_base + A_PLANE + 8192 + j * 32), ds, 1u);
+              }
+            }
+            wgmma_commit();
+            wgmma_wait0(d0);
+            wgmma_wait0(d1);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&a_empty[sl]);   // this K-half may be refilled
+          }
+          float o0[32], o1[32];
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            o0[i] = NN == 128 ? d0[i] + d0[(i + 32) % (NN / 2)] : d0[i];
+            o1[i] = NN == 128 ? d1[i] + d1[(i + 32) % (NN / 2)] : d1[i];
+          }
+          asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");   // the previous tile's rows have been read
+          acc_store<64>(o0, acc_tile, ACC_LD);
+          acc_store<64>(o1, acc_tile + 64 * ACC_LD, ACC_LD);
+          asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+        }
         if (r == 0) TRACE(it, 5);
-        tc_fence_after_sync();
         const float4* prms = reinterpret_cast<const float4*>(smem + OFF_PARAM + (it % NPARAM) * 32);
         const float4 prm = prms[f];
         int sx0, sx1;
@@ -341,25 +343,15 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
         const float wy = __shfl_sync(0xffffffffu, wy_l, f * 8 + min(py, 6));   // this lane's row weight (fast path)
         // ---- x-blend: h[k] = (1-wx) D[(row, x0), k] + wx D[(row, x1), k]  for (texel row py, sample column a)
         float h[H_A];
-        // drain the accumulator first (h[k] = (A_hi + A_lo) S_hi + A_hi S_lo, 16 columns at a time) and hand it back to
-        // the MMA issuer before any blending: TMEM is the resource the next-but-one tile waits for
+        // h[k] = (A_hi + A_lo) S_hi + A_hi S_lo, 16 columns at a time
 #pragma unroll
         for (int c4 = 0; c4 < 4; ++c4) {
           float v[16];
-          tmem_ld16(taddr + 16 * c4, v);
-          if (MODE >= 2) {
-            float w[16];
-            tmem_ld16(taddr + 64 + 16 * c4, w);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] += w[j];
-          }
+          acc_row_ld<16>(acc_tile + r * ACC_LD + 16 * c4, v);
 #pragma unroll
           for (int j = 0; j < 16; ++j)
             if (16 * c4 + j < H_A) h[16 * c4 + j] = (16 * c4 + j < kP) ? v[j] : 0.f;
         }
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&d_empty[acc]);
         if (r == 0) TRACE(it, 6);
 #pragma unroll
         for (int k = 0; k < kP; ++k) {
@@ -475,13 +467,12 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
           TRACE(it, 7);
         }
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(s_empty);         // this warp's MMAs of the unit have all completed
     }
   }
 
   if (warp >= EPI_WARP0 && (threadIdx.x & 127) == 0) bulk_wait0();   // outstanding volume-row copies
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == MMA_WARP) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 // fp32 channels-last level -> [hi plane | lo plane] bf16, 4 channels per thread
@@ -532,7 +523,7 @@ cudaError_t launch_split_pyramid(const float* pyr, int T, int H4, int W4, __nv_b
     const int64_t n = (int64_t)T * lay.h[l] * lay.w[l] * kD;
     __nv_bfloat16* dst = pyr_split + 2 * lay.off[l];   // level l always starts at the same offset, whatever the mode
     const int64_t n4 = n / 4;
-    const int grid = (int)((n4 + 255) / 256 < 148 * 16 ? (n4 + 255) / 256 : 148 * 16);
+    const int grid = (int)((n4 + 255) / 256 < 132 * 16 ? (n4 + 255) / 256 : 132 * 16);
     if (mode == 3)
       split_level_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<const float4*>(pyr + lay.off[l]),
                                               reinterpret_cast<uint2*>(dst), reinterpret_cast<uint2*>(dst + n), n4);

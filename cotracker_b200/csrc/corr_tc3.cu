@@ -10,25 +10,23 @@
 // correlate the RAW 8x8 texel patch around the track with the 49 support vectors and the epilogue blends the 64 raw
 // correlations into the 49 sampled ones), but with the MMA TRANSPOSED: the support vectors are the M side and the
 // texels the N side, so a thread of the epilogue owns ONE support vector k and sees all 64 raw correlations of a
-// frame as TMEM columns.  Both blends (x, then y) become plain FMAs on the thread's own registers with warp-uniform
-// weights: no shuffles, no exchange of texel rows between lanes -- corr_tc2.cu's epilogue (98 + 52 shuffles and a
-// shared-memory y-blend per tile) was what bounded that kernel (profiles/r2_corr_tc3_history.txt).
+// frame in its accumulator row.  Both blends (x, then y) become plain FMAs on the thread's own registers with
+// warp-uniform weights: no shuffles, no exchange of texel rows between lanes.
 //
 //   pyramid  : ONE fp16 plane per level [T][H][W][128] (made once per update-loop call); texels are rounded to fp16
 //              (2^-12 relative), the support vectors are exact to a split fp16 pair (prec.corr = 2, DESIGN.md section 2)
 //   B tile   [128 texel rows x 64 ch] : rows f*64 + y*8 + x = the raw texels of 2 frames; each (frame, K-half) is ONE
-//              4-D TMA box (64 ch x 8 x 8 x 1) landing in the 128B-swizzled K-major operand layout; ring of 5 K-half
-//              slots (16 KiB), each freed as soon as its MMAs retire
+//              4-D TMA box (64 ch x 8 x 8 x 1) landing in the 128B-swizzled K-major operand layout; ring of 3 K-half
+//              slots (16 KiB), each freed as soon as the MMAs reading it have completed
 //   A tiles  4 x [128 x 64 ch] : {hi, lo} plane x K-half of the 49 support vectors of (n,l) in rows 0..48 (rows 49..127
 //              stay zero), built once per unit by 2 warps.  The hi and lo planes are CONCATENATED ALONG K:
-//              D += S_hi[kh] . F[kh]^T  and  D += S_lo[kh] . F[kh]^T  accumulate into the same TMEM lanes, so lane k
+//              D += S_hi[kh] . F[kh]^T  and  D += S_lo[kh] . F[kh]^T  accumulate into the same registers, so row k
 //              holds the complete (S_hi + S_lo)[k] . F and the epilogue needs no exchange between warps.
 //              (prec.corr = 1 skips the lo MMAs: single fp16 product.)
-//   D        [128 x 128] fp32 in TMEM, lanes 0..48 live, columns = texels (f*64 + y*8 + x); 4 accumulators
-//   epilogue : 4 groups x 2 warps (TMEM lane quarters 0 and 1) take tiles round-robin; thread = support vector k.
-//              (Each epilogue warp is a latency-bound dependent chain -- ~0.2 IPC -- so throughput comes from the number
-//              of groups: 128 registers per thread buy the fourth one.)
-//              Per frame: 4 x tcgen05.ld (two texel rows each) -> x-blend -> y-blend -> 49 sampled correlations ->
+//   D        [64 x 128] fp32: one m64n128 wgmma accumulator of the MMA warpgroup (rows 0..48 live, columns = texels
+//              f*64 + y*8 + x), stored to one of 2 accumulator tiles in shared memory (rows 0..48)
+//   epilogue : 2 groups x 2 warps take tiles round-robin; thread = support vector k.
+//              Per frame: 64 accumulator columns -> x-blend -> y-blend -> 49 sampled correlations ->
 //              convert -> volume-row image in shared memory -> bulk shared->global copy of the whole 9.5 KiB row.
 //              A border clamp only turns the tap indices into a clamped SHIFT of the interior pattern
 //              (idx = clamp(a + d, 0, 7), d uniform per frame and axis), so every case -- interior, any border, far
@@ -36,16 +34,13 @@
 //              (exactly grid_sample's border-clamped taps, canonicalised to the shift pattern;
 //              tests/test_host_logic.py brute-forces that this always works) are computed once per tile by the
 //              otherwise idle lanes of the TMA warp.  The blend code exists ONCE (frame loop not unrolled): a fully
-//              unrolled epilogue is 290 KB of SASS and ran 5x slower on instruction-cache misses
-//              (profiles/r2_corr_tc3_history.txt).
+//              unrolled epilogue is hundreds of KB of SASS and thrashes the instruction cache.
 //   schedule : persistent CTAs; a unit = (track n, level l) = T frames of one support operand.  A CTA's first unit is
-//              blockIdx.x, the others come from a global counter (SMs differ by up to 10 % in speed on this kernel).
+//              blockIdx.x, the others come from a global counter (SMs differ in speed on this kernel).
 //   L2       : texel boxes are loaded evict_last, volume rows stored evict_first (the 3.9 GB write stream would
-//              otherwise push the 67 MB pyramid, read ~100x, out of L2)
-// What was measured and NOT adopted (support rows duplicated into TMEM lanes 64..112 for a four-partition epilogue, the
-// A operand in tensor memory, rolling / two-phase packed-FMA epilogues): profiles/r2_corr_tc3_history.txt.
-// Warps (14): 0,1 / 4,5 / 8,9 / 12,13 epilogue groups (warp % 4 = TMEM lane quarter), 2 TMA issuer (+ tap tables),
-// 3 MMA issuer (+ TMEM alloc), 6,7 support builders (6 also draws the units), 10,11 idle.
+//              otherwise push the pyramid, read ~100x, out of L2)
+// Warps (12): 0,1 / 4,5 epilogue groups, 2 TMA issuer (+ tap tables), 3 idle, 6,7 support builders (6 also draws
+// the units), 8..11 MMA warpgroup.
 #include "gemm.cuh"
 #include "kernels.cuh"
 
@@ -53,16 +48,18 @@ namespace ct3 {
 namespace {
 
 constexpr int TMA_WARP = 2;
-constexpr int MMA_WARP = 3;
 constexpr int SB_WARP0 = 6;               // warps 6, 7 build the support operand
-constexpr int NGROUP = 4;                 // epilogue groups: warps {0,1}, {4,5}, {8,9}, {12,13}  (warps 10, 11 idle)
-constexpr int THREADS = 14 * 32;          // 128 registers per thread
-constexpr int NSLOT = 5;                  // texel ring: slots of one K-half (64 channels) of a 2-frame tile
+constexpr int MMA_WARP0 = 8;              // warps 8..11: the MMA warpgroup
+constexpr int MMA_WARPS = 4;
+constexpr int NGROUP = 2;                 // epilogue groups: warps {0,1}, {4,5}  (warp 3 idle)
+constexpr int THREADS = 12 * 32;          // 168 registers per thread
+constexpr int NSLOT = 3;                  // texel ring: slots of one K-half (64 channels) of a 2-frame tile
 constexpr int A_SLOT = 16384;             // [128 texel rows x 128 B] fp16
 constexpr int S_TILE = 16384;             // one (plane, K-half) of S: [128 rows x 128 B], rows 49..127 zero
 constexpr int S_BYTES = 4 * S_TILE;       // tile index = plane * 2 + K-half
-constexpr int NACC = 4;
-constexpr uint32_t TMEM_COLS = NACC * 128;
+constexpr int NACC = 2;                   // accumulator tiles in shared memory: [64 rows][ACC_LD] fp32, rows 0..48 live
+constexpr int ACC_LD = 128 + 4;
+constexpr int ACC_BYTES = 64 * ACC_LD * 4;
 constexpr int NPARAM = 8;                 // tap-table ring (a tile's slot is rewritten only after its epilogue read it)
 constexpr int PRM_WORDS = 64;             // per tile: [frame 2][axis 2]{u[7], w[7]} = 56 floats, d[2][2] ints, flag
 constexpr int ROW_BYTES_SPLIT = 2 * kVolPad * 2;   // 9728
@@ -71,7 +68,8 @@ constexpr int IMG_GROUP = 2 * ROW_BYTES_SPLIT;
 constexpr int OFF_A = 0;
 constexpr int OFF_S = OFF_A + NSLOT * A_SLOT;
 constexpr int OFF_IMG = OFF_S + S_BYTES;
-constexpr int OFF_PARAM = OFF_IMG + NGROUP * IMG_GROUP;
+constexpr int OFF_ACC = OFF_IMG + NGROUP * IMG_GROUP;
+constexpr int OFF_PARAM = OFF_ACC + NACC * ACC_BYTES;
 constexpr int OFF_BAR = OFF_PARAM + NPARAM * PRM_WORDS * 4;
 constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
 static_assert(SMEM_BYTES <= 232448, "shared memory budget");
@@ -177,16 +175,16 @@ __device__ __forceinline__ void yblend_dispatch(int d, const float (&hx)[8][7], 
   }
 }
 
-// Epilogue of one 2-frame tile for one thread = support vector k (TMEM lane k).  The blend code exists ONCE (the
+// Epilogue of one 2-frame tile for one thread = support vector k (accumulator row k).  The blend code exists ONCE (the
 // frame loop is not unrolled; see the file header).
 template <bool V16>
-__device__ __forceinline__ void epilogue_tile(uint32_t tmem_base, int acc, int q, int lane, int grp, int nf,
+__device__ __forceinline__ void epilogue_tile(const float* acc_tile, int q, int lane, int grp, int nf,
                                               const float* prm, uint16_t* img, uint64_t* d_empty_bar, uint16_t* vrow) {
   constexpr int ROW_BYTES = V16 ? ROW_BYTES_H16 : ROW_BYTES_SPLIT;
   const int k = q * 32 + lane;                        // q in {0, 1}
   const bool live = k < kP;
   const int bar_id = 1 + grp;                         // named barrier of this group (64 threads)
-  const uint32_t tlane = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * 128);
+  const float* arow = acc_tile + k * ACC_LD;         // rows >= 49 are never written and their results never stored
   const int* iprm = reinterpret_cast<const int*>(prm) + 56;
   if (iprm[4] == 0) asm volatile("trap;");   // a sample outside the shift pattern: impossible (see file header)
   if (k == 0) bulk_wait_read0();             // previous tile's row images have left shared memory ...
@@ -196,7 +194,7 @@ __device__ __forceinline__ void epilogue_tile(uint32_t tmem_base, int acc, int q
     float hx[8][7];
     {
       float v[64];
-      tmem_ld64(tlane + (uint32_t)(f * 64), v);
+      acc_row_ld<64>(arow + f * 64, v);
       float ux[7], wx[7];
 #pragma unroll
       for (int a = 0; a < 7; ++a) { ux[a] = prm[(f * 2 + 0) * 14 + a]; wx[a] = prm[(f * 2 + 0) * 14 + 7 + a]; }
@@ -207,9 +205,8 @@ __device__ __forceinline__ void epilogue_tile(uint32_t tmem_base, int acc, int q
     for (int b = 0; b < 7; ++b) { uy[b] = prm[(f * 2 + 1) * 14 + b]; wy[b] = prm[(f * 2 + 1) * 14 + 7 + b]; }
     const int dy = iprm[2 * f + 1];
     if (f == nf - 1) {
-      // every TMEM read of this tile has completed (tcgen05.wait::ld inside tmem_ld64) and nothing below reads the
-      // tap table any more: releasing the accumulator is also what eventually lets the TMA warp recycle the table slot
-      tc_fence_before_sync();
+      // every accumulator read of this tile has completed and nothing below reads the tap table any more: releasing the
+      // accumulator is also what eventually lets the TMA warp recycle the table slot
       __syncwarp();
       if (lane == 0) mbar_arrive(d_empty_bar);
     }
@@ -260,18 +257,18 @@ corr_patch_t_kernel(const __grid_constant__ Corr3Args g, const __grid_constant__
   uint8_t* smem = smem_align1024(smem_raw);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* a_full = bars;                          // [NSLOT] TMA -> MMA         (count 1 + tx bytes)
-  uint64_t* a_empty = bars + NSLOT;                 // [NSLOT] MMA -> TMA         (tcgen05.commit)
-  uint64_t* d_full = bars + 2 * NSLOT;              // [NACC] MMA -> epilogue group  (tcgen05.commit)
+  uint64_t* a_empty = bars + NSLOT;                 // [NSLOT] MMA -> TMA         (one arrive per MMA warp)
+  uint64_t* d_full = bars + 2 * NSLOT;              // [NACC] MMA -> epilogue group  (one arrive per MMA warp)
   uint64_t* d_empty = bars + 2 * NSLOT + NACC;      // [NACC] epilogue group -> MMA  (count 2)
   uint64_t* s_full = bars + 2 * NSLOT + 2 * NACC;       // builders -> MMA, per unit  (count 2)
-  uint64_t* s_empty = bars + 2 * NSLOT + 2 * NACC + 1;  // MMA -> builders, per unit  (tcgen05.commit)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * NSLOT + 2 * NACC + 2);
+  uint64_t* s_empty = bars + 2 * NSLOT + 2 * NACC + 1;  // MMA -> builders, per unit  (one arrive per MMA warp)
+  float* acc_base = reinterpret_cast<float*>(smem + OFF_ACC);
   // Unit queue.  A unit = (track n, level l) = T frames of one support operand; SMs differ by up to 10 % in speed on
   // this kernel (distance to the L2 slices), so only the first unit of a CTA is static (blockIdx.x) and the others
   // come from a global counter.  The first builder warp -- the role that runs furthest ahead -- draws the numbers and
   // publishes them here in order; every other role reads entry ui when it gets there (an entry is rewritten 8 units
   // later, no role lags that far).  -1 ends every role's loop.
-  volatile int* unit_q = reinterpret_cast<volatile int*>(tmem_slot + 1);   // [8]
+  volatile int* unit_q = reinterpret_cast<volatile int*>(bars + 2 * NSLOT + 2 * NACC + 2);   // [8]
   volatile int* unit_tail = unit_q + 8;                                    // number of published entries
   auto unit_at = [&](uint32_t ui) -> int {
     uint32_t spins = 0;
@@ -290,24 +287,20 @@ corr_patch_t_kernel(const __grid_constant__ Corr3Args g, const __grid_constant__
   if (threadIdx.x == 0) {
     for (int i = 0; i < NSLOT; ++i) {
       mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 1);
+      mbar_init(&a_empty[i], MMA_WARPS);
     }
     for (int i = 0; i < NACC; ++i) {
-      mbar_init(&d_full[i], 1);
+      mbar_init(&d_full[i], MMA_WARPS);
       mbar_init(&d_empty[i], 2);
     }
     mbar_init(s_full, 2);
-    mbar_init(s_empty, 1);
+    mbar_init(s_empty, MMA_WARPS);
     unit_q[0] = (int)blockIdx.x < num_units ? (int)blockIdx.x : -1;
     *unit_tail = 1;
     fence_barrier_init();
     for (int l = 0; l < kL; ++l) tma_prefetch_desc(&maps.m[l]);
   }
-  if (warp == MMA_WARP) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == TMA_WARP) {
     // ================================================================== TMA issuer + tap tables (whole warp)
@@ -337,8 +330,8 @@ corr_patch_t_kernel(const __grid_constant__ Corr3Args g, const __grid_constant__
           box_origin8(cx1, W, bx1, dx1);
           box_origin8(cy1, H, by1, dy1);
           // The first K-half slot of this tile doubles as the gate of the table slot: slot it % 8 was last used by
-          // tile it - 8; the ring slot waited for here was freed by MMAs of tile it - 3, which were issued after
-          // tile it - 4's, which needed the accumulator that tile it - 8's epilogue had released after reading its table.
+          // tile it - 8; the ring slot waited for here was freed by MMAs of tile it - 2, which were issued after
+          // they had the accumulator that tile it - 4's epilogue had released after reading its table.
           mbar_wait_spin(&a_empty[hc % NSLOT], ((hc / NSLOT) & 1u) ^ 1u);
           {
             float* prm = reinterpret_cast<float*>(smem + OFF_PARAM) + (it % NPARAM) * PRM_WORDS;
@@ -379,40 +372,43 @@ corr_patch_t_kernel(const __grid_constant__ Corr3Args g, const __grid_constant__
         }
       }
     }
-  } else if (warp == MMA_WARP) {
-    // ================================================================== MMA issuer
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_16(128, 128, /*fp16*/ true);
-      uint32_t it = 0, ui = 0, hc = 0;
-      const uint32_t s_base = smem_u32(smem + OFF_S);
-      for (;; ++ui) {
-        if (unit_at(ui) < 0) break;
-        mbar_wait_spin(s_full, ui & 1u);
-        for (int tp = 0; tp < tiles_per_unit; ++tp, ++it) {
-          const int acc = it % NACC;
-          const uint32_t d_tmem = tmem_base + (uint32_t)(acc * 128);
+  } else if (warp >= MMA_WARP0) {
+    // ================================================================== MMA warpgroup
+    uint32_t it = 0, ui = 0, hc = 0;
+    const uint32_t s_base = smem_u32(smem + OFF_S);
+    for (;; ++ui) {
+      if (unit_at(ui) < 0) break;
+      mbar_wait(s_full, ui & 1u);
+      for (int tp = 0; tp < tiles_per_unit; ++tp, ++it) {
+        const int acc = it % NACC;
+        float d[64];   // D[support k][texel]: rows 0..63 of S (49 live) x the 128 texels of the tile
 #pragma unroll
-          for (int kh = 0; kh < 2; ++kh, ++hc) {
-            const int sl = hc % NSLOT;
-            mbar_wait_spin(&a_full[sl], (hc / NSLOT) & 1u);
-            if (kh == 0) mbar_wait_spin(&d_empty[acc], ((it / NACC) & 1u) ^ 1u);
-            tc_fence_after_sync();
-            const uint32_t f_base = smem_u32(smem + OFF_A + sl * A_SLOT);
+        for (int kh = 0; kh < 2; ++kh, ++hc) {
+          const int sl = hc % NSLOT;
+          mbar_wait(&a_full[sl], (hc / NSLOT) & 1u);
+          if (kh == 0) mbar_wait(&d_empty[acc], ((it / NACC) & 1u) ^ 1u);
+          wgmma_fence();
+          const uint32_t f_base = smem_u32(smem + OFF_A + sl * A_SLOT);
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              // D[support k][texel] += S_lo[k] . F^T + S_hi[k] . F^T over this K-half (hi and lo concatenated along K)
-              const uint64_t df = umma_desc_sw128(f_base + j * 32);
-              if (!ONEPROD)
-                umma_bf16(d_tmem, umma_desc_sw128(s_base + (uint32_t)((2 + kh) * S_TILE + j * 32)), df, idesc, (kh | j) != 0 ? 1u : 0u);
-              umma_bf16(d_tmem, umma_desc_sw128(s_base + (uint32_t)(kh * S_TILE + j * 32)), df, idesc,
-                        (!ONEPROD || (kh | j) != 0) ? 1u : 0u);
-            }
-            umma_commit(&a_empty[sl]);
+          for (int j = 0; j < 4; ++j) {
+            // D[support k][texel] += S_lo[k] . F^T + S_hi[k] . F^T over this K-half (hi and lo concatenated along K)
+            const uint64_t df = gmma_desc_sw128(f_base + j * 32);
+            if (!ONEPROD)
+              wgmma_tile<128, true>(d, gmma_desc_sw128(s_base + (uint32_t)((2 + kh) * S_TILE + j * 32)), df, (kh | j) != 0 ? 1u : 0u);
+            wgmma_tile<128, true>(d, gmma_desc_sw128(s_base + (uint32_t)(kh * S_TILE + j * 32)), df,
+                                  (!ONEPROD || (kh | j) != 0) ? 1u : 0u);
           }
-          umma_commit(&d_full[acc]);
+          wgmma_commit();
+          wgmma_wait0(d);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&a_empty[sl]);
         }
-        umma_commit(s_empty);
+        acc_store<128>(d, acc_base + acc * (ACC_BYTES / 4), ACC_LD, kP);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&d_full[acc]);
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(s_empty);       // this warp's MMAs of the unit have all completed
     }
   } else if (warp == SB_WARP0 || warp == SB_WARP0 + 1) {
     // ================================================================== support builders (A operand, once per unit)
@@ -461,9 +457,9 @@ corr_patch_t_kernel(const __grid_constant__ Corr3Args g, const __grid_constant__
       if (lane == 0) mbar_arrive(s_full);
     }
   } else if ((warp & 3) < 2) {
-    // ================================================================== epilogue: warps {0,1}, {4,5}, {8,9}, {12,13}
+    // ================================================================== epilogue: warps {0,1}, {4,5}
     const int grp = warp >> 2;                 // tiles with it % NGROUP == grp
-    const int q = warp & 3;                    // TMEM lane quarter 0 or 1
+    const int q = warp & 3;                    // rows 32q .. 32q+31 of the accumulator tile
     uint16_t* img = reinterpret_cast<uint16_t*>(smem + OFF_IMG + grp * IMG_GROUP);
     const float* prm_base = reinterpret_cast<const float*>(smem + OFF_PARAM);
     uint32_t it = 0;
@@ -475,19 +471,14 @@ corr_patch_t_kernel(const __grid_constant__ Corr3Args g, const __grid_constant__
         if ((int)(it % NGROUP) != grp) continue;
         const int acc = it % NACC;
         mbar_wait(&d_full[acc], (it / NACC) & 1u);
-        tc_fence_after_sync();
         const float* prm = prm_base + (it % NPARAM) * PRM_WORDS;
         const int nf = (2 * tp + 1 < g.T) ? 2 : 1;
         uint16_t* vrow = g.vol + (((int64_t)n * g.T + 2 * tp) * kL + l) * (ROW_BYTES / 2);
-        epilogue_tile<V16>(tmem_base, acc, q, lane, grp, nf, prm, img, &d_empty[acc], vrow);
+        epilogue_tile<V16>(acc_base + acc * (ACC_BYTES / 4), q, lane, grp, nf, prm, img, &d_empty[acc], vrow);
       }
     }
     if (q == 0 && lane == 0) bulk_wait0();     // outstanding volume-row copies of this group
   }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == MMA_WARP) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 template <bool V16, bool ONEPROD>

@@ -2,7 +2,7 @@
 // channels-last throughout (SURVEY.md 8(f) rank 1):
 //
 //   conv1 7x7/2 (3->64)            : direct fp32 SIMT kernel (K = 147 is too thin for the tensor cores; 0.9 GFLOP/frame)
-//   every 3x3 stride-1 convolution : conv3x3_tc_kernel -- IMPLICIT GEMM on tcgen05: the A tile of filter tap (ky,kx) is a
+//   every 3x3 stride-1 convolution : conv3x3_tc_kernel -- IMPLICIT GEMM on wgmma: the A tile of filter tap (ky,kx) is a
 //                                    4-D TMA box of the NHWC activation shifted by (kx-1, ky-1); out-of-bounds texels
 //                                    arrive as zeros, which IS the convolution's zero padding.  No im2col buffer exists
 //                                    (the explicit one of the previous encoder tail was 2.9 GB per 16 frames).
@@ -85,17 +85,22 @@ conv_stem_kernel(const float* __restrict__ in /*[T,3,H,W]*/, const float* __rest
 // 3x3 stride-1 pad-1 convolution as an implicit GEMM:  Y[(t,y,x), co] = sum_{ky,kx,c} X[t, y+ky-1, x+kx-1, c] W[co, ky, kx, c]
 //   A tile (128 pixels = th rows x tw columns of one frame, 64 channels of one tap) = ONE 4-D TMA box per bf16 plane
 //   B tile (BN output channels x 64 channels of one tap) from the packed weights [Cout, 2 * 9*C]  (K index = tap*C + c)
-//   warp 0 TMA producer, warp 1 MMA issuer (3 MMAs per k16: split x split), warps 2..9 epilogue (bias, fp32 NHWC stores)
-constexpr int CBM = 128, CBK = 64, CACC = 2;
+//   warps 0..3 MMA warpgroup (wgmma, 3 MMAs per k16: split x split), warp 4 TMA producer, warps 5..8 epilogue (bias,
+//   fp32 NHWC stores); the accumulator tile goes from the MMA registers to the epilogue through shared memory
+constexpr int CBM = 128, CBK = 64;
 constexpr int CTILE_A = CBM * CBK * 2;       // 16 KiB per plane
-constexpr int CEPI_WARPS = 8;
-constexpr int CTHREADS = (2 + CEPI_WARPS) * 32;
+constexpr int CMMA_WARPS = 4, CTMA_WARP = 4, CEPI_WARP0 = 5;
+constexpr int CEPI_WARPS = 4;
+constexpr int CTHREADS = (CMMA_WARPS + 1 + CEPI_WARPS) * 32;
 template <int BN> struct ConvCfg {
   static constexpr int TILE_B = BN * CBK * 2;
   static constexpr int STAGE = 2 * CTILE_A + 2 * TILE_B;          // 64 KiB (BN 128) / 48 KiB (BN 64)
-  static constexpr int STAGES = BN == 128 ? 3 : 4;
-  static constexpr int OFF_BAR = STAGES * STAGE;
+  static constexpr int STAGES = BN == 128 ? 2 : 3;
+  static constexpr int ACC_LD = BN + 4;
+  static constexpr int OFF_ACC = STAGES * STAGE;
+  static constexpr int OFF_BAR = OFF_ACC + CBM * ACC_LD * 4;
   static constexpr int SMEM = OFF_BAR + 256 + 1024;
+  static_assert(SMEM <= 232448, "shared memory budget");
 };
 struct ConvGeom {
   int T, H, W, C, Cout;      // C, Cout multiples of 64; Cout % BN == 0
@@ -114,27 +119,21 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* tfull_bar = empty_bar + STAGES;
-  uint64_t* tempty_bar = tfull_bar + CACC;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + CACC);
+  uint64_t* tempty_bar = tfull_bar + 1;
+  float* acc_tile = reinterpret_cast<float*>(smem + C::OFF_ACC);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmW);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], CMMA_WARPS);
     }
-    for (int i = 0; i < CACC; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], CEPI_WARPS);
-    }
+    mbar_init(tfull_bar, CMMA_WARPS);
+    mbar_init(tempty_bar, CEPI_WARPS);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, CACC * BN < 32 ? 32 : CACC * BN);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int num_nt = g.Cout / BN;
   const int tiles_per_frame = g.tiles_x * g.tiles_y;
@@ -143,7 +142,7 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
   const int num_kb = 9 * cblocks;
   const int Kp = 9 * g.C;
 
-  if (warp == 0) {
+  if (warp == CTMA_WARP) {
     if (elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
@@ -165,42 +164,34 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(CBM, BN);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after_sync();
-          const uint32_t s = smem_u32(smem + stage * C::STAGE);
-          const uint32_t a_hi = s, a_lo = s + CTILE_A, b_hi = s + 2 * CTILE_A, b_lo = b_hi + C::TILE_B;
-#pragma unroll
-          for (int kk = 0; kk < CBK / 16; ++kk) {
-            const uint32_t koff = kk * 32;
-            const uint64_t dah = umma_desc_sw128(a_hi + koff), dbh = umma_desc_sw128(b_hi + koff);
-            umma_bf16(d_tmem, umma_desc_sw128(a_lo + koff), dbh, idesc, (kb | kk) != 0 ? 1u : 0u);
-            umma_bf16(d_tmem, dah, umma_desc_sw128(b_lo + koff), idesc, 1u);
-            umma_bf16(d_tmem, dah, dbh, idesc, 1u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit(&tfull_bar[acc]);
-        if (++acc == CACC) { acc = 0; acc_phase ^= 1u; }
+  } else if (warp < CMMA_WARPS) {
+    int stage = 0;
+    uint32_t phase = 0, acc_phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      float d0[BN / 2], d1[BN / 2];
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        wgmma_fence();
+        mma_kblock<3, BN, false>(d0, d1, smem_u32(smem + stage * C::STAGE), CTILE_A, 2 * CTILE_A, C::TILE_B, kb == 0);
+        wgmma_commit();
+        wgmma_wait0(d0);
+        wgmma_wait0(d1);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
+      mbar_wait(tempty_bar, acc_phase ^ 1u);
+      acc_store<BN>(d0, acc_tile, C::ACC_LD);
+      acc_store<BN>(d1, acc_tile + 64 * C::ACC_LD, C::ACC_LD);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(tfull_bar);
+      acc_phase ^= 1u;
     }
   } else {
-    // epilogue: 8 warps = 4 TMEM lane quarters x 2 column halves; thread = one pixel, 16 channels per tcgen05.ld
-    const int quarter = warp & 3, half = (warp - 2) >> 2;
-    const int r = quarter * 32 + lane;                 // tile row = pixel (dy, dx)
+    // epilogue: 4 warps = 4 row quarters; thread = one pixel, 16 channels per chunk
+    const int r = (warp - CEPI_WARP0) * 32 + lane;     // tile row = pixel (dy, dx)
     const int dy = r / g.tw, dx = r % g.tw;
-    constexpr int CH = BN / 16 / 2;                    // 16-column chunks per warp
-    int acc = 0;
+    const float* arow = acc_tile + r * C::ACC_LD;
     uint32_t acc_phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int nt = tile % num_nt, pt = tile / num_nt;
@@ -208,13 +199,12 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
       const int y = (rr / g.tiles_x) * g.th + dy, x = (rr % g.tiles_x) * g.tw + dx;
       const bool valid = y < g.H && x < g.W;
       float* orow = out + (((int64_t)t * g.H + y) * g.W + x) * g.Cout + nt * BN;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after_sync();
+      mbar_wait(tfull_bar, acc_phase);
 #pragma unroll
-      for (int c = 0; c < CH; ++c) {
-        const int col = (half * CH + c) * 16;
+      for (int c = 0; c < BN / 16; ++c) {
+        const int col = c * 16;
         float v[16];
-        tmem_ld16(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BN + col), v);
+        acc_row_ld<16>(arow + col, v);
         if (valid) {
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
@@ -224,15 +214,11 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
           }
         }
       }
-      tc_fence_before_sync();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      if (++acc == CACC) { acc = 0; acc_phase ^= 1u; }
+      if (lane == 0) mbar_arrive(tempty_bar);
+      acc_phase ^= 1u;
     }
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, CACC * BN < 32 ? 32 : CACC * BN);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -366,7 +352,7 @@ __global__ void upsample_concat_split_kernel(UpArgsN a, int T, int Ctot, int Cp,
 
 inline int grid_cap(int64_t total, int block, int per_sm) {
   int64_t b = (total + block - 1) / block;
-  const int64_t cap = 148LL * per_sm;
+  const int64_t cap = 132LL * per_sm;
   return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 

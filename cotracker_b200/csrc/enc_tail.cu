@@ -174,7 +174,7 @@ cudaError_t launch_upsample_concat(const float* const src[4], const int c[4], co
   int off = 0;
   for (int k = 0; k < 4; ++k) { a.src[k] = src[k]; a.c[k] = c[k]; a.h[k] = h[k]; a.w[k] = w[k]; a.coff[k] = off; off += c[k]; }
   const int64_t total = (int64_t)T * off * H * W;
-  const int blocks = (int)((total + 255) / 256 > 148 * 64 ? 148 * 64 : (total + 255) / 256);
+  const int blocks = (int)((total + 255) / 256 > 132 * 64 ? 132 * 64 : (total + 255) / 256);
   upsample_concat_kernel<<<blocks, 256, 0, s>>>(a, T, off, H, W, out);
   return cudaGetLastError();
 }
@@ -197,7 +197,7 @@ cudaError_t launch_instnorm_stats(const float* y, int T, int HW, int C, float ep
 cudaError_t launch_instnorm_relu_split(const float* y, const float* stats, int64_t rows, int HW, int C,
                                        __nv_bfloat16* out, cudaStream_t s) {
   const int64_t total = rows * (C / 4);
-  const int blocks = (int)((total + 255) / 256 > 148 * 32 ? 148 * 32 : (total + 255) / 256);
+  const int blocks = (int)((total + 255) / 256 > 132 * 32 ? 132 * 32 : (total + 255) / 256);
   instnorm_relu_split_kernel<<<blocks, 256, 0, s>>>(y, stats, rows, HW, C, out);
   return cudaGetLastError();
 }

@@ -1,12 +1,14 @@
-// gemm.cu -- split-bf16x3 linear layers on the 5th-gen tensor cores.
+// gemm.cu -- split-bf16x3 linear layers on the Hopper tensor cores (wgmma).
 //
 // Persistent warp-specialised kernel, one CTA per SM:
-//   warp 0      : TMA producer   (cp.async.bulk.tensor, 128B-swizzled K-major tiles, 3-stage ring)
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer (3 MMAs per k16 step: hi*hi, lo*hi, hi*lo)
-//   warps 2..17 : epilogue       (tcgen05.ld -> bias / row-bias / GELU / residual -> fp32 and/or split-bf16 stores)
-// Two 128-column fp32 accumulators in TMEM are double buffered so the epilogue of tile i overlaps the
-// main loop of tile i+1.  Tiles are 128 x 128; consecutive tile ids share the X (activation) tile so the
-// big operand is read from HBM once and hit in L2 by the CTAs working on its other N-tiles.
+//   warps 0..3  : MMA warpgroup   (wgmma m64n128k16 on both 64-row halves of the tile, 3 MMAs per k16 step:
+//                                  lo*hi, hi*lo, hi*hi; fp32 accumulators in registers)
+//   warp 4      : TMA producer    (cp.async.bulk.tensor, 128B-swizzled K-major tiles, ring of 2-4 stages)
+//   warps 5..8  : epilogue        (bias / row-bias / GELU / residual -> fp32 and/or split-bf16 stores)
+// The accumulator tile goes from the MMA registers to the epilogue through one fp32 tile in shared memory; the MMA
+// warpgroup computes tile i+1 in registers while the epilogue drains tile i.  Tiles are 128 x 128; consecutive tile
+// ids share the X (activation) tile so the big operand is read from HBM once and hit in L2 by the CTAs working on
+// its other N-tiles.
 //
 // A second, deliberately simple SIMT kernel computes the same contraction from the same split operands
 // (reconstructing hi+lo in fp32); tests use it to cross-check the tensor-core path on the GPU.
@@ -16,35 +18,37 @@ namespace ct3 {
 namespace {
 
 constexpr int BM = 128, BN = 128, BK = 64;
-constexpr int ACC = 2;
 constexpr int TILE_A = BM * BK * 2;                    // 16 KiB (one 16-bit plane)
 constexpr int TILE_B = BN * BK * 2;                    // 16 KiB
-constexpr int EPI_WARPS = 16;                          // four warps per TMEM lane quarter, a quarter of the columns each
+constexpr int MMA_WARPS = 4;                           // one warpgroup: warps 0..3
+constexpr int TMA_WARP = 4;
+constexpr int EPI_WARP0 = 5;
+constexpr int EPI_WARPS = 4;                           // one warp per 32-row quarter (9 warps: 168 registers per thread)
 constexpr int CW = 16;                                 // epilogue chunk width (columns)
 constexpr int STG_WORDS = 32 * CW;                     // per-warp transpose buffer (rotated rows: conflict-free both ways)
-constexpr int MAX_STAGES = 6;
-// Per products-per-FLOP variant: which operand planes a stage holds and how deep the ring is (always 192 KiB).
-//   3: A hi|lo, W hi|lo (64 KiB x 3)   2: A hi, W hi|lo (48 KiB x 4)   1: A hi, W hi (32 KiB x 6)
+constexpr int MAX_STAGES = 4;
+// Per products-per-FLOP variant: which operand planes a stage holds and how deep the ring is (at most 128 KiB).
+//   3: A hi|lo, W hi|lo (64 KiB x 2)   2: A hi, W hi|lo (48 KiB x 2)   1: A hi, W hi (32 KiB x 4)
 template <int NPROD>
 struct Cfg {
   // NPROD == 4 / 5: 3 products + the LayerNorm-producer epilogue (raw split rows + partial statistics) / the
   // LayerNorm-consumer epilogue -- separate instantiations so that the default kernels do not carry their registers
-  // (compiled into every kernel they cost each GEMM 20-64 bytes of spills and ~7 % of its time)
   static constexpr int AP = NPROD >= 3 ? 2 : 1;
   static constexpr int BP = NPROD >= 2 ? 2 : 1;
   static constexpr int STAGE_BYTES = AP * TILE_A + BP * TILE_B;
-  static constexpr int STAGES = NPROD >= 3 ? 3 : (NPROD == 2 ? 4 : 6);
+  static constexpr int STAGES = NPROD >= 2 ? 2 : 4;
   static constexpr int OFF_B = AP * TILE_A;
 };
-constexpr int OFF_STG = 3 * 65536;                     // = STAGES * STAGE_BYTES of every variant
-static_assert(Cfg<1>::STAGES * Cfg<1>::STAGE_BYTES == OFF_STG && Cfg<2>::STAGES * Cfg<2>::STAGE_BYTES == OFF_STG &&
-              Cfg<3>::STAGES * Cfg<3>::STAGE_BYTES == OFF_STG && Cfg<4>::STAGES * Cfg<4>::STAGE_BYTES == OFF_STG &&
-              Cfg<5>::STAGES * Cfg<5>::STAGE_BYTES == OFF_STG, "ring size");
+constexpr int RING_BYTES = 2 * 65536;
+static_assert(Cfg<1>::STAGES * Cfg<1>::STAGE_BYTES <= RING_BYTES && Cfg<2>::STAGES * Cfg<2>::STAGE_BYTES <= RING_BYTES &&
+              Cfg<3>::STAGES * Cfg<3>::STAGE_BYTES <= RING_BYTES, "ring size");
+constexpr int ACC_LD = BN + 4;                         // fp32 accumulator tile [BM][ACC_LD]
+constexpr int OFF_ACC = RING_BYTES;
+constexpr int OFF_STG = OFF_ACC + BM * ACC_LD * 4;
 constexpr int OFF_BAR = OFF_STG + EPI_WARPS * STG_WORDS * 4;
 constexpr int SMEM_BYTES = OFF_BAR + 256 /*barriers*/ + 1024 /*align slack*/;
 static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-constexpr int THREADS = (2 + EPI_WARPS) * 32;
-constexpr uint32_t TMEM_COLS = ACC * BN;               // 256 columns (power of two)
+constexpr int THREADS = (MMA_WARPS + 1 + EPI_WARPS) * 32;
 
 __device__ __forceinline__ float apply_act(float x, int act) {
   if (act == 1) return gelu_erf(x);
@@ -52,7 +56,7 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   return x;
 }
 
-// Epilogue of one 32-row x 16-column chunk by one warp.  Phase 1 (lane = row, straight out of tcgen05.ld): bias /
+// Epilogue of one 32-row x 16-column chunk by one warp.  Phase 1 (lane = row, read from the accumulator tile): bias /
 // row-bias / activation, then the 16 output words of the row (16 fp32, or 8 packed-hi | 8 packed-lo bf16 pairs) go to
 // a per-warp staging buffer whose rows are rotated by row/2 words (conflict-free for both access patterns without
 // padding).  Phase 2 (lane = (row in a group of 8, 16-byte column group)): every warp instruction moves 8 rows x 64 B
@@ -179,37 +183,31 @@ gemm_split3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
   uint8_t* smem = smem_align1024(smem_raw);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* tfull_bar = empty_bar + MAX_STAGES;
-  uint64_t* tempty_bar = tfull_bar + ACC;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + ACC);
+  uint64_t* tfull_bar = empty_bar + MAX_STAGES;   // accumulator tile written (MMA warps -> epilogue)
+  uint64_t* tempty_bar = tfull_bar + 1;           // accumulator tile drained (epilogue -> MMA warps)
+  float* acc_tile = reinterpret_cast<float*>(smem + OFF_ACC);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmW);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], MMA_WARPS);
     }
-    for (int i = 0; i < ACC; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], EPI_WARPS * 32);
-    }
+    mbar_init(tfull_bar, MMA_WARPS);
+    mbar_init(tempty_bar, EPI_WARPS * 32);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int num_mt = (M + BM - 1) / BM;
   const int num_nt = N / BN;
   const int num_tiles = num_mt * num_nt;
   const int num_kb = Kpad / BK;
 
-  if (warp == 0) {
+  if (warp == TMA_WARP) {
     // ------------------------------------------------------------------ TMA producer
     if (elect_one()) {
       int stage = 0;
@@ -228,57 +226,45 @@ gemm_split3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (one thread)
-    if (elect_one()) {
-      const uint32_t idesc = umma_idesc_16(BM, BN, fp16 != 0);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);   // epilogue has drained this accumulator
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);          // TMA bytes have landed
-          tc_fence_after_sync();
-          const uint32_t s = smem_u32(smem + stage * STAGE_BYTES);
-          const uint32_t a_hi = s, a_lo = s + TILE_A, b_hi = s + C::OFF_B, b_lo = b_hi + TILE_B;
-#pragma unroll
-          for (int kk = 0; kk < BK / 16; ++kk) {
-            const uint32_t koff = kk * 32;  // 16 elements = 32 bytes inside the 128-byte swizzle atom
-            const uint64_t dah = umma_desc_sw128(a_hi + koff), dbh = umma_desc_sw128(b_hi + koff);
-            const uint32_t first = (kb | kk) != 0 ? 1u : 0u;
-            if (NPROD >= 3) {   // small terms first
-              umma_bf16(d_tmem, umma_desc_sw128(a_lo + koff), dbh, idesc, first);
-              umma_bf16(d_tmem, dah, umma_desc_sw128(b_lo + koff), idesc, 1u);
-              umma_bf16(d_tmem, dah, dbh, idesc, 1u);
-            } else if (NPROD == 2) {
-              umma_bf16(d_tmem, dah, umma_desc_sw128(b_lo + koff), idesc, first);
-              umma_bf16(d_tmem, dah, dbh, idesc, 1u);
-            } else {
-              umma_bf16(d_tmem, dah, dbh, idesc, first);
-            }
-          }
-          umma_commit(&empty_bar[stage]);              // frees the smem slot when these MMAs retire
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit(&tfull_bar[acc]);                  // accumulator complete -> epilogue
-        if (++acc == ACC) { acc = 0; acc_phase ^= 1u; }
+  } else if (warp < MMA_WARPS) {
+    // ------------------------------------------------------------------ MMA warpgroup
+    int stage = 0;
+    uint32_t phase = 0, acc_phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      float d0[BN / 2], d1[BN / 2];
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);          // TMA bytes have landed
+        wgmma_fence();
+        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+        if (fp16) mma_kblock<NPROD, BN, true>(d0, d1, sa, TILE_A, C::OFF_B, TILE_B, kb == 0);
+        else mma_kblock<NPROD, BN, false>(d0, d1, sa, TILE_A, C::OFF_B, TILE_B, kb == 0);
+        wgmma_commit();
+        wgmma_wait0(d0);
+        wgmma_wait0(d1);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);   // this warp's MMAs no longer read the slot
+        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
+      mbar_wait(tempty_bar, acc_phase ^ 1u);           // the epilogue has drained the previous tile
+      acc_store<BN>(d0, acc_tile, ACC_LD);
+      acc_store<BN>(d1, acc_tile + 64 * ACC_LD, ACC_LD);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(tfull_bar);
+      acc_phase ^= 1u;
     }
   } else {
     // ------------------------------------------------------------------ epilogue warps
-    const int quarter = warp & 3;        // TMEM lane quarter this warp may access (warp id % 4)
+    const int e = warp - EPI_WARP0;
+    const int quarter = e & 3;                         // 32-row quarter of the tile
     constexpr int CH = BN / CW / (EPI_WARPS / 4);      // 16-column chunks per warp
-    const int chunk0 = ((warp - 2) >> 2) * CH;
-    int acc = 0;
+    const int chunk0 = (e >> 2) * CH;
     uint32_t acc_phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int mt = tile / num_nt, nt = tile % num_nt;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after_sync();
+      mbar_wait(tfull_bar, acc_phase);
       const int row0 = mt * BM + quarter * 32;
-      uint32_t* stg = reinterpret_cast<uint32_t*>(smem + OFF_STG) + (warp - 2) * STG_WORDS;
+      uint32_t* stg = reinterpret_cast<uint32_t*>(smem + OFF_STG) + e * STG_WORDS;
+      const float* arow = acc_tile + (quarter * 32 + lane) * ACC_LD;
       float ln_mean = 0.f, ln_rstd = 1.f;
       if constexpr (NPROD == 5) {
         if (row0 + lane < M) ln_row_stats(epi.ln_part + (int64_t)(row0 + lane) * kLnParts * 2, epi.ln_eps, ln_mean, ln_rstd);
@@ -286,168 +272,13 @@ gemm_split3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
 #pragma unroll 1
       for (int chunk = chunk0; chunk < chunk0 + CH; ++chunk) {
         float v[CW];
-        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BN + chunk * CW);
-        tmem_ld16(taddr, v);
+        acc_row_ld<CW>(arow + chunk * CW, v);
         epilogue_chunk<NPROD == 4, NPROD == 5>(epi, M, N, row0, nt * BN + chunk * CW, lane, v, stg, ln_mean, ln_rstd);
       }
-      tc_fence_before_sync();
-      mbar_arrive(&tempty_bar[acc]);
-      if (++acc == ACC) { acc = 0; acc_phase ^= 1u; }
+      mbar_arrive(tempty_bar);
+      acc_phase ^= 1u;
     }
   }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// CTA-pair variant (tcgen05 cta_group::2).  With 128x128 tiles the tensor pipe stalls at ~55 %: every SM must
-// ingest 64 KiB of operands per 768 MMA cycles (83 B/cycle) while the L2->SM path delivers ~45 B/cycle (measured:
-// 12.7 TB/s chip-wide, profiles/).  A pair of SMs works on a 256 x BN tile instead: each CTA loads only ITS 128 rows
-// of X and ITS half (BN/2 rows) of W, one leader thread issues M=256 MMAs that read both shared memories and write
-// both TMEMs, so the bytes ingested per FLOP halve.  Both CTAs run the same producer / epilogue code on their own
-// 128 rows; barriers: full (leader, tx from both CTAs), empty + tmem_full (multicast commit to both),
-// tmem_empty (leader, remote arrives from the peer's epilogue warps).
-template <int BNP, int NPROD>
-__global__ void __launch_bounds__(THREADS, 1)
-gemm_split3_pair_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, int M,
-                        int N, int Kpad, int fp16, GemmEpilogue epi) {
-  using C = Cfg<NPROD>;
-  constexpr int STAGES = C::STAGES, STAGE_BYTES = C::STAGE_BYTES;
-  constexpr int TILE_BH = (BNP / 2) * BK * 2;                 // this CTA's half of the W tile, one plane
-  constexpr uint32_t TX_BYTES = 2u * ((uint32_t)C::AP * TILE_A + (uint32_t)C::BP * TILE_BH);   // both CTAs, all planes
-  constexpr uint32_t TCOLS = 512;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_align1024(smem_raw);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
-  uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* tfull_bar = empty_bar + MAX_STAGES;
-  uint64_t* tempty_bar = tfull_bar + ACC;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + ACC);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();       // 0 = leader
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmX);
-    tma_prefetch_desc(&tmW);
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < ACC; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 2 * EPI_WARPS);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_2sm(tmem_slot, TCOLS);
-  tc_fence_before_sync();
-  __syncthreads();
-  cluster_sync_all();                            // both CTAs: barriers initialised, TMEM allocated
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-
-  const int num_mp = ((M + BM - 1) / BM + 1) / 2;   // pairs of M-tiles
-  const int num_nt = N / BNP;
-  const int num_tiles = num_mp * num_nt;
-  const int num_kb = Kpad / BK;
-  const int first = blockIdx.x >> 1, step = gridDim.x >> 1;
-
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer (both CTAs)
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = first; tile < num_tiles; tile += step) {
-        const int mt = (tile / num_nt) * 2 + (int)rank, nt = tile % num_nt;
-        const int wrow = nt * BNP + (int)rank * (BNP / 2);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], TX_BYTES);
-          uint8_t* s = smem + stage * STAGE_BYTES;
-          tma_load_2d_2sm(s, &tmX, kb * BK, mt * BM, &full_bar[stage]);
-          if (C::AP == 2) tma_load_2d_2sm(s + TILE_A, &tmX, Kpad + kb * BK, mt * BM, &full_bar[stage]);
-          tma_load_2d_2sm(s + C::OFF_B, &tmW, kb * BK, wrow, &full_bar[stage]);
-          if (C::BP == 2) tma_load_2d_2sm(s + C::OFF_B + TILE_B, &tmW, Kpad + kb * BK, wrow, &full_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (leader CTA, one thread)
-    if (rank == 0 && elect_one()) {
-      const uint32_t idesc = umma_idesc_16(256, BNP, fp16 != 0);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int tile = first; tile < num_tiles; tile += step) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);   // both epilogues have drained this accumulator
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BNP);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);          // both CTAs' TMA bytes have landed
-          tc_fence_after_sync();
-          const uint32_t s = smem_u32(smem + stage * STAGE_BYTES);
-          const uint32_t a_hi = s, a_lo = s + TILE_A, b_hi = s + C::OFF_B, b_lo = b_hi + TILE_B;
-#pragma unroll
-          for (int kk = 0; kk < BK / 16; ++kk) {
-            const uint32_t koff = kk * 32;
-            const uint64_t dah = umma_desc_sw128(a_hi + koff), dbh = umma_desc_sw128(b_hi + koff);
-            const uint32_t first = (kb | kk) != 0 ? 1u : 0u;
-            if (NPROD >= 3) {
-              umma_bf16_2sm(d_tmem, umma_desc_sw128(a_lo + koff), dbh, idesc, first);
-              umma_bf16_2sm(d_tmem, dah, umma_desc_sw128(b_lo + koff), idesc, 1u);
-              umma_bf16_2sm(d_tmem, dah, dbh, idesc, 1u);
-            } else if (NPROD == 2) {
-              umma_bf16_2sm(d_tmem, dah, umma_desc_sw128(b_lo + koff), idesc, first);
-              umma_bf16_2sm(d_tmem, dah, dbh, idesc, 1u);
-            } else {
-              umma_bf16_2sm(d_tmem, dah, dbh, idesc, first);
-            }
-          }
-          umma_commit_2sm(&empty_bar[stage]);          // frees the stage in both CTAs
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit_2sm(&tfull_bar[acc]);              // accumulator complete -> both epilogues
-        if (++acc == ACC) { acc = 0; acc_phase ^= 1u; }
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue warps (both CTAs, own 128 rows)
-    const int quarter = warp & 3;
-    constexpr int CH = BNP / CW / (EPI_WARPS / 4);     // 16-column chunks per warp
-    const int chunk0 = ((warp - 2) >> 2) * CH;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = first; tile < num_tiles; tile += step) {
-      const int mt = (tile / num_nt) * 2 + (int)rank, nt = tile % num_nt;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after_sync();
-      const int row0 = mt * BM + quarter * 32;
-      uint32_t* stg = reinterpret_cast<uint32_t*>(smem + OFF_STG) + (warp - 2) * STG_WORDS;
-      float ln_mean = 0.f, ln_rstd = 1.f;
-      if constexpr (NPROD == 5) {
-        if (row0 + lane < M) ln_row_stats(epi.ln_part + (int64_t)(row0 + lane) * kLnParts * 2, epi.ln_eps, ln_mean, ln_rstd);
-      }
-#pragma unroll 1
-      for (int chunk = chunk0; chunk < chunk0 + CH; ++chunk) {
-        float v[CW];
-        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BNP + chunk * CW);
-        tmem_ld16(taddr, v);
-        epilogue_chunk<NPROD == 4, NPROD == 5>(epi, M, N, row0, nt * BNP + chunk * CW, lane, v, stg, ln_mean, ln_rstd);
-      }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(&tempty_bar[acc], 0);   // leader's barrier (local for the leader itself)
-      if (++acc == ACC) { acc = 0; acc_phase ^= 1u; }
-    }
-  }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  cluster_sync_all();                            // the pair retires together
-  if (warp == 1) tmem_dealloc_2sm(tmem_base, TCOLS);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -458,27 +289,29 @@ gemm_split3_pair_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
 // so one 128 x 144 output tile holds everything head h needs for the tracks of a row tile.  Token rows are
 // track-major (row = n*T + t): a tile starts at row mt*R with R = floor(128 / T) * T, i.e. it owns whole tracks
 // (the MMA still multiplies 128 rows; the rows past R belong to the next tile and are ignored).
-// cta_group::2 pairs as in gemm_split3_pair_kernel (256-row MMA, each CTA loads its 128 rows of X and 72 of the 144
-// weight rows).  Epilogue, per CTA on its own 128 rows: 2 independent groups of 4 warps (TMEM lane quarters) take
-// alternate tiles (group g owns accumulator g and its own K/V buffer), so two tiles are in their epilogue at once.
-// Per tile a thread (= row) reads q (+ bias) into registers, writes k and v (+ bias) to shared [row][k 48 | v 48] fp32,
-// releases the accumulator, and -- after the group's named barrier -- runs exact fp32 online-softmax attention of its
-// row against the T key rows of its track, then writes the 48 outputs as split bf16 straight into the
-// out-projection's operand buffer.
+// Three warpgroups: warps 0..3 MMA (wgmma m64n144k16 on both 64-row halves: 144 fp32 accumulators per thread),
+// warps 4..7 producer (warp 4 issues the TMA loads), warps 8..11 epilogue (thread = row of the tile).  setmaxnreg moves
+// registers from the producer warpgroup (40) to the other two (232 each) so that neither spills and the wgmmas are not
+// serialised for lack of registers.  The accumulator tile is written to shared memory [row][q 48 | k 48 |
+// v 48] fp32; each thread adds the bias (and the folded LayerNorm) to its row in place, keeping q in registers, and --
+// after the group's named barrier -- runs exact fp32 online-softmax attention of its row against the T key rows of its
+// track, then writes the 48 outputs as split bf16 straight into the out-projection's operand buffer.  The MMA
+// warpgroup computes the next tile in registers meanwhile.
 // The fp32 q|k|v tensor (4.6 KB per token) never reaches HBM and the separate attention launch disappears.
 namespace qa {
 constexpr int BNQ = 144;                               // q|k|v of one head
-constexpr int TILE_BQ = (BNQ / 2) * BK * 2;            // 9216 B: this CTA's 72 weight rows, one plane
-constexpr int STAGE = 2 * TILE_A + 2 * TILE_BQ;        // 51200 B
-constexpr int NSTAGE = 2;                              // the kernel is epilogue-bound: a shallow ring buys the second K/V buffer
-constexpr int KV_LD = 100;                             // floats per row of a K/V buffer (96 + 4: conflict-free float4)
-constexpr int KV_BYTES = BM * KV_LD * 4;               // 51200 per epilogue group
-constexpr int OFF_KV = NSTAGE * STAGE;                 // 102400
-constexpr int OFF_BARQ = OFF_KV + 2 * KV_BYTES;        // + 102400
+constexpr int TILE_BQ = BNQ * BK * 2;                  // 18432 B: the 144 weight rows, one plane
+constexpr int STAGE = 2 * TILE_A + 2 * TILE_BQ;        // 69632 B
+constexpr int NSTAGE = 2;
+constexpr int QACC_LD = BNQ + 4;                        // floats per row of the accumulator tile (conflict-free float4)
+constexpr int QOFF_ACC = NSTAGE * STAGE;
+constexpr int OFF_BARQ = QOFF_ACC + BM * QACC_LD * 4;
 constexpr int SMEM = OFF_BARQ + 256 + 1024;
-constexpr int EPIW = 8;
-constexpr int NTHREADS = (2 + EPIW) * 32;              // 320 threads (10 warps): up to 168 registers per thread
-constexpr int ACC_STRIDE = 256;                        // TMEM columns between the two accumulators
+constexpr int EPIW = 4;
+constexpr int QEPI_WARP0 = 8;
+constexpr int NTHREADS = 12 * 32;                      // 168 registers per thread at launch, rebalanced by setmaxnreg
+constexpr int REG_PRODUCER = 40, REG_COMPUTE = 232;    // 128 x (40 + 232 + 232) <= 384 x 168
+static_assert(128 * (REG_PRODUCER + 2 * REG_COMPUTE) <= NTHREADS * 168, "register budget");
 static_assert(SMEM <= 232448, "shared memory budget");
 }  // namespace qa
 
@@ -486,117 +319,94 @@ __global__ void __launch_bounds__(qa::NTHREADS, 1)
 gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, int M,
                           int Kpad, int T, int R, float scale_log2e, GemmEpilogue epi) {
   using namespace qa;
-  constexpr uint32_t TX_BYTES = 2u * (2u * TILE_A + 2u * TILE_BQ);
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_align1024(smem_raw);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + OFF_BARQ);
   uint64_t* empty_bar = full_bar + NSTAGE;
   uint64_t* tfull_bar = empty_bar + NSTAGE;
-  uint64_t* tempty_bar = tfull_bar + ACC;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + ACC);
-  float* kvs = reinterpret_cast<float*>(smem + OFF_KV);
+  uint64_t* tempty_bar = tfull_bar + 1;
+  float* acc = reinterpret_cast<float*>(smem + QOFF_ACC);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmW);
     for (int i = 0; i < NSTAGE; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], MMA_WARPS);
     }
-    for (int i = 0; i < ACC; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 2 * 4);        // one epilogue group (4 warps) per CTA of the pair
-    }
+    mbar_init(tfull_bar, MMA_WARPS);
+    mbar_init(tempty_bar, EPIW * 32);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc_2sm(tmem_slot, 512);
-  tc_fence_before_sync();
   __syncthreads();
-  cluster_sync_all();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int num_mt = (M + R - 1) / R;
-  const int num_mp = (num_mt + 1) / 2;
-  const int num_tiles = num_mp * kHeads;       // consecutive tiles = the 8 heads of one row-tile pair (X stays in L2)
+  const int num_tiles = num_mt * kHeads;       // consecutive tiles = the 8 heads of one row tile (X stays in L2)
   const int num_kb = Kpad / BK;
-  const int first = blockIdx.x >> 1, step = gridDim.x >> 1;
 
-  if (warp == 0) {
-    if (elect_one()) {
+  if (warp >= MMA_WARPS && warp < QEPI_WARP0) {
+    setmaxnreg_dec<REG_PRODUCER>();
+    if (warp == TMA_WARP && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = first; tile < num_tiles; tile += step) {
-        const int mt = (tile / kHeads) * 2 + (int)rank, h = tile % kHeads;
-        const int wrow = h * BNQ + (int)rank * (BNQ / 2);
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int mt = tile / kHeads, h = tile % kHeads;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1u);
-          if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], TX_BYTES);
+          mbar_arrive_expect_tx(&full_bar[stage], STAGE);
           uint8_t* s = smem + stage * STAGE;
-          tma_load_2d_2sm(s, &tmX, kb * BK, mt * R, &full_bar[stage]);
-          tma_load_2d_2sm(s + TILE_A, &tmX, Kpad + kb * BK, mt * R, &full_bar[stage]);
-          tma_load_2d_2sm(s + 2 * TILE_A, &tmW, kb * BK, wrow, &full_bar[stage]);
-          tma_load_2d_2sm(s + 2 * TILE_A + TILE_BQ, &tmW, Kpad + kb * BK, wrow, &full_bar[stage]);
+          tma_load_2d(s, &tmX, kb * BK, mt * R, &full_bar[stage]);
+          tma_load_2d(s + TILE_A, &tmX, Kpad + kb * BK, mt * R, &full_bar[stage]);
+          tma_load_2d(s + 2 * TILE_A, &tmW, kb * BK, h * BNQ, &full_bar[stage]);
+          tma_load_2d(s + 2 * TILE_A + TILE_BQ, &tmW, Kpad + kb * BK, h * BNQ, &full_bar[stage]);
           if (++stage == NSTAGE) { stage = 0; phase ^= 1u; }
         }
       }
     }
-  } else if (warp == 1) {
-    if (rank == 0 && elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(256, BNQ);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int tile = first; tile < num_tiles; tile += step) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * ACC_STRIDE);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after_sync();
-          const uint32_t s = smem_u32(smem + stage * STAGE);
-          const uint32_t a_hi = s, a_lo = s + TILE_A, b_hi = s + 2 * TILE_A, b_lo = b_hi + TILE_BQ;
-#pragma unroll
-          for (int kk = 0; kk < BK / 16; ++kk) {
-            const uint32_t koff = kk * 32;
-            const uint64_t dah = umma_desc_sw128(a_hi + koff), dbh = umma_desc_sw128(b_hi + koff);
-            umma_bf16_2sm(d_tmem, umma_desc_sw128(a_lo + koff), dbh, idesc, (kb | kk) != 0 ? 1u : 0u);
-            umma_bf16_2sm(d_tmem, dah, umma_desc_sw128(b_lo + koff), idesc, 1u);
-            umma_bf16_2sm(d_tmem, dah, dbh, idesc, 1u);
-          }
-          umma_commit_2sm(&empty_bar[stage]);
-          if (++stage == NSTAGE) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit_2sm(&tfull_bar[acc]);
-        if (++acc == ACC) { acc = 0; acc_phase ^= 1u; }
+  } else if (warp < MMA_WARPS) {
+    setmaxnreg_inc<REG_COMPUTE>();
+    int stage = 0;
+    uint32_t phase = 0, acc_phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      float d0[BNQ / 2], d1[BNQ / 2];
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        wgmma_fence();
+        mma_kblock<3, BNQ, false>(d0, d1, smem_u32(smem + stage * STAGE), TILE_A, 2 * TILE_A, TILE_BQ, kb == 0);
+        wgmma_commit();
+        wgmma_wait0(d0);
+        wgmma_wait0(d1);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        if (++stage == NSTAGE) { stage = 0; phase ^= 1u; }
       }
+      mbar_wait(tempty_bar, acc_phase ^ 1u);           // the epilogue is done with the previous tile's K/V
+      acc_store<BNQ>(d0, acc, QACC_LD);
+      acc_store<BNQ>(d1, acc + 64 * QACC_LD, QACC_LD);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(tfull_bar);
+      acc_phase ^= 1u;
     }
   } else {
-    const int quarter = warp & 3;
-    const int group = (warp - 2) >> 2;             // tiles alternate between the two groups; group g <-> accumulator g
-    const int r = quarter * 32 + lane;             // row of the tile = TMEM lane
+    setmaxnreg_inc<REG_COMPUTE>();
+    const int r = (warp - QEPI_WARP0) * 32 + lane;  // row of the tile
     const int tracks = R / T;
     const int jtrack = min(r / T, tracks - 1);     // rows past R are computed on a clamped track and never stored
-    float* kvg = kvs + group * (KV_BYTES / 4);
-    const float* kbase = kvg + (int64_t)jtrack * T * KV_LD;
-    const int bar_id = 1 + group;
-    int it = 0;
-    for (int tile = first; tile < num_tiles; tile += step, ++it) {
-      if ((it & 1) != group) continue;
-      const int acc = group;
-      const uint32_t acc_phase = (uint32_t)((it >> 1) & 1);
-      const int mt = (tile / kHeads) * 2 + (int)rank, h = tile % kHeads;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after_sync();
-      const uint32_t tlane = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * ACC_STRIDE);
+    const float* kbase = acc + (int64_t)jtrack * T * QACC_LD + kDh;
+    float* arow = acc + r * QACC_LD;
+    uint32_t acc_phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int mt = tile / kHeads, h = tile % kHeads;
+      mbar_wait(tfull_bar, acc_phase);
+      acc_phase ^= 1u;
       float ln_mean = 0.f, ln_rstd = 1.f;
       {
         const int64_t grow_ln = (int64_t)mt * R + r;
         if (epi.ln_part && grow_ln < M) ln_row_stats(epi.ln_part + grow_ln * kLnParts * 2, epi.ln_eps, ln_mean, ln_rstd);
       }
       float xq[kDh];
-      // k, v -> shared memory first, q (kept in registers for the attention) last
+      // k, v + bias back into the tile in place, q (kept in registers for the attention) last
 #pragma unroll
       for (int pi = 0; pi < 3; ++pi) {
         const int part = (pi + 1) % 3;   // 1 = k, 2 = v, 0 = q
@@ -605,7 +415,7 @@ gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
 #pragma unroll
         for (int c = 0; c < kDh / 16; ++c) {
           float v[16];
-          tmem_ld16(tlane + (uint32_t)(col0 + 16 * c), v);
+          acc_row_ld<16>(arow + col0 + 16 * c, v);
           const float4* b4 = reinterpret_cast<const float4*>(epi.bias + h * BNQ + col0 + 16 * c);
           if (epi.ln_part) {
             const float4* w4 = reinterpret_cast<const float4*>(epi.ln_wsum + h * BNQ + col0 + 16 * c);
@@ -627,15 +437,12 @@ gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
 #pragma unroll
           for (int i = 0; i < kDh; ++i) xq[i] = x[i];
         } else {
-          float4* dst = reinterpret_cast<float4*>(kvg + r * KV_LD + (part - 1) * kDh);
+          float4* dst = reinterpret_cast<float4*>(arow + col0);
 #pragma unroll
           for (int i = 0; i < kDh / 4; ++i) dst[i] = make_float4(x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
         }
       }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(&tempty_bar[acc], 0);   // accumulator drained (leader's barrier)
-      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");   // K/V of this tile are in shared memory
+      named_bar_sync(1, EPIW * 32);                  // K/V of this tile are final in shared memory
       {
         float m = -INFINITY, l = 0.f;
         float o[kDh];
@@ -649,7 +456,7 @@ gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
           for (int d4 = 0; d4 < kDh / 4; ++d4) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
-              const float4 kk = *reinterpret_cast<const float4*>(kbase + min(t0 + i, T - 1) * KV_LD + 4 * d4);
+              const float4 kk = *reinterpret_cast<const float4*>(kbase + min(t0 + i, T - 1) * QACC_LD + 4 * d4);
               sc[i] = fmaf(xq[4 * d4 + 0], kk.x, sc[i]);
               sc[i] = fmaf(xq[4 * d4 + 1], kk.y, sc[i]);
               sc[i] = fmaf(xq[4 * d4 + 2], kk.z, sc[i]);
@@ -670,7 +477,7 @@ gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
           for (int i = 0; i < 8; ++i) {
             const float pi = exp2f(sc[i] - mnew);      // 0 for the masked tail
             l += pi;
-            const float* vr = kbase + min(t0 + i, T - 1) * KV_LD + kDh;
+            const float* vr = kbase + min(t0 + i, T - 1) * QACC_LD + kDh;
 #pragma unroll
             for (int d4 = 0; d4 < kDh / 4; ++d4) {
               const float4 vv = *reinterpret_cast<const float4*>(vr + 4 * d4);
@@ -682,6 +489,7 @@ gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
           }
           m = mnew;
         }
+        mbar_arrive(tempty_bar);                     // this thread no longer reads the tile
         const int64_t grow = (int64_t)mt * R + r;
         if (r < R && grow < M) {
           const float inv = 1.0f / l;
@@ -697,14 +505,8 @@ gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
           }
         }
       }
-      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");   // K/V consumed: this group's next tile may overwrite
     }
   }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 1) tmem_dealloc_2sm(tmem_base, 512);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -825,41 +627,16 @@ bool encode_tensor_map(CUtensorMap* m, CUtensorMapDataType dtype, int rank, cons
 namespace {
 
 template <int NPROD>
-cudaError_t set_attrs() {
-  cudaError_t e = cudaFuncSetAttribute(gemm_split3_tc_kernel<NPROD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_split3_pair_kernel<256, NPROD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_split3_pair_kernel<192, NPROD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-  return e;
-}
-
-template <int NPROD>
-cudaError_t launch_tc(const GemmProblem& p, const CUtensorMap& tmX, const CUtensorMap& tmW, int bnp, int num_mt,
-                      int num_sms, cudaStream_t stream) {
-  if (bnp == 0) {
-    const int num_tiles = num_mt * (p.N / BN);
-    const int grid = num_tiles < num_sms ? num_tiles : num_sms;
-    gemm_split3_tc_kernel<NPROD><<<grid, THREADS, SMEM_BYTES, stream>>>(tmX, tmW, p.M, p.N, p.Kpad, p.fp16, p.epi);
-    return cudaGetLastError();
-  }
-  const int groups = ((num_mt + 1) / 2) * (p.N / bnp);
-  int pairs = num_sms / 2;
-  if (pairs > groups) pairs = groups;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(2 * pairs);
-  cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2;
-  at[0].val.clusterDim.y = 1;
-  at[0].val.clusterDim.z = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  cudaError_t e = (bnp == 256)
-      ? cudaLaunchKernelEx(&cfg, gemm_split3_pair_kernel<256, NPROD>, tmX, tmW, p.M, p.N, p.Kpad, p.fp16, p.epi)
-      : cudaLaunchKernelEx(&cfg, gemm_split3_pair_kernel<192, NPROD>, tmX, tmW, p.M, p.N, p.Kpad, p.fp16, p.epi);
+cudaError_t launch_tc(const GemmProblem& p, const CUtensorMap& tmX, const CUtensorMap& tmW, int num_mt, int num_sms,
+                      cudaStream_t stream) {
+  static DeviceOnce attr;
+  cudaError_t e = once_per_device(attr, [&] {
+    return cudaFuncSetAttribute(gemm_split3_tc_kernel<NPROD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+  });
   if (e != cudaSuccess) return e;
+  const int num_tiles = num_mt * (p.N / BN);
+  const int grid = num_tiles < num_sms ? num_tiles : num_sms;
+  gemm_split3_tc_kernel<NPROD><<<grid, THREADS, SMEM_BYTES, stream>>>(tmX, tmW, p.M, p.N, p.Kpad, p.fp16, p.epi);
   return cudaGetLastError();
 }
 
@@ -884,7 +661,7 @@ int gemm_qkv_time_attn_launch(const __nv_bfloat16* x_split, const __nv_bfloat16*
   const int R = (BM / T) * T;
   CUtensorMap tmX, tmW;
   if (!make_tmap(&tmX, x_split, (uint64_t)M, 2ull * Kpad) ||
-      !make_tmap(&tmW, w_heads, (uint64_t)(kHeads * qa::BNQ), 2ull * Kpad, (uint32_t)(qa::BNQ / 2))) {
+      !make_tmap(&tmW, w_heads, (uint64_t)(kHeads * qa::BNQ), 2ull * Kpad, (uint32_t)qa::BNQ)) {
     *err = "qkv_time_attn: cuTensorMapEncodeTiled failed";
     return (int)cudaErrorInvalidValue;
   }
@@ -893,10 +670,7 @@ int gemm_qkv_time_attn_launch(const __nv_bfloat16* x_split, const __nv_bfloat16*
     return cudaFuncSetAttribute(gemm_qkv_time_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, qa::SMEM);
   });
   if (e != cudaSuccess) { *err = "qkv_time_attn: cudaFuncSetAttribute failed"; return (int)e; }
-  const int num_mt = (M + R - 1) / R;
-  const int groups = ((num_mt + 1) / 2) * kHeads;
-  int pairs = num_sms / 2;
-  if (pairs > groups) pairs = groups;
+  const int num_tiles = ((M + R - 1) / R) * kHeads;
   GemmEpilogue epi;
   epi.bias = bias_heads;
   epi.out_split = att_split;
@@ -905,21 +679,8 @@ int gemm_qkv_time_attn_launch(const __nv_bfloat16* x_split, const __nv_bfloat16*
   epi.ln_part = ln_part;
   epi.ln_wsum = ln_wsum;
   epi.ln_eps = ln_eps;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(2 * pairs);
-  cfg.blockDim = dim3(qa::NTHREADS);
-  cfg.dynamicSmemBytes = qa::SMEM;
-  cfg.stream = stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2;
-  at[0].val.clusterDim.y = 1;
-  at[0].val.clusterDim.z = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  e = cudaLaunchKernelEx(&cfg, gemm_qkv_time_attn_kernel, tmX, tmW, M, Kpad, T, R,
-                         scale * 1.44269504088896340736f, epi);
-  if (e != cudaSuccess) return (int)e;
+  gemm_qkv_time_attn_kernel<<<num_tiles < num_sms ? num_tiles : num_sms, qa::NTHREADS, qa::SMEM, stream>>>(
+      tmX, tmW, M, Kpad, T, R, scale * 1.44269504088896340736f, epi);
   return (int)cudaGetLastError();
 }
 
@@ -957,36 +718,21 @@ int gemm_launch(const GemmProblem& p, int impl, int num_sms, cudaStream_t stream
     return (int)cudaGetLastError();
   }
   const int num_mt = (p.M + BM - 1) / BM;
-  // CTA pairs (cta_group::2) once there is enough work to fill the machine with 256-row tiles
-  int bnp = 0;
-  if (impl == 0 && num_mt >= 2 * num_sms) bnp = (p.N % 256 == 0) ? 256 : ((p.N % 192 == 0) ? 192 : 0);
   CUtensorMap tmX, tmW;
   if (!make_tmap(&tmX, p.x_split, (uint64_t)p.M, (uint64_t)x_ld) ||
-      !make_tmap(&tmW, p.w_split, (uint64_t)p.N, 2ull * p.Kpad, bnp ? (uint32_t)(bnp / 2) : 128u)) {
+      !make_tmap(&tmW, p.w_split, (uint64_t)p.N, 2ull * p.Kpad)) {
     *err = "gemm: cuTensorMapEncodeTiled failed";
     return (int)cudaErrorInvalidValue;
-  }
-  static DeviceOnce attr_set;
-  {
-    cudaError_t e = once_per_device(attr_set, [&] {
-      cudaError_t e = set_attrs<3>();
-      if (e == cudaSuccess) e = set_attrs<4>();
-      if (e == cudaSuccess) e = set_attrs<5>();
-      if (e == cudaSuccess) e = set_attrs<2>();
-      if (e == cudaSuccess) e = set_attrs<1>();
-      return e;
-    });
-    if (e != cudaSuccess) { *err = "gemm: cudaFuncSetAttribute(max dynamic smem) failed"; return (int)e; }
   }
   if (p.epi.ln_part && (p.products != 3 || p.epi.raw_split)) {
     *err = "gemm: the LayerNorm-consumer epilogue needs 3 products and cannot be combined with raw_split";
     return (int)cudaErrorInvalidValue;
   }
-  cudaError_t e = (p.products == 3 && p.epi.raw_split) ? launch_tc<4>(p, tmX, tmW, bnp, num_mt, num_sms, stream)
-                : (p.products == 3 && p.epi.ln_part) ? launch_tc<5>(p, tmX, tmW, bnp, num_mt, num_sms, stream)
-                : p.products == 3 ? launch_tc<3>(p, tmX, tmW, bnp, num_mt, num_sms, stream)
-                : p.products == 2 ? launch_tc<2>(p, tmX, tmW, bnp, num_mt, num_sms, stream)
-                                  : launch_tc<1>(p, tmX, tmW, bnp, num_mt, num_sms, stream);
+  cudaError_t e = (p.products == 3 && p.epi.raw_split) ? launch_tc<4>(p, tmX, tmW, num_mt, num_sms, stream)
+                : (p.products == 3 && p.epi.ln_part) ? launch_tc<5>(p, tmX, tmW, num_mt, num_sms, stream)
+                : p.products == 3 ? launch_tc<3>(p, tmX, tmW, num_mt, num_sms, stream)
+                : p.products == 2 ? launch_tc<2>(p, tmX, tmW, num_mt, num_sms, stream)
+                                  : launch_tc<1>(p, tmX, tmW, num_mt, num_sms, stream);
   return (int)e;
 }
 

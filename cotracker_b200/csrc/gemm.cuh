@@ -3,7 +3,7 @@
 //   Y[M, N] = epilogue( X[M, K] * W[N, K]^T )      (nn.Linear; blocks.py:61-67, :375-377, cotracker.py:409-412)
 //
 // Operands are stored "split": X_split[M, 2*Kpad] = [hi(Kpad) | lo(Kpad)] bf16 with x = hi + lo,
-// likewise W_split[N, 2*Kpad].  The tensor cores accumulate hi*hi + lo*hi + hi*lo in fp32 (TMEM),
+// likewise W_split[N, 2*Kpad].  The tensor cores accumulate hi*hi + lo*hi + hi*lo in fp32 (registers),
 // i.e. all first-order terms of the fp32 product (rel. error ~2^-17 per product, vs 2^-11 for TF32).
 #pragma once
 #include "common.cuh"
@@ -59,7 +59,7 @@ struct GemmProblem {
 bool encode_tensor_map(CUtensorMap* m, CUtensorMapDataType dtype, int rank, const void* base, const uint64_t* dims,
                        const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle);
 
-// 0 = tcgen05 path, 1 = SIMT verification path.  Returns cudaError_t as int (0 = ok).
+// 0 = wgmma path, 1 = SIMT verification path.  Returns cudaError_t as int (0 = ok).
 int gemm_launch(const GemmProblem& p, int impl, int num_sms, cudaStream_t stream, const char** err);
 
 // Fused q|k|v projection + per-track time attention (gemm.cu, gemm_qkv_time_attn_kernel).

@@ -118,13 +118,14 @@ struct AttnParams {
 };
 cudaError_t launch_attention(const AttnParams& p, cudaStream_t s);   // exact-fp32 SIMT (verification)
 
-// ---- attention_p2v.cu : point <- virtual cross attention (Lk == 64 keys) on tcgen05 ----------------------------------
-bool attention_p2v_supported(const AttnParams& p);
-cudaError_t launch_attention_p2v(const AttnParams& p, cudaStream_t s);
 
 // ---- attention_tc.cu : tensor-core (mma.sync split-bf16x3) production path ------------------------
 constexpr int kAttnMaxSplits = 32;
 size_t attention_partial_bytes(int num_seq, int Lq, int max_splits);
 cudaError_t launch_attention_tc(const AttnParams& p, bool per_warp, float* part, int num_sms, cudaStream_t s);
+
+// ---- attention_p2v.cu : point <- virtual cross attention (Lk == 64 keys) on wgmma --------------------------------------
+bool attention_p2v_supported(const AttnParams& p);
+cudaError_t launch_attention_p2v(const AttnParams& p, cudaStream_t s);
 
 }  // namespace ct3

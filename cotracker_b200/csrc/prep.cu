@@ -116,7 +116,7 @@ cudaError_t launch_pyramid_pools(int T, int H4, int W4, float* pyr, cudaStream_t
   for (int l = 1; l < kL; ++l) {
     const int64_t total = (int64_t)T * lay.h[l] * lay.w[l] * (kD / 4);
     if (total == 0) continue;
-    const int blocks = (int)((total + 255) / 256 > 148 * 16 ? 148 * 16 : (total + 255) / 256);
+    const int blocks = (int)((total + 255) / 256 > 132 * 16 ? 132 * 16 : (total + 255) / 256);
     avgpool2_channels_last_kernel<<<blocks, 256, 0, s>>>(pyr + lay.off[l - 1], pyr + lay.off[l], T, lay.h[l - 1],
                                                         lay.w[l - 1], lay.h[l], lay.w[l]);
   }
@@ -130,7 +130,7 @@ cudaError_t launch_prepare_pyramid(const float* fmaps, int T, int H4, int W4, fl
   for (int l = 1; l < kL; ++l) {
     const int64_t total = (int64_t)T * lay.h[l] * lay.w[l] * (kD / 4);
     if (total == 0) continue;
-    const int blocks = (int)((total + 255) / 256 > 148 * 16 ? 148 * 16 : (total + 255) / 256);
+    const int blocks = (int)((total + 255) / 256 > 132 * 16 ? 132 * 16 : (total + 255) / 256);
     avgpool2_channels_last_kernel<<<blocks, 256, 0, s>>>(pyr + lay.off[l - 1], pyr + lay.off[l], T, lay.h[l - 1],
                                                         lay.w[l - 1], lay.h[l], lay.w[l]);
   }

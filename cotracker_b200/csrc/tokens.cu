@@ -235,7 +235,7 @@ affine_fold_kernel(const float* __restrict__ w, const float* __restrict__ b, con
 
 inline int grid_for(int64_t total, int block) {
   int64_t b = (total + block - 1) / block;
-  const int64_t cap = 148 * 32;
+  const int64_t cap = 132 * 32;
   return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 

@@ -303,7 +303,7 @@ def split_rows(x: torch.Tensor, Kpad: int, fp16: bool = False) -> torch.Tensor:
 
 def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], act: int = 0, products: int = 3,
            fp16: bool = False) -> torch.Tensor:
-    """Y = act(x w^T + b) through the tcgen05 GEMM engine; x [M,K], w [Nout,K] fp32.  products / fp16: the
+    """Y = act(x w^T + b) through the wgmma GEMM engine; x [M,K], w [Nout,K] fp32.  products / fp16: the
     precision switches (3 = split x split, 2 = x_hi x split w, 1 = x_hi x w_hi; bf16 or fp16 planes)."""
     M, K = x.shape
     Nout = w.shape[0]

@@ -8,7 +8,7 @@ Jaccard (AJ) at 1/2/4/8/16 px.  `EvaluationPredictor` wraps a cotracker_b200 off
 reference's benchmark code drives it: one query point at a time with an 8x8 local grid and a 5x5 global grid as
 helper tracks (single_point=True, the TAP-Vid protocol), or all queries jointly.  The model behind it is the same
 CUDA path as everywhere else (libct3_b200.so); SIFT helper points (sift_size > 0) are not provided.
-With no datasets or checkpoints in this environment the harness is exercised by scoring the B200 tracks against
+With no datasets or checkpoints in this environment the harness is exercised by scoring the CUDA tracks against
 the reference's tracks on synthetic clips (tests/test_evaluation.py): identical outputs score 1.0 everywhere.
 """
 from __future__ import annotations
@@ -87,7 +87,7 @@ class EvaluationPredictor(torch.nn.Module):
                  num_uniformly_sampled_pts: int = 0, n_iters: int = 6, local_extent: int = 50) -> None:
         super().__init__()
         if sift_size > 0:
-            raise NotImplementedError("SIFT helper points are not provided by the B200 build")
+            raise NotImplementedError("SIFT helper points are not provided by this build")
         self.grid_size = grid_size
         self.local_grid_size = local_grid_size
         self.single_point = single_point

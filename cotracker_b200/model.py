@@ -8,7 +8,7 @@ state-dict keys (SURVEY.md Appendix B), so `load_state_dict(strict=True)` of the
 
 The nn.Module tree below is a *parameter container*: nothing executes through PyTorch modules.  The CNN
 encoder, L2-normalisation + pyramid, support sampling, correlation sampling, the correlation MLP, the whole
-EfficientUpdateFormer and the delta heads run as hand-written sm_100a CUDA behind the C ABI
+EfficientUpdateFormer and the delta heads run as hand-written sm_90a CUDA behind the C ABI
 (`cotracker_b200.engine`).  Inference only; B must be 1 (as in the reference, SURVEY.md §0).
 """
 from __future__ import annotations
@@ -149,7 +149,7 @@ class CoTrackerThreeBase(nn.Module):
         """video [T,3,H,W] already scaled to [-1,1] -> L2-normalised channels-last 4-level pyramid (flat fp32).
 
         The whole BasicEncoder (reference blocks.py:141-219) runs in libct3_b200.so (csrc/enc_front.cu + the GEMM
-        engine): conv1 as fp32 SIMT, every other convolution as split-bf16x3 tcgen05 GEMMs, channels-last.  The
+        engine): conv1 as fp32 SIMT, every other convolution as split-bf16x3 wgmma GEMMs, channels-last.  The
         library walks the clip in chunks of 16 frames itself (`chunk` = the reference's fmaps_chunk_size only bounds
         memory there and has no numerical effect: the encoder is strictly per frame)."""
         dev = video.device
@@ -173,7 +173,7 @@ class CoTrackerThreeBase(nn.Module):
             raise ValueError("CoTracker3 inference requires B == 1 (the reference fails for B > 1 as well)")
         assert H % self.stride == 0 and W % self.stride == 0
         if not video.is_cuda:
-            raise engine.EngineError("cotracker_b200 runs on CUDA only; move the module and inputs to a B200")
+            raise engine.EngineError("cotracker_b200 runs on CUDA only; move the module and inputs to a GPU")
 
     def _refine(self, pyr, H4, W4, support, track_valid, coords, vis, conf, iters):
         T, N, _ = coords.shape

@@ -3,7 +3,7 @@
     torch.hub.load("<this repo>", "cotracker3_offline", source="local", pretrained=False)
 
 `pretrained=True` downloads the released CoTracker3 checkpoints (same URLs as the reference) and loads them
-with strict=True; the CoTracker2 entry points are outside the B200 hot path and raise NotImplementedError.
+with strict=True; the CoTracker2 entry points are outside the H100 hot path and raise NotImplementedError.
 """
 import torch
 
@@ -39,7 +39,7 @@ def cotracker3_online(*, pretrained: bool = True, **kwargs):
 
 
 def _v2(*args, **kwargs):
-    raise NotImplementedError("CoTracker2 entry points are not provided by the B200 hot-path build")
+    raise NotImplementedError("CoTracker2 entry points are not provided by the H100 hot-path build")
 
 
 cotracker2 = cotracker2_online = cotracker2v1 = cotracker2v1_online = _v2

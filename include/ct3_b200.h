@@ -1,7 +1,7 @@
 /*
  * ct3_b200.h -- C ABI of libct3_b200.so: the CoTracker3 iterative update loop
  * (correlation sampling + correlation MLP + EfficientUpdateFormer + delta heads)
- * as hand-written sm_100a CUDA.
+ * as hand-written sm_90a CUDA.
  *
  * This is the drop-in boundary for the reference's inference hot path
  * (citations are file:line inside facebookresearch/co-tracker):
@@ -73,7 +73,7 @@ const char* ct3_last_error(void);
 /* Debug/verification options ("gemm", "corr", "attn": 0 = tensor-core path (default),
  * 1 = SIMT fp32 verification kernel used by the tests to cross-check; "corr" = 2 forces the
  * sample-then-correlate tensor-core kernel that otherwise only serves pyramids with a level below 8x8;
- * "attn" = 2 runs the point<-virtual attention on the mma.sync kernel instead of the tcgen05 one, for A/B). */
+ * "attn" = 2 runs the point<-virtual attention on the mma.sync kernel instead of the wgmma one, for A/B). */
 int ct3_set_option(const char* name, int value);
 int ct3_get_option(const char* name, int* value);
 /* Precision switches of the correlation branch ("prec.corr", "prec.fc1": tensor-core products per FLOP, 3 | 2 | 1;
@@ -156,7 +156,7 @@ int ct3_update_loop(const void* packed, const float* pyr, int H4, int W4, const 
                     size_t workspace_bytes, ct3_stream_t stream);
 
 /* ---- live profiler (bench.py roofline): CUDA events around every launch of the library, summed per
- * kernel category: 0 corr_sample, 1 gemm (tcgen05), 2 attention, 3 layernorm, 4 misc.
+ * kernel category: 0 corr_sample, 1 gemm (wgmma), 2 attention, 3 layernorm, 4 misc.
  * ct3_profile_enable(1) clears and starts recording; ct3_profile_read synchronises and sums. */
 int ct3_profile_enable(int on);
 int ct3_profile_read(double ms[7], int launches[7], double* gemm_flops);
@@ -199,7 +199,7 @@ int ct3_updateformer(const void* packed, const float* x, int T, int N, float* de
 /* ---- the whole CNN encoder (BasicEncoder.forward, blocks.py:190-219; normalise + pyramid,
  * cotracker3_offline.py:92-117) on the tensor-core engine, channels-last ------------------------------------
  * frames [T,3,H,W] fp32 already scaled to [-1,1] (cotracker3_offline.py:63) -> pyr (ct3_pyramid_layout(T, H/4, W/4)).
- * conv1 7x7/2 runs as fp32 SIMT, every other convolution as split-bf16x3 tcgen05 GEMMs (3x3 stride-1: implicit GEMM
+ * conv1 7x7/2 runs as fp32 SIMT, every other convolution as split-bf16x3 wgmma GEMMs (3x3 stride-1: implicit GEMM
  * over TMA-shifted NHWC boxes; strided ones: gather + GEMM); InstanceNorm statistics in fp64.
  * Weight tensors in the order of ct3_encoder_weight_name() (state-dict keys below `fnet.`). */
 int ct3_encoder_num_weight_tensors(void);

@@ -146,3 +146,33 @@ def compare(got, want, tol_px=1e-3, tol_logit=1e-3):
             tol = tol_px if ("coords" in k or "tracks" in k) else tol_logit
             assert err <= tol, f"{k}: max abs err {err:.3e} > {tol:.1e}"
     return report
+
+
+def stage_inputs():
+    """Seeded inputs of the stage-level comparisons with the reference (tests/test_oracle_vs_reference.py); the
+    reference's outputs on them are pinned in tests/golden/reference_stages.npz (oracle/make_reference_stages.py)."""
+    from cotracker_b200.synthetic import random_queries, texture_video
+    x = {"uf_x": torch.randn(1, 33, 7, 1110, generator=torch.Generator().manual_seed(1)) * 2}
+    g = torch.Generator().manual_seed(2)
+    T, N, H, W = 3, 11, 12, 16
+    x["corr_fm"] = torch.randn(1, T, 128, H, W, generator=g)
+    x["corr_coords"] = torch.rand(1 * T, N, 2, generator=g) * torch.tensor([W + 4.0, H + 4.0]) - 2.0   # some outside
+    x["corr_sup"] = torch.randn(1, 49, N, 128, generator=g)
+    g = torch.Generator().manual_seed(3)
+    T, N, H, W = 4, 9, 12, 16
+    x["sup_fm"] = torch.randn(1, T, 128, H, W, generator=g)
+    x["sup_qf"] = torch.randint(0, T, (1, N), generator=g)
+    x["sup_qc"] = torch.rand(1, N, 2, generator=g) * torch.tensor([W - 1.0, H - 1.0])
+    x["posenc_x"] = torch.randn(5, 3, 4, generator=torch.Generator().manual_seed(4)) * 0.1
+    x["enc_v"] = texture_video(2, 64, 96, seed=5)[0] / 255 * 2 - 1
+    x["fwd_video"] = texture_video(5, 64, 96, seed=6)
+    x["fwd_q"] = random_queries(9, 5, 64, 96, seed=7)
+    return x
+
+
+def reference_golden(name, key):
+    """A value pinned from the reference: the full array, or (flat indices, values) of its seeded sample."""
+    with np.load(os.path.join(GOLDEN_DIR, name + ".npz")) as z:
+        if key + "__idx" in z.files:
+            return torch.from_numpy(z[key + "__idx"].astype(np.int64)), torch.from_numpy(z[key])
+        return None, torch.from_numpy(z[key])

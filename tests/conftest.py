@@ -10,16 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
-
-
-@pytest.fixture(scope="session")
-def reference_path():
-    """Path of the unmodified reference checkout (build container only)."""
-    p = os.environ.get("COTRACKER_REFERENCE", "/root/reference")
-    if not os.path.isdir(os.path.join(p, "cotracker")):
-        pytest.skip("reference checkout not present on this machine")
-    return p
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 # product defaults of the per-thread library options (api.cu); a test that changes one must put it back

@@ -1,12 +1,14 @@
-"""Evaluation harness (SURVEY 8(f4)): the numpy TAP-Vid metrics against the LIVE reference implementation (build
-container) and, on the GPU, EvaluationPredictor against the reference's EvaluationPredictor output pinned in a golden."""
-import sys
+"""Evaluation harness (SURVEY 8(f4)): the numpy TAP-Vid metrics against the reference implementation's values pinned
+in tests/golden/reference_host.npz and, on the GPU, EvaluationPredictor against the reference's EvaluationPredictor output pinned in a golden."""
+import os
 
 import numpy as np
 import pytest
 import torch
 
 from cotracker_b200.evaluation import EvaluationPredictor, points_on_a_grid, tapvid_metrics
+
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def _random_problem(seed, b=2, n=17, t=11):
@@ -41,30 +43,30 @@ def test_hand_computed_case():
 
 
 @pytest.mark.parametrize("mode", ["first", "strided"])
-def test_metrics_match_live_reference(reference_path, mode):
-    sys.path.insert(0, reference_path)
-    from cotracker.evaluation.core.eval_utils import compute_tapvid_metrics
-    for seed in range(4):
-        args = _random_problem(seed)
-        want = compute_tapvid_metrics(*args, mode)
-        got = tapvid_metrics(*args, mode)
-        assert set(want) == set(got)
-        for k in want:
-            assert np.allclose(got[k], want[k], rtol=0, atol=1e-12), k
+def test_metrics_match_live_reference(mode):
+    """Against the reference's compute_tapvid_metrics on the same problems (tests/golden/reference_host.npz)."""
+    with np.load(os.path.join(GOLDEN, "reference_host.npz")) as z:
+        for seed in range(4):
+            prefix = f"tapvid_{mode}_{seed}_"
+            want = {k[len(prefix):]: z[k] for k in z.files if k.startswith(prefix)}
+            got = tapvid_metrics(*_random_problem(seed), mode)
+            assert set(want) == set(got)
+            for k in want:
+                assert np.allclose(got[k], want[k], rtol=0, atol=1e-12), k
 
 
-def test_grid_with_centre_matches_live_reference(reference_path):
-    sys.path.insert(0, reference_path)
-    from cotracker.models.core.model_utils import get_points_on_a_grid
-    for size, extent, centre in ((8, (50, 50), (120.5, 77.25)), (5, (384, 512), None), (1, (384, 512), None)):
-        assert torch.equal(points_on_a_grid(size, extent, centre), get_points_on_a_grid(size, extent, centre))
+def test_grid_with_centre_matches_live_reference():
+    with np.load(os.path.join(GOLDEN, "reference_host.npz")) as z:
+        for i, (size, extent, centre) in enumerate(((8, (50, 50), (120.5, 77.25)), (5, (384, 512), None),
+                                                    (1, (384, 512), None))):
+            assert torch.equal(points_on_a_grid(size, extent, centre), torch.from_numpy(z[f"grid_{i}"]))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("single_point", [True, False])
 def test_evaluation_predictor_matches_reference_golden(single_point):
     """tests/golden/eval_predictor.npz: the reference's EvaluationPredictor on a seeded clip (oracle/make_golden.py);
-    tracks within 1e-3 px, and the TAP-Vid metrics of B200-vs-reference tracks are exactly 1."""
+    tracks within 1e-3 px, and the TAP-Vid metrics of CUDA-vs-reference tracks are exactly 1."""
     from cases import load_golden
     from cotracker_b200.build import build_cotracker
     from oracle.make_golden import eval_case_inputs

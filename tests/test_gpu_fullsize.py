@@ -2,7 +2,7 @@
 here, so parity is carried by size-independent properties of the path:
   * determinism           -- two runs of the same call are bit-identical (no atomics / racy reductions anywhere)
   * duplicated queries    -- the same query listed twice yields the same track (the virtual-token coupling is symmetric)
-  * tensor-core vs SIMT   -- the production kernels (tcgen05 GEMM pairs, tcgen05 correlation, mma attention) against the
+  * tensor-core vs SIMT   -- the production kernels (wgmma GEMMs, wgmma correlation, mma attention) against the
                              exact-fp32 SIMT verification kernels on the same inputs, within the 1e-3 px budget
   * query-frame identity  -- predictor output at the query frame is the query itself and visible (reference :173-185)
 """

@@ -26,7 +26,7 @@ def _rel_err(got, want):
 @pytest.mark.parametrize("impl", [0, 1])
 @pytest.mark.parametrize("M,K,N", [(128, 64, 128), (300, 384, 384), (1000, 2401, 384), (257, 1110, 384),
                                    (640, 1536, 384), (4100, 384, 1536), (129, 384, 256), (64, 384, 1152),
-                                   (38000, 384, 384), (40100, 1110, 256)])   # >= 296 M-tiles: 2-CTA cluster path (odd tile count)
+                                   (38000, 384, 384), (40100, 1110, 256)])   # many tiles per persistent CTA, odd tile count
 def test_linear_matches_fp64(eng, impl, M, K, N):
     g = torch.Generator().manual_seed(M * 7 + K)
     x = torch.randn(M, K, generator=g)
@@ -219,9 +219,9 @@ def test_updateformer_stage(eng, impl):
     assert err < 2e-4 * max(scale, 1.0), (err, scale)
 
 
-# 0: product kernels (fused tcgen05 time attention, tcgen05 + TMA point<-virtual attention for more than 64 points,
+# 0: product kernels (fused wgmma time attention, wgmma + TMA point<-virtual attention for more than 64 points,
 #    mma.sync kernels for the other space patterns), 1: exact-fp32 SIMT cross-check,
-# 2: like 0 with the mma.sync kernel for point<-virtual too (the kernel attention_p2v.cu replaced)
+# 2: like 0 with the mma.sync kernel for point<-virtual too
 @pytest.mark.parametrize("attn", [0, 1, 2])
 @pytest.mark.parametrize("N,T", [(70, 6), (600, 20), (130, 40), (1030, 16), (129, 5), (3, 2)])
 def test_updateformer_attention_shapes(eng, attn, N, T):
@@ -318,7 +318,7 @@ def test_update_loop_vs_oracle(eng, impl, H4, W4):
 
 
 def test_update_loop_cluster_gemm_vs_simt_at_scale(eng):
-    """N=2400, T=16: every big GEMM takes the 2-CTA multicast path; the SIMT fp32 GEMM is the on-GPU yardstick."""
+    """N=2400, T=16: every big GEMM runs many tiles per persistent CTA; the SIMT fp32 GEMM is the on-GPU yardstick."""
     sd = _amplified_sd(seed=9, head_gain=10.0, vis_gain=100.0)
     T, N, H4, W4, iters = 16, 2400, 48, 64, 2
     fmaps = _pyramid_case(T, H4, W4, seed=6)

@@ -5,6 +5,7 @@ import re
 import subprocess
 import sys
 
+import numpy as np
 import pytest
 import torch
 
@@ -80,17 +81,15 @@ def test_grid_queries_match_reference_contract():
     assert get_points_on_a_grid(1, (384, 512)).tolist() == [[[256.0, 192.0]]]
 
 
-def test_grid_and_time_embedding_match_live_reference(reference_path):
-    sys.path.insert(0, reference_path)
-    from cotracker.models.core.model_utils import get_points_on_a_grid as ref_grid
-    from cotracker.models.core.embeddings import get_1d_sincos_pos_embed_from_grid
+def test_grid_and_time_embedding_match_live_reference():
+    """Against the reference's get_points_on_a_grid / sincos embedding (tests/golden/reference_host.npz)."""
     from cotracker_b200.model import sincos_time_embedding
     from cotracker_b200.predictor import get_points_on_a_grid
-    for size in (1, 5, 30):
-        assert torch.equal(get_points_on_a_grid(size, (384, 512)), ref_grid(size, (384, 512)))
-    for L in (16, 60):
-        ref = get_1d_sincos_pos_embed_from_grid(1110, torch.linspace(0, L - 1, L).reshape(1, L, 1)[0])
-        assert torch.equal(sincos_time_embedding(1110, L), ref)
+    with np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_host.npz")) as z:
+        for i, size in ((2, 1), (1, 5), (3, 30)):
+            assert torch.equal(get_points_on_a_grid(size, (384, 512)), torch.from_numpy(z[f"grid_{i}"]))
+        for L in (16, 60):
+            assert torch.equal(sincos_time_embedding(1110, L), torch.from_numpy(z[f"sincos_{L}"]))
 
 
 def test_shard_clips():

@@ -42,7 +42,7 @@ def corr_stage():
 def model_cases():
     sd = seeded_state_dict(11, offline=True, window_len=60, head_gain=10.0, vis_gain=100.0)
     video = texture_video(4, 256, 288, seed=3)
-    queries = random_queries(80, 4, 256, 288, seed=4)   # > 64 points: the tcgen05 point<-virtual kernel runs
+    queries = random_queries(80, 4, 256, 288, seed=4)   # > 64 points: point<-virtual attention over many tiles
     with torch.no_grad():
         want_c, want_v, _ = O.offline_forward(sd, video, queries, iters=2)
     model = build_cotracker(None, offline=True, window_len=60).eval()
