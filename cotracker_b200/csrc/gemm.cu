@@ -1,10 +1,12 @@
 // gemm.cu -- split-bf16x3 linear layers on the Hopper tensor cores (wgmma).
 //
-// Persistent warp-specialised kernel, one CTA per SM:
+// Persistent warp-specialised kernel, one CTA per SM, four warpgroups:
 //   warps 0..3  : MMA warpgroup   (wgmma m64n128k16 on both 64-row halves of the tile, 3 MMAs per k16 step:
 //                                  lo*hi, hi*lo, hi*hi; fp32 accumulators in registers)
-//   warp 4      : TMA producer    (cp.async.bulk.tensor, 128B-swizzled K-major tiles, ring of 2-4 stages)
-//   warps 5..8  : epilogue        (bias / row-bias / GELU / residual -> fp32 and/or split-bf16 stores)
+//   warp 4      : TMA producer    (cp.async.bulk.tensor, 128B-swizzled K-major tiles, ring of 2-4 stages); warps 5..7
+//                                  only hand their registers to the MMA warpgroup (setmaxnreg)
+//   warps 8..15 : epilogue        (bias / row-bias / GELU / residual -> fp32 and/or split-bf16 stores); two warps per
+//                                  32-row quarter, so a tile drains in half the time of one warp per quarter
 // The accumulator tile goes from the MMA registers to the epilogue through one fp32 tile in shared memory; the MMA
 // warpgroup computes tile i+1 in registers while the epilogue drains tile i.  Tiles are 128 x 128; consecutive tile
 // ids share the X (activation) tile so the big operand is read from HBM once and hit in L2 by the CTAs working on
@@ -22,8 +24,8 @@ constexpr int TILE_A = BM * BK * 2;                    // 16 KiB (one 16-bit pla
 constexpr int TILE_B = BN * BK * 2;                    // 16 KiB
 constexpr int MMA_WARPS = 4;                           // one warpgroup: warps 0..3
 constexpr int TMA_WARP = 4;
-constexpr int EPI_WARP0 = 5;
-constexpr int EPI_WARPS = 4;                           // one warp per 32-row quarter (9 warps: 168 registers per thread)
+constexpr int EPI_WARP0 = 8;                           // warps 5..7 of the producer warpgroup stay idle
+constexpr int EPI_WARPS = 8;                           // two warps per 32-row quarter, each 64 columns
 constexpr int CW = 16;                                 // epilogue chunk width (columns)
 constexpr int STG_WORDS = 32 * CW;                     // per-warp transpose buffer (rotated rows: conflict-free both ways)
 constexpr int MAX_STAGES = 4;
@@ -48,7 +50,11 @@ constexpr int OFF_STG = OFF_ACC + BM * ACC_LD * 4;
 constexpr int OFF_BAR = OFF_STG + EPI_WARPS * STG_WORDS * 4;
 constexpr int SMEM_BYTES = OFF_BAR + 256 /*barriers*/ + 1024 /*align slack*/;
 static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-constexpr int THREADS = (MMA_WARPS + 1 + EPI_WARPS) * 32;
+constexpr int THREADS = (EPI_WARP0 + EPI_WARPS) * 32;  // 4 warpgroups: 128 registers per thread at launch
+// setmaxnreg moves registers from the producer warpgroup to the MMA warpgroup (2 x 64 fp32 accumulators per thread);
+// the epilogue warpgroups keep the launch budget
+constexpr int REG_TMA = 40, REG_MMA = 216, REG_EPI = 65536 / THREADS;
+static_assert(128 * (REG_TMA + REG_MMA + 2 * REG_EPI) <= 65536, "register budget");
 
 __device__ __forceinline__ float apply_act(float x, int act) {
   if (act == 1) return gelu_erf(x);
@@ -207,9 +213,10 @@ gemm_split3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
   const int num_tiles = num_mt * num_nt;
   const int num_kb = Kpad / BK;
 
-  if (warp == TMA_WARP) {
+  if (warp >= MMA_WARPS && warp < EPI_WARP0) {
     // ------------------------------------------------------------------ TMA producer
-    if (elect_one()) {
+    setmaxnreg_dec<REG_TMA>();
+    if (warp == TMA_WARP && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -228,6 +235,7 @@ gemm_split3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
     }
   } else if (warp < MMA_WARPS) {
     // ------------------------------------------------------------------ MMA warpgroup
+    setmaxnreg_inc<REG_MMA>();
     int stage = 0;
     uint32_t phase = 0, acc_phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
