@@ -218,11 +218,22 @@ struct Workspace {
   float* row_bias;        // [T, 384]
   float* att_part;        // split-K partials of the virtual<-point attention
   __nv_bfloat16* pyr_split;  // split-bf16 copy of the pyramid (corr_tc2.cu); null when H4 == 0
+  int32_t* groups;        // device group table of a grouped call (GroupPlan); null when G == 1
   size_t total;
 };
-Workspace carve(void* base, int T, int N, int H4 = 0, int W4 = 0) {
+// split-K slots of the virtual<-point partials: a group of n tracks splits at most min(32, ceil(n/64)/2) ways
+// (attention_tc_splits), so G groups of N tracks in all need at most (N + 63 G)/128 slots beyond one group's 32
+int partial_slots(int N, int G) {
+  if (G == 1) return kAttnMaxSplits;
+  const int64_t s = kAttnMaxSplits + ((int64_t)N + 63LL * G) / 128;
+  return (int)(s < (int64_t)kAttnMaxSplits * G ? s : (int64_t)kAttnMaxSplits * G);
+}
+// int32 entries of the group table: offsets [G+1] | all [G] | split [G] | slot [G] | small [G] | tiles [2 * max tiles]
+int64_t group_table_ints(int N, int G) { return G == 1 ? 0 : (int64_t)5 * G + 1 + 2 * ((int64_t)N / 128 + G); }
+
+Workspace carve(void* base, int T, int N, int H4 = 0, int W4 = 0, int G = 1) {
   Workspace w;
-  const size_t R = (size_t)(N + kV) * T, Rp = (size_t)N * T, Rv = (size_t)kV * T, Mc = Rp * kL;
+  const size_t R = (size_t)(N + (size_t)kV * G) * T, Rp = (size_t)N * T, Rv = (size_t)kV * G * T, Mc = Rp * kL;
   uint8_t* p = reinterpret_cast<uint8_t*>(base);
   size_t off = 0;
   auto take = [&](size_t bytes) { uint8_t* r = p + off; off = align_up(off + bytes, 1024); return r; };
@@ -238,10 +249,11 @@ Workspace carve(void* base, int T, int N, int H4 = 0, int W4 = 0) {
   w.vqkv = (float*)take(Rv * 3 * kC * 4);
   w.hmid = (__nv_bfloat16*)take(R * 2 * kMlpHid * 2);
   w.row_bias = (float*)take((size_t)T * kC * 4);
-  w.att_part = (float*)take(attention_partial_bytes(T, kV, kAttnMaxSplits));
+  w.att_part = (float*)take(attention_partial_bytes(T, kV, partial_slots(N, G)));
   w.pyr_split = nullptr;
   if (H4 > 0 && W4 > 0 && corr_patch_supported(T, H4, W4))
     w.pyr_split = (__nv_bfloat16*)take((size_t)pyramid_layout(T, H4, W4).total * 4);
+  w.groups = G > 1 ? (int32_t*)take((size_t)group_table_ints(N, G) * 4) : nullptr;
   w.total = off;
   return w;
 }
@@ -301,6 +313,93 @@ int run_attention(Runner& R, const Workspace& W, const AttnParams& a, bool per_w
   return (int)launch_attention_tc(a, per_warp, W.att_part, num_sms(), R.s);
 }
 
+// Track groups of a grouped call (ct3_update_loop_groups): G contiguous track ranges, each with its own kV virtual
+// tokens at rows (N + kV*g + i)*T + t.  G == 1 is the plain call (no table; every kernel indexes as it always did).
+// For G > 1 the host builds the table below, uploads it into the workspace in stream order, and each space attention
+// runs over (group, frame) sequences, choosing per group what a standalone call on that group's tracks would.
+struct GroupPlan {
+  int G = 1, max_n = 0;
+  const int32_t *off = nullptr, *all = nullptr, *split = nullptr, *slot = nullptr, *small = nullptr, *tile = nullptr;
+  int n_small = 0, n_tiles = 0, split_max = 1, split_slots = 0;
+};
+
+int plan_groups(GroupPlan& gp, const int32_t* sizes, int G, int T, int N, int32_t* dev, cudaStream_t s) {
+  gp.G = G;
+  if (G == 1) return 0;
+  std::vector<int32_t> h((size_t)group_table_ints(N, G), 0);
+  int32_t* off = h.data();
+  int32_t *all = off + G + 1, *split = all + G, *slot = split + G, *small = slot + G, *tile = small + G;
+  const int nsm = num_sms();
+  for (int g = 0; g < G; ++g) {
+    const int n = sizes[g];
+    off[g + 1] = off[g] + n;
+    if (n > gp.max_n) gp.max_n = n;
+    all[g] = g;
+    // virtual <- point: the split-K count of a standalone call (T sequences of kV queries over n keys)
+    split[g] = attention_tc_splits(T, kV, n, nsm);
+    if (split[g] > 1) {
+      slot[g] = gp.split_slots;
+      gp.split_slots += split[g];
+      if (split[g] > gp.split_max) gp.split_max = split[g];
+    }
+    // point <- virtual: a standalone call runs more than kV tracks on the wgmma kernel, fewer on mma.sync (run_attention)
+    if (n > kV) {
+      for (int n0 = off[g]; n0 < off[g + 1]; n0 += 128, ++gp.n_tiles) {
+        tile[2 * gp.n_tiles] = g;
+        tile[2 * gp.n_tiles + 1] = n0;
+      }
+    } else {
+      small[gp.n_small++] = g;
+    }
+  }
+  if (gp.split_slots > partial_slots(N, G)) return fail(CT3_EINVAL, "split-K partials exceed the workspace%s");
+  CK(launch_upload_i32(dev, h.data(), (int)h.size(), s), "upload group table");
+  gp.off = dev;
+  gp.all = dev + (all - off);
+  gp.split = dev + (split - off);
+  gp.slot = dev + (slot - off);
+  gp.small = dev + (small - off);
+  gp.tile = dev + (tile - off);
+  return 0;
+}
+
+// One space attention of a block (cotracker.py:510-517) over every group.  `a` describes it for one group of N tracks
+// (sequence = frame); q_pts / k_pts tell which side holds the point tokens.
+int space_attention(Runner& R, const Workspace& W, const GroupPlan& gp, AttnParams a, bool q_pts, bool k_pts) {
+  if (gp.G == 1) return run_attention(R, W, a, false);
+  const int T = a.num_seq, n_all = a.Lq;
+  a.goff = gp.off;
+  a.frames = T;
+  a.q_grp_stride = q_pts ? 0 : (int64_t)kV * a.q_tok_stride;
+  a.k_grp_stride = k_pts ? 0 : (int64_t)kV * a.k_tok_stride;
+  a.Lq = q_pts ? gp.max_n : kV;
+  a.Lk = k_pts ? gp.max_n : kV;
+  AttnParams b = a;
+  b.gl = gp.all;
+  b.num_seq = T * gp.G;
+  if (g_opt_attn == 1) return (int)launch_attention(b, R.s);
+  if (!q_pts) {   // virtual <- point (split-K per group) and virtual self attention
+    if (k_pts) { b.gsplit = gp.split; b.gslot = gp.slot; b.split_max = gp.split_max; b.split_slots = gp.split_slots; }
+    return (int)launch_attention_tc(b, false, W.att_part, num_sms(), R.s);
+  }
+  // point <- virtual
+  if (gp.n_small > 0) {
+    b.gl = gp.small;
+    b.num_seq = T * gp.n_small;
+    b.Lq = kV;
+    if (int rc = (int)launch_attention_tc(b, false, W.att_part, num_sms(), R.s)) return rc;
+  }
+  if (gp.n_tiles > 0) {
+    AttnParams c = a;
+    c.gtile = gp.tile;
+    c.tiles = gp.n_tiles;
+    c.Lq = n_all;
+    c.Lk = kV * gp.G;
+    return (int)launch_attention_p2v(c, R.s);
+  }
+  return 0;
+}
+
 // x += to_out(attn(...)); x += mlp(LN(x))   for the rows [row0, row0+rows) of the token buffer
 int mlp_half(Runner& R, const Workspace& W, const Block& b, int64_t row0, int rows) {
   float* x = W.tokens + row0 * kC;
@@ -313,12 +412,12 @@ int mlp_half(Runner& R, const Workspace& W, const Block& b, int64_t row0, int ro
 }
 
 // EfficientUpdateFormer body on W.tokens (point rows already hold input_transform output) -- cotracker.py:486-524
-int transformer_body(Runner& R, const Workspace& W, int T, int N) {
+int transformer_body(Runner& R, const Workspace& W, int T, int N, const GroupPlan& gp) {
   const Layout& L = R.L;
-  const int Rp = N * T, Rv = kV * T, Rall = Rp + Rv;
+  const int Rp = N * T, Rv = kV * gp.G * T, Rall = Rp + Rv;
   const float scale = 1.0f / sqrtf((float)kDh);
   const uint8_t* pk = R.pk;
-  RUNC(CAT_MISC, launch_init_virtual(W.tokens, reinterpret_cast<const float*>(pk + L.virt), T, N, R.s));
+  RUNC(CAT_MISC, launch_init_virtual(W.tokens, reinterpret_cast<const float*>(pk + L.virt), T, N, gp.G, R.s));
   float* vtok = W.tokens + (int64_t)Rp * kC;
   __nv_bfloat16* ln_p = W.ln;
   __nv_bfloat16* ln_v = W.ln + (int64_t)Rp * 2 * kC;
@@ -346,7 +445,7 @@ int transformer_body(Runner& R, const Workspace& W, int T, int N) {
         a.q = W.qkv; a.q_ld = 3 * kC; a.q_col = 0;
         a.kv = W.qkv; a.kv_ld = 3 * kC; a.k_col = kC; a.v_col = 2 * kC;
         a.out = W.att; a.out_ld = 2 * kC; a.lo_off = kC;
-        a.num_seq = N + kV; a.Lq = T; a.Lk = T;
+        a.num_seq = N + kV * gp.G; a.Lq = T; a.Lk = T;
         a.q_seq_stride = T; a.q_tok_stride = 1; a.k_seq_stride = T; a.k_tok_stride = 1;
         a.scale = scale;
         RUNC(CAT_ATTN, run_attention(R, W, a, true));
@@ -368,7 +467,7 @@ int transformer_body(Runner& R, const Workspace& W, int T, int N) {
       a.num_seq = T; a.Lq = kV; a.Lk = N;
       a.q_seq_stride = 1; a.q_tok_stride = T; a.k_seq_stride = 1; a.k_tok_stride = T;
       a.scale = scale;
-      RUNC(CAT_ATTN, run_attention(R, W, a, false));
+      RUNC(CAT_ATTN, space_attention(R, W, gp, a, false, true));
       RUNC(-1, R.gemm(att_v, b.out, Rv, Runner::to_f32(vtok, kC, true)));
       if (int rc = mlp_half(R, W, b, Rp, Rv)) return rc;
     }
@@ -383,7 +482,7 @@ int transformer_body(Runner& R, const Workspace& W, int T, int N) {
       a.num_seq = T; a.Lq = kV; a.Lk = kV;
       a.q_seq_stride = 1; a.q_tok_stride = T; a.k_seq_stride = 1; a.k_tok_stride = T;
       a.scale = scale;
-      RUNC(CAT_ATTN, run_attention(R, W, a, false));
+      RUNC(CAT_ATTN, space_attention(R, W, gp, a, false, false));
       RUNC(-1, R.gemm(att_v, b.out, Rv, Runner::to_f32(vtok, kC, true)));
       if (int rc = mlp_half(R, W, b, Rp, Rv)) return rc;
     }
@@ -401,7 +500,7 @@ int transformer_body(Runner& R, const Workspace& W, int T, int N) {
       a.num_seq = T; a.Lq = N; a.Lk = kV;
       a.q_seq_stride = 1; a.q_tok_stride = T; a.k_seq_stride = 1; a.k_tok_stride = T;
       a.scale = scale;
-      RUNC(CAT_ATTN, run_attention(R, W, a, false));
+      RUNC(CAT_ATTN, space_attention(R, W, gp, a, true, false));
       RUNC(-1, R.gemm(att_p, b.out, Rp, Runner::to_f32(W.tokens, kC, true)));
       if (int rc = mlp_half(R, W, b, 0, Rp)) return rc;
     }
@@ -438,7 +537,7 @@ int transformer_body_fold(Runner& R, const Workspace& W, int T, int N) {
   const int Rp = N * T, Rv = kV * T, Rall = Rp + Rv;
   const float scale = 1.0f / sqrtf((float)kDh);
   const uint8_t* pk = R.pk;
-  RUNC(CAT_MISC, launch_init_virtual(W.tokens, reinterpret_cast<const float*>(pk + L.virt), T, N, R.s));
+  RUNC(CAT_MISC, launch_init_virtual(W.tokens, reinterpret_cast<const float*>(pk + L.virt), T, N, 1, R.s));
   float* vtok = W.tokens + (int64_t)Rp * kC;
   __nv_bfloat16* raw_p = W.traw;
   __nv_bfloat16* raw_v = W.traw + (int64_t)Rp * 2 * kC;
@@ -519,11 +618,35 @@ int transformer_body_fold(Runner& R, const Workspace& W, int T, int N) {
   return 0;
 }
 
-int check_TN(int T, int N) {
+int check_TN(int T, int N, int G = 1) {
   if (T < 1 || N < 1) return fail(CT3_EINVAL, "T and N must be >= 1%s");
-  if ((int64_t)(N + kV) * T * 3 * kC >= (int64_t)1 << 40) return fail(CT3_EINVAL, "problem too large%s");
+  if (G < 1 || G > N) return fail(CT3_EINVAL, "G must be in [1, N]%s");
+  if (((int64_t)N + (int64_t)kV * G) * T * 3 * kC >= (int64_t)1 << 40) return fail(CT3_EINVAL, "problem too large%s");
   return 0;
 }
+
+// group arguments of the grouped entry points; N < 0: the sizes define N (ct3_updateformer_groups)
+int check_groups(const int32_t* sizes, int G, int N, int* total) {
+  if (!sizes) return fail(CT3_EINVAL, "null group_sizes_host%s");
+  if (G < 1) return fail(CT3_EINVAL, "G must be >= 1%s");
+  int64_t sum = 0;
+  for (int g = 0; g < G; ++g) {
+    if (sizes[g] < 1) return fail(CT3_EINVAL, "every group size must be >= 1%s");
+    sum += sizes[g];
+  }
+  if (sum > (int64_t)1 << 30) return fail(CT3_EINVAL, "problem too large%s");
+  if (N >= 0 && sum != N) return fail(CT3_EINVAL, "group sizes must sum to N%s");
+  if (G > 1 && (g_opt[OPT_FUSE] == 2 || g_opt_attn == 2))
+    return fail(CT3_EUNSUPPORTED, "grouped calls do not support fuse = 2 or attn = 2%s");
+  *total = (int)sum;
+  return 0;
+}
+
+int update_loop(const void* packed, const float* pyr, int H4, int W4, const float* support, const uint8_t* track_valid,
+                float* coords, float* vis, float* conf, const float* time_emb, int T, int N, const int32_t* sizes,
+                int G, int iters, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+int updateformer(const void* packed, const float* x, int T, int N, const int32_t* sizes, int G, float* delta,
+                 void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
 }  // namespace
 
@@ -713,11 +836,15 @@ int ct3_profile_read(double* ms, int* launches, double* gemm_flops) {
 }
 
 int ct3_workspace_bytes(int T, int N, int H4, int W4, size_t* out_bytes) {
+  return ct3_workspace_bytes_groups(T, N, 1, H4, W4, out_bytes);
+}
+
+int ct3_workspace_bytes_groups(int T, int N, int G, int H4, int W4, size_t* out_bytes) {
   if (!out_bytes) return fail(CT3_EINVAL, "null out_bytes%s");
-  if (int rc = check_TN(T, N)) return rc;
+  if (int rc = check_TN(T, N, G)) return rc;
   if ((H4 != 0 || W4 != 0))
     if (int rc = ct3_pyramid_layout(T, H4, W4, nullptr, nullptr, nullptr, nullptr)) return rc;
-  *out_bytes = carve(nullptr, T, N, H4, W4).total;
+  *out_bytes = carve(nullptr, T, N, H4, W4, G).total;
   return 0;
 }
 
@@ -786,17 +913,53 @@ int ct3_linear_prec(const void* x_split, const void* w_split, const float* bias,
 int ct3_update_loop(const void* packed, const float* pyr, int H4, int W4, const float* support,
                     const uint8_t* track_valid, float* coords, float* vis, float* conf, const float* time_emb,
                     int T, int N, int iters, void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+  const int32_t one = N;
+  return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, &one, 1, iters,
+                     workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int ct3_update_loop_groups(const void* packed, const float* pyr, int H4, int W4, const float* support,
+                           const uint8_t* track_valid, float* coords, float* vis, float* conf, const float* time_emb,
+                           int T, int N, int iters, void* workspace, size_t workspace_bytes, ct3_stream_t stream,
+                           const int32_t* group_sizes_host, int G) {
+  return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, group_sizes_host, G,
+                     iters, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int ct3_updateformer(const void* packed, const float* x, int T, int N, float* delta, void* workspace,
+                     size_t workspace_bytes, ct3_stream_t stream) {
+  const int32_t one = N;
+  return updateformer(packed, x, T, N, &one, 1, delta, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int ct3_updateformer_groups(const void* packed, const float* x, int T, const int32_t* group_sizes_host, int G,
+                            float* delta, void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+  return updateformer(packed, x, T, -1, group_sizes_host, G, delta, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+}  // extern "C"
+
+namespace {
+
+int update_loop(const void* packed, const float* pyr, int H4, int W4, const float* support, const uint8_t* track_valid,
+                float* coords, float* vis, float* conf, const float* time_emb, int T, int N, const int32_t* sizes,
+                int G, int iters, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   if (!packed || !pyr || !support || !coords || !vis || !conf || !time_emb || !workspace)
     return fail(CT3_EINVAL, "null argument%s");
   if (int rc = check_TN(T, N)) return rc;
+  int total = 0;
+  if (int rc = check_groups(sizes, G, N, &total)) return rc;
+  if (int rc = check_TN(T, N, G)) return rc;
   if (iters < 0) return fail(CT3_EINVAL, "iters must be >= 0%s");
   if (int rc = ct3_pyramid_layout(T, H4, W4, nullptr, nullptr, nullptr, nullptr)) return rc;
   if ((uintptr_t)workspace & 255) return fail(CT3_EINVAL, "workspace must be 256-byte aligned%s");
-  const Workspace W = carve(workspace, T, N, H4, W4);
+  const Workspace W = carve(workspace, T, N, H4, W4, G);
   if (workspace_bytes < W.total) return fail(CT3_ENOSPC, "workspace too small%s");
   const Layout& L = layout();
-  Runner R{reinterpret_cast<const uint8_t*>(packed), L, (cudaStream_t)stream, g_opt_gemm};
+  Runner R{reinterpret_cast<const uint8_t*>(packed), L, stream, g_opt_gemm};
   const uint8_t* pk = R.pk;
+  GroupPlan gp;
+  if (int rc = plan_groups(gp, sizes, G, T, N, W.groups, R.s)) return rc;
   const int Rp = N * T, Mc = Rp * kL;
   // split-bf16 copy of the window's pyramid: the TMA source of the correlation kernel, made once per call
   const Prec pr = effective_prec(W.pyr_split != nullptr, T, H4, W4);
@@ -833,7 +996,7 @@ int ct3_update_loop(const void* packed, const float* pyr, int H4, int W4, const 
       if (fold_enabled(R, T)) { e.raw_split = W.traw; e.stat_part = W.tstat; }
       RUNC(-1, R.gemm(W.xs, L.in_tr, Rp, e));
     }
-    if (int rc = fold_enabled(R, T) ? transformer_body_fold(R, W, T, N) : transformer_body(R, W, T, N)) return rc;
+    if (int rc = fold_enabled(R, T) ? transformer_body_fold(R, W, T, N) : transformer_body(R, W, T, N, gp)) return rc;
     // (v) heads + state update
     RUNC(CAT_MISC, launch_heads(W.tokens, reinterpret_cast<const float*>(pk + L.heads_w),
                      reinterpret_cast<const float*>(pk + L.heads_b), coords, vis, conf, nullptr, T, N, R.s));
@@ -841,29 +1004,36 @@ int ct3_update_loop(const void* packed, const float* pyr, int H4, int W4, const 
   return 0;
 }
 
-int ct3_updateformer(const void* packed, const float* x, int T, int N, float* delta, void* workspace,
-                     size_t workspace_bytes, ct3_stream_t stream) {
+int updateformer(const void* packed, const float* x, int T, int N, const int32_t* sizes, int G, float* delta,
+                 void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   if (!packed || !x || !delta || !workspace) return fail(CT3_EINVAL, "null argument%s");
-  if (int rc = check_TN(T, N)) return rc;
+  if (N >= 0)
+    if (int rc = check_TN(T, N)) return rc;
+  int total = 0;
+  if (int rc = check_groups(sizes, G, N, &total)) return rc;
+  N = total;
+  if (int rc = check_TN(T, N, G)) return rc;
   if ((uintptr_t)workspace & 255) return fail(CT3_EINVAL, "workspace must be 256-byte aligned%s");
-  const Workspace W = carve(workspace, T, N);
+  const Workspace W = carve(workspace, T, N, 0, 0, G);
   if (workspace_bytes < W.total) return fail(CT3_ENOSPC, "workspace too small%s");
   const Layout& L = layout();
-  Runner R{reinterpret_cast<const uint8_t*>(packed), L, (cudaStream_t)stream, g_opt_gemm};
+  Runner R{reinterpret_cast<const uint8_t*>(packed), L, stream, g_opt_gemm};
   const int Rp = N * T;
+  GroupPlan gp;
+  if (int rc = plan_groups(gp, sizes, G, T, N, W.groups, R.s)) return rc;
   RUNC(CAT_MISC, launch_split_rows(x, Rp, kX, kXPad, /*perm_x*/ 1, W.xs, 0, R.s));
   {
     GemmEpilogue e = Runner::to_f32(W.tokens, kC, false);
     if (fold_enabled(R, T)) { e.raw_split = W.traw; e.stat_part = W.tstat; }
     RUNC(-1, R.gemm(W.xs, L.in_tr, Rp, e));
   }
-  if (int rc = fold_enabled(R, T) ? transformer_body_fold(R, W, T, N) : transformer_body(R, W, T, N)) return rc;
+  if (int rc = fold_enabled(R, T) ? transformer_body_fold(R, W, T, N) : transformer_body(R, W, T, N, gp)) return rc;
   RUNC(CAT_MISC, launch_heads(W.tokens, reinterpret_cast<const float*>(R.pk + L.heads_w),
                    reinterpret_cast<const float*>(R.pk + L.heads_b), nullptr, nullptr, nullptr, delta, T, N, R.s));
   return 0;
 }
 
-}  // extern "C"
+}  // namespace
 
 // ------------------------------------------------------------------------------------------------
 // encoder tail (conv2 -> InstanceNorm -> ReLU -> conv3 -> L2-normalise -> pyramid), see enc_tail.cu

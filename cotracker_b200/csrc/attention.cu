@@ -5,6 +5,7 @@
 //     v <- p  : sequence = frame,  Lq = 64, Lk = N        q rows i*T + s (virtual), k rows j*T + s (points)
 //     v self  : sequence = frame,  Lq = Lk = 64
 //     p <- v  : sequence = frame,  Lq = N,  Lk = 64
+// In a grouped call the space patterns run per (group, frame) sequence over that group's rows (seq_rows).
 // One physical token layout (track-major) serves both orders: the reference's two permute().contiguous()
 // copies per space block (cotracker.py:504,520) disappear into the row strides.
 // Attention proper is ~2 % of the block FLOPs (SURVEY.md 8a); it runs exact fp32 flash-style (online softmax)
@@ -25,15 +26,18 @@ attention_kernel(AttnParams p) {
   __shared__ float Vs[KC * KLD];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int h = blockIdx.y, s = blockIdx.x;
+  const SeqRows sr = seq_rows(p, s);
+  const int Lq = sr.Lq, Lk = sr.Lk;
+  if ((int)blockIdx.z * WARPS * RQ >= Lq) return;   // grouped: this sequence is shorter than the longest one
   const int q0 = (blockIdx.z * WARPS + warp) * RQ;
 
   float q[RQ][kDh];
   float m[RQ], l[RQ], o0[RQ], o1[RQ];
 #pragma unroll
   for (int r = 0; r < RQ; ++r) {
-    const int qi = min(q0 + r, p.Lq - 1);
+    const int qi = min(q0 + r, Lq - 1);
     const float4* qp = reinterpret_cast<const float4*>(
-        p.q + ((int64_t)s * p.q_seq_stride + (int64_t)qi * p.q_tok_stride) * p.q_ld + p.q_col + h * kDh);
+        p.q + (sr.q0 + (int64_t)qi * p.q_tok_stride) * p.q_ld + p.q_col + h * kDh);
 #pragma unroll
     for (int d4 = 0; d4 < kDh / 4; ++d4) {
       const float4 v = __ldg(qp + d4);
@@ -42,13 +46,13 @@ attention_kernel(AttnParams p) {
     m[r] = -INFINITY; l[r] = 0.f; o0[r] = 0.f; o1[r] = 0.f;
   }
 
-  for (int kc0 = 0; kc0 < p.Lk; kc0 += KC) {
+  for (int kc0 = 0; kc0 < Lk; kc0 += KC) {
     // stage K and V rows of this chunk (zero-filled past Lk)
     for (int idx = threadIdx.x; idx < KC * (kDh / 4); idx += WARPS * 32) {
       const int j = idx / (kDh / 4), d4 = idx % (kDh / 4);
       float4 kv = make_float4(0.f, 0.f, 0.f, 0.f), vv = kv;
-      if (kc0 + j < p.Lk) {
-        const float* base = p.kv + ((int64_t)s * p.k_seq_stride + (int64_t)(kc0 + j) * p.k_tok_stride) * p.kv_ld + h * kDh;
+      if (kc0 + j < Lk) {
+        const float* base = p.kv + (sr.k0 + (int64_t)(kc0 + j) * p.k_tok_stride) * p.kv_ld + h * kDh;
         kv = __ldg(reinterpret_cast<const float4*>(base + p.k_col) + d4);
         vv = __ldg(reinterpret_cast<const float4*>(base + p.v_col) + d4);
       }
@@ -60,9 +64,9 @@ attention_kernel(AttnParams p) {
     __syncthreads();
 #pragma unroll 1
     for (int sub = 0; sub < KC / 32; ++sub) {
-      if (kc0 + sub * 32 >= p.Lk) break;  // warp-uniform
+      if (kc0 + sub * 32 >= Lk) break;  // warp-uniform
       const int j = sub * 32 + lane;
-      const bool valid = kc0 + j < p.Lk;
+      const bool valid = kc0 + j < Lk;
       float sc[RQ];
 #pragma unroll
       for (int r = 0; r < RQ; ++r) sc[r] = 0.f;
@@ -104,9 +108,9 @@ attention_kernel(AttnParams p) {
 #pragma unroll
   for (int r = 0; r < RQ; ++r) {
     const int qi = q0 + r;
-    if (qi >= p.Lq) continue;
+    if (qi >= Lq) continue;
     const float inv = 1.0f / l[r];
-    __nv_bfloat16* orow = p.out + ((int64_t)s * p.q_seq_stride + (int64_t)qi * p.q_tok_stride) * p.out_ld + h * kDh;
+    __nv_bfloat16* orow = p.out + (sr.q0 + (int64_t)qi * p.q_tok_stride) * p.out_ld + h * kDh;
     const bf16pair a = split_bf16(o0[r] * inv);
     orow[lane] = a.hi;
     orow[p.lo_off + lane] = a.lo;

@@ -18,6 +18,9 @@
 // A first version with one global load / store stream per thread (= per row, rows T*ld*4 bytes apart) was bound by the
 // LSU request rate (252 us per call at N=6400, T=16; long_scoreboard 5.6 per issue); TMA moves whole rows instead.
 // Two CTAs are resident per SM (113 KiB of shared memory each = the 228 KiB of the SM exactly).
+// Grouped calls (AttnParams::gtile): every 128-track tile lies inside one group and reads that group's 64 key / value
+// rows.  A TMA store clips only at the tensor-map bounds, so a group's last partial tile (unless it ends the track
+// range) stores its valid rows with plain 16-byte stores instead: it never writes a row of the next group.
 #include "gemm.cuh"
 #include "kernels.cuh"
 
@@ -53,7 +56,15 @@ attn_p2v_tc_kernel(const __grid_constant__ P2vMaps maps, AttnParams p, int tiles
   uint8_t* smem = smem_align1024(smem_raw);
   uint64_t* bar_ld = reinterpret_cast<uint64_t*>(smem + PV_OFF_BAR);
   const int r = threadIdx.x, warp = r >> 5, lane = r & 31;
-  const int t = blockIdx.x / tiles_per_seq, n0 = (blockIdx.x % tiles_per_seq) * 128;
+  const int t = blockIdx.x / tiles_per_seq, tile = blockIdx.x % tiles_per_seq;
+  int n0 = tile * 128, kv0 = 0, n_end = p.Lq;   // tracks [n0, n_end) of this tile's group; its keys start at token kv0
+  if (p.gtile) {
+    const int g = p.gtile[2 * tile];
+    n0 = p.gtile[2 * tile + 1];
+    kv0 = g * kV;
+    n_end = p.goff[g + 1];
+  }
+  const bool tma_store = n0 + 128 <= n_end || n_end == p.Lq;
 
   // zero the operand tiles once (V^T rows are fully rewritten per head, the K padding columns 48..63 never are)
   for (int i = r; i < (PV_OFF_END - PV_OFF_Q) / 16; i += PV_THREADS)
@@ -78,8 +89,8 @@ attn_p2v_tc_kernel(const __grid_constant__ P2vMaps maps, AttnParams p, int tiles
   auto issue_loads = [&](int h) {   // one thread
     mbar_arrive_expect_tx(bar_ld, PV_LOAD_BYTES);
     tma_load_3d(smem + PV_OFF_SQ, &maps.q, p.q_col + h * kDh, t, n0, bar_ld);
-    tma_load_3d(smem + PV_OFF_SK, &maps.kv, p.k_col + h * kDh, t, 0, bar_ld);
-    tma_load_3d(smem + PV_OFF_SV, &maps.kv, p.v_col + h * kDh, t, 0, bar_ld);
+    tma_load_3d(smem + PV_OFF_SK, &maps.kv, p.k_col + h * kDh, t, kv0, bar_ld);
+    tma_load_3d(smem + PV_OFF_SV, &maps.kv, p.v_col + h * kDh, t, kv0, bar_ld);
   };
   if (r == 0) issue_loads(0);
 
@@ -224,11 +235,22 @@ attn_p2v_tc_kernel(const __grid_constant__ P2vMaps maps, AttnParams p, int tiles
     }
     fence_proxy_async_smem();
     __syncthreads();
-    if (r == 0) {
-      tma_store_3d(&maps.out, h * kDh, t, n0, smem + PV_OFF_Q);
-      tma_store_3d(&maps.out, p.lo_off + h * kDh, t, n0, smem + PV_OFF_Q + PV_TILE_Q);
-      bulk_commit();
-      bulk_wait_read0();      // the stores have read the rows: the next head may rewrite the Q tiles
+    if (tma_store) {
+      if (r == 0) {
+        tma_store_3d(&maps.out, h * kDh, t, n0, smem + PV_OFF_Q);
+        tma_store_3d(&maps.out, p.lo_off + h * kDh, t, n0, smem + PV_OFF_Q + PV_TILE_Q);
+        bulk_commit();
+        bulk_wait_read0();    // the stores have read the rows: the next head may rewrite the Q tiles
+      }
+    } else {
+      // rows [n0, n_end) only: 2 planes x 6 chunks of 16 bytes per 96-byte row
+      for (int i = r; i < (n_end - n0) * 12; i += PV_THREADS) {
+        const int row = i / 12, plane = (i % 12) / 6, c = i % 6;
+        const uint4 v = *reinterpret_cast<const uint4*>(smem + PV_OFF_Q + plane * PV_TILE_Q + row * (kDh * 2) + c * 16);
+        __nv_bfloat16* dst = p.out + ((int64_t)t * p.q_seq_stride + (int64_t)(n0 + row) * p.q_tok_stride) * p.out_ld +
+                             plane * p.lo_off + h * kDh + c * 8;
+        *reinterpret_cast<uint4*>(dst) = v;
+      }
     }
     __syncthreads();
   }
@@ -238,7 +260,7 @@ attn_p2v_tc_kernel(const __grid_constant__ P2vMaps maps, AttnParams p, int tiles
 }  // namespace
 
 bool attention_p2v_supported(const AttnParams& p) {
-  return p.Lk == kV && p.Lq >= 1 && (p.q_ld % 4) == 0 && (p.kv_ld % 4) == 0 && (p.q_col % 4) == 0 && (p.k_col % 4) == 0 &&
+  return (p.gtile ? p.Lk >= kV && p.Lk % kV == 0 : p.Lk == kV) && p.Lq >= 1 && (p.q_ld % 4) == 0 && (p.kv_ld % 4) == 0 && (p.q_col % 4) == 0 && (p.k_col % 4) == 0 &&
          (p.v_col % 4) == 0 && (p.out_ld % 8) == 0 && (p.lo_off % 8) == 0 &&
          ((reinterpret_cast<uintptr_t>(p.q) | reinterpret_cast<uintptr_t>(p.kv) | reinterpret_cast<uintptr_t>(p.out)) & 15) == 0;
 }
@@ -267,7 +289,7 @@ cudaError_t launch_attention_p2v(const AttnParams& p, cudaStream_t s) {
     return cudaFuncSetAttribute(attn_p2v_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PV_SMEM);
   });
   if (e != cudaSuccess) return e;
-  const int tiles = (p.Lq + 127) / 128;
+  const int tiles = p.gtile ? p.tiles : (p.Lq + 127) / 128;
   attn_p2v_tc_kernel<<<p.num_seq * tiles, PV_THREADS, PV_SMEM, s>>>(maps, p, tiles);
   return cudaGetLastError();
 }

@@ -14,6 +14,8 @@
 //         shared    = the 4 warps of a CTA share one (sequence, head) K/V chunk (space attention)
 //         split-K   = the key range is split over gridDim.z CTAs that emit (m, l, O) partials (virtual <- point:
 //                     64 queries x N keys), merged by attention_combine_kernel.
+// Grouped calls (AttnParams::gl) run the shared mode over (group, frame) sequences of different lengths in one launch;
+// each entry has its own split-K count, so every group's chunk ranges and combine order are those of a standalone call.
 #include "kernels.cuh"
 
 namespace ct3 {
@@ -56,6 +58,14 @@ attention_tc_kernel(AttnParams p, int q_tiles, int num_splits, int qtw, float* p
     qt = (qb * WARPS + warp) * qtw;   // first of the qtw query tiles this warp walks (single-chunk K/V only)
     split = blockIdx.z;
   }
+  const SeqRows sr = seq_rows(p, s);   // PER_WARP (time attention) is never grouped
+  const int Lq = sr.Lq, Lk = sr.Lk;
+  const int nsp = p.gl ? (p.gsplit ? p.gsplit[sr.e] : 1) : num_splits;
+  if (!PER_WARP) {
+    q_tiles = (Lq + 15) / 16;
+    // grouped: CTAs past this sequence's queries or split count (CTA-uniform, before any barrier)
+    if (split >= nsp || (int)(blockIdx.y / kHeads) * WARPS * qtw >= q_tiles) return;
+  }
   const int qt_first = qt;
   const bool item_ok = active;
   __nv_bfloat16* slice = reinterpret_cast<__nv_bfloat16*>(att_smem) + (PER_WARP ? warp * SLICE : 0);
@@ -65,8 +75,8 @@ attention_tc_kernel(AttnParams p, int q_tiles, int num_splits, int qtw, float* p
   __nv_bfloat16* Vl = Vh + kDh * VPAD;
 
   // key range of this CTA (split-K) in units of chunks
-  const int chunks = (p.Lk + KB - 1) / KB;
-  const int c_per = (chunks + num_splits - 1) / num_splits;
+  const int chunks = (Lk + KB - 1) / KB;
+  const int c_per = (chunks + nsp - 1) / nsp;
   const int c_begin = split * c_per, c_end = min(chunks, c_begin + c_per);
 
   // K/V are staged once when they fit one chunk; the warp then walks qtw query tiles against them
@@ -79,9 +89,9 @@ attention_tc_kernel(AttnParams p, int q_tiles, int num_splits, int qtw, float* p
   const int q_row0 = qt * 16 + g, q_row1 = q_row0 + 8;
   uint32_t qh[3][4], ql[3][4];
   {
-    const int r0 = min(q_row0, p.Lq - 1), r1 = min(q_row1, p.Lq - 1);
-    const float* qp0 = p.q + ((int64_t)s * p.q_seq_stride + (int64_t)r0 * p.q_tok_stride) * p.q_ld + p.q_col + h * kDh;
-    const float* qp1 = p.q + ((int64_t)s * p.q_seq_stride + (int64_t)r1 * p.q_tok_stride) * p.q_ld + p.q_col + h * kDh;
+    const int r0 = min(q_row0, Lq - 1), r1 = min(q_row1, Lq - 1);
+    const float* qp0 = p.q + (sr.q0 + (int64_t)r0 * p.q_tok_stride) * p.q_ld + p.q_col + h * kDh;
+    const float* qp1 = p.q + (sr.q0 + (int64_t)r1 * p.q_tok_stride) * p.q_ld + p.q_col + h * kDh;
 #pragma unroll
     for (int ks = 0; ks < 3; ++ks) {
       const float2 a0 = __ldg(reinterpret_cast<const float2*>(qp0 + 16 * ks + 2 * t4));
@@ -111,13 +121,13 @@ attention_tc_kernel(AttnParams p, int q_tiles, int num_splits, int qtw, float* p
       for (int idx = tid; idx < (KB / 2) * (kDh / 4); idx += nthr) {
         const int j = 2 * (idx / (kDh / 4)), d4 = idx % (kDh / 4);
         float4 k0 = make_float4(0.f, 0.f, 0.f, 0.f), k1 = k0, v0 = k0, v1 = k0;
-        if (kc0 + j < p.Lk) {
-          const float* base = p.kv + ((int64_t)s * p.k_seq_stride + (int64_t)(kc0 + j) * p.k_tok_stride) * p.kv_ld + h * kDh;
+        if (kc0 + j < Lk) {
+          const float* base = p.kv + (sr.k0 + (int64_t)(kc0 + j) * p.k_tok_stride) * p.kv_ld + h * kDh;
           k0 = __ldg(reinterpret_cast<const float4*>(base + p.k_col) + d4);
           v0 = __ldg(reinterpret_cast<const float4*>(base + p.v_col) + d4);
         }
-        if (kc0 + j + 1 < p.Lk) {
-          const float* base = p.kv + ((int64_t)s * p.k_seq_stride + (int64_t)(kc0 + j + 1) * p.k_tok_stride) * p.kv_ld + h * kDh;
+        if (kc0 + j + 1 < Lk) {
+          const float* base = p.kv + (sr.k0 + (int64_t)(kc0 + j + 1) * p.k_tok_stride) * p.kv_ld + h * kDh;
           k1 = __ldg(reinterpret_cast<const float4*>(base + p.k_col) + d4);
           v1 = __ldg(reinterpret_cast<const float4*>(base + p.v_col) + d4);
         }
@@ -163,7 +173,7 @@ attention_tc_kernel(AttnParams p, int q_tiles, int num_splits, int qtw, float* p
 #pragma unroll
     for (int nt = 0; nt < KB / 8; ++nt) {
       const int key = kc0 + nt * 8 + 2 * t4;
-      const bool v0 = key < p.Lk, v1 = key + 1 < p.Lk;
+      const bool v0 = key < Lk, v1 = key + 1 < Lk;
       sc[nt][0] = v0 ? sc[nt][0] * p.scale : -INFINITY;
       sc[nt][1] = v1 ? sc[nt][1] * p.scale : -INFINITY;
       sc[nt][2] = v0 ? sc[nt][2] * p.scale : -INFINITY;
@@ -215,17 +225,17 @@ attention_tc_kernel(AttnParams p, int q_tiles, int num_splits, int qtw, float* p
   l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
   if (!active) continue;
-  if (num_splits > 1) {
-    // partials: item = ((s*heads + h)*num_splits + split); rows indexed by query
-    const int64_t item = ((int64_t)s * kHeads + h) * num_splits + split;
+  if (nsp > 1) {
+    // partials: item = (slot * frames + frame) * heads + h, rows indexed by query
+    const int64_t item = (((p.gl ? p.gslot[sr.e] : 0) + (int64_t)split) * (p.gl ? p.frames : p.num_seq) + sr.t) * kHeads + h;
     float* pml = part_ml + item * p.Lq * 2;
     float* po = part_o + item * p.Lq * kDh;
-    if (q_row0 < p.Lq) {
+    if (q_row0 < Lq) {
       if (t4 == 0) { pml[q_row0 * 2] = m0; pml[q_row0 * 2 + 1] = l0; }
 #pragma unroll
       for (int nd = 0; nd < 6; ++nd) *reinterpret_cast<float2*>(po + (int64_t)q_row0 * kDh + nd * 8 + 2 * t4) = make_float2(o[nd][0], o[nd][1]);
     }
-    if (q_row1 < p.Lq) {
+    if (q_row1 < Lq) {
       if (t4 == 0) { pml[q_row1 * 2] = m1; pml[q_row1 * 2 + 1] = l1; }
 #pragma unroll
       for (int nd = 0; nd < 6; ++nd) *reinterpret_cast<float2*>(po + (int64_t)q_row1 * kDh + nd * 8 + 2 * t4) = make_float2(o[nd][2], o[nd][3]);
@@ -233,8 +243,8 @@ attention_tc_kernel(AttnParams p, int q_tiles, int num_splits, int qtw, float* p
     continue;
   }
   const float i0 = 1.0f / l0, i1 = 1.0f / l1;
-  if (q_row0 < p.Lq) {
-    __nv_bfloat16* orow = p.out + ((int64_t)s * p.q_seq_stride + (int64_t)q_row0 * p.q_tok_stride) * p.out_ld + h * kDh;
+  if (q_row0 < Lq) {
+    __nv_bfloat16* orow = p.out + (sr.q0 + (int64_t)q_row0 * p.q_tok_stride) * p.out_ld + h * kDh;
 #pragma unroll
     for (int nd = 0; nd < 6; ++nd) {
       uint32_t hi, lo;
@@ -243,8 +253,8 @@ attention_tc_kernel(AttnParams p, int q_tiles, int num_splits, int qtw, float* p
       *reinterpret_cast<uint32_t*>(orow + p.lo_off + nd * 8 + 2 * t4) = lo;
     }
   }
-  if (q_row1 < p.Lq) {
-    __nv_bfloat16* orow = p.out + ((int64_t)s * p.q_seq_stride + (int64_t)q_row1 * p.q_tok_stride) * p.out_ld + h * kDh;
+  if (q_row1 < Lq) {
+    __nv_bfloat16* orow = p.out + (sr.q0 + (int64_t)q_row1 * p.q_tok_stride) * p.out_ld + h * kDh;
 #pragma unroll
     for (int nd = 0; nd < 6; ++nd) {
       uint32_t hi, lo;
@@ -266,14 +276,18 @@ attention_combine_kernel(AttnParams p, int num_splits, const float* __restrict__
   const int qi = (int)(w % p.Lq);
   const int h = (int)((w / p.Lq) % kHeads);
   const int s = (int)(w / ((int64_t)p.Lq * kHeads));
+  const SeqRows sr = seq_rows(p, s);
+  const int nsp = p.gl ? (p.gsplit ? p.gsplit[sr.e] : 1) : num_splits;
+  if (nsp <= 1 || qi >= sr.Lq) return;   // grouped: this entry wrote its output directly
+  const int64_t slot0 = p.gl ? p.gslot[sr.e] : 0, frames = p.gl ? p.frames : p.num_seq;
   float m = -INFINITY;
-  for (int k = 0; k < num_splits; ++k) {
-    const int64_t item = ((int64_t)s * kHeads + h) * num_splits + k;
+  for (int k = 0; k < nsp; ++k) {
+    const int64_t item = ((slot0 + k) * frames + sr.t) * kHeads + h;
     m = fmaxf(m, part_ml[(item * p.Lq + qi) * 2]);
   }
   float l = 0.f, a0 = 0.f, a1 = 0.f;
-  for (int k = 0; k < num_splits; ++k) {
-    const int64_t item = ((int64_t)s * kHeads + h) * num_splits + k;
+  for (int k = 0; k < nsp; ++k) {
+    const int64_t item = ((slot0 + k) * frames + sr.t) * kHeads + h;
     const float mk = part_ml[(item * p.Lq + qi) * 2], lk = part_ml[(item * p.Lq + qi) * 2 + 1];
     const float wgt = (mk == -INFINITY) ? 0.f : expf(mk - m);
     l += wgt * lk;
@@ -282,7 +296,7 @@ attention_combine_kernel(AttnParams p, int num_splits, const float* __restrict__
     if (lane < kDh - 32) a1 += wgt * po[32 + lane];
   }
   const float inv = 1.0f / l;
-  __nv_bfloat16* orow = p.out + ((int64_t)s * p.q_seq_stride + (int64_t)qi * p.q_tok_stride) * p.out_ld + h * kDh;
+  __nv_bfloat16* orow = p.out + (sr.q0 + (int64_t)qi * p.q_tok_stride) * p.out_ld + h * kDh;
   const bf16pair x = split_bf16(a0 * inv);
   orow[lane] = x.hi;
   orow[p.lo_off + lane] = x.lo;
@@ -326,21 +340,13 @@ size_t attention_partial_bytes(int num_seq, int Lq, int max_splits) {
   return (size_t)num_seq * kHeads * max_splits * Lq * (kDh + 2) * sizeof(float);
 }
 
-// per_warp: sequences are short and independent (time attention); otherwise the CTA shares K/V.
-// part: scratch of attention_partial_bytes(num_seq, Lq, kAttnMaxSplits) bytes or null (then no split-K).
-cudaError_t launch_attention_tc(const AttnParams& p, bool per_warp, float* part, int num_sms, cudaStream_t s) {
-  if (p.num_seq <= 0 || p.Lq <= 0 || p.Lk <= 0) return cudaSuccess;
-  if (per_warp) {
-    if (p.Lk <= 16) return launch_variant<16, true>(p, 1, 1, nullptr, nullptr, s);
-    if (p.Lk <= 32) return launch_variant<32, true>(p, 1, 1, nullptr, nullptr, s);
-    return launch_variant<64, true>(p, 1, 1, nullptr, nullptr, s);
-  }
-  // split-K when the query side alone cannot fill the machine
-  const int q_tiles = (p.Lq + 15) / 16;
-  const int ctas = p.num_seq * kHeads * ((q_tiles + WARPS - 1) / WARPS);
-  const int chunks = (p.Lk + 63) / 64;
+// split-K when the query side alone cannot fill the machine
+int attention_tc_splits(int num_seq, int Lq, int Lk, int num_sms) {
+  const int q_tiles = (Lq + 15) / 16;
+  const int ctas = num_seq * kHeads * ((q_tiles + WARPS - 1) / WARPS);
+  const int chunks = (Lk + 63) / 64;
   int splits = 1;
-  if (part != nullptr && ctas < 2 * num_sms && chunks >= 8) {
+  if (ctas < 2 * num_sms && chunks >= 8) {
     // split-K so that the grid fills whole waves of the 4-CTA/SM occupancy: minimise waves x chunks-per-split
     const int slots = 4 * num_sms;
     long long best = -1;
@@ -351,6 +357,30 @@ cudaError_t launch_attention_tc(const AttnParams& p, bool per_warp, float* part,
       if (best < 0 || cost < best) { best = cost; splits = sp; }
     }
   }
+  return splits;
+}
+
+// per_warp: sequences are short and independent (time attention); otherwise the CTA shares K/V.
+// part: scratch of attention_partial_bytes(num_seq, Lq, kAttnMaxSplits) bytes or null (then no split-K).
+cudaError_t launch_attention_tc(const AttnParams& p, bool per_warp, float* part, int num_sms, cudaStream_t s) {
+  if (p.num_seq <= 0 || p.Lq <= 0 || p.Lk <= 0) return cudaSuccess;
+  if (per_warp) {
+    if (p.Lk <= 16) return launch_variant<16, true>(p, 1, 1, nullptr, nullptr, s);
+    if (p.Lk <= 32) return launch_variant<32, true>(p, 1, 1, nullptr, nullptr, s);
+    return launch_variant<64, true>(p, 1, 1, nullptr, nullptr, s);
+  }
+  const int q_tiles = (p.Lq + 15) / 16;
+  const int chunks = (p.Lk + 63) / 64;
+  int splits = 1, slots = 1;
+  if (p.gl) {   // grouped: the caller chose every entry's count with attention_tc_splits
+    if (p.split_max > 1) {
+      if (!part || !p.gsplit || !p.gslot) return cudaErrorInvalidValue;
+      splits = p.split_max;
+      slots = p.split_slots;
+    }
+  } else if (part != nullptr) {
+    splits = slots = attention_tc_splits(p.num_seq, p.Lq, p.Lk, num_sms);
+  }
   if (splits == 1) {
     // K/V of one chunk are staged once per CTA: amortise the conversion over several query tiles per warp while
     // still leaving >= 4 CTAs per SM
@@ -359,7 +389,7 @@ cudaError_t launch_attention_tc(const AttnParams& p, bool per_warp, float* part,
     return launch_variant<64, false>(p, 1, qtw, nullptr, nullptr, s);
   }
   float* part_ml = part;
-  float* part_o = part + (size_t)p.num_seq * kHeads * splits * p.Lq * 2;
+  float* part_o = part + (size_t)slots * (p.gl ? p.frames : p.num_seq) * kHeads * p.Lq * 2;
   cudaError_t e = launch_variant<64, false>(p, splits, 1, part_ml, part_o, s);
   if (e != cudaSuccess) return e;
   const int64_t rows = (int64_t)p.num_seq * kHeads * p.Lq;

@@ -96,7 +96,10 @@ cudaError_t launch_affine_fold(const float* w, const float* b, const float* gamm
                                float* w2, float* b2, cudaStream_t s);
 cudaError_t launch_build_x_small(const float* coords, const float* vis, const float* conf, int T, int N,
                                  __nv_bfloat16* x_split, cudaStream_t s);
-cudaError_t launch_init_virtual(float* tokens, const float* virt, int T, int N, cudaStream_t s);
+// one copy of the kV virtual tokens per group: rows (N + kV*g + i)*T + t, g < G
+cudaError_t launch_init_virtual(float* tokens, const float* virt, int T, int N, int G, cudaStream_t s);
+// host int32 array -> device, stream-ordered (kernel arguments carry the values: src may be freed on return)
+cudaError_t launch_upload_i32(int32_t* dst, const int32_t* src_host, int n, cudaStream_t s);
 // delta_out == nullptr: in-place state update; else write delta [N,T,4] and leave the state alone
 cudaError_t launch_heads(const float* tokens, const float* w4, const float* b4, float* coords, float* vis,
                          float* conf, float* delta_out, int T, int N, cudaStream_t s);
@@ -115,13 +118,46 @@ struct AttnParams {
   int64_t q_seq_stride, q_tok_stride;  // q/out row = s*q_seq_stride + i*q_tok_stride
   int64_t k_seq_stride, k_tok_stride;  // k/v row  = s*k_seq_stride + j*k_tok_stride
   float scale;
+  // Grouped space attention (ct3_update_loop_groups): the tracks form contiguous groups, each with its own kV virtual
+  // tokens.  gl == nullptr: one group, rows as above.  Otherwise sequence s = (entry s / frames, frame s % frames),
+  // entry e covers group gl[e], and Lq / Lk are upper bounds.  A side with grp_stride != 0 is virtual (group g starts
+  // at row g * grp_stride, kV tokens); a side with grp_stride == 0 holds points (group g = tracks [goff[g], goff[g+1])).
+  const int32_t* gl;
+  const int32_t* goff;     // [G+1] first track of every group
+  const int32_t* gsplit;   // attention_tc.cu: [entries] split-K count (null: 1)
+  const int32_t* gslot;    //                  [entries] first partial slot of a split entry
+  int frames, split_max, split_slots;   // split_max: largest gsplit entry; split_slots: sum of gsplit over split entries
+  int64_t q_grp_stride, k_grp_stride;
+  // attention_p2v.cu: [tiles] (group, first track) of each 128-track tile; Lq = all tracks, Lk = kV * groups
+  const int32_t* gtile;
+  int tiles;
 };
+// rows and lengths of sequence s (grouped or not)
+struct SeqRows { int64_t q0, k0; int Lq, Lk, e, t; };
+__device__ __forceinline__ SeqRows seq_rows(const AttnParams& p, int s) {
+  SeqRows r;
+  if (!p.gl) {
+    r.q0 = (int64_t)s * p.q_seq_stride; r.k0 = (int64_t)s * p.k_seq_stride;
+    r.Lq = p.Lq; r.Lk = p.Lk; r.e = 0; r.t = s;
+    return r;
+  }
+  r.e = s / p.frames;
+  r.t = s - r.e * p.frames;
+  const int g = p.gl[r.e], n0 = p.goff[g], n = p.goff[g + 1] - n0;
+  r.q0 = (int64_t)r.t * p.q_seq_stride + (p.q_grp_stride ? (int64_t)g * p.q_grp_stride : (int64_t)n0 * p.q_tok_stride);
+  r.k0 = (int64_t)r.t * p.k_seq_stride + (p.k_grp_stride ? (int64_t)g * p.k_grp_stride : (int64_t)n0 * p.k_tok_stride);
+  r.Lq = p.q_grp_stride ? kV : n;
+  r.Lk = p.k_grp_stride ? kV : n;
+  return r;
+}
 cudaError_t launch_attention(const AttnParams& p, cudaStream_t s);   // exact-fp32 SIMT (verification)
 
 
 // ---- attention_tc.cu : tensor-core (mma.sync split-bf16x3) production path ------------------------
 constexpr int kAttnMaxSplits = 32;
 size_t attention_partial_bytes(int num_seq, int Lq, int max_splits);
+// split-K count launch_attention_tc chooses for an ungrouped shared-K/V launch of this shape
+int attention_tc_splits(int num_seq, int Lq, int Lk, int num_sms);
 cudaError_t launch_attention_tc(const AttnParams& p, bool per_warp, float* part, int num_sms, cudaStream_t s);
 
 // ---- attention_p2v.cu : point <- virtual cross attention (Lk == 64 keys) on wgmma --------------------------------------

@@ -93,14 +93,14 @@ build_x_small_kernel(const float* __restrict__ coords, const float* __restrict__
   o[kXPad] = p.lo;
 }
 
-__global__ void init_virtual_kernel(float* __restrict__ tokens, const float* __restrict__ virt, int T, int N) {
-  // tokens[(N+i)*T + t][:] = virt[i][:]
-  const int64_t total = (int64_t)kV * T * (kC / 4);
+__global__ void init_virtual_kernel(float* __restrict__ tokens, const float* __restrict__ virt, int T, int N, int G) {
+  // tokens[(N + kV*g + i)*T + t][:] = virt[i][:]
+  const int64_t total = (int64_t)kV * G * T * (kC / 4);
   for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total;
        idx += (int64_t)gridDim.x * blockDim.x) {
     const int c4 = (int)(idx % (kC / 4));
-    const int64_t r = idx / (kC / 4);  // i*T + t
-    const int i = (int)(r / T);
+    const int64_t r = idx / (kC / 4);  // (kV*g + i)*T + t
+    const int i = (int)((r / T) % kV);
     reinterpret_cast<float4*>(tokens + ((int64_t)N * T + r) * kC)[c4] =
         reinterpret_cast<const float4*>(virt + (int64_t)i * kC)[c4];
   }
@@ -233,6 +233,13 @@ affine_fold_kernel(const float* __restrict__ w, const float* __restrict__ b, con
   if (lane == 0) b2[j] = b[j] + s;
 }
 
+// a chunk of a host int32 table passed by value (kernel arguments stay below 4 KiB)
+constexpr int kI32Chunk = 960;
+struct I32Chunk { int32_t v[kI32Chunk]; };
+__global__ void upload_i32_kernel(int32_t* __restrict__ dst, const I32Chunk c, int n) {
+  for (int i = threadIdx.x; i < n; i += blockDim.x) dst[i] = c.v[i];
+}
+
 inline int grid_for(int64_t total, int block) {
   int64_t b = (total + block - 1) / block;
   const int64_t cap = 132 * 32;
@@ -252,9 +259,20 @@ cudaError_t launch_build_x_small(const float* coords, const float* vis, const fl
   build_x_small_kernel<<<N * T, 128, 0, s>>>(coords, vis, conf, T, N, x_split);
   return cudaGetLastError();
 }
-cudaError_t launch_init_virtual(float* tokens, const float* virt, int T, int N, cudaStream_t s) {
-  init_virtual_kernel<<<grid_for((int64_t)kV * T * (kC / 4), 256), 256, 0, s>>>(tokens, virt, T, N);
+cudaError_t launch_init_virtual(float* tokens, const float* virt, int T, int N, int G, cudaStream_t s) {
+  init_virtual_kernel<<<grid_for((int64_t)kV * G * T * (kC / 4), 256), 256, 0, s>>>(tokens, virt, T, N, G);
   return cudaGetLastError();
+}
+cudaError_t launch_upload_i32(int32_t* dst, const int32_t* src_host, int n, cudaStream_t s) {
+  for (int i0 = 0; i0 < n; i0 += kI32Chunk) {
+    I32Chunk c;
+    const int m = n - i0 < kI32Chunk ? n - i0 : kI32Chunk;
+    for (int i = 0; i < m; ++i) c.v[i] = src_host[i0 + i];
+    upload_i32_kernel<<<1, 256, 0, s>>>(dst + i0, c, m);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 cudaError_t launch_heads(const float* tokens, const float* w4, const float* b4, float* coords, float* vis,
                          float* conf, float* delta_out, int T, int N, cudaStream_t s) {

@@ -53,6 +53,12 @@ def _declare(lib):
         "ct3_split_rows_fp16": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_linear_prec": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_updateformer": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+        "ct3_workspace_bytes_groups": (c_int, [c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+        "ct3_update_loop_groups": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p,
+                                           ctypes.POINTER(ctypes.c_int32), c_int]),
+        "ct3_updateformer_groups": (c_int, [c_void_p, c_void_p, c_int, ctypes.POINTER(ctypes.c_int32), c_int, c_void_p,
+                                            c_void_p, c_size_t, c_void_p]),
         "ct3_upsample_concat": (c_int, [ctypes.POINTER(c_void_p), intp, intp, intp, c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_enc_tail_packed_bytes": (c_int, [ctypes.POINTER(c_size_t)]),
         "ct3_enc_tail_pack": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
@@ -82,6 +88,7 @@ EXPORTED_SYMBOLS = [
     "ct3_encoder_num_weight_tensors", "ct3_encoder_weight_name", "ct3_encoder_packed_bytes", "ct3_encoder_pack",
     "ct3_encoder_workspace_bytes", "ct3_encoder",
     "ct3_upsample_concat", "ct3_enc_tail_packed_bytes", "ct3_enc_tail_pack", "ct3_enc_tail_workspace_bytes", "ct3_enc_tail",
+    "ct3_workspace_bytes_groups", "ct3_update_loop_groups", "ct3_updateformer_groups",
 ]
 
 
@@ -228,11 +235,24 @@ def sample_support(pyr, T, H4, W4, qframes, qcoords, support=None, accumulate_ma
     return support
 
 
-def workspace_bytes(T: int, N: int, H4: int = 0, W4: int = 0) -> int:
-    """Scratch of ct3_update_loop for T frames of H4 x W4 feature maps and N tracks (H4 = W4 = 0: updateformer only)."""
+def workspace_bytes(T: int, N: int, H4: int = 0, W4: int = 0, groups: int = 1) -> int:
+    """Scratch of ct3_update_loop for T frames of H4 x W4 feature maps and N tracks (H4 = W4 = 0: updateformer only),
+    split into `groups` track groups (ct3_update_loop_groups)."""
     n = ctypes.c_size_t(0)
-    _check(lib().ct3_workspace_bytes(T, N, H4, W4, ctypes.byref(n)), "ct3_workspace_bytes")
+    _check(lib().ct3_workspace_bytes_groups(int(T), int(N), int(groups), int(H4), int(W4), ctypes.byref(n)),
+           "ct3_workspace_bytes_groups")
     return n.value
+
+
+def _group_array(group_sizes):
+    """Host int32 array of the group sizes (ct3_*_groups); the library validates the values."""
+    try:
+        sizes = [int(g) for g in group_sizes]
+    except (TypeError, ValueError) as e:
+        raise EngineError(f"group_sizes must be a sequence of integers: {e}") from e
+    if any(not (-2 ** 31 <= g < 2 ** 31) for g in sizes):
+        raise EngineError("group sizes must fit in int32")
+    return (ctypes.c_int32 * max(1, len(sizes)))(*sizes), len(sizes)
 
 
 class WorkspaceCache:
@@ -241,16 +261,19 @@ class WorkspaceCache:
     def __init__(self):
         self.buf: Optional[torch.Tensor] = None
 
-    def get(self, T: int, N: int, device, H4: int = 0, W4: int = 0) -> torch.Tensor:
-        need = workspace_bytes(T, N, H4, W4)
+    def get(self, T: int, N: int, device, H4: int = 0, W4: int = 0, groups: int = 1) -> torch.Tensor:
+        need = workspace_bytes(T, N, H4, W4, groups)
         if self.buf is None or self.buf.numel() < need or self.buf.device != torch.device(device):
             self.buf = None
             self.buf = torch.empty(need, dtype=torch.uint8, device=device)
         return self.buf
 
 
-def update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, iters, workspace):
-    """In-place refinement of coords [T,N,2], vis [T,N], conf [T,N] (fp32, feature-grid units / logits)."""
+def update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, iters, workspace,
+                group_sizes: Optional[Sequence[int]] = None):
+    """In-place refinement of coords [T,N,2], vis [T,N], conf [T,N] (fp32, feature-grid units / logits).
+    group_sizes: the N tracks as contiguous independent groups (ct3_update_loop_groups); each group's result is
+    bit-identical to a call on its tracks alone.  None = one group."""
     _req(coords, torch.float32, "coords"); _req(vis, torch.float32, "vis"); _req(conf, torch.float32, "conf")
     _req(pyr, torch.float32, "pyr"); _req(support, torch.float32, "support"); _req(time_emb, torch.float32, "time_emb")
     T, N, _ = coords.shape
@@ -258,6 +281,14 @@ def update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, ti
         raise EngineError(f"time_emb must be [{T},{XDIM}]")
     if track_valid is not None:
         _req(track_valid, torch.uint8, "track_valid")
+    if group_sizes is not None:
+        arr, G = _group_array(group_sizes)
+        with torch.cuda.device(coords.device):
+            _check(lib().ct3_update_loop_groups(_ptr(packed), _ptr(pyr), H4, W4, _ptr(support), _ptr(track_valid),
+                                                _ptr(coords), _ptr(vis), _ptr(conf), _ptr(time_emb), T, N, int(iters),
+                                                _ptr(workspace), workspace.numel(), _stream(coords.device), arr, G),
+                   "ct3_update_loop_groups")
+        return
     with torch.cuda.device(coords.device):
         _check(lib().ct3_update_loop(_ptr(packed), _ptr(pyr), H4, W4, _ptr(support), _ptr(track_valid), _ptr(coords),
                                      _ptr(vis), _ptr(conf), _ptr(time_emb), T, N, int(iters), _ptr(workspace),
@@ -316,15 +347,27 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], act: 
     return y
 
 
-def updateformer(packed, x: torch.Tensor, workspace: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """x [N,T,1110] fp32 (reference column order, time embedding added) -> delta [N,T,4]."""
+def updateformer(packed, x: torch.Tensor, workspace: Optional[torch.Tensor] = None,
+                 group_sizes: Optional[Sequence[int]] = None) -> torch.Tensor:
+    """x [N,T,1110] fp32 (reference column order, time embedding added) -> delta [N,T,4].
+    group_sizes: contiguous independent track groups (ct3_updateformer_groups), None = one group."""
     _req(x, torch.float32, "x")
     N, T, D = x.shape
     if D != XDIM:
         raise EngineError("x must be [N,T,1110]")
+    delta = torch.empty(N, T, 4, dtype=torch.float32, device=x.device)
+    if group_sizes is not None:
+        arr, G = _group_array(group_sizes)
+        if sum(arr[:G]) != N:
+            raise EngineError(f"group sizes sum to {sum(arr[:G])}, x has {N} tracks")
+        if workspace is None:
+            workspace = torch.empty(workspace_bytes(T, N, groups=G), dtype=torch.uint8, device=x.device)
+        with torch.cuda.device(x.device):
+            _check(lib().ct3_updateformer_groups(_ptr(packed), _ptr(x), T, arr, G, _ptr(delta), _ptr(workspace),
+                                                 workspace.numel(), _stream(x.device)), "ct3_updateformer_groups")
+        return delta
     if workspace is None:
         workspace = torch.empty(workspace_bytes(T, N), dtype=torch.uint8, device=x.device)
-    delta = torch.empty(N, T, 4, dtype=torch.float32, device=x.device)
     with torch.cuda.device(x.device):
         _check(lib().ct3_updateformer(_ptr(packed), _ptr(x), T, N, _ptr(delta), _ptr(workspace), workspace.numel(),
                                       _stream(x.device)), "ct3_updateformer")

@@ -8,12 +8,15 @@ Jaccard (AJ) at 1/2/4/8/16 px.  `EvaluationPredictor` wraps a cotracker_b200 off
 reference's benchmark code drives it: one query point at a time with an 8x8 local grid and a 5x5 global grid as
 helper tracks (single_point=True, the TAP-Vid protocol), or all queries jointly.  The model behind it is the same
 CUDA path as everywhere else (libct3_b200.so); SIFT helper points (sift_size > 0) are not provided.
+In single-point mode every query's 90-track set is one group of `forward_groups`: the clip is encoded once per pass
+and all groups share one update loop, in as few passes as fit in device memory (`plan_passes`).  Each group's result
+is bit-identical to a model call on that group alone, so the split into passes does not change the output.
 With no datasets or checkpoints in this environment the harness is exercised by scoring the CUDA tracks against
 the reference's tracks on synthetic clips (tests/test_evaluation.py): identical outputs score 1.0 everywhere.
 """
 from __future__ import annotations
 
-from typing import Dict, Optional, Tuple
+from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -75,6 +78,30 @@ def points_on_a_grid(size: int, extent, center=None, device="cpu") -> torch.Tens
     return torch.stack([gx, gy], dim=-1).reshape(1, -1, 2)
 
 
+def pass_bytes(T: int, N: int, G: int, H4: int, W4: int) -> int:
+    """Device memory of one grouped update-loop pass over N tracks in G groups and T frames: the library workspace
+    plus the per-track support features [4,49,N,128] and the per-frame state and outputs (about 16 floats)."""
+    from . import engine
+    return engine.workspace_bytes(T, N, H4, W4, groups=G) + N * (4 * 49 * 128 * 4 + T * 16 * 4)
+
+
+def plan_passes(group_sizes: Sequence[int], T: int, H4: int, W4: int, budget_bytes: int,
+                bytes_fn: Optional[Callable[[int, int, int, int, int], int]] = None) -> List[Tuple[int, int]]:
+    """Split the groups, in order, into as few passes [g0, g1) as keep bytes_fn(T, N, G, H4, W4) (default
+    `pass_bytes`) within `budget_bytes`.  A pure host function; a group that alone exceeds the budget gets a pass of
+    its own."""
+    fn = bytes_fn or pass_bytes
+    passes, g0, n = [], 0, 0
+    for g, size in enumerate(group_sizes):
+        if g > g0 and fn(T, n + size, g + 1 - g0, H4, W4) > budget_bytes:
+            passes.append((g0, g))
+            g0, n = g, 0
+        n += size
+    if len(group_sizes) > 0:
+        passes.append((g0, len(group_sizes)))
+    return passes
+
+
 class EvaluationPredictor(torch.nn.Module):
     """Benchmark-protocol wrapper around an offline CoTracker3 model (B = 1).
 
@@ -84,7 +111,9 @@ class EvaluationPredictor(torch.nn.Module):
 
     def __init__(self, cotracker_model, interp_shape: Tuple[int, int] = (384, 512), grid_size: int = 5,
                  local_grid_size: int = 8, single_point: bool = True, sift_size: int = 0,
-                 num_uniformly_sampled_pts: int = 0, n_iters: int = 6, local_extent: int = 50) -> None:
+                 num_uniformly_sampled_pts: int = 0, n_iters: int = 6, local_extent: int = 50,
+                 pass_budget_bytes: Optional[int] = None) -> None:
+        """pass_budget_bytes: device memory one single-point pass may use (None: derived from free device memory)."""
         super().__init__()
         if sift_size > 0:
             raise NotImplementedError("SIFT helper points are not provided by this build")
@@ -96,6 +125,7 @@ class EvaluationPredictor(torch.nn.Module):
         self.n_iters = n_iters
         self.num_uniformly_sampled_pts = num_uniformly_sampled_pts
         self.local_extent = local_extent
+        self.pass_budget_bytes = pass_budget_bytes
         self.model = cotracker_model
         self.model.eval()
 
@@ -116,6 +146,20 @@ class EvaluationPredictor(torch.nn.Module):
             extra.append(torch.cat([tt, xy], dim=1)[None])
         return torch.cat(extra, dim=1) if extra else video.new_zeros(1, 0, 3)
 
+    def _free_bytes(self, video, T, ih, iw) -> int:
+        """Pass budget from free device memory: what is free plus the model's cached update-loop workspace (it is
+        regrown per pass), less the encoder's workspace and two copies of the pyramid."""
+        from . import engine
+        free, _ = torch.cuda.mem_get_info(video.device)
+        free += torch.cuda.memory_reserved(video.device) - torch.cuda.memory_allocated(video.device)
+        ws = self.model._ws.buf
+        if ws is not None and ws.device == video.device:
+            free += ws.numel()
+        s = self.model.stride
+        pyr = engine.pyramid_layout(T, ih // s, iw // s)[3] * 4
+        reserve = engine.encoder_workspace_bytes(T, ih, iw) + 2 * pyr + (1 << 30)
+        return int(0.9 * max(0, free - reserve))
+
     @torch.no_grad()
     def forward(self, video, queries):
         B, T, C, H, W = video.shape
@@ -131,11 +175,24 @@ class EvaluationPredictor(torch.nn.Module):
             tracks = video.new_zeros(B, T, N, 2)
             vis = video.new_zeros(B, T, N)
             conf = video.new_zeros(B, T, N)
-            for i in range(N):
-                q = queries[:, i:i + 1]
-                q_all = torch.cat([q, self._helpers(video, q)], dim=1)
-                tr, vi, cf, _ = self.model(video=video, queries=q_all, iters=self.n_iters)
-                tracks[:, :, i], vis[:, :, i], conf[:, :, i] = tr[:, :, 0, :2], vi[:, :, 0], cf[:, :, 0]
+            # one group per query: the query followed by its helpers (random draws in the reference's per-query order)
+            groups = [torch.cat([queries[:, i:i + 1], self._helpers(video, queries[:, i:i + 1])], dim=1)
+                      for i in range(N)]
+            sizes = [g.shape[1] for g in groups]
+            first = np.concatenate([[0], np.cumsum(sizes)]).tolist()
+            q_all = torch.cat(groups, dim=1)
+            stride = self.model.stride
+            T_loop = T if not hasattr(self.model, "init_video_online_processing") else self.model.window_len
+            budget = self.pass_budget_bytes
+            if budget is None:
+                budget = self._free_bytes(video, T, ih, iw)
+            for g0, g1 in plan_passes(sizes, T_loop, ih // stride, iw // stride, budget):
+                a, b = first[g0], first[g1]
+                tr, vi, cf, _ = self.model.forward_groups(video, q_all[:, a:b], sizes[g0:g1], iters=self.n_iters)
+                cols = [first[g] - a for g in range(g0, g1)]
+                tracks[:, :, g0:g1] = tr[:, :, cols, :2]
+                vis[:, :, g0:g1] = vi[:, :, cols]
+                conf[:, :, g0:g1] = cf[:, :, cols]
         else:
             q_all = torch.cat([queries, self._helpers(video, None)], dim=1)
             tr, vi, cf, _ = self.model(video=video, queries=q_all, iters=self.n_iters)

@@ -175,11 +175,27 @@ class CoTrackerThreeBase(nn.Module):
         if not video.is_cuda:
             raise engine.EngineError("cotracker_b200 runs on CUDA only; move the module and inputs to a GPU")
 
-    def _refine(self, pyr, H4, W4, support, track_valid, coords, vis, conf, iters):
+    def _refine(self, pyr, H4, W4, support, track_valid, coords, vis, conf, iters, group_sizes):
         T, N, _ = coords.shape
         dev = coords.device
+        G = len(group_sizes)
         engine.update_loop(self.packed_weights(dev), pyr, H4, W4, support, track_valid, coords, vis, conf,
-                           self.interpolate_time_embed(T).to(dev), iters, self._ws.get(T, N, dev, H4, W4))
+                           self.interpolate_time_embed(T).to(dev), iters, self._ws.get(T, N, dev, H4, W4, G),
+                           group_sizes=group_sizes if G > 1 else None)
+
+    @torch.no_grad()
+    def forward_groups(self, video, queries, group_sizes, iters=4, fmaps_chunk_size=200):
+        """Track G independent query sets over one clip in one pass.
+
+        queries [1, sum(group_sizes), 3] holds the groups one after another.  The clip is encoded once and the support
+        features are sampled once; each window runs one update loop for all groups together (ct3_update_loop_groups),
+        where every group keeps its own virtual tokens.  Returns the 4-tuple of `forward`; the columns of each group
+        are bit-identical to `forward(video, that group's queries)`.  Streaming (is_online=True) is not grouped."""
+        sizes = [int(g) for g in group_sizes]
+        if not sizes or any(g < 1 for g in sizes) or sum(sizes) != queries.shape[1]:
+            raise engine.EngineError(f"group_sizes {sizes} must be >= 1 each and sum to the {queries.shape[1]} queries")
+        self._check_inputs(video, queries, False)
+        return self._track(video, queries, iters, fmaps_chunk_size, sizes)
 
 
 class CoTrackerThreeOffline(CoTrackerThreeBase):
@@ -188,6 +204,9 @@ class CoTrackerThreeOffline(CoTrackerThreeBase):
     @torch.no_grad()
     def forward(self, video, queries, iters=4, is_train=False, add_space_attn=True, fmaps_chunk_size=200):
         self._check_inputs(video, queries, is_train)
+        return self._track(video, queries, iters, fmaps_chunk_size, [queries.shape[1]])
+
+    def _track(self, video, queries, iters, fmaps_chunk_size, group_sizes):
         B, T, C, H, W = video.shape
         assert T >= 1
         N = queries.shape[1]
@@ -200,7 +219,7 @@ class CoTrackerThreeOffline(CoTrackerThreeBase):
         coords = qcoords[None].expand(T, N, 2).contiguous()
         vis = torch.zeros(T, N, device=video.device)
         conf = torch.zeros(T, N, device=video.device)
-        self._refine(pyr, H4, W4, support, None, coords, vis, conf, iters)
+        self._refine(pyr, H4, W4, support, None, coords, vis, conf, iters, group_sizes)
         return (coords * float(self.stride))[None], torch.sigmoid(vis)[None], torch.sigmoid(conf)[None], None
 
 
@@ -253,6 +272,9 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
     def forward(self, video, queries, iters=4, is_train=False, add_space_attn=True, fmaps_chunk_size=200,
                 is_online=False):
         self._check_inputs(video, queries, is_train)
+        return self._track(video, queries, iters, fmaps_chunk_size, [queries.shape[1]], is_online)
+
+    def _track(self, video, queries, iters, fmaps_chunk_size, group_sizes, is_online=False):
         B, T, C, H, W = video.shape
         dev = video.device
         N = queries.shape[1]
@@ -327,7 +349,7 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
             coords = coords_init.clone().contiguous()
             vis = vis_init.clone().contiguous()
             conf = conf_init.clone().contiguous()
-            self._refine(pyr, H4, W4, support, valid, coords, vis, conf, iters)
+            self._refine(pyr, H4, W4, support, valid, coords, vis, conf, iters, group_sizes)
             S_trim = T if is_online else min(T - ind, S)
             coords_pred[ind:ind + S] = (coords * float(self.stride))[:S_trim]
             vis_pred[ind:ind + S] = vis[:S_trim]

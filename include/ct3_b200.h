@@ -155,6 +155,24 @@ int ct3_update_loop(const void* packed, const float* pyr, int H4, int W4, const 
                     const float* time_emb, int T, int N, int iters, void* workspace,
                     size_t workspace_bytes, ct3_stream_t stream);
 
+/* ---- grouped calls: G independent query sets over one clip in one pass ---------------------------------
+ * The N tracks form G contiguous groups of group_sizes_host[0..G-1] tracks (sum = N).  Each group has its own 64
+ * virtual tokens, and the space attention stays inside its group, so for every group coords/vis/conf (delta) are
+ * BIT-IDENTICAL to a standalone call on that group's tracks alone, whatever the other groups are (default options,
+ * same device).  The groups share every other launch: correlation, corr_mlp, GEMMs, LayerNorms, time attention, heads.
+ * G = 1 is ct3_update_loop / ct3_updateformer.
+ *   group_sizes_host : HOST array of G sizes >= 1; it may be freed when the call returns (the device-side group table
+ *                      lives in the workspace and is filled in stream order; the library still allocates nothing)
+ *   workspace        : ct3_workspace_bytes_groups(T, N, G, H4, W4) bytes (grows by 64*T*G virtual token rows)
+ * A null group array, G < 1, a size < 1 or sizes not summing to N return CT3_EINVAL before anything is enqueued.
+ * Options: the default kernels and the exact-fp32 verification kernels ("gemm" / "corr" / "attn" = 1) support
+ * G > 1; "fuse" = 2 and "attn" = 2 return CT3_EUNSUPPORTED for G > 1. */
+int ct3_workspace_bytes_groups(int T, int N, int G, int H4, int W4, size_t* out_bytes);
+int ct3_update_loop_groups(const void* packed, const float* pyr, int H4, int W4, const float* support,
+                           const uint8_t* track_valid, float* coords, float* vis, float* conf,
+                           const float* time_emb, int T, int N, int iters, void* workspace,
+                           size_t workspace_bytes, ct3_stream_t stream, const int32_t* group_sizes_host, int G);
+
 /* ---- live profiler (bench.py roofline): CUDA events around every launch of the library, summed per
  * kernel category: 0 corr_sample, 1 gemm (wgmma), 2 attention, 3 layernorm, 4 misc.
  * ct3_profile_enable(1) clears and starts recording; ct3_profile_read synchronises and sums. */
@@ -195,6 +213,10 @@ int ct3_split_rows_fp16(const float* x, int rows, int K, int Kpad, void* x_split
  * delta out [N, T, 4] fp32. */
 int ct3_updateformer(const void* packed, const float* x, int T, int N, float* delta, void* workspace,
                      size_t workspace_bytes, ct3_stream_t stream);
+/* The same over G track groups (see ct3_update_loop_groups): N = sum of group_sizes_host; workspace:
+ * ct3_workspace_bytes_groups(T, N, G, 0, 0). */
+int ct3_updateformer_groups(const void* packed, const float* x, int T, const int32_t* group_sizes_host, int G,
+                            float* delta, void* workspace, size_t workspace_bytes, ct3_stream_t stream);
 
 /* ---- the whole CNN encoder (BasicEncoder.forward, blocks.py:190-219; normalise + pyramid,
  * cotracker3_offline.py:92-117) on the tensor-core engine, channels-last ------------------------------------
