@@ -802,6 +802,30 @@ int ct3_prepare_pyramid(const float* fmaps, int T, int H4, int W4, float* pyr, c
   return 0;
 }
 
+int ct3_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c,
+                       int64_t stride_h, int64_t stride_w, int out_h, int out_w, float* out, ct3_stream_t stream) {
+  if (!src || !out) return fail(CT3_EINVAL, "null argument%s");
+  if (T < 1 || H < 1 || W < 1 || out_h < 1 || out_w < 1) return fail(CT3_EINVAL, "T, H, W, out_h and out_w must be >= 1%s");
+  if (dtype != CT3_FRAMES_U8 && dtype != CT3_FRAMES_F32) return fail(CT3_EINVAL, "unknown frame dtype%s");
+  // every source offset sum |stride| * index must fit in int64, in bytes
+  const int64_t sizes[4] = {T, 3, H, W}, strides[4] = {stride_t, stride_c, stride_h, stride_w};
+  const int64_t esize = dtype == CT3_FRAMES_U8 ? 1 : 4;
+  int64_t extent = 0;
+  for (int i = 0; i < 4; ++i) {
+    if (strides[i] == INT64_MIN) return fail(CT3_EINVAL, "stride extent overflows int64%s");
+    const int64_t a = strides[i] < 0 ? -strides[i] : strides[i], m = sizes[i] - 1;
+    if (m > 0 && a > (INT64_MAX - extent) / m) return fail(CT3_EINVAL, "stride extent overflows int64%s");
+    extent += a * m;
+  }
+  if (extent > INT64_MAX / esize) return fail(CT3_EINVAL, "stride extent overflows int64%s");
+  // the kernel indexes the pixels of one output plane with int
+  if ((int64_t)out_h * out_w > INT32_MAX) return fail(CT3_EINVAL, "output plane too large%s");
+  if ((int64_t)out_h * out_w > INT64_MAX / 12 / T) return fail(CT3_EINVAL, "output too large%s");
+  CK(launch_prepare_frames(src, dtype, T, H, W, stride_t, stride_c, stride_h, stride_w, out_h, out_w, out,
+                           (cudaStream_t)stream), "prepare_frames");
+  return 0;
+}
+
 int ct3_sample_support(const float* pyr, int T, int H4, int W4, const int32_t* queried_frames,
                        const float* queried_coords, int N, const uint8_t* accumulate_mask, float* support,
                        ct3_stream_t stream) {

@@ -19,6 +19,12 @@ cudaError_t launch_sample_support(const float* pyr, int T, int H4, int W4, const
 // pools levels 1..3 from an already normalised channels-last level 0 living in `pyr`
 cudaError_t launch_pyramid_pools(int T, int H4, int W4, float* pyr, cudaStream_t s);
 
+// ---- ingest.cu : raw frames -> encoder input ------------------------------------------------------
+// src [T,3,H,W] (element strides st, sc, sh, sw; dtype CT3_FRAMES_U8 | CT3_FRAMES_F32) -> out [T,3,oh,ow] fp32 contiguous
+// = 2 * (bilinear(align_corners=True) / 255) - 1, bit-identical to the ATen expression (see ingest.cu)
+cudaError_t launch_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t st, int64_t sc, int64_t sh,
+                                  int64_t sw, int oh, int ow, float* out, cudaStream_t s);
+
 // ---- enc_tail.cu : conv2 -> InstanceNorm -> ReLU -> conv3 of the encoder on the GEMM engine --------
 cudaError_t launch_im2col3x3_split(const float* in, int T, int C, int H, int W, int Kpad, __nv_bfloat16* out,
                                    cudaStream_t s);

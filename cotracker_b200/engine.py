@@ -27,7 +27,7 @@ class EngineError(RuntimeError):
 
 def _declare(lib):
     c_int, c_size_t, c_void_p, c_char_p = ctypes.c_int, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_char_p
-    i64p = ctypes.POINTER(ctypes.c_int64)
+    i64, i64p = ctypes.c_int64, ctypes.POINTER(ctypes.c_int64)
     intp = ctypes.POINTER(ctypes.c_int)
     sig = {
         "ct3_version": (c_int, []),
@@ -42,6 +42,8 @@ def _declare(lib):
         "ct3_pack_weights": (c_int, [ctypes.POINTER(c_void_p), c_int, c_void_p, c_size_t, c_void_p]),
         "ct3_pyramid_layout": (c_int, [c_int, c_int, c_int, i64p, intp, intp, i64p]),
         "ct3_prepare_pyramid": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+        "ct3_prepare_frames": (c_int, [c_void_p, c_int, c_int, c_int, c_int, i64, i64, i64, i64, c_int, c_int, c_void_p,
+                                       c_void_p]),
         "ct3_sample_support": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
         "ct3_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
         "ct3_update_loop": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -89,6 +91,7 @@ EXPORTED_SYMBOLS = [
     "ct3_encoder_workspace_bytes", "ct3_encoder",
     "ct3_upsample_concat", "ct3_enc_tail_packed_bytes", "ct3_enc_tail_pack", "ct3_enc_tail_workspace_bytes", "ct3_enc_tail",
     "ct3_workspace_bytes_groups", "ct3_update_loop_groups", "ct3_updateformer_groups",
+    "ct3_prepare_frames",
 ]
 
 
@@ -211,6 +214,32 @@ def prepare_pyramid(fmaps: torch.Tensor) -> torch.Tensor:
     with torch.cuda.device(fmaps.device):
         _check(lib().ct3_prepare_pyramid(_ptr(fmaps), T, H4, W4, _ptr(pyr), _stream(fmaps.device)), "ct3_prepare_pyramid")
     return pyr
+
+
+FRAME_DTYPES = {torch.uint8: 0, torch.float32: 1}   # CT3_FRAMES_U8, CT3_FRAMES_F32
+
+
+def prepare_frames(src: torch.Tensor, out_hw, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """src [T,3,H,W] uint8 or float32 CUDA tensor with any strides (e.g. a permuted [T,H,W,3] decoder buffer) ->
+    [T,3,oh,ow] fp32 = 2 * (bilinear(align_corners=True) resize / 255) - 1, bit-identical to the ATen expression.
+    out: optional contiguous fp32 destination of that shape."""
+    if not src.is_cuda:
+        raise EngineError("src must be a CUDA tensor (no CPU fallback)")
+    if src.dtype not in FRAME_DTYPES:
+        raise EngineError(f"src must be uint8 or float32, got {src.dtype}")
+    if src.dim() != 4 or src.shape[1] != 3:
+        raise EngineError(f"src must be [T,3,H,W], got {tuple(src.shape)}")
+    T, _, H, W = src.shape
+    oh, ow = int(out_hw[0]), int(out_hw[1])
+    if out is None:
+        out = torch.empty(T, 3, oh, ow, dtype=torch.float32, device=src.device)
+    _req(out, torch.float32, "out")
+    if tuple(out.shape) != (T, 3, oh, ow) or out.device != src.device:
+        raise EngineError(f"out must be [{T},3,{oh},{ow}] on {src.device}")
+    with torch.cuda.device(src.device):
+        _check(lib().ct3_prepare_frames(_ptr(src), FRAME_DTYPES[src.dtype], T, H, W, *src.stride(), oh, ow, _ptr(out),
+                                        _stream(src.device)), "ct3_prepare_frames")
+    return out
 
 
 def pyramid_levels(pyr: torch.Tensor, T: int, H4: int, W4: int) -> List[torch.Tensor]:
@@ -471,6 +500,25 @@ def slice_pyramid(pyr: torch.Tensor, T: int, H4: int, W4: int, t0: int, S: int) 
         per = h[l] * w[l] * LATENT
         parts.append(pyr[off[l] + t0 * per: off[l] + (t0 + S) * per])
     return torch.cat(parts)
+
+
+def reverse_pyramid_(pyr: torch.Tensor, T: int, H4: int, W4: int, pad: int = 0, block: int = 4) -> torch.Tensor:
+    """In place: turn the flat pyramid of a clip's T frames plus `pad` copies of frame T-1 into the pyramid of the clip
+    played backwards, frames T-1 .. 0 plus `pad` copies of (original) frame 0.  The encoder is strictly per frame, so
+    this is the pyramid of the reversed, likewise padded clip, without encoding it again.  Applying it twice restores
+    the original bit for bit.  Frames are swapped `block` mirrored pairs at a time, so the scratch is at most 3 * block
+    frames of level 0, never a second pyramid."""
+    for lv in pyramid_levels(pyr, T + pad, H4, W4):
+        half = T // 2
+        for i in range(0, half, block):
+            m = min(block, half - i)
+            a, b = lv[i:i + m], lv[T - i - m:T - i]      # disjoint: i + m <= T // 2 <= T - i - m
+            tmp = a.clone()
+            a.copy_(b.flip(0))
+            b.copy_(tmp.flip(0))
+        if pad > 0:
+            lv[T:].copy_(lv[T - 1:T].expand(pad, -1, -1, -1))
+    return pyr
 
 
 def concat_pyramid_frames(pyr_a: torch.Tensor, Ta: int, a0: int, pyr_b: torch.Tensor, Tb: int, H4: int, W4: int):

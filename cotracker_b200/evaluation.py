@@ -8,8 +8,9 @@ Jaccard (AJ) at 1/2/4/8/16 px.  `EvaluationPredictor` wraps a cotracker_b200 off
 reference's benchmark code drives it: one query point at a time with an 8x8 local grid and a 5x5 global grid as
 helper tracks (single_point=True, the TAP-Vid protocol), or all queries jointly.  The model behind it is the same
 CUDA path as everywhere else (libct3_b200.so); SIFT helper points (sift_size > 0) are not provided.
-In single-point mode every query's 90-track set is one group of `forward_groups`: the clip is encoded once per pass
-and all groups share one update loop, in as few passes as fit in device memory (`plan_passes`).  Each group's result
+In single-point mode every query's 90-track set is one group of a grouped update loop (as `forward_groups`): the clip
+is resized (cotracker_b200.ingest) and encoded once, and all groups share one update loop, in as few passes as fit in
+device memory (`plan_passes`).  Each group's result
 is bit-identical to a model call on that group alone, so the split into passes does not change the output.
 With no datasets or checkpoints in this environment the harness is exercised by scoring the CUDA tracks against
 the reference's tracks on synthetic clips (tests/test_evaluation.py): identical outputs score 1.0 everywhere.
@@ -20,7 +21,6 @@ from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
-import torch.nn.functional as F
 
 THRESHOLDS = (1, 2, 4, 8, 16)
 
@@ -162,13 +162,15 @@ class EvaluationPredictor(torch.nn.Module):
 
     @torch.no_grad()
     def forward(self, video, queries):
+        from . import ingest
         B, T, C, H, W = video.shape
         assert queries.shape[0] == 1 and queries.shape[2] == 3 and B == 1
         N = queries.shape[1]
         ih, iw = self.interp_shape
-        video = F.interpolate(video.reshape(B * T, C, H, W), (ih, iw), mode="bilinear", align_corners=True)
-        video = video.reshape(B, T, 3, ih, iw)
-        queries = queries.clone()
+        dev = ingest.model_device(self.model)
+        frames = ingest.prepare_video(video, (ih, iw), dev)
+        video = frames[None]                               # [1,T,3,ih,iw]: the shape and device the helpers use
+        queries = queries.to(dev).clone()
         queries[:, :, 1] *= (iw - 1) / (W - 1)
         queries[:, :, 2] *= (ih - 1) / (H - 1)
         if self.single_point:
@@ -186,16 +188,18 @@ class EvaluationPredictor(torch.nn.Module):
             budget = self.pass_budget_bytes
             if budget is None:
                 budget = self._free_bytes(video, T, ih, iw)
+            pyr = self.model._encode_clip(frames)          # every pass runs on the same pyramid
+            del frames, video
             for g0, g1 in plan_passes(sizes, T_loop, ih // stride, iw // stride, budget):
                 a, b = first[g0], first[g1]
-                tr, vi, cf, _ = self.model.forward_groups(video, q_all[:, a:b], sizes[g0:g1], iters=self.n_iters)
+                tr, vi, cf, _ = self.model._track_pyramid(pyr, T, ih, iw, q_all[:, a:b], self.n_iters, sizes[g0:g1])
                 cols = [first[g] - a for g in range(g0, g1)]
                 tracks[:, :, g0:g1] = tr[:, :, cols, :2]
                 vis[:, :, g0:g1] = vi[:, :, cols]
                 conf[:, :, g0:g1] = cf[:, :, cols]
         else:
             q_all = torch.cat([queries, self._helpers(video, None)], dim=1)
-            tr, vi, cf, _ = self.model(video=video, queries=q_all, iters=self.n_iters)
+            tr, vi, cf, _ = self.model._track_frames(frames, q_all, iters=self.n_iters)
             tracks, vis, conf = tr[:, :, :N].clone(), vi[:, :, :N], cf[:, :, :N]
         tracks[..., 0] *= (W - 1) / float(iw - 1)
         tracks[..., 1] *= (H - 1) / float(ih - 1)

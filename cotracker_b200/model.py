@@ -197,6 +197,37 @@ class CoTrackerThreeBase(nn.Module):
         self._check_inputs(video, queries, False)
         return self._track(video, queries, iters, fmaps_chunk_size, sizes)
 
+    # -- internal entry points of the predictors: frames already resized and normalised (cotracker_b200.ingest) --------
+    def _check_frames(self, frames, queries):
+        if frames.dim() != 4 or frames.shape[1] != 3 or queries.shape[0] != 1:
+            raise ValueError("frames must be [T,3,H,W] and queries [1,N,3] (B == 1)")
+        if not frames.is_cuda:
+            raise engine.EngineError("cotracker_b200 runs on CUDA only; move the module and inputs to a GPU")
+        assert frames.shape[2] % self.stride == 0 and frames.shape[3] % self.stride == 0
+
+    def _clip_pad(self, T: int) -> int:
+        """Frames the model appends (copies of the last frame) before encoding a T-frame clip."""
+        return 0
+
+    def _encode_clip(self, frames, fmaps_chunk_size=200) -> torch.Tensor:
+        """frames [T,3,H,W] in [-1,1] -> the pyramid `_track_pyramid` expects (with the model's padding frames)."""
+        pad = self._clip_pad(frames.shape[0])
+        if pad > 0:
+            frames = torch.cat([frames, frames[-1:].expand(pad, -1, -1, -1)], 0)
+        return self._encode(frames.contiguous(), fmaps_chunk_size)
+
+    def _reverse_clip_pyramid_(self, pyr, T: int, H: int, W: int) -> torch.Tensor:
+        """In place: `_encode_clip` of a T-frame clip -> `_encode_clip` of the clip played backwards (no encoder pass,
+        no second pyramid); applying it again restores the original."""
+        return engine.reverse_pyramid_(pyr, T, H // self.stride, W // self.stride, self._clip_pad(T))
+
+    def _track_frames(self, frames, queries, iters=4, group_sizes=None, fmaps_chunk_size=200):
+        """`forward` on frames [T,3,H,W] already scaled to [-1,1] (the predictors' path)."""
+        self._check_frames(frames, queries)
+        T, _, H, W = frames.shape
+        return self._track_pyramid(self._encode_clip(frames, fmaps_chunk_size), T, H, W, queries, iters,
+                                   group_sizes or [queries.shape[1]])
+
 
 class CoTrackerThreeOffline(CoTrackerThreeBase):
     """Whole clip = one window (reference cotracker3_offline.py)."""
@@ -209,16 +240,20 @@ class CoTrackerThreeOffline(CoTrackerThreeBase):
     def _track(self, video, queries, iters, fmaps_chunk_size, group_sizes):
         B, T, C, H, W = video.shape
         assert T >= 1
-        N = queries.shape[1]
-        H4, W4 = H // self.stride, W // self.stride
         frames = 2.0 * (video[0].float() / 255.0) - 1.0
         pyr = self._encode(frames, fmaps_chunk_size)
+        return self._track_pyramid(pyr, T, H, W, queries, iters, group_sizes)
+
+    def _track_pyramid(self, pyr, T, H, W, queries, iters, group_sizes):
+        """The model after the encoder: pyr = the clip's pyramid (`_encode_clip`), T frames of H x W pixels."""
+        N = queries.shape[1]
+        H4, W4 = H // self.stride, W // self.stride
         qframes = queries[0, :, 0].long().to(torch.int32).contiguous()
         qcoords = (queries[0, :, 1:3].float() / self.stride).contiguous()
         support = engine.sample_support(pyr, T, H4, W4, qframes, qcoords)
         coords = qcoords[None].expand(T, N, 2).contiguous()
-        vis = torch.zeros(T, N, device=video.device)
-        conf = torch.zeros(T, N, device=video.device)
+        vis = torch.zeros(T, N, device=pyr.device)
+        conf = torch.zeros(T, N, device=pyr.device)
         self._refine(pyr, H4, W4, support, None, coords, vis, conf, iters, group_sizes)
         return (coords * float(self.stride))[None], torch.sigmoid(vis)[None], torch.sigmoid(conf)[None], None
 
@@ -274,23 +309,41 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
         self._check_inputs(video, queries, is_train)
         return self._track(video, queries, iters, fmaps_chunk_size, [queries.shape[1]], is_online)
 
+    def _clip_pad(self, T: int) -> int:
+        S = self.window_len
+        return (S - T % S) % S
+
     def _track(self, video, queries, iters, fmaps_chunk_size, group_sizes, is_online=False):
-        B, T, C, H, W = video.shape
-        dev = video.device
-        N = queries.shape[1]
+        frames = 2.0 * (video[0].float() / 255.0) - 1.0
+        return self._track_normalised(frames, queries, iters, fmaps_chunk_size, group_sizes, is_online)
+
+    def _track_frames(self, frames, queries, iters=4, group_sizes=None, fmaps_chunk_size=200, is_online=False):
+        self._check_frames(frames, queries)
+        return self._track_normalised(frames, queries, iters, fmaps_chunk_size, group_sizes or [queries.shape[1]],
+                                      is_online)
+
+    def _track_normalised(self, frames, queries, iters, fmaps_chunk_size, group_sizes, is_online):
+        T, _, H, W = frames.shape
         S = self.window_len
         assert S >= 2
         if is_online:
             assert T <= S, "Online mode: video chunk must be <= window size."
             assert getattr(self, "online_ind", None) is not None, "Call model.init_video_online_processing() first."
+            H4, W4 = H // self.stride, W // self.stride
+            frames = torch.cat([frames, frames[-1:].expand(S - T, -1, -1, -1)], 0) if S > T else frames
+            pyr_all = self._encode_online(frames, fmaps_chunk_size, S // 2, H4, W4)
+        else:
+            pyr_all = self._encode_clip(frames, fmaps_chunk_size)
+        return self._track_pyramid(pyr_all, T, H, W, queries, iters, group_sizes, is_online)
+
+    def _track_pyramid(self, pyr_all, T, H, W, queries, iters, group_sizes, is_online=False):
+        """The model after the encoder: pyr_all = the pyramid of the T frames and the padding (`_encode_clip`)."""
+        dev = pyr_all.device
+        N = queries.shape[1]
+        S = self.window_len
         step = S // 2
         H4, W4 = H // self.stride, W // self.stride
-
-        frames = 2.0 * (video[0].float() / 255.0) - 1.0
-        pad = (S - T) if is_online else (S - T % S) % S
-        if pad > 0:
-            frames = torch.cat([frames, frames[-1:].expand(pad, -1, -1, -1)], 0)
-        T_pad = frames.shape[0]
+        T_pad = T + ((S - T) if is_online else self._clip_pad(T))
         qframes_l = queries[0, :, 0].long()
         qcoords = (queries[0, :, 1:3].float() / self.stride).contiguous()
 
@@ -302,9 +355,6 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
             coords_pred = F.pad(self.online_coords_predicted, (0, 0, 0, 0, 0, grow))
             vis_pred = F.pad(self.online_vis_predicted, (0, 0, 0, grow))
             conf_pred = F.pad(self.online_conf_predicted, (0, 0, 0, grow))
-
-        pyr_all = self._encode_online(frames, fmaps_chunk_size, step, H4, W4) if is_online \
-            else self._encode(frames, fmaps_chunk_size)
 
         # support features of every track at its query frame
         if is_online:

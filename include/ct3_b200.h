@@ -96,6 +96,19 @@ int ct3_packed_weights_bytes(size_t* out_bytes);
 int ct3_pack_weights(const float* const* tensors_host_array_of_device_ptrs, int n_tensors,
                      void* packed, size_t packed_bytes, ct3_stream_t stream);
 
+/* ---- raw frames -> encoder input -------------------------------------------
+ * ct3_prepare_frames: the predictors' resize + normalisation (predictor.py:60-64, cotracker3_offline.py:63) in one
+ * kernel.  src: T frames [T,3,H,W] of element type `dtype` (CT3_FRAMES_*) at arbitrary int64 ELEMENT strides
+ * (stride_t, stride_c, stride_h, stride_w), so a channels-last [T,H,W,3] decoder buffer is read in place.
+ * out: [T,3,out_h,out_w] fp32 contiguous, bit-identical to
+ *     2 * (F.interpolate(src.float(), (out_h, out_w), mode="bilinear", align_corners=True) / 255) - 1
+ * as PyTorch evaluates it on the GPU.  Null pointers, T/H/W/out_h/out_w < 1, an unknown dtype or a stride extent
+ * (sum of |stride| * (size - 1), in bytes) or output size beyond int64, or an output plane out_h * out_w above
+ * INT32_MAX pixels return CT3_EINVAL before any launch. */
+enum { CT3_FRAMES_U8 = 0, CT3_FRAMES_F32 = 1 };
+int ct3_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c,
+                       int64_t stride_h, int64_t stride_w, int out_h, int out_w, float* out, ct3_stream_t stream);
+
 /* ---- per-clip preparation ---------------------------------------------------
  * ct3_prepare_pyramid: cotracker3_offline.py:92-117 (L2-normalise over channels,
  * 3x avg_pool2d(2,2)).  in: fnet output [T,128,H4,W4] fp32 channel-planar.
