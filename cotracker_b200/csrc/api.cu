@@ -802,27 +802,80 @@ int ct3_prepare_pyramid(const float* fmaps, int T, int H4, int W4, float* pyr, c
   return 0;
 }
 
+// every source offset sum |stride| * index of a [T,3,H,W] frame tensor must fit in int64, in bytes
+static bool frame_extent_fits(int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c, int64_t stride_h,
+                              int64_t stride_w) {
+  const int64_t sizes[4] = {T, 3, H, W}, strides[4] = {stride_t, stride_c, stride_h, stride_w};
+  const int64_t esize = dtype == CT3_FRAMES_U8 ? 1 : 4;
+  int64_t extent = 0;
+  for (int i = 0; i < 4; ++i) {
+    if (strides[i] == INT64_MIN) return false;
+    const int64_t a = strides[i] < 0 ? -strides[i] : strides[i], m = sizes[i] - 1;
+    if (m > 0 && a > (INT64_MAX - extent) / m) return false;
+    extent += a * m;
+  }
+  return extent <= INT64_MAX / esize;
+}
+
 int ct3_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c,
                        int64_t stride_h, int64_t stride_w, int out_h, int out_w, float* out, ct3_stream_t stream) {
   if (!src || !out) return fail(CT3_EINVAL, "null argument%s");
   if (T < 1 || H < 1 || W < 1 || out_h < 1 || out_w < 1) return fail(CT3_EINVAL, "T, H, W, out_h and out_w must be >= 1%s");
   if (dtype != CT3_FRAMES_U8 && dtype != CT3_FRAMES_F32) return fail(CT3_EINVAL, "unknown frame dtype%s");
-  // every source offset sum |stride| * index must fit in int64, in bytes
-  const int64_t sizes[4] = {T, 3, H, W}, strides[4] = {stride_t, stride_c, stride_h, stride_w};
-  const int64_t esize = dtype == CT3_FRAMES_U8 ? 1 : 4;
-  int64_t extent = 0;
-  for (int i = 0; i < 4; ++i) {
-    if (strides[i] == INT64_MIN) return fail(CT3_EINVAL, "stride extent overflows int64%s");
-    const int64_t a = strides[i] < 0 ? -strides[i] : strides[i], m = sizes[i] - 1;
-    if (m > 0 && a > (INT64_MAX - extent) / m) return fail(CT3_EINVAL, "stride extent overflows int64%s");
-    extent += a * m;
-  }
-  if (extent > INT64_MAX / esize) return fail(CT3_EINVAL, "stride extent overflows int64%s");
+  if (!frame_extent_fits(dtype, T, H, W, stride_t, stride_c, stride_h, stride_w))
+    return fail(CT3_EINVAL, "stride extent overflows int64%s");
   // the kernel indexes the pixels of one output plane with int
   if ((int64_t)out_h * out_w > INT32_MAX) return fail(CT3_EINVAL, "output plane too large%s");
   if ((int64_t)out_h * out_w > INT64_MAX / 12 / T) return fail(CT3_EINVAL, "output too large%s");
   CK(launch_prepare_frames(src, dtype, T, H, W, stride_t, stride_c, stride_h, stride_w, out_h, out_w, out,
                            (cudaStream_t)stream), "prepare_frames");
+  return 0;
+}
+
+// ---- track visualiser (render.cu) ------------------------------------------------------------------------------
+int ct3_render_prepare(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c,
+                       int64_t stride_h, int64_t stride_w, int pad, int grayscale, uint8_t* out, ct3_stream_t stream) {
+  if (!src || !out) return fail(CT3_EINVAL, "null argument%s");
+  if (T < 1 || H < 1 || W < 1) return fail(CT3_EINVAL, "T, H and W must be >= 1%s");
+  if (T > 65535) return fail(CT3_EINVAL, "T must be <= 65535%s");
+  if (pad < 0) return fail(CT3_EINVAL, "pad must be >= 0%s");
+  if (grayscale != 0 && grayscale != 1) return fail(CT3_EINVAL, "grayscale must be 0 or 1%s");
+  if (dtype != CT3_FRAMES_U8 && dtype != CT3_FRAMES_F32) return fail(CT3_EINVAL, "unknown frame dtype%s");
+  if (!frame_extent_fits(dtype, T, H, W, stride_t, stride_c, stride_h, stride_w))
+    return fail(CT3_EINVAL, "stride extent overflows int64%s");
+  const int64_t ho = (int64_t)H + 2 * (int64_t)pad, wo = (int64_t)W + 2 * (int64_t)pad;
+  if (ho > INT32_MAX || wo > INT32_MAX || ho * wo > INT32_MAX) return fail(CT3_EINVAL, "output plane too large%s");
+  CK(launch_render_prepare(src, dtype, T, H, W, stride_t, stride_c, stride_h, stride_w, pad, grayscale, out,
+                           (cudaStream_t)stream), "render_prepare");
+  return 0;
+}
+
+int ct3_render_workspace_bytes(int T, int H, int W, int N, int trail, size_t* out_bytes) {
+  if (!out_bytes) return fail(CT3_EINVAL, "null argument%s");
+  if (T < 1 || H < 1 || W < 1 || N < 1) return fail(CT3_EINVAL, "T, H, W and N must be >= 1%s");
+  if (T > 65535) return fail(CT3_EINVAL, "T must be <= 65535%s");
+  if (trail < -1) return fail(CT3_EINVAL, "trail must be >= -1%s");
+  if ((int64_t)H * W > INT32_MAX) return fail(CT3_EINVAL, "frame plane too large%s");
+  if ((int64_t)T * N > INT32_MAX) return fail(CT3_EINVAL, "T * N too large%s");   // draw-order keys u * N + i
+  *out_bytes = align_up((size_t)T * H * W * sizeof(int32_t));
+  return 0;
+}
+
+int ct3_render_tracks(uint8_t* frames, int T, int H, int W, const float* pts, const uint8_t* visible,
+                      const uint8_t* colors, const uint8_t* draw_mask, int N, int radius, int linewidth, int trail,
+                      int query_frame, const double* alphas, const double* diff, void* workspace,
+                      size_t workspace_bytes, ct3_stream_t stream) {
+  if (!frames || !pts || !colors || !workspace) return fail(CT3_EINVAL, "null argument%s");
+  size_t need = 0;
+  if (int rc = ct3_render_workspace_bytes(T, H, W, N, trail, &need)) return rc;
+  if (radius < 0 || radius > kRenderMaxRadius) return fail(CT3_EINVAL, "radius must be in [0, 255]%s");
+  if (linewidth < 0) return fail(CT3_EINVAL, "linewidth must be >= 0%s");
+  if (query_frame < 0 || query_frame >= T) return fail(CT3_EINVAL, "query_frame must be in [0, T)%s");
+  if (trail > 0 && !alphas) return fail(CT3_EINVAL, "trail > 0 needs the blend weights (alphas)%s");
+  if (workspace_bytes < need) return fail(CT3_ENOSPC, "workspace too small%s");
+  CK(launch_render_tracks(frames, T, H, W, pts, visible, colors, draw_mask, N, radius, linewidth, trail, query_frame,
+                          alphas, diff, static_cast<int*>(workspace), (cudaStream_t)stream),
+     "render_tracks");
   return 0;
 }
 

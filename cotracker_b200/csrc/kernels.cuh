@@ -25,6 +25,16 @@ cudaError_t launch_pyramid_pools(int T, int H4, int W4, float* pyr, cudaStream_t
 cudaError_t launch_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t st, int64_t sc, int64_t sh,
                                   int64_t sw, int oh, int ow, float* out, cudaStream_t s);
 
+// ---- render.cu : the track visualiser on uint8 frames [T,H,W,3] (arguments validated by ct3_render_*) ----------
+constexpr int kRenderMaxRadius = 255;   // largest point radius (int(linewidth * 2)) the footprint table holds
+cudaError_t launch_render_prepare(const void* src, int dtype, int T, int H, int W, int64_t st, int64_t sc, int64_t sh,
+                                  int64_t sw, int pad, int gray, uint8_t* out, cudaStream_t s);
+// keys: T*H*W int32 scratch, any content on entry, all -1 on return
+cudaError_t launch_render_tracks(uint8_t* frames, int T, int H, int W, const float* pts, const uint8_t* visible,
+                                 const uint8_t* colors, const uint8_t* draw_mask, int N, int radius, int linewidth,
+                                 int trail, int query_frame, const double* alphas, const double* diff, int* keys,
+                                 cudaStream_t s);
+
 // ---- enc_tail.cu : conv2 -> InstanceNorm -> ReLU -> conv3 of the encoder on the GEMM engine --------
 cudaError_t launch_im2col3x3_split(const float* in, int T, int C, int H, int W, int Kpad, __nv_bfloat16* out,
                                    cudaStream_t s);

@@ -44,6 +44,11 @@ def _declare(lib):
         "ct3_prepare_pyramid": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_prepare_frames": (c_int, [c_void_p, c_int, c_int, c_int, c_int, i64, i64, i64, i64, c_int, c_int, c_void_p,
                                        c_void_p]),
+        "ct3_render_prepare": (c_int, [c_void_p, c_int, c_int, c_int, c_int, i64, i64, i64, i64, c_int, c_int, c_void_p,
+                                       c_void_p]),
+        "ct3_render_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+        "ct3_render_tracks": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                      c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
         "ct3_sample_support": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
         "ct3_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
         "ct3_update_loop": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -92,6 +97,7 @@ EXPORTED_SYMBOLS = [
     "ct3_upsample_concat", "ct3_enc_tail_packed_bytes", "ct3_enc_tail_pack", "ct3_enc_tail_workspace_bytes", "ct3_enc_tail",
     "ct3_workspace_bytes_groups", "ct3_update_loop_groups", "ct3_updateformer_groups",
     "ct3_prepare_frames",
+    "ct3_render_prepare", "ct3_render_workspace_bytes", "ct3_render_tracks",
 ]
 
 
@@ -240,6 +246,63 @@ def prepare_frames(src: torch.Tensor, out_hw, out: Optional[torch.Tensor] = None
         _check(lib().ct3_prepare_frames(_ptr(src), FRAME_DTYPES[src.dtype], T, H, W, *src.stride(), oh, ow, _ptr(out),
                                         _stream(src.device)), "ct3_prepare_frames")
     return out
+
+
+def render_prepare(src: torch.Tensor, pad: int, grayscale: bool) -> torch.Tensor:
+    """src [T,3,H,W] uint8 or float32 CUDA tensor, any strides -> [T,H+2p,W+2p,3] uint8: the visualiser's pad with
+    255, optional Grayscale (repeated to 3 channels) and .byte(), bit-identical to the reference's CPU ops."""
+    if not src.is_cuda:
+        raise EngineError("src must be a CUDA tensor (no CPU fallback)")
+    if src.dtype not in FRAME_DTYPES:
+        raise EngineError(f"src must be uint8 or float32, got {src.dtype}")
+    if src.dim() != 4 or src.shape[1] != 3:
+        raise EngineError(f"src must be [T,3,H,W], got {tuple(src.shape)}")
+    T, _, H, W = src.shape
+    p = int(pad)
+    out = torch.empty(T, H + 2 * p, W + 2 * p, 3, dtype=torch.uint8, device=src.device)
+    with torch.cuda.device(src.device):
+        _check(lib().ct3_render_prepare(_ptr(src), FRAME_DTYPES[src.dtype], T, H, W, *src.stride(), p, int(bool(grayscale)),
+                                        _ptr(out), _stream(src.device)), "ct3_render_prepare")
+    return out
+
+
+def render_workspace_bytes(T: int, H: int, W: int, N: int, trail: int) -> int:
+    n = ctypes.c_size_t(0)
+    _check(lib().ct3_render_workspace_bytes(T, H, W, N, trail, ctypes.byref(n)), "ct3_render_workspace_bytes")
+    return n.value
+
+
+def render_tracks(frames: torch.Tensor, pts: torch.Tensor, colors: torch.Tensor, radius: int, linewidth: int,
+                  trail: int = 0, query_frame: int = 0, visible: Optional[torch.Tensor] = None,
+                  draw_mask: Optional[torch.Tensor] = None, alphas: Optional[torch.Tensor] = None,
+                  diff: Optional[torch.Tensor] = None, workspace: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Draw trails and points in place on frames [T,H,W,3] uint8 (see ct3_render_tracks in include/ct3_b200.h).
+    pts [T,N,2] fp32, colors [T,N,3] uint8, visible [T,N] uint8, draw_mask [N] uint8, alphas [T,S,2] / diff [T,S+1,2]
+    fp64; all on the frames' device.  Returns frames."""
+    _req(frames, torch.uint8, "frames")
+    if frames.dim() != 4 or frames.shape[3] != 3:
+        raise EngineError(f"frames must be [T,H,W,3], got {tuple(frames.shape)}")
+    T, H, W, _ = frames.shape
+    dev = frames.device
+    N = pts.shape[1] if pts.dim() == 3 else -1
+    want = {"pts": (pts, torch.float32, (T, N, 2)), "colors": (colors, torch.uint8, (T, N, 3)),
+            "visible": (visible, torch.uint8, (T, N)), "draw_mask": (draw_mask, torch.uint8, (N,)),
+            "alphas": (alphas, torch.float64, None), "diff": (diff, torch.float64, None)}
+    for name, (t, dtype, shape) in want.items():
+        if t is None:
+            continue
+        _req(t, dtype, name)
+        if t.device != dev or (shape is not None and tuple(t.shape) != shape):
+            raise EngineError(f"{name} must be {shape} on {dev}, got {tuple(t.shape)} on {t.device}")
+    nbytes = render_workspace_bytes(T, H, W, N, trail)
+    if workspace is None:
+        workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _check(lib().ct3_render_tracks(_ptr(frames), T, H, W, _ptr(pts), _ptr(visible), _ptr(colors), _ptr(draw_mask), N,
+                                       int(radius), int(linewidth), int(trail), int(query_frame), _ptr(alphas),
+                                       _ptr(diff), _ptr(workspace), workspace.numel(), _stream(dev)),
+               "ct3_render_tracks")
+    return frames
 
 
 def pyramid_levels(pyr: torch.Tensor, T: int, H4: int, W4: int) -> List[torch.Tensor]:

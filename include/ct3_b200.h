@@ -109,6 +109,41 @@ enum { CT3_FRAMES_U8 = 0, CT3_FRAMES_F32 = 1 };
 int ct3_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c,
                        int64_t stride_h, int64_t stride_w, int out_h, int out_w, float* out, ct3_stream_t stream);
 
+/* ---- track visualiser (reference cotracker/utils/visualizer.py) ---------------
+ * Frames are uint8 [T,H,W,3] contiguous on the device, drawn in place; every result is bit-identical to the reference's
+ * PIL drawing (footprint rules: render.cu).  T <= 65535.
+ *
+ * ct3_render_prepare: visualize()'s F.pad(video, (pad,)*4, value=255), optional transforms.Grayscale() repeated to 3
+ * channels (float32 arithmetic, no contraction) and .byte() (truncation) in one kernel.  src: T frames [T,3,H,W] of
+ * element type `dtype` (CT3_FRAMES_*) at any int64 element strides.  out: [T, H+2*pad, W+2*pad, 3] uint8.
+ * Null pointers, T/H/W < 1, pad < 0, grayscale not 0|1, an unknown dtype, a stride extent beyond int64 bytes or an
+ * output plane above INT32_MAX pixels return CT3_EINVAL before any launch. */
+int ct3_render_prepare(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c,
+                       int64_t stride_h, int64_t stride_w, int pad, int grayscale, uint8_t* out, ct3_stream_t stream);
+/* Scratch of ct3_render_tracks: one int32 draw-order key per pixel.  CT3_EINVAL unless T, H, W, N >= 1, trail >= -1,
+ * H*W <= INT32_MAX and T*N <= INT32_MAX. */
+int ct3_render_workspace_bytes(int T, int H, int W, int N, int trail, size_t* out_bytes);
+/* ct3_render_tracks: draw_tracks_on_video's trails and points (visualizer.py:238-288) on `frames`.
+ *   pts        [T,N,2] fp32 (x, y) frame pixel coordinates, truncated toward zero as tracks.long() does; a point is
+ *              drawn when both truncated coordinates are non-zero.  Coordinates that are not finite or whose magnitude
+ *              is at least 2^30 draw nothing.
+ *   visible    [T,N] uint8 or NULL (all visible): a visible point is a filled disc, a hidden one its outline only
+ *   colors     [T,N,3] uint8: colour of track i at frame t (trail segments use the colour of their start frame)
+ *   draw_mask  [N] uint8 or NULL: only tracks with a non-zero entry are drawn (compensate_for_camera_motion)
+ *   radius     point radius int(linewidth * 2), 0..255;  linewidth: trail line width, >= 0
+ *   trail      tracks_leave_trace: 0 no trails; -1 every earlier step, unblended; > 0 the last `trail` steps, each
+ *              step blended with the frame it was drawn on.  Trails are drawn on frames query_frame+1 .. T-1.
+ *              With S = min(trail, T-1) (T-1 for -1) steps at most per frame and first(t) = max(0, t - trail) (0 for
+ *              -1), step s of frame t is the segment from frame first(t)+s to first(t)+s+1.
+ *   alphas     [T,S,2] fp64 (a, 1-a) with a = (s/L)**2, L = t - first(t) + 1; required when trail > 0
+ *   diff       [T,S+1,2] fp64 or NULL: camera-motion offset of frame first(t)+j in the window of frame t; segment
+ *              endpoints become int(int(track) - diff)
+ * Invalid arguments return CT3_EINVAL (a too small workspace CT3_ENOSPC) before any launch. */
+int ct3_render_tracks(uint8_t* frames, int T, int H, int W, const float* pts, const uint8_t* visible,
+                      const uint8_t* colors, const uint8_t* draw_mask, int N, int radius, int linewidth, int trail,
+                      int query_frame, const double* alphas, const double* diff, void* workspace,
+                      size_t workspace_bytes, ct3_stream_t stream);
+
 /* ---- per-clip preparation ---------------------------------------------------
  * ct3_prepare_pyramid: cotracker3_offline.py:92-117 (L2-normalise over channels,
  * 3x avg_pool2d(2,2)).  in: fnet output [T,128,H4,W4] fp32 channel-planar.
