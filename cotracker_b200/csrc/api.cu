@@ -219,6 +219,7 @@ struct Workspace {
   float* att_part;        // split-K partials of the virtual<-point attention
   __nv_bfloat16* pyr_split;  // split-bf16 copy of the pyramid (corr_tc2.cu); null when H4 == 0
   int32_t* groups;        // device group table of a grouped call (GroupPlan); null when G == 1
+  int32_t* frames;        // device frame map [G, T] of ct3_update_loop_frames; null without one
   size_t total;
 };
 // split-K slots of the virtual<-point partials: a group of n tracks splits at most min(32, ceil(n/64)/2) ways
@@ -231,8 +232,10 @@ int partial_slots(int N, int G) {
 // int32 entries of the group table: offsets [G+1] | all [G] | split [G] | slot [G] | small [G] | tiles [2 * max tiles]
 int64_t group_table_ints(int N, int G) { return G == 1 ? 0 : (int64_t)5 * G + 1 + 2 * ((int64_t)N / 128 + G); }
 
-Workspace carve(void* base, int T, int N, int H4 = 0, int W4 = 0, int G = 1) {
+// T_pyr: frames of the pyramid the correlation reads (sizes the split copy; 0 = T); frames: room for a [G, T] frame map
+Workspace carve(void* base, int T, int N, int H4 = 0, int W4 = 0, int G = 1, int T_pyr = 0, bool frames = false) {
   Workspace w;
+  if (T_pyr == 0) T_pyr = T;
   const size_t R = (size_t)(N + (size_t)kV * G) * T, Rp = (size_t)N * T, Rv = (size_t)kV * G * T, Mc = Rp * kL;
   uint8_t* p = reinterpret_cast<uint8_t*>(base);
   size_t off = 0;
@@ -251,9 +254,10 @@ Workspace carve(void* base, int T, int N, int H4 = 0, int W4 = 0, int G = 1) {
   w.row_bias = (float*)take((size_t)T * kC * 4);
   w.att_part = (float*)take(attention_partial_bytes(T, kV, partial_slots(N, G)));
   w.pyr_split = nullptr;
-  if (H4 > 0 && W4 > 0 && corr_patch_supported(T, H4, W4))
-    w.pyr_split = (__nv_bfloat16*)take((size_t)pyramid_layout(T, H4, W4).total * 4);
+  if (H4 > 0 && W4 > 0 && corr_patch_supported(T_pyr, H4, W4))
+    w.pyr_split = (__nv_bfloat16*)take((size_t)pyramid_layout(T_pyr, H4, W4).total * 4);
   w.groups = G > 1 ? (int32_t*)take((size_t)group_table_ints(N, G) * 4) : nullptr;
+  w.frames = frames ? (int32_t*)take((size_t)G * T * 4) : nullptr;
   w.total = off;
   return w;
 }
@@ -642,9 +646,22 @@ int check_groups(const int32_t* sizes, int G, int N, int* total) {
   return 0;
 }
 
+// frames: host frame map [G, T] into the T_pyr pyramid frames, or null (frame t, T_pyr == T)
 int update_loop(const void* packed, const float* pyr, int H4, int W4, const float* support, const uint8_t* track_valid,
                 float* coords, float* vis, float* conf, const float* time_emb, int T, int N, const int32_t* sizes,
-                int G, int iters, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+                int G, int iters, void* workspace, size_t workspace_bytes, cudaStream_t stream, int T_pyr,
+                const int32_t* frames);
+
+// frame-map arguments of ct3_update_loop_frames / ct3_workspace_bytes_frames (frames == nullptr: not checked here)
+int check_frames(const int32_t* frames, int G, int T, int T_pyr) {
+  if (T_pyr < 1) return fail(CT3_EINVAL, "T_pyr must be >= 1%s");
+  if ((int64_t)T_pyr * T >= (int64_t)1 << 31 || (int64_t)G * T >= (int64_t)1 << 31)
+    return fail(CT3_EINVAL, "problem too large%s");
+  if (!frames) return 0;
+  for (int64_t i = 0; i < (int64_t)G * T; ++i)
+    if (frames[i] < 0 || frames[i] >= T_pyr) return fail(CT3_EINVAL, "frame index outside [0, T_pyr)%s");
+  return 0;
+}
 int updateformer(const void* packed, const float* x, int T, int N, const int32_t* sizes, int G, float* delta,
                  void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
@@ -940,7 +957,8 @@ int ct3_corr_sample(const float* pyr, int H4, int W4, const float* support, cons
     pyr_split = (const __nv_bfloat16*)scratch;
   }
   CK(launch_corr_sample(pyr, pyr_split, H4, W4, support, track_valid, coords, T, N, (__nv_bfloat16*)vol_split,
-                        g_opt_corr, pr.corr, pr.vol16() ? 1 : 0, num_sms(), (cudaStream_t)stream), "corr_sample");
+                        g_opt_corr, pr.corr, pr.vol16() ? 1 : 0, num_sms(), (cudaStream_t)stream, T, FrameMap{}),
+     "corr_sample");
   return 0;
 }
 
@@ -992,7 +1010,7 @@ int ct3_update_loop(const void* packed, const float* pyr, int H4, int W4, const 
                     int T, int N, int iters, void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
   const int32_t one = N;
   return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, &one, 1, iters,
-                     workspace, workspace_bytes, (cudaStream_t)stream);
+                     workspace, workspace_bytes, (cudaStream_t)stream, T, nullptr);
 }
 
 int ct3_update_loop_groups(const void* packed, const float* pyr, int H4, int W4, const float* support,
@@ -1000,7 +1018,25 @@ int ct3_update_loop_groups(const void* packed, const float* pyr, int H4, int W4,
                            int T, int N, int iters, void* workspace, size_t workspace_bytes, ct3_stream_t stream,
                            const int32_t* group_sizes_host, int G) {
   return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, group_sizes_host, G,
-                     iters, workspace, workspace_bytes, (cudaStream_t)stream);
+                     iters, workspace, workspace_bytes, (cudaStream_t)stream, T, nullptr);
+}
+
+int ct3_workspace_bytes_frames(int T, int T_pyr, int N, int G, int H4, int W4, size_t* out_bytes) {
+  if (!out_bytes) return fail(CT3_EINVAL, "null out_bytes%s");
+  if (int rc = check_TN(T, N, G)) return rc;
+  if (int rc = check_frames(nullptr, G, T, T_pyr)) return rc;
+  if (int rc = ct3_pyramid_layout(T_pyr, H4, W4, nullptr, nullptr, nullptr, nullptr)) return rc;
+  *out_bytes = carve(nullptr, T, N, H4, W4, G, T_pyr, true).total;
+  return 0;
+}
+
+int ct3_update_loop_frames(const void* packed, const float* pyr, int T_pyr, int H4, int W4, const float* support,
+                           const uint8_t* track_valid, float* coords, float* vis, float* conf, const float* time_emb,
+                           int T, int N, int iters, void* workspace, size_t workspace_bytes, ct3_stream_t stream,
+                           const int32_t* group_sizes_host, int G, const int32_t* group_frames_host) {
+  if (!group_frames_host) return fail(CT3_EINVAL, "null group_frames_host%s");
+  return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, group_sizes_host, G,
+                     iters, workspace, workspace_bytes, (cudaStream_t)stream, T_pyr, group_frames_host);
 }
 
 int ct3_updateformer(const void* packed, const float* x, int T, int N, float* delta, void* workspace,
@@ -1020,7 +1056,8 @@ namespace {
 
 int update_loop(const void* packed, const float* pyr, int H4, int W4, const float* support, const uint8_t* track_valid,
                 float* coords, float* vis, float* conf, const float* time_emb, int T, int N, const int32_t* sizes,
-                int G, int iters, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+                int G, int iters, void* workspace, size_t workspace_bytes, cudaStream_t stream, int T_pyr,
+                const int32_t* frames) {
   if (!packed || !pyr || !support || !coords || !vis || !conf || !time_emb || !workspace)
     return fail(CT3_EINVAL, "null argument%s");
   if (int rc = check_TN(T, N)) return rc;
@@ -1028,20 +1065,28 @@ int update_loop(const void* packed, const float* pyr, int H4, int W4, const floa
   if (int rc = check_groups(sizes, G, N, &total)) return rc;
   if (int rc = check_TN(T, N, G)) return rc;
   if (iters < 0) return fail(CT3_EINVAL, "iters must be >= 0%s");
-  if (int rc = ct3_pyramid_layout(T, H4, W4, nullptr, nullptr, nullptr, nullptr)) return rc;
+  if (int rc = check_frames(frames, G, T, T_pyr)) return rc;
+  if (int rc = ct3_pyramid_layout(T_pyr, H4, W4, nullptr, nullptr, nullptr, nullptr)) return rc;
   if ((uintptr_t)workspace & 255) return fail(CT3_EINVAL, "workspace must be 256-byte aligned%s");
-  const Workspace W = carve(workspace, T, N, H4, W4, G);
+  const Workspace W = carve(workspace, T, N, H4, W4, G, T_pyr, frames != nullptr);
   if (workspace_bytes < W.total) return fail(CT3_ENOSPC, "workspace too small%s");
   const Layout& L = layout();
   Runner R{reinterpret_cast<const uint8_t*>(packed), L, stream, g_opt_gemm};
   const uint8_t* pk = R.pk;
   GroupPlan gp;
   if (int rc = plan_groups(gp, sizes, G, T, N, W.groups, R.s)) return rc;
+  FrameMap fm;
+  if (frames) {   // the frame map reaches the device like the group table: in stream order, through kernel arguments
+    CK(launch_upload_i32(W.frames, frames, G * T, R.s), "upload frame map");
+    fm.frames = W.frames;
+    fm.goff = G > 1 ? gp.off : nullptr;
+    fm.G = G;
+  }
   const int Rp = N * T, Mc = Rp * kL;
-  // split-bf16 copy of the window's pyramid: the TMA source of the correlation kernel, made once per call
-  const Prec pr = effective_prec(W.pyr_split != nullptr, T, H4, W4);
+  // split-bf16 copy of the pyramid: the TMA source of the correlation kernel, made once per call
+  const Prec pr = effective_prec(W.pyr_split != nullptr, T_pyr, H4, W4);
   const __nv_bfloat16* pyr_split = (pr.patch && iters > 0) ? W.pyr_split : nullptr;
-  if (pyr_split) RUNC(CAT_MISC, launch_split_pyramid(pyr, T, H4, W4, W.pyr_split, pr.corr, R.s));
+  if (pyr_split) RUNC(CAT_MISC, launch_split_pyramid(pyr, T_pyr, H4, W4, W.pyr_split, pr.corr, R.s));
 
   // W_in * time_emb[t]: x + time_emb is folded into a per-frame bias of input_transform (cotracker3_offline.py:196)
   RUNC(CAT_MISC, launch_row_bias(time_emb, reinterpret_cast<const float*>(pk + L.win_f32), T, W.row_bias, R.s));
@@ -1049,7 +1094,7 @@ int update_loop(const void* packed, const float* pyr, int H4, int W4, const floa
   for (int it = 0; it < iters; ++it) {
     // (i)+(ii) sampling + 4-D correlation, all levels -> split volume
     RUNC(CAT_CORR, launch_corr_sample(pyr, pyr_split, H4, W4, support, track_valid, coords, T, N, W.vol, g_opt_corr,
-                                      pr.corr, pr.vol16() ? 1 : 0, num_sms(), R.s));
+                                      pr.corr, pr.vol16() ? 1 : 0, num_sms(), R.s, T_pyr, fm));
     // (iii) corr_mlp: 2401 -> 384 (GELU erf) -> 256, written straight into X columns [256*l, 256*l+256)
     if (pr.vol16()) {   // single fp16 volume plane x split fp16 weights: 2 (or 1) tensor-core products per FLOP
       RUNC(-1, R.gemm(W.vol, pr.support_major() ? L.corr_fc1_th : L.corr_fc1_h, Mc,

@@ -22,6 +22,7 @@ struct CorrArgs {
   const float* coords;         // [T, N, 2]
   int T, N;
   __nv_bfloat16* vol;          // [N*T*4, 2*kVolPad]
+  FrameMap fm;                 // pyramid frame of (track, t)
 };
 
 // v1: SIMT fp32.  block = (track n, level l), loops over frames.  256 threads.
@@ -48,11 +49,12 @@ corr_sample_simt_kernel(CorrArgs g) {
 
   const float inv = 1.0f / (float)(1 << l);
   const int ti = tid / 13, tj = tid % 13;  // output tile (rows ti*4.., cols tj*4..) for tid < 169
+  const int32_t* frow = frame_row(g.fm, n, g.T);
 
   for (int t = 0; t < g.T; ++t) {
     const float cx = g.coords[((int64_t)t * g.N + n) * 2 + 0] * inv;
     const float cy = g.coords[((int64_t)t * g.N + n) * 2 + 1] * inv;
-    const float* fm = g.pyr + g.lay.off[l] + (int64_t)t * H * W * kD;
+    const float* fm = g.pyr + g.lay.off[l] + (int64_t)map_frame(frow, t) * H * W * kD;
     for (int p = warp; p < kP; p += 8) {
       const int a = p / 7, b = p % 7;
       const float x = fminf(fmaxf(cx + (float)(a - kR), 0.f), (float)(W - 1));
@@ -127,23 +129,28 @@ bool corr_uses_patch_kernel(int impl, bool have_pyr_split, int T, int H4, int W4
 
 cudaError_t launch_corr_sample(const float* pyr, const __nv_bfloat16* pyr_split, int H4, int W4, const float* support,
                                const uint8_t* track_valid, const float* coords, int T, int N,
-                               __nv_bfloat16* vol_split, int impl, int mode, int vol16, int num_sms, cudaStream_t s) {
-  if (corr_uses_patch_kernel(impl, pyr_split != nullptr, T, H4, W4)) {
+                               __nv_bfloat16* vol_split, int impl, int mode, int vol16, int num_sms, cudaStream_t s,
+                               int T_pyr, const FrameMap& fm) {
+  if (corr_uses_patch_kernel(impl, pyr_split != nullptr, T_pyr, H4, W4)) {
     if (impl == 0 && mode != 3)
-      return launch_corr_patch_t(pyr_split, H4, W4, support, track_valid, coords, T, N, vol_split, vol16, mode == 1, num_sms, s);
-    return launch_corr_patch_tc(pyr_split, H4, W4, support, track_valid, coords, T, N, vol_split, mode, vol16, num_sms, s);
+      return launch_corr_patch_t(pyr_split, H4, W4, support, track_valid, coords, T, N, vol_split, vol16, mode == 1,
+                                 num_sms, s, T_pyr, fm);
+    return launch_corr_patch_tc(pyr_split, H4, W4, support, track_valid, coords, T, N, vol_split, mode, vol16, num_sms,
+                                s, T_pyr, fm);
   }
   if (vol16) return cudaErrorInvalidValue;   // only the patch kernel writes the single-plane volume
-  if (impl != 1) return launch_corr_sample_tc(pyr, H4, W4, support, track_valid, coords, T, N, vol_split, num_sms, s);
+  if (impl != 1)
+    return launch_corr_sample_tc(pyr, H4, W4, support, track_valid, coords, T, N, vol_split, num_sms, s, T_pyr, fm);
   CorrArgs g;  // impl 1: exact-fp32 SIMT verification kernel
   g.pyr = pyr;
-  g.lay = pyramid_layout(T, H4, W4);
+  g.lay = pyramid_layout(T_pyr, H4, W4);
   g.support = support;
   g.track_valid = track_valid;
   g.coords = coords;
   g.T = T;
   g.N = N;
   g.vol = vol_split;
+  g.fm = fm;
   const int smem = 2 * 52 * kLd * (int)sizeof(float);  // 54.9 KB
   static DeviceOnce attr;
   {

@@ -56,9 +56,10 @@ struct CorrTcArgs {
   const float* coords;         // [T, N, 2]
   int T, N;
   __nv_bfloat16* vol;          // [N*T*4, 2*kVolPad]
+  FrameMap fm;                 // pyramid frame of (track, t): the unit's patches all come from its own frame row
 };
 struct CorrMaps {
-  CUtensorMap m[kL];           // per level: dims (128, W, H, T), box (128, min(W,8), min(H,8), 1), fp32, no swizzle
+  CUtensorMap m[kL];           // per level: dims (128, W, H, T_pyr), box (128, min(W,8), min(H,8), 1), fp32, no swizzle
 };
 
 // byte offset of (row r, 16-byte chunk c) inside one [rows x 128 B] swizzle-128B K-atom
@@ -133,6 +134,7 @@ corr_sample_tc_kernel(const __grid_constant__ CorrTcArgs g, const __grid_constan
       const int n = u / kL, l = u % kL;
       const int H = g.lay.h[l], W = g.lay.w[l];
       const int bw = min(W, 8), bh = min(H, 8);        // box extent (maps narrower than 8 texels: whole map)
+      const int32_t* frow = frame_row(g.fm, n, g.T);
       // ---- support tile (B operand), once per unit
       if (ui > 0) mbar_wait(s_empty, (ui - 1) & 1u);   // MMAs of the previous unit have retired
       {
@@ -199,7 +201,7 @@ corr_sample_tc_kernel(const __grid_constant__ CorrTcArgs g, const __grid_constan
               outv[b] = lerp4(h0, hrow[b + 1], wy[b]);
             }
           } else {
-            const float* fm = g.pyr + g.lay.off[l] + (int64_t)t * H * W * kD + lane * 4;
+            const float* fm = g.pyr + g.lay.off[l] + (int64_t)map_frame(frow, t) * H * W * kD + lane * 4;
 #pragma unroll
             for (int b = 0; b < 7; ++b) {
               const int y1 = yl[b + 1];
@@ -238,6 +240,7 @@ corr_sample_tc_kernel(const __grid_constant__ CorrTcArgs g, const __grid_constan
       const int n = u / kL, l = u % kL;
       const int H = g.lay.h[l], W = g.lay.w[l];
       const float inv = 1.0f / (float)(1 << l);
+      const int32_t* frow = frame_row(g.fm, n, g.T);
       for (int t0 = 0; t0 < g.T; t0 += 32) {
         // coordinates of up to 32 frames in one round trip (lane = frame), then broadcast per frame
         const int tl = min(t0 + lane, g.T - 1);
@@ -253,7 +256,8 @@ corr_sample_tc_kernel(const __grid_constant__ CorrTcArgs g, const __grid_constan
             *reinterpret_cast<float4*>(smem + OFF_PARAM + slot * 16) =
                 make_float4(cx, cy, __int_as_float(bx), __int_as_float(by));
             mbar_arrive_expect_tx(&p_full[slot], (uint32_t)(min(W, 8) * min(H, 8) * kD * 4));
-            tma_load_4d(smem + OFF_PATCH + slot * PATCH_BYTES, &maps.m[l], 0, bx, by, t0 + k, &p_full[slot]);
+            tma_load_4d(smem + OFF_PATCH + slot * PATCH_BYTES, &maps.m[l], 0, bx, by, map_frame(frow, t0 + k),
+                        &p_full[slot]);
           }
         }
         __syncwarp();
@@ -380,20 +384,22 @@ corr_sample_tc_kernel(const __grid_constant__ CorrTcArgs g, const __grid_constan
 
 cudaError_t launch_corr_sample_tc(const float* pyr, int H4, int W4, const float* support,
                                   const uint8_t* track_valid, const float* coords, int T, int N,
-                                  __nv_bfloat16* vol_split, int num_sms, cudaStream_t s) {
+                                  __nv_bfloat16* vol_split, int num_sms, cudaStream_t s, int T_pyr,
+                                  const FrameMap& fm) {
   CorrTcArgs g;
   g.pyr = pyr;
-  g.lay = pyramid_layout(T, H4, W4);
+  g.lay = pyramid_layout(T_pyr, H4, W4);
   g.support = support;
   g.track_valid = track_valid;
   g.coords = coords;
   g.T = T;
   g.N = N;
   g.vol = vol_split;
+  g.fm = fm;
   CorrMaps maps;
   for (int l = 0; l < kL; ++l) {
     const uint64_t W = (uint64_t)g.lay.w[l], H = (uint64_t)g.lay.h[l];
-    const uint64_t dims[4] = {(uint64_t)kD, W, H, (uint64_t)T};
+    const uint64_t dims[4] = {(uint64_t)kD, W, H, (uint64_t)T_pyr};
     const uint64_t strides[3] = {(uint64_t)kD * 4, W * kD * 4, H * W * kD * 4};
     const uint32_t box[4] = {(uint32_t)kD, (uint32_t)(W < 8 ? W : 8), (uint32_t)(H < 8 ? H : 8), 1};
     if (!encode_tensor_map(&maps.m[l], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, pyr + g.lay.off[l], dims, strides, box,

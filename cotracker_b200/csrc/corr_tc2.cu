@@ -93,8 +93,10 @@ struct Corr2Args {
   const uint8_t* track_valid;  // [N] or null
   const float* coords;         // [T, N, 2]
   int T, N;
+  int T_pyr;                   // frames of the pyramid copy (plane stride of the TMA map's dim 3)
   uint16_t* vol;               // [N*T*4, 2*kVolPad] split bf16, or [N*T*4, kVolPad] fp16 (V16)
   long long* trace;            // CT3_TRACE builds: [256 tiles][8 events] clock64 of CTA 0
+  FrameMap fm;                 // pyramid frame of (track, t): each box is one frame of the unit's own frame row
 };
 #ifdef CT3_TRACE
 #define TRACE(tile, ev) do { if (blockIdx.x == 0 && (tile) < 256) g.trace[(tile) * 8 + (ev)] = clock64(); } while (0)
@@ -102,7 +104,7 @@ struct Corr2Args {
 #define TRACE(tile, ev) do { } while (0)
 #endif
 struct Corr2Maps {
-  CUtensorMap m[kL];           // per level: 16-bit dims (128, W, H, planes*T), box (64, 8, 8, 1), 128B swizzle
+  CUtensorMap m[kL];           // per level: 16-bit dims (128, W, H, planes*T_pyr), box (64, 8, 8, 1), 128B swizzle
 };
 
 __device__ __forceinline__ uint32_t sw128(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
@@ -163,6 +165,7 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
       const int n = u / kL, l = u % kL;
       const int H = g.lay.h[l], W = g.lay.w[l];
       const float inv = 1.0f / (float)(1 << l);
+      const int32_t* frow = frame_row(g.fm, n, g.T);
       for (int t0 = 0; t0 < g.T; t0 += 32) {
         // coordinates of up to 32 frames in one round trip (lane = frame), then broadcast per tile
         const int tl = min(t0 + lane, g.T - 1);
@@ -197,8 +200,8 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
                   const int bx = f ? bx1 : bx0, by = f ? by1 : by0;
 #pragma unroll
                   for (int pl = 0; pl < (MODE == 3 ? 2 : 1); ++pl)
-                    tma_load_4d(dst + pl * A_PLANE + f * 8192, &maps.m[l], kh * 64, bx, by, pl * g.T + t0 + k + f,
-                                &a_full[sl]);
+                    tma_load_4d(dst + pl * A_PLANE + f * 8192, &maps.m[l], kh * 64, bx, by,
+                                pl * g.T_pyr + map_frame(frow, t0 + k + f), &a_full[sl]);
                 }
               }
             }
@@ -536,17 +539,20 @@ cudaError_t launch_split_pyramid(const float* pyr, int T, int H4, int W4, __nv_b
 
 cudaError_t launch_corr_patch_tc(const __nv_bfloat16* pyr_split, int H4, int W4, const float* support,
                                  const uint8_t* track_valid, const float* coords, int T, int N,
-                                 __nv_bfloat16* vol_split, int mode, int vol16, int num_sms, cudaStream_t s) {
+                                 __nv_bfloat16* vol_split, int mode, int vol16, int num_sms, cudaStream_t s, int T_pyr,
+                                 const FrameMap& fm) {
   if (mode < 1 || mode > 3) return cudaErrorInvalidValue;
   Corr2Args g;
-  g.lay = pyramid_layout(T, H4, W4);
+  g.lay = pyramid_layout(T_pyr, H4, W4);
   g.support = support;
   g.track_valid = track_valid;
   g.coords = coords;
   g.T = T;
   g.N = N;
+  g.T_pyr = T_pyr;
   g.vol = reinterpret_cast<uint16_t*>(vol_split);
   g.trace = nullptr;
+  g.fm = fm;
 #ifdef CT3_TRACE
   static long long* trace_buf = nullptr;
   if (!trace_buf) cudaMalloc(&trace_buf, 256 * 8 * sizeof(long long));
@@ -556,7 +562,7 @@ cudaError_t launch_corr_patch_tc(const __nv_bfloat16* pyr_split, int H4, int W4,
   for (int l = 0; l < kL; ++l) {
     const uint64_t W = (uint64_t)g.lay.w[l], H = (uint64_t)g.lay.h[l];
     if (W < 8 || H < 8) return cudaErrorInvalidValue;
-    const uint64_t dims[4] = {(uint64_t)kD, W, H, (uint64_t)((mode == 3 ? 2 : 1) * T)};   // dim 3 = plane*T + t
+    const uint64_t dims[4] = {(uint64_t)kD, W, H, (uint64_t)((mode == 3 ? 2 : 1) * T_pyr)};   // dim 3 = plane*T_pyr + frame
     const uint64_t strides[3] = {(uint64_t)kD * 2, W * kD * 2, H * W * kD * 2};
     const uint32_t box[4] = {64, 8, 8, 1};
     if (!encode_tensor_map(&maps.m[l], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, pyr_split + 2 * g.lay.off[l], dims, strides,

@@ -82,9 +82,10 @@ struct Corr3Args {
   int T, N;
   uint16_t* vol;               // [N*T*4, 2*kVolPad] split bf16, or [N*T*4, kVolPad] fp16 (V16)
   int* unit_counter;           // zeroed before the launch: units beyond the first one per CTA are handed out dynamically
+  FrameMap fm;                 // pyramid frame of (track, t): each box is one frame of the unit's own frame row
 };
 struct Corr3Maps {
-  CUtensorMap m[kL];           // per level: fp16 dims (128, W, H, T), box (64, 8, 8, 1), 128B swizzle
+  CUtensorMap m[kL];           // per level: fp16 dims (128, W, H, T_pyr), box (64, 8, 8, 1), 128B swizzle
 };
 
 __device__ __forceinline__ uint32_t sw128(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
@@ -316,6 +317,7 @@ corr_patch_t_kernel(const __grid_constant__ Corr3Args g, const __grid_constant__
       const int n = u / kL, l = u % kL;
       const int H = g.lay.h[l], W = g.lay.w[l];
       const float inv = 1.0f / (float)(1 << l);
+      const int32_t* frow = frame_row(g.fm, n, g.T);
       for (int t0 = 0; t0 < g.T; t0 += 32) {
         const int tl = min(t0 + lane, g.T - 1);
         const float2 c = __ldg(reinterpret_cast<const float2*>(g.coords + ((int64_t)tl * g.N + n) * 2));
@@ -363,8 +365,9 @@ corr_patch_t_kernel(const __grid_constant__ Corr3Args g, const __grid_constant__
               if (kh == 1) mbar_wait_spin(&a_empty[sl], ((h / NSLOT) & 1u) ^ 1u);
               mbar_arrive_expect_tx(&a_full[sl], (uint32_t)(nf * (A_SLOT / 2)));
               uint8_t* dst = smem + OFF_A + sl * A_SLOT;
-              tma_load_4d_hint(dst, &maps.m[l], kh * 64, bx0, by0, t0 + k, &a_full[sl], keep);
-              if (nf == 2) tma_load_4d_hint(dst + 8192, &maps.m[l], kh * 64, bx1, by1, t0 + k + 1, &a_full[sl], keep);
+              tma_load_4d_hint(dst, &maps.m[l], kh * 64, bx0, by0, map_frame(frow, t0 + k), &a_full[sl], keep);
+              if (nf == 2)
+                tma_load_4d_hint(dst + 8192, &maps.m[l], kh * 64, bx1, by1, map_frame(frow, t0 + k + 1), &a_full[sl], keep);
             }
           }
           hc += 2;        // every lane tracks the slot counter (the table gate above is a warp-wide wait)
@@ -497,18 +500,20 @@ cudaError_t launch_variant(const Corr3Args& g, const Corr3Maps& maps, int num_un
 
 cudaError_t launch_corr_patch_t(const __nv_bfloat16* pyr_half, int H4, int W4, const float* support,
                                 const uint8_t* track_valid, const float* coords, int T, int N,
-                                __nv_bfloat16* vol, int vol16, int one_product, int num_sms, cudaStream_t s) {
+                                __nv_bfloat16* vol, int vol16, int one_product, int num_sms, cudaStream_t s, int T_pyr,
+                                const FrameMap& fm) {
   Corr3Args g;
-  g.lay = pyramid_layout(T, H4, W4);
+  g.lay = pyramid_layout(T_pyr, H4, W4);
   g.support = support;
   g.track_valid = track_valid;
   g.coords = coords;
   g.T = T;
   g.N = N;
   g.vol = reinterpret_cast<uint16_t*>(vol);
+  g.fm = fm;
   // every level of the pyramid workspace has room for two 16-bit planes (launch_split_pyramid); this kernel's single
   // fp16 plane uses the first half, so the unit counter can live right behind level 0's plane
-  const size_t plane0 = (size_t)T * g.lay.h[0] * g.lay.w[0] * kD * 2;
+  const size_t plane0 = (size_t)T_pyr * g.lay.h[0] * g.lay.w[0] * kD * 2;
   g.unit_counter = reinterpret_cast<int*>(reinterpret_cast<uintptr_t>(pyr_half) + ((plane0 + 15) & ~(size_t)15));
   cudaError_t e0 = cudaMemsetAsync(g.unit_counter, 0, sizeof(int), s);
   if (e0 != cudaSuccess) return e0;
@@ -516,7 +521,7 @@ cudaError_t launch_corr_patch_t(const __nv_bfloat16* pyr_half, int H4, int W4, c
   for (int l = 0; l < kL; ++l) {
     const uint64_t W = (uint64_t)g.lay.w[l], H = (uint64_t)g.lay.h[l];
     if (W < 8 || H < 8) return cudaErrorInvalidValue;
-    const uint64_t dims[4] = {(uint64_t)kD, W, H, (uint64_t)T};
+    const uint64_t dims[4] = {(uint64_t)kD, W, H, (uint64_t)T_pyr};
     const uint64_t strides[3] = {(uint64_t)kD * 2, W * kD * 2, H * W * kD * 2};
     const uint32_t box[4] = {64, 8, 8, 1};
     if (!encode_tensor_map(&maps.m[l], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, pyr_half + 2 * g.lay.off[l], dims, strides,

@@ -70,7 +70,32 @@ cudaError_t launch_upsample_concat_split(const float* const src[4], const int c[
                                          const int w[4], int T, int Cp, int H, int W, __nv_bfloat16* out, cudaStream_t s);
 
 // ---- corr.cu : correlation sampling ---------------------------------------------------------------
-// vol_split [N*T*4, 2*kVolPad] bf16, row (n*T+t)*4+level
+// Frame map of ct3_update_loop_frames: at time step t, track n of group g reads pyramid frame frames[g*T + t] (an index
+// into the T_pyr frames of the pyramid).  frames == nullptr: frame t.  goff: [G+1] first track of every group (nullptr
+// when G == 1).  Every correlation kernel works on units of ONE track, so the lookup is per (track, t): no tile or TMA
+// box ever spans two tracks' frames.
+struct FrameMap {
+  const int32_t* frames = nullptr;
+  const int32_t* goff = nullptr;
+  int G = 1;
+};
+// the T-entry frame row of track n (nullptr: identity)
+__device__ __forceinline__ const int32_t* frame_row(const FrameMap& m, int n, int T) {
+  if (!m.frames) return nullptr;
+  int g = 0;
+  if (m.goff) {   // largest g with goff[g] <= n
+    int hi = m.G - 1;
+    while (g < hi) {
+      const int mid = (g + hi + 1) >> 1;
+      if (__ldg(m.goff + mid) <= n) g = mid; else hi = mid - 1;
+    }
+  }
+  return m.frames + (int64_t)g * T;
+}
+__device__ __forceinline__ int map_frame(const int32_t* row, int t) { return row ? __ldg(row + t) : t; }
+
+// vol_split [N*T*4, 2*kVolPad] bf16, row (n*T+t)*4+level; pyr holds T_pyr frames (T_pyr = T and fm = {} unless a frame
+// map is given)
 // impl: 0 tensor cores (correlate-then-interpolate when pyr_split is given and every level is >= 8x8: corr_tc3.cu for
 //         mode 2, corr_tc2.cu for modes 3 / 1; else corr_tc.cu),
 //       1 exact-fp32 SIMT, 2 corr_tc.cu always, 3 like 0 but corr_tc2.cu for every mode (A/B of the two kernels)
@@ -80,11 +105,12 @@ cudaError_t launch_upsample_concat_split(const float* const src[4], const int c[
 bool corr_uses_patch_kernel(int impl, bool have_pyr_split, int T, int H4, int W4);
 cudaError_t launch_corr_sample(const float* pyr, const __nv_bfloat16* pyr_split, int H4, int W4, const float* support,
                                const uint8_t* track_valid, const float* coords, int T, int N,
-                               __nv_bfloat16* vol_split, int impl, int mode, int vol16, int num_sms, cudaStream_t s);
+                               __nv_bfloat16* vol_split, int impl, int mode, int vol16, int num_sms, cudaStream_t s,
+                               int T_pyr, const FrameMap& fm);
 
 cudaError_t launch_corr_sample_tc(const float* pyr, int H4, int W4, const float* support,
                                   const uint8_t* track_valid, const float* coords, int T, int N,
-                                  __nv_bfloat16* vol_split, int num_sms, cudaStream_t s);
+                                  __nv_bfloat16* vol_split, int num_sms, cudaStream_t s, int T_pyr, const FrameMap& fm);
 
 // corr_tc2.cu: correlate-then-interpolate on a split-bf16 copy of the pyramid
 //   pyr_split: per level at bf16 offset 2*off[l]: [plane hi|lo][T][H][W][128]   (same bytes as the fp32 pyramid)
@@ -94,13 +120,15 @@ cudaError_t launch_split_pyramid(const float* pyr, int T, int H4, int W4, __nv_b
                                  cudaStream_t s);
 cudaError_t launch_corr_patch_tc(const __nv_bfloat16* pyr_split, int H4, int W4, const float* support,
                                  const uint8_t* track_valid, const float* coords, int T, int N,
-                                 __nv_bfloat16* vol_split, int mode, int vol16, int num_sms, cudaStream_t s);
+                                 __nv_bfloat16* vol_split, int mode, int vol16, int num_sms, cudaStream_t s, int T_pyr,
+                                 const FrameMap& fm);
 
 // corr_tc3.cu: the production kernel -- same algorithm with the MMA transposed (supports = M side), one fp16 texel
 // plane (pyr_split made with mode 1 or 2), supports split fp16 (mode 2) or one fp16 plane (one_product, mode 1)
 cudaError_t launch_corr_patch_t(const __nv_bfloat16* pyr_half, int H4, int W4, const float* support,
                                 const uint8_t* track_valid, const float* coords, int T, int N,
-                                __nv_bfloat16* vol, int vol16, int one_product, int num_sms, cudaStream_t s);
+                                __nv_bfloat16* vol, int vol16, int one_product, int num_sms, cudaStream_t s, int T_pyr,
+                                const FrameMap& fm);
 
 // ---- tokens.cu : elementwise / row-wise pieces of the transformer ---------------------------------
 cudaError_t launch_layernorm_split(const float* x, int rows, const float* gamma, const float* beta, float eps,

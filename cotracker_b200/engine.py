@@ -66,6 +66,10 @@ def _declare(lib):
                                            ctypes.POINTER(ctypes.c_int32), c_int]),
         "ct3_updateformer_groups": (c_int, [c_void_p, c_void_p, c_int, ctypes.POINTER(ctypes.c_int32), c_int, c_void_p,
                                             c_void_p, c_size_t, c_void_p]),
+        "ct3_workspace_bytes_frames": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+        "ct3_update_loop_frames": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p,
+                                           ctypes.POINTER(ctypes.c_int32), c_int, ctypes.POINTER(ctypes.c_int32)]),
         "ct3_upsample_concat": (c_int, [ctypes.POINTER(c_void_p), intp, intp, intp, c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_enc_tail_packed_bytes": (c_int, [ctypes.POINTER(c_size_t)]),
         "ct3_enc_tail_pack": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
@@ -96,6 +100,7 @@ EXPORTED_SYMBOLS = [
     "ct3_encoder_workspace_bytes", "ct3_encoder",
     "ct3_upsample_concat", "ct3_enc_tail_packed_bytes", "ct3_enc_tail_pack", "ct3_enc_tail_workspace_bytes", "ct3_enc_tail",
     "ct3_workspace_bytes_groups", "ct3_update_loop_groups", "ct3_updateformer_groups",
+    "ct3_workspace_bytes_frames", "ct3_update_loop_frames",
     "ct3_prepare_frames",
     "ct3_render_prepare", "ct3_render_workspace_bytes", "ct3_render_tracks",
 ]
@@ -327,13 +332,26 @@ def sample_support(pyr, T, H4, W4, qframes, qcoords, support=None, accumulate_ma
     return support
 
 
-def workspace_bytes(T: int, N: int, H4: int = 0, W4: int = 0, groups: int = 1) -> int:
+def workspace_bytes(T: int, N: int, H4: int = 0, W4: int = 0, groups: int = 1, frames: Optional[int] = None) -> int:
     """Scratch of ct3_update_loop for T frames of H4 x W4 feature maps and N tracks (H4 = W4 = 0: updateformer only),
-    split into `groups` track groups (ct3_update_loop_groups)."""
+    split into `groups` track groups (ct3_update_loop_groups).  frames: the T_pyr pyramid frames of a call with a
+    frame map (ct3_update_loop_frames)."""
     n = ctypes.c_size_t(0)
+    if frames is not None:
+        _check(lib().ct3_workspace_bytes_frames(int(T), int(frames), int(N), int(groups), int(H4), int(W4),
+                                                ctypes.byref(n)), "ct3_workspace_bytes_frames")
+        return n.value
     _check(lib().ct3_workspace_bytes_groups(int(T), int(N), int(groups), int(H4), int(W4), ctypes.byref(n)),
            "ct3_workspace_bytes_groups")
     return n.value
+
+
+def pyramid_frames(pyr: torch.Tensor, H4: int, W4: int) -> int:
+    """Number of frames of a flat pyramid (its size is linear in the frame count)."""
+    per = pyramid_layout(1, H4, W4)[3]
+    if pyr.numel() % per or pyr.numel() == 0:
+        raise EngineError(f"a pyramid of {pyr.numel()} floats is not a whole number of {H4}x{W4} frames")
+    return pyr.numel() // per
 
 
 def _group_array(group_sizes):
@@ -353,19 +371,36 @@ class WorkspaceCache:
     def __init__(self):
         self.buf: Optional[torch.Tensor] = None
 
-    def get(self, T: int, N: int, device, H4: int = 0, W4: int = 0, groups: int = 1) -> torch.Tensor:
-        need = workspace_bytes(T, N, H4, W4, groups)
+    def get(self, T: int, N: int, device, H4: int = 0, W4: int = 0, groups: int = 1,
+            frames: Optional[int] = None) -> torch.Tensor:
+        need = workspace_bytes(T, N, H4, W4, groups, frames)
         if self.buf is None or self.buf.numel() < need or self.buf.device != torch.device(device):
             self.buf = None
             self.buf = torch.empty(need, dtype=torch.uint8, device=device)
         return self.buf
 
 
+def _frame_array(group_frames, G: int, T: int):
+    """Host int32 array [G*T] of a frame map given as a [G, T] nested sequence, array or tensor."""
+    try:
+        fr = torch.as_tensor(group_frames, dtype=torch.int64, device="cpu")
+    except (TypeError, ValueError, RuntimeError) as e:
+        raise EngineError(f"group_frames must be a [G, T] table of integers: {e}") from e
+    if tuple(fr.shape) != (G, T):
+        raise EngineError(f"group_frames must be [{G}, {T}], got {tuple(fr.shape)}")
+    if fr.numel() and (int(fr.min()) < -2 ** 31 or int(fr.max()) >= 2 ** 31):
+        raise EngineError("frame indices must fit in int32")
+    return (ctypes.c_int32 * max(1, fr.numel()))(*fr.reshape(-1).tolist())
+
+
 def update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, iters, workspace,
-                group_sizes: Optional[Sequence[int]] = None):
+                group_sizes: Optional[Sequence[int]] = None, group_frames=None):
     """In-place refinement of coords [T,N,2], vis [T,N], conf [T,N] (fp32, feature-grid units / logits).
     group_sizes: the N tracks as contiguous independent groups (ct3_update_loop_groups); each group's result is
-    bit-identical to a call on its tracks alone.  None = one group."""
+    bit-identical to a call on its tracks alone.  None = one group.
+    group_frames: [G, T] frame map (ct3_update_loop_frames): group g reads frame group_frames[g][t] of `pyr` (which may
+    hold any number of frames) at time step t; each group's result is bit-identical to a call on a pyramid of exactly
+    those frames.  None = frame t."""
     _req(coords, torch.float32, "coords"); _req(vis, torch.float32, "vis"); _req(conf, torch.float32, "conf")
     _req(pyr, torch.float32, "pyr"); _req(support, torch.float32, "support"); _req(time_emb, torch.float32, "time_emb")
     T, N, _ = coords.shape
@@ -373,6 +408,15 @@ def update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, ti
         raise EngineError(f"time_emb must be [{T},{XDIM}]")
     if track_valid is not None:
         _req(track_valid, torch.uint8, "track_valid")
+    if group_frames is not None:
+        arr, G = _group_array(group_sizes if group_sizes is not None else [N])
+        frames = _frame_array(group_frames, G, T)
+        with torch.cuda.device(coords.device):
+            _check(lib().ct3_update_loop_frames(_ptr(packed), _ptr(pyr), pyramid_frames(pyr, H4, W4), H4, W4,
+                                                _ptr(support), _ptr(track_valid), _ptr(coords), _ptr(vis), _ptr(conf),
+                                                _ptr(time_emb), T, N, int(iters), _ptr(workspace), workspace.numel(),
+                                                _stream(coords.device), arr, G, frames), "ct3_update_loop_frames")
+        return
     if group_sizes is not None:
         arr, G = _group_array(group_sizes)
         with torch.cuda.device(coords.device):

@@ -78,11 +78,37 @@ def points_on_a_grid(size: int, extent, center=None, device="cpu") -> torch.Tens
     return torch.stack([gx, gy], dim=-1).reshape(1, -1, 2)
 
 
-def pass_bytes(T: int, N: int, G: int, H4: int, W4: int) -> int:
+def pass_bytes(T: int, N: int, G: int, H4: int, W4: int, frames: Optional[int] = None) -> int:
     """Device memory of one grouped update-loop pass over N tracks in G groups and T frames: the library workspace
-    plus the per-track support features [4,49,N,128] and the per-frame state and outputs (about 16 floats)."""
+    plus the per-track support features [4,49,N,128] and the per-frame state and outputs (about 16 floats).
+    frames: the pyramid frames of a pass with a frame map (engine.workspace_bytes)."""
     from . import engine
-    return engine.workspace_bytes(T, N, H4, W4, groups=G) + N * (4 * 49 * 128 * 4 + T * 16 * 4)
+    return engine.workspace_bytes(T, N, H4, W4, groups=G, frames=frames) + N * (4 * 49 * 128 * 4 + T * 16 * 4)
+
+
+def pass_budget_bytes(model, device, T: int, ih: int, iw: int) -> int:
+    """Device memory one grouped pass of `model` on a T-frame clip at ih x iw may use: what is free plus the model's
+    cached update-loop workspace (it is regrown per pass), less the encoder's workspace and two copies of the pyramid."""
+    from . import engine
+    free, _ = torch.cuda.mem_get_info(device)
+    free += torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)
+    ws = model._ws.buf
+    if ws is not None and ws.device == torch.device(device):
+        free += ws.numel()
+    s = model.stride
+    pyr = engine.pyramid_layout(T, ih // s, iw // s)[3] * 4
+    reserve = engine.encoder_workspace_bytes(T, ih, iw) + 2 * pyr + (1 << 30)
+    return int(0.9 * max(0, free - reserve))
+
+
+def plan_dense_passes(n_offsets: int, n_tracks: int, backward: bool, T: int, H4: int, W4: int, budget_bytes: int,
+                      frames: Optional[int] = None) -> Tuple[List[int], List[Tuple[int, int]]]:
+    """Groups and passes of the predictor's dense mode: one group of n_tracks per grid offset, followed by that
+    offset's reversed group with backward tracking, split by `plan_passes` (T: frames of one update loop; frames: the
+    pyramid frames a pass with reversed groups reads, None when it has none).  -> (group sizes, passes)."""
+    sizes = [n_tracks] * (n_offsets * (2 if backward else 1))
+    return sizes, plan_passes(sizes, T, H4, W4, budget_bytes,
+                              lambda T_, N, G, H4_, W4_: pass_bytes(T_, N, G, H4_, W4_, frames))
 
 
 def plan_passes(group_sizes: Sequence[int], T: int, H4: int, W4: int, budget_bytes: int,
@@ -146,20 +172,6 @@ class EvaluationPredictor(torch.nn.Module):
             extra.append(torch.cat([tt, xy], dim=1)[None])
         return torch.cat(extra, dim=1) if extra else video.new_zeros(1, 0, 3)
 
-    def _free_bytes(self, video, T, ih, iw) -> int:
-        """Pass budget from free device memory: what is free plus the model's cached update-loop workspace (it is
-        regrown per pass), less the encoder's workspace and two copies of the pyramid."""
-        from . import engine
-        free, _ = torch.cuda.mem_get_info(video.device)
-        free += torch.cuda.memory_reserved(video.device) - torch.cuda.memory_allocated(video.device)
-        ws = self.model._ws.buf
-        if ws is not None and ws.device == video.device:
-            free += ws.numel()
-        s = self.model.stride
-        pyr = engine.pyramid_layout(T, ih // s, iw // s)[3] * 4
-        reserve = engine.encoder_workspace_bytes(T, ih, iw) + 2 * pyr + (1 << 30)
-        return int(0.9 * max(0, free - reserve))
-
     @torch.no_grad()
     def forward(self, video, queries):
         from . import ingest
@@ -187,7 +199,7 @@ class EvaluationPredictor(torch.nn.Module):
             T_loop = T if not hasattr(self.model, "init_video_online_processing") else self.model.window_len
             budget = self.pass_budget_bytes
             if budget is None:
-                budget = self._free_bytes(video, T, ih, iw)
+                budget = pass_budget_bytes(self.model, video.device, T, ih, iw)
             pyr = self.model._encode_clip(frames)          # every pass runs on the same pyramid
             del frames, video
             for g0, g1 in plan_passes(sizes, T_loop, ih // stride, iw // stride, budget):

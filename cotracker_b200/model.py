@@ -88,6 +88,50 @@ def sincos_time_embedding(dim: int, length: int) -> torch.Tensor:
 
 
 # ------------------------------------------------------------------------------------------------------
+# frame maps (ct3_update_loop_frames): which pyramid frame each group reads at each time step
+def clip_frame_map(T: int, reversed_groups) -> List[List[int]]:
+    """Offline model: a forward group reads frame t, a group on the clip played backwards frame T-1-t."""
+    return [list(range(T - 1, -1, -1)) if r else list(range(T)) for r in reversed_groups]
+
+
+def window_frame_map(T: int, S: int, ind: int, reversed_groups) -> List[List[int]]:
+    """Sliding-window model, window starting at `ind` (non-streaming): frames of the clip padded to a multiple of S with
+    copies of frame T-1.  A forward group reads ind+t.  The reversed clip is padded with copies of the original frame 0,
+    so a reversed group reads max(T-1-ind-t, 0)."""
+    return [[max(T - 1 - ind - t, 0) for t in range(S)] if r else [ind + t for t in range(S)] for r in reversed_groups]
+
+
+def gather_plan(frame_map):
+    """The runs [a, b) of consecutive frames a frame map references, in order, and the map remapped into the pyramid
+    that concatenates those runs (each referenced frame once)."""
+    used = sorted({f for row in frame_map for f in row})
+    pos = {f: i for i, f in enumerate(used)}
+    runs = []
+    for f in used:
+        if runs and runs[-1][1] == f:
+            runs[-1][1] = f + 1
+        else:
+            runs.append([f, f + 1])
+    return [tuple(r) for r in runs], [[pos[f] for f in row] for row in frame_map]
+
+
+def gather_pyramid(pyr, T: int, H4: int, W4: int, runs) -> torch.Tensor:
+    """Flat pyramid of the frame runs [a, b) of the T-frame pyramid `pyr`, concatenated in order."""
+    out, n = None, 0
+    for a, b in runs:
+        part = engine.slice_pyramid(pyr, T, H4, W4, a, b - a)
+        out = part if out is None else engine.concat_pyramid_frames(out, n, 0, part, b - a, H4, W4)
+        n += b - a
+    return out
+
+
+def _reversed_flags(reversed_groups, G: int) -> List[bool]:
+    flags = [False] * G if reversed_groups is None else [bool(r) for r in reversed_groups]
+    if len(flags) != G:
+        raise engine.EngineError(f"reversed_groups has {len(flags)} entries for {G} groups")
+    return flags
+
+
 class CoTrackerThreeBase(nn.Module):
     def __init__(self, window_len=8, stride=4, corr_radius=3, corr_levels=4, num_virtual_tracks=64,
                  model_resolution=(384, 512), add_space_attn=True, linear_layer_for_vis_conf=True):
@@ -175,27 +219,40 @@ class CoTrackerThreeBase(nn.Module):
         if not video.is_cuda:
             raise engine.EngineError("cotracker_b200 runs on CUDA only; move the module and inputs to a GPU")
 
-    def _refine(self, pyr, H4, W4, support, track_valid, coords, vis, conf, iters, group_sizes):
+    def _refine(self, pyr, H4, W4, support, track_valid, coords, vis, conf, iters, group_sizes, group_frames=None):
+        """group_frames: [G, T] frame map into `pyr` (ct3_update_loop_frames), None = frame t."""
         T, N, _ = coords.shape
         dev = coords.device
         G = len(group_sizes)
+        T_pyr = None if group_frames is None else engine.pyramid_frames(pyr, H4, W4)
         engine.update_loop(self.packed_weights(dev), pyr, H4, W4, support, track_valid, coords, vis, conf,
-                           self.interpolate_time_embed(T).to(dev), iters, self._ws.get(T, N, dev, H4, W4, G),
-                           group_sizes=group_sizes if G > 1 else None)
+                           self.interpolate_time_embed(T).to(dev), iters, self._ws.get(T, N, dev, H4, W4, G, T_pyr),
+                           group_sizes=group_sizes if G > 1 or group_frames is not None else None,
+                           group_frames=group_frames)
+
+    @staticmethod
+    def _track_reversed(group_sizes, flags, device) -> torch.Tensor:
+        """[N] bool: the tracks of the groups flagged as reversed."""
+        return torch.repeat_interleave(torch.tensor(flags, dtype=torch.bool),
+                                       torch.tensor(group_sizes, dtype=torch.int64)).to(device)
 
     @torch.no_grad()
-    def forward_groups(self, video, queries, group_sizes, iters=4, fmaps_chunk_size=200):
+    def forward_groups(self, video, queries, group_sizes, iters=4, fmaps_chunk_size=200, reversed_groups=None):
         """Track G independent query sets over one clip in one pass.
 
         queries [1, sum(group_sizes), 3] holds the groups one after another.  The clip is encoded once and the support
         features are sampled once; each window runs one update loop for all groups together (ct3_update_loop_groups),
         where every group keeps its own virtual tokens.  Returns the 4-tuple of `forward`; the columns of each group
-        are bit-identical to `forward(video, that group's queries)`.  Streaming (is_online=True) is not grouped."""
+        are bit-identical to `forward(video, that group's queries)`.  Streaming (is_online=True) is not grouped.
+        reversed_groups: G flags; a flagged group is tracked on the clip played backwards (its query frames and its
+        output are in reversed-clip time) and its columns are bit-identical to `forward(video.flip(1), its queries)`.
+        The reversed clip is never encoded: those groups read the forward pyramid through a frame map."""
         sizes = [int(g) for g in group_sizes]
         if not sizes or any(g < 1 for g in sizes) or sum(sizes) != queries.shape[1]:
             raise engine.EngineError(f"group_sizes {sizes} must be >= 1 each and sum to the {queries.shape[1]} queries")
+        _reversed_flags(reversed_groups, len(sizes))
         self._check_inputs(video, queries, False)
-        return self._track(video, queries, iters, fmaps_chunk_size, sizes)
+        return self._track(video, queries, iters, fmaps_chunk_size, sizes, reversed_groups=reversed_groups)
 
     # -- internal entry points of the predictors: frames already resized and normalised (cotracker_b200.ingest) --------
     def _check_frames(self, frames, queries):
@@ -237,24 +294,30 @@ class CoTrackerThreeOffline(CoTrackerThreeBase):
         self._check_inputs(video, queries, is_train)
         return self._track(video, queries, iters, fmaps_chunk_size, [queries.shape[1]])
 
-    def _track(self, video, queries, iters, fmaps_chunk_size, group_sizes):
+    def _track(self, video, queries, iters, fmaps_chunk_size, group_sizes, reversed_groups=None):
         B, T, C, H, W = video.shape
         assert T >= 1
         frames = 2.0 * (video[0].float() / 255.0) - 1.0
         pyr = self._encode(frames, fmaps_chunk_size)
-        return self._track_pyramid(pyr, T, H, W, queries, iters, group_sizes)
+        return self._track_pyramid(pyr, T, H, W, queries, iters, group_sizes, reversed_groups)
 
-    def _track_pyramid(self, pyr, T, H, W, queries, iters, group_sizes):
-        """The model after the encoder: pyr = the clip's pyramid (`_encode_clip`), T frames of H x W pixels."""
+    def _track_pyramid(self, pyr, T, H, W, queries, iters, group_sizes, reversed_groups=None):
+        """The model after the encoder: pyr = the clip's pyramid (`_encode_clip`), T frames of H x W pixels.
+        reversed_groups: G flags; a flagged group tracks the clip played backwards (see `forward_groups`)."""
         N = queries.shape[1]
         H4, W4 = H // self.stride, W // self.stride
-        qframes = queries[0, :, 0].long().to(torch.int32).contiguous()
+        flags = _reversed_flags(reversed_groups, len(group_sizes))
+        qframes = queries[0, :, 0].long()
+        if any(flags):   # a reversed group's query frame q is frame T-1-q of the forward pyramid
+            qframes = torch.where(self._track_reversed(group_sizes, flags, qframes.device), T - 1 - qframes, qframes)
+        qframes = qframes.to(torch.int32).contiguous()
         qcoords = (queries[0, :, 1:3].float() / self.stride).contiguous()
         support = engine.sample_support(pyr, T, H4, W4, qframes, qcoords)
         coords = qcoords[None].expand(T, N, 2).contiguous()
         vis = torch.zeros(T, N, device=pyr.device)
         conf = torch.zeros(T, N, device=pyr.device)
-        self._refine(pyr, H4, W4, support, None, coords, vis, conf, iters, group_sizes)
+        self._refine(pyr, H4, W4, support, None, coords, vis, conf, iters, group_sizes,
+                     clip_frame_map(T, flags) if any(flags) else None)
         return (coords * float(self.stride))[None], torch.sigmoid(vis)[None], torch.sigmoid(conf)[None], None
 
 
@@ -313,16 +376,16 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
         S = self.window_len
         return (S - T % S) % S
 
-    def _track(self, video, queries, iters, fmaps_chunk_size, group_sizes, is_online=False):
+    def _track(self, video, queries, iters, fmaps_chunk_size, group_sizes, is_online=False, reversed_groups=None):
         frames = 2.0 * (video[0].float() / 255.0) - 1.0
-        return self._track_normalised(frames, queries, iters, fmaps_chunk_size, group_sizes, is_online)
+        return self._track_normalised(frames, queries, iters, fmaps_chunk_size, group_sizes, is_online, reversed_groups)
 
     def _track_frames(self, frames, queries, iters=4, group_sizes=None, fmaps_chunk_size=200, is_online=False):
         self._check_frames(frames, queries)
         return self._track_normalised(frames, queries, iters, fmaps_chunk_size, group_sizes or [queries.shape[1]],
                                       is_online)
 
-    def _track_normalised(self, frames, queries, iters, fmaps_chunk_size, group_sizes, is_online):
+    def _track_normalised(self, frames, queries, iters, fmaps_chunk_size, group_sizes, is_online, reversed_groups=None):
         T, _, H, W = frames.shape
         S = self.window_len
         assert S >= 2
@@ -334,16 +397,21 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
             pyr_all = self._encode_online(frames, fmaps_chunk_size, S // 2, H4, W4)
         else:
             pyr_all = self._encode_clip(frames, fmaps_chunk_size)
-        return self._track_pyramid(pyr_all, T, H, W, queries, iters, group_sizes, is_online)
+        return self._track_pyramid(pyr_all, T, H, W, queries, iters, group_sizes, is_online, reversed_groups)
 
-    def _track_pyramid(self, pyr_all, T, H, W, queries, iters, group_sizes, is_online=False):
-        """The model after the encoder: pyr_all = the pyramid of the T frames and the padding (`_encode_clip`)."""
+    def _track_pyramid(self, pyr_all, T, H, W, queries, iters, group_sizes, is_online=False, reversed_groups=None):
+        """The model after the encoder: pyr_all = the pyramid of the T frames and the padding (`_encode_clip`).
+        reversed_groups: G flags; a flagged group tracks the clip played backwards (see `forward_groups`).  Each window
+        then runs on the frames its groups reference (at most 2 S), gathered from pyr_all, through a frame map."""
         dev = pyr_all.device
         N = queries.shape[1]
         S = self.window_len
         step = S // 2
         H4, W4 = H // self.stride, W // self.stride
         T_pad = T + ((S - T) if is_online else self._clip_pad(T))
+        flags = _reversed_flags(reversed_groups, len(group_sizes))
+        if is_online and any(flags):
+            raise NotImplementedError("streaming (is_online=True) does not track reversed groups")
         qframes_l = queries[0, :, 0].long()
         qcoords = (queries[0, :, 1:3].float() / self.stride).contiguous()
 
@@ -368,8 +436,10 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
                                   accumulate_mask=entering)
             support = self.online_track_support
         else:
-            support = engine.sample_support(pyr_all, T_pad, H4, W4,
-                                            qframes_l.clamp(0, T_pad - 1).to(torch.int32).contiguous(), qcoords)
+            qf = qframes_l.clamp(0, T_pad - 1)
+            if any(flags):   # frame q of the reversed, padded clip is forward frame max(T-1-q, 0)
+                qf = torch.where(self._track_reversed(group_sizes, flags, dev), (T - 1 - qf).clamp(min=0), qf)
+            support = engine.sample_support(pyr_all, T_pad, H4, W4, qf.to(torch.int32).contiguous(), qcoords)
 
         coords_init = qcoords[None].expand(S, N, 2).contiguous()
         vis_init = torch.zeros(S, N, device=dev)
@@ -392,14 +462,18 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
                 vis_init = torch.where(carry, prev_v, vis_init)
                 conf_init = torch.where(carry, prev_q, conf_init)
             valid = (qframes_l < ind + S).to(torch.uint8).contiguous()                      # reference :484,:493-496
+            frame_map = None
             if is_online:
                 pyr = pyr_all
+            elif any(flags):
+                runs, frame_map = gather_plan(window_frame_map(T, S, ind, flags))
+                pyr = gather_pyramid(pyr_all, T_pad, H4, W4, runs)
             else:
                 pyr = engine.slice_pyramid(pyr_all, T_pad, H4, W4, ind, S)
             coords = coords_init.clone().contiguous()
             vis = vis_init.clone().contiguous()
             conf = conf_init.clone().contiguous()
-            self._refine(pyr, H4, W4, support, valid, coords, vis, conf, iters, group_sizes)
+            self._refine(pyr, H4, W4, support, valid, coords, vis, conf, iters, group_sizes, frame_map)
             S_trim = T if is_online else min(T - ind, S)
             coords_pred[ind:ind + S] = (coords * float(self.stride))[:S_trim]
             vis_pred[ind:ind + S] = vis[:S_trim]

@@ -14,6 +14,13 @@ import torch.nn.functional as F
 
 from . import ingest
 from .build import build_cotracker
+from .evaluation import pass_budget_bytes, plan_dense_passes
+
+# Backward tracking runs the forward and the reversed queries as two groups of one update-loop pass while one direction
+# has at most this many tracks x loop frames, and as two passes above it.  Measured on an H100 (DESIGN.md 4.4.2): one
+# pass is faster at 136 x 50 (-10 %) and 6436 x 16 (-2 %); at 6436 x 50 the loop is throughput-bound, one pass is not
+# faster (+0.3 %) and needs twice the update-loop workspace (45.8 instead of 24.6 GiB).
+BACKWARD_GROUP_TRACK_FRAMES = 1 << 17
 
 
 def get_points_on_a_grid(size: int, extent, device="cpu") -> torch.Tensor:
@@ -50,21 +57,36 @@ class CoTrackerPredictor(torch.nn.Module):
                                            grid_query_frame=grid_query_frame, backward_tracking=backward_tracking)
 
     def _compute_dense_tracks(self, video, grid_query_frame, grid_size=80, backward_tracking=False):
+        """grid_step^2 shifted grids, one query group per offset (and one reversed group per offset with backward
+        tracking), tracked in as few grouped passes over one encoded clip as fit in device memory."""
         *_, H, W = video.shape
         grid_step = W // grid_size
         gw, gh = W // grid_step, H // grid_step
         clip = _EncodedClip(self.model, video, self.interp_shape)   # one resize + encoder pass for every offset
         dev = clip.device
-        tracks = visibilities = None
-        pts = torch.zeros((video.shape[0], gw * gh, 3), device=dev)
-        pts[:, :, 0] = grid_query_frame
+        n_off = grid_step * grid_step
         base_x = (torch.arange(gw, device=dev).repeat(gh) * grid_step).float()
         base_y = (torch.arange(gh, device=dev).repeat_interleave(gw) * grid_step).float()
-        for offset in range(grid_step * grid_step):
-            print(f"step {offset} / {grid_step * grid_step}")
+        queries = []
+        for offset in range(n_off):
+            pts = torch.zeros((video.shape[0], gw * gh, 3), device=dev)
+            pts[:, :, 0] = grid_query_frame
             pts[:, :, 1] = base_x + offset % grid_step
             pts[:, :, 2] = base_y + offset // grid_step
-            t_step, v_step = self._sparse_tracks(clip, video.shape, queries=pts, backward_tracking=backward_tracking)
+            queries.append(self._model_queries(clip, video.shape, pts))
+        per = 2 if backward_tracking else 1
+        groups = [g for q in queries for g in ([q, _reversed_queries(q, clip.T)] if backward_tracking else [q])]
+        _, passes = plan_dense_passes(n_off, gw * gh, backward_tracking, *clip.pass_shape(backward_tracking))
+        outs = []
+        for g0, g1 in passes:
+            for g in range(g0, g1):
+                if g % per == 0:
+                    print(f"step {g // per} / {n_off}")
+            outs += clip.track_groups(groups[g0:g1], [g % per == 1 for g in range(g0, g1)])
+        tracks = visibilities = None
+        for i in range(n_off):
+            t_step, v_step = self._finish(queries[i], outs[per * i], outs[per * i + 1] if backward_tracking else None,
+                                          video.shape)
             tracks = t_step if tracks is None else torch.cat([tracks, t_step], dim=2)
             visibilities = v_step if visibilities is None else torch.cat([visibilities, v_step], dim=2)
         return tracks, visibilities
@@ -77,6 +99,21 @@ class CoTrackerPredictor(torch.nn.Module):
 
     def _sparse_tracks(self, clip, video_shape, queries, segm_mask=None, grid_size=0, add_support_grid=False,
                        grid_query_frame=0, backward_tracking=False):
+        queries = self._model_queries(clip, video_shape, queries, segm_mask, grid_size, add_support_grid,
+                                      grid_query_frame)
+        if backward_tracking:   # the clip played backwards (reference :187-209) is a reversed group
+            inv = _reversed_queries(queries, clip.T)
+            if queries.shape[1] * clip.loop_frames() <= BACKWARD_GROUP_TRACK_FRAMES:
+                fwd, bwd = clip.track_groups([queries, inv], [False, True])
+            else:
+                (fwd,), (bwd,) = clip.track_groups([queries], [False]), clip.track_groups([inv], [True])
+        else:
+            (fwd,), bwd = clip.track_groups([queries], [False]), None
+        return self._finish(queries, fwd, bwd, video_shape, add_support_grid)
+
+    def _model_queries(self, clip, video_shape, queries, segm_mask=None, grid_size=0, add_support_grid=False,
+                       grid_query_frame=0):
+        """The queries [1,N,3] at model resolution (reference :100-160), support grid appended."""
         B, T, C, H, W = video_shape
         ih, iw = self.interp_shape
         dev = clip.device
@@ -93,16 +130,24 @@ class CoTrackerPredictor(torch.nn.Module):
                                        (grid_pts[0, :, 0]).round().long().cpu()].bool()
                 grid_pts = grid_pts[:, keep]
             queries = torch.cat([torch.ones_like(grid_pts[:, :, :1]) * grid_query_frame, grid_pts], dim=2).repeat(B, 1, 1)
-        n_support = self.support_grid_size ** 2
         if add_support_grid:
             sup = get_points_on_a_grid(self.support_grid_size, self.interp_shape, device=dev)
             sup = torch.cat([torch.zeros_like(sup[:, :, :1]), sup], dim=2).repeat(B, 1, 1)
             queries = torch.cat([queries, sup], dim=1)
+        return queries
 
-        tracks, visibilities, *_ = clip.track(queries)
-
-        if backward_tracking:
-            tracks, visibilities = self._compute_backward_tracks(clip, queries, tracks, visibilities)
+    def _finish(self, queries, fwd, bwd, video_shape, add_support_grid=False):
+        """(tracks, visibility) of the forward pass, merged with the backward pass's before each query frame
+        (reference :187-209), support grid dropped, query points pinned, scaled to the input (reference :161-190)."""
+        B, T, C, H, W = video_shape
+        ih, iw = self.interp_shape
+        n_support = self.support_grid_size ** 2
+        tracks, visibilities = fwd
+        if bwd is not None:
+            inv_tracks, inv_vis = bwd[0].flip(1), bwd[1].flip(1)
+            before_query = torch.arange(T, device=queries.device)[None, :, None] < queries[:, None, :, 0]
+            tracks = torch.where(before_query[..., None], inv_tracks, tracks)
+            visibilities = torch.where(before_query, inv_vis, visibilities)
             if add_support_grid:
                 queries[:, -n_support:, 0] = T - 1
         if add_support_grid:
@@ -121,24 +166,19 @@ class CoTrackerPredictor(torch.nn.Module):
         tracks *= tracks.new_tensor([(W - 1) / (iw - 1), (H - 1) / (ih - 1)])
         return tracks, visibilities
 
-    def _compute_backward_tracks(self, clip, queries, tracks, visibilities):
-        """The model on the clip played backwards (reference :187-209), on the forward pass's pyramid reversed in place."""
-        T = clip.T
-        inv_queries = queries.clone()
-        inv_queries[:, :, 0] = T - inv_queries[:, :, 0] - 1
-        inv_tracks, inv_vis, *_ = clip.track(inv_queries, reverse=True)
-        inv_tracks, inv_vis = inv_tracks.flip(1), inv_vis.flip(1)
-        before_query = torch.arange(T, device=queries.device)[None, :, None] < queries[:, None, :, 0]
-        tracks = torch.where(before_query[..., None], inv_tracks, tracks)
-        visibilities = torch.where(before_query, inv_vis, visibilities)
-        return tracks, visibilities
+
+def _reversed_queries(queries, T: int):
+    """The queries on the clip played backwards: query frame t becomes T-1-t (reference :192-195)."""
+    inv = queries.clone()
+    inv[:, :, 0] = T - inv[:, :, 0] - 1
+    return inv
 
 
 class _EncodedClip:
     """One predictor call's clip, resized + normalised (cotracker_b200.ingest) and encoded once; every model pass of
-    the call (dense offsets, backward tracking) runs on this one pyramid.  A pass on the clip played backwards reverses
-    the frames of the pyramid in place (the encoder is strictly per frame, so that is the reversed clip's pyramid), and
-    a later forward pass reverses them back: device memory never holds a second pyramid."""
+    the call (dense offsets, backward tracking) runs on this one pyramid.  A pass on the clip played backwards is a
+    reversed query group (model `reversed_groups`): it reads the forward pyramid through a frame map, so device memory
+    never holds a second pyramid and the pyramid is never reversed."""
 
     ITERS = 6
 
@@ -147,16 +187,34 @@ class _EncodedClip:
         self.model, self.device = model, frames.device
         self.T, _, self.H, self.W = frames.shape
         self.pyr = model._encode_clip(frames)
-        self._reversed = False
 
-    def track(self, queries, reverse=False):
-        """The model's 4-tuple for queries [1,N,3] (model resolution) on the clip, or on the clip played backwards."""
-        if queries.shape[0] != 1:
+    def track_groups(self, groups, reversed_groups):
+        """Query groups [1,n_g,3] (model resolution) in one pass; a flagged group tracks the clip played backwards,
+        with query frames in reversed-clip time.  -> [(tracks [1,T,n_g,2], visibility [1,T,n_g])] per group."""
+        if any(q.shape[0] != 1 for q in groups):
             raise ValueError("CoTracker3 inference requires B == 1 (the reference fails for B > 1 as well)")
-        if reverse != self._reversed:
-            self.model._reverse_clip_pyramid_(self.pyr, self.T, self.H, self.W)
-            self._reversed = reverse
-        return self.model._track_pyramid(self.pyr, self.T, self.H, self.W, queries, self.ITERS, [queries.shape[1]])
+        sizes = [q.shape[1] for q in groups]
+        tr, vi, *_ = self.model._track_pyramid(self.pyr, self.T, self.H, self.W, torch.cat(groups, dim=1), self.ITERS,
+                                               sizes, reversed_groups=list(reversed_groups))
+        out, a = [], 0
+        for n in sizes:
+            out.append((tr[:, :, a:a + n], vi[:, :, a:a + n]))
+            a += n
+        return out
+
+    def loop_frames(self) -> int:
+        """Frames of one update loop: the clip, or the window of the sliding-window model."""
+        return self.model.window_len if hasattr(self.model, "init_video_online_processing") else self.T
+
+    def pass_shape(self, backward: bool):
+        """(T, H4, W4, budget, frames) of `plan_dense_passes`: one update loop's frames (the window of the
+        sliding-window model), the feature map, the free-memory budget of a pass and the pyramid frames a pass with
+        reversed groups reads (a window's gather holds at most two windows)."""
+        s = self.model.stride
+        T_loop = self.loop_frames()
+        frames = (self.T if T_loop == self.T else 2 * T_loop) if backward else None
+        budget = pass_budget_bytes(self.model, self.device, self.T, self.H, self.W)
+        return T_loop, self.H // s, self.W // s, budget, frames
 
 
 class CoTrackerOnlinePredictor(torch.nn.Module):

@@ -221,6 +221,27 @@ int ct3_update_loop_groups(const void* packed, const float* pyr, int H4, int W4,
                            const float* time_emb, int T, int N, int iters, void* workspace,
                            size_t workspace_bytes, ct3_stream_t stream, const int32_t* group_sizes_host, int G);
 
+/* ---- frame maps: groups whose time step t reads a pyramid frame other than t ----------------------------------
+ * ct3_update_loop_groups plus one HOST table group_frames_host [G, T]: at time step t, group g reads pyramid frame
+ * group_frames_host[g*T + t], an index into the T_pyr frames of `pyr` (ct3_pyramid_layout(T_pyr, H4, W4)).  The identity
+ * map (T_pyr = T) is ct3_update_loop_groups; a group tracking the clip played backwards uses T-1-t; a padded window of
+ * the sliding-window model uses clamped indices.  Only correlation sampling reads frames: time attention, the time
+ * embedding, tokens and heads work on the group's own time axis.
+ * Contract: group g's coords/vis/conf are BIT-IDENTICAL to a standalone ct3_update_loop on a pyramid holding frames
+ * group_frames_host[g][0..T) in that order (default options, same device).
+ *   group_frames_host : may be freed when the call returns (the device copy lives in the workspace, filled in stream
+ *                       order like the group table)
+ *   workspace         : ct3_workspace_bytes_frames(T, T_pyr, N, G, H4, W4) bytes (the split-bf16 pyramid copy is sized
+ *                       by T_pyr and made once per call)
+ * A null table, a frame index outside [0, T_pyr), T_pyr < 1 and every invalid argument of ct3_update_loop_groups return
+ * CT3_EINVAL before anything is enqueued; "fuse" = 2 and "attn" = 2 return CT3_EUNSUPPORTED for G > 1. */
+int ct3_workspace_bytes_frames(int T, int T_pyr, int N, int G, int H4, int W4, size_t* out_bytes);
+int ct3_update_loop_frames(const void* packed, const float* pyr, int T_pyr, int H4, int W4, const float* support,
+                           const uint8_t* track_valid, float* coords, float* vis, float* conf,
+                           const float* time_emb, int T, int N, int iters, void* workspace,
+                           size_t workspace_bytes, ct3_stream_t stream, const int32_t* group_sizes_host, int G,
+                           const int32_t* group_frames_host);
+
 /* ---- live profiler (bench.py roofline): CUDA events around every launch of the library, summed per
  * kernel category: 0 corr_sample, 1 gemm (wgmma), 2 attention, 3 layernorm, 4 misc.
  * ct3_profile_enable(1) clears and starts recording; ct3_profile_read synchronises and sums. */
