@@ -896,6 +896,25 @@ int ct3_render_tracks(uint8_t* frames, int T, int H, int W, const float* pts, co
   return 0;
 }
 
+int ct3_render_flow_workspace_bytes(int T, int N, size_t* out_bytes) {
+  if (!out_bytes) return fail(CT3_EINVAL, "null argument%s");
+  if (T < 1 || N < 1) return fail(CT3_EINVAL, "T and N must be >= 1%s");
+  if ((int64_t)T * N > INT32_MAX) return fail(CT3_EINVAL, "T * N too large%s");
+  *out_bytes = align_up(sizeof(unsigned long long));
+  return 0;
+}
+
+int ct3_render_flow_colors(const float* pts, int T, int N, int query_frame, uint8_t* colors, void* workspace,
+                           size_t workspace_bytes, ct3_stream_t stream) {
+  if (!pts || !colors || !workspace) return fail(CT3_EINVAL, "null argument%s");
+  size_t need = 0;
+  if (int rc = ct3_render_flow_workspace_bytes(T, N, &need)) return rc;
+  if (query_frame < 0 || query_frame >= T) return fail(CT3_EINVAL, "query_frame must be in [0, T)%s");
+  if (workspace_bytes < need) return fail(CT3_EINVAL, "workspace too small%s");
+  CK(launch_render_flow_colors(pts, T, N, query_frame, colors, workspace, (cudaStream_t)stream), "render_flow_colors");
+  return 0;
+}
+
 int ct3_sample_support(const float* pyr, int T, int H4, int W4, const int32_t* queried_frames,
                        const float* queried_coords, int N, const uint8_t* accumulate_mask, float* support,
                        ct3_stream_t stream) {

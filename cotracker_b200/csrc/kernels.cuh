@@ -34,6 +34,9 @@ cudaError_t launch_render_tracks(uint8_t* frames, int T, int H, int W, const flo
                                  const uint8_t* colors, const uint8_t* draw_mask, int N, int radius, int linewidth,
                                  int trail, int query_frame, const double* alphas, const double* diff, int* keys,
                                  cudaStream_t s);
+// pts [T,N,2] fp32 -> colors [T,N,3] uint8 (flow_vis colours of the flow from query_frame); workspace: one u64
+cudaError_t launch_render_flow_colors(const float* pts, int T, int N, int query_frame, uint8_t* colors, void* workspace,
+                                      cudaStream_t s);
 
 // ---- enc_tail.cu : conv2 -> InstanceNorm -> ReLU -> conv3 of the encoder on the GEMM engine --------
 cudaError_t launch_im2col3x3_split(const float* in, int T, int C, int H, int W, int Kpad, __nv_bfloat16* out,

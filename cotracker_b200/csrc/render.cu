@@ -312,9 +312,109 @@ __global__ void __launch_bounds__(kThreads) resolve_kernel(uint8_t* __restrict__
   }
 }
 
+// ---- optical-flow colours: flow_vis.flow_to_color(tracks - tracks[query_frame]) ---------------------------------
+// Every operation is the float64 one numpy performs, as an explicit _rn intrinsic (no contraction); only atan2 is
+// CUDA's (within 2 ulp of the correctly rounded value, as numpy's own SIMD and libm atan2 are not exact either).
+constexpr int kWheel = 55;   // Middlebury colour wheel: RY 15, YG 6, GC 4, CB 11, BM 13, MR 6
+struct ColorWheel { uint8_t c[kWheel][3]; };
+
+// make_colorwheel(): floor(255 * i / n) is exact in integers for these sizes
+ColorWheel make_colorwheel() {
+  ColorWheel w;
+  const int n[6] = {15, 6, 4, 11, 13, 6};
+  // per segment: the channel held at 255, the channel that ramps, and whether it ramps up (floor(255*i/n)) or down
+  const int full[6] = {0, 1, 1, 2, 2, 0}, ramp[6] = {1, 0, 2, 1, 0, 2}, up[6] = {1, 0, 1, 0, 1, 0};
+  int k = 0;
+  for (int s = 0; s < 6; ++s)
+    for (int i = 0; i < n[s]; ++i, ++k) {
+      w.c[k][0] = w.c[k][1] = w.c[k][2] = 0;
+      const int r = 255 * i / n[s];
+      w.c[k][full[s]] = 255;
+      w.c[k][ramp[s]] = (uint8_t)(up[s] ? r : 255 - r);
+    }
+  return w;
+}
+
+// tracks.long() of one coordinate, kept where |x|, |y| < 2^30 so that squared norms of differences fit in int64:
+// NaN counts as 0 and anything at or beyond +-2^30 (infinities included) as +-(2^30 - 1)
+__device__ __forceinline__ int64_t flow_coord(float v) {
+  if (v != v) return 0;
+  if (!(fabsf(v) < kCoordLimit)) return v > 0.0f ? (1 << 30) - 1 : -((1 << 30) - 1);
+  return (int64_t)(int)v;
+}
+
+__device__ __forceinline__ void flow_at(const float* __restrict__ pts, int N, int query_frame, int64_t e, int64_t* u,
+                                        int64_t* v) {
+  const int64_t i = e % N;
+  const float* p = pts + e * 2;
+  const float* q = pts + ((int64_t)query_frame * N + i) * 2;
+  *u = flow_coord(p[0]) - flow_coord(q[0]);
+  *v = flow_coord(p[1]) - flow_coord(q[1]);
+}
+
+// rad2max = max over all (t, n) of u*u + v*v in int64 (max of sqrt(float64(.)) is sqrt(float64(max)): both monotone).
+// Grid-stride, one atomicMax per warp on a zeroed u64: the maximum does not depend on the order.
+__global__ void __launch_bounds__(kThreads) flow_radmax_kernel(const float* __restrict__ pts, int N, int query_frame,
+                                                               int64_t total, unsigned long long* __restrict__ rad2max) {
+  unsigned long long m = 0;
+  for (int64_t e = (int64_t)blockIdx.x * kThreads + threadIdx.x; e < total; e += (int64_t)gridDim.x * kThreads) {
+    int64_t u, v;
+    flow_at(pts, N, query_frame, e, &u, &v);
+    const unsigned long long r2 = (unsigned long long)(u * u + v * v);
+    m = r2 > m ? r2 : m;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long x = __shfl_xor_sync(0xffffffffu, m, o);
+    m = x > m ? x : m;
+  }
+  if ((threadIdx.x & 31) == 0 && m > 0) atomicMax(rad2max, m);
+}
+
+// thread = entry (t, n): flow_uv_to_colors after the normalisation by rad_max + 1e-5
+__global__ void __launch_bounds__(kThreads) flow_color_kernel(const float* __restrict__ pts, int N, int query_frame,
+                                                              int64_t total,
+                                                              const unsigned long long* __restrict__ rad2max,
+                                                              ColorWheel wheel, uint8_t* __restrict__ colors) {
+  const int64_t e = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+  if (e >= total) return;
+  int64_t iu, iv;
+  flow_at(pts, N, query_frame, e, &iu, &iv);
+  const double den = __dadd_rn(__dsqrt_rn(__ull2double_rn(*rad2max)), 1e-5);
+  const double u = __ddiv_rn(__ll2double_rn(iu), den), v = __ddiv_rn(__ll2double_rn(iv), den);
+  const double rad = __dsqrt_rn(__dadd_rn(__dmul_rn(u, u), __dmul_rn(v, v)));
+  const double a = __ddiv_rn(atan2(-v, -u), 3.141592653589793);              // np.arctan2(-v, -u) / np.pi
+  const double fk = __dmul_rn(__ddiv_rn(__dadd_rn(a, 1.0), 2.0), (double)(kWheel - 1));
+  const int k0 = (int)floor(fk);
+  const int k1 = k0 + 1 == kWheel ? 0 : k0 + 1;
+  const double f = __dsub_rn(fk, (double)k0), g = __dsub_rn(1.0, f);
+  // an atan2 a few ulp below -pi gives k0 = -1, which numpy's indexing reads as the last row
+  const int r0 = k0 < 0 ? k0 + kWheel : k0;
+  uint8_t* out = colors + e * 3;
+#pragma unroll
+  for (int ch = 0; ch < 3; ++ch) {
+    const double c0 = __ddiv_rn((double)wheel.c[r0][ch], 255.0), c1 = __ddiv_rn((double)wheel.c[k1][ch], 255.0);
+    double col = __dadd_rn(__dmul_rn(g, c0), __dmul_rn(f, c1));
+    col = rad <= 1.0 ? __dsub_rn(1.0, __dmul_rn(rad, __dsub_rn(1.0, col))) : __dmul_rn(col, 0.75);
+    out[ch] = (uint8_t)(int)floor(__dmul_rn(255.0, col));
+  }
+}
+
 unsigned blocks(int64_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
 
 }  // namespace
+
+cudaError_t launch_render_flow_colors(const float* pts, int T, int N, int query_frame, uint8_t* colors, void* workspace,
+                                      cudaStream_t s) {
+  const int64_t total = (int64_t)T * N;
+  unsigned long long* rad2max = static_cast<unsigned long long*>(workspace);
+  cudaError_t e = cudaMemsetAsync(rad2max, 0, sizeof(unsigned long long), s);
+  if (e != cudaSuccess) return e;
+  const unsigned nb = blocks(total);
+  flow_radmax_kernel<<<nb < 1024 ? nb : 1024, kThreads, 0, s>>>(pts, N, query_frame, total, rad2max);
+  flow_color_kernel<<<nb, kThreads, 0, s>>>(pts, N, query_frame, total, rad2max, make_colorwheel(), colors);
+  return cudaGetLastError();
+}
 
 cudaError_t launch_render_prepare(const void* src, int dtype, int T, int H, int W, int64_t st, int64_t sc, int64_t sh,
                                   int64_t sw, int pad, int gray, uint8_t* out, cudaStream_t s) {

@@ -49,6 +49,8 @@ def _declare(lib):
         "ct3_render_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
         "ct3_render_tracks": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                       c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+        "ct3_render_flow_workspace_bytes": (c_int, [c_int, c_int, ctypes.POINTER(c_size_t)]),
+        "ct3_render_flow_colors": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
         "ct3_sample_support": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
         "ct3_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
         "ct3_update_loop": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -103,6 +105,7 @@ EXPORTED_SYMBOLS = [
     "ct3_workspace_bytes_frames", "ct3_update_loop_frames",
     "ct3_prepare_frames",
     "ct3_render_prepare", "ct3_render_workspace_bytes", "ct3_render_tracks",
+    "ct3_render_flow_workspace_bytes", "ct3_render_flow_colors",
 ]
 
 
@@ -308,6 +311,29 @@ def render_tracks(frames: torch.Tensor, pts: torch.Tensor, colors: torch.Tensor,
                                        _ptr(diff), _ptr(workspace), workspace.numel(), _stream(dev)),
                "ct3_render_tracks")
     return frames
+
+
+def render_flow_workspace_bytes(T: int, N: int) -> int:
+    n = ctypes.c_size_t(0)
+    _check(lib().ct3_render_flow_workspace_bytes(T, N, ctypes.byref(n)), "ct3_render_flow_workspace_bytes")
+    return n.value
+
+
+def render_flow_colors(pts: torch.Tensor, query_frame: int) -> torch.Tensor:
+    """pts [T,N,2] fp32 CUDA tensor (the frame pixel coordinates render_tracks takes) -> [T,N,3] uint8 on its device:
+    flow_vis.flow_to_color(pts.long() - pts[query_frame].long()), the colours of the visualiser's optical_flow mode
+    (see ct3_render_flow_colors in include/ct3_b200.h for the atan2 tolerance)."""
+    _req(pts, torch.float32, "pts")
+    if pts.dim() != 3 or pts.shape[2] != 2:
+        raise EngineError(f"pts must be [T,N,2], got {tuple(pts.shape)}")
+    T, N, _ = pts.shape
+    dev = pts.device
+    workspace = torch.empty(render_flow_workspace_bytes(T, N), dtype=torch.uint8, device=dev)
+    colors = torch.empty(T, N, 3, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _check(lib().ct3_render_flow_colors(_ptr(pts), T, N, int(query_frame), _ptr(colors), _ptr(workspace),
+                                            workspace.numel(), _stream(dev)), "ct3_render_flow_colors")
+    return colors
 
 
 def pyramid_levels(pyr: torch.Tensor, T: int, H4: int, W4: int) -> List[torch.Tensor]:

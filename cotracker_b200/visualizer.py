@@ -6,12 +6,16 @@
 The frames are bit-identical to the reference's PIL drawing.  The padding, grayscale, discs, outlines and trails run
 as CUDA kernels (ct3_render_prepare / ct3_render_tracks, csrc/render.cu) on the device copy of the clip; the host only
 computes colours ([T,N] numbers) and, with compensate_for_camera_motion, the per-frame camera offsets, exactly as the
-reference does, and copies the finished frames back once.
+reference does, and copies the finished frames back once.  mode="optical_flow" colours every (t, n) by its flow from
+query_frame (flow_vis.flow_to_color); those colours come from a kernel too (ct3_render_flow_colors), so the tracks
+never come to the host.  Every operation there is the reference's float64 one except atan2, the one IEEE leaves open
+(numpy's own result depends on the CPU); a colour that depended on its last bits could differ by 1 (DESIGN.md §4.9.1).
+On a host without a CUDA device the constructor raises NotImplementedError for this mode, as it has no host path.
 
 Video may be on the host or the device, uint8 or float (other float dtypes are cast to float32 first); tracks and
 visibility may be on either too.  matplotlib and imageio are imported only when a colour map or a video file is needed.
-Not provided: mode="optical_flow" (needs flow_vis) and gt_tracks (the reference's _draw_gt_tracks rebinds its own input
-inside the loop and fails for more than one point, so it has no behaviour to match).
+Not provided: gt_tracks (the reference's _draw_gt_tracks rebinds its own input inside the loop and fails for more than
+one point, so it has no behaviour to match).
 """
 from __future__ import annotations
 
@@ -107,8 +111,10 @@ class Visualizer:
         show_first_frame: int = 10,
         tracks_leave_trace: int = 0,  # -1 for infinite
     ):
-        if mode == "optical_flow":
-            raise NotImplementedError("mode='optical_flow' is not provided: it needs the flow_vis package")
+        if mode == "optical_flow" and not torch.cuda.is_available():
+            # the colours of this mode exist only as a library kernel (no host flow_vis path), so say so at once
+            raise NotImplementedError("mode='optical_flow' computes flow_vis's colour code on the GPU "
+                                      "(ct3_render_flow_colors); no CUDA device is available")
         self.mode = mode
         self.save_dir = save_dir
         self._color_map = None   # resolved from matplotlib on first use unless a caller sets color_map
@@ -257,11 +263,13 @@ class Visualizer:
         if tp.dtype != torch.float32:
             tp = torch.where(torch.isfinite(tp.double()), torch.trunc(tp.double()), tp.double()).float()
         pts = tp.to(dev).contiguous()
-        # colours: only [N] slices of the tracks come to the host
-        y_query = (tracks[0, query_frame, :, 1] + pad).long().cpu().numpy()
-        y_first = (tracks[0, 0, :, 1] + pad).long().cpu().numpy()
         segm = None if segm_mask is None else torch.as_tensor(segm_mask).reshape(-1).cpu().numpy()
-        colors = torch.from_numpy(self._colors(y_query, y_first, segm, T)).to(dev)
+        if self.mode == "optical_flow":   # every (t, n) has its own colour: computed where the tracks are
+            colors = engine.render_flow_colors(pts, query_frame)
+        else:   # only [N] slices of the tracks come to the host
+            y_query = (tracks[0, query_frame, :, 1] + pad).long().cpu().numpy()
+            y_first = (tracks[0, 0, :, 1] + pad).long().cpu().numpy()
+            colors = torch.from_numpy(self._colors(y_query, y_first, segm, T)).to(dev)
         vis = None
         if visibility is not None:
             vis = (visibility[0].reshape(T, N) != 0).to(device=dev, dtype=torch.uint8).contiguous()

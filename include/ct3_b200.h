@@ -143,6 +143,20 @@ int ct3_render_tracks(uint8_t* frames, int T, int H, int W, const float* pts, co
                       const uint8_t* colors, const uint8_t* draw_mask, int N, int radius, int linewidth, int trail,
                       int query_frame, const double* alphas, const double* diff, void* workspace,
                       size_t workspace_bytes, ct3_stream_t stream);
+/* Scratch of ct3_render_flow_colors (one u64).  CT3_EINVAL unless T, N >= 1 and T*N <= INT32_MAX. */
+int ct3_render_flow_workspace_bytes(int T, int N, size_t* out_bytes);
+/* ct3_render_flow_colors: the colours of mode="optical_flow" (visualizer.py:191-194),
+ *     flow_vis.flow_to_color(tracks - tracks[query_frame]) with tracks = pts.long(),
+ * the Middlebury colour code normalised by the largest flow magnitude over all T*N entries, into `colors` [T,N,3]
+ * uint8 in the layout ct3_render_tracks reads.  pts [T,N,2] fp32 as ct3_render_tracks takes it, truncated toward zero.
+ * Every float64 operation is numpy's, correctly rounded and uncontracted, except atan2, which is CUDA's (within 2 ulp
+ * of the correctly rounded value); an entry whose colour depends on atan2's last bits may differ by 1 from a CPU's.
+ * The result is exact for points whose truncated coordinates have magnitude below 2^30; beyond that a coordinate
+ * counts as +-(2^30 - 1) and NaN as 0, so every result is defined and deterministic.  The maximum is reduced on the
+ * device, in stream order, without host synchronisation.  Null pointers, T or N < 1, T*N > INT32_MAX, query_frame
+ * outside [0, T) or a too small workspace return CT3_EINVAL before any launch. */
+int ct3_render_flow_colors(const float* pts, int T, int N, int query_frame, uint8_t* colors, void* workspace,
+                           size_t workspace_bytes, ct3_stream_t stream);
 
 /* ---- per-clip preparation ---------------------------------------------------
  * ct3_prepare_pyramid: cotracker3_offline.py:92-117 (L2-normalise over channels,
