@@ -1,0 +1,844 @@
+// api_loop.cu -- the update loop of the C ABI (see include/ct3_b200.h): weight packing, workspace carving and the
+// launch sequence of one refinement iteration (cotracker3_offline.py:139-216, cotracker.py:483-531).
+#include <math.h>
+
+#include <string>
+#include <vector>
+
+#include "abi.cuh"
+
+using namespace ct3;
+
+namespace {
+
+// ------------------------------------------------------------------------------------------------
+// packed-weights layout
+struct Block {
+  Lin qkv_h;  // time blocks only: q|k|v regrouped per head, rows h*144 + [q_h(48) | k_h(48) | v_h(48)] (fused attention)
+  Lin q;    // self-attention blocks: fused q|k|v (N = 1152); cross blocks: to_q (N = 384)
+  Lin kv;   // cross blocks only: to_kv (N = 768)
+  Lin kv_f; // cross blocks only: to_kv with the affine norm_context folded in (W diag(gamma), b + W beta)
+  Lin out, fc1, fc2;
+  size_t ctx_g = 0, ctx_b = 0;  // cross blocks: norm_context weight / bias (fp32 [384])
+  bool cross = false;
+};
+struct Layout {
+  Lin corr_fc1, corr_fc2, in_tr;
+  Lin corr_fc1_h;   // corr_mlp.fc1 once more as split fp16 planes (prec.fc1 = 1 | 2); shares corr_fc1's bias
+  Lin corr_fc1_t, corr_fc1_th;   // the same two with the columns in corr_tc3.cu's support-major volume order
+  Block time[kDepth], vself[kDepth], p2v[kDepth], v2p[kDepth];
+  size_t heads_w = 0, heads_b = 0, virt = 0, win_f32 = 0;
+  size_t scratch = 0;   // pack-time scratch: one folded to_kv weight [768, 384] + bias [768] in fp32
+  size_t total = 0;
+};
+
+void place_block(Block& b, bool cross, size_t& off, bool time = false) {
+  b.cross = cross;
+  if (time) place_lin(b.qkv_h, 3 * kC, kC, off);
+  if (cross) {
+    b.ctx_g = off; off = align_up(off + kC * sizeof(float));
+    b.ctx_b = off; off = align_up(off + kC * sizeof(float));
+    place_lin(b.q, kC, kC, off);
+    place_lin(b.kv, 2 * kC, kC, off);
+    place_lin(b.kv_f, 2 * kC, kC, off);
+  } else {
+    place_lin(b.q, 3 * kC, kC, off);
+  }
+  place_lin(b.out, kC, kC, off);
+  place_lin(b.fc1, kMlpHid, kC, off);
+  place_lin(b.fc2, kC, kMlpHid, off);
+}
+const Layout& layout() {
+  static const Layout L0 = [] {   // C++11 thread-safe one-time initialisation
+    Layout L;
+    size_t off = 0;
+    place_lin(L.corr_fc1, kCorrHid, kVol, off);
+    place_lin(L.corr_fc1_h, kCorrHid, kVol, off);
+    place_lin(L.corr_fc1_t, kCorrHid, kVol, off);
+    place_lin(L.corr_fc1_th, kCorrHid, kVol, off);
+    place_lin(L.corr_fc2, kCorrOut, kCorrHid, off);
+    place_lin(L.in_tr, kC, kX, off);
+    L.win_f32 = off; off = align_up(off + (size_t)kC * kX * sizeof(float));
+    L.virt = off;    off = align_up(off + (size_t)kV * kC * sizeof(float));
+    L.heads_w = off; off = align_up(off + 4 * kC * sizeof(float));
+    L.heads_b = off; off = align_up(off + 4 * sizeof(float));
+    for (int i = 0; i < kDepth; ++i) {
+      place_block(L.time[i], false, off, /*time*/ true);
+      place_block(L.vself[i], false, off);
+      place_block(L.p2v[i], true, off);
+      place_block(L.v2p[i], true, off);
+    }
+    L.scratch = off;
+    off = align_up(off + (size_t)2 * kC * kC * sizeof(float) + (size_t)2 * kC * sizeof(float));
+    L.total = off;
+    return L;
+  }();
+  return L0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// weight tensor order expected by ct3_pack_weights
+const std::vector<std::string>& weight_names() {
+  static const std::vector<std::string> names0 = [] {
+    std::vector<std::string> names;
+    const char* head[] = {"corr_mlp.fc1.weight", "corr_mlp.fc1.bias", "corr_mlp.fc2.weight", "corr_mlp.fc2.bias",
+                          "updateformer.input_transform.weight", "updateformer.input_transform.bias",
+                          "updateformer.virual_tracks", "updateformer.flow_head.weight", "updateformer.flow_head.bias",
+                          "updateformer.vis_conf_head.weight", "updateformer.vis_conf_head.bias"};
+    for (const char* h : head) names.push_back(h);
+    const char* self_t[] = {"attn.to_q.weight", "attn.to_q.bias", "attn.to_kv.weight", "attn.to_kv.bias",
+                            "attn.to_out.weight", "attn.to_out.bias", "mlp.fc1.weight", "mlp.fc1.bias",
+                            "mlp.fc2.weight", "mlp.fc2.bias"};
+    const char* cross_t[] = {"norm_context.weight", "norm_context.bias", "cross_attn.to_q.weight",
+                             "cross_attn.to_q.bias", "cross_attn.to_kv.weight", "cross_attn.to_kv.bias",
+                             "cross_attn.to_out.weight", "cross_attn.to_out.bias", "mlp.fc1.weight", "mlp.fc1.bias",
+                             "mlp.fc2.weight", "mlp.fc2.bias"};
+    for (int i = 0; i < kDepth; ++i) {
+      const std::string idx = std::to_string(i) + ".";
+      for (const char* t : self_t) names.push_back("updateformer.time_blocks." + idx + t);
+      for (const char* t : self_t) names.push_back("updateformer.space_virtual_blocks." + idx + t);
+      for (const char* t : cross_t) names.push_back("updateformer.space_point2virtual_blocks." + idx + t);
+      for (const char* t : cross_t) names.push_back("updateformer.space_virtual2point_blocks." + idx + t);
+    }
+    return names;
+  }();
+  return names0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// workspace
+struct Workspace {
+  __nv_bfloat16* vol;     // [N*T*4, 2*2432]
+  __nv_bfloat16* h1;      // [N*T*4, 2*384]
+  __nv_bfloat16* xs;      // [N*T, 2*1152]
+  float* tokens;          // [(N+64)*T, 384]
+  __nv_bfloat16* traw;    // [(N+64)*T, 2*384]  the token rows once more as a split operand (LayerNorm fold)
+  float* tstat;           // [(N+64)*T, 24, 2]  partial (sum, sum of squares) of every token row
+  __nv_bfloat16* ln;      // [(N+64)*T, 2*384]
+  __nv_bfloat16* att;     // [(N+64)*T, 2*384]
+  float* qkv;             // [(N+64)*T, 1152]   (also point q [N*T,384] / point kv [N*T,768])
+  float* vqkv;            // [64*T, 1152]       (virtual q / kv / qkv)
+  __nv_bfloat16* hmid;    // [(N+64)*T, 2*1536]
+  float* row_bias;        // [T, 384]
+  float* att_part;        // split-K partials of the virtual<-point attention
+  __nv_bfloat16* pyr_split;  // split-bf16 copy of the pyramid (corr_tc2.cu); null when H4 == 0
+  int32_t* groups;        // device group table of a grouped call (GroupPlan); null when G == 1
+  int32_t* frames;        // device frame map [G, T] of ct3_update_loop_frames; null without one
+  size_t total;
+};
+// split-K slots of the virtual<-point partials: a group of n tracks splits at most min(32, ceil(n/64)/2) ways
+// (attention_tc_splits), so G groups of N tracks in all need at most (N + 63 G)/128 slots beyond one group's 32
+int partial_slots(int N, int G) {
+  if (G == 1) return kAttnMaxSplits;
+  const int64_t s = kAttnMaxSplits + ((int64_t)N + 63LL * G) / 128;
+  return (int)(s < (int64_t)kAttnMaxSplits * G ? s : (int64_t)kAttnMaxSplits * G);
+}
+// int32 entries of the group table: offsets [G+1] | all [G] | split [G] | slot [G] | small [G] | tiles [2 * max tiles]
+int64_t group_table_ints(int N, int G) { return G == 1 ? 0 : (int64_t)5 * G + 1 + 2 * ((int64_t)N / 128 + G); }
+
+// T_pyr: frames of the pyramid the correlation reads (sizes the split copy; 0 = T); frames: room for a [G, T] frame map
+Workspace carve(void* base, int T, int N, int H4 = 0, int W4 = 0, int G = 1, int T_pyr = 0, bool frames = false) {
+  Workspace w;
+  if (T_pyr == 0) T_pyr = T;
+  const size_t R = (size_t)(N + (size_t)kV * G) * T, Rp = (size_t)N * T, Rv = (size_t)kV * G * T, Mc = Rp * kL;
+  Carver c(base);
+  w.vol = (__nv_bfloat16*)c.take(Mc * 2 * kVolPad * 2);
+  w.h1 = (__nv_bfloat16*)c.take(Mc * 2 * kCorrHid * 2);
+  w.xs = (__nv_bfloat16*)c.take(Rp * 2 * kXPad * 2);
+  w.tokens = (float*)c.take(R * kC * 4);
+  w.traw = (__nv_bfloat16*)c.take(R * 2 * kC * 2);
+  w.tstat = (float*)c.take(R * kLnParts * 2 * 4);
+  w.ln = (__nv_bfloat16*)c.take(R * 2 * kC * 2);
+  w.att = (__nv_bfloat16*)c.take(R * 2 * kC * 2);
+  w.qkv = (float*)c.take(R * 3 * kC * 4);
+  w.vqkv = (float*)c.take(Rv * 3 * kC * 4);
+  w.hmid = (__nv_bfloat16*)c.take(R * 2 * kMlpHid * 2);
+  w.row_bias = (float*)c.take((size_t)T * kC * 4);
+  w.att_part = (float*)c.take(attention_partial_bytes(T, kV, partial_slots(N, G)));
+  w.pyr_split = nullptr;
+  if (H4 > 0 && W4 > 0 && corr_patch_supported(T_pyr, H4, W4))
+    w.pyr_split = (__nv_bfloat16*)c.take((size_t)pyramid_layout(T_pyr, H4, W4).total * 4);
+  w.groups = G > 1 ? (int32_t*)c.take((size_t)group_table_ints(N, G) * 4) : nullptr;
+  w.frames = frames ? (int32_t*)c.take((size_t)G * T * 4) : nullptr;
+  w.total = c.off;
+  return w;
+}
+
+// ------------------------------------------------------------------------------------------------
+struct Runner {
+  const uint8_t* pk;
+  const Layout& L;
+  cudaStream_t s;
+  int impl;
+
+  int gemm(const char* what, const __nv_bfloat16* x, const Lin& lin, int M, const GemmEpilogue& e, int products = 3,
+           int fp16 = 0, int64_t x_ld = 0) {
+    GemmProblem p;
+    p.products = products;
+    p.fp16 = fp16;
+    p.x_ld = x_ld;
+    p.x_split = x;
+    p.w_split = reinterpret_cast<const __nv_bfloat16*>(pk + lin.w);
+    p.M = M;
+    p.N = lin.N;
+    p.Kpad = lin.Kpad;
+    p.epi = e;
+    if (!p.epi.bias) p.epi.bias = reinterpret_cast<const float*>(pk + lin.b);
+    if (M == 0) return 0;
+    ProfScope ps(s, CAT_GEMM, 2.0 * (double)M * lin.N * lin.K);
+    return run_gemm(p, impl, s, what);
+  }
+  static GemmEpilogue to_f32(float* out, int ld, bool residual) {
+    GemmEpilogue e;
+    e.out_f32 = out; e.ld_f32 = ld; e.residual = residual ? 1 : 0;
+    return e;
+  }
+  static GemmEpilogue to_split(__nv_bfloat16* out, int ld, int lo_off, int act) {
+    GemmEpilogue e;
+    e.out_split = out; e.ld_split = ld; e.lo_off = lo_off; e.act = act;
+    return e;
+  }
+};
+
+// a kernel launch returning cudaError_t, inside a profiler scope of category cat
+#define RUNC(cat, call)                                        \
+  do {                                                         \
+    cudaError_t e__;                                           \
+    { ProfScope ps__(R.s, cat); e__ = (cudaError_t)(call); }   \
+    if (e__ != cudaSuccess) return fail_cuda(e__, #call);      \
+  } while (0)
+// a linear layer through R.gemm; the call's text names the layer in the error message
+#define GEMM(...)                                                              \
+  do {                                                                         \
+    if (int rc__ = R.gemm("gemm(" #__VA_ARGS__ ")", __VA_ARGS__)) return rc__; \
+  } while (0)
+
+int run_attention(Runner& R, const Workspace& W, const AttnParams& a, bool per_warp) {
+  if (g_opt_attn == 1) return (int)launch_attention(a, R.s);
+  // point <- virtual (64 keys per frame, thousands of queries): wgmma kernel with TMA row staging (attention_p2v.cu)
+  if (g_opt_attn == 0 && !per_warp && a.Lq > kV && attention_p2v_supported(a)) return (int)launch_attention_p2v(a, R.s);
+  return (int)launch_attention_tc(a, per_warp, W.att_part, num_sms(), R.s);
+}
+
+// One attention of a transformer block: q at column 0 of q, k / v at columns k_col / v_col of kv, the result as split
+// rows of `out` (pitch 2*kC).  Space attention (tracks == 0): one sequence per frame t < T of Lq queries over Lk keys,
+// token i at row i*T + t.  Time attention: one sequence per track (`tracks` of them) over its T frames, rows n*T + t.
+AttnParams attn_params(const float* q, int q_ld, const float* kv, int kv_ld, int k_col, int v_col, __nv_bfloat16* out,
+                       int Lq, int Lk, int T, int tracks = 0) {
+  AttnParams a{};
+  a.q = q; a.q_ld = q_ld; a.q_col = 0;
+  a.kv = kv; a.kv_ld = kv_ld; a.k_col = k_col; a.v_col = v_col;
+  a.out = out; a.out_ld = 2 * kC; a.lo_off = kC;
+  a.num_seq = tracks ? tracks : T; a.Lq = Lq; a.Lk = Lk;
+  a.q_seq_stride = a.k_seq_stride = tracks ? T : 1;
+  a.q_tok_stride = a.k_tok_stride = tracks ? 1 : T;
+  a.scale = 1.0f / sqrtf((float)kDh);
+  return a;
+}
+
+// Track groups of a grouped call (ct3_update_loop_groups): G contiguous track ranges, each with its own kV virtual
+// tokens at rows (N + kV*g + i)*T + t.  G == 1 is the plain call (no table; every kernel indexes as it always did).
+// For G > 1 the host builds the table below, uploads it into the workspace in stream order, and each space attention
+// runs over (group, frame) sequences, choosing per group what a standalone call on that group's tracks would.
+struct GroupPlan {
+  int G = 1, max_n = 0;
+  const int32_t *off = nullptr, *all = nullptr, *split = nullptr, *slot = nullptr, *small = nullptr, *tile = nullptr;
+  int n_small = 0, n_tiles = 0, split_max = 1, split_slots = 0;
+};
+
+int plan_groups(GroupPlan& gp, const int32_t* sizes, int G, int T, int N, int32_t* dev, cudaStream_t s) {
+  gp.G = G;
+  if (G == 1) return 0;
+  std::vector<int32_t> h((size_t)group_table_ints(N, G), 0);
+  int32_t* off = h.data();
+  int32_t *all = off + G + 1, *split = all + G, *slot = split + G, *small = slot + G, *tile = small + G;
+  const int nsm = num_sms();
+  for (int g = 0; g < G; ++g) {
+    const int n = sizes[g];
+    off[g + 1] = off[g] + n;
+    if (n > gp.max_n) gp.max_n = n;
+    all[g] = g;
+    // virtual <- point: the split-K count of a standalone call (T sequences of kV queries over n keys)
+    split[g] = attention_tc_splits(T, kV, n, nsm);
+    if (split[g] > 1) {
+      slot[g] = gp.split_slots;
+      gp.split_slots += split[g];
+      if (split[g] > gp.split_max) gp.split_max = split[g];
+    }
+    // point <- virtual: a standalone call runs more than kV tracks on the wgmma kernel, fewer on mma.sync (run_attention)
+    if (n > kV) {
+      for (int n0 = off[g]; n0 < off[g + 1]; n0 += 128, ++gp.n_tiles) {
+        tile[2 * gp.n_tiles] = g;
+        tile[2 * gp.n_tiles + 1] = n0;
+      }
+    } else {
+      small[gp.n_small++] = g;
+    }
+  }
+  if (gp.split_slots > partial_slots(N, G)) return fail(CT3_EINVAL, "split-K partials exceed the workspace%s");
+  CK(launch_upload_i32(dev, h.data(), (int)h.size(), s), "upload group table");
+  gp.off = dev;
+  gp.all = dev + (all - off);
+  gp.split = dev + (split - off);
+  gp.slot = dev + (slot - off);
+  gp.small = dev + (small - off);
+  gp.tile = dev + (tile - off);
+  return 0;
+}
+
+// One space attention of a block (cotracker.py:510-517) over every group.  `a` describes it for one group of N tracks
+// (sequence = frame); q_pts / k_pts tell which side holds the point tokens.
+int space_attention(Runner& R, const Workspace& W, const GroupPlan& gp, AttnParams a, bool q_pts, bool k_pts) {
+  if (gp.G == 1) return run_attention(R, W, a, false);
+  const int T = a.num_seq, n_all = a.Lq;
+  a.goff = gp.off;
+  a.frames = T;
+  a.q_grp_stride = q_pts ? 0 : (int64_t)kV * a.q_tok_stride;
+  a.k_grp_stride = k_pts ? 0 : (int64_t)kV * a.k_tok_stride;
+  a.Lq = q_pts ? gp.max_n : kV;
+  a.Lk = k_pts ? gp.max_n : kV;
+  AttnParams b = a;
+  b.gl = gp.all;
+  b.num_seq = T * gp.G;
+  if (g_opt_attn == 1) return (int)launch_attention(b, R.s);
+  if (!q_pts) {   // virtual <- point (split-K per group) and virtual self attention
+    if (k_pts) { b.gsplit = gp.split; b.gslot = gp.slot; b.split_max = gp.split_max; b.split_slots = gp.split_slots; }
+    return (int)launch_attention_tc(b, false, W.att_part, num_sms(), R.s);
+  }
+  // point <- virtual
+  if (gp.n_small > 0) {
+    b.gl = gp.small;
+    b.num_seq = T * gp.n_small;
+    b.Lq = kV;
+    if (int rc = (int)launch_attention_tc(b, false, W.att_part, num_sms(), R.s)) return rc;
+  }
+  if (gp.n_tiles > 0) {
+    AttnParams c = a;
+    c.gtile = gp.tile;
+    c.tiles = gp.n_tiles;
+    c.Lq = n_all;
+    c.Lk = kV * gp.G;
+    return (int)launch_attention_p2v(c, R.s);
+  }
+  return 0;
+}
+
+// q|k|v projection and the per-track T x T attention of time block b in ONE kernel: fp32 q|k|v never reaches HBM.
+// ln_part: x holds the raw token rows and the LayerNorm is applied in the epilogue (transformer_body_fold).
+int qkv_time_attention(Runner& R, const Workspace& W, const Block& b, const __nv_bfloat16* x, const float* ln_part,
+                       int rows, int T) {
+  ProfScope ps(R.s, CAT_QKVA, 0.0);
+  const char* gerr = nullptr;
+  const int rc = gemm_qkv_time_attn_launch(
+      x, reinterpret_cast<const __nv_bfloat16*>(R.pk + b.qkv_h.w), reinterpret_cast<const float*>(R.pk + b.qkv_h.b),
+      rows, kC, T, W.att, 2 * kC, kC, 1.0f / sqrtf((float)kDh), ln_part,
+      ln_part ? reinterpret_cast<const float*>(R.pk + b.qkv_h.ws) : nullptr, ln_part ? 1e-6f : 0.f, num_sms(), R.s,
+      &gerr);
+  return rc ? fail_launch(rc, "fused qkv + time attention", gerr) : 0;
+}
+
+// x += to_out(attn(...)); x += mlp(LN(x))   for the rows [row0, row0+rows) of the token buffer
+int mlp_half(Runner& R, const Workspace& W, const Block& b, int64_t row0, int rows) {
+  float* x = W.tokens + row0 * kC;
+  __nv_bfloat16* ln = W.ln + row0 * 2 * kC;
+  __nv_bfloat16* hm = W.hmid + row0 * 2 * kMlpHid;
+  RUNC(CAT_LN, launch_layernorm_split(x, rows, nullptr, nullptr, 1e-6f, ln, R.s));
+  GEMM(ln, b.fc1, rows, Runner::to_split(hm, 2 * kMlpHid, kMlpHid, /*tanh*/ 2));
+  GEMM(hm, b.fc2, rows, Runner::to_f32(x, kC, true));
+  return 0;
+}
+
+// EfficientUpdateFormer body on W.tokens (point rows already hold input_transform output) -- cotracker.py:486-524
+int transformer_body(Runner& R, const Workspace& W, int T, int N, const GroupPlan& gp) {
+  const Layout& L = R.L;
+  const int Rp = N * T, Rv = kV * gp.G * T, Rall = Rp + Rv;
+  const uint8_t* pk = R.pk;
+  RUNC(CAT_MISC, launch_init_virtual(W.tokens, reinterpret_cast<const float*>(pk + L.virt), T, N, gp.G, R.s));
+  float* vtok = W.tokens + (int64_t)Rp * kC;
+  __nv_bfloat16* ln_p = W.ln;
+  __nv_bfloat16* ln_v = W.ln + (int64_t)Rp * 2 * kC;
+  __nv_bfloat16* att_p = W.att;
+  __nv_bfloat16* att_v = W.att + (int64_t)Rp * 2 * kC;
+
+  for (int i = 0; i < kDepth; ++i) {
+    {  // ---- time block over every token row (points + virtual): sequence = track (cotracker.py:494-495)
+      const Block& b = L.time[i];
+      RUNC(CAT_LN, launch_layernorm_split(W.tokens, Rall, nullptr, nullptr, 1e-6f, W.ln, R.s));
+      if (g_opt[OPT_FUSE] >= 1 && R.impl == 0 && g_opt_attn != 1 && qkv_time_attn_supported(T)) {
+        if (int rc = qkv_time_attention(R, W, b, W.ln, nullptr, Rall, T)) return rc;
+      } else {
+        GEMM(W.ln, b.q, Rall, Runner::to_f32(W.qkv, 3 * kC, false));
+        RUNC(CAT_ATTN, run_attention(R, W, attn_params(W.qkv, 3 * kC, W.qkv, 3 * kC, kC, 2 * kC, W.att, T, T, T,
+                                                       N + kV * gp.G), true));
+      }
+      GEMM(W.att, b.out, Rall, Runner::to_f32(W.tokens, kC, true));
+      if (int rc = mlp_half(R, W, b, 0, Rall)) return rc;
+    }
+    {  // ---- virtual <- point cross attention (cotracker.py:510-512): x = virtual, context = points
+      const Block& b = L.v2p[i];
+      RUNC(CAT_LN, launch_layernorm_split(vtok, Rv, nullptr, nullptr, 1e-6f, ln_v, R.s));
+      RUNC(CAT_LN, launch_layernorm_split(W.tokens, Rp, reinterpret_cast<const float*>(pk + b.ctx_g),
+                                 reinterpret_cast<const float*>(pk + b.ctx_b), 1e-5f, ln_p, R.s));
+      GEMM(ln_v, b.q, Rv, Runner::to_f32(W.vqkv, kC, false));
+      GEMM(ln_p, b.kv, Rp, Runner::to_f32(W.qkv, 2 * kC, false));
+      RUNC(CAT_ATTN, space_attention(R, W, gp, attn_params(W.vqkv, kC, W.qkv, 2 * kC, 0, kC, att_v, kV, N, T), false,
+                                     true));
+      GEMM(att_v, b.out, Rv, Runner::to_f32(vtok, kC, true));
+      if (int rc = mlp_half(R, W, b, Rp, Rv)) return rc;
+    }
+    {  // ---- virtual self attention (cotracker.py:514): sequence = frame over the 64 virtual tokens
+      const Block& b = L.vself[i];
+      RUNC(CAT_LN, launch_layernorm_split(vtok, Rv, nullptr, nullptr, 1e-6f, ln_v, R.s));
+      GEMM(ln_v, b.q, Rv, Runner::to_f32(W.vqkv, 3 * kC, false));
+      RUNC(CAT_ATTN, space_attention(R, W, gp, attn_params(W.vqkv, 3 * kC, W.vqkv, 3 * kC, kC, 2 * kC, att_v, kV, kV,
+                                                           T), false, false));
+      GEMM(att_v, b.out, Rv, Runner::to_f32(vtok, kC, true));
+      if (int rc = mlp_half(R, W, b, Rp, Rv)) return rc;
+    }
+    {  // ---- point <- virtual cross attention (cotracker.py:515-517): x = points, context = virtual
+      const Block& b = L.p2v[i];
+      RUNC(CAT_LN, launch_layernorm_split(W.tokens, Rp, nullptr, nullptr, 1e-6f, ln_p, R.s));
+      RUNC(CAT_LN, launch_layernorm_split(vtok, Rv, reinterpret_cast<const float*>(pk + b.ctx_g),
+                                 reinterpret_cast<const float*>(pk + b.ctx_b), 1e-5f, ln_v, R.s));
+      GEMM(ln_p, b.q, Rp, Runner::to_f32(W.qkv, kC, false));
+      GEMM(ln_v, b.kv, Rv, Runner::to_f32(W.vqkv, 2 * kC, false));
+      RUNC(CAT_ATTN, space_attention(R, W, gp, attn_params(W.qkv, kC, W.vqkv, 2 * kC, 0, kC, att_p, N, kV, T), true,
+                                     false));
+      GEMM(att_p, b.out, Rp, Runner::to_f32(W.tokens, kC, true));
+      if (int rc = mlp_half(R, W, b, 0, Rp)) return rc;
+    }
+  }
+  return 0;
+}
+
+// effective precision of the correlation branch for this thread's options: the single-plane / fewer-product modes
+// exist in corr_tc2.cu only, so whenever another correlation kernel runs the branch computes split x split
+struct Prec {
+  int corr, fc1; bool patch;
+  bool vol16() const { return fc1 < 3; }
+  bool support_major() const { return patch && corr != 3 && g_opt_corr == 0; }   // corr_tc3.cu writes k*49 + i
+};
+Prec effective_prec(bool have_pyr_split, int T, int H4, int W4) {
+  Prec p;
+  p.patch = corr_uses_patch_kernel(g_opt_corr, have_pyr_split, T, H4, W4);
+  p.corr = p.patch ? g_opt[OPT_PREC_CORR] : 3;
+  p.fc1 = p.patch ? g_opt[OPT_PREC_FC1] : 3;
+  return p;
+}
+
+// LayerNorm-folded variant of transformer_body (option fuse = 2, tensor-core kernels, T <= 128): no LayerNorm kernel
+// runs.  Every GEMM that writes token rows (input_transform, to_out, mlp.fc2) also emits them as a split-bf16 operand
+// plus partial row statistics (GemmEpilogue::raw_split / stat_part); every GEMM that consumes LN(x) multiplies the
+// RAW rows and applies  rstd * (W.x - mean * wsum) + b  in its epilogue; the affine norm_context of the cross blocks
+// (cotracker.py:539-540) is folded into to_kv's weights and bias at pack time (Block::kv_f).
+bool fold_enabled(const Runner& R, int T) {
+  return g_opt[OPT_FUSE] == 2 && R.impl == 0 && g_opt_attn != 1 && qkv_time_attn_supported(T);
+}
+
+int transformer_body_fold(Runner& R, const Workspace& W, int T, int N) {
+  const Layout& L = R.L;
+  const int Rp = N * T, Rv = kV * T, Rall = Rp + Rv;
+  const uint8_t* pk = R.pk;
+  RUNC(CAT_MISC, launch_init_virtual(W.tokens, reinterpret_cast<const float*>(pk + L.virt), T, N, 1, R.s));
+  float* vtok = W.tokens + (int64_t)Rp * kC;
+  __nv_bfloat16* raw_p = W.traw;
+  __nv_bfloat16* raw_v = W.traw + (int64_t)Rp * 2 * kC;
+  float* st_p = W.tstat;
+  float* st_v = W.tstat + (int64_t)Rp * kLnParts * 2;
+  __nv_bfloat16* att_p = W.att;
+  __nv_bfloat16* att_v = W.att + (int64_t)Rp * 2 * kC;
+  RUNC(CAT_LN, launch_rowstats_split(vtok, Rv, raw_v, st_v, R.s));
+  auto ln = [&](GemmEpilogue e, const float* part, const Lin& lin, float eps) {
+    e.ln_part = part; e.ln_wsum = reinterpret_cast<const float*>(pk + lin.ws); e.ln_eps = eps;
+    return e;
+  };
+  auto prod = [&](GemmEpilogue e, __nv_bfloat16* raw, float* stat) { e.raw_split = raw; e.stat_part = stat; return e; };
+  // x += mlp(LN(x)) on rows [row0, row0 + rows)
+  auto mlp = [&](const Block& b, int64_t row0, int rows) -> int {
+    float* x = W.tokens + row0 * kC;
+    __nv_bfloat16* raw = W.traw + row0 * 2 * kC;
+    float* st = W.tstat + row0 * kLnParts * 2;
+    __nv_bfloat16* hm = W.hmid + row0 * 2 * kMlpHid;
+    GEMM(raw, b.fc1, rows, ln(Runner::to_split(hm, 2 * kMlpHid, kMlpHid, /*tanh*/ 2), st, b.fc1, 1e-6f));
+    GEMM(hm, b.fc2, rows, prod(Runner::to_f32(x, kC, true), raw, st));
+    return 0;
+  };
+  for (int i = 0; i < kDepth; ++i) {
+    {  // ---- time block (cotracker.py:494-495)
+      const Block& b = L.time[i];
+      if (int rc = qkv_time_attention(R, W, b, W.traw, W.tstat, Rall, T)) return rc;
+      GEMM(W.att, b.out, Rall, prod(Runner::to_f32(W.tokens, kC, true), W.traw, W.tstat));
+      if (int rc = mlp(b, 0, Rall)) return rc;
+    }
+    {  // ---- virtual <- point cross attention (cotracker.py:510-512)
+      const Block& b = L.v2p[i];
+      GEMM(raw_v, b.q, Rv, ln(Runner::to_f32(W.vqkv, kC, false), st_v, b.q, 1e-6f));
+      GEMM(raw_p, b.kv_f, Rp, ln(Runner::to_f32(W.qkv, 2 * kC, false), st_p, b.kv_f, 1e-5f));
+      RUNC(CAT_ATTN, run_attention(R, W, attn_params(W.vqkv, kC, W.qkv, 2 * kC, 0, kC, att_v, kV, N, T), false));
+      GEMM(att_v, b.out, Rv, prod(Runner::to_f32(vtok, kC, true), raw_v, st_v));
+      if (int rc = mlp(b, Rp, Rv)) return rc;
+    }
+    {  // ---- virtual self attention (cotracker.py:514)
+      const Block& b = L.vself[i];
+      GEMM(raw_v, b.q, Rv, ln(Runner::to_f32(W.vqkv, 3 * kC, false), st_v, b.q, 1e-6f));
+      RUNC(CAT_ATTN, run_attention(R, W, attn_params(W.vqkv, 3 * kC, W.vqkv, 3 * kC, kC, 2 * kC, att_v, kV, kV, T),
+                                   false));
+      GEMM(att_v, b.out, Rv, prod(Runner::to_f32(vtok, kC, true), raw_v, st_v));
+      if (int rc = mlp(b, Rp, Rv)) return rc;
+    }
+    {  // ---- point <- virtual cross attention (cotracker.py:515-517)
+      const Block& b = L.p2v[i];
+      GEMM(raw_p, b.q, Rp, ln(Runner::to_f32(W.qkv, kC, false), st_p, b.q, 1e-6f));
+      GEMM(raw_v, b.kv_f, Rv, ln(Runner::to_f32(W.vqkv, 2 * kC, false), st_v, b.kv_f, 1e-5f));
+      RUNC(CAT_ATTN, run_attention(R, W, attn_params(W.qkv, kC, W.vqkv, 2 * kC, 0, kC, att_p, N, kV, T), false));
+      GEMM(att_p, b.out, Rp, prod(Runner::to_f32(W.tokens, kC, true), raw_p, st_p));
+      if (int rc = mlp(b, 0, Rp)) return rc;
+    }
+  }
+  return 0;
+}
+
+// The steps update_loop and updateformer share: input_transform of the X rows in W.xs into the point tokens (with the
+// per-frame bias row_bias [T, kC] when given), the transformer body, then the heads: the state update of coords / vis /
+// conf, or with delta != nullptr the raw deltas [N,T,4] instead.
+int transform_and_heads(Runner& R, const Workspace& W, int T, int N, const GroupPlan& gp, const float* row_bias,
+                        float* coords, float* vis, float* conf, float* delta) {
+  const Layout& L = R.L;
+  const bool fold = fold_enabled(R, T);
+  GemmEpilogue e = Runner::to_f32(W.tokens, kC, false);
+  if (row_bias) { e.row_bias = row_bias; e.row_mod = T; }
+  if (fold) { e.raw_split = W.traw; e.stat_part = W.tstat; }
+  GEMM(W.xs, L.in_tr, N * T, e);
+  if (int rc = fold ? transformer_body_fold(R, W, T, N) : transformer_body(R, W, T, N, gp)) return rc;
+  RUNC(CAT_MISC, launch_heads(W.tokens, reinterpret_cast<const float*>(R.pk + L.heads_w),
+                              reinterpret_cast<const float*>(R.pk + L.heads_b), coords, vis, conf, delta, T, N, R.s));
+  return 0;
+}
+
+int check_TN(int T, int N, int G = 1) {
+  if (T < 1 || N < 1) return fail(CT3_EINVAL, "T and N must be >= 1%s");
+  if (G < 1 || G > N) return fail(CT3_EINVAL, "G must be in [1, N]%s");
+  if (((int64_t)N + (int64_t)kV * G) * T * 3 * kC >= (int64_t)1 << 40) return fail(CT3_EINVAL, "problem too large%s");
+  return 0;
+}
+
+// T, N and the track groups of update_loop / updateformer, in this order; *total = the tracks the sizes add up to.
+// n_from_sizes (updateformer with N < 0): the sizes define N, which is then checked after them.
+int check_groups(int T, int N, const int32_t* sizes, int G, int* total, bool n_from_sizes) {
+  if (!n_from_sizes)
+    if (int rc = check_TN(T, N)) return rc;
+  if (!sizes) return fail(CT3_EINVAL, "null group_sizes_host%s");
+  if (G < 1) return fail(CT3_EINVAL, "G must be >= 1%s");
+  int64_t sum = 0;
+  for (int g = 0; g < G; ++g) {
+    if (sizes[g] < 1) return fail(CT3_EINVAL, "every group size must be >= 1%s");
+    sum += sizes[g];
+  }
+  if (sum > (int64_t)1 << 30) return fail(CT3_EINVAL, "problem too large%s");
+  if (!n_from_sizes && sum != N) return fail(CT3_EINVAL, "group sizes must sum to N%s");
+  if (G > 1 && (g_opt[OPT_FUSE] == 2 || g_opt_attn == 2))
+    return fail(CT3_EUNSUPPORTED, "grouped calls do not support fuse = 2 or attn = 2%s");
+  *total = (int)sum;
+  return check_TN(T, *total, G);
+}
+
+// frame-map arguments of ct3_update_loop_frames / ct3_workspace_bytes_frames (frames == nullptr: not checked here)
+int check_frames(const int32_t* frames, int G, int T, int T_pyr) {
+  if (T_pyr < 1) return fail(CT3_EINVAL, "T_pyr must be >= 1%s");
+  if ((int64_t)T_pyr * T >= (int64_t)1 << 31 || (int64_t)G * T >= (int64_t)1 << 31)
+    return fail(CT3_EINVAL, "problem too large%s");
+  if (!frames) return 0;
+  for (int64_t i = 0; i < (int64_t)G * T; ++i)
+    if (frames[i] < 0 || frames[i] >= T_pyr) return fail(CT3_EINVAL, "frame index outside [0, T_pyr)%s");
+  return 0;
+}
+
+// ct3_workspace_bytes_groups (frames == false, T_pyr == T: the pyramid shape is checked only when given) and
+// ct3_workspace_bytes_frames
+int loop_workspace_bytes(int T, int T_pyr, int N, int G, int H4, int W4, bool frames, size_t* out_bytes) {
+  if (!out_bytes) return fail(CT3_EINVAL, "null out_bytes%s");
+  if (int rc = check_TN(T, N, G)) return rc;
+  if (frames)
+    if (int rc = check_frames(nullptr, G, T, T_pyr)) return rc;
+  if (frames || H4 != 0 || W4 != 0)
+    if (int rc = check_pyramid(T_pyr, H4, W4)) return rc;
+  *out_bytes = carve(nullptr, T, N, H4, W4, G, T_pyr, frames).total;
+  return 0;
+}
+
+// frames: host frame map [G, T] into the T_pyr pyramid frames, or null (frame t, T_pyr == T)
+int update_loop(const void* packed, const float* pyr, int H4, int W4, const float* support, const uint8_t* track_valid,
+                float* coords, float* vis, float* conf, const float* time_emb, int T, int N, const int32_t* sizes,
+                int G, int iters, void* workspace, size_t workspace_bytes, cudaStream_t stream, int T_pyr,
+                const int32_t* frames) {
+  if (!packed || !pyr || !support || !coords || !vis || !conf || !time_emb || !workspace)
+    return fail(CT3_EINVAL, "null argument%s");
+  int total = 0;
+  if (int rc = check_groups(T, N, sizes, G, &total, false)) return rc;
+  if (iters < 0) return fail(CT3_EINVAL, "iters must be >= 0%s");
+  if (int rc = check_frames(frames, G, T, T_pyr)) return rc;
+  if (int rc = check_pyramid(T_pyr, H4, W4)) return rc;
+  if (int rc = check_aligned(workspace, "workspace")) return rc;
+  const Workspace W = carve(workspace, T, N, H4, W4, G, T_pyr, frames != nullptr);
+  if (int rc = check_space(workspace_bytes, W.total, "workspace")) return rc;
+  const Layout& L = layout();
+  Runner R{reinterpret_cast<const uint8_t*>(packed), L, stream, g_opt_gemm};
+  GroupPlan gp;
+  if (int rc = plan_groups(gp, sizes, G, T, N, W.groups, R.s)) return rc;
+  FrameMap fm;
+  if (frames) {   // the frame map reaches the device like the group table: in stream order, through kernel arguments
+    CK(launch_upload_i32(W.frames, frames, G * T, R.s), "upload frame map");
+    fm.frames = W.frames;
+    fm.goff = G > 1 ? gp.off : nullptr;
+    fm.G = G;
+  }
+  const int Mc = N * T * kL;
+  // split-bf16 copy of the pyramid: the TMA source of the correlation kernel, made once per call
+  const Prec pr = effective_prec(W.pyr_split != nullptr, T_pyr, H4, W4);
+  const __nv_bfloat16* pyr_split = (pr.patch && iters > 0) ? W.pyr_split : nullptr;
+  if (pyr_split) RUNC(CAT_MISC, launch_split_pyramid(pyr, T_pyr, H4, W4, W.pyr_split, pr.corr, R.s));
+
+  // W_in * time_emb[t]: x + time_emb is folded into a per-frame bias of input_transform (cotracker3_offline.py:196)
+  RUNC(CAT_MISC, launch_row_bias(time_emb, reinterpret_cast<const float*>(R.pk + L.win_f32), T, W.row_bias, R.s));
+
+  for (int it = 0; it < iters; ++it) {
+    // (i)+(ii) sampling + 4-D correlation, all levels -> split volume
+    RUNC(CAT_CORR, launch_corr_sample(pyr, pyr_split, H4, W4, support, track_valid, coords, T, N, W.vol, g_opt_corr,
+                                      pr.corr, pr.vol16() ? 1 : 0, num_sms(), R.s, T_pyr, fm));
+    // (iii) corr_mlp: 2401 -> 384 (GELU erf) -> 256, written straight into X columns [256*l, 256*l+256)
+    if (pr.vol16()) {   // single fp16 volume plane x split fp16 weights: 2 (or 1) tensor-core products per FLOP
+      GEMM(W.vol, pr.support_major() ? L.corr_fc1_th : L.corr_fc1_h, Mc,
+           Runner::to_split(W.h1, 2 * kCorrHid, kCorrHid, /*erf*/ 1), pr.fc1, /*fp16*/ 1, kVolPad);
+    } else {
+      GEMM(W.vol, pr.support_major() ? L.corr_fc1_t : L.corr_fc1, Mc,
+           Runner::to_split(W.h1, 2 * kCorrHid, kCorrHid, /*erf*/ 1));
+    }
+    {
+      GemmEpilogue e = Runner::to_split(W.xs, 2 * kXPad, kXPad, 0);
+      e.row_group = kL;
+      GEMM(W.h1, L.corr_fc2, Mc, e);
+    }
+    // vis, conf, posenc(rel. motion), zero pad -> X columns [1024,1152)
+    RUNC(CAT_MISC, launch_build_x_small(coords, vis, conf, T, N, W.xs, R.s));
+    // (iv) input_transform (+ folded time embedding) -> point tokens -> transformer; (v) heads + state update
+    if (int rc = transform_and_heads(R, W, T, N, gp, W.row_bias, coords, vis, conf, nullptr)) return rc;
+  }
+  return 0;
+}
+
+// N < 0: the group sizes define N (ct3_updateformer_groups)
+int updateformer(const void* packed, const float* x, int T, int N, const int32_t* sizes, int G, float* delta,
+                 void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (!packed || !x || !delta || !workspace) return fail(CT3_EINVAL, "null argument%s");
+  if (int rc = check_groups(T, N, sizes, G, &N, N < 0)) return rc;
+  if (int rc = check_aligned(workspace, "workspace")) return rc;
+  const Workspace W = carve(workspace, T, N, 0, 0, G);
+  if (int rc = check_space(workspace_bytes, W.total, "workspace")) return rc;
+  Runner R{reinterpret_cast<const uint8_t*>(packed), layout(), stream, g_opt_gemm};
+  GroupPlan gp;
+  if (int rc = plan_groups(gp, sizes, G, T, N, W.groups, R.s)) return rc;
+  RUNC(CAT_MISC, launch_split_rows(x, N * T, kX, kXPad, /*perm_x*/ 1, W.xs, 0, R.s));
+  return transform_and_heads(R, W, T, N, gp, nullptr, nullptr, nullptr, nullptr, delta);
+}
+
+}  // namespace
+
+// ================================================================================================
+extern "C" {
+
+int ct3_volume_is_support_major(int T, int H4, int W4, int* flag) {
+  if (!flag) return fail(CT3_EINVAL, "null argument%s");
+  if (int rc = check_pyramid(T, H4, W4)) return rc;
+  *flag = effective_prec(true, T, H4, W4).support_major() ? 1 : 0;
+  return 0;
+}
+
+int ct3_precision_info(int T, int H4, int W4, int* corr_products, int* fc1_products, int* volume_bytes_per_element) {
+  if (int rc = check_pyramid(T, H4, W4)) return rc;
+  const Prec pr = effective_prec(true, T, H4, W4);
+  if (corr_products) *corr_products = pr.corr;
+  if (fc1_products) *fc1_products = pr.fc1;
+  if (volume_bytes_per_element) *volume_bytes_per_element = pr.vol16() ? 2 : 4;
+  return 0;
+}
+
+int ct3_num_weight_tensors(void) { return (int)weight_names().size(); }
+const char* ct3_weight_name(int index) {
+  const auto& n = weight_names();
+  if (index < 0 || index >= (int)n.size()) return nullptr;
+  return n[index].c_str();
+}
+
+int ct3_packed_weights_bytes(size_t* out_bytes) {
+  if (!out_bytes) return fail(CT3_EINVAL, "null out_bytes%s");
+  *out_bytes = layout().total;
+  return 0;
+}
+
+int ct3_pack_weights(const float* const* t, int n_tensors, void* packed, size_t packed_bytes, ct3_stream_t stream) {
+  const Layout& L = layout();
+  if (!t || !packed) return fail(CT3_EINVAL, "null argument%s");
+  if (n_tensors != (int)weight_names().size()) return fail(CT3_EINVAL, "wrong number of weight tensors%s");
+  if (int rc = check_space(packed_bytes, L.total, "packed buffer")) return rc;
+  for (int i = 0; i < n_tensors; ++i)
+    if (!t[i]) return fail(CT3_EINVAL, "null weight tensor: %s", weight_names()[i].c_str());
+  cudaStream_t s = (cudaStream_t)stream;
+  uint8_t* pk = reinterpret_cast<uint8_t*>(packed);
+  CK(cudaMemsetAsync(pk, 0, L.total, s), "memset packed");
+  auto put_lin = [&](const Lin& l, const float* w, const float* b, int rows, int row_off, int perm,
+                     int fp16 = 0) -> cudaError_t {
+    cudaError_t e = launch_split_rows(w, rows, l.K, l.Kpad, perm, reinterpret_cast<__nv_bfloat16*>(pk + l.w), row_off, s, fp16);
+    if (e != cudaSuccess) return e;
+    e = launch_rowsum(w, rows, l.K, reinterpret_cast<float*>(pk + l.ws) + row_off, s);
+    if (e != cudaSuccess) return e;
+    return cudaMemcpyAsync(pk + l.b + (size_t)row_off * 4, b, (size_t)rows * 4, cudaMemcpyDeviceToDevice, s);
+  };
+  auto put_f32 = [&](size_t off, const float* src, size_t count) {
+    return cudaMemcpyAsync(pk + off, src, count * 4, cudaMemcpyDeviceToDevice, s);
+  };
+  int k = 0;
+  CK(put_lin(L.corr_fc1, t[k], t[k + 1], kCorrHid, 0, 0), "pack corr_fc1");
+  CK(put_lin(L.corr_fc1_h, t[k], t[k + 1], kCorrHid, 0, 0, /*fp16*/ 1), "pack corr_fc1 (fp16 planes)");
+  CK(put_lin(L.corr_fc1_t, t[k], t[k + 1], kCorrHid, 0, /*volume transpose*/ 2), "pack corr_fc1 (support-major)");
+  CK(put_lin(L.corr_fc1_th, t[k], t[k + 1], kCorrHid, 0, 2, /*fp16*/ 1), "pack corr_fc1 (support-major, fp16)"); k += 2;
+  CK(put_lin(L.corr_fc2, t[k], t[k + 1], kCorrOut, 0, 0), "pack corr_fc2"); k += 2;
+  CK(put_lin(L.in_tr, t[k], t[k + 1], kC, 0, /*perm_x*/ 1), "pack input_transform");
+  CK(put_f32(L.win_f32, t[k], (size_t)kC * kX), "pack input_transform fp32"); k += 2;
+  CK(put_f32(L.virt, t[k], (size_t)kV * kC), "pack virtual tracks"); k += 1;
+  CK(put_f32(L.heads_w, t[k], 2 * kC), "pack flow_head.w");
+  CK(put_f32(L.heads_b, t[k + 1], 2), "pack flow_head.b"); k += 2;
+  CK(put_f32(L.heads_w + 2 * kC * 4, t[k], 2 * kC), "pack vis_conf_head.w");
+  CK(put_f32(L.heads_b + 2 * 4, t[k + 1], 2), "pack vis_conf_head.b"); k += 2;
+  auto put_self = [&](const Block& b) -> cudaError_t {
+    cudaError_t e;
+    if ((e = put_lin(b.q, t[k], t[k + 1], kC, 0, 0)) != cudaSuccess) return e;            // to_q  -> rows [0,384)
+    if ((e = put_lin(b.q, t[k + 2], t[k + 3], 2 * kC, kC, 0)) != cudaSuccess) return e;   // to_kv -> rows [384,1152)
+    if (b.qkv_h.N != 0) {   // per-head regrouping for the fused projection + time attention kernel
+      for (int h = 0; h < kHeads; ++h) {
+        const size_t wo = (size_t)h * kDh * kC;
+        if ((e = put_lin(b.qkv_h, t[k] + wo, t[k + 1] + h * kDh, kDh, h * 3 * kDh, 0)) != cudaSuccess) return e;                         // q_h
+        if ((e = put_lin(b.qkv_h, t[k + 2] + wo, t[k + 3] + h * kDh, kDh, h * 3 * kDh + kDh, 0)) != cudaSuccess) return e;               // k_h
+        if ((e = put_lin(b.qkv_h, t[k + 2] + (size_t)kC * kC + wo, t[k + 3] + kC + h * kDh, kDh, h * 3 * kDh + 2 * kDh, 0)) != cudaSuccess) return e;   // v_h
+      }
+    }
+    if ((e = put_lin(b.out, t[k + 4], t[k + 5], kC, 0, 0)) != cudaSuccess) return e;
+    if ((e = put_lin(b.fc1, t[k + 6], t[k + 7], kMlpHid, 0, 0)) != cudaSuccess) return e;
+    if ((e = put_lin(b.fc2, t[k + 8], t[k + 9], kC, 0, 0)) != cudaSuccess) return e;
+    k += 10;
+    return cudaSuccess;
+  };
+  auto put_cross = [&](const Block& b) -> cudaError_t {
+    cudaError_t e;
+    if ((e = put_f32(b.ctx_g, t[k], kC)) != cudaSuccess) return e;
+    if ((e = put_f32(b.ctx_b, t[k + 1], kC)) != cudaSuccess) return e;
+    if ((e = put_lin(b.q, t[k + 2], t[k + 3], kC, 0, 0)) != cudaSuccess) return e;
+    if ((e = put_lin(b.kv, t[k + 4], t[k + 5], 2 * kC, 0, 0)) != cudaSuccess) return e;
+    {   // to_kv(norm_context(x)) with the affine part folded into the layer (stream-ordered reuse of the scratch)
+      float* w2 = reinterpret_cast<float*>(pk + L.scratch);
+      float* b2 = w2 + (size_t)2 * kC * kC;
+      if ((e = launch_affine_fold(t[k + 4], t[k + 5], t[k], t[k + 1], 2 * kC, kC, w2, b2, s)) != cudaSuccess) return e;
+      if ((e = put_lin(b.kv_f, w2, b2, 2 * kC, 0, 0)) != cudaSuccess) return e;
+    }
+    if ((e = put_lin(b.out, t[k + 6], t[k + 7], kC, 0, 0)) != cudaSuccess) return e;
+    if ((e = put_lin(b.fc1, t[k + 8], t[k + 9], kMlpHid, 0, 0)) != cudaSuccess) return e;
+    if ((e = put_lin(b.fc2, t[k + 10], t[k + 11], kC, 0, 0)) != cudaSuccess) return e;
+    k += 12;
+    return cudaSuccess;
+  };
+  for (int i = 0; i < kDepth; ++i) {
+    CK(put_self(L.time[i]), "pack time block");
+    CK(put_self(L.vself[i]), "pack virtual block");
+    CK(put_cross(L.p2v[i]), "pack point2virtual block");
+    CK(put_cross(L.v2p[i]), "pack virtual2point block");
+  }
+  return 0;
+}
+
+int ct3_workspace_bytes(int T, int N, int H4, int W4, size_t* out_bytes) {
+  return loop_workspace_bytes(T, T, N, 1, H4, W4, false, out_bytes);
+}
+
+int ct3_workspace_bytes_groups(int T, int N, int G, int H4, int W4, size_t* out_bytes) {
+  return loop_workspace_bytes(T, T, N, G, H4, W4, false, out_bytes);
+}
+
+int ct3_workspace_bytes_frames(int T, int T_pyr, int N, int G, int H4, int W4, size_t* out_bytes) {
+  return loop_workspace_bytes(T, T_pyr, N, G, H4, W4, true, out_bytes);
+}
+
+int ct3_corr_sample(const float* pyr, int H4, int W4, const float* support, const uint8_t* track_valid,
+                    const float* coords, int T, int N, void* vol_split, void* scratch, size_t scratch_bytes,
+                    ct3_stream_t stream) {
+  if (!pyr || !support || !coords || !vol_split) return fail(CT3_EINVAL, "null argument%s");
+  if (int rc = check_TN(T, N)) return rc;
+  if (int rc = check_pyramid(T, H4, W4)) return rc;
+  const __nv_bfloat16* pyr_split = nullptr;
+  const Prec pr = effective_prec(scratch != nullptr, T, H4, W4);
+  if (pr.patch) {
+    if (int rc = check_aligned(scratch, "scratch")) return rc;
+    if (int rc = check_space(scratch_bytes, (size_t)pyramid_layout(T, H4, W4).total * 4, "scratch")) return rc;
+    CK(launch_split_pyramid(pyr, T, H4, W4, (__nv_bfloat16*)scratch, pr.corr, (cudaStream_t)stream), "split_pyramid");
+    pyr_split = (const __nv_bfloat16*)scratch;
+  }
+  CK(launch_corr_sample(pyr, pyr_split, H4, W4, support, track_valid, coords, T, N, (__nv_bfloat16*)vol_split,
+                        g_opt_corr, pr.corr, pr.vol16() ? 1 : 0, num_sms(), (cudaStream_t)stream, T, FrameMap{}),
+     "corr_sample");
+  return 0;
+}
+
+int ct3_linear(const void* x_split, const void* w_split, const float* bias, int M, int Nout, int Kpad, int act,
+               float* y, ct3_stream_t stream) {
+  return ct3_linear_prec(x_split, w_split, bias, M, Nout, Kpad, act, 3, 0, y, stream);
+}
+
+int ct3_linear_prec(const void* x_split, const void* w_split, const float* bias, int M, int Nout, int Kpad, int act,
+                    int products, int fp16, float* y, ct3_stream_t stream) {
+  if (!x_split || !w_split || !y) return fail(CT3_EINVAL, "null argument%s");
+  if (M < 1 || Nout < 1 || (Nout % 128) || Kpad < 64 || (Kpad % 64) || act < 0 || act > 2)
+    return fail(CT3_EINVAL, "ct3_linear: need M>=1, Nout %% 128 == 0, Kpad %% 64 == 0, act in 0..2%s");
+  if (products < 1 || products > 3 || fp16 < 0 || fp16 > 1)
+    return fail(CT3_EINVAL, "ct3_linear_prec: products in 1..3, fp16 in 0..1%s");
+  GemmProblem p = linear_problem(x_split, w_split, bias, M, Nout, Kpad, y);
+  p.products = products;
+  p.fp16 = fp16;
+  p.epi.act = act;
+  return run_gemm(p, g_opt_gemm, (cudaStream_t)stream, "ct3_linear");
+}
+
+int ct3_update_loop(const void* packed, const float* pyr, int H4, int W4, const float* support,
+                    const uint8_t* track_valid, float* coords, float* vis, float* conf, const float* time_emb,
+                    int T, int N, int iters, void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+  const int32_t one = N;
+  return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, &one, 1, iters,
+                     workspace, workspace_bytes, (cudaStream_t)stream, T, nullptr);
+}
+
+int ct3_update_loop_groups(const void* packed, const float* pyr, int H4, int W4, const float* support,
+                           const uint8_t* track_valid, float* coords, float* vis, float* conf, const float* time_emb,
+                           int T, int N, int iters, void* workspace, size_t workspace_bytes, ct3_stream_t stream,
+                           const int32_t* group_sizes_host, int G) {
+  return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, group_sizes_host, G,
+                     iters, workspace, workspace_bytes, (cudaStream_t)stream, T, nullptr);
+}
+
+int ct3_update_loop_frames(const void* packed, const float* pyr, int T_pyr, int H4, int W4, const float* support,
+                           const uint8_t* track_valid, float* coords, float* vis, float* conf, const float* time_emb,
+                           int T, int N, int iters, void* workspace, size_t workspace_bytes, ct3_stream_t stream,
+                           const int32_t* group_sizes_host, int G, const int32_t* group_frames_host) {
+  if (!group_frames_host) return fail(CT3_EINVAL, "null group_frames_host%s");
+  return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, group_sizes_host, G,
+                     iters, workspace, workspace_bytes, (cudaStream_t)stream, T_pyr, group_frames_host);
+}
+
+int ct3_updateformer(const void* packed, const float* x, int T, int N, float* delta, void* workspace,
+                     size_t workspace_bytes, ct3_stream_t stream) {
+  const int32_t one = N;
+  return updateformer(packed, x, T, N, &one, 1, delta, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int ct3_updateformer_groups(const void* packed, const float* x, int T, const int32_t* group_sizes_host, int G,
+                            float* delta, void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+  return updateformer(packed, x, T, -1, group_sizes_host, G, delta, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+}  // extern "C"

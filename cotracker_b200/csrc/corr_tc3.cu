@@ -4,7 +4,7 @@
 //   (get_correlation_feat + einsum, cotracker3_online.py:130-143, cotracker3_offline.py:144-156)
 // NB the volume row is SUPPORT-MAJOR here (the reference and the other correlation kernels emit (a*7+b)*49 + k): a
 // thread owns one support vector k, so its 49 values are one contiguous run of the row; corr_mlp.fc1 is multiplied with
-// a copy of its weights whose columns are permuted the same way (api.cu, Layout::corr_fc1_t).
+// a copy of its weights whose columns are permuted the same way (api_loop.cu, Layout::corr_fc1_t).
 //
 // Correlate-then-interpolate like corr_tc2.cu (bilinear sampling is linear in the feature map, so the tensor cores
 // correlate the RAW 8x8 texel patch around the track with the 49 support vectors and the epilogue blends the 64 raw

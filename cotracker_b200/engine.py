@@ -25,11 +25,12 @@ class EngineError(RuntimeError):
     pass
 
 
-def _declare(lib):
+def _signatures():
+    """name -> (restype, argtypes) of every entry point of include/ct3_b200.h"""
     c_int, c_size_t, c_void_p, c_char_p = ctypes.c_int, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_char_p
     i64, i64p = ctypes.c_int64, ctypes.POINTER(ctypes.c_int64)
     intp = ctypes.POINTER(ctypes.c_int)
-    sig = {
+    return {
         "ct3_version": (c_int, []),
         "ct3_last_error": (c_char_p, []),
         "ct3_set_option": (c_int, [c_char_p, c_int]),
@@ -86,27 +87,10 @@ def _declare(lib):
         "ct3_profile_enable": (c_int, [c_int]),
         "ct3_profile_read": (c_int, [ctypes.POINTER(ctypes.c_double), intp, ctypes.POINTER(ctypes.c_double)]),
     }
-    for name, (res, args) in sig.items():
-        fn = getattr(lib, name)  # AttributeError if the symbol is missing -> loud
-        fn.restype = res
-        fn.argtypes = args
-    return sig
 
 
-EXPORTED_SYMBOLS = [
-    "ct3_version", "ct3_last_error", "ct3_set_option", "ct3_get_option", "ct3_precision_info", "ct3_volume_is_support_major", "ct3_num_weight_tensors",
-    "ct3_weight_name", "ct3_packed_weights_bytes", "ct3_pack_weights", "ct3_pyramid_layout",
-    "ct3_prepare_pyramid", "ct3_sample_support", "ct3_workspace_bytes", "ct3_update_loop",
-    "ct3_corr_sample", "ct3_linear", "ct3_linear_prec", "ct3_split_rows", "ct3_split_rows_fp16", "ct3_updateformer", "ct3_profile_enable", "ct3_profile_read",
-    "ct3_encoder_num_weight_tensors", "ct3_encoder_weight_name", "ct3_encoder_packed_bytes", "ct3_encoder_pack",
-    "ct3_encoder_workspace_bytes", "ct3_encoder",
-    "ct3_upsample_concat", "ct3_enc_tail_packed_bytes", "ct3_enc_tail_pack", "ct3_enc_tail_workspace_bytes", "ct3_enc_tail",
-    "ct3_workspace_bytes_groups", "ct3_update_loop_groups", "ct3_updateformer_groups",
-    "ct3_workspace_bytes_frames", "ct3_update_loop_frames",
-    "ct3_prepare_frames",
-    "ct3_render_prepare", "ct3_render_workspace_bytes", "ct3_render_tracks",
-    "ct3_render_flow_workspace_bytes", "ct3_render_flow_colors",
-]
+_SIGNATURES = _signatures()
+EXPORTED_SYMBOLS = list(_SIGNATURES)
 
 
 def lib():
@@ -121,7 +105,10 @@ def lib():
             handle = ctypes.CDLL(LIB_PATH)
         except OSError as e:  # pragma: no cover
             raise EngineError(f"cannot load {LIB_PATH}: {e}") from e
-        _declare(handle)
+        for name, (res, args) in _SIGNATURES.items():
+            fn = getattr(handle, name)  # AttributeError if the symbol is missing -> loud
+            fn.restype = res
+            fn.argtypes = args
         _lib = handle
     return _lib
 
@@ -130,6 +117,19 @@ def _check(rc: int, what: str):
     if rc != 0:
         msg = lib().ct3_last_error().decode("utf-8", "replace")
         raise EngineError(f"{what} failed (code {rc}): {msg}")
+
+
+def _call(name: str, device, *args):
+    """lib().<name>(*args) with `device` current; raises EngineError naming the entry point if it fails."""
+    with torch.cuda.device(device):
+        _check(getattr(lib(), name)(*args), name)
+
+
+def _size(name: str, *args) -> int:
+    """A size query: lib().<name>(*args, &out) -> out."""
+    n = ctypes.c_size_t(0)
+    _check(getattr(lib(), name)(*args, ctypes.byref(n)), name)
+    return n.value
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -186,9 +186,7 @@ def weight_names() -> List[str]:
 
 
 def packed_weights_bytes() -> int:
-    n = ctypes.c_size_t(0)
-    _check(lib().ct3_packed_weights_bytes(ctypes.byref(n)), "ct3_packed_weights_bytes")
-    return n.value
+    return _size("ct3_packed_weights_bytes")
 
 
 def pack_weights(state: dict, device) -> torch.Tensor:
@@ -202,9 +200,8 @@ def pack_weights(state: dict, device) -> torch.Tensor:
     arr = (ctypes.c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
     nbytes = packed_weights_bytes()
     packed = torch.empty(nbytes, dtype=torch.uint8, device=device)
-    with torch.cuda.device(device):
-        _check(lib().ct3_pack_weights(arr, len(tensors), _ptr(packed), nbytes, _stream(device)), "ct3_pack_weights")
-        torch.cuda.current_stream(device).synchronize()  # `tensors` may be temporaries
+    _call("ct3_pack_weights", device, arr, len(tensors), _ptr(packed), nbytes, _stream(device))
+    torch.cuda.current_stream(device).synchronize()  # `tensors` may be temporaries
     return packed
 
 
@@ -225,8 +222,7 @@ def prepare_pyramid(fmaps: torch.Tensor) -> torch.Tensor:
         raise EngineError("fmaps must have 128 channels")
     *_, total = pyramid_layout(T, H4, W4)
     pyr = torch.empty(total, dtype=torch.float32, device=fmaps.device)
-    with torch.cuda.device(fmaps.device):
-        _check(lib().ct3_prepare_pyramid(_ptr(fmaps), T, H4, W4, _ptr(pyr), _stream(fmaps.device)), "ct3_prepare_pyramid")
+    _call("ct3_prepare_pyramid", fmaps.device, _ptr(fmaps), T, H4, W4, _ptr(pyr), _stream(fmaps.device))
     return pyr
 
 
@@ -250,9 +246,8 @@ def prepare_frames(src: torch.Tensor, out_hw, out: Optional[torch.Tensor] = None
     _req(out, torch.float32, "out")
     if tuple(out.shape) != (T, 3, oh, ow) or out.device != src.device:
         raise EngineError(f"out must be [{T},3,{oh},{ow}] on {src.device}")
-    with torch.cuda.device(src.device):
-        _check(lib().ct3_prepare_frames(_ptr(src), FRAME_DTYPES[src.dtype], T, H, W, *src.stride(), oh, ow, _ptr(out),
-                                        _stream(src.device)), "ct3_prepare_frames")
+    _call("ct3_prepare_frames", src.device, _ptr(src), FRAME_DTYPES[src.dtype], T, H, W, *src.stride(), oh, ow, _ptr(out),
+          _stream(src.device))
     return out
 
 
@@ -268,16 +263,13 @@ def render_prepare(src: torch.Tensor, pad: int, grayscale: bool) -> torch.Tensor
     T, _, H, W = src.shape
     p = int(pad)
     out = torch.empty(T, H + 2 * p, W + 2 * p, 3, dtype=torch.uint8, device=src.device)
-    with torch.cuda.device(src.device):
-        _check(lib().ct3_render_prepare(_ptr(src), FRAME_DTYPES[src.dtype], T, H, W, *src.stride(), p, int(bool(grayscale)),
-                                        _ptr(out), _stream(src.device)), "ct3_render_prepare")
+    _call("ct3_render_prepare", src.device, _ptr(src), FRAME_DTYPES[src.dtype], T, H, W, *src.stride(), p,
+          int(bool(grayscale)), _ptr(out), _stream(src.device))
     return out
 
 
 def render_workspace_bytes(T: int, H: int, W: int, N: int, trail: int) -> int:
-    n = ctypes.c_size_t(0)
-    _check(lib().ct3_render_workspace_bytes(T, H, W, N, trail, ctypes.byref(n)), "ct3_render_workspace_bytes")
-    return n.value
+    return _size("ct3_render_workspace_bytes", T, H, W, N, trail)
 
 
 def render_tracks(frames: torch.Tensor, pts: torch.Tensor, colors: torch.Tensor, radius: int, linewidth: int,
@@ -305,18 +297,14 @@ def render_tracks(frames: torch.Tensor, pts: torch.Tensor, colors: torch.Tensor,
     nbytes = render_workspace_bytes(T, H, W, N, trail)
     if workspace is None:
         workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _check(lib().ct3_render_tracks(_ptr(frames), T, H, W, _ptr(pts), _ptr(visible), _ptr(colors), _ptr(draw_mask), N,
-                                       int(radius), int(linewidth), int(trail), int(query_frame), _ptr(alphas),
-                                       _ptr(diff), _ptr(workspace), workspace.numel(), _stream(dev)),
-               "ct3_render_tracks")
+    _call("ct3_render_tracks", dev, _ptr(frames), T, H, W, _ptr(pts), _ptr(visible), _ptr(colors), _ptr(draw_mask), N,
+          int(radius), int(linewidth), int(trail), int(query_frame), _ptr(alphas), _ptr(diff), _ptr(workspace),
+          workspace.numel(), _stream(dev))
     return frames
 
 
 def render_flow_workspace_bytes(T: int, N: int) -> int:
-    n = ctypes.c_size_t(0)
-    _check(lib().ct3_render_flow_workspace_bytes(T, N, ctypes.byref(n)), "ct3_render_flow_workspace_bytes")
-    return n.value
+    return _size("ct3_render_flow_workspace_bytes", T, N)
 
 
 def render_flow_colors(pts: torch.Tensor, query_frame: int) -> torch.Tensor:
@@ -330,9 +318,8 @@ def render_flow_colors(pts: torch.Tensor, query_frame: int) -> torch.Tensor:
     dev = pts.device
     workspace = torch.empty(render_flow_workspace_bytes(T, N), dtype=torch.uint8, device=dev)
     colors = torch.empty(T, N, 3, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _check(lib().ct3_render_flow_colors(_ptr(pts), T, N, int(query_frame), _ptr(colors), _ptr(workspace),
-                                            workspace.numel(), _stream(dev)), "ct3_render_flow_colors")
+    _call("ct3_render_flow_colors", dev, _ptr(pts), T, N, int(query_frame), _ptr(colors), _ptr(workspace),
+          workspace.numel(), _stream(dev))
     return colors
 
 
@@ -352,9 +339,8 @@ def sample_support(pyr, T, H4, W4, qframes, qcoords, support=None, accumulate_ma
     _req(support, torch.float32, "support")
     if accumulate_mask is not None:
         _req(accumulate_mask, torch.uint8, "accumulate_mask")
-    with torch.cuda.device(pyr.device):
-        _check(lib().ct3_sample_support(_ptr(pyr), T, H4, W4, _ptr(qframes), _ptr(qcoords), N, _ptr(accumulate_mask),
-                                        _ptr(support), _stream(pyr.device)), "ct3_sample_support")
+    _call("ct3_sample_support", pyr.device, _ptr(pyr), T, H4, W4, _ptr(qframes), _ptr(qcoords), N, _ptr(accumulate_mask),
+          _ptr(support), _stream(pyr.device))
     return support
 
 
@@ -362,14 +348,9 @@ def workspace_bytes(T: int, N: int, H4: int = 0, W4: int = 0, groups: int = 1, f
     """Scratch of ct3_update_loop for T frames of H4 x W4 feature maps and N tracks (H4 = W4 = 0: updateformer only),
     split into `groups` track groups (ct3_update_loop_groups).  frames: the T_pyr pyramid frames of a call with a
     frame map (ct3_update_loop_frames)."""
-    n = ctypes.c_size_t(0)
     if frames is not None:
-        _check(lib().ct3_workspace_bytes_frames(int(T), int(frames), int(N), int(groups), int(H4), int(W4),
-                                                ctypes.byref(n)), "ct3_workspace_bytes_frames")
-        return n.value
-    _check(lib().ct3_workspace_bytes_groups(int(T), int(N), int(groups), int(H4), int(W4), ctypes.byref(n)),
-           "ct3_workspace_bytes_groups")
-    return n.value
+        return _size("ct3_workspace_bytes_frames", int(T), int(frames), int(N), int(groups), int(H4), int(W4))
+    return _size("ct3_workspace_bytes_groups", int(T), int(N), int(groups), int(H4), int(W4))
 
 
 def pyramid_frames(pyr: torch.Tensor, H4: int, W4: int) -> int:
@@ -434,27 +415,14 @@ def update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, ti
         raise EngineError(f"time_emb must be [{T},{XDIM}]")
     if track_valid is not None:
         _req(track_valid, torch.uint8, "track_valid")
-    if group_frames is not None:
-        arr, G = _group_array(group_sizes if group_sizes is not None else [N])
-        frames = _frame_array(group_frames, G, T)
-        with torch.cuda.device(coords.device):
-            _check(lib().ct3_update_loop_frames(_ptr(packed), _ptr(pyr), pyramid_frames(pyr, H4, W4), H4, W4,
-                                                _ptr(support), _ptr(track_valid), _ptr(coords), _ptr(vis), _ptr(conf),
-                                                _ptr(time_emb), T, N, int(iters), _ptr(workspace), workspace.numel(),
-                                                _stream(coords.device), arr, G, frames), "ct3_update_loop_frames")
-        return
-    if group_sizes is not None:
-        arr, G = _group_array(group_sizes)
-        with torch.cuda.device(coords.device):
-            _check(lib().ct3_update_loop_groups(_ptr(packed), _ptr(pyr), H4, W4, _ptr(support), _ptr(track_valid),
-                                                _ptr(coords), _ptr(vis), _ptr(conf), _ptr(time_emb), T, N, int(iters),
-                                                _ptr(workspace), workspace.numel(), _stream(coords.device), arr, G),
-                   "ct3_update_loop_groups")
-        return
-    with torch.cuda.device(coords.device):
-        _check(lib().ct3_update_loop(_ptr(packed), _ptr(pyr), H4, W4, _ptr(support), _ptr(track_valid), _ptr(coords),
-                                     _ptr(vis), _ptr(conf), _ptr(time_emb), T, N, int(iters), _ptr(workspace),
-                                     workspace.numel(), _stream(coords.device)), "ct3_update_loop")
+    arr, G = _group_array(group_sizes if group_sizes is not None else [N])
+    state = (_ptr(support), _ptr(track_valid), _ptr(coords), _ptr(vis), _ptr(conf), _ptr(time_emb), T, N, int(iters),
+             _ptr(workspace), workspace.numel(), _stream(coords.device), arr, G)
+    if group_frames is None:
+        _call("ct3_update_loop_groups", coords.device, _ptr(packed), _ptr(pyr), H4, W4, *state)
+    else:
+        _call("ct3_update_loop_frames", coords.device, _ptr(packed), _ptr(pyr), pyramid_frames(pyr, H4, W4), H4, W4,
+              *state, _frame_array(group_frames, G, T))
 
 
 # ---- stage-level wrappers (tests, profiles) -----------------------------------------------------------
@@ -466,10 +434,8 @@ def corr_sample(pyr, H4, W4, support, track_valid, coords, scratch: bool = True)
     scr = torch.empty(pyr.numel() * 4, dtype=torch.uint8, device=coords.device) if scratch else None
     # a single fp16 plane [rows, 2432] when the correlate-then-interpolate kernel runs with prec.fc1 < 3
     vb = precision_info(T, H4, W4)[2] if (scratch and get_option("corr") in (0, 3)) else 4
-    with torch.cuda.device(coords.device):
-        _check(lib().ct3_corr_sample(_ptr(pyr), H4, W4, _ptr(support), _ptr(track_valid), _ptr(coords), T, N, _ptr(vol),
-                                     _ptr(scr), scr.numel() if scratch else 0, _stream(coords.device)),
-               "ct3_corr_sample")
+    _call("ct3_corr_sample", coords.device, _ptr(pyr), H4, W4, _ptr(support), _ptr(track_valid), _ptr(coords), T, N,
+          _ptr(vol), _ptr(scr), scr.numel() if scratch else 0, _stream(coords.device))
     if vb == 2:
         full = vol.reshape(-1).view(torch.float16)[:N * T * LEVELS * VOL_PAD].reshape(-1, VOL_PAD).float()
     else:
@@ -488,9 +454,8 @@ def split_rows(x: torch.Tensor, Kpad: int, fp16: bool = False) -> torch.Tensor:
     _req(x, torch.float32, "x")
     rows, K = x.shape
     out = torch.empty(rows, 2 * Kpad, dtype=torch.bfloat16, device=x.device)   # 16-bit planes (bf16 or fp16 bits)
-    fn = lib().ct3_split_rows_fp16 if fp16 else lib().ct3_split_rows
-    with torch.cuda.device(x.device):
-        _check(fn(_ptr(x), rows, K, Kpad, _ptr(out), _stream(x.device)), "ct3_split_rows")
+    _call("ct3_split_rows_fp16" if fp16 else "ct3_split_rows", x.device, _ptr(x), rows, K, Kpad, _ptr(out),
+          _stream(x.device))
     return out
 
 
@@ -503,9 +468,8 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], act: 
     Kpad = (K + 63) // 64 * 64
     xs, ws = split_rows(x.contiguous(), Kpad, fp16), split_rows(w.contiguous(), Kpad, fp16)
     y = torch.empty(M, Nout, dtype=torch.float32, device=x.device)
-    with torch.cuda.device(x.device):
-        _check(lib().ct3_linear_prec(_ptr(xs), _ptr(ws), _ptr(bias), M, Nout, Kpad, act, products, 1 if fp16 else 0,
-                                     _ptr(y), _stream(x.device)), "ct3_linear_prec")
+    _call("ct3_linear_prec", x.device, _ptr(xs), _ptr(ws), _ptr(bias), M, Nout, Kpad, act, products, 1 if fp16 else 0,
+          _ptr(y), _stream(x.device))
     return y
 
 
@@ -524,15 +488,13 @@ def updateformer(packed, x: torch.Tensor, workspace: Optional[torch.Tensor] = No
             raise EngineError(f"group sizes sum to {sum(arr[:G])}, x has {N} tracks")
         if workspace is None:
             workspace = torch.empty(workspace_bytes(T, N, groups=G), dtype=torch.uint8, device=x.device)
-        with torch.cuda.device(x.device):
-            _check(lib().ct3_updateformer_groups(_ptr(packed), _ptr(x), T, arr, G, _ptr(delta), _ptr(workspace),
-                                                 workspace.numel(), _stream(x.device)), "ct3_updateformer_groups")
+        _call("ct3_updateformer_groups", x.device, _ptr(packed), _ptr(x), T, arr, G, _ptr(delta), _ptr(workspace),
+              workspace.numel(), _stream(x.device))
         return delta
     if workspace is None:
         workspace = torch.empty(workspace_bytes(T, N), dtype=torch.uint8, device=x.device)
-    with torch.cuda.device(x.device):
-        _check(lib().ct3_updateformer(_ptr(packed), _ptr(x), T, N, _ptr(delta), _ptr(workspace), workspace.numel(),
-                                      _stream(x.device)), "ct3_updateformer")
+    _call("ct3_updateformer", x.device, _ptr(packed), _ptr(x), T, N, _ptr(delta), _ptr(workspace), workspace.numel(),
+          _stream(x.device))
     return delta
 
 
@@ -554,21 +516,16 @@ def profile_read():
 
 # ---- encoder tail -------------------------------------------------------------------------------------
 def enc_tail_pack(conv2_w, conv2_b, conv3_w, conv3_b, device) -> torch.Tensor:
-    n = ctypes.c_size_t(0)
-    _check(lib().ct3_enc_tail_packed_bytes(ctypes.byref(n)), "ct3_enc_tail_packed_bytes")
+    n = _size("ct3_enc_tail_packed_bytes")
     ts = [x.detach().to(device=device, dtype=torch.float32).contiguous() for x in (conv2_w, conv2_b, conv3_w, conv3_b)]
-    packed = torch.empty(n.value, dtype=torch.uint8, device=device)
-    with torch.cuda.device(device):
-        _check(lib().ct3_enc_tail_pack(_ptr(ts[0]), _ptr(ts[1]), _ptr(ts[2]), _ptr(ts[3]), _ptr(packed), n.value,
-                                       _stream(device)), "ct3_enc_tail_pack")
-        torch.cuda.current_stream(device).synchronize()
+    packed = torch.empty(n, dtype=torch.uint8, device=device)
+    _call("ct3_enc_tail_pack", device, *[_ptr(t) for t in ts], _ptr(packed), n, _stream(device))
+    torch.cuda.current_stream(device).synchronize()
     return packed
 
 
 def enc_tail_workspace_bytes(T: int, H4: int, W4: int) -> int:
-    n = ctypes.c_size_t(0)
-    _check(lib().ct3_enc_tail_workspace_bytes(T, H4, W4, ctypes.byref(n)), "ct3_enc_tail_workspace_bytes")
-    return n.value
+    return _size("ct3_enc_tail_workspace_bytes", T, H4, W4)
 
 
 def enc_tail(packed, cat: torch.Tensor, workspace: torch.Tensor) -> torch.Tensor:
@@ -579,9 +536,8 @@ def enc_tail(packed, cat: torch.Tensor, workspace: torch.Tensor) -> torch.Tensor
         raise EngineError("cat must have 416 channels")
     *_, total = pyramid_layout(T, H4, W4)
     pyr = torch.empty(total, dtype=torch.float32, device=cat.device)
-    with torch.cuda.device(cat.device):
-        _check(lib().ct3_enc_tail(_ptr(packed), _ptr(cat), T, H4, W4, _ptr(pyr), _ptr(workspace), workspace.numel(),
-                                  _stream(cat.device)), "ct3_enc_tail")
+    _call("ct3_enc_tail", cat.device, _ptr(packed), _ptr(cat), T, H4, W4, _ptr(pyr), _ptr(workspace), workspace.numel(),
+          _stream(cat.device))
     return pyr
 
 
@@ -595,20 +551,16 @@ def encoder_pack(state: dict, device) -> torch.Tensor:
     """state: mapping `fnet` state-dict key (without the `fnet.` prefix) -> tensor; returns the packed device buffer."""
     names = encoder_weight_names()
     ts = [state[k].detach().to(device=device, dtype=torch.float32).contiguous() for k in names]
-    n = ctypes.c_size_t(0)
-    _check(lib().ct3_encoder_packed_bytes(ctypes.byref(n)), "ct3_encoder_packed_bytes")
-    packed = torch.empty(n.value, dtype=torch.uint8, device=device)
+    n = _size("ct3_encoder_packed_bytes")
+    packed = torch.empty(n, dtype=torch.uint8, device=device)
     ptrs = (ctypes.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
-    with torch.cuda.device(device):
-        _check(lib().ct3_encoder_pack(ptrs, len(ts), _ptr(packed), n.value, _stream(device)), "ct3_encoder_pack")
-        torch.cuda.current_stream(device).synchronize()   # `ts` may be temporaries
+    _call("ct3_encoder_pack", device, ptrs, len(ts), _ptr(packed), n, _stream(device))
+    torch.cuda.current_stream(device).synchronize()   # `ts` may be temporaries
     return packed
 
 
 def encoder_workspace_bytes(T: int, H: int, W: int) -> int:
-    n = ctypes.c_size_t(0)
-    _check(lib().ct3_encoder_workspace_bytes(T, H, W, ctypes.byref(n)), "ct3_encoder_workspace_bytes")
-    return n.value
+    return _size("ct3_encoder_workspace_bytes", T, H, W)
 
 
 def encoder(packed: torch.Tensor, frames: torch.Tensor, workspace: torch.Tensor) -> torch.Tensor:
@@ -619,9 +571,8 @@ def encoder(packed: torch.Tensor, frames: torch.Tensor, workspace: torch.Tensor)
         raise EngineError("frames must be [T,3,H,W]")
     *_, total = pyramid_layout(T, H // 4, W // 4)
     pyr = torch.empty(total, dtype=torch.float32, device=frames.device)
-    with torch.cuda.device(frames.device):
-        _check(lib().ct3_encoder(_ptr(packed), _ptr(frames), T, H, W, _ptr(pyr), _ptr(workspace), workspace.numel(),
-                                 _stream(frames.device)), "ct3_encoder")
+    _call("ct3_encoder", frames.device, _ptr(packed), _ptr(frames), T, H, W, _ptr(pyr), _ptr(workspace), workspace.numel(),
+          _stream(frames.device))
     return pyr
 
 
@@ -677,6 +628,5 @@ def upsample_concat(feats: Sequence[torch.Tensor], H: int, W: int) -> torch.Tens
     ch = (ctypes.c_int * 4)(*[f.shape[1] for f in fs])
     hh = (ctypes.c_int * 4)(*[f.shape[2] for f in fs])
     ww = (ctypes.c_int * 4)(*[f.shape[3] for f in fs])
-    with torch.cuda.device(out.device):
-        _check(lib().ct3_upsample_concat(src, ch, hh, ww, T, H, W, _ptr(out), _stream(out.device)), "ct3_upsample_concat")
+    _call("ct3_upsample_concat", out.device, src, ch, hh, ww, T, H, W, _ptr(out), _stream(out.device))
     return out
