@@ -641,6 +641,49 @@ int updateformer(const void* packed, const float* x, int T, int N, const int32_t
   return transform_and_heads(R, W, T, N, gp, nullptr, nullptr, nullptr, nullptr, delta);
 }
 
+// ct3_attention: the split-K partials and the group table, the attention parts of carve()
+Workspace carve_attention(void* base, int T, int N, int G) {
+  Workspace w{};
+  Carver c(base);
+  w.att_part = (float*)c.take(attention_partial_bytes(T, kV, partial_slots(N, G)));
+  w.groups = G > 1 ? (int32_t*)c.take((size_t)group_table_ints(N, G) * 4) : nullptr;
+  w.total = c.off;
+  return w;
+}
+
+// One attention of transformer_body on caller buffers of (N + kV*G)*T token rows, dispatched as the body does
+int attention_stage(int kind, const float* q, const float* kv, int T, int N, const int32_t* sizes, int G, void* out,
+                    void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (!q || !kv || !out || !workspace) return fail(CT3_EINVAL, "null argument%s");
+  if (kind < CT3_ATTN_TIME || kind > CT3_ATTN_POINT_FROM_VIRTUAL) return fail(CT3_EINVAL, "unknown attention kind%s");
+  int total = 0;
+  if (int rc = check_groups(T, N, sizes, G, &total, false)) return rc;
+  if (((uintptr_t)q | (uintptr_t)kv | (uintptr_t)out) & 15) return fail(CT3_EINVAL, "q, kv and out must be 16-byte aligned%s");
+  if (int rc = check_aligned(workspace, "workspace")) return rc;
+  const Workspace W = carve_attention(workspace, T, N, G);
+  if (int rc = check_space(workspace_bytes, W.total, "workspace")) return rc;
+  Runner R{nullptr, layout(), stream, g_opt_gemm};
+  const int64_t Rp = (int64_t)N * T;
+  __nv_bfloat16* att = reinterpret_cast<__nv_bfloat16*>(out);
+  if (kind == CT3_ATTN_TIME) {   // the unfused path of the time block: every track, points and virtual
+    RUNC(CAT_ATTN, run_attention(R, W, attn_params(q, 3 * kC, kv, 3 * kC, kC, 2 * kC, att, T, T, T, N + kV * G), true));
+    return 0;
+  }
+  GroupPlan gp;
+  if (int rc = plan_groups(gp, sizes, G, T, N, W.groups, R.s)) return rc;
+  __nv_bfloat16* att_v = att + Rp * 2 * kC;
+  if (kind == CT3_ATTN_VIRTUAL_FROM_POINT)
+    RUNC(CAT_ATTN, space_attention(R, W, gp, attn_params(q + Rp * kC, kC, kv, 2 * kC, 0, kC, att_v, kV, N, T), false,
+                                   true));
+  else if (kind == CT3_ATTN_VIRTUAL_SELF)
+    RUNC(CAT_ATTN, space_attention(R, W, gp, attn_params(q + Rp * 3 * kC, 3 * kC, kv + Rp * 3 * kC, 3 * kC, kC, 2 * kC,
+                                                         att_v, kV, kV, T), false, false));
+  else
+    RUNC(CAT_ATTN, space_attention(R, W, gp, attn_params(q, kC, kv + Rp * 2 * kC, 2 * kC, 0, kC, att, N, kV, T), true,
+                                   false));
+  return 0;
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -839,6 +882,19 @@ int ct3_updateformer(const void* packed, const float* x, int T, int N, float* de
 int ct3_updateformer_groups(const void* packed, const float* x, int T, const int32_t* group_sizes_host, int G,
                             float* delta, void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
   return updateformer(packed, x, T, -1, group_sizes_host, G, delta, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int ct3_attention_workspace_bytes(int T, int N, int G, size_t* out_bytes) {
+  if (!out_bytes) return fail(CT3_EINVAL, "null out_bytes%s");
+  if (int rc = check_TN(T, N, G)) return rc;
+  *out_bytes = carve_attention(nullptr, T, N, G).total;
+  return 0;
+}
+
+int ct3_attention(int kind, const float* q, const float* kv, int T, int N, const int32_t* group_sizes_host, int G,
+                  void* out_split, void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+  return attention_stage(kind, q, kv, T, N, group_sizes_host, G, out_split, workspace, workspace_bytes,
+                         (cudaStream_t)stream);
 }
 
 }  // extern "C"

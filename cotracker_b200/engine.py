@@ -69,6 +69,9 @@ def _signatures():
                                            ctypes.POINTER(ctypes.c_int32), c_int]),
         "ct3_updateformer_groups": (c_int, [c_void_p, c_void_p, c_int, ctypes.POINTER(ctypes.c_int32), c_int, c_void_p,
                                             c_void_p, c_size_t, c_void_p]),
+        "ct3_attention_workspace_bytes": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+        "ct3_attention": (c_int, [c_int, c_void_p, c_void_p, c_int, c_int, ctypes.POINTER(ctypes.c_int32), c_int, c_void_p,
+                                  c_void_p, c_size_t, c_void_p]),
         "ct3_workspace_bytes_frames": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
         "ct3_update_loop_frames": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p,
@@ -496,6 +499,35 @@ def updateformer(packed, x: torch.Tensor, workspace: Optional[torch.Tensor] = No
     _call("ct3_updateformer", x.device, _ptr(packed), _ptr(x), T, N, _ptr(delta), _ptr(workspace), workspace.numel(),
           _stream(x.device))
     return delta
+
+
+# ct3_attention kinds (CT3_ATTN_*) and the column widths of their q and kv rows
+ATTENTION_KINDS = {"time": 0, "virtual_from_point": 1, "virtual_self": 2, "point_from_virtual": 3}
+_ATTENTION_WIDTHS = {0: (3 * HID, 3 * HID), 1: (HID, 2 * HID), 2: (3 * HID, 3 * HID), 3: (HID, 2 * HID)}
+
+
+def attention(kind, q: torch.Tensor, kv: torch.Tensor, T: int, N: int,
+              group_sizes: Optional[Sequence[int]] = None) -> torch.Tensor:
+    """One attention core of the transformer body (ct3_attention in include/ct3_b200.h), dispatched as the body does
+    under this thread's "attn" option.  kind: a name of ATTENTION_KINDS or its number.  q, kv: fp32 token rows
+    [(N + 64 G) * T, width] (time / virtual_self: q|k|v rows of 1152, possibly the same tensor; the cross kinds: q rows
+    of 384 and k|v rows of 768).  -> fp32 [(N + 64 G) * T, 384] = hi + lo of the split output; rows the kind does not
+    write are 0."""
+    k = ATTENTION_KINDS[kind] if isinstance(kind, str) else int(kind)
+    _req(q, torch.float32, "q")
+    _req(kv, torch.float32, "kv")
+    arr, G = _group_array(group_sizes if group_sizes is not None else [N])
+    rows = (int(N) + VIRT * G) * int(T)
+    wq, wkv = _ATTENTION_WIDTHS.get(k, (q.shape[-1], kv.shape[-1]))
+    if tuple(q.shape) != (rows, wq) or tuple(kv.shape) != (rows, wkv) or kv.device != q.device:
+        raise EngineError(f"attention kind {kind}: q must be [{rows},{wq}] and kv [{rows},{wkv}] on one device, "
+                          f"got {tuple(q.shape)} and {tuple(kv.shape)}")
+    dev = q.device
+    out = torch.zeros(rows, 2 * HID, dtype=torch.bfloat16, device=dev)
+    workspace = torch.empty(_size("ct3_attention_workspace_bytes", int(T), int(N), G), dtype=torch.uint8, device=dev)
+    _call("ct3_attention", dev, k, _ptr(q), _ptr(kv), int(T), int(N), arr, G, _ptr(out), _ptr(workspace),
+          workspace.numel(), _stream(dev))
+    return out[:, :HID].float() + out[:, HID:].float()
 
 
 PROFILE_CATEGORIES = ["corr_sample", "gemm", "attention", "layernorm", "misc", "encoder", "qkv_time_attention"]

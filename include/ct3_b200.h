@@ -301,6 +301,30 @@ int ct3_updateformer(const void* packed, const float* x, int T, int N, float* de
 int ct3_updateformer_groups(const void* packed, const float* x, int T, const int32_t* group_sizes_host, int G,
                             float* delta, void* workspace, size_t workspace_bytes, ct3_stream_t stream);
 
+/* One attention core  out = softmax(q k^T * 48^-1/2) v  per head (8 x 48; Attention.forward, blocks.py:391-397) of
+ * the transformer body, chosen and launched exactly as ct3_updateformer_groups does it under the calling thread's
+ * "attn" option (time attention always takes the unfused path that T > 128 takes in the body).
+ * Every buffer holds the body's (N + 64*G)*T token rows: point n at row n*T + t, virtual token i of group g at row
+ * (N + 64*g + i)*T + t.
+ *   kind CT3_ATTN_TIME                : per track (all N + 64*G of them) over its T frames; q = kv = fused q|k|v rows
+ *                                       [rows, 1152] (q cols 0.., k 384.., v 768..)
+ *        CT3_ATTN_VIRTUAL_FROM_POINT  : per (group, frame), the group's 64 virtual queries over its points;
+ *                                       q [rows, 384], kv = k|v [rows, 768]
+ *        CT3_ATTN_VIRTUAL_SELF        : per (group, frame), 64 virtual tokens over themselves; q, kv [rows, 1152]
+ *        CT3_ATTN_POINT_FROM_VIRTUAL  : per (group, frame), the group's points over its 64 virtual tokens;
+ *                                       q [rows, 384], kv [rows, 768]
+ *   q, kv          : fp32 device buffers (may alias), 16-byte aligned; only the rows the kind reads are read
+ *   out_split      : bf16 [rows, 768] (hi cols 0..383 | lo cols 384..767); the query rows of the kind are written,
+ *                    no other row
+ *   group_sizes_host, G : as ct3_updateformer_groups (sum = N)
+ *   workspace      : ct3_attention_workspace_bytes(T, N, G) bytes, 256-byte aligned (split-K partials, group table)
+ * Null pointers, an unknown kind, bad T/N/groups, misalignment return CT3_EINVAL and a too small workspace
+ * CT3_ENOSPC, before any launch; "fuse" = 2 or "attn" = 2 with G > 1 return CT3_EUNSUPPORTED. */
+enum { CT3_ATTN_TIME = 0, CT3_ATTN_VIRTUAL_FROM_POINT = 1, CT3_ATTN_VIRTUAL_SELF = 2, CT3_ATTN_POINT_FROM_VIRTUAL = 3 };
+int ct3_attention_workspace_bytes(int T, int N, int G, size_t* out_bytes);
+int ct3_attention(int kind, const float* q, const float* kv, int T, int N, const int32_t* group_sizes_host, int G,
+                  void* out_split, void* workspace, size_t workspace_bytes, ct3_stream_t stream);
+
 /* ---- the whole CNN encoder (BasicEncoder.forward, blocks.py:190-219; normalise + pyramid,
  * cotracker3_offline.py:92-117) on the tensor-core engine, channels-last ------------------------------------
  * frames [T,3,H,W] fp32 already scaled to [-1,1] (cotracker3_offline.py:63) -> pyr (ct3_pyramid_layout(T, H/4, W/4)).

@@ -52,6 +52,43 @@ def test_abi_argument_validation_without_gpu():
     assert lib.ct3_corr_sample(one, 96, 128, one, None, one, 2, 5, one, ctypes.c_void_p(512), 1024, None) == -3   # CT3_ENOSPC
 
 
+def test_attention_stage_argument_validation_without_gpu():
+    """ct3_attention / ct3_attention_workspace_bytes reject bad arguments with CT3_EINVAL / CT3_ENOSPC before any
+    launch (the pointers below are never dereferenced)."""
+    from cotracker_b200 import engine
+    lib = engine.lib()
+    n, m = ctypes.c_size_t(0), ctypes.c_size_t(0)
+    assert lib.ct3_attention_workspace_bytes(16, 6400, 1, ctypes.byref(n)) == 0 and n.value > 0
+    assert lib.ct3_attention_workspace_bytes(16, 6400, 8, ctypes.byref(m)) == 0 and m.value > n.value   # + group table
+    assert lib.ct3_attention_workspace_bytes(16, 6400, 1, None) == -1
+    assert lib.ct3_attention_workspace_bytes(0, 10, 1, ctypes.byref(n)) == -1
+    assert lib.ct3_attention_workspace_bytes(4, 10, 11, ctypes.byref(n)) == -1          # G > N
+    assert lib.ct3_attention_workspace_bytes(4, 10, 0, ctypes.byref(n)) == -1
+    assert lib.ct3_attention_workspace_bytes(4, 10, 1, ctypes.byref(n)) == 0
+    need = n.value
+    p, ws = ctypes.c_void_p(1 << 20), ctypes.c_void_p(1 << 21)
+    one = (ctypes.c_int32 * 1)(10)
+
+    def call(kind=1, q=p, kv=p, T=4, N=10, sizes=one, G=1, out=p, w=ws, nbytes=need):
+        return lib.ct3_attention(kind, q, kv, T, N, sizes, G, out, w, nbytes, None)
+
+    assert call(q=None) == -1 and call(kv=None) == -1 and call(out=None) == -1 and call(w=None) == -1
+    assert call(kind=-1) == -1 and call(kind=4) == -1 and b"kind" in lib.ct3_last_error()
+    assert call(T=0) == -1 and call(N=0) == -1
+    assert call(sizes=None) == -1 and call(G=0) == -1
+    assert call(sizes=(ctypes.c_int32 * 2)(4, 5), G=2) == -1 and b"sum to N" in lib.ct3_last_error()
+    assert call(sizes=(ctypes.c_int32 * 2)(10, 0), G=2, N=10) == -1
+    assert call(q=ctypes.c_void_p((1 << 20) + 4)) == -1 and b"16-byte" in lib.ct3_last_error()
+    assert call(out=ctypes.c_void_p((1 << 20) + 8)) == -1
+    assert call(w=ctypes.c_void_p((1 << 21) + 16)) == -1 and b"256-byte" in lib.ct3_last_error()
+    assert call(nbytes=need - 1) == -3                                                   # CT3_ENOSPC
+    assert lib.ct3_set_option(b"attn", 2) == 0
+    try:   # attn = 2 has no grouped point<-virtual path, as for the grouped update loop
+        assert call(kind=3, N=10, sizes=(ctypes.c_int32 * 2)(5, 5), G=2, nbytes=1 << 40) == -4
+    finally:
+        assert lib.ct3_set_option(b"attn", 0) == 0
+
+
 def test_weight_names_match_state_dict():
     from cotracker_b200 import engine
     from cotracker_b200.build import build_cotracker
