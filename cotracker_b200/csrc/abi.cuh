@@ -44,7 +44,6 @@ inline int pad64(int k) { return (k + 63) / 64 * 64; }
 // ---- packed weights: a linear layer at byte offsets of the caller's packed buffer
 struct Lin {
   size_t w = 0, b = 0;  // byte offsets: split weights [N, 2*Kpad] bf16 ; bias [N] fp32
-  size_t ws = 0;        // fp32 [N]: sum_k W[n][k], the correction vector of a LayerNorm folded into this layer
   int N = 0, K = 0, Kpad = 0;
 };
 inline void place_lin(Lin& l, int N, int K, size_t& off) {
@@ -54,8 +53,6 @@ inline void place_lin(Lin& l, int N, int K, size_t& off) {
   l.w = off;
   off = align_up(off + (size_t)N * 2 * l.Kpad * sizeof(__nv_bfloat16));
   l.b = off;
-  off = align_up(off + (size_t)N * sizeof(float));
-  l.ws = off;
   off = align_up(off + (size_t)N * sizeof(float));
 }
 

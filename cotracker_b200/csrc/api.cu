@@ -27,11 +27,11 @@ constexpr OptDef kOptDefs[OPT_COUNT] = {
     // switch: SURVEY 7.3 measured that every transformer GEMM breaks the 1e-3 px budget with fewer than 3 products.
     {"prec.corr", 1, 3},   // the 49x128x49 correlation contraction (corr_tc2.cu)
     {"prec.fc1", 1, 3},    // corr_mlp.fc1 (K = 2401): 1|2 also make the correlation volume a single fp16 plane
-    // 0: separate LayerNorm / projection / attention kernels; 1: q|k|v projection + time attention in one kernel
-    // (gemm_qkv_time_attn_kernel); 2: additionally every LayerNorm folded into the GEMMs around it (no LN kernels)
-    {"fuse", 0, 2},
+    // time blocks: 0 = separate q|k|v projection and attention kernels (what T > 128 always runs; the tests'
+    // cross-check), 1 = both in one kernel (gemm_qkv_time_attn_kernel)
+    {"fuse", 0, 1},
 };
-thread_local int g_opt[OPT_COUNT] = {0, 0, 0, kDefPrecCorr, kDefPrecFc1, 1};   // fuse = 2 measured slower (DESIGN.md 4.6)
+thread_local int g_opt[OPT_COUNT] = {0, 0, 0, kDefPrecCorr, kDefPrecFc1, 1};
 
 int fail(int code, const char* fmt, const char* detail) {
   snprintf(g_err, sizeof(g_err), fmt, detail);

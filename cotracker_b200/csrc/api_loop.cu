@@ -17,7 +17,6 @@ struct Block {
   Lin qkv_h;  // time blocks only: q|k|v regrouped per head, rows h*144 + [q_h(48) | k_h(48) | v_h(48)] (fused attention)
   Lin q;    // self-attention blocks: fused q|k|v (N = 1152); cross blocks: to_q (N = 384)
   Lin kv;   // cross blocks only: to_kv (N = 768)
-  Lin kv_f; // cross blocks only: to_kv with the affine norm_context folded in (W diag(gamma), b + W beta)
   Lin out, fc1, fc2;
   size_t ctx_g = 0, ctx_b = 0;  // cross blocks: norm_context weight / bias (fp32 [384])
   bool cross = false;
@@ -28,7 +27,6 @@ struct Layout {
   Lin corr_fc1_t, corr_fc1_th;   // the same two with the columns in corr_tc3.cu's support-major volume order
   Block time[kDepth], vself[kDepth], p2v[kDepth], v2p[kDepth];
   size_t heads_w = 0, heads_b = 0, virt = 0, win_f32 = 0;
-  size_t scratch = 0;   // pack-time scratch: one folded to_kv weight [768, 384] + bias [768] in fp32
   size_t total = 0;
 };
 
@@ -40,7 +38,6 @@ void place_block(Block& b, bool cross, size_t& off, bool time = false) {
     b.ctx_b = off; off = align_up(off + kC * sizeof(float));
     place_lin(b.q, kC, kC, off);
     place_lin(b.kv, 2 * kC, kC, off);
-    place_lin(b.kv_f, 2 * kC, kC, off);
   } else {
     place_lin(b.q, 3 * kC, kC, off);
   }
@@ -68,8 +65,6 @@ const Layout& layout() {
       place_block(L.p2v[i], true, off);
       place_block(L.v2p[i], true, off);
     }
-    L.scratch = off;
-    off = align_up(off + (size_t)2 * kC * kC * sizeof(float) + (size_t)2 * kC * sizeof(float));
     L.total = off;
     return L;
   }();
@@ -112,8 +107,6 @@ struct Workspace {
   __nv_bfloat16* h1;      // [N*T*4, 2*384]
   __nv_bfloat16* xs;      // [N*T, 2*1152]
   float* tokens;          // [(N+64)*T, 384]
-  __nv_bfloat16* traw;    // [(N+64)*T, 2*384]  the token rows once more as a split operand (LayerNorm fold)
-  float* tstat;           // [(N+64)*T, 24, 2]  partial (sum, sum of squares) of every token row
   __nv_bfloat16* ln;      // [(N+64)*T, 2*384]
   __nv_bfloat16* att;     // [(N+64)*T, 2*384]
   float* qkv;             // [(N+64)*T, 1152]   (also point q [N*T,384] / point kv [N*T,768])
@@ -146,8 +139,6 @@ Workspace carve(void* base, int T, int N, int H4 = 0, int W4 = 0, int G = 1, int
   w.h1 = (__nv_bfloat16*)c.take(Mc * 2 * kCorrHid * 2);
   w.xs = (__nv_bfloat16*)c.take(Rp * 2 * kXPad * 2);
   w.tokens = (float*)c.take(R * kC * 4);
-  w.traw = (__nv_bfloat16*)c.take(R * 2 * kC * 2);
-  w.tstat = (float*)c.take(R * kLnParts * 2 * 4);
   w.ln = (__nv_bfloat16*)c.take(R * 2 * kC * 2);
   w.att = (__nv_bfloat16*)c.take(R * 2 * kC * 2);
   w.qkv = (float*)c.take(R * 3 * kC * 4);
@@ -324,16 +315,12 @@ int space_attention(Runner& R, const Workspace& W, const GroupPlan& gp, AttnPara
 }
 
 // q|k|v projection and the per-track T x T attention of time block b in ONE kernel: fp32 q|k|v never reaches HBM.
-// ln_part: x holds the raw token rows and the LayerNorm is applied in the epilogue (transformer_body_fold).
-int qkv_time_attention(Runner& R, const Workspace& W, const Block& b, const __nv_bfloat16* x, const float* ln_part,
-                       int rows, int T) {
+int qkv_time_attention(Runner& R, const Workspace& W, const Block& b, const __nv_bfloat16* x, int rows, int T) {
   ProfScope ps(R.s, CAT_QKVA, 0.0);
   const char* gerr = nullptr;
   const int rc = gemm_qkv_time_attn_launch(
       x, reinterpret_cast<const __nv_bfloat16*>(R.pk + b.qkv_h.w), reinterpret_cast<const float*>(R.pk + b.qkv_h.b),
-      rows, kC, T, W.att, 2 * kC, kC, 1.0f / sqrtf((float)kDh), ln_part,
-      ln_part ? reinterpret_cast<const float*>(R.pk + b.qkv_h.ws) : nullptr, ln_part ? 1e-6f : 0.f, num_sms(), R.s,
-      &gerr);
+      rows, kC, T, W.att, 2 * kC, kC, 1.0f / sqrtf((float)kDh), num_sms(), R.s, &gerr);
   return rc ? fail_launch(rc, "fused qkv + time attention", gerr) : 0;
 }
 
@@ -364,8 +351,8 @@ int transformer_body(Runner& R, const Workspace& W, int T, int N, const GroupPla
     {  // ---- time block over every token row (points + virtual): sequence = track (cotracker.py:494-495)
       const Block& b = L.time[i];
       RUNC(CAT_LN, launch_layernorm_split(W.tokens, Rall, nullptr, nullptr, 1e-6f, W.ln, R.s));
-      if (g_opt[OPT_FUSE] >= 1 && R.impl == 0 && g_opt_attn != 1 && qkv_time_attn_supported(T)) {
-        if (int rc = qkv_time_attention(R, W, b, W.ln, nullptr, Rall, T)) return rc;
+      if (g_opt[OPT_FUSE] == 1 && R.impl == 0 && g_opt_attn != 1 && qkv_time_attn_supported(T)) {
+        if (int rc = qkv_time_attention(R, W, b, W.ln, Rall, T)) return rc;
       } else {
         GEMM(W.ln, b.q, Rall, Runner::to_f32(W.qkv, 3 * kC, false));
         RUNC(CAT_ATTN, run_attention(R, W, attn_params(W.qkv, 3 * kC, W.qkv, 3 * kC, kC, 2 * kC, W.att, T, T, T,
@@ -426,90 +413,16 @@ Prec effective_prec(bool have_pyr_split, int T, int H4, int W4) {
   return p;
 }
 
-// LayerNorm-folded variant of transformer_body (option fuse = 2, tensor-core kernels, T <= 128): no LayerNorm kernel
-// runs.  Every GEMM that writes token rows (input_transform, to_out, mlp.fc2) also emits them as a split-bf16 operand
-// plus partial row statistics (GemmEpilogue::raw_split / stat_part); every GEMM that consumes LN(x) multiplies the
-// RAW rows and applies  rstd * (W.x - mean * wsum) + b  in its epilogue; the affine norm_context of the cross blocks
-// (cotracker.py:539-540) is folded into to_kv's weights and bias at pack time (Block::kv_f).
-bool fold_enabled(const Runner& R, int T) {
-  return g_opt[OPT_FUSE] == 2 && R.impl == 0 && g_opt_attn != 1 && qkv_time_attn_supported(T);
-}
-
-int transformer_body_fold(Runner& R, const Workspace& W, int T, int N) {
-  const Layout& L = R.L;
-  const int Rp = N * T, Rv = kV * T, Rall = Rp + Rv;
-  const uint8_t* pk = R.pk;
-  RUNC(CAT_MISC, launch_init_virtual(W.tokens, reinterpret_cast<const float*>(pk + L.virt), T, N, 1, R.s));
-  float* vtok = W.tokens + (int64_t)Rp * kC;
-  __nv_bfloat16* raw_p = W.traw;
-  __nv_bfloat16* raw_v = W.traw + (int64_t)Rp * 2 * kC;
-  float* st_p = W.tstat;
-  float* st_v = W.tstat + (int64_t)Rp * kLnParts * 2;
-  __nv_bfloat16* att_p = W.att;
-  __nv_bfloat16* att_v = W.att + (int64_t)Rp * 2 * kC;
-  RUNC(CAT_LN, launch_rowstats_split(vtok, Rv, raw_v, st_v, R.s));
-  auto ln = [&](GemmEpilogue e, const float* part, const Lin& lin, float eps) {
-    e.ln_part = part; e.ln_wsum = reinterpret_cast<const float*>(pk + lin.ws); e.ln_eps = eps;
-    return e;
-  };
-  auto prod = [&](GemmEpilogue e, __nv_bfloat16* raw, float* stat) { e.raw_split = raw; e.stat_part = stat; return e; };
-  // x += mlp(LN(x)) on rows [row0, row0 + rows)
-  auto mlp = [&](const Block& b, int64_t row0, int rows) -> int {
-    float* x = W.tokens + row0 * kC;
-    __nv_bfloat16* raw = W.traw + row0 * 2 * kC;
-    float* st = W.tstat + row0 * kLnParts * 2;
-    __nv_bfloat16* hm = W.hmid + row0 * 2 * kMlpHid;
-    GEMM(raw, b.fc1, rows, ln(Runner::to_split(hm, 2 * kMlpHid, kMlpHid, /*tanh*/ 2), st, b.fc1, 1e-6f));
-    GEMM(hm, b.fc2, rows, prod(Runner::to_f32(x, kC, true), raw, st));
-    return 0;
-  };
-  for (int i = 0; i < kDepth; ++i) {
-    {  // ---- time block (cotracker.py:494-495)
-      const Block& b = L.time[i];
-      if (int rc = qkv_time_attention(R, W, b, W.traw, W.tstat, Rall, T)) return rc;
-      GEMM(W.att, b.out, Rall, prod(Runner::to_f32(W.tokens, kC, true), W.traw, W.tstat));
-      if (int rc = mlp(b, 0, Rall)) return rc;
-    }
-    {  // ---- virtual <- point cross attention (cotracker.py:510-512)
-      const Block& b = L.v2p[i];
-      GEMM(raw_v, b.q, Rv, ln(Runner::to_f32(W.vqkv, kC, false), st_v, b.q, 1e-6f));
-      GEMM(raw_p, b.kv_f, Rp, ln(Runner::to_f32(W.qkv, 2 * kC, false), st_p, b.kv_f, 1e-5f));
-      RUNC(CAT_ATTN, run_attention(R, W, attn_params(W.vqkv, kC, W.qkv, 2 * kC, 0, kC, att_v, kV, N, T), false));
-      GEMM(att_v, b.out, Rv, prod(Runner::to_f32(vtok, kC, true), raw_v, st_v));
-      if (int rc = mlp(b, Rp, Rv)) return rc;
-    }
-    {  // ---- virtual self attention (cotracker.py:514)
-      const Block& b = L.vself[i];
-      GEMM(raw_v, b.q, Rv, ln(Runner::to_f32(W.vqkv, 3 * kC, false), st_v, b.q, 1e-6f));
-      RUNC(CAT_ATTN, run_attention(R, W, attn_params(W.vqkv, 3 * kC, W.vqkv, 3 * kC, kC, 2 * kC, att_v, kV, kV, T),
-                                   false));
-      GEMM(att_v, b.out, Rv, prod(Runner::to_f32(vtok, kC, true), raw_v, st_v));
-      if (int rc = mlp(b, Rp, Rv)) return rc;
-    }
-    {  // ---- point <- virtual cross attention (cotracker.py:515-517)
-      const Block& b = L.p2v[i];
-      GEMM(raw_p, b.q, Rp, ln(Runner::to_f32(W.qkv, kC, false), st_p, b.q, 1e-6f));
-      GEMM(raw_v, b.kv_f, Rv, ln(Runner::to_f32(W.vqkv, 2 * kC, false), st_v, b.kv_f, 1e-5f));
-      RUNC(CAT_ATTN, run_attention(R, W, attn_params(W.qkv, kC, W.vqkv, 2 * kC, 0, kC, att_p, N, kV, T), false));
-      GEMM(att_p, b.out, Rp, prod(Runner::to_f32(W.tokens, kC, true), raw_p, st_p));
-      if (int rc = mlp(b, 0, Rp)) return rc;
-    }
-  }
-  return 0;
-}
-
 // The steps update_loop and updateformer share: input_transform of the X rows in W.xs into the point tokens (with the
 // per-frame bias row_bias [T, kC] when given), the transformer body, then the heads: the state update of coords / vis /
 // conf, or with delta != nullptr the raw deltas [N,T,4] instead.
 int transform_and_heads(Runner& R, const Workspace& W, int T, int N, const GroupPlan& gp, const float* row_bias,
                         float* coords, float* vis, float* conf, float* delta) {
   const Layout& L = R.L;
-  const bool fold = fold_enabled(R, T);
   GemmEpilogue e = Runner::to_f32(W.tokens, kC, false);
   if (row_bias) { e.row_bias = row_bias; e.row_mod = T; }
-  if (fold) { e.raw_split = W.traw; e.stat_part = W.tstat; }
   GEMM(W.xs, L.in_tr, N * T, e);
-  if (int rc = fold ? transformer_body_fold(R, W, T, N) : transformer_body(R, W, T, N, gp)) return rc;
+  if (int rc = transformer_body(R, W, T, N, gp)) return rc;
   RUNC(CAT_MISC, launch_heads(W.tokens, reinterpret_cast<const float*>(R.pk + L.heads_w),
                               reinterpret_cast<const float*>(R.pk + L.heads_b), coords, vis, conf, delta, T, N, R.s));
   return 0;
@@ -536,8 +449,7 @@ int check_groups(int T, int N, const int32_t* sizes, int G, int* total, bool n_f
   }
   if (sum > (int64_t)1 << 30) return fail(CT3_EINVAL, "problem too large%s");
   if (!n_from_sizes && sum != N) return fail(CT3_EINVAL, "group sizes must sum to N%s");
-  if (G > 1 && (g_opt[OPT_FUSE] == 2 || g_opt_attn == 2))
-    return fail(CT3_EUNSUPPORTED, "grouped calls do not support fuse = 2 or attn = 2%s");
+  if (G > 1 && g_opt_attn == 2) return fail(CT3_EUNSUPPORTED, "grouped calls do not support attn = 2%s");
   *total = (int)sum;
   return check_TN(T, *total, G);
 }
@@ -732,8 +644,6 @@ int ct3_pack_weights(const float* const* t, int n_tensors, void* packed, size_t 
                      int fp16 = 0) -> cudaError_t {
     cudaError_t e = launch_split_rows(w, rows, l.K, l.Kpad, perm, reinterpret_cast<__nv_bfloat16*>(pk + l.w), row_off, s, fp16);
     if (e != cudaSuccess) return e;
-    e = launch_rowsum(w, rows, l.K, reinterpret_cast<float*>(pk + l.ws) + row_off, s);
-    if (e != cudaSuccess) return e;
     return cudaMemcpyAsync(pk + l.b + (size_t)row_off * 4, b, (size_t)rows * 4, cudaMemcpyDeviceToDevice, s);
   };
   auto put_f32 = [&](size_t off, const float* src, size_t count) {
@@ -776,12 +686,6 @@ int ct3_pack_weights(const float* const* t, int n_tensors, void* packed, size_t 
     if ((e = put_f32(b.ctx_b, t[k + 1], kC)) != cudaSuccess) return e;
     if ((e = put_lin(b.q, t[k + 2], t[k + 3], kC, 0, 0)) != cudaSuccess) return e;
     if ((e = put_lin(b.kv, t[k + 4], t[k + 5], 2 * kC, 0, 0)) != cudaSuccess) return e;
-    {   // to_kv(norm_context(x)) with the affine part folded into the layer (stream-ordered reuse of the scratch)
-      float* w2 = reinterpret_cast<float*>(pk + L.scratch);
-      float* b2 = w2 + (size_t)2 * kC * kC;
-      if ((e = launch_affine_fold(t[k + 4], t[k + 5], t[k], t[k + 1], 2 * kC, kC, w2, b2, s)) != cudaSuccess) return e;
-      if ((e = put_lin(b.kv_f, w2, b2, 2 * kC, 0, 0)) != cudaSuccess) return e;
-    }
     if ((e = put_lin(b.out, t[k + 6], t[k + 7], kC, 0, 0)) != cudaSuccess) return e;
     if ((e = put_lin(b.fc1, t[k + 8], t[k + 9], kMlpHid, 0, 0)) != cudaSuccess) return e;
     if ((e = put_lin(b.fc2, t[k + 10], t[k + 11], kC, 0, 0)) != cudaSuccess) return e;

@@ -33,8 +33,6 @@ constexpr int MAX_STAGES = 4;
 //   3: A hi|lo, W hi|lo (64 KiB x 2)   2: A hi, W hi|lo (48 KiB x 2)   1: A hi, W hi (32 KiB x 4)
 template <int NPROD>
 struct Cfg {
-  // NPROD == 4 / 5: 3 products + the LayerNorm-producer epilogue (raw split rows + partial statistics) / the
-  // LayerNorm-consumer epilogue -- separate instantiations so that the default kernels do not carry their registers
   static constexpr int AP = NPROD >= 3 ? 2 : 1;
   static constexpr int BP = NPROD >= 2 ? 2 : 1;
   static constexpr int STAGE_BYTES = AP * TILE_A + BP * TILE_B;
@@ -69,19 +67,9 @@ __device__ __forceinline__ float apply_act(float x, int act) {
 // of global memory in whole 32-byte sectors.
 __device__ __forceinline__ int stg_idx(int row, int word) { return row * CW + ((word + (row >> 1)) & (CW - 1)); }
 
-template <bool PROD, bool CONS>
 __device__ __forceinline__ void epilogue_chunk(const GemmEpilogue& e, int M, int N, int row0, int col0, int lane,
-                                               float (&v)[CW], uint32_t* stg, float ln_mean = 0.f, float ln_rstd = 1.f) {
+                                               float (&v)[CW], uint32_t* stg) {
   const int row = row0 + lane;
-  if constexpr (CONS) {   // LayerNorm of the A rows applied after the contraction (see GemmEpilogue)
-    const float4* w4 = reinterpret_cast<const float4*>(e.ln_wsum + col0);
-#pragma unroll
-    for (int i = 0; i < CW / 4; ++i) {
-      const float4 ws = __ldg(w4 + i);
-      v[4 * i + 0] = ln_rstd * (v[4 * i + 0] - ln_mean * ws.x); v[4 * i + 1] = ln_rstd * (v[4 * i + 1] - ln_mean * ws.y);
-      v[4 * i + 2] = ln_rstd * (v[4 * i + 2] - ln_mean * ws.z); v[4 * i + 3] = ln_rstd * (v[4 * i + 3] - ln_mean * ws.w);
-    }
-  }
   if (e.bias) {
     const float4* b4 = reinterpret_cast<const float4*>(e.bias + col0);
 #pragma unroll
@@ -127,27 +115,6 @@ __device__ __forceinline__ void epilogue_chunk(const GemmEpilogue& e, int M, int
 #pragma unroll
     for (int k = 0; k < 4; ++k)
       if (row0 + 8 * k + rsub < M) *reinterpret_cast<float4*>(base + k * rstep) = x[k];
-    if constexpr (PROD) {
-      // the final rows once more as a split-bf16 operand + the partial LayerNorm statistics of this 16-column chunk
-      const int chunk = col0 >> 4;
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const int64_t r = row0 + 8 * k + rsub;
-        float s1 = x[k].x + x[k].y + x[k].z + x[k].w;
-        float s2 = x[k].x * x[k].x + x[k].y * x[k].y + x[k].z * x[k].z + x[k].w * x[k].w;
-        s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, 2); s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
-        if (r < M) {
-          uint32_t h0, l0, h1, l1;
-          split2(x[k].x, x[k].y, h0, l0);
-          split2(x[k].z, x[k].w, h1, l1);
-          __nv_bfloat16* o = e.raw_split + r * (2 * kLnDim) + col0 + 4 * q;
-          *reinterpret_cast<uint2*>(o) = make_uint2(h0, h1);
-          *reinterpret_cast<uint2*>(o + kLnDim) = make_uint2(l0, l1);
-          if (q == 0) *reinterpret_cast<float2*>(e.stat_part + (r * kLnParts + chunk) * 2) = make_float2(s1, s2);
-        }
-      }
-    }
     __syncwarp();
   }
   if (e.out_split) {
@@ -273,15 +240,11 @@ gemm_split3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
       const int row0 = mt * BM + quarter * 32;
       uint32_t* stg = reinterpret_cast<uint32_t*>(smem + OFF_STG) + e * STG_WORDS;
       const float* arow = acc_tile + (quarter * 32 + lane) * ACC_LD;
-      float ln_mean = 0.f, ln_rstd = 1.f;
-      if constexpr (NPROD == 5) {
-        if (row0 + lane < M) ln_row_stats(epi.ln_part + (int64_t)(row0 + lane) * kLnParts * 2, epi.ln_eps, ln_mean, ln_rstd);
-      }
 #pragma unroll 1
       for (int chunk = chunk0; chunk < chunk0 + CH; ++chunk) {
         float v[CW];
         acc_row_ld<CW>(arow + chunk * CW, v);
-        epilogue_chunk<NPROD == 4, NPROD == 5>(epi, M, N, row0, nt * BN + chunk * CW, lane, v, stg, ln_mean, ln_rstd);
+        epilogue_chunk(epi, M, N, row0, nt * BN + chunk * CW, lane, v, stg);
       }
       mbar_arrive(tempty_bar);
       acc_phase ^= 1u;
@@ -301,7 +264,7 @@ gemm_split3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
 // warps 4..7 producer (warp 4 issues the TMA loads), warps 8..11 epilogue (thread = row of the tile).  setmaxnreg moves
 // registers from the producer warpgroup (40) to the other two (232 each) so that neither spills and the wgmmas are not
 // serialised for lack of registers.  The accumulator tile is written to shared memory [row][q 48 | k 48 |
-// v 48] fp32; each thread adds the bias (and the folded LayerNorm) to its row in place, keeping q in registers, and --
+// v 48] fp32; each thread adds the bias to its row in place, keeping q in registers, and --
 // after the group's named barrier -- runs exact fp32 online-softmax attention of its row against the T key rows of its
 // track, then writes the 48 outputs as split bf16 straight into the out-projection's operand buffer.  The MMA
 // warpgroup computes the next tile in registers meanwhile.
@@ -408,11 +371,6 @@ gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
       const int mt = tile / kHeads, h = tile % kHeads;
       mbar_wait(tfull_bar, acc_phase);
       acc_phase ^= 1u;
-      float ln_mean = 0.f, ln_rstd = 1.f;
-      {
-        const int64_t grow_ln = (int64_t)mt * R + r;
-        if (epi.ln_part && grow_ln < M) ln_row_stats(epi.ln_part + grow_ln * kLnParts * 2, epi.ln_eps, ln_mean, ln_rstd);
-      }
       float xq[kDh];
       // k, v + bias back into the tile in place, q (kept in registers for the attention) last
 #pragma unroll
@@ -425,15 +383,6 @@ gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
           float v[16];
           acc_row_ld<16>(arow + col0 + 16 * c, v);
           const float4* b4 = reinterpret_cast<const float4*>(epi.bias + h * BNQ + col0 + 16 * c);
-          if (epi.ln_part) {
-            const float4* w4 = reinterpret_cast<const float4*>(epi.ln_wsum + h * BNQ + col0 + 16 * c);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float4 ws = __ldg(w4 + i);
-              v[4 * i + 0] = ln_rstd * (v[4 * i + 0] - ln_mean * ws.x); v[4 * i + 1] = ln_rstd * (v[4 * i + 1] - ln_mean * ws.y);
-              v[4 * i + 2] = ln_rstd * (v[4 * i + 2] - ln_mean * ws.z); v[4 * i + 3] = ln_rstd * (v[4 * i + 3] - ln_mean * ws.w);
-            }
-          }
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             const float4 b = __ldg(b4 + i);
@@ -520,11 +469,6 @@ gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
 // ------------------------------------------------------------------------------------------------
 // SIMT verification kernel: 64x64 tile, 256 threads, each 4x4 outputs; fp32 FMA on hi+lo.
 __device__ __forceinline__ void epilogue_store1(const GemmEpilogue& e, int N, int row, int col, float v) {
-  if (e.ln_part) {
-    float mean, rstd;
-    ln_row_stats(e.ln_part + (int64_t)row * kLnParts * 2, e.ln_eps, mean, rstd);
-    v = rstd * (v - mean * e.ln_wsum[col]);
-  }
   if (e.bias) v += e.bias[col];
   if (e.row_bias) v += e.row_bias[(int64_t)(row % e.row_mod) * N + col];
   v = apply_act(v, e.act);
@@ -654,8 +598,7 @@ bool qkv_time_attn_supported(int T) { return T >= 1 && T <= BM; }
 
 int gemm_qkv_time_attn_launch(const __nv_bfloat16* x_split, const __nv_bfloat16* w_heads, const float* bias_heads,
                               int M, int Kpad, int T, __nv_bfloat16* att_split, int64_t ld_split, int lo_off,
-                              float scale, const float* ln_part, const float* ln_wsum, float ln_eps, int num_sms,
-                              cudaStream_t stream, const char** err) {
+                              float scale, int num_sms, cudaStream_t stream, const char** err) {
   *err = nullptr;
   if (M <= 0 || Kpad <= 0 || (Kpad % BK) != 0 || !qkv_time_attn_supported(T) || (M % T) != 0) {
     *err = "qkv_time_attn: need M > 0, M % T == 0, 1 <= T <= 128, Kpad % 64 == 0";
@@ -684,9 +627,6 @@ int gemm_qkv_time_attn_launch(const __nv_bfloat16* x_split, const __nv_bfloat16*
   epi.out_split = att_split;
   epi.ld_split = ld_split;
   epi.lo_off = lo_off;
-  epi.ln_part = ln_part;
-  epi.ln_wsum = ln_wsum;
-  epi.ln_eps = ln_eps;
   gemm_qkv_time_attn_kernel<<<num_tiles < num_sms ? num_tiles : num_sms, qa::NTHREADS, qa::SMEM, stream>>>(
       tmX, tmW, M, Kpad, T, R, scale * 1.44269504088896340736f, epi);
   return (int)cudaGetLastError();
@@ -711,14 +651,6 @@ int gemm_launch(const GemmProblem& p, int impl, int num_sms, cudaStream_t stream
     *err = "gemm: operands must be 16-byte aligned";
     return (int)cudaErrorInvalidValue;
   }
-  if (p.epi.raw_split && (p.N != kLnDim || !p.epi.out_f32 || !p.epi.stat_part || impl == 1)) {
-    *err = "gemm: raw_split/stat_part need the fp32 output path of the tensor-core kernels with N == 384";
-    return (int)cudaErrorInvalidValue;
-  }
-  if (p.epi.ln_part && !p.epi.ln_wsum) {
-    *err = "gemm: ln_part needs ln_wsum";
-    return (int)cudaErrorInvalidValue;
-  }
   if (impl == 1) {
     dim3 grid((p.N + 63) / 64, (p.M + 63) / 64);
     gemm_split3_simt_kernel<<<grid, 256, 0, stream>>>(p.x_split, p.w_split, p.M, p.N, p.Kpad, x_ld, p.products,
@@ -732,13 +664,7 @@ int gemm_launch(const GemmProblem& p, int impl, int num_sms, cudaStream_t stream
     *err = "gemm: cuTensorMapEncodeTiled failed";
     return (int)cudaErrorInvalidValue;
   }
-  if (p.epi.ln_part && (p.products != 3 || p.epi.raw_split)) {
-    *err = "gemm: the LayerNorm-consumer epilogue needs 3 products and cannot be combined with raw_split";
-    return (int)cudaErrorInvalidValue;
-  }
-  cudaError_t e = (p.products == 3 && p.epi.raw_split) ? launch_tc<4>(p, tmX, tmW, num_mt, num_sms, stream)
-                : (p.products == 3 && p.epi.ln_part) ? launch_tc<5>(p, tmX, tmW, num_mt, num_sms, stream)
-                : p.products == 3 ? launch_tc<3>(p, tmX, tmW, num_mt, num_sms, stream)
+  cudaError_t e = p.products == 3 ? launch_tc<3>(p, tmX, tmW, num_mt, num_sms, stream)
                 : p.products == 2 ? launch_tc<2>(p, tmX, tmW, num_mt, num_sms, stream)
                                   : launch_tc<1>(p, tmX, tmW, num_mt, num_sms, stream);
   return (int)e;

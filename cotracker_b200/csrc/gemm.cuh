@@ -25,20 +25,7 @@ struct GemmEpilogue {
   int64_t ld_split = 0;
   int lo_off = 0;
   int row_group = 1;
-  // ---- LayerNorm folded into the GEMMs (no-affine LN, blocks.py:411,416; affine norm_context is folded into W, b) ----
-  // Consumer side: the A operand holds the RAW (un-normalised) rows x; with mean / rstd of the row,
-  //   W . LN(x) + b = rstd * (W . x - mean * wsum) + b,   wsum[col] = sum_k W[col][k].
-  // Row statistics arrive as kLnParts partial (sum, sum of squares) pairs per row, added in index order (deterministic).
-  const float* ln_part = nullptr;   // [M, kLnParts, 2]
-  const float* ln_wsum = nullptr;   // [N]
-  float ln_eps = 0.f;
-  // Producer side (fp32 output path only; N must be kLnDim): additionally emit the FINAL fp32 rows as a split-bf16
-  // operand and their per-16-column partial statistics, i.e. everything the next LayerNorm-consuming GEMM needs.
-  __nv_bfloat16* raw_split = nullptr;   // [M, 2*kLnDim]: hi | lo
-  float* stat_part = nullptr;           // [M, kLnParts, 2]
 };
-constexpr int kLnDim = 384;             // LayerNorm width (transformer hidden size)
-constexpr int kLnParts = kLnDim / 16;   // one partial per 16-column epilogue chunk
 
 struct GemmProblem {
   const __nv_bfloat16* x_split;  // [M, x_ld]: hi plane at column 0, lo plane (if any) at column Kpad
@@ -67,25 +54,8 @@ int gemm_launch(const GemmProblem& p, int impl, int num_sms, cudaStream_t stream
 //   rows of head h = [q_h | k_h | v_h], bias_heads [8*144] likewise; att_split[row*ld_split + h*48 + c] (hi) and
 //   + lo_off (lo) = softmax(q k^T scale) v.   T <= 128.
 bool qkv_time_attn_supported(int T);
-//   ln_part / ln_wsum / ln_eps: when given, x_split holds RAW rows and the LayerNorm is applied in the epilogue (see
-//   GemmEpilogue); ln_wsum follows the per-head row order of w_heads.
 int gemm_qkv_time_attn_launch(const __nv_bfloat16* x_split, const __nv_bfloat16* w_heads, const float* bias_heads,
                               int M, int Kpad, int T, __nv_bfloat16* att_split, int64_t ld_split, int lo_off,
-                              float scale, const float* ln_part, const float* ln_wsum, float ln_eps, int num_sms,
-                              cudaStream_t stream, const char** err);
-
-// mean / rstd of a row from its kLnParts partial sums (the one definition every consumer uses)
-__device__ __forceinline__ void ln_row_stats(const float* part, float eps, float& mean, float& rstd) {
-  float s = 0.f, ss = 0.f;
-#pragma unroll
-  for (int i = 0; i < kLnParts; ++i) {
-    const float2 p = __ldg(reinterpret_cast<const float2*>(part) + i);
-    s += p.x;
-    ss += p.y;
-  }
-  mean = s * (1.0f / kLnDim);
-  const float var = fmaxf(ss * (1.0f / kLnDim) - mean * mean, 0.f);
-  rstd = rsqrtf(var + eps);
-}
+                              float scale, int num_sms, cudaStream_t stream, const char** err);
 
 }  // namespace ct3

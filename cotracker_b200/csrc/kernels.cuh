@@ -136,11 +136,6 @@ cudaError_t launch_corr_patch_t(const __nv_bfloat16* pyr_half, int H4, int W4, c
 // ---- tokens.cu : elementwise / row-wise pieces of the transformer ---------------------------------
 cudaError_t launch_layernorm_split(const float* x, int rows, const float* gamma, const float* beta, float eps,
                                    __nv_bfloat16* out_split, cudaStream_t s);
-// LayerNorm fold helpers: split copy + partial row statistics of fp32 token rows; rowsum / affine fold at pack time
-cudaError_t launch_rowstats_split(const float* x, int rows, __nv_bfloat16* raw_split, float* stat_part, cudaStream_t s);
-cudaError_t launch_rowsum(const float* w, int N, int K, float* out, cudaStream_t s);
-cudaError_t launch_affine_fold(const float* w, const float* b, const float* gamma, const float* beta, int N, int K,
-                               float* w2, float* b2, cudaStream_t s);
 cudaError_t launch_build_x_small(const float* coords, const float* vis, const float* conf, int T, int N,
                                  __nv_bfloat16* x_split, cudaStream_t s);
 // one copy of the kV virtual tokens per group: rows (N + kV*g + i)*T + t, g < G

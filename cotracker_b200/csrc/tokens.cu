@@ -177,62 +177,6 @@ __global__ void split_rows_kernel(const float* __restrict__ x, int rows, int K, 
   }
 }
 
-// fp32 rows [rows, 384] -> split-bf16 copy [rows, 768] + the 24 per-16-column partial (sum, sum of squares) pairs the
-// LayerNorm-folding GEMMs consume (same partition as the GEMM epilogue's producer side); one warp per row
-__global__ void __launch_bounds__(256)
-rowstats_split_kernel(const float* __restrict__ x, int rows, __nv_bfloat16* __restrict__ raw, float* __restrict__ part) {
-  const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (row >= rows) return;
-  const float4* xr = reinterpret_cast<const float4*>(x + (int64_t)row * kC);
-  __nv_bfloat16* o = raw + (int64_t)row * (2 * kC);
-#pragma unroll
-  for (int i = 0; i < 3; ++i) {
-    const float4 v = xr[lane + 32 * i];
-    float s1 = v.x + v.y + v.z + v.w;
-    float s2 = v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
-    s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
-    s1 += __shfl_xor_sync(0xffffffffu, s1, 2); s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
-    const int c = (lane + 32 * i) * 4;
-    if ((lane & 3) == 0) *reinterpret_cast<float2*>(part + ((int64_t)row * (kC / 16) + (c >> 4)) * 2) = make_float2(s1, s2);
-    uint32_t h0, l0, h1, l1;
-    split2(v.x, v.y, h0, l0);
-    split2(v.z, v.w, h1, l1);
-    *reinterpret_cast<uint2*>(o + c) = make_uint2(h0, h1);
-    *reinterpret_cast<uint2*>(o + kC + c) = make_uint2(l0, l1);
-  }
-}
-
-// out[j] = sum_k w[j][k]   (the LayerNorm-fold correction vector of a linear layer); one warp per row
-__global__ void __launch_bounds__(256)
-rowsum_kernel(const float* __restrict__ w, int N, int K, float* __restrict__ out) {
-  const int j = blockIdx.x * 8 + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (j >= N) return;
-  float s = 0.f;
-  for (int k = lane; k < K; k += 32) s += w[(int64_t)j * K + k];
-  s = warp_sum(s);
-  if (lane == 0) out[j] = s;
-}
-
-// affine LayerNorm folded into the linear layer that consumes it:  W (gamma * xhat + beta) + b = (W diag(gamma)) xhat + (b + W beta)
-//   w2[j][k] = w[j][k] * gamma[k],  b2[j] = b[j] + sum_k w[j][k] * beta[k];  one warp per row
-__global__ void __launch_bounds__(256)
-affine_fold_kernel(const float* __restrict__ w, const float* __restrict__ b, const float* __restrict__ gamma,
-                   const float* __restrict__ beta, int N, int K, float* __restrict__ w2, float* __restrict__ b2) {
-  const int j = blockIdx.x * 8 + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (j >= N) return;
-  float s = 0.f;
-  for (int k = lane; k < K; k += 32) {
-    const float v = w[(int64_t)j * K + k];
-    w2[(int64_t)j * K + k] = v * gamma[k];
-    s = fmaf(v, beta[k], s);
-  }
-  s = warp_sum(s);
-  if (lane == 0) b2[j] = b[j] + s;
-}
-
 // a chunk of a host int32 table passed by value (kernel arguments stay below 4 KiB)
 constexpr int kI32Chunk = 960;
 struct I32Chunk { int32_t v[kI32Chunk]; };
@@ -281,20 +225,6 @@ cudaError_t launch_heads(const float* tokens, const float* w4, const float* b4, 
 }
 cudaError_t launch_row_bias(const float* time_emb, const float* w_in, int T, float* out, cudaStream_t s) {
   row_bias_kernel<<<(T * kC + 7) / 8, 256, 0, s>>>(time_emb, w_in, T, out);
-  return cudaGetLastError();
-}
-cudaError_t launch_rowstats_split(const float* x, int rows, __nv_bfloat16* raw_split, float* stat_part, cudaStream_t s) {
-  if (rows <= 0) return cudaSuccess;
-  rowstats_split_kernel<<<(rows + 7) / 8, 256, 0, s>>>(x, rows, raw_split, stat_part);
-  return cudaGetLastError();
-}
-cudaError_t launch_rowsum(const float* w, int N, int K, float* out, cudaStream_t s) {
-  rowsum_kernel<<<(N + 7) / 8, 256, 0, s>>>(w, N, K, out);
-  return cudaGetLastError();
-}
-cudaError_t launch_affine_fold(const float* w, const float* b, const float* gamma, const float* beta, int N, int K,
-                               float* w2, float* b2, cudaStream_t s) {
-  affine_fold_kernel<<<(N + 7) / 8, 256, 0, s>>>(w, b, gamma, beta, N, K, w2, b2);
   return cudaGetLastError();
 }
 cudaError_t launch_split_rows(const float* x, int rows, int K, int Kpad, int perm_x, __nv_bfloat16* out,

@@ -72,15 +72,14 @@ def test_grouped_calls_reject_unsupported_options():
     lib = engine.lib()
     fake = ctypes.c_void_p(1 << 20)
     ws = ctypes.c_void_p(1 << 24)
-    for name in ("fuse", "attn"):
-        old = engine.get_option(name)
-        engine.set_option(name, 2)
-        try:
-            rc = lib.ct3_updateformer_groups(fake, fake, 4, _sizes(3, 4), 2, fake, ws, 1 << 40, None)
-        finally:
-            engine.set_option(name, old)
-        assert rc == -4, name                                            # CT3_EUNSUPPORTED
-        assert b"fuse = 2 or attn = 2" in lib.ct3_last_error()
+    old = engine.get_option("attn")
+    engine.set_option("attn", 2)
+    try:
+        rc = lib.ct3_updateformer_groups(fake, fake, 4, _sizes(3, 4), 2, fake, ws, 1 << 40, None)
+    finally:
+        engine.set_option("attn", old)
+    assert rc == -4                                                      # CT3_EUNSUPPORTED
+    assert b"grouped calls do not support attn = 2" in lib.ct3_last_error()
 
 
 def _check_plan(sizes, T, budget, fn):

@@ -235,6 +235,10 @@ def test_options_are_validated_and_thread_local():
     lib = engine.lib()
     assert lib.ct3_set_option(b"corr", 7) == -1 and b"out of range" in lib.ct3_last_error()
     assert lib.ct3_set_option(b"attn", -1) == -1
+    assert engine.get_option("fuse") == 1
+    assert lib.ct3_set_option(b"fuse", 2) == -1 and b"out of range" in lib.ct3_last_error()
+    assert lib.ct3_set_option(b"fuse", 0) == 0 and engine.get_option("fuse") == 0
+    assert lib.ct3_set_option(b"fuse", 1) == 0
     assert lib.ct3_set_option(b"gemm", 1) == 0 and engine.get_option("gemm") == 1
     seen = []
     t = threading.Thread(target=lambda: seen.append(engine.get_option("gemm")))   # another host thread: defaults

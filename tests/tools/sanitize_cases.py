@@ -48,7 +48,7 @@ def model_cases():
     model = build_cotracker(None, offline=True, window_len=60).eval()
     model.load_state_dict(sd)
     model = model.to(DEV)
-    for fuse, attn in ((1, 0), (2, 0), (0, 0), (1, 2)):
+    for fuse, attn in ((1, 0), (0, 0), (1, 2)):
         eng.set_option("fuse", fuse); eng.set_option("attn", attn)
         c, v, q, _ = model(video.to(DEV), queries.to(DEV), iters=2)
         torch.cuda.synchronize()
