@@ -413,15 +413,50 @@ Prec effective_prec(bool have_pyr_split, int T, int H4, int W4) {
   return p;
 }
 
-// The steps update_loop and updateformer share: input_transform of the X rows in W.xs into the point tokens (with the
-// per-frame bias row_bias [T, kC] when given), the transformer body, then the heads: the state update of coords / vis /
-// conf, or with delta != nullptr the raw deltas [N,T,4] instead.
-int transform_and_heads(Runner& R, const Workspace& W, int T, int N, const GroupPlan& gp, const float* row_bias,
-                        float* coords, float* vis, float* conf, float* delta) {
-  const Layout& L = R.L;
+// input_transform of the X rows in W.xs into the point tokens, with the per-frame bias row_bias [T, kC] when given
+int input_transform(Runner& R, const Workspace& W, int T, int N, const float* row_bias) {
   GemmEpilogue e = Runner::to_f32(W.tokens, kC, false);
   if (row_bias) { e.row_bias = row_bias; e.row_mod = T; }
-  GEMM(W.xs, L.in_tr, N * T, e);
+  GEMM(W.xs, R.L.in_tr, N * T, e);
+  return 0;
+}
+
+// The first half of one update-loop iteration, from the state to the point tokens: the correlation volume (W.vol),
+// corr_mlp into the correlation columns of X and build_x_small into the rest (W.xs), then input_transform with the
+// time-embedding fold W.row_bias into the point rows of W.tokens.  Reads coords / vis / conf, writes none of them.
+// pyr_split: the split pyramid when the patch kernel runs (pr.patch), else null.
+int point_tokens(Runner& R, const Workspace& W, const Prec& pr, const float* pyr, const __nv_bfloat16* pyr_split,
+                 int H4, int W4, const float* support, const uint8_t* track_valid, const float* coords,
+                 const float* vis, const float* conf, int T, int N, int T_pyr, const FrameMap& fm) {
+  const Layout& L = R.L;
+  const int Mc = N * T * kL;
+  // (i)+(ii) sampling + 4-D correlation, all levels -> split volume
+  RUNC(CAT_CORR, launch_corr_sample(pyr, pyr_split, H4, W4, support, track_valid, coords, T, N, W.vol, g_opt_corr,
+                                    pr.corr, pr.vol16() ? 1 : 0, num_sms(), R.s, T_pyr, fm));
+  // (iii) corr_mlp: 2401 -> 384 (GELU erf) -> 256, written straight into X columns [256*l, 256*l+256)
+  if (pr.vol16()) {   // single fp16 volume plane x split fp16 weights: 2 (or 1) tensor-core products per FLOP
+    GEMM(W.vol, pr.support_major() ? L.corr_fc1_th : L.corr_fc1_h, Mc,
+         Runner::to_split(W.h1, 2 * kCorrHid, kCorrHid, /*erf*/ 1), pr.fc1, /*fp16*/ 1, kVolPad);
+  } else {
+    GEMM(W.vol, pr.support_major() ? L.corr_fc1_t : L.corr_fc1, Mc,
+         Runner::to_split(W.h1, 2 * kCorrHid, kCorrHid, /*erf*/ 1));
+  }
+  {
+    GemmEpilogue e = Runner::to_split(W.xs, 2 * kXPad, kXPad, 0);
+    e.row_group = kL;
+    GEMM(W.h1, L.corr_fc2, Mc, e);
+  }
+  // vis, conf, posenc(rel. motion), zero pad -> X columns [1024,1152)
+  RUNC(CAT_MISC, launch_build_x_small(coords, vis, conf, T, N, W.xs, R.s));
+  // (iv) input_transform (+ folded time embedding) -> point tokens
+  return input_transform(R, W, T, N, W.row_bias);
+}
+
+// The steps update_loop and updateformer share once the point tokens are in W.tokens: the transformer body, then the
+// heads: the state update of coords / vis / conf, or with delta != nullptr the raw deltas [N,T,4] instead.
+int transform_and_heads(Runner& R, const Workspace& W, int T, int N, const GroupPlan& gp, float* coords, float* vis,
+                        float* conf, float* delta) {
+  const Layout& L = R.L;
   if (int rc = transformer_body(R, W, T, N, gp)) return rc;
   RUNC(CAT_MISC, launch_heads(W.tokens, reinterpret_cast<const float*>(R.pk + L.heads_w),
                               reinterpret_cast<const float*>(R.pk + L.heads_b), coords, vis, conf, delta, T, N, R.s));
@@ -504,7 +539,6 @@ int update_loop(const void* packed, const float* pyr, int H4, int W4, const floa
     fm.goff = G > 1 ? gp.off : nullptr;
     fm.G = G;
   }
-  const int Mc = N * T * kL;
   // split-bf16 copy of the pyramid: the TMA source of the correlation kernel, made once per call
   const Prec pr = effective_prec(W.pyr_split != nullptr, T_pyr, H4, W4);
   const __nv_bfloat16* pyr_split = (pr.patch && iters > 0) ? W.pyr_split : nullptr;
@@ -514,27 +548,47 @@ int update_loop(const void* packed, const float* pyr, int H4, int W4, const floa
   RUNC(CAT_MISC, launch_row_bias(time_emb, reinterpret_cast<const float*>(R.pk + L.win_f32), T, W.row_bias, R.s));
 
   for (int it = 0; it < iters; ++it) {
-    // (i)+(ii) sampling + 4-D correlation, all levels -> split volume
-    RUNC(CAT_CORR, launch_corr_sample(pyr, pyr_split, H4, W4, support, track_valid, coords, T, N, W.vol, g_opt_corr,
-                                      pr.corr, pr.vol16() ? 1 : 0, num_sms(), R.s, T_pyr, fm));
-    // (iii) corr_mlp: 2401 -> 384 (GELU erf) -> 256, written straight into X columns [256*l, 256*l+256)
-    if (pr.vol16()) {   // single fp16 volume plane x split fp16 weights: 2 (or 1) tensor-core products per FLOP
-      GEMM(W.vol, pr.support_major() ? L.corr_fc1_th : L.corr_fc1_h, Mc,
-           Runner::to_split(W.h1, 2 * kCorrHid, kCorrHid, /*erf*/ 1), pr.fc1, /*fp16*/ 1, kVolPad);
-    } else {
-      GEMM(W.vol, pr.support_major() ? L.corr_fc1_t : L.corr_fc1, Mc,
-           Runner::to_split(W.h1, 2 * kCorrHid, kCorrHid, /*erf*/ 1));
-    }
-    {
-      GemmEpilogue e = Runner::to_split(W.xs, 2 * kXPad, kXPad, 0);
-      e.row_group = kL;
-      GEMM(W.h1, L.corr_fc2, Mc, e);
-    }
-    // vis, conf, posenc(rel. motion), zero pad -> X columns [1024,1152)
-    RUNC(CAT_MISC, launch_build_x_small(coords, vis, conf, T, N, W.xs, R.s));
-    // (iv) input_transform (+ folded time embedding) -> point tokens -> transformer; (v) heads + state update
-    if (int rc = transform_and_heads(R, W, T, N, gp, W.row_bias, coords, vis, conf, nullptr)) return rc;
+    // (i)-(iv) correlation, corr_mlp, X, input_transform -> point tokens
+    if (int rc = point_tokens(R, W, pr, pyr, pyr_split, H4, W4, support, track_valid, coords, vis, conf, T, N, T_pyr,
+                              fm))
+      return rc;
+    // transformer; (v) heads + state update
+    if (int rc = transform_and_heads(R, W, T, N, gp, coords, vis, conf, nullptr)) return rc;
   }
+  return 0;
+}
+
+// ct3_loop_tokens: the pyramid split, the time-embedding fold and point_tokens exactly as one update_loop iteration
+// runs them (G = 1, no frame map), then copies of the volume, X and the point tokens.  Checks as update_loop.
+int loop_tokens(const void* packed, const float* pyr, int H4, int W4, const float* support,
+                const uint8_t* track_valid, const float* coords, const float* vis, const float* conf,
+                const float* time_emb, int T, int N, void* vol_out, void* x_out, float* tokens_out, void* workspace,
+                size_t workspace_bytes, cudaStream_t stream) {
+  if (!packed || !pyr || !support || !coords || !vis || !conf || !time_emb || !workspace)
+    return fail(CT3_EINVAL, "null argument%s");
+  const int32_t one = N;
+  int total = 0;
+  if (int rc = check_groups(T, N, &one, 1, &total, false)) return rc;
+  if (int rc = check_frames(nullptr, 1, T, T)) return rc;
+  if (int rc = check_pyramid(T, H4, W4)) return rc;
+  if (int rc = check_aligned(workspace, "workspace")) return rc;
+  const Workspace W = carve(workspace, T, N, H4, W4);
+  if (int rc = check_space(workspace_bytes, W.total, "workspace")) return rc;
+  const Layout& L = layout();
+  Runner R{reinterpret_cast<const uint8_t*>(packed), L, stream, g_opt_gemm};
+  const Prec pr = effective_prec(W.pyr_split != nullptr, T, H4, W4);
+  const __nv_bfloat16* pyr_split = pr.patch ? W.pyr_split : nullptr;
+  if (pyr_split) RUNC(CAT_MISC, launch_split_pyramid(pyr, T, H4, W4, W.pyr_split, pr.corr, R.s));
+  RUNC(CAT_MISC, launch_row_bias(time_emb, reinterpret_cast<const float*>(R.pk + L.win_f32), T, W.row_bias, R.s));
+  if (int rc = point_tokens(R, W, pr, pyr, pyr_split, H4, W4, support, track_valid, coords, vis, conf, T, N, T,
+                            FrameMap{}))
+    return rc;
+  const size_t Rp = (size_t)N * T;
+  // the volume as ct3_corr_sample writes it: [Rp*4, 2*kVolPad] split bf16, or one fp16 plane [Rp*4, kVolPad]
+  if (vol_out) CK(cudaMemcpyAsync(vol_out, W.vol, Rp * kL * kVolPad * (pr.vol16() ? 2 : 4), cudaMemcpyDeviceToDevice,
+                                  R.s), "copy volume");
+  if (x_out) CK(cudaMemcpyAsync(x_out, W.xs, Rp * 2 * kXPad * 2, cudaMemcpyDeviceToDevice, R.s), "copy X");
+  if (tokens_out) CK(cudaMemcpyAsync(tokens_out, W.tokens, Rp * kC * 4, cudaMemcpyDeviceToDevice, R.s), "copy tokens");
   return 0;
 }
 
@@ -550,7 +604,8 @@ int updateformer(const void* packed, const float* x, int T, int N, const int32_t
   GroupPlan gp;
   if (int rc = plan_groups(gp, sizes, G, T, N, W.groups, R.s)) return rc;
   RUNC(CAT_MISC, launch_split_rows(x, N * T, kX, kXPad, /*perm_x*/ 1, W.xs, 0, R.s));
-  return transform_and_heads(R, W, T, N, gp, nullptr, nullptr, nullptr, nullptr, delta);
+  if (int rc = input_transform(R, W, T, N, nullptr)) return rc;
+  return transform_and_heads(R, W, T, N, gp, nullptr, nullptr, nullptr, delta);
 }
 
 // ct3_attention: the split-K partials and the group table, the attention parts of carve()
@@ -775,6 +830,14 @@ int ct3_update_loop_frames(const void* packed, const float* pyr, int T_pyr, int 
   if (!group_frames_host) return fail(CT3_EINVAL, "null group_frames_host%s");
   return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, group_sizes_host, G,
                      iters, workspace, workspace_bytes, (cudaStream_t)stream, T_pyr, group_frames_host);
+}
+
+int ct3_loop_tokens(const void* packed, const float* pyr, int H4, int W4, const float* support,
+                    const uint8_t* track_valid, const float* coords, const float* vis, const float* conf,
+                    const float* time_emb, int T, int N, void* vol_out, void* x_out, float* tokens_out,
+                    void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+  return loop_tokens(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, vol_out, x_out,
+                     tokens_out, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int ct3_updateformer(const void* packed, const float* x, int T, int N, float* delta, void* workspace,

@@ -100,7 +100,7 @@ __device__ __forceinline__ int map_frame(const int32_t* row, int t) { return row
 // vol_split [N*T*4, 2*kVolPad] bf16, row (n*T+t)*4+level; pyr holds T_pyr frames (T_pyr = T and fm = {} unless a frame
 // map is given)
 // impl: 0 tensor cores (correlate-then-interpolate when pyr_split is given and every level is >= 8x8: corr_tc3.cu for
-//         mode 2, corr_tc2.cu for modes 3 / 1; else corr_tc.cu),
+//         modes 2 / 1, corr_tc2.cu for mode 3; else corr_tc.cu),
 //       1 exact-fp32 SIMT, 2 corr_tc.cu always, 3 like 0 but corr_tc2.cu for every mode (A/B of the two kernels)
 // mode / vol16 apply to the corr_tc2.cu path only (corr_uses_patch_kernel): products per correlation FLOP (3|2|1;
 // pyr_split must have been made with the same mode) and a single-fp16-plane volume [N*T*4, kVolPad] instead of the

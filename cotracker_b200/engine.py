@@ -58,6 +58,8 @@ def _signatures():
                                     c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
         "ct3_corr_sample": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                     c_size_t, c_void_p]),
+        "ct3_loop_tokens": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
         "ct3_linear": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_split_rows": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_split_rows_fp16": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
@@ -435,22 +437,81 @@ def corr_sample(pyr, H4, W4, support, track_valid, coords, scratch: bool = True)
     T, N, _ = coords.shape
     vol = torch.zeros(N * T * LEVELS, 2 * VOL_PAD, dtype=torch.bfloat16, device=coords.device)
     scr = torch.empty(pyr.numel() * 4, dtype=torch.uint8, device=coords.device) if scratch else None
-    # a single fp16 plane [rows, 2432] when the correlate-then-interpolate kernel runs with prec.fc1 < 3
-    vb = precision_info(T, H4, W4)[2] if (scratch and get_option("corr") in (0, 3)) else 4
     _call("ct3_corr_sample", coords.device, _ptr(pyr), H4, W4, _ptr(support), _ptr(track_valid), _ptr(coords), T, N,
           _ptr(vol), _ptr(scr), scr.numel() if scratch else 0, _stream(coords.device))
+    return volume_planes(vol, T, N, H4, W4, scratch).sum(0).reshape(N, T, LEVELS, VOL)
+
+
+def volume_planes(vol: torch.Tensor, T: int, N: int, H4: int, W4: int, patch: bool = True) -> torch.Tensor:
+    """Decode a correlation volume in the device layout of ct3_corr_sample / ct3_loop_tokens (`vol`: the bytes as a
+    [N*T*4, 2*2432] 16-bit tensor) -> fp32 [planes, N*T*4, 2401] in the reference's element order, planes = (hi, lo) of
+    the split bf16 volume or the one fp16 plane; their sum is the volume.  patch: the split pyramid was available, so
+    the correlate-then-interpolate kernels could run and this thread's options decide the format and element order."""
+    rows = N * T * LEVELS
+    # a single fp16 plane [rows, 2432] when the correlate-then-interpolate kernel runs with prec.fc1 < 3
+    vb = precision_info(T, H4, W4)[2] if (patch and get_option("corr") in (0, 3)) else 4
     if vb == 2:
-        full = vol.reshape(-1).view(torch.float16)[:N * T * LEVELS * VOL_PAD].reshape(-1, VOL_PAD).float()
+        planes = vol.reshape(-1).view(torch.float16)[:rows * VOL_PAD].reshape(1, rows, VOL_PAD).float()
     else:
-        v = vol.float()
-        full = v[:, :VOL_PAD] + v[:, VOL_PAD:]
-    assert bool((full[:, VOL:] == 0).all()), "K padding of the correlation volume must be zero"
-    full = full[:, :VOL]
+        planes = vol.reshape(rows, 2, VOL_PAD).transpose(0, 1).float()
+    assert bool((planes[:, :, VOL:] == 0).all()), "K padding of the correlation volume must be zero"
+    planes = planes[:, :, :VOL]
     flag = ctypes.c_int(0)
     _check(lib().ct3_volume_is_support_major(T, H4, W4, ctypes.byref(flag)), "ct3_volume_is_support_major")
-    if scratch and flag.value:   # corr_tc3.cu: rows are [k][a*7+b]; hand back the reference order [(a*7+b)][k]
-        full = full.reshape(-1, P, P).transpose(1, 2).reshape(-1, VOL)
-    return full.reshape(N, T, LEVELS, VOL)
+    if patch and flag.value:   # corr_tc3.cu: rows are [k][a*7+b]; hand back the reference order [(a*7+b)][k]
+        planes = planes.reshape(len(planes), rows, P, P).transpose(2, 3).reshape(len(planes), rows, VOL)
+    return planes
+
+
+def x_src_col(dst: int) -> int:
+    """Reference column of device X column `dst` (x_src_col in csrc/common.cuh): the correlation embeddings first, then
+    vis, conf, posenc and zero padding; -1 = padding."""
+    if dst < 1024:
+        return dst + 2
+    if dst in (1024, 1025):
+        return dst - 1024
+    return dst if dst < XDIM else -1
+
+
+def x_planes(xs: torch.Tensor) -> torch.Tensor:
+    """Split X rows [R, 2*1152] (bf16 hi | lo, device column order) -> fp32 [2, R, 1110] in the reference's column
+    order; their sum is X."""
+    dst = [c for c in range(XDIM_PAD) if x_src_col(c) >= 0]
+    src = torch.tensor([x_src_col(c) for c in dst], device=xs.device)
+    planes = xs.reshape(-1, 2, XDIM_PAD).transpose(0, 1).float()
+    out = torch.empty(2, planes.shape[1], XDIM, dtype=torch.float32, device=xs.device)
+    out[:, :, src] = planes[:, :, dst]
+    return out
+
+
+def loop_tokens(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, workspace=None,
+                raw: bool = False):
+    """ct3_loop_tokens: the first half of one update-loop iteration, from the state (read only) to the point tokens,
+    under this thread's options -> fp32 (volume [N,T,4,2401] in reference order, X [N,T,1110] = hi + lo in reference
+    column order without the time embedding, tokens [N,T,384]).  raw=True returns the device buffers instead: the
+    volume bytes as [N*T*4, 2*2432] bf16 (volume_planes decodes them), X [N*T, 2*1152] bf16 (x_planes), tokens
+    [N*T, 384]."""
+    for t, name in ((coords, "coords"), (vis, "vis"), (conf, "conf"), (pyr, "pyr"), (support, "support"),
+                    (time_emb, "time_emb")):
+        _req(t, torch.float32, name)
+    T, N, _ = coords.shape
+    if time_emb.shape != (T, XDIM):
+        raise EngineError(f"time_emb must be [{T},{XDIM}]")
+    if track_valid is not None:
+        _req(track_valid, torch.uint8, "track_valid")
+    dev = coords.device
+    if workspace is None:
+        workspace = torch.empty(workspace_bytes(T, N, H4, W4), dtype=torch.uint8, device=dev)
+    vol = torch.zeros(N * T * LEVELS, 2 * VOL_PAD, dtype=torch.bfloat16, device=dev)
+    xs = torch.empty(N * T, 2 * XDIM_PAD, dtype=torch.bfloat16, device=dev)
+    tokens = torch.empty(N * T, HID, dtype=torch.float32, device=dev)
+    _call("ct3_loop_tokens", dev, _ptr(packed), _ptr(pyr), H4, W4, _ptr(support), _ptr(track_valid), _ptr(coords),
+          _ptr(vis), _ptr(conf), _ptr(time_emb), T, N, _ptr(vol), _ptr(xs), _ptr(tokens), _ptr(workspace),
+          workspace.numel(), _stream(dev))
+    if raw:
+        return vol, xs, tokens
+    return (volume_planes(vol, T, N, H4, W4).sum(0).reshape(N, T, LEVELS, VOL),
+            x_planes(xs).sum(0).reshape(N, T, XDIM), tokens.reshape(N, T, HID))
 
 
 def split_rows(x: torch.Tensor, Kpad: int, fp16: bool = False) -> torch.Tensor:

@@ -278,6 +278,26 @@ int ct3_corr_sample(const float* pyr, int H4, int W4, const float* support,
                     const uint8_t* track_valid, const float* coords, int T, int N,
                     void* vol_split, void* scratch, size_t scratch_bytes, ct3_stream_t stream);
 
+/* The first half of one ct3_update_loop iteration, from the state to the point tokens, run by the loop's own code
+ * under the calling thread's "gemm" / "corr" / "prec.*" options: correlation sampling (the split pyramid copy when the
+ * correlate-then-interpolate kernel runs), corr_mlp (cotracker3_offline.py:142-160) into X, vis / conf / posenc
+ * (:162-188), and input_transform with the time embedding folded in as a per-frame bias (:196, cotracker.py:486).
+ * Arguments as ct3_update_loop; coords / vis / conf are only read.  Outputs, each optional (NULL = not copied), written
+ * in stream order:
+ *   vol_out    : the correlation volume with ct3_corr_sample's layout and bytes: [N*T*4, 2*2432] split bf16, or one
+ *                fp16 plane [N*T*4, 2432] when ct3_precision_info reports 2 bytes per element; rows support-major when
+ *                ct3_volume_is_support_major says so
+ *   x_out      : X [N*T, 2*1152] split 16-bit rows (bf16 hi cols 0..1151 | lo cols 1152..2303), row n*T + t, in the
+ *                device column order (DESIGN.md: correlation embeddings 0..1023, vis 1024, conf 1025, posenc
+ *                1026..1109, zero 1110..1151), WITHOUT the time embedding
+ *   tokens_out : the point tokens fp32 [N*T, 384], row n*T + t
+ * workspace: ct3_workspace_bytes(T, N, H4, W4) bytes, 256-byte aligned.  Invalid arguments return CT3_EINVAL and a too
+ * small workspace CT3_ENOSPC, with ct3_update_loop's checks and messages, before any launch. */
+int ct3_loop_tokens(const void* packed, const float* pyr, int H4, int W4, const float* support,
+                    const uint8_t* track_valid, const float* coords, const float* vis, const float* conf,
+                    const float* time_emb, int T, int N, void* vol_out, void* x_out, float* tokens_out,
+                    void* workspace, size_t workspace_bytes, ct3_stream_t stream);
+
 /* Generic split-bf16x3 linear layer  Y = act(X W^T + b)  (nn.Linear, blocks.py:61-67)
  *   x_split [M, 2*Kpad] bf16 (hi|lo), w_split [Nout, 2*Kpad] bf16, bias [Nout] fp32 or NULL
  *   act: 0 none, 1 GELU(erf), 2 GELU(tanh);  y fp32 [M, Nout] */

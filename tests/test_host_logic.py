@@ -89,6 +89,60 @@ def test_attention_stage_argument_validation_without_gpu():
         assert lib.ct3_set_option(b"attn", 0) == 0
 
 
+def test_loop_tokens_argument_validation_without_gpu():
+    """ct3_loop_tokens rejects bad arguments with update_loop's checks and messages (CT3_EINVAL / CT3_ENOSPC) before
+    any launch (the pointers below are never dereferenced)."""
+    from cotracker_b200 import engine
+    lib = engine.lib()
+    T, N, H4, W4 = 4, 10, 64, 72
+    need = engine.workspace_bytes(T, N, H4, W4)
+    p, ws = ctypes.c_void_p(1 << 20), ctypes.c_void_p(1 << 21)
+
+    def call(packed=p, pyr=p, H4=H4, W4=W4, support=p, coords=p, vis=p, conf=p, te=p, T=T, N=N, w=ws, nbytes=need,
+             outs=(None, None, None)):
+        return lib.ct3_loop_tokens(packed, pyr, H4, W4, support, None, coords, vis, conf, te, T, N, *outs, w, nbytes,
+                                   None)
+
+    for k in ("packed", "pyr", "support", "coords", "vis", "conf", "te", "w"):
+        assert call(**{k: None}) == -1 and b"null argument" in lib.ct3_last_error(), k
+    assert call(T=0) == -1 and b"T and N" in lib.ct3_last_error()
+    assert call(N=0) == -1 and b"T and N" in lib.ct3_last_error()
+    assert call(N=1 << 30) == -1 and b"too large" in lib.ct3_last_error()
+    assert call(H4=4, W4=4) == -1                                                       # level 3 would be 0x0
+    assert call(w=ctypes.c_void_p((1 << 21) + 16)) == -1 and b"256-byte" in lib.ct3_last_error()
+    assert call(nbytes=need - 1) == -3 and b"workspace too small" in lib.ct3_last_error()   # CT3_ENOSPC
+    # the same messages as ct3_update_loop for the same faults
+    assert lib.ct3_update_loop(p, p, H4, W4, p, None, p, p, p, p, T, N, 1, ws, need - 1, None) == -3
+    assert b"workspace too small" in lib.ct3_last_error()
+
+
+def test_loop_tokens_branch_map_matches_library():
+    """The branch map of test_gpu_tokens.py (which correlation kernel, volume format, fc1 weights and products a call
+    runs) against what the compiled library reports, across the options and pyramid shapes (every level >= 8x8 or not)."""
+    import itertools
+    from cotracker_b200 import engine
+    from test_gpu_tokens import loop_branch
+    lib = engine.lib()
+    flag = ctypes.c_int(0)
+    try:
+        for corr, pc, pf, (H4, W4) in itertools.product(range(4), (1, 2, 3), (1, 2, 3),
+                                                        [(24, 32), (64, 72), (96, 128), (64, 63), (63, 64), (8, 8)]):
+            for k, v in (("corr", corr), ("prec.corr", pc), ("prec.fc1", pf)):
+                engine.set_option(k, v)
+            b = loop_branch(16, H4, W4, corr, pc, pf)
+            assert engine.precision_info(16, H4, W4) == (b["corr_products"], b["products"],
+                                                         2 if b["volume"] == "fp16" else 4), (corr, pc, pf, H4, W4)
+            assert lib.ct3_volume_is_support_major(16, H4, W4, ctypes.byref(flag)) == 0
+            assert bool(flag.value) == b["support_major"], (corr, pc, pf, H4, W4)
+    finally:
+        for k, v in (("corr", 0), ("prec.corr", 2), ("prec.fc1", 3)):
+            engine.set_option(k, v)
+    assert loop_branch(16, 96, 128)["weights"] == "corr_fc1_t"
+    assert loop_branch(16, 96, 128, prec_fc1=2)["weights"] == "corr_fc1_th"
+    assert loop_branch(16, 96, 128, corr=3, prec_fc1=1)["weights"] == "corr_fc1_h"
+    assert loop_branch(16, 24, 32, prec_fc1=1) == loop_branch(16, 24, 32, corr=2)    # no patch kernel: split x split
+
+
 def test_weight_names_match_state_dict():
     from cotracker_b200 import engine
     from cotracker_b200.build import build_cotracker
