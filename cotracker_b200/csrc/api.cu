@@ -198,6 +198,25 @@ int ct3_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t 
   return 0;
 }
 
+// ---- the predictor's tail (finish.cu) ----------------------------------------------------------------------------
+int ct3_finish_tracks(const float* fwd_tracks, const float* fwd_vis, const float* bwd_tracks, const float* bwd_vis,
+                      const float* queries, int B, int T, int N, int n_keep, float threshold, float scale_x,
+                      float scale_y, float* tracks, uint8_t* visibility, ct3_stream_t stream) {
+  if (!fwd_tracks || !fwd_vis || !queries || !tracks || !visibility) return fail(CT3_EINVAL, "null argument%s");
+  if ((bwd_tracks == nullptr) != (bwd_vis == nullptr))
+    return fail(CT3_EINVAL, "bwd_tracks and bwd_vis must be given together%s");
+  if (B < 1 || T < 1 || N < 1) return fail(CT3_EINVAL, "B, T and N must be >= 1%s");
+  if (n_keep < 1 || n_keep > N) return fail(CT3_EINVAL, "n_keep must be in [1, N]%s");
+  if (((uintptr_t)fwd_tracks | (uintptr_t)bwd_tracks | (uintptr_t)tracks) & 7)
+    return fail(CT3_EINVAL, "tracks must be 8-byte aligned%s");
+  // one thread per output element, one-dimensional grid
+  if ((int64_t)B * T > (INT64_MAX >> 12) / N || (int64_t)B * T * N > (int64_t)INT32_MAX * 256)
+    return fail(CT3_EINVAL, "problem too large%s");
+  CK(launch_finish_tracks(fwd_tracks, fwd_vis, bwd_tracks, bwd_vis, queries, B, T, N, n_keep, threshold, scale_x,
+                          scale_y, tracks, visibility, (cudaStream_t)stream), "finish_tracks");
+  return 0;
+}
+
 // ---- track visualiser (render.cu) ------------------------------------------------------------------------------
 int ct3_render_prepare(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c,
                        int64_t stride_h, int64_t stride_w, int pad, int grayscale, uint8_t* out, ct3_stream_t stream) {

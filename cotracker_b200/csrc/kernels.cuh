@@ -25,6 +25,14 @@ cudaError_t launch_pyramid_pools(int T, int H4, int W4, float* pyr, cudaStream_t
 cudaError_t launch_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t st, int64_t sc, int64_t sh,
                                   int64_t sw, int oh, int ow, float* out, cudaStream_t s);
 
+// ---- finish.cu : the predictor's tail (arguments validated by ct3_finish_tracks) --------------------
+// forward (+ optional backward, reversed-clip time) tracks [B,T,N,2] / visibility probabilities [B,T,N], queries
+// [B,N,3] -> tracks [B,T,n_keep,2] fp32 and visibility [B,T,n_keep] uint8 (0 | 1), bit-identical to the ATen sequence
+cudaError_t launch_finish_tracks(const float* fwd_tracks, const float* fwd_vis, const float* bwd_tracks,
+                                 const float* bwd_vis, const float* queries, int B, int T, int N, int n_keep,
+                                 float threshold, float scale_x, float scale_y, float* tracks, uint8_t* visibility,
+                                 cudaStream_t s);
+
 // ---- render.cu : the track visualiser on uint8 frames [T,H,W,3] (arguments validated by ct3_render_*) ----------
 constexpr int kRenderMaxRadius = 255;   // largest point radius (int(linewidth * 2)) the footprint table holds
 cudaError_t launch_render_prepare(const void* src, int dtype, int T, int H, int W, int64_t st, int64_t sc, int64_t sh,

@@ -45,6 +45,8 @@ def _signatures():
         "ct3_prepare_pyramid": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_prepare_frames": (c_int, [c_void_p, c_int, c_int, c_int, c_int, i64, i64, i64, i64, c_int, c_int, c_void_p,
                                        c_void_p]),
+        "ct3_finish_tracks": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                      ctypes.c_float, ctypes.c_float, ctypes.c_float, c_void_p, c_void_p, c_void_p]),
         "ct3_render_prepare": (c_int, [c_void_p, c_int, c_int, c_int, c_int, i64, i64, i64, i64, c_int, c_int, c_void_p,
                                        c_void_p]),
         "ct3_render_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
@@ -254,6 +256,34 @@ def prepare_frames(src: torch.Tensor, out_hw, out: Optional[torch.Tensor] = None
     _call("ct3_prepare_frames", src.device, _ptr(src), FRAME_DTYPES[src.dtype], T, H, W, *src.stride(), oh, ow, _ptr(out),
           _stream(src.device))
     return out
+
+
+def finish_tracks(fwd, bwd, queries: torch.Tensor, n_keep: int, threshold: float, scale_xy):
+    """The predictor's tail in one kernel (ct3_finish_tracks in include/ct3_b200.h).  fwd = (tracks [B,T,N,2],
+    visibility probabilities [B,T,N]) of the forward pass, bwd = the same of the pass on the clip played backwards (in
+    reversed-clip time) or None, queries [B,N,3] at model resolution; all fp32 on one device.
+    -> (tracks [B,T,n_keep,2] fp32 scaled by scale_xy, visibility [B,T,n_keep] bool)."""
+    tensors = [("fwd tracks", fwd[0]), ("fwd visibility", fwd[1]), ("queries", queries)]
+    if bwd is not None:
+        tensors += [("bwd tracks", bwd[0]), ("bwd visibility", bwd[1])]
+    for name, t in tensors:
+        _req(t, torch.float32, name)
+    if queries.dim() != 3 or queries.shape[2] != 3:
+        raise EngineError(f"queries must be [B,N,3], got {tuple(queries.shape)}")
+    B, N, _ = queries.shape
+    dev = queries.device
+    T = fwd[0].shape[1] if fwd[0].dim() == 4 else -1
+    for name, t in tensors:
+        want = (B, N, 3) if name == "queries" else (B, T, N, 2) if name.endswith("tracks") else (B, T, N)
+        if tuple(t.shape) != want or t.device != dev:
+            raise EngineError(f"{name} must be {want} on {dev}, got {tuple(t.shape)} on {t.device}")
+    n_keep = int(n_keep)
+    tracks = torch.empty(B, T, max(n_keep, 0), 2, dtype=torch.float32, device=dev)
+    visibility = torch.empty(B, T, max(n_keep, 0), dtype=torch.bool, device=dev)
+    _call("ct3_finish_tracks", dev, _ptr(fwd[0]), _ptr(fwd[1]), _ptr(None if bwd is None else bwd[0]),
+          _ptr(None if bwd is None else bwd[1]), _ptr(queries), B, T, N, n_keep, float(threshold), float(scale_xy[0]),
+          float(scale_xy[1]), _ptr(tracks), _ptr(visibility), _stream(dev))
+    return tracks, visibility
 
 
 def render_prepare(src: torch.Tensor, pad: int, grayscale: bool) -> torch.Tensor:
@@ -707,6 +737,21 @@ def concat_pyramid_frames(pyr_a: torch.Tensor, Ta: int, a0: int, pyr_b: torch.Te
         per = h[l] * w[l] * LATENT
         parts.append(pyr_a[off_a[l] + a0 * per: off_a[l] + Ta * per])
         parts.append(pyr_b[off_b[l]: off_b[l] + Tb * per])
+    return torch.cat(parts)
+
+
+def concat_pyramid_runs(runs, H4: int, W4: int) -> torch.Tensor:
+    """Flat pyramid of the frame runs (pyr, T, a, b) = frames [a, b) of the T-frame flat pyramid `pyr`, concatenated in
+    order: one copy, whatever the number of runs and source pyramids."""
+    parts = []
+    layouts = {}
+    for l in range(LEVELS):
+        for pyr, T, a, b in runs:
+            if T not in layouts:
+                layouts[T] = pyramid_layout(T, H4, W4)
+            off, h, w, _ = layouts[T]
+            per = h[l] * w[l] * LATENT
+            parts.append(pyr[off[l] + a * per: off[l] + b * per])
     return torch.cat(parts)
 
 

@@ -128,6 +128,24 @@ def plan_passes(group_sizes: Sequence[int], T: int, H4: int, W4: int, budget_byt
     return passes
 
 
+def plan_clip_passes(n_clips: int, group_sizes: Sequence[int], T: int, H4: int, W4: int, budget_bytes: int,
+                     frames_fn: Optional[Callable[[int], Optional[int]]] = None) -> List[Tuple[int, int]]:
+    """Split the clips of a batch, in order, into passes [b0, b1): as few as keep a pass within `budget_bytes`, and
+    of even size.  Every clip brings the same groups (`group_sizes`, T frames per update loop), so a pass over n clips
+    costs pass_bytes(T, n * sum(group_sizes), n * len(group_sizes), H4, W4, frames_fn(n)); frames_fn(n): the pyramid
+    frames such a pass reads through its frame map (None: it has none).  A pure host function; a clip that alone
+    exceeds the budget gets a pass of its own.  The library takes any number of groups up to the number of tracks,
+    which a batch of clips with at least one track per group cannot exceed."""
+    N, G = sum(group_sizes), len(group_sizes)
+    fit = 1
+    while fit < n_clips and pass_bytes(T, (fit + 1) * N, (fit + 1) * G, H4, W4,
+                                       frames_fn(fit + 1) if frames_fn else None) <= budget_bytes:
+        fit += 1
+    n_passes = -(-n_clips // fit)
+    per = -(-n_clips // n_passes)
+    return [(b0, min(n_clips, b0 + per)) for b0 in range(0, n_clips, per)]
+
+
 class EvaluationPredictor(torch.nn.Module):
     """Benchmark-protocol wrapper around an offline CoTracker3 model (B = 1).
 

@@ -1,6 +1,8 @@
 """One ingestion step for every predictor: the clip as the caller holds it -> normalised encoder input on the GPU.
 
-    prepare_video(video [1,T,3,H,W], (ih, iw), device) -> frames [T,3,ih,iw] fp32 in [-1,1] on `device`
+    prepare_video(video [B,T,3,H,W], (ih, iw), device) -> frames [B*T,3,ih,iw] fp32 in [-1,1] on `device`
+
+The frames of a batch come out clip after clip (clip b's at b*T ..), the order the encoder and the models take them in.
 
 `video` may be uint8 (what decoders return) or float32 in 0..255, with any strides (a channels-last [T,H,W,3]
 buffer seen through `permute` is read in place), on the device or on the host.  The resize and normalisation are one
@@ -11,7 +13,8 @@ A device clip is one kernel call on the strided tensor.  A host clip is uploaded
 pinned staging slots on a side stream: the host copy of chunk c+1 and its upload overlap the kernel on chunk c, and the
 device never holds more than two raw chunks.  Staging memory is bounded: 2 * k * frame_bytes pinned host bytes plus
 the same on the device, with k = max(1, min(T, STAGING_SLOT_BYTES // frame_bytes)) -- at most
-2 * max(STAGING_SLOT_BYTES, frame_bytes) each (`staging_bytes`).
+2 * max(STAGING_SLOT_BYTES, frame_bytes) each (`staging_bytes`).  The clips of a host batch go through the same two
+slots one after another, so the bound does not grow with B.
 """
 from __future__ import annotations
 
@@ -67,29 +70,37 @@ def model_device(model: torch.nn.Module) -> torch.device:
 
 
 def prepare_video(video: torch.Tensor, out_hw, device) -> torch.Tensor:
-    """video [1,T,3,H,W] uint8 or float (0..255), host or device, any strides -> [T,3,oh,ow] fp32 in [-1,1] on device.
+    """video [B,T,3,H,W] uint8 or float (0..255), host or device, any strides -> [B*T,3,oh,ow] fp32 in [-1,1] on device,
+    clip after clip; each clip's frames are bit-identical to the call on that clip alone.
     Other dtypes (float16, float64, ...) are cast to float32 first and then take the float32 path; for pixel values
     0..255 that cast is exact.  (Before this step existed they were resized in their own dtype, so results for them can
     differ from that in the last bits.)"""
     device = torch.device(device)
     if device.type != "cuda":
         raise engine.EngineError("cotracker_b200 runs on CUDA only; move the module to a GPU")
-    if video.dim() != 5 or video.shape[0] != 1 or video.shape[2] != 3:
-        raise ValueError(f"video must be [1,T,3,H,W], got {tuple(video.shape)}")
+    if video.dim() != 5 or video.shape[0] < 1 or video.shape[1] < 1 or video.shape[2] != 3:
+        raise ValueError(f"video must be [B,T,3,H,W] with B, T >= 1, got {tuple(video.shape)}")
     if video.dtype not in engine.FRAME_DTYPES:
         video = video.float()
-    v = video[0]
-    if v.is_cuda:
-        if v.device != device:
-            v = v.to(device)
-        return engine.prepare_frames(v, out_hw)
-    return _prepare_host(v, out_hw, device)
+    B, T = video.shape[:2]
+    if video.is_cuda and video.device != device:
+        video = video.to(device)
+    out = torch.empty(B * T, 3, int(out_hw[0]), int(out_hw[1]), dtype=torch.float32, device=device)
+    staging = None
+    for b in range(B):
+        if video.is_cuda:
+            engine.prepare_frames(video[b], out_hw, out=out[b * T:(b + 1) * T])
+        else:
+            staging = _prepare_host(video[b], out_hw, out[b * T:(b + 1) * T], staging)
+    return out
 
 
-def _prepare_host(v: torch.Tensor, out_hw, device) -> torch.Tensor:
+def _prepare_host(v: torch.Tensor, out_hw, out: torch.Tensor, staging=None):
+    """One host clip [T,3,H,W] -> out [T,3,oh,ow] on the device.  Returns its staging buffers (pinned slots, device
+    slots), which the next clip of a batch takes as `staging`."""
     T, C, H, W = v.shape
     oh, ow = int(out_hw[0]), int(out_hw[1])
-    out = torch.empty(T, 3, oh, ow, dtype=torch.float32, device=device)
+    device = out.device
     fe = C * H * W                                  # elements per frame
     esize = v.element_size()
     chunks = plan_chunks(T, fe * esize)
@@ -99,8 +110,10 @@ def _prepare_host(v: torch.Tensor, out_hw, device) -> torch.Tensor:
 
     main = torch.cuda.current_stream(device)
     side = torch.cuda.Stream(device)
-    pinned = [torch.empty(k * fe, dtype=v.dtype, pin_memory=True) for _ in range(2)]
-    raw = [torch.empty(k * fe, dtype=v.dtype, device=device) for _ in range(2)]
+    if staging is None:
+        staging = ([torch.empty(k * fe, dtype=v.dtype, pin_memory=True) for _ in range(2)],
+                   [torch.empty(k * fe, dtype=v.dtype, device=device) for _ in range(2)])
+    pinned, raw = staging
     copied = [torch.cuda.Event() for _ in range(2)]     # upload of the slot finished (side stream)
     consumed = [torch.cuda.Event() for _ in range(2)]   # kernel reading the slot finished (main stream)
     used = [False, False]
@@ -135,4 +148,4 @@ def _prepare_host(v: torch.Tensor, out_hw, device) -> torch.Tensor:
     for slot in range(2):
         if used[slot]:
             copied[slot].synchronize()
-    return out
+    return staging

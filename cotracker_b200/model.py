@@ -9,7 +9,9 @@ state-dict keys (SURVEY.md Appendix B), so `load_state_dict(strict=True)` of the
 The nn.Module tree below is a *parameter container*: nothing executes through PyTorch modules.  The CNN
 encoder, L2-normalisation + pyramid, support sampling, correlation sampling, the correlation MLP, the whole
 EfficientUpdateFormer and the delta heads run as hand-written sm_90a CUDA behind the C ABI
-(`cotracker_b200.engine`).  Inference only; B must be 1 (as in the reference, SURVEY.md §0).
+(`cotracker_b200.engine`).  Inference only.  A batch of B clips (same length and size) is tracked in one pass: clip b's
+queries are query groups of one update loop that read clip b's frames of one pyramid holding all B clips, and slot b of
+the result is bit-identical to the call on `video[b:b+1]`, `queries[b:b+1]` (DESIGN.md 4.4.3).
 """
 from __future__ import annotations
 
@@ -117,12 +119,24 @@ def gather_plan(frame_map):
 
 def gather_pyramid(pyr, T: int, H4: int, W4: int, runs) -> torch.Tensor:
     """Flat pyramid of the frame runs [a, b) of the T-frame pyramid `pyr`, concatenated in order."""
-    out, n = None, 0
-    for a, b in runs:
-        part = engine.slice_pyramid(pyr, T, H4, W4, a, b - a)
-        out = part if out is None else engine.concat_pyramid_frames(out, n, 0, part, b - a, H4, W4)
-        n += b - a
-    return out
+    return engine.concat_pyramid_runs([(pyr, T, a, b) for a, b in runs], H4, W4)
+
+
+# A batch is stored clip after clip: clip c's frames are frames c * T_clip ... of one pyramid, its tracks follow clip
+# c-1's, and its query groups are groups of the same update loop.  `clips` names the clips a pass tracks (all of them,
+# or a sub-batch when the whole batch does not fit in device memory).
+def batch_frame_map(frame_map, clips, T_clip: int) -> List[List[int]]:
+    """The one-clip frame map repeated for each of `clips`: the groups of clip c read the same frames plus c * T_clip."""
+    return [[f + c * T_clip for f in row] for c in clips for row in frame_map]
+
+
+def batch_gather_plan(frame_map, clips, T_clip: int):
+    """`gather_plan` of `batch_frame_map(frame_map, clips, T_clip)` with every run inside one clip: the one-clip plan
+    repeated per clip, so clip number i of `clips` owns frames [i * n, (i + 1) * n) of the gathered pyramid."""
+    runs, remap = gather_plan(frame_map)
+    n = sum(b - a for a, b in runs)
+    return ([(a + c * T_clip, b + c * T_clip) for c in clips for a, b in runs],
+            [[p + i * n for p in row] for i in range(len(clips)) for row in remap])
 
 
 def _reversed_flags(reversed_groups, G: int) -> List[bool]:
@@ -213,8 +227,9 @@ class CoTrackerThreeBase(nn.Module):
         if is_train:
             raise NotImplementedError("cotracker_b200 is inference-only (training is out of scope, SURVEY.md §2)")
         B, T, C, H, W = video.shape
-        if B != 1 or queries.shape[0] != 1:
-            raise ValueError("CoTracker3 inference requires B == 1 (the reference fails for B > 1 as well)")
+        if B < 1 or queries.dim() != 3 or queries.shape[0] != B:
+            raise ValueError(f"video [B,T,3,H,W] and queries [B,N,3] must hold the same B >= 1 clips, got "
+                             f"{tuple(video.shape)} and {tuple(queries.shape)}")
         assert H % self.stride == 0 and W % self.stride == 0
         if not video.is_cuda:
             raise engine.EngineError("cotracker_b200 runs on CUDA only; move the module and inputs to a GPU")
@@ -256,8 +271,10 @@ class CoTrackerThreeBase(nn.Module):
 
     # -- internal entry points of the predictors: frames already resized and normalised (cotracker_b200.ingest) --------
     def _check_frames(self, frames, queries):
-        if frames.dim() != 4 or frames.shape[1] != 3 or queries.shape[0] != 1:
-            raise ValueError("frames must be [T,3,H,W] and queries [1,N,3] (B == 1)")
+        B = queries.shape[0] if queries.dim() == 3 else 0
+        if frames.dim() != 4 or frames.shape[1] != 3 or B < 1 or frames.shape[0] % B or frames.shape[0] < B:
+            raise ValueError(f"frames must be [B*T,3,H,W] (clip after clip) and queries [B,N,3], got "
+                             f"{tuple(frames.shape)} and {tuple(queries.shape)}")
         if not frames.is_cuda:
             raise engine.EngineError("cotracker_b200 runs on CUDA only; move the module and inputs to a GPU")
         assert frames.shape[2] % self.stride == 0 and frames.shape[3] % self.stride == 0
@@ -266,11 +283,13 @@ class CoTrackerThreeBase(nn.Module):
         """Frames the model appends (copies of the last frame) before encoding a T-frame clip."""
         return 0
 
-    def _encode_clip(self, frames, fmaps_chunk_size=200) -> torch.Tensor:
-        """frames [T,3,H,W] in [-1,1] -> the pyramid `_track_pyramid` expects (with the model's padding frames)."""
-        pad = self._clip_pad(frames.shape[0])
+    def _encode_clip(self, frames, fmaps_chunk_size=200, B: int = 1) -> torch.Tensor:
+        """frames [B*T,3,H,W] in [-1,1], clip after clip -> the pyramid `_track_pyramid` expects: every clip's frames
+        followed by the model's padding frames, in one encoder pass."""
+        pad = self._clip_pad(frames.shape[0] // B)
         if pad > 0:
-            frames = torch.cat([frames, frames[-1:].expand(pad, -1, -1, -1)], 0)
+            v = frames.unflatten(0, (B, -1))
+            frames = torch.cat([v, v[:, -1:].expand(-1, pad, -1, -1, -1)], 1).flatten(0, 1)
         return self._encode(frames.contiguous(), fmaps_chunk_size)
 
     def _reverse_clip_pyramid_(self, pyr, T: int, H: int, W: int) -> torch.Tensor:
@@ -279,11 +298,33 @@ class CoTrackerThreeBase(nn.Module):
         return engine.reverse_pyramid_(pyr, T, H // self.stride, W // self.stride, self._clip_pad(T))
 
     def _track_frames(self, frames, queries, iters=4, group_sizes=None, fmaps_chunk_size=200):
-        """`forward` on frames [T,3,H,W] already scaled to [-1,1] (the predictors' path)."""
+        """`forward` on frames [B*T,3,H,W] (clip after clip) already scaled to [-1,1] (the predictors' path)."""
         self._check_frames(frames, queries)
-        T, _, H, W = frames.shape
-        return self._track_pyramid(self._encode_clip(frames, fmaps_chunk_size), T, H, W, queries, iters,
+        B = queries.shape[0]
+        BT, _, H, W = frames.shape
+        return self._track_pyramid(self._encode_clip(frames, fmaps_chunk_size, B), BT // B, H, W, queries, iters,
                                    group_sizes or [queries.shape[1]])
+
+    # -- batches: B clips in one pyramid, tracks and groups clip after clip ---------------------------------------------
+    @staticmethod
+    def _pass_clips(B: int, clips):
+        """(clips a pass tracks, whether it is today's one-clip pass that needs neither clip offsets nor a frame map)."""
+        if clips is None:
+            return list(range(B)), B == 1
+        clips = [int(c) for c in clips]
+        if len(clips) != B:
+            raise engine.EngineError(f"{B} query sets for clips {clips}")
+        return clips, False
+
+    @staticmethod
+    def _clip_offsets(clips, T_clip: int, N: int, device) -> torch.Tensor:
+        """[B*N] int64: the first pyramid frame of each track's clip."""
+        return torch.tensor([c * T_clip for c in clips], dtype=torch.int64).repeat_interleave(N).to(device)
+
+    @staticmethod
+    def _batched(x: torch.Tensor, B: int) -> torch.Tensor:
+        """[T, B*N, ...] (tracks clip after clip) -> [B, T, N, ...]; no copy for B = 1."""
+        return x.unflatten(1, (B, -1)).transpose(0, 1).contiguous()
 
 
 class CoTrackerThreeOffline(CoTrackerThreeBase):
@@ -297,28 +338,38 @@ class CoTrackerThreeOffline(CoTrackerThreeBase):
     def _track(self, video, queries, iters, fmaps_chunk_size, group_sizes, reversed_groups=None):
         B, T, C, H, W = video.shape
         assert T >= 1
-        frames = 2.0 * (video[0].float() / 255.0) - 1.0
+        frames = 2.0 * (video.flatten(0, 1).float() / 255.0) - 1.0
         pyr = self._encode(frames, fmaps_chunk_size)
         return self._track_pyramid(pyr, T, H, W, queries, iters, group_sizes, reversed_groups)
 
-    def _track_pyramid(self, pyr, T, H, W, queries, iters, group_sizes, reversed_groups=None):
-        """The model after the encoder: pyr = the clip's pyramid (`_encode_clip`), T frames of H x W pixels.
-        reversed_groups: G flags; a flagged group tracks the clip played backwards (see `forward_groups`)."""
-        N = queries.shape[1]
+    def _track_pyramid(self, pyr, T, H, W, queries, iters, group_sizes, reversed_groups=None, clips=None):
+        """The model after the encoder: pyr = the pyramid of the clips (`_encode_clip`), T frames of H x W pixels each.
+        group_sizes, reversed_groups: the G groups of one clip's N queries (every clip has the same), G flags; a
+        flagged group tracks the clip played backwards (see `forward_groups`).
+        clips: the clip of the pyramid each of the B rows of `queries` tracks (None: 0 .. B-1, the whole pyramid)."""
+        B, N = queries.shape[:2]
+        dev = pyr.device
         H4, W4 = H // self.stride, W // self.stride
+        group_sizes = list(group_sizes)
         flags = _reversed_flags(reversed_groups, len(group_sizes))
-        qframes = queries[0, :, 0].long()
+        clips, plain = self._pass_clips(B, clips)
+        qframes = queries[:, :, 0].long().reshape(-1)
         if any(flags):   # a reversed group's query frame q is frame T-1-q of the forward pyramid
-            qframes = torch.where(self._track_reversed(group_sizes, flags, qframes.device), T - 1 - qframes, qframes)
+            qframes = torch.where(self._track_reversed(group_sizes * B, flags * B, dev), T - 1 - qframes, qframes)
+        if not plain:
+            qframes = qframes + self._clip_offsets(clips, T, N, dev)
         qframes = qframes.to(torch.int32).contiguous()
-        qcoords = (queries[0, :, 1:3].float() / self.stride).contiguous()
-        support = engine.sample_support(pyr, T, H4, W4, qframes, qcoords)
-        coords = qcoords[None].expand(T, N, 2).contiguous()
-        vis = torch.zeros(T, N, device=pyr.device)
-        conf = torch.zeros(T, N, device=pyr.device)
-        self._refine(pyr, H4, W4, support, None, coords, vis, conf, iters, group_sizes,
-                     clip_frame_map(T, flags) if any(flags) else None)
-        return (coords * float(self.stride))[None], torch.sigmoid(vis)[None], torch.sigmoid(conf)[None], None
+        qcoords = (queries[:, :, 1:3].float() / self.stride).reshape(-1, 2).contiguous()
+        support = engine.sample_support(pyr, T if plain else engine.pyramid_frames(pyr, H4, W4), H4, W4, qframes, qcoords)
+        coords = qcoords[None].expand(T, B * N, 2).contiguous()
+        vis = torch.zeros(T, B * N, device=dev)
+        conf = torch.zeros(T, B * N, device=dev)
+        frame_map = clip_frame_map(T, flags) if any(flags) or not plain else None
+        if not plain:
+            frame_map = batch_frame_map(frame_map, clips, T)
+        self._refine(pyr, H4, W4, support, None, coords, vis, conf, iters, group_sizes * B, frame_map)
+        return (self._batched(coords * float(self.stride), B), self._batched(torch.sigmoid(vis), B),
+                self._batched(torch.sigmoid(conf), B), None)
 
 
 class CoTrackerThreeOnline(CoTrackerThreeBase):
@@ -326,26 +377,43 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
 
     def init_video_online_processing(self):
         self.online_ind = 0
-        self.online_track_support = None          # [4,49,N,128], accumulated as queries enter the window
-        self.online_coords_predicted = None
-        self.online_vis_predicted = None
-        self.online_conf_predicted = None
-        self._online_enc_cache = None             # (per-frame checksums, pyramid) of the previous chunk
+        # The state of B streams that advance in lockstep holds the tracks clip after clip, as the update loop does:
+        self.online_track_support = None          # [4,49,B*N,128], accumulated as queries enter the window
+        self.online_coords_predicted = None       # [T,B*N,2]
+        self.online_vis_predicted = None          # [T,B*N]
+        self.online_conf_predicted = None         # [T,B*N]
+        self._online_enc_cache = None             # ([B,S,2] per-frame checksums, chunk shape, pyramid) of the last chunk
 
-    def _encode_online(self, frames, chunk, step, H4, W4):
-        """Consecutive online chunks overlap by window_len - step frames and the encoder is strictly per-frame
-        (InstanceNorm statistics are per sample), so the features of the overlap are reused bit-for-bit from the
-        previous call and only the new frames are encoded (SURVEY.md 8(f1): the reference re-encodes all 16)."""
-        S = frames.shape[0]
+    def _encode_online(self, frames, chunk, step, H4, W4, B=1):
+        """frames [B*S,3,H,W]: the S-frame chunks of the B streams.  Consecutive online chunks overlap by window_len -
+        step frames and the encoder is strictly per-frame (InstanceNorm statistics are per sample), so the features of
+        the overlap are reused bit-for-bit from the previous call and only the new frames are encoded (SURVEY.md 8(f1):
+        the reference re-encodes all 16).  A stream whose overlap does not match its cache is encoded whole, in the
+        same encoder pass as the other streams' new frames."""
+        S = frames.shape[0] // B
         keep = S - step
         cache = getattr(self, "_online_enc_cache", None)
-        sig = self._frame_signatures(frames)           # [S,2] float64: one pass over the chunk, 16 numbers to the host
+        # [B,S,2] float64: one pass over the chunk, 16 numbers per stream to the host
+        sig = self._frame_signatures(frames).unflatten(0, (B, S))
         pyr = None
         if cache is not None and self.online_ind > 0 and keep > 0:
             prev_sig, prev_shape, prev_pyr = cache
-            if prev_shape == frames.shape and torch.equal(sig[:keep], prev_sig[step:]):
-                new = self._encode(frames[keep:].contiguous(), chunk)
-                pyr = engine.concat_pyramid_frames(prev_pyr, S, step, new, S - keep, H4, W4)
+            same = [False] * B
+            if prev_shape == frames.shape and prev_sig.shape == sig.shape:
+                same = (sig[:, :keep] == prev_sig[:, step:]).flatten(1).all(1).tolist()
+            if any(same):
+                v = frames.unflatten(0, (B, S))
+                fresh = [v[b, keep:] if same[b] else v[b] for b in range(B)]
+                fresh = fresh[0] if B == 1 else torch.cat(fresh, 0)
+                new = self._encode(fresh.contiguous(), chunk)
+                runs, n = [], 0
+                for b in range(B):
+                    if same[b]:
+                        runs.append((prev_pyr, B * S, b * S + step, (b + 1) * S))
+                    k = step if same[b] else S
+                    runs.append((new, fresh.shape[0], n, n + k))
+                    n += k
+                pyr = engine.concat_pyramid_runs(runs, H4, W4)
         if pyr is None:
             pyr = self._encode(frames, chunk)
         self._online_enc_cache = (sig, frames.shape, pyr)
@@ -377,7 +445,7 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
         return (S - T % S) % S
 
     def _track(self, video, queries, iters, fmaps_chunk_size, group_sizes, is_online=False, reversed_groups=None):
-        frames = 2.0 * (video[0].float() / 255.0) - 1.0
+        frames = 2.0 * (video.flatten(0, 1).float() / 255.0) - 1.0
         return self._track_normalised(frames, queries, iters, fmaps_chunk_size, group_sizes, is_online, reversed_groups)
 
     def _track_frames(self, frames, queries, iters=4, group_sizes=None, fmaps_chunk_size=200, is_online=False):
@@ -386,25 +454,36 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
                                       is_online)
 
     def _track_normalised(self, frames, queries, iters, fmaps_chunk_size, group_sizes, is_online, reversed_groups=None):
-        T, _, H, W = frames.shape
+        """frames [B*T,3,H,W], clip after clip, B = queries.shape[0]."""
+        B = queries.shape[0]
+        BT, _, H, W = frames.shape
+        T = BT // B
         S = self.window_len
         assert S >= 2
         if is_online:
             assert T <= S, "Online mode: video chunk must be <= window size."
             assert getattr(self, "online_ind", None) is not None, "Call model.init_video_online_processing() first."
             H4, W4 = H // self.stride, W // self.stride
-            frames = torch.cat([frames, frames[-1:].expand(S - T, -1, -1, -1)], 0) if S > T else frames
-            pyr_all = self._encode_online(frames, fmaps_chunk_size, S // 2, H4, W4)
+            if S > T:
+                v = frames.unflatten(0, (B, T))
+                frames = torch.cat([v, v[:, -1:].expand(-1, S - T, -1, -1, -1)], 1).flatten(0, 1)
+            pyr_all = self._encode_online(frames, fmaps_chunk_size, S // 2, H4, W4, B)
         else:
-            pyr_all = self._encode_clip(frames, fmaps_chunk_size)
+            pyr_all = self._encode_clip(frames, fmaps_chunk_size, B)
         return self._track_pyramid(pyr_all, T, H, W, queries, iters, group_sizes, is_online, reversed_groups)
 
-    def _track_pyramid(self, pyr_all, T, H, W, queries, iters, group_sizes, is_online=False, reversed_groups=None):
-        """The model after the encoder: pyr_all = the pyramid of the T frames and the padding (`_encode_clip`).
-        reversed_groups: G flags; a flagged group tracks the clip played backwards (see `forward_groups`).  Each window
-        then runs on the frames its groups reference (at most 2 S), gathered from pyr_all, through a frame map."""
+    def _track_pyramid(self, pyr_all, T, H, W, queries, iters, group_sizes, is_online=False, reversed_groups=None,
+                       clips=None):
+        """The model after the encoder: pyr_all = the pyramid of the clips, each T frames and the padding
+        (`_encode_clip`).  group_sizes, reversed_groups: the G groups of one clip's N queries (every clip has the same),
+        G flags; a flagged group tracks the clip played backwards (see `forward_groups`).  With reversed groups or more
+        than one clip each window runs on the frames its groups reference (at most 2 S per clip), gathered from
+        pyr_all, through a frame map.
+        clips: the clip of the pyramid each of the B rows of `queries` tracks (None: 0 .. B-1, the whole pyramid).
+        Below, N counts the tracks of all B clips, clip after clip."""
         dev = pyr_all.device
-        N = queries.shape[1]
+        B = queries.shape[0]
+        N = B * queries.shape[1]
         S = self.window_len
         step = S // 2
         H4, W4 = H // self.stride, W // self.stride
@@ -412,8 +491,15 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
         flags = _reversed_flags(reversed_groups, len(group_sizes))
         if is_online and any(flags):
             raise NotImplementedError("streaming (is_online=True) does not track reversed groups")
-        qframes_l = queries[0, :, 0].long()
-        qcoords = (queries[0, :, 1:3].float() / self.stride).contiguous()
+        clips, plain = self._pass_clips(B, clips)
+        if is_online and clips != list(range(B)):
+            raise NotImplementedError("streaming (is_online=True) advances every stream of the batch together")
+        T_all = T_pad if plain else engine.pyramid_frames(pyr_all, H4, W4)
+        clip_off = None if plain else self._clip_offsets(clips, T_pad, queries.shape[1], dev)
+        G1 = len(flags)                                   # groups of one clip
+        group_sizes, flags = list(group_sizes) * B, flags * B
+        qframes_l = queries[:, :, 0].long().reshape(-1)
+        qcoords = (queries[:, :, 1:3].float() / self.stride).reshape(-1, 2).contiguous()
 
         coords_pred = torch.zeros(T, N, 2, device=dev)
         vis_pred = torch.zeros(T, N, device=dev)
@@ -431,15 +517,19 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
             entering = ((qframes_l >= left) & (qframes_l < right)).to(torch.uint8).contiguous()
             if self.online_track_support is None:
                 self.online_track_support = torch.zeros(4, 49, N, 128, device=dev)
-            rel = (qframes_l - self.online_ind).clamp(0, T_pad - 1).to(torch.int32).contiguous()
-            engine.sample_support(pyr_all, T_pad, H4, W4, rel, qcoords, support=self.online_track_support,
-                                  accumulate_mask=entering)
+            rel = (qframes_l - self.online_ind).clamp(0, T_pad - 1)
+            if not plain:
+                rel = rel + clip_off
+            engine.sample_support(pyr_all, T_all, H4, W4, rel.to(torch.int32).contiguous(), qcoords,
+                                  support=self.online_track_support, accumulate_mask=entering)
             support = self.online_track_support
         else:
             qf = qframes_l.clamp(0, T_pad - 1)
             if any(flags):   # frame q of the reversed, padded clip is forward frame max(T-1-q, 0)
                 qf = torch.where(self._track_reversed(group_sizes, flags, dev), (T - 1 - qf).clamp(min=0), qf)
-            support = engine.sample_support(pyr_all, T_pad, H4, W4, qf.to(torch.int32).contiguous(), qcoords)
+            if not plain:
+                qf = qf + clip_off
+            support = engine.sample_support(pyr_all, T_all, H4, W4, qf.to(torch.int32).contiguous(), qcoords)
 
         coords_init = qcoords[None].expand(S, N, 2).contiguous()
         vis_init = torch.zeros(S, N, device=dev)
@@ -464,10 +554,12 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
             valid = (qframes_l < ind + S).to(torch.uint8).contiguous()                      # reference :484,:493-496
             frame_map = None
             if is_online:
-                pyr = pyr_all
-            elif any(flags):
-                runs, frame_map = gather_plan(window_frame_map(T, S, ind, flags))
-                pyr = gather_pyramid(pyr_all, T_pad, H4, W4, runs)
+                pyr = pyr_all       # the S-frame chunks of the streams, one after another
+                if not plain:
+                    frame_map = batch_frame_map([list(range(S))] * G1, clips, S)
+            elif any(flags) or not plain:
+                runs, frame_map = batch_gather_plan(window_frame_map(T, S, ind, flags[:G1]), clips, T_pad)
+                pyr = gather_pyramid(pyr_all, T_all, H4, W4, runs)
             else:
                 pyr = engine.slice_pyramid(pyr_all, T_pad, H4, W4, ind, S)
             coords = coords_init.clone().contiguous()
@@ -484,4 +576,5 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
             self.online_coords_predicted = coords_pred
             self.online_vis_predicted = vis_pred
             self.online_conf_predicted = conf_pred
-        return coords_pred[None], torch.sigmoid(vis_pred)[None], torch.sigmoid(conf_pred)[None], None
+        return (self._batched(coords_pred, B), self._batched(torch.sigmoid(vis_pred), B),
+                self._batched(torch.sigmoid(conf_pred), B), None)

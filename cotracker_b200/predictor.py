@@ -6,15 +6,19 @@
 Same constructor arguments, call signatures, return types ((tracks[B,T,N,2] float32 in input pixels,
 visibility[B,T,N] bool)), attributes (`model`, `interp_shape`, `support_grid_size`, `step`) and online state
 machine.  The model behind it is `cotracker_b200.model` whose update loop runs in libct3_b200.so.
+
+B clips of one length and size are tracked together (the reference fails for B > 1): one resize, one encoder pass and,
+memory permitting, one update-loop pass for the whole batch; slot b of the result is bit-identical to the call on
+`video[b:b+1]` (and `queries[b:b+1]`).  `segm_mask` keeps a different number of points per clip and is for B = 1 only.
 """
 from __future__ import annotations
 
 import torch
 import torch.nn.functional as F
 
-from . import ingest
+from . import engine, ingest
 from .build import build_cotracker
-from .evaluation import pass_budget_bytes, plan_dense_passes
+from .evaluation import pass_budget_bytes, plan_clip_passes, plan_dense_passes
 
 # Backward tracking runs the forward and the reversed queries as two groups of one update-loop pass while one direction
 # has at most this many tracks x loop frames, and as two passes above it.  Measured on an H100 (DESIGN.md 4.4.2): one
@@ -49,6 +53,8 @@ class CoTrackerPredictor(torch.nn.Module):
     @torch.no_grad()
     def forward(self, video, queries: torch.Tensor = None, segm_mask: torch.Tensor = None, grid_size: int = 0,
                 grid_query_frame: int = 0, backward_tracking: bool = False):
+        if segm_mask is not None and video.shape[0] != 1:
+            raise ValueError("segm_mask keeps a different number of grid points per clip: it needs B == 1")
         if queries is None and grid_size == 0:
             return self._compute_dense_tracks(video, grid_query_frame=grid_query_frame,
                                               backward_tracking=backward_tracking)
@@ -113,7 +119,7 @@ class CoTrackerPredictor(torch.nn.Module):
 
     def _model_queries(self, clip, video_shape, queries, segm_mask=None, grid_size=0, add_support_grid=False,
                        grid_query_frame=0):
-        """The queries [1,N,3] at model resolution (reference :100-160), support grid appended."""
+        """The queries [B,N,3] at model resolution (reference :100-160), support grid appended."""
         B, T, C, H, W = video_shape
         ih, iw = self.interp_shape
         dev = clip.device
@@ -141,30 +147,11 @@ class CoTrackerPredictor(torch.nn.Module):
         (reference :187-209), support grid dropped, query points pinned, scaled to the input (reference :161-190)."""
         B, T, C, H, W = video_shape
         ih, iw = self.interp_shape
-        n_support = self.support_grid_size ** 2
-        tracks, visibilities = fwd
-        if bwd is not None:
-            inv_tracks, inv_vis = bwd[0].flip(1), bwd[1].flip(1)
-            before_query = torch.arange(T, device=queries.device)[None, :, None] < queries[:, None, :, 0]
-            tracks = torch.where(before_query[..., None], inv_tracks, tracks)
-            visibilities = torch.where(before_query, inv_vis, visibilities)
-            if add_support_grid:
-                queries[:, -n_support:, 0] = T - 1
-        if add_support_grid:
-            tracks = tracks[:, :, :-n_support]
-            visibilities = visibilities[:, :, :-n_support]
-        visibilities = visibilities > 0.9
-
-        # query points are, by definition, where they were asked for and visible (reference :173-185)
-        n = tracks.size(2)
-        idx = torch.arange(n, device=tracks.device)
-        for b in range(len(queries)):
-            qt = queries[b, :n, 0].to(torch.int64)
-            tracks[b, qt, idx] = queries[b, :n, 1:]
-            visibilities[b, qt, idx] = True
-
-        tracks *= tracks.new_tensor([(W - 1) / (iw - 1), (H - 1) / (ih - 1)])
-        return tracks, visibilities
+        n_keep = queries.shape[1] - (self.support_grid_size ** 2 if add_support_grid else 0)
+        # query points are, by definition, where they were asked for and visible (reference :173-185); one kernel
+        fwd, bwd = [None if p is None else (p[0].contiguous(), p[1].contiguous()) for p in (fwd, bwd)]
+        return engine.finish_tracks(fwd, bwd, queries.float().contiguous(), n_keep, 0.9,
+                                    ((W - 1) / (iw - 1), (H - 1) / (ih - 1)))
 
 
 def _reversed_queries(queries, T: int):
@@ -175,8 +162,9 @@ def _reversed_queries(queries, T: int):
 
 
 class _EncodedClip:
-    """One predictor call's clip, resized + normalised (cotracker_b200.ingest) and encoded once; every model pass of
-    the call (dense offsets, backward tracking) runs on this one pyramid.  A pass on the clip played backwards is a
+    """One predictor call's clips (a batch of B), resized + normalised (cotracker_b200.ingest) and encoded once into
+    one pyramid; every model pass of the call (dense offsets, backward tracking, the sub-batches of a batch that does
+    not fit in device memory at once) runs on this one pyramid.  A pass on the clip played backwards is a
     reversed query group (model `reversed_groups`): it reads the forward pyramid through a frame map, so device memory
     never holds a second pyramid and the pyramid is never reversed."""
 
@@ -185,17 +173,29 @@ class _EncodedClip:
     def __init__(self, model, video, interp_shape):
         frames = ingest.prepare_video(video, interp_shape, ingest.model_device(model))
         self.model, self.device = model, frames.device
-        self.T, _, self.H, self.W = frames.shape
-        self.pyr = model._encode_clip(frames)
+        self.B = video.shape[0]
+        BT, _, self.H, self.W = frames.shape
+        self.T = BT // self.B
+        self.pyr = model._encode_clip(frames, B=self.B)
 
     def track_groups(self, groups, reversed_groups):
-        """Query groups [1,n_g,3] (model resolution) in one pass; a flagged group tracks the clip played backwards,
-        with query frames in reversed-clip time.  -> [(tracks [1,T,n_g,2], visibility [1,T,n_g])] per group."""
-        if any(q.shape[0] != 1 for q in groups):
-            raise ValueError("CoTracker3 inference requires B == 1 (the reference fails for B > 1 as well)")
+        """Query groups [B,n_g,3] (model resolution) of every clip in one pass, or, when the batch does not fit in
+        device memory, in one pass per sub-batch of clips (`plan_clip_passes`; groups are independent, so the split
+        does not change a bit).  A flagged group tracks the clip played backwards, with query frames in reversed-clip
+        time.  -> [(tracks [B,T,n_g,2], visibility [B,T,n_g])] per group."""
+        if any(q.shape[0] != self.B for q in groups):
+            raise ValueError(f"every query group must hold the batch's {self.B} clips")
         sizes = [q.shape[1] for q in groups]
-        tr, vi, *_ = self.model._track_pyramid(self.pyr, self.T, self.H, self.W, torch.cat(groups, dim=1), self.ITERS,
-                                               sizes, reversed_groups=list(reversed_groups))
+        flags = list(reversed_groups)
+        queries = torch.cat(groups, dim=1)
+        passes = [(0, 1)]
+        if self.B > 1:
+            T_loop, H4, W4, budget, _ = self.pass_shape(any(flags))
+            passes = plan_clip_passes(self.B, sizes, T_loop, H4, W4, budget, lambda n: self.pass_frames(any(flags), n))
+        outs = [self.model._track_pyramid(self.pyr, self.T, self.H, self.W, queries[b0:b1], self.ITERS, sizes,
+                                          reversed_groups=flags, clips=None if len(passes) == 1 else range(b0, b1))[:2]
+                for b0, b1 in passes]
+        tr, vi = outs[0] if len(outs) == 1 else (torch.cat([o[i] for o in outs], dim=0) for i in range(2))
         out, a = [], 0
         for n in sizes:
             out.append((tr[:, :, a:a + n], vi[:, :, a:a + n]))
@@ -206,15 +206,22 @@ class _EncodedClip:
         """Frames of one update loop: the clip, or the window of the sliding-window model."""
         return self.model.window_len if hasattr(self.model, "init_video_online_processing") else self.T
 
+    def pass_frames(self, backward: bool, n_clips: int = 1):
+        """Pyramid frames a pass over n_clips clips reads through its frame map: the whole pyramid in place for the
+        one-window model, a gather of at most two windows per clip (one without reversed groups) for the sliding-window
+        model.  None: one clip without reversed groups has no frame map."""
+        if self.B == 1 and not backward:
+            return None
+        T_loop = self.loop_frames()
+        return self.B * self.T if T_loop == self.T else n_clips * (2 if backward else 1) * T_loop
+
     def pass_shape(self, backward: bool):
         """(T, H4, W4, budget, frames) of `plan_dense_passes`: one update loop's frames (the window of the
-        sliding-window model), the feature map, the free-memory budget of a pass and the pyramid frames a pass with
-        reversed groups reads (a window's gather holds at most two windows)."""
+        sliding-window model), the feature map, the free-memory budget of a pass and the pyramid frames a one-clip pass
+        reads (`pass_frames`)."""
         s = self.model.stride
-        T_loop = self.loop_frames()
-        frames = (self.T if T_loop == self.T else 2 * T_loop) if backward else None
-        budget = pass_budget_bytes(self.model, self.device, self.T, self.H, self.W)
-        return T_loop, self.H // s, self.W // s, budget, frames
+        budget = pass_budget_bytes(self.model, self.device, self.B * self.T, self.H, self.W)
+        return self.loop_frames(), self.H // s, self.W // s, budget, self.pass_frames(backward)
 
 
 class CoTrackerOnlinePredictor(torch.nn.Module):
@@ -245,15 +252,18 @@ class CoTrackerOnlinePredictor(torch.nn.Module):
                 queries[:, :, 1:] *= queries.new_tensor([(iw - 1) / (W - 1), (ih - 1) / (H - 1)])
                 if add_support_grid:
                     sup = get_points_on_a_grid(self.support_grid_size, self.interp_shape, device=dev)
-                    sup = torch.cat([torch.zeros_like(sup[:, :, :1]), sup], dim=2)
+                    sup = torch.cat([torch.zeros_like(sup[:, :, :1]), sup], dim=2).repeat(B, 1, 1)
                     queries = torch.cat([queries, sup], dim=1)
             elif grid_size > 0:
                 grid_pts = get_points_on_a_grid(grid_size, self.interp_shape, device=dev)
                 self.N = grid_size ** 2
                 queries = torch.cat([torch.ones_like(grid_pts[:, :, :1]) * grid_query_frame, grid_pts], dim=2)
+                queries = queries.repeat(B, 1, 1)
             self.queries = queries
             return (None, None)
 
+        if self.queries.shape[0] != B:   # the B streams of the first step advance together
+            raise ValueError(f"the video was started with {self.queries.shape[0]} streams, this chunk holds {B}")
         frames = ingest.prepare_video(video_chunk, self.interp_shape, dev)
         tracks, visibilities, confidence, __ = self.model._track_frames(frames, self.queries, iters=6, is_online=True)
         if add_support_grid:

@@ -17,7 +17,8 @@
  *   - every entry point returns 0 on success, a negative CT3_E* code otherwise,
  *     never throws / exits; ct3_last_error() returns a thread-local message;
  *   - all work is enqueued on the given cudaStream_t and is asynchronous w.r.t.
- *     the host; B (batch) is 1 as in the reference (cotracker3_offline.py:135,141).
+ *     the host; the update loop has no batch dimension (cotracker3_offline.py:135,141): a batch of clips is
+ *     more query groups of one ct3_update_loop_frames call, each reading its own frames of one pyramid.
  *
  * Symbols (all extern "C"):  see the declarations below; tests/test_host_logic.py checks
  * that the built library exports each of them.
@@ -110,6 +111,24 @@ int ct3_pack_weights(const float* const* tensors_host_array_of_device_ptrs, int 
 enum { CT3_FRAMES_U8 = 0, CT3_FRAMES_F32 = 1 };
 int ct3_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c,
                        int64_t stride_h, int64_t stride_w, int out_h, int out_w, float* out, ct3_stream_t stream);
+
+/* ---- the predictor's tail ---------------------------------------------------
+ * ct3_finish_tracks: what CoTrackerPredictor does with the model's output (predictor.py:161-209), for B clips in one
+ * kernel.  fwd_tracks [B,T,N,2] fp32 at model resolution and fwd_vis [B,T,N] fp32 visibility probabilities of the
+ * forward pass; bwd_tracks / bwd_vis: the same of the pass on the clip played backwards, in reversed-clip time (frame
+ * T-1-t is read for frame t), or both NULL; queries [B,N,3] fp32 (t, x, y) at model resolution.  Output element
+ * (b, t, i), i < n_keep (the N - n_keep trailing tracks, the support grid, are dropped):
+ *   the backward pass where (float)t < queries[b,i,0] and it is given, the forward pass elsewhere;
+ *   visibility = probability > threshold;
+ *   at t == (int64)queries[b,i,0] the track is the query point and visible (a query frame outside [0,T) pins nothing);
+ *   tracks * (scale_x, scale_y), one fp32 multiply each.
+ * tracks [B,T,n_keep,2] fp32, visibility [B,T,n_keep] uint8 (0 | 1), both contiguous and distinct from the inputs;
+ * bit-identical to the torch expression.  Null pointers, one of the backward pair without the other, B/T/N < 1, n_keep
+ * outside [1,N], track pointers not 8-byte aligned or more than 2^31 * 256 elements return CT3_EINVAL before any
+ * launch. */
+int ct3_finish_tracks(const float* fwd_tracks, const float* fwd_vis, const float* bwd_tracks, const float* bwd_vis,
+                      const float* queries, int B, int T, int N, int n_keep, float threshold, float scale_x,
+                      float scale_y, float* tracks, uint8_t* visibility, ct3_stream_t stream);
 
 /* ---- track visualiser (reference cotracker/utils/visualizer.py) ---------------
  * Frames are uint8 [T,H,W,3] contiguous on the device, drawn in place; every result is bit-identical to the reference's
