@@ -18,10 +18,8 @@ struct OptDef { const char* name; int lo, hi; };
 constexpr int kDefPrecCorr = 2, kDefPrecFc1 = 3;   // DESIGN.md section 2
 constexpr OptDef kOptDefs[OPT_COUNT] = {
     {"gemm", 0, 1},   // 0 wgmma, 1 SIMT verification
-    {"corr", 0, 3},   // 0 wgmma correlate-then-interpolate (corr_tc3.cu / corr_tc2.cu), 1 exact-fp32 SIMT, 2 corr_tc.cu,
-                      // 3 correlate-then-interpolate with corr_tc2.cu for every precision mode (A/B)
-    {"attn", 0, 2},   // 0 tensor-core kernels (wgmma point<-virtual, mma.sync elsewhere), 1 exact-fp32 SIMT verification,
-                      // 2 = mma.sync for point<-virtual too (A/B against attention_p2v.cu)
+    {"corr", 0, 2},   // 0 wgmma correlate-then-interpolate (corr_tc3.cu / corr_tc2.cu), 1 exact-fp32 SIMT, 2 corr_tc.cu
+    {"attn", 0, 1},   // 0 tensor-core kernels (wgmma point<-virtual, mma.sync elsewhere), 1 exact-fp32 SIMT verification
     // tensor-core products per FLOP of a GEMM group (DESIGN.md section 2): 3 = split x split (hi*hi + lo*hi + hi*lo),
     // 2 = fp16 activation plane x split fp16 weights, 1 = single fp16 product.  Only the correlation branch has the
     // switch: SURVEY 7.3 measured that every transformer GEMM breaks the 1e-3 px budget with fewer than 3 products.

@@ -207,7 +207,7 @@ struct Runner {
 int run_attention(Runner& R, const Workspace& W, const AttnParams& a, bool per_warp) {
   if (g_opt_attn == 1) return (int)launch_attention(a, R.s);
   // point <- virtual (64 keys per frame, thousands of queries): wgmma kernel with TMA row staging (attention_p2v.cu)
-  if (g_opt_attn == 0 && !per_warp && a.Lq > kV && attention_p2v_supported(a)) return (int)launch_attention_p2v(a, R.s);
+  if (!per_warp && a.Lq > kV && attention_p2v_supported(a)) return (int)launch_attention_p2v(a, R.s);
   return (int)launch_attention_tc(a, per_warp, W.att_part, num_sms(), R.s);
 }
 
@@ -399,11 +399,12 @@ int transformer_body(Runner& R, const Workspace& W, int T, int N, const GroupPla
 }
 
 // effective precision of the correlation branch for this thread's options: the single-plane / fewer-product modes
-// exist in corr_tc2.cu only, so whenever another correlation kernel runs the branch computes split x split
+// exist in the correlate-then-interpolate kernels only (corr_tc3.cu, corr_tc2.cu), so whenever another correlation
+// kernel runs the branch computes split x split
 struct Prec {
   int corr, fc1; bool patch;
   bool vol16() const { return fc1 < 3; }
-  bool support_major() const { return patch && corr != 3 && g_opt_corr == 0; }   // corr_tc3.cu writes k*49 + i
+  bool support_major() const { return patch && corr != 3; }   // corr_tc3.cu writes k*49 + i
 };
 Prec effective_prec(bool have_pyr_split, int T, int H4, int W4) {
   Prec p;
@@ -484,7 +485,6 @@ int check_groups(int T, int N, const int32_t* sizes, int G, int* total, bool n_f
   }
   if (sum > (int64_t)1 << 30) return fail(CT3_EINVAL, "problem too large%s");
   if (!n_from_sizes && sum != N) return fail(CT3_EINVAL, "group sizes must sum to N%s");
-  if (G > 1 && g_opt_attn == 2) return fail(CT3_EUNSUPPORTED, "grouped calls do not support attn = 2%s");
   *total = (int)sum;
   return check_TN(T, *total, G);
 }

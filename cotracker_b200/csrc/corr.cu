@@ -124,7 +124,7 @@ corr_sample_simt_kernel(CorrArgs g) {
 }  // namespace
 
 bool corr_uses_patch_kernel(int impl, bool have_pyr_split, int T, int H4, int W4) {
-  return (impl == 0 || impl == 3) && have_pyr_split && corr_patch_supported(T, H4, W4);
+  return impl == 0 && have_pyr_split && corr_patch_supported(T, H4, W4);
 }
 
 cudaError_t launch_corr_sample(const float* pyr, const __nv_bfloat16* pyr_split, int H4, int W4, const float* support,
@@ -132,11 +132,11 @@ cudaError_t launch_corr_sample(const float* pyr, const __nv_bfloat16* pyr_split,
                                __nv_bfloat16* vol_split, int impl, int mode, int vol16, int num_sms, cudaStream_t s,
                                int T_pyr, const FrameMap& fm) {
   if (corr_uses_patch_kernel(impl, pyr_split != nullptr, T_pyr, H4, W4)) {
-    if (impl == 0 && mode != 3)
+    if (mode != 3)
       return launch_corr_patch_t(pyr_split, H4, W4, support, track_valid, coords, T, N, vol_split, vol16, mode == 1,
                                  num_sms, s, T_pyr, fm);
-    return launch_corr_patch_tc(pyr_split, H4, W4, support, track_valid, coords, T, N, vol_split, mode, vol16, num_sms,
-                                s, T_pyr, fm);
+    return launch_corr_patch_tc(pyr_split, H4, W4, support, track_valid, coords, T, N, vol_split, vol16, num_sms, s,
+                                T_pyr, fm);
   }
   if (vol16) return cudaErrorInvalidValue;   // only the patch kernel writes the single-plane volume
   if (impl != 1)

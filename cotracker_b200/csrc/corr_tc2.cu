@@ -1,5 +1,6 @@
-// corr_tc2.cu -- correlate-then-interpolate form of the fused sampling + 4-D correlation (production path when
-// every pyramid level is at least 8x8 texels; corr_tc.cu covers smaller maps, corr.cu is the fp32 SIMT check).
+// corr_tc2.cu -- the split-bf16 (prec.corr = 3) kernel of the correlate-then-interpolate form of the fused sampling +
+// 4-D correlation (every pyramid level at least 8x8 texels; corr_tc3.cu runs prec.corr 1 and 2, corr_tc.cu covers
+// smaller maps, corr.cu is the fp32 SIMT check).
 //
 //   vol[(n,t,l)][(a*7+b)*49 + k] = < bilinear(F_l[t], cx/2^l + a-3, cy/2^l + b-3) , S_l[n, k, :] >
 //   (get_correlation_feat + einsum, cotracker3_online.py:130-143, cotracker3_offline.py:144-156)
@@ -40,29 +41,22 @@ constexpr int TMA_WARP = 0;               // warp 1 idle
 constexpr int SB_WARP0 = 2;               // 2 support-builder warps
 constexpr int EPI_WARP0 = 4;              // warps 4..7 group 0, 8..11 group 1: each a warpgroup, MMA (wgmma) + epilogue
 constexpr int THREADS = 12 * 32;
-// Precision modes (products per correlation FLOP; DESIGN.md section 2):
-//   MODE 3: texels split bf16 hi|lo, support split bf16: A_hi x [S_hi;S_lo] + A_lo x S_hi      (rel. err ~2^-17)
-//   MODE 2: texels ONE fp16 plane (rounded, 2^-12), support split fp16: A x [S_hi;S_lo] as one N=128 MMA
-//   MODE 1: texels one fp16 plane, support one fp16 plane: A x S_hi (N=64)
-// MODE <= 2 halves the bytes every tile pulls through the L2->SM path (the resource this kernel saturates:
-// 64 KiB per 2-frame tile in MODE 3) and doubles the tiles in flight for the same 64 KiB ring.
+// Precision (products per correlation FLOP; DESIGN.md section 2): texels split bf16 hi|lo, support split bf16,
+// A_hi x [S_hi;S_lo] + A_lo x S_hi (rel. err ~2^-17).
 constexpr int A_PLANE = 16384;            // one 16-bit plane of a slot: [128 rows x 128 B]
-constexpr int A_RING = 65536;             // ring bytes: 2 slots of hi|lo (MODE 3) or 4 single-plane slots
-template <int MODE> struct Ring {
-  static constexpr int A_SLOT = MODE == 3 ? 2 * A_PLANE : A_PLANE;   // one K-half (64 channels) of a 2-frame tile
-  static constexpr int NSLOT = A_RING / A_SLOT;
-};
+constexpr int A_RING = 65536;             // ring bytes: 2 slots of hi|lo
+constexpr int A_SLOT = 2 * A_PLANE;       // one K-half (64 channels) of a 2-frame tile
+constexpr int NSLOT = A_RING / A_SLOT;
 // Tiles alternate between the two MMA + epilogue groups, and each group owns half of the ring: K-half kh of tile it
 // goes to slot (it & 1) * NSLOT/2 + u % (NSLOT/2), u = (it >> 1) * 2 + kh, in phase u / (NSLOT/2).  A slot is then only
 // ever consumed by one group, in order, so a parity wait can never alias a phase two completions ahead.
-template <int NSLOT>
 __device__ __forceinline__ void ring_slot(uint32_t it, int kh, int& sl, uint32_t& parity) {
   constexpr uint32_t SPG = NSLOT / 2;
   const uint32_t u = (it >> 1) * 2u + (uint32_t)kh;
   sl = (int)((it & 1u) * SPG + u % SPG);
   parity = (u / SPG) & 1u;
 }
-constexpr int MAX_NSLOT = 4;
+constexpr int BAR_STRIDE = 4;             // barrier words per ring array in the barrier block (>= NSLOT)
 constexpr int S_HALF = 2 * 8192;          // one K-half of S: [hi rows 0..63 | lo rows 64..127] x 128 B = one N=128 operand
 constexpr int S_BYTES = 2 * S_HALF;       // 32 KiB
 constexpr int H_A = 52;                   // floats per (texel row, a): 49 + pad, keeps every vector 16-byte aligned
@@ -126,19 +120,17 @@ __device__ __forceinline__ void tap_pair(float c, int off, int size, int origin,
   s1 = (w > 0.f) ? min(max(min(x0 + 1, size - 1) - origin, 0), 7) : s0;
 }
 
-template <int MODE, bool V16>
+template <bool V16>
 __global__ void __launch_bounds__(THREADS, 1)
 corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant__ Corr2Maps maps, int num_units) {
-  constexpr int NSLOT = Ring<MODE>::NSLOT, A_SLOT = Ring<MODE>::A_SLOT;
   constexpr int ROW_BYTES = V16 ? ROW_BYTES_H16 : ROW_BYTES_SPLIT;
-  constexpr bool F16 = MODE != 3;           // operand planes are IEEE fp16 (else bf16)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_align1024(smem_raw);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* a_full = bars;                  // [NSLOT] TMA -> MMA         (count 1 + tx bytes)
-  uint64_t* a_empty = bars + MAX_NSLOT;     // [NSLOT] MMA -> TMA         (one arrive per warp of the consuming group)
-  uint64_t* s_full = bars + 2 * MAX_NSLOT;      // builders -> MMA, per unit  (count 2)
-  uint64_t* s_empty = bars + 2 * MAX_NSLOT + 1; // MMA -> builders, per unit  (one arrive per warp of both groups)
+  uint64_t* a_empty = bars + BAR_STRIDE;    // [NSLOT] MMA -> TMA         (one arrive per warp of the consuming group)
+  uint64_t* s_full = bars + 2 * BAR_STRIDE;      // builders -> MMA, per unit  (count 2)
+  uint64_t* s_empty = bars + 2 * BAR_STRIDE + 1; // MMA -> builders, per unit  (one arrive per warp of both groups)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_per_unit = (g.T + 1) / 2;
@@ -183,7 +175,7 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
             for (int kh = 0; kh < 2; ++kh) {
               int sl;
               uint32_t par;
-              ring_slot<NSLOT>(it, kh, sl, par);
+              ring_slot(it, kh, sl, par);
               if (kh == 0) TRACE(it, 0);
               mbar_wait_spin(&a_empty[sl], par ^ 1u);
               if (kh == 0) TRACE(it, 1);
@@ -199,7 +191,7 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
                 if (f < nf) {
                   const int bx = f ? bx1 : bx0, by = f ? by1 : by0;
 #pragma unroll
-                  for (int pl = 0; pl < (MODE == 3 ? 2 : 1); ++pl)
+                  for (int pl = 0; pl < 2; ++pl)
                     tma_load_4d(dst + pl * A_PLANE + f * 8192, &maps.m[l], kh * 64, bx, by,
                                 pl * g.T_pyr + map_frame(frow, t0 + k + f), &a_full[sl]);
                 }
@@ -233,13 +225,8 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
         const int p = sb + 2 * j;
         if (p < kP) {
           uint32_t h0, l0, h1, l1;
-          if (F16) {
-            split2_h(rows[j].x, rows[j].y, h0, l0);
-            split2_h(rows[j].z, rows[j].w, h1, l1);
-          } else {
-            split2(rows[j].x, rows[j].y, h0, l0);
-            split2(rows[j].z, rows[j].w, h1, l1);
-          }
+          split2(rows[j].x, rows[j].y, h0, l0);
+          split2(rows[j].z, rows[j].w, h1, l1);
           const uint32_t off = (uint32_t)(atom * S_HALF) + sw128(p, chunk) + (uint32_t)(half * 8);
           *reinterpret_cast<uint2*>(s_hi + off) = make_uint2(h0, h1);          // rows 0..63 of the K-half: hi plane
           *reinterpret_cast<uint2*>(s_hi + 8192 + off) = make_uint2(l0, l1);   // rows 64..127: lo plane
@@ -283,15 +270,14 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
         if ((int)(it & 1u) != grp) continue;
         {
           // D[texel row][k] over both K-halves: A x [S_hi ; S_lo] as ONE N=128 MMA (columns 0..63 += A_hi S_hi,
-          // 64..127 += A_hi S_lo), then A_lo x S_hi (N=64) on columns 0..63 (MODE 3); the halves are added in
-          // registers, so the tile handed to the epilogue is [128 rows][64 columns]
-          constexpr int NN = MODE == 1 ? 64 : 128;
-          float d0[NN / 2], d1[NN / 2];
+          // 64..127 += A_hi S_lo), then A_lo x S_hi (N=64) on columns 0..63; the halves are added in registers, so
+          // the tile handed to the epilogue is [128 rows][64 columns]
+          float d0[64], d1[64];
 #pragma unroll
           for (int kh = 0; kh < 2; ++kh) {
             int sl;
             uint32_t par;
-            ring_slot<NSLOT>(it, kh, sl, par);
+            ring_slot(it, kh, sl, par);
             mbar_wait(&a_full[sl], par);
             if (kh == 0) TRACE(it, 2);
             wgmma_fence();
@@ -300,12 +286,10 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
             for (int j = 0; j < 4; ++j) {
               const uint64_t ds = gmma_desc_sw128(s_base + (uint32_t)(kh * S_HALF + j * 32));
               const uint32_t first = (kh | j) != 0 ? 1u : 0u;
-              wgmma_tile<NN, F16>(d0, gmma_desc_sw128(a_base + j * 32), ds, first);
-              wgmma_tile<NN, F16>(d1, gmma_desc_sw128(a_base + 8192 + j * 32), ds, first);
-              if constexpr (MODE == 3) {
-                wgmma_m64n64_bf16_head(d0, gmma_desc_sw128(a_base + A_PLANE + j * 32), ds, 1u);
-                wgmma_m64n64_bf16_head(d1, gmma_desc_sw128(a_base + A_PLANE + 8192 + j * 32), ds, 1u);
-              }
+              wgmma_tile<128, false>(d0, gmma_desc_sw128(a_base + j * 32), ds, first);
+              wgmma_tile<128, false>(d1, gmma_desc_sw128(a_base + 8192 + j * 32), ds, first);
+              wgmma_m64n64_bf16_head(d0, gmma_desc_sw128(a_base + A_PLANE + j * 32), ds, 1u);
+              wgmma_m64n64_bf16_head(d1, gmma_desc_sw128(a_base + A_PLANE + 8192 + j * 32), ds, 1u);
             }
             wgmma_commit();
             wgmma_wait0(d0);
@@ -316,8 +300,8 @@ corr_patch_tc_kernel(const __grid_constant__ Corr2Args g, const __grid_constant_
           float o0[32], o1[32];
 #pragma unroll
           for (int i = 0; i < 32; ++i) {
-            o0[i] = NN == 128 ? d0[i] + d0[(i + 32) % (NN / 2)] : d0[i];
-            o1[i] = NN == 128 ? d1[i] + d1[(i + 32) % (NN / 2)] : d1[i];
+            o0[i] = d0[i] + d0[i + 32];
+            o1[i] = d1[i] + d1[i + 32];
           }
           asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");   // the previous tile's rows have been read
           acc_store<64>(o0, acc_tile, ACC_LD);
@@ -491,7 +475,7 @@ split_level_kernel(const float4* __restrict__ in, uint2* __restrict__ hi, uint2*
   }
 }
 
-// fp32 channels-last level -> one fp16 plane (MODE 1 / 2), 4 channels per thread
+// fp32 channels-last level -> one fp16 plane (mode 1 / 2, read by corr_tc3.cu), 4 channels per thread
 __global__ void __launch_bounds__(256)
 half_level_kernel(const float4* __restrict__ in, uint2* __restrict__ out, int64_t n4) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
@@ -500,15 +484,15 @@ half_level_kernel(const float4* __restrict__ in, uint2* __restrict__ out, int64_
   }
 }
 
-template <int MODE, bool V16>
+template <bool V16>
 cudaError_t launch_variant(const Corr2Args& g, const Corr2Maps& maps, int num_units, int num_sms, cudaStream_t s) {
   static DeviceOnce attr;
   cudaError_t e = once_per_device(attr, [&] {
-    return cudaFuncSetAttribute(corr_patch_tc_kernel<MODE, V16>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    return cudaFuncSetAttribute(corr_patch_tc_kernel<V16>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   });
   if (e != cudaSuccess) return e;
   const int grid = num_units < num_sms ? num_units : num_sms;
-  corr_patch_tc_kernel<MODE, V16><<<grid, THREADS, SMEM_BYTES, s>>>(g, maps, num_units);
+  corr_patch_tc_kernel<V16><<<grid, THREADS, SMEM_BYTES, s>>>(g, maps, num_units);
   return cudaGetLastError();
 }
 
@@ -539,9 +523,8 @@ cudaError_t launch_split_pyramid(const float* pyr, int T, int H4, int W4, __nv_b
 
 cudaError_t launch_corr_patch_tc(const __nv_bfloat16* pyr_split, int H4, int W4, const float* support,
                                  const uint8_t* track_valid, const float* coords, int T, int N,
-                                 __nv_bfloat16* vol_split, int mode, int vol16, int num_sms, cudaStream_t s, int T_pyr,
+                                 __nv_bfloat16* vol_split, int vol16, int num_sms, cudaStream_t s, int T_pyr,
                                  const FrameMap& fm) {
-  if (mode < 1 || mode > 3) return cudaErrorInvalidValue;
   Corr2Args g;
   g.lay = pyramid_layout(T_pyr, H4, W4);
   g.support = support;
@@ -562,7 +545,7 @@ cudaError_t launch_corr_patch_tc(const __nv_bfloat16* pyr_split, int H4, int W4,
   for (int l = 0; l < kL; ++l) {
     const uint64_t W = (uint64_t)g.lay.w[l], H = (uint64_t)g.lay.h[l];
     if (W < 8 || H < 8) return cudaErrorInvalidValue;
-    const uint64_t dims[4] = {(uint64_t)kD, W, H, (uint64_t)((mode == 3 ? 2 : 1) * T_pyr)};   // dim 3 = plane*T_pyr + frame
+    const uint64_t dims[4] = {(uint64_t)kD, W, H, (uint64_t)(2 * T_pyr)};   // dim 3 = plane*T_pyr + frame
     const uint64_t strides[3] = {(uint64_t)kD * 2, W * kD * 2, H * W * kD * 2};
     const uint32_t box[4] = {64, 8, 8, 1};
     if (!encode_tensor_map(&maps.m[l], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, pyr_split + 2 * g.lay.off[l], dims, strides,
@@ -570,13 +553,8 @@ cudaError_t launch_corr_patch_tc(const __nv_bfloat16* pyr_split, int H4, int W4,
       return cudaErrorInvalidValue;
   }
   const int num_units = N * kL;
-  cudaError_t le;
-  if (vol16) le = mode == 3 ? launch_variant<3, true>(g, maps, num_units, num_sms, s)
-                : mode == 2 ? launch_variant<2, true>(g, maps, num_units, num_sms, s)
-                            : launch_variant<1, true>(g, maps, num_units, num_sms, s);
-  else       le = mode == 3 ? launch_variant<3, false>(g, maps, num_units, num_sms, s)
-                : mode == 2 ? launch_variant<2, false>(g, maps, num_units, num_sms, s)
-                            : launch_variant<1, false>(g, maps, num_units, num_sms, s);
+  const cudaError_t le = vol16 ? launch_variant<true>(g, maps, num_units, num_sms, s)
+                               : launch_variant<false>(g, maps, num_units, num_sms, s);
   if (le != cudaSuccess) return le;
 #ifdef CT3_TRACE
   {

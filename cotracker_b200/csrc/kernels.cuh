@@ -109,10 +109,10 @@ __device__ __forceinline__ int map_frame(const int32_t* row, int t) { return row
 // map is given)
 // impl: 0 tensor cores (correlate-then-interpolate when pyr_split is given and every level is >= 8x8: corr_tc3.cu for
 //         modes 2 / 1, corr_tc2.cu for mode 3; else corr_tc.cu),
-//       1 exact-fp32 SIMT, 2 corr_tc.cu always, 3 like 0 but corr_tc2.cu for every mode (A/B of the two kernels)
-// mode / vol16 apply to the corr_tc2.cu path only (corr_uses_patch_kernel): products per correlation FLOP (3|2|1;
-// pyr_split must have been made with the same mode) and a single-fp16-plane volume [N*T*4, kVolPad] instead of the
-// split one; the other kernels always compute in fp32 / bf16x3 and write the split volume.
+//       1 exact-fp32 SIMT, 2 corr_tc.cu always
+// mode / vol16 apply to the correlate-then-interpolate path only (corr_uses_patch_kernel): products per correlation
+// FLOP (3|2|1; pyr_split must have been made with the same mode) and a single-fp16-plane volume [N*T*4, kVolPad]
+// instead of the split one; the other kernels always compute in fp32 / bf16x3 and write the split volume.
 bool corr_uses_patch_kernel(int impl, bool have_pyr_split, int T, int H4, int W4);
 cudaError_t launch_corr_sample(const float* pyr, const __nv_bfloat16* pyr_split, int H4, int W4, const float* support,
                                const uint8_t* track_valid, const float* coords, int T, int N,
@@ -123,7 +123,7 @@ cudaError_t launch_corr_sample_tc(const float* pyr, int H4, int W4, const float*
                                   const uint8_t* track_valid, const float* coords, int T, int N,
                                   __nv_bfloat16* vol_split, int num_sms, cudaStream_t s, int T_pyr, const FrameMap& fm);
 
-// corr_tc2.cu: correlate-then-interpolate on a split-bf16 copy of the pyramid
+// corr_tc2.cu: correlate-then-interpolate on a split-bf16 copy of the pyramid (mode 3)
 //   pyr_split: per level at bf16 offset 2*off[l]: [plane hi|lo][T][H][W][128]   (same bytes as the fp32 pyramid)
 bool corr_patch_supported(int T, int H4, int W4);
 //   mode 3: [plane hi|lo][T][H][W][128] bf16;  mode 1/2: one fp16 plane [T][H][W][128] at the same level offset
@@ -131,7 +131,7 @@ cudaError_t launch_split_pyramid(const float* pyr, int T, int H4, int W4, __nv_b
                                  cudaStream_t s);
 cudaError_t launch_corr_patch_tc(const __nv_bfloat16* pyr_split, int H4, int W4, const float* support,
                                  const uint8_t* track_valid, const float* coords, int T, int N,
-                                 __nv_bfloat16* vol_split, int mode, int vol16, int num_sms, cudaStream_t s, int T_pyr,
+                                 __nv_bfloat16* vol_split, int vol16, int num_sms, cudaStream_t s, int T_pyr,
                                  const FrameMap& fm);
 
 // corr_tc3.cu: the production kernel -- same algorithm with the MMA transposed (supports = M side), one fp16 texel

@@ -479,7 +479,7 @@ def volume_planes(vol: torch.Tensor, T: int, N: int, H4: int, W4: int, patch: bo
     the correlate-then-interpolate kernels could run and this thread's options decide the format and element order."""
     rows = N * T * LEVELS
     # a single fp16 plane [rows, 2432] when the correlate-then-interpolate kernel runs with prec.fc1 < 3
-    vb = precision_info(T, H4, W4)[2] if (patch and get_option("corr") in (0, 3)) else 4
+    vb = precision_info(T, H4, W4)[2] if (patch and get_option("corr") == 0) else 4
     if vb == 2:
         planes = vol.reshape(-1).view(torch.float16)[:rows * VOL_PAD].reshape(1, rows, VOL_PAD).float()
     else:

@@ -39,8 +39,7 @@ enum {
   CT3_OK = 0,
   CT3_EINVAL = -1,   /* bad argument (shape, null pointer, alignment)          */
   CT3_ECUDA = -2,    /* a CUDA runtime/driver call failed (see ct3_last_error) */
-  CT3_ENOSPC = -3,   /* workspace / packed buffer too small                    */
-  CT3_EUNSUPPORTED = -4
+  CT3_ENOSPC = -3    /* workspace / packed buffer too small                    */
 };
 
 /* Model constants fixed by the reference architecture
@@ -73,8 +72,7 @@ const char* ct3_last_error(void);
 
 /* Debug/verification options ("gemm", "corr", "attn": 0 = tensor-core path (default),
  * 1 = SIMT fp32 verification kernel used by the tests to cross-check; "corr" = 2 forces the
- * sample-then-correlate tensor-core kernel that otherwise only serves pyramids with a level below 8x8;
- * "attn" = 2 runs the point<-virtual attention on the mma.sync kernel instead of the wgmma one, for A/B).
+ * sample-then-correlate tensor-core kernel that otherwise only serves pyramids with a level below 8x8).
  * "fuse" (time blocks, T <= 128): 1 = q|k|v projection and time attention in one kernel (default), 0 = separate
  * projection and attention kernels, which T > 128 always runs and the tests use as the cross-check. */
 int ct3_set_option(const char* name, int value);
@@ -249,7 +247,7 @@ int ct3_update_loop(const void* packed, const float* pyr, int H4, int W4, const 
  *   workspace        : ct3_workspace_bytes_groups(T, N, G, H4, W4) bytes (grows by 64*T*G virtual token rows)
  * A null group array, G < 1, a size < 1 or sizes not summing to N return CT3_EINVAL before anything is enqueued.
  * Options: the default kernels and the exact-fp32 verification kernels ("gemm" / "corr" / "attn" = 1) support
- * G > 1; "attn" = 2 returns CT3_EUNSUPPORTED for G > 1. */
+ * G > 1. */
 int ct3_workspace_bytes_groups(int T, int N, int G, int H4, int W4, size_t* out_bytes);
 int ct3_update_loop_groups(const void* packed, const float* pyr, int H4, int W4, const float* support,
                            const uint8_t* track_valid, float* coords, float* vis, float* conf,
@@ -269,7 +267,7 @@ int ct3_update_loop_groups(const void* packed, const float* pyr, int H4, int W4,
  *   workspace         : ct3_workspace_bytes_frames(T, T_pyr, N, G, H4, W4) bytes (the split-bf16 pyramid copy is sized
  *                       by T_pyr and made once per call)
  * A null table, a frame index outside [0, T_pyr), T_pyr < 1 and every invalid argument of ct3_update_loop_groups return
- * CT3_EINVAL before anything is enqueued; "attn" = 2 returns CT3_EUNSUPPORTED for G > 1. */
+ * CT3_EINVAL before anything is enqueued. */
 int ct3_workspace_bytes_frames(int T, int T_pyr, int N, int G, int H4, int W4, size_t* out_bytes);
 int ct3_update_loop_frames(const void* packed, const float* pyr, int T_pyr, int H4, int W4, const float* support,
                            const uint8_t* track_valid, float* coords, float* vis, float* conf,
@@ -360,7 +358,7 @@ int ct3_updateformer_groups(const void* packed, const float* x, int T, const int
  *   group_sizes_host, G : as ct3_updateformer_groups (sum = N)
  *   workspace      : ct3_attention_workspace_bytes(T, N, G) bytes, 256-byte aligned (split-K partials, group table)
  * Null pointers, an unknown kind, bad T/N/groups, misalignment return CT3_EINVAL and a too small workspace
- * CT3_ENOSPC, before any launch; "attn" = 2 with G > 1 returns CT3_EUNSUPPORTED. */
+ * CT3_ENOSPC, before any launch. */
 enum { CT3_ATTN_TIME = 0, CT3_ATTN_VIRTUAL_FROM_POINT = 1, CT3_ATTN_VIRTUAL_SELF = 2, CT3_ATTN_POINT_FROM_VIRTUAL = 3 };
 int ct3_attention_workspace_bytes(int T, int N, int G, size_t* out_bytes);
 int ct3_attention(int kind, const float* q, const float* kv, int T, int N, const int32_t* group_sizes_host, int G,

@@ -1,5 +1,7 @@
 """Correlation stage alone at the headline size (N=6400, T=16, 96x128 feature maps): ms per launch, CUDA events.
-    CT3_B200_LIB=<variant .so> python scripts/corr_bench.py [impl [prec.corr [prec.fc1]]]"""
+    CT3_B200_LIB=<variant .so> python scripts/corr_bench.py [impl [prec.corr [prec.fc1]]]
+impl is the "corr" option: 0 correlate-then-interpolate (corr_tc3.cu for prec.corr 1 | 2, corr_tc2.cu for 3), 1 exact-fp32
+SIMT, 2 sample-then-correlate (corr_tc.cu)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

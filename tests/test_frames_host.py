@@ -68,21 +68,6 @@ def test_update_loop_frames_rejects_bad_arguments_without_gpu():
         assert msg in lib.ct3_last_error(), lib.ct3_last_error()
 
 
-def test_update_loop_frames_unsupported_options():
-    lib = engine.lib()
-    fake = ctypes.c_void_p(1 << 20)
-    frames = _i32(0, 1, 2, 3, 3, 2, 1, 0)
-    before = engine.get_option("attn")
-    try:
-        engine.set_option("attn", 2)
-        rc = lib.ct3_update_loop_frames(fake, fake, 4, 24, 32, fake, None, fake, fake, fake, fake, 4, 10, 1,
-                                        ctypes.c_void_p(1 << 24), 1 << 40, None, _i32(5, 5), 2, frames)
-        assert rc == -4
-        assert b"grouped calls do not support attn = 2" in lib.ct3_last_error()
-    finally:
-        engine.set_option("attn", before)
-
-
 # ---- host frame-map builders --------------------------------------------------------------------------------
 def _padded_clip(T, pad, reverse):
     """Frame ids of the clip the reference's model encodes: played backwards if `reverse` (video.flip(1)), then padded

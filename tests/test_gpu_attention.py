@@ -10,7 +10,7 @@ device it runs on, so a change to the heuristics cannot silently drop one from c
 Tolerances (err = max |got - want| over the written rows, want in float64):
   Labs  = max over (sequence, head, query, key) of sum_d |q_d k_d| / sqrt(48), the scale of a logit's rounding error;
   vmax  = max |v|, the scale of the output.
-  attn 0 / 2 (split-bf16x3 tensor cores): q, k, P and V are each held as hi + lo bf16 pairs, 2^-18 relative, and the
+  attn 0 (split-bf16x3 tensor cores): q, k, P and V are each held as hi + lo bf16 pairs, 2^-18 relative, and the
     lo*lo product is dropped, so a logit is off by at most ~3 * 2^-18 * Labs < 2^-16 * Labs.  A probability
     exp(s - m) / l carries that error twice (numerator and sum), and P V adds 2^-16 * vmax for its own splits and the
     split of the output:   err <= 2 * (1 + Labs) * 2^-16 * vmax.
@@ -69,7 +69,7 @@ def branch(kind, T, N, sizes, attn, sms):
     if kind == TIME:   # run_attention(per_warp): every track, KB by the key count
         return {"path": "per_warp", "kb": 16 if T <= 16 else 32 if T <= 32 else 64, "T": T}
     if G == 1:
-        if kind == P_FROM_V and attn == 0 and N > KV:
+        if kind == P_FROM_V and N > KV:
             return {"path": "wgmma"}
         Lq, Lk = {V_FROM_P: (KV, N), V_SELF: (KV, KV), P_FROM_V: (N, KV)}[kind]
         s = tc_splits(T, Lq, Lk, sms)
@@ -105,7 +105,7 @@ def coverage(branches):
         if not any(b["T"] == T for b in pw):
             missing.append(f"time attention at T={T}")
     qtws = {b["qtw"] for b in branches if "qtw" in b}
-    missing += [f"qtw={q}" for q in (1, 2, 4, 8) if q not in qtws]
+    missing += [f"qtw={q}" for q in (1, 8) if q not in qtws]
     if not any(b["path"] == "split_k" for b in branches):
         missing.append("ungrouped split-K")
     if not any(b["path"] == "grouped_split_k" and len(set(b["group_splits"])) >= 3 and 1 in b["group_splits"]
@@ -126,8 +126,6 @@ MIXED = (3000, 1, 449, 448, 700, 64, 65, 90)
 CASES = []
 for _n in (1, 15, 16, 17, 63, 64, 65, 127, 128, 129, 1030, 3000):      # ragged query tiles of point<-virtual
     CASES.append((P_FROM_V, 8, _n, None, "soft", 0))
-for _n in (300, 600, 1030, 3000, 6400):                                # mma.sync point<-virtual: qtw 1, 2, 4, 8, 8
-    CASES.append((P_FROM_V, 16, _n, None, "soft", 2))
 for _n in (1, 64, 65, 448, 449, 1030, 6400):                           # key counts around chunk and split boundaries
     CASES.append((V_FROM_P, 16, _n, None, "soft", 0))
 CASES += [(V_SELF, 8, 5, None, "soft", 0), (V_SELF, 66, 3, None, "soft", 0), (V_SELF, 16, 40, None, "soft", 1)]
@@ -138,7 +136,6 @@ for _t in (16, 48):                                                    # full si
     for _attn in (0, 1):
         CASES.append((P_FROM_V, _t, 6400, None, "soft", _attn))
         CASES.append((V_FROM_P, _t, 6400, None, "soft", _attn))
-    CASES.append((P_FROM_V, _t, 6400, None, "soft", 2))
 for _regime in ("sharp30", "sharp80", "dominant", "underflow_last", "underflow_first"):
     CASES += [(TIME, 17, 37, None, _regime, 0), (TIME, 65, 37, None, _regime, 0), (TIME, 150, 37, None, _regime, 0),
               (TIME, 200, 20, None, _regime, 0), (TIME, 150, 37, None, _regime, 1),
@@ -146,7 +143,7 @@ for _regime in ("sharp30", "sharp80", "dominant", "underflow_last", "underflow_f
               (V_FROM_P, 16, 6400, None, _regime, 0), (V_FROM_P, 48, 6400, None, _regime, 0),
               (V_FROM_P, 16, 6400, None, _regime, 1), (V_FROM_P, 8, sum(MIXED), MIXED, _regime, 0),
               (P_FROM_V, 16, 17, None, _regime, 0), (P_FROM_V, 16, 1030, None, _regime, 0),
-              (P_FROM_V, 16, 1030, None, _regime, 2), (P_FROM_V, 16, 6400, None, _regime, 1)]
+              (P_FROM_V, 16, 6400, None, _regime, 1)]
     if not _regime.startswith("underflow"):   # 64 keys are one chunk: nothing to underflow across
         CASES += [(V_SELF, 8, 5, None, _regime, 0), (V_SELF, 66, 3, None, _regime, 0)]
 CASES = list(dict.fromkeys(CASES))   # the full-size loop repeats two shapes of the lists above
@@ -318,7 +315,6 @@ def test_branch_map_matches_the_cpp():
     assert [branch(TIME, t, 5, None, 0, 132)["kb"] for t in (1, 16, 17, 32, 33, 200)] == [16, 16, 32, 32, 64, 64]
     assert branch(P_FROM_V, 16, 65, None, 0, 132) == {"path": "wgmma"}
     assert branch(P_FROM_V, 16, 64, None, 0, 132)["path"] == "shared"
-    assert branch(P_FROM_V, 16, 6400, None, 2, 132) == {"path": "shared", "qtw": 8}
     assert branch(V_FROM_P, 8, sum(MIXED), MIXED, 0, 132)["group_splits"] == [8, 1, 4, 1, 4, 1, 1, 1]
     assert branch(P_FROM_V, 8, sum(MIXED), MIXED, 0, 132) == {"path": "grouped_p2v", "wgmma_groups": 6,
                                                               "mma_groups": 2, "qtw": 1}
@@ -376,17 +372,6 @@ def test_grouped_attention_matches_fp64_and_standalone_calls(eng, kind, T, attn)
         off += n
 
 
-@pytest.mark.gpu
-def test_grouped_attn2_is_unsupported(eng):
-    q, kv = make_inputs(P_FROM_V, 4, 130, [65, 65], "soft", 1)
-    eng.set_option("attn", 2)
-    try:
-        with pytest.raises(eng.EngineError, match="code -4"):
-            eng.attention(P_FROM_V, q, kv, 4, 130, group_sizes=[65, 65])
-    finally:
-        eng.set_option("attn", 0)
-
-
 # ---------------------------------------------------------------------------------------------------------------------
 # sharp attention through the whole transformer
 SHARP = 30.0
@@ -436,7 +421,7 @@ def sharp_cases():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("fuse", [0, 1])
-@pytest.mark.parametrize("attn", [0, 1, 2])
+@pytest.mark.parametrize("attn", [0, 1])
 @pytest.mark.parametrize("N,T", [(130, 40), (40, 150)])
 def test_updateformer_at_sharp_attention_matches_fp64(eng, sharp_cases, N, T, fuse, attn):
     """EfficientUpdateFormer with every attention at max |logit| ~ 30 against the oracle in float64.  T = 40 runs the

@@ -107,12 +107,15 @@ def test_identity_map_is_the_grouped_call(eng, sd):
         assert torch.equal(x, y)
 
 
-@pytest.mark.parametrize("corr", [2, 3])   # with the sample-then-correlate and the correlate-then-interpolate kernel
-def test_frames_on_other_tensor_core_kernels(eng, sd, corr):
+# with the sample-then-correlate kernel (corr_tc.cu) and the split-bf16 correlate-then-interpolate kernel (corr_tc2.cu)
+@pytest.mark.parametrize("opts", [{"corr": 2}, {"prec.corr": 3}], ids=["corr2", "prec.corr3"])
+def test_frames_on_other_tensor_core_kernels(eng, sd, opts):
     T, H4, W4 = 12, 64, 72
     fmaps, maps, qf, qc, valid, pyr, support, c0, te = _frames_case(eng, sd, T, H4, W4, seed=11)
     packed = eng.pack_weights(sd, DEV)
-    eng.set_option("corr", corr)
+    before = {k: eng.get_option(k) for k in opts}
+    for k, v in opts.items():
+        eng.set_option(k, v)
     try:
         got = _loop(eng, packed, pyr, H4, W4, support, valid, c0, te, 2, SIZES, maps)
         for k, (a, b) in enumerate(_bounds(SIZES)):
@@ -120,9 +123,10 @@ def test_frames_on_other_tensor_core_kernels(eng, sd, corr):
             want = _loop(eng, packed, pyr_g, H4, W4, support[:, :, a:b].contiguous(), valid[a:b].contiguous(),
                          c0[:, a:b].contiguous(), te, 2)
             for x, y in zip(got, want):
-                assert torch.equal(x[:, a:b], y), (corr, k)
+                assert torch.equal(x[:, a:b], y), (opts, k)
     finally:
-        eng.set_option("corr", 0)
+        for k, v in before.items():
+            eng.set_option(k, v)
 
 
 def test_frames_simt_cross_check(eng, sd):

@@ -4,7 +4,9 @@ against the float64 CPU oracle, for every correlation kernel, volume format, cor
 count, on both GEMM engines.
 
 The branch map below restates in Python which path a call takes (api_loop.cu: effective_prec, Prec; corr.cu:
-corr_uses_patch_kernel, launch_corr_sample; corr_tc2.cu: corr_patch_supported).  test_host_logic.py pins it to the
+corr_uses_patch_kernel, launch_corr_sample; corr_tc2.cu: corr_patch_supported): with the default "corr" = 0 and every
+pyramid level at least 8x8, corr_tc3.cu runs prec.corr 1 and 2 and corr_tc2.cu prec.corr 3; "corr" 1 and 2 and smaller
+pyramids run the SIMT and corr_tc.cu kernels at full precision.  test_host_logic.py pins it to the
 compiled ct3_precision_info / ct3_volume_is_support_major; the GPU test prints every case's branch and asserts that the
 case list reaches every reachable combination.
 
@@ -59,10 +61,10 @@ OPTION_DEFAULTS = {"gemm": 0, "corr": 0, "attn": 0, "prec.corr": 2, "prec.fc1": 
 def loop_branch(T, H4, W4, corr=0, prec_corr=2, prec_fc1=3, gemm=0):
     """What ct3_loop_tokens / one update_loop iteration runs for these options and this pyramid shape."""
     # the workspace holds the split pyramid iff every level is >= 8x8 texels (corr_patch_supported)
-    patch = corr in (0, 3) and (H4 >> 3) >= 8 and (W4 >> 3) >= 8
+    patch = corr == 0 and (H4 >> 3) >= 8 and (W4 >> 3) >= 8
     pc, pf = (prec_corr, prec_fc1) if patch else (3, 3)
     if patch:
-        kernel = "corr_tc3" if corr == 0 and pc != 3 else "corr_tc2"
+        kernel = "corr_tc3" if pc != 3 else "corr_tc2"
     else:
         kernel = "simt" if corr == 1 else "corr_tc"
     support_major = kernel == "corr_tc3"
@@ -93,13 +95,13 @@ CASES = [
     ({"prec.fc1": 2, "gemm": 1}, 2, 37, 64, 72, "dead"),
     ({"prec.corr": 1, "prec.fc1": 1}, 2, 37, 64, 72, "motion"),
     ({"prec.corr": 1, "prec.fc1": 1, "gemm": 1}, 1, 1, 64, 72, "base"),
-    ({"corr": 3}, 48, 11, 64, 72, "base"),
+    ({"prec.corr": 3}, 48, 11, 64, 72, "base"),
     ({"prec.corr": 3}, 16, 8, 96, 128, "gelu"),
-    ({"corr": 3, "gemm": 1}, 7, 37, 64, 72, "time"),
-    ({"corr": 3, "prec.fc1": 2}, 7, 37, 64, 72, "state"),
-    ({"corr": 3, "prec.fc1": 2, "gemm": 1}, 1, 37, 64, 72, "base"),
-    ({"corr": 3, "prec.fc1": 1}, 1, 1, 64, 72, "base"),
-    ({"corr": 3, "prec.fc1": 1, "gemm": 1}, 7, 37, 64, 72, "dead"),
+    ({"prec.corr": 3, "gemm": 1}, 7, 37, 64, 72, "time"),
+    ({"prec.corr": 3, "prec.fc1": 2}, 7, 37, 64, 72, "state"),
+    ({"prec.corr": 3, "prec.fc1": 2, "gemm": 1}, 1, 37, 64, 72, "base"),
+    ({"prec.corr": 3, "prec.fc1": 1}, 1, 1, 64, 72, "base"),
+    ({"prec.corr": 3, "prec.fc1": 1, "gemm": 1}, 7, 37, 64, 72, "dead"),
     ({}, 7, 37, 24, 32, "base"),
     ({}, 60, 5, 24, 32, "base"),
     ({"corr": 2}, 16, 37, 64, 72, "motion"),

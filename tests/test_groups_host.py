@@ -68,20 +68,6 @@ def test_grouped_calls_reject_bad_groups_without_gpu():
         engine._group_array(["x"])
 
 
-def test_grouped_calls_reject_unsupported_options():
-    lib = engine.lib()
-    fake = ctypes.c_void_p(1 << 20)
-    ws = ctypes.c_void_p(1 << 24)
-    old = engine.get_option("attn")
-    engine.set_option("attn", 2)
-    try:
-        rc = lib.ct3_updateformer_groups(fake, fake, 4, _sizes(3, 4), 2, fake, ws, 1 << 40, None)
-    finally:
-        engine.set_option("attn", old)
-    assert rc == -4                                                      # CT3_EUNSUPPORTED
-    assert b"grouped calls do not support attn = 2" in lib.ct3_last_error()
-
-
 def _check_plan(sizes, T, budget, fn):
     passes = plan_passes(sizes, T, 96, 128, budget, fn)
     covered = [g for a, b in passes for g in range(a, b)]

@@ -82,11 +82,6 @@ def test_attention_stage_argument_validation_without_gpu():
     assert call(out=ctypes.c_void_p((1 << 20) + 8)) == -1
     assert call(w=ctypes.c_void_p((1 << 21) + 16)) == -1 and b"256-byte" in lib.ct3_last_error()
     assert call(nbytes=need - 1) == -3                                                   # CT3_ENOSPC
-    assert lib.ct3_set_option(b"attn", 2) == 0
-    try:   # attn = 2 has no grouped point<-virtual path, as for the grouped update loop
-        assert call(kind=3, N=10, sizes=(ctypes.c_int32 * 2)(5, 5), G=2, nbytes=1 << 40) == -4
-    finally:
-        assert lib.ct3_set_option(b"attn", 0) == 0
 
 
 def test_loop_tokens_argument_validation_without_gpu():
@@ -125,7 +120,7 @@ def test_loop_tokens_branch_map_matches_library():
     lib = engine.lib()
     flag = ctypes.c_int(0)
     try:
-        for corr, pc, pf, (H4, W4) in itertools.product(range(4), (1, 2, 3), (1, 2, 3),
+        for corr, pc, pf, (H4, W4) in itertools.product(range(3), (1, 2, 3), (1, 2, 3),
                                                         [(24, 32), (64, 72), (96, 128), (64, 63), (63, 64), (8, 8)]):
             for k, v in (("corr", corr), ("prec.corr", pc), ("prec.fc1", pf)):
                 engine.set_option(k, v)
@@ -139,7 +134,7 @@ def test_loop_tokens_branch_map_matches_library():
             engine.set_option(k, v)
     assert loop_branch(16, 96, 128)["weights"] == "corr_fc1_t"
     assert loop_branch(16, 96, 128, prec_fc1=2)["weights"] == "corr_fc1_th"
-    assert loop_branch(16, 96, 128, corr=3, prec_fc1=1)["weights"] == "corr_fc1_h"
+    assert loop_branch(16, 96, 128, prec_corr=3, prec_fc1=1)["weights"] == "corr_fc1_h"
     assert loop_branch(16, 24, 32, prec_fc1=1) == loop_branch(16, 24, 32, corr=2)    # no patch kernel: split x split
 
 
@@ -289,6 +284,9 @@ def test_options_are_validated_and_thread_local():
     lib = engine.lib()
     assert lib.ct3_set_option(b"corr", 7) == -1 and b"out of range" in lib.ct3_last_error()
     assert lib.ct3_set_option(b"attn", -1) == -1
+    assert lib.ct3_set_option(b"corr", 3) == -1 and b"out of range" in lib.ct3_last_error()
+    assert lib.ct3_set_option(b"attn", 2) == -1 and b"out of range" in lib.ct3_last_error()
+    assert engine.get_option("corr") == 0 and engine.get_option("attn") == 0
     assert engine.get_option("fuse") == 1
     assert lib.ct3_set_option(b"fuse", 2) == -1 and b"out of range" in lib.ct3_last_error()
     assert lib.ct3_set_option(b"fuse", 0) == 0 and engine.get_option("fuse") == 0

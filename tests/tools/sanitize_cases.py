@@ -29,7 +29,7 @@ def corr_stage():
     support = support / support.norm(dim=-1, keepdim=True)
     coords = torch.rand(T, N, 2, generator=g) * torch.tensor([W4 + 6.0, H4 + 6.0]) - 3.0
     valid = torch.ones(N, dtype=torch.uint8)
-    for impl, corr, fc1 in ((0, 2, 3), (0, 1, 2), (3, 3, 3), (2, 3, 3), (1, 3, 3)):
+    for impl, corr, fc1 in ((0, 2, 3), (0, 1, 2), (0, 3, 3), (2, 3, 3), (1, 3, 3)):
         eng.set_option("corr", impl); eng.set_option("prec.corr", corr); eng.set_option("prec.fc1", fc1)
         got = eng.corr_sample(pyr, H4, W4, support.to(DEV), valid.to(DEV), coords.to(DEV)).cpu()
         err = max(float((got[:, :, l].permute(1, 0, 2) - O.correlation_volume(want_pyr[l], support[l], coords / 2 ** l)).abs().max())
@@ -48,7 +48,7 @@ def model_cases():
     model = build_cotracker(None, offline=True, window_len=60).eval()
     model.load_state_dict(sd)
     model = model.to(DEV)
-    for fuse, attn in ((1, 0), (0, 0), (1, 2)):
+    for fuse, attn in ((1, 0), (0, 0)):
         eng.set_option("fuse", fuse); eng.set_option("attn", attn)
         c, v, q, _ = model(video.to(DEV), queries.to(DEV), iters=2)
         torch.cuda.synchronize()
