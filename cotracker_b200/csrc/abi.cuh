@@ -82,7 +82,8 @@ struct Carver {
 // a plain linear layer y[M, N] = x_split w_split^T + bias, fp32 rows of pitch N
 GemmProblem linear_problem(const void* x_split, const void* w_split, const void* bias, int64_t M, int N, int Kpad,
                            float* y);
-// launches p on engine impl (0 wgmma, 1 SIMT); a failure becomes CT3_ECUDA with "what: error (detail)"
+// launches p on engine impl (0 wgmma, 1 SIMT); a problem gemm_check rejects becomes CT3_EINVAL with "what: reason"
+// before any launch, a failed launch CT3_ECUDA with "what: error (detail)"
 int run_gemm(const GemmProblem& p, int impl, cudaStream_t s, const char* what);
 
 }  // namespace ct3

@@ -80,6 +80,10 @@ GemmProblem linear_problem(const void* x_split, const void* w_split, const void*
   return p;
 }
 int run_gemm(const GemmProblem& p, int impl, cudaStream_t s, const char* what) {
+  if (const char* bad = gemm_check(p)) {
+    snprintf(g_err, sizeof(g_err), "%s: %s", what, bad);
+    return CT3_EINVAL;
+  }
   const char* gerr = nullptr;
   const int rc = gemm_launch(p, impl, num_sms(), s, &gerr);
   return rc ? fail_launch(rc, what, gerr) : 0;

@@ -314,14 +314,24 @@ int space_attention(Runner& R, const Workspace& W, const GroupPlan& gp, AttnPara
   return 0;
 }
 
-// q|k|v projection and the per-track T x T attention of time block b in ONE kernel: fp32 q|k|v never reaches HBM.
-int qkv_time_attention(Runner& R, const Workspace& W, const Block& b, const __nv_bfloat16* x, int rows, int T) {
-  ProfScope ps(R.s, CAT_QKVA, 0.0);
-  const char* gerr = nullptr;
-  const int rc = gemm_qkv_time_attn_launch(
-      x, reinterpret_cast<const __nv_bfloat16*>(R.pk + b.qkv_h.w), reinterpret_cast<const float*>(R.pk + b.qkv_h.b),
-      rows, kC, T, W.att, 2 * kC, kC, 1.0f / sqrtf((float)kDh), num_sms(), R.s, &gerr);
-  return rc ? fail_launch(rc, "fused qkv + time attention", gerr) : 0;
+// q|k|v projection and the per-track T x T attention of time block b on the LayerNorm output x [rows, 2*kC] (rows
+// n*T + t) into att (split rows of pitch 2*kC).  With fuse = 1 on the product kernels (gemm 0, attn != 1) and T <= 128
+// both run in ONE kernel, so fp32 q|k|v never reaches HBM; otherwise the b.q GEMM writes q|k|v to W.qkv [rows, 3*kC]
+// and the per-warp attention kernel reads it.
+int time_attention(Runner& R, const Workspace& W, const Block& b, const __nv_bfloat16* x, __nv_bfloat16* att,
+                   int rows, int T) {
+  if (g_opt[OPT_FUSE] == 1 && R.impl == 0 && g_opt_attn != 1 && qkv_time_attn_supported(T)) {
+    ProfScope ps(R.s, CAT_QKVA, 0.0);
+    const char* gerr = nullptr;
+    const int rc = gemm_qkv_time_attn_launch(
+        x, reinterpret_cast<const __nv_bfloat16*>(R.pk + b.qkv_h.w), reinterpret_cast<const float*>(R.pk + b.qkv_h.b),
+        rows, kC, T, att, 2 * kC, kC, 1.0f / sqrtf((float)kDh), num_sms(), R.s, &gerr);
+    return rc ? fail_launch(rc, "fused qkv + time attention", gerr) : 0;
+  }
+  GEMM(x, b.q, rows, Runner::to_f32(W.qkv, 3 * kC, false));
+  RUNC(CAT_ATTN, run_attention(R, W, attn_params(W.qkv, 3 * kC, W.qkv, 3 * kC, kC, 2 * kC, att, T, T, T, rows / T),
+                               true));
+  return 0;
 }
 
 // x += to_out(attn(...)); x += mlp(LN(x))   for the rows [row0, row0+rows) of the token buffer
@@ -351,13 +361,7 @@ int transformer_body(Runner& R, const Workspace& W, int T, int N, const GroupPla
     {  // ---- time block over every token row (points + virtual): sequence = track (cotracker.py:494-495)
       const Block& b = L.time[i];
       RUNC(CAT_LN, launch_layernorm_split(W.tokens, Rall, nullptr, nullptr, 1e-6f, W.ln, R.s));
-      if (g_opt[OPT_FUSE] == 1 && R.impl == 0 && g_opt_attn != 1 && qkv_time_attn_supported(T)) {
-        if (int rc = qkv_time_attention(R, W, b, W.ln, Rall, T)) return rc;
-      } else {
-        GEMM(W.ln, b.q, Rall, Runner::to_f32(W.qkv, 3 * kC, false));
-        RUNC(CAT_ATTN, run_attention(R, W, attn_params(W.qkv, 3 * kC, W.qkv, 3 * kC, kC, 2 * kC, W.att, T, T, T,
-                                                       N + kV * gp.G), true));
-      }
+      if (int rc = time_attention(R, W, b, W.ln, W.att, Rall, T)) return rc;   // Rall / T = N + kV*G tracks
       GEMM(W.att, b.out, Rall, Runner::to_f32(W.tokens, kC, true));
       if (int rc = mlp_half(R, W, b, 0, Rall)) return rc;
     }
@@ -651,6 +655,36 @@ int attention_stage(int kind, const float* q, const float* kv, int T, int N, con
   return 0;
 }
 
+// ct3_time_block_attention: the fp32 q|k|v of the unfused route, the only scratch time_attention reads
+Workspace carve_time_block(void* base, int rows) {
+  Workspace w{};
+  Carver c(base);
+  w.qkv = (float*)c.take((size_t)rows * 3 * kC * 4);
+  w.total = c.off;
+  return w;
+}
+
+int check_time_block(int T, int rows) {
+  if (T < 1 || rows < 1 || rows % T) return fail(CT3_EINVAL, "need T >= 1, rows >= 1 and rows %% T == 0%s");
+  return 0;
+}
+
+// q|k|v projection and attention of time block `depth` on caller buffers, routed as transformer_body routes it
+int time_block_stage(const void* packed, int depth, const void* x_split, int T, int rows, void* out_split,
+                     void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (!packed || !x_split || !out_split || !workspace) return fail(CT3_EINVAL, "null argument%s");
+  if (depth < 0 || depth >= kDepth) return fail(CT3_EINVAL, "depth must be in [0, 3)%s");
+  if (int rc = check_time_block(T, rows)) return rc;
+  if (((uintptr_t)packed | (uintptr_t)x_split | (uintptr_t)out_split) & 15)
+    return fail(CT3_EINVAL, "packed, x_split and out_split must be 16-byte aligned%s");
+  if (int rc = check_aligned(workspace, "workspace")) return rc;
+  const Workspace W = carve_time_block(workspace, rows);
+  if (int rc = check_space(workspace_bytes, W.total, "workspace")) return rc;
+  Runner R{reinterpret_cast<const uint8_t*>(packed), layout(), stream, g_opt_gemm};
+  return time_attention(R, W, R.L.time[depth], reinterpret_cast<const __nv_bfloat16*>(x_split),
+                        reinterpret_cast<__nv_bfloat16*>(out_split), rows, T);
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -790,21 +824,60 @@ int ct3_corr_sample(const float* pyr, int H4, int W4, const float* support, cons
 
 int ct3_linear(const void* x_split, const void* w_split, const float* bias, int M, int Nout, int Kpad, int act,
                float* y, ct3_stream_t stream) {
-  return ct3_linear_prec(x_split, w_split, bias, M, Nout, Kpad, act, 3, 0, y, stream);
+  return ct3_linear_ex(x_split, 0, w_split, bias, M, Nout, Kpad, 3, 0, act, nullptr, 1, y, Nout, 0, nullptr, 0, 0, 1,
+                       stream);
 }
 
 int ct3_linear_prec(const void* x_split, const void* w_split, const float* bias, int M, int Nout, int Kpad, int act,
                     int products, int fp16, float* y, ct3_stream_t stream) {
-  if (!x_split || !w_split || !y) return fail(CT3_EINVAL, "null argument%s");
-  if (M < 1 || Nout < 1 || (Nout % 128) || Kpad < 64 || (Kpad % 64) || act < 0 || act > 2)
-    return fail(CT3_EINVAL, "ct3_linear: need M>=1, Nout %% 128 == 0, Kpad %% 64 == 0, act in 0..2%s");
-  if (products < 1 || products > 3 || fp16 < 0 || fp16 > 1)
-    return fail(CT3_EINVAL, "ct3_linear_prec: products in 1..3, fp16 in 0..1%s");
+  return ct3_linear_ex(x_split, 0, w_split, bias, M, Nout, Kpad, products, fp16, act, nullptr, 1, y, Nout, 0, nullptr,
+                       0, 0, 1, stream);
+}
+
+int ct3_linear_ex(const void* x_split, int64_t x_ld, const void* w_split, const float* bias, int M, int Nout, int Kpad,
+                  int products, int fp16, int act, const float* row_bias, int row_mod, float* y, int64_t ld_y,
+                  int residual, void* y_split, int64_t ld_split, int lo_off, int row_group, ct3_stream_t stream) {
+  if (!x_split || !w_split) return fail(CT3_EINVAL, "null argument%s");
+  if (residual != 0 && (residual != 1 || !y)) return fail(CT3_EINVAL, "ct3_linear: residual is 0, or 1 with y%s");
   GemmProblem p = linear_problem(x_split, w_split, bias, M, Nout, Kpad, y);
+  p.x_ld = x_ld;
   p.products = products;
   p.fp16 = fp16;
   p.epi.act = act;
+  p.epi.row_bias = row_bias;
+  p.epi.row_mod = row_mod;
+  p.epi.ld_f32 = ld_y;
+  p.epi.residual = residual;
+  p.epi.out_split = static_cast<__nv_bfloat16*>(y_split);
+  p.epi.ld_split = ld_split;
+  p.epi.lo_off = lo_off;
+  p.epi.row_group = row_group;
   return run_gemm(p, g_opt_gemm, (cudaStream_t)stream, "ct3_linear");
+}
+
+int ct3_time_block_attention_workspace_bytes(int T, int rows, size_t* out_bytes) {
+  if (!out_bytes) return fail(CT3_EINVAL, "null out_bytes%s");
+  if (int rc = check_time_block(T, rows)) return rc;
+  *out_bytes = carve_time_block(nullptr, rows).total;
+  return 0;
+}
+
+int ct3_time_block_attention(const void* packed, int depth, const void* x_split, int T, int rows, void* out_split,
+                             void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+  return time_block_stage(packed, depth, x_split, T, rows, out_split, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int ct3_layernorm(const float* x, int rows, const float* gamma, const float* beta, float eps, void* out_split,
+                  ct3_stream_t stream) {
+  if (!x || !out_split) return fail(CT3_EINVAL, "null argument%s");
+  if ((gamma == nullptr) != (beta == nullptr)) return fail(CT3_EINVAL, "gamma and beta must be given together%s");
+  if (rows < 1) return fail(CT3_EINVAL, "rows must be >= 1%s");
+  if (!(eps >= 0.f && eps <= 1e30f)) return fail(CT3_EINVAL, "eps must be finite and >= 0%s");
+  if (((uintptr_t)x | (uintptr_t)gamma | (uintptr_t)beta | (uintptr_t)out_split) & 15)
+    return fail(CT3_EINVAL, "x, gamma, beta and out_split must be 16-byte aligned%s");
+  CK(launch_layernorm_split(x, rows, gamma, beta, eps, static_cast<__nv_bfloat16*>(out_split), (cudaStream_t)stream),
+     "layernorm");
+  return 0;
 }
 
 int ct3_update_loop(const void* packed, const float* pyr, int H4, int W4, const float* support,

@@ -632,25 +632,36 @@ int gemm_qkv_time_attn_launch(const __nv_bfloat16* x_split, const __nv_bfloat16*
   return (int)cudaGetLastError();
 }
 
-int gemm_launch(const GemmProblem& p, int impl, int num_sms, cudaStream_t stream, const char** err) {
-  *err = nullptr;
-  if (p.M <= 0 || p.N <= 0 || p.Kpad <= 0 || (p.N % BN) != 0 || (p.Kpad % BK) != 0) {
-    *err = "gemm: need M>0, N % 128 == 0, Kpad % 64 == 0";
-    return (int)cudaErrorInvalidValue;
-  }
-  if (p.products < 1 || p.products > 3) {
-    *err = "gemm: products must be 1, 2 or 3";
-    return (int)cudaErrorInvalidValue;
-  }
+const char* gemm_check(const GemmProblem& p) {
+  if (p.M <= 0 || p.N <= 0 || p.Kpad <= 0 || (p.N % BN) != 0 || (p.Kpad % BK) != 0)
+    return "gemm: need M>0, N % 128 == 0, Kpad % 64 == 0";
+  if (p.products < 1 || p.products > 3 || p.fp16 < 0 || p.fp16 > 1) return "gemm: products in 1..3, fp16 in 0..1";
   const int64_t x_ld = p.x_ld ? p.x_ld : 2 * (int64_t)p.Kpad;
-  if (x_ld < (p.products == 3 ? 2 : 1) * (int64_t)p.Kpad || (x_ld % 8) != 0) {
-    *err = "gemm: x_ld too small for the operand planes this product count reads";
-    return (int)cudaErrorInvalidValue;
+  if (x_ld < (p.products == 3 ? 2 : 1) * (int64_t)p.Kpad || (x_ld % 8) != 0)
+    return "gemm: x_ld too small for the operand planes this product count reads";
+  if ((reinterpret_cast<uintptr_t>(p.x_split) | reinterpret_cast<uintptr_t>(p.w_split)) & 15)
+    return "gemm: operands must be 16-byte aligned";
+  // The tensor-core epilogue reads bias / row bias and reads and writes the fp32 output as float4, and addresses the
+  // split output in 16-byte units (epilogue_chunk): anything else would land in the wrong place without an error.
+  const GemmEpilogue& e = p.epi;
+  if (!e.out_f32 && !e.out_split) return "gemm: no output";
+  if (e.row_mod < 1 || e.row_group < 1 || e.act < 0 || e.act > 2) return "gemm: need row_mod >= 1, row_group >= 1, act in 0..2";
+  if (e.out_f32 && (e.ld_f32 < p.N || (e.ld_f32 % 4) != 0)) return "gemm: fp32 output pitch must be >= N and a multiple of 4";
+  if (e.out_split) {
+    const int64_t width = (int64_t)e.row_group * p.N;   // one plane of an output row
+    if ((e.ld_split % 8) != 0 || (e.lo_off % 8) != 0) return "gemm: split output pitch and lo offset must be multiples of 8";
+    if (e.lo_off < width || e.ld_split < e.lo_off + width) return "gemm: hi and lo planes of the split output overlap";
   }
-  if ((reinterpret_cast<uintptr_t>(p.x_split) | reinterpret_cast<uintptr_t>(p.w_split)) & 15) {
-    *err = "gemm: operands must be 16-byte aligned";
-    return (int)cudaErrorInvalidValue;
-  }
+  if ((reinterpret_cast<uintptr_t>(e.bias) | reinterpret_cast<uintptr_t>(e.row_bias) |
+       reinterpret_cast<uintptr_t>(e.out_f32) | reinterpret_cast<uintptr_t>(e.out_split)) & 15)
+    return "gemm: bias, row bias and outputs must be 16-byte aligned";
+  return nullptr;
+}
+
+int gemm_launch(const GemmProblem& p, int impl, int num_sms, cudaStream_t stream, const char** err) {
+  *err = gemm_check(p);
+  if (*err) return (int)cudaErrorInvalidValue;
+  const int64_t x_ld = p.x_ld ? p.x_ld : 2 * (int64_t)p.Kpad;
   if (impl == 1) {
     dim3 grid((p.N + 63) / 64, (p.M + 63) / 64);
     gemm_split3_simt_kernel<<<grid, 256, 0, stream>>>(p.x_split, p.w_split, p.M, p.N, p.Kpad, x_ld, p.products,

@@ -46,7 +46,11 @@ struct GemmProblem {
 bool encode_tensor_map(CUtensorMap* m, CUtensorMapDataType dtype, int rank, const void* base, const uint64_t* dims,
                        const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle);
 
-// 0 = wgmma path, 1 = SIMT verification path.  Returns cudaError_t as int (0 = ok).
+// The argument checks of gemm_launch: null if p can run, else what is wrong with it (shapes, pitches, overlapping
+// hi/lo planes, alignment).
+const char* gemm_check(const GemmProblem& p);
+// 0 = wgmma path, 1 = SIMT verification path.  Returns cudaError_t as int (0 = ok); a problem gemm_check rejects
+// returns cudaErrorInvalidValue with *err set, before any launch.
 int gemm_launch(const GemmProblem& p, int impl, int num_sms, cudaStream_t stream, const char** err);
 
 // Fused q|k|v projection + per-track time attention (gemm.cu, gemm_qkv_time_attn_kernel).

@@ -66,6 +66,12 @@ def _signatures():
         "ct3_split_rows": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_split_rows_fp16": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_linear_prec": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+        "ct3_linear_ex": (c_int, [c_void_p, i64, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int,
+                                  c_void_p, i64, c_int, c_void_p, i64, c_int, c_int, c_void_p]),
+        "ct3_layernorm": (c_int, [c_void_p, c_int, c_void_p, c_void_p, ctypes.c_float, c_void_p, c_void_p]),
+        "ct3_time_block_attention_workspace_bytes": (c_int, [c_int, c_int, ctypes.POINTER(c_size_t)]),
+        "ct3_time_block_attention": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t,
+                                             c_void_p]),
         "ct3_updateformer": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
         "ct3_workspace_bytes_groups": (c_int, [c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
         "ct3_update_loop_groups": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -565,6 +571,82 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], act: 
     _call("ct3_linear_prec", x.device, _ptr(xs), _ptr(ws), _ptr(bias), M, Nout, Kpad, act, products, 1 if fp16 else 0,
           _ptr(y), _stream(x.device))
     return y
+
+
+def _req16(t: torch.Tensor, name: str, dev):
+    """a contiguous 16-bit CUDA tensor on dev (split planes: bf16 or fp16 bits)"""
+    if not t.is_cuda or t.device != torch.device(dev) or t.element_size() != 2 or not t.is_contiguous():
+        raise EngineError(f"{name} must be a contiguous 16-bit tensor on {dev}")
+    return t
+
+
+def linear_ex(x_split: torch.Tensor, w_split: torch.Tensor, bias: Optional[torch.Tensor], M: int, Nout: int, Kpad: int,
+              *, x_ld: int = 0, products: int = 3, fp16: bool = False, act: int = 0,
+              row_bias: Optional[torch.Tensor] = None, row_mod: int = 1, y: Optional[torch.Tensor] = None,
+              ld_y: int = 0, residual: bool = False, y_split: Optional[torch.Tensor] = None, ld_split: int = 0,
+              lo_off: int = 0, row_group: int = 1):
+    """ct3_linear_ex (include/ct3_b200.h): the GEMM engine with its whole epilogue, written in place into the caller's
+    y (fp32) and / or y_split (16-bit).  Every buffer is flat or shaped as the caller likes; each must hold the elements
+    the pitches address, which is checked here (the library can only check the pitches)."""
+    dev = x_split.device
+    _req16(x_split, "x_split", dev)
+    _req16(w_split, "w_split", dev)
+    xl = int(x_ld) if x_ld else 2 * int(Kpad)
+    need = {"x_split": (x_split, (M - 1) * xl + (2 if products == 3 else 1) * Kpad), "w_split": (w_split, Nout * 2 * Kpad)}
+    for name, t, n in (("bias", bias, Nout), ("row_bias", row_bias, max(row_mod, 1) * Nout)):
+        if t is not None:
+            _req(t, torch.float32, name)
+            need[name] = (t, n)
+    if y is not None:
+        _req(y, torch.float32, "y")
+        need["y"] = (y, (M - 1) * ld_y + Nout)
+    if y_split is not None:
+        _req16(y_split, "y_split", dev)
+        need["y_split"] = (y_split, ((M + row_group - 1) // max(row_group, 1) - 1) * ld_split + lo_off + row_group * Nout)
+    for name, (t, n) in need.items():
+        if t.device != dev or t.numel() < n:
+            raise EngineError(f"{name} must hold at least {n} elements on {dev}, has {t.numel()} on {t.device}")
+    _call("ct3_linear_ex", dev, _ptr(x_split), int(x_ld), _ptr(w_split), _ptr(bias), int(M), int(Nout), int(Kpad),
+          int(products), 1 if fp16 else 0, int(act), _ptr(row_bias), int(row_mod), _ptr(y), int(ld_y), 1 if residual else 0,
+          _ptr(y_split), int(ld_split), int(lo_off), int(row_group), _stream(dev))
+
+
+def layernorm(x: torch.Tensor, gamma: Optional[torch.Tensor] = None, beta: Optional[torch.Tensor] = None,
+              eps: float = 1e-6) -> torch.Tensor:
+    """ct3_layernorm: x [rows, 384] fp32 -> split bf16 rows [rows, 768] (hi | lo) of LayerNorm(x) with the optional
+    affine gamma / beta [384], the kernel the transformer body runs."""
+    _req(x, torch.float32, "x")
+    if x.dim() != 2 or x.shape[1] != HID:
+        raise EngineError(f"x must be [rows, {HID}], got {tuple(x.shape)}")
+    for name, t in (("gamma", gamma), ("beta", beta)):
+        if t is not None and (_req(t, torch.float32, name).numel() != HID or t.device != x.device):
+            raise EngineError(f"{name} must be [{HID}] on {x.device}")
+    out = torch.empty(x.shape[0], 2 * HID, dtype=torch.bfloat16, device=x.device)
+    _call("ct3_layernorm", x.device, _ptr(x), x.shape[0], _ptr(gamma), _ptr(beta), float(eps), _ptr(out),
+          _stream(x.device))
+    return out
+
+
+def time_block_attention(packed, depth: int, x_split: torch.Tensor, T: int,
+                         out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """ct3_time_block_attention: q|k|v projection and per-track attention of time block `depth` on the LayerNorm
+    output x_split [rows, 768] (split bf16, rows n*T + t), routed as the transformer body routes it under this thread's
+    options -> split bf16 [rows, 768].  out: a 16-bit buffer of at least rows rows of 768 to write into (rows beyond
+    are left as they are)."""
+    dev = x_split.device
+    _req16(x_split, "x_split", dev)
+    rows = x_split.shape[0]
+    if x_split.dim() != 2 or x_split.shape[1] != 2 * HID:
+        raise EngineError(f"x_split must be [rows, {2 * HID}], got {tuple(x_split.shape)}")
+    if out is None:
+        out = torch.empty(rows, 2 * HID, dtype=torch.bfloat16, device=dev)
+    _req16(out, "out", dev)
+    if out.numel() < rows * 2 * HID:
+        raise EngineError(f"out must hold {rows} rows of {2 * HID}")
+    workspace = torch.empty(_size("ct3_time_block_attention_workspace_bytes", int(T), rows), dtype=torch.uint8, device=dev)
+    _call("ct3_time_block_attention", dev, _ptr(packed), int(depth), _ptr(x_split), int(T), rows, _ptr(out),
+          _ptr(workspace), workspace.numel(), _stream(dev))
+    return out
 
 
 def updateformer(packed, x: torch.Tensor, workspace: Optional[torch.Tensor] = None,

@@ -326,6 +326,47 @@ int ct3_linear(const void* x_split, const void* w_split, const float* bias, int 
 int ct3_linear_prec(const void* x_split, const void* w_split, const float* bias, int M, int Nout,
                     int Kpad, int act, int products, int fp16, float* y, ct3_stream_t stream);
 
+/* The whole epilogue of the GEMM engine, as the update loop and the encoder use it (ct3_linear and ct3_linear_prec are
+ * this call with x_ld = 0, no row bias, y of pitch Nout and no split output), under the thread's "gemm" option:
+ *   v[r, c] = act( sum_k x[r, k] w[c, k] + bias[c] + row_bias[(r % row_mod) * Nout + c] )
+ *   x_split   [M, x_ld] 16-bit planes: hi at column 0, lo at column Kpad (read when products == 3); x_ld = 0 means
+ *             2*Kpad, Kpad a single hi plane (products 1 | 2)
+ *   w_split   [Nout, 2*Kpad];  bias [Nout] and row_bias [row_mod, Nout] fp32 or NULL
+ *   y         fp32 or NULL:  y[r*ld_y + c] = v, or += v when residual = 1
+ *   y_split   16-bit or NULL: output row o = r / row_group holds rows o*row_group .. of v side by side,
+ *             hi at y_split[o*ld_split + (r % row_group)*Nout + c], lo lo_off elements further (hi + lo = v)
+ * Outputs are written on the M (split: ceil(M / row_group)) rows and the Nout (split: row_group*Nout) columns they own,
+ * nothing else.  CT3_EINVAL before any launch: null x / w, no output, M < 1, Nout % 128, Kpad % 64, act outside
+ * 0..2, products outside 1..3, fp16 outside 0..1, x_ld below the planes read or not a multiple of 8, row_mod or
+ * row_group < 1 (also when unused), residual without y, ld_y < Nout or not a multiple of 4, ld_split or lo_off not a
+ * multiple of 8, hi and lo planes that overlap (lo_off < row_group*Nout or ld_split < lo_off + row_group*Nout), and
+ * x, w, bias, row_bias, y or y_split not 16-byte aligned. */
+int ct3_linear_ex(const void* x_split, int64_t x_ld, const void* w_split, const float* bias, int M, int Nout,
+                  int Kpad, int products, int fp16, int act, const float* row_bias, int row_mod, float* y,
+                  int64_t ld_y, int residual, void* y_split, int64_t ld_split, int lo_off, int row_group,
+                  ct3_stream_t stream);
+
+/* LayerNorm over rows of 384 (blocks.py:411,416; the norm_context of the cross blocks, cotracker.py:549) into split
+ * bf16 rows [rows, 768] (hi cols 0..383 | lo cols 384..767), the kernel the transformer body runs:
+ *   out = (x - mean) / sqrt(var + eps) * gamma + beta     (gamma = beta = NULL: no affine)
+ * x [rows, 384] fp32.  Null x / out, only one of gamma and beta, rows < 1, eps negative or not finite, or a pointer
+ * that is not 16-byte aligned return CT3_EINVAL before any launch. */
+int ct3_layernorm(const float* x, int rows, const float* gamma, const float* beta, float eps, void* out_split,
+                  ct3_stream_t stream);
+
+/* q|k|v projection and per-track attention of time block `depth` (0..2) of the transformer body, routed as the body
+ * routes it under the thread's options: the fused kernel when "fuse" = 1, "gemm" = 0, "attn" != 1 and T <= 128,
+ * otherwise the q|k|v GEMM into fp32 and the time-attention kernel.
+ *   x_split   [rows, 768] split bf16: the LayerNorm output of the block's token rows, track-major (row n*T + t)
+ *   out_split [rows, 768] split bf16 (hi cols 0..383 | lo 384..767): softmax(q k^T / sqrt(48)) v per track and head;
+ *             no other row is written
+ *   workspace ct3_time_block_attention_workspace_bytes(T, rows) bytes, 256-byte aligned
+ * Null pointers, depth outside 0..2, T < 1, rows < 1, rows % T != 0, packed / x_split / out_split not 16-byte aligned
+ * return CT3_EINVAL and a too small workspace CT3_ENOSPC, before any launch. */
+int ct3_time_block_attention_workspace_bytes(int T, int rows, size_t* out_bytes);
+int ct3_time_block_attention(const void* packed, int depth, const void* x_split, int T, int rows, void* out_split,
+                             void* workspace, size_t workspace_bytes, ct3_stream_t stream);
+
 /* fp32 [rows, K] -> split bf16 [rows, 2*Kpad] (zero padded); _fp16: the planes hold IEEE fp16 instead */
 int ct3_split_rows(const float* x, int rows, int K, int Kpad, void* x_split, ct3_stream_t stream);
 int ct3_split_rows_fp16(const float* x, int rows, int K, int Kpad, void* x_split, ct3_stream_t stream);

@@ -202,23 +202,57 @@ def _amplified_sd(seed=1234, **kw):
     return seeded_state_dict(seed, offline=True, window_len=60, **kw)
 
 
+def _with_norm_context(sd, seed=8, token_scale=3e-3):
+    """sd with a trained-like affine norm_context in every cross block (gamma ~ 1 + 0.7 N(0, 1), some negative; beta ~
+    0.5 N(0, 1); a fresh module has 1 and 0) and the point tokens scaled down by token_scale (input_transform and every
+    time block's to_out and fc2), so that the tokens the first virtual<-point block normalises have a variance of about
+    1e-6, below norm_context's eps of 1e-5: eps then decides that LayerNorm."""
+    g = torch.Generator().manual_seed(seed)
+    sd = dict(sd)
+    for k in [k for k in sd if k.endswith("norm_context.weight")]:
+        sd[k] = 1 + 0.7 * torch.randn(sd[k].shape, generator=g)
+        sd[k[:-len("weight")] + "bias"] = 0.5 * torch.randn(sd[k].shape, generator=g)
+    for k in [k for k in sd if k.startswith("updateformer.input_transform.") or
+              (k.startswith("updateformer.time_blocks.") and (".attn.to_out." in k or ".mlp.fc2." in k))]:
+        sd[k] = sd[k] * token_scale
+    return sd
+
+
 @pytest.mark.parametrize("impl", [0, 1])
 def test_updateformer_stage(eng, impl):
-    sd = _amplified_sd(head_gain=100.0, vis_gain=100.0)
+    """Also with non-trivial norm_context weights (every seeded state dict has gamma = 1, beta = 0 there) on tokens
+    whose variance is below its eps: the affine and the eps must each move the oracle's output far beyond the tolerance,
+    so that the case cannot pass without them."""
+    sd0 = _amplified_sd(head_gain=100.0, vis_gain=100.0)
     g = torch.Generator().manual_seed(21)
     N, T = 70, 6
     x = torch.randn(N, T, 1110, generator=g)
+    sd_nc = _with_norm_context(sd0)
+    for sd in (sd0, sd_nc):
+        with torch.no_grad():
+            want = O.updateformer(sd, x[None])[0]
+        packed = eng.pack_weights(sd, DEV)
+        eng.set_option("gemm", impl)
+        try:
+            got = eng.updateformer(packed, x.to(DEV)).cpu()
+        finally:
+            eng.set_option("gemm", 0)
+        scale = float(want.abs().max())
+        err = float((got - want).abs().max())
+        assert err < 2e-4 * max(scale, 1.0), (sd is sd_nc, err, scale)
+    # the same tokens with norm_context back at gamma = 1, beta = 0, and with eps 1e-6 in place of its 1e-5
+    plain = {k: (torch.ones_like(v) if k.endswith("norm_context.weight") else
+                 torch.zeros_like(v) if k.endswith("norm_context.bias") else v) for k, v in sd_nc.items()}
+    ln = O.ln
     with torch.no_grad():
-        want = O.updateformer(sd, x[None])[0]
-    packed = eng.pack_weights(sd, DEV)
-    eng.set_option("gemm", impl)
-    try:
-        got = eng.updateformer(packed, x.to(DEV)).cpu()
-    finally:
-        eng.set_option("gemm", 0)
-    scale = float(want.abs().max())
-    err = float((got - want).abs().max())
-    assert err < 2e-4 * max(scale, 1.0), (err, scale)
+        moved_affine = float((O.updateformer(plain, x[None])[0] - want).abs().max())
+        O.ln = lambda xx, eps, w=None, b=None: ln(xx, 1e-6 if eps == 1e-5 else eps, w, b)
+        try:
+            moved_eps = float((O.updateformer(sd_nc, x[None])[0] - want).abs().max())
+        finally:
+            O.ln = ln
+    tol = 2e-4 * max(scale, 1.0)
+    assert moved_affine > 100 * tol and moved_eps > 100 * tol, (moved_affine, moved_eps, tol)
 
 
 # 0: product kernels (fused wgmma time attention, wgmma + TMA point<-virtual attention for more than 64 points,
