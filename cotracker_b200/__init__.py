@@ -2,5 +2,6 @@
 reference's `cotracker.predictor` API.  See DESIGN.md and include/ct3_b200.h."""
 from .build import build_cotracker  # noqa: F401
 from .predictor import CoTrackerOnlinePredictor, CoTrackerPredictor  # noqa: F401
+from .streams import OnlineStreams  # noqa: F401
 
 __version__ = "0.1.0"

@@ -219,6 +219,89 @@ int ct3_finish_tracks(const float* fwd_tracks, const float* fwd_vis, const float
   return 0;
 }
 
+// ---- streaming windows (online.cu) -----------------------------------------------------------------------------
+namespace {
+constexpr int kOnlineMaxInd = 1 << 30;   // ind + S and |query frame| stay below this: int32 arithmetic in the kernels
+
+// the checks both ct3_online_window_* share; end = window_end's extra conditions.  max_elems: the largest per-stream
+// element count of the kernel (S * n for begin, (ind + T) * n for end)
+int check_online(const ct3_online_stream* st, int K, int S, int step, int stride, int N, bool end, int64_t* max_elems,
+                 const void* workspace, size_t workspace_bytes) {
+  if (!st || !workspace) return fail(CT3_EINVAL, "null argument%s");
+  if (K < 1 || K > 65535) return fail(CT3_EINVAL, "K must be in [1, 65535]%s");
+  if (S < 2 || stride < 1 || N < 1) return fail(CT3_EINVAL, "S must be >= 2, stride and N >= 1%s");
+  if (!end && (step < 1 || step >= S)) return fail(CT3_EINVAL, "step must be in [1, S)%s");
+  if (((uintptr_t)workspace & 15)) return fail(CT3_EINVAL, "workspace must be 16-byte aligned%s");
+  if (workspace_bytes < (size_t)K * sizeof(ct3_online_stream)) return fail(CT3_ENOSPC, "workspace too small%s");
+  int64_t next = 0;
+  *max_elems = 0;
+  for (int k = 0; k < K; ++k) {
+    const ct3_online_stream& s = st[k];
+    if (s.n < 1 || s.first != next || (int64_t)s.first + s.n > N)
+      return fail(CT3_EINVAL, "the streams' tracks must tile [0, N) in order%s");
+    next += s.n;
+    if (s.T < 1 || s.T > S) return fail(CT3_EINVAL, "a stream's T must be in [1, S]%s");
+    if (s.ind < 0 || (int64_t)s.ind + S > kOnlineMaxInd) return fail(CT3_EINVAL, "a stream's ind must be in [0, 2^30 - S]%s");
+    if (s.cap < s.len || s.len < 0) return fail(CT3_EINVAL, "a stream's history must have 0 <= len <= cap%s");
+    const bool reads = end || s.ind > 0;
+    if (reads && (!s.coords || !s.vis || !s.conf)) return fail(CT3_EINVAL, "a stream's history is null%s");
+    if (reads && ((uintptr_t)s.coords & 7)) return fail(CT3_EINVAL, "history coords must be 8-byte aligned%s");
+    int64_t elems = (int64_t)S * s.n;
+    if (!end) {
+      if (s.ind > 0 && s.len < (int64_t)s.ind + (S - step))
+        return fail(CT3_EINVAL, "a stream's history must hold the window's overlap frames%s");
+    } else {
+      if (s.cap < (int64_t)s.ind + s.T) return fail(CT3_EINVAL, "a stream's history must hold ind + T frames%s");
+      if (s.len < s.ind) return fail(CT3_EINVAL, "a stream's history must hold the frames before its window%s");
+      if (s.tracks && (!s.visibility || s.n_keep < 1 || s.n_keep > s.n))
+        return fail(CT3_EINVAL, "a stream's output needs visibility and n_keep in [1, n]%s");
+      if (s.tracks && ((uintptr_t)s.tracks & 7)) return fail(CT3_EINVAL, "output tracks must be 8-byte aligned%s");
+      elems = ((int64_t)s.ind + s.T) * s.n;
+    }
+    if (elems > *max_elems) *max_elems = elems;
+  }
+  if (next != N) return fail(CT3_EINVAL, "the streams' tracks must tile [0, N) in order%s");
+  return 0;
+}
+}  // namespace
+
+int ct3_online_window_begin(const ct3_online_stream* streams_host, int K, int S, int step, int stride, int T_pyr,
+                            const int32_t* qframes, const float* qcoords, int N, uint8_t* valid, uint8_t* entering,
+                            int32_t* rel, float* coords_init, float* vis_init, float* conf_init, void* workspace,
+                            size_t workspace_bytes, ct3_stream_t stream) {
+  if (!qframes || !qcoords || !valid || !entering || !rel || !coords_init || !vis_init || !conf_init)
+    return fail(CT3_EINVAL, "null argument%s");
+  if (((uintptr_t)qcoords | (uintptr_t)coords_init) & 7) return fail(CT3_EINVAL, "coords must be 8-byte aligned%s");
+  int64_t max_elems = 0;
+  if (int rc = check_online(streams_host, K, S, step, stride, N, false, &max_elems, workspace, workspace_bytes)) return rc;
+  for (int k = 0; k < K; ++k)
+    if (streams_host[k].frame0 < 0 || (int64_t)streams_host[k].frame0 + S > T_pyr)
+      return fail(CT3_EINVAL, "a stream's window must lie in the T_pyr pyramid frames%s");
+  cudaStream_t s = (cudaStream_t)stream;
+  auto* dev = reinterpret_cast<ct3_online_stream*>(workspace);
+  CK(cudaMemcpyAsync(dev, streams_host, (size_t)K * sizeof(ct3_online_stream), cudaMemcpyHostToDevice, s),
+     "online_window_begin");
+  CK(launch_online_window_begin(dev, K, max_elems, S, step, 1.0f / (float)stride, qframes, qcoords, N, valid, entering,
+                                rel, coords_init, vis_init, conf_init, s),
+     "online_window_begin");
+  return 0;
+}
+
+int ct3_online_window_end(const ct3_online_stream* streams_host, int K, int S, int stride, const float* coords,
+                          const float* vis, const float* conf, int N, float threshold, void* workspace,
+                          size_t workspace_bytes, ct3_stream_t stream) {
+  if (!coords || !vis || !conf) return fail(CT3_EINVAL, "null argument%s");
+  if ((uintptr_t)coords & 7) return fail(CT3_EINVAL, "coords must be 8-byte aligned%s");
+  int64_t max_elems = 0;
+  if (int rc = check_online(streams_host, K, S, 1, stride, N, true, &max_elems, workspace, workspace_bytes)) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  auto* dev = reinterpret_cast<ct3_online_stream*>(workspace);
+  CK(cudaMemcpyAsync(dev, streams_host, (size_t)K * sizeof(ct3_online_stream), cudaMemcpyHostToDevice, s),
+     "online_window_end");
+  CK(launch_online_window_end(dev, K, max_elems, (float)stride, coords, vis, conf, N, threshold, s), "online_window_end");
+  return 0;
+}
+
 // ---- track visualiser (render.cu) ------------------------------------------------------------------------------
 int ct3_render_prepare(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c,
                        int64_t stride_h, int64_t stride_w, int pad, int grayscale, uint8_t* out, ct3_stream_t stream) {

@@ -1,5 +1,6 @@
 // kernels.cuh -- launchers of the non-GEMM kernels of the update loop (definitions in *.cu).
 #pragma once
+#include "../../include/ct3_b200.h"
 #include "common.cuh"
 
 namespace ct3 {
@@ -32,6 +33,16 @@ cudaError_t launch_finish_tracks(const float* fwd_tracks, const float* fwd_vis, 
                                  const float* bwd_vis, const float* queries, int B, int T, int N, int n_keep,
                                  float threshold, float scale_x, float scale_y, float* tracks, uint8_t* visibility,
                                  cudaStream_t s);
+
+// ---- online.cu : per-window state of K streams (arguments validated by ct3_online_window_*) -------------------
+// streams: the device copy of the K entries; max_elems: the largest per-stream element count (S * n or (ind + T) * n)
+cudaError_t launch_online_window_begin(const ct3_online_stream* streams, int K, int64_t max_elems, int S, int step,
+                                       float inv_stride, const int32_t* qframes, const float* qcoords, int N,
+                                       uint8_t* valid, uint8_t* entering, int32_t* rel, float* coords_init,
+                                       float* vis_init, float* conf_init, cudaStream_t s);
+cudaError_t launch_online_window_end(const ct3_online_stream* streams, int K, int64_t max_elems, float stride,
+                                     const float* coords, const float* vis, const float* conf, int N, float threshold,
+                                     cudaStream_t s);
 
 // ---- render.cu : the track visualiser on uint8 frames [T,H,W,3] (arguments validated by ct3_render_*) ----------
 constexpr int kRenderMaxRadius = 255;   // largest point radius (int(linewidth * 2)) the footprint table holds

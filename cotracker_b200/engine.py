@@ -25,6 +25,15 @@ class EngineError(RuntimeError):
     pass
 
 
+class OnlineStream(ctypes.Structure):
+    """ct3_online_stream (include/ct3_b200.h): one stream of a streaming window pass."""
+    _fields_ = [("coords", ctypes.c_void_p), ("vis", ctypes.c_void_p), ("conf", ctypes.c_void_p),
+                ("cap", ctypes.c_int64), ("len", ctypes.c_int64), ("tracks", ctypes.c_void_p),
+                ("visibility", ctypes.c_void_p), ("ind", ctypes.c_int32), ("T", ctypes.c_int32), ("n", ctypes.c_int32),
+                ("first", ctypes.c_int32), ("frame0", ctypes.c_int32), ("n_keep", ctypes.c_int32),
+                ("scale_x", ctypes.c_float), ("scale_y", ctypes.c_float)]
+
+
 def _signatures():
     """name -> (restype, argtypes) of every entry point of include/ct3_b200.h"""
     c_int, c_size_t, c_void_p, c_char_p = ctypes.c_int, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_char_p
@@ -47,6 +56,11 @@ def _signatures():
                                        c_void_p]),
         "ct3_finish_tracks": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                       ctypes.c_float, ctypes.c_float, ctypes.c_float, c_void_p, c_void_p, c_void_p]),
+        "ct3_online_window_begin": (c_int, [ctypes.POINTER(OnlineStream), c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                            c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_size_t, c_void_p]),
+        "ct3_online_window_end": (c_int, [ctypes.POINTER(OnlineStream), c_int, c_int, c_int, c_void_p, c_void_p,
+                                          c_void_p, c_int, ctypes.c_float, c_void_p, c_size_t, c_void_p]),
         "ct3_render_prepare": (c_int, [c_void_p, c_int, c_int, c_int, c_int, i64, i64, i64, i64, c_int, c_int, c_void_p,
                                        c_void_p]),
         "ct3_render_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
@@ -290,6 +304,84 @@ def finish_tracks(fwd, bwd, queries: torch.Tensor, n_keep: int, threshold: float
           _ptr(None if bwd is None else bwd[1]), _ptr(queries), B, T, N, n_keep, float(threshold), float(scale_xy[0]),
           float(scale_xy[1]), _ptr(tracks), _ptr(visibility), _stream(dev))
     return tracks, visibility
+
+
+QUERY_FRAME_LIMIT = 1 << 30   # ct3_online_window_begin compares query frames clamped to +-2^30
+
+
+def online_stream(hist, length: int, ind: int, T: int, first: int, frame0: int, out=None, n_keep: int = 0,
+                  scale_xy=(1.0, 1.0)) -> OnlineStream:
+    """One entry of a streaming window pass (ct3_online_stream): hist = (coords [cap,n,2], vis [cap,n], conf [cap,n])
+    fp32 histories with `length` valid frames, the window at stream frame `ind` with T real frames, the stream's tracks
+    from `first` in the pass and its window at pyramid frame `frame0`; out = (tracks [ind+T,n_keep,2] fp32,
+    visibility [ind+T,n_keep] bool or uint8) for window_end's predictor output, or None."""
+    c, v, q = hist
+    for t, dtype, name in ((c, torch.float32, "history coords"), (v, torch.float32, "history vis"),
+                           (q, torch.float32, "history conf")):
+        _req(t, dtype, name)
+    cap, n = v.shape
+    if tuple(c.shape) != (cap, n, 2) or tuple(q.shape) != (cap, n):
+        raise EngineError(f"histories must be [cap,n,2], [cap,n], [cap,n], got {tuple(c.shape)}, {tuple(v.shape)}, "
+                          f"{tuple(q.shape)}")
+    e = OnlineStream(c.data_ptr(), v.data_ptr(), q.data_ptr(), cap, int(length), None, None, int(ind), int(T), n,
+                     int(first), int(frame0), 0, float(scale_xy[0]), float(scale_xy[1]))
+    if out is not None:
+        tr, vi = out
+        _req(tr, torch.float32, "tracks")
+        if not vi.is_cuda or vi.dtype not in (torch.bool, torch.uint8) or not vi.is_contiguous():
+            raise EngineError("visibility must be a contiguous CUDA bool or uint8 tensor")
+        rows = int(ind) + int(T)
+        if tuple(tr.shape) != (rows, int(n_keep), 2) or tuple(vi.shape) != (rows, int(n_keep)):
+            raise EngineError(f"output must be [{rows},{n_keep},2] and [{rows},{n_keep}], got {tuple(tr.shape)} and "
+                              f"{tuple(vi.shape)}")
+        e.tracks, e.visibility, e.n_keep = tr.data_ptr(), vi.data_ptr(), int(n_keep)
+    return e
+
+
+def _online_table(streams, device):
+    """Host array of the entries and the device scratch the library copies it into."""
+    table = (OnlineStream * max(1, len(streams)))(*streams)
+    ws = torch.empty(ctypes.sizeof(table), dtype=torch.uint8, device=device)
+    return table, ws
+
+
+def online_window_begin(streams, S: int, step: int, stride: int, T_pyr: int, qframes: torch.Tensor,
+                        qcoords: torch.Tensor):
+    """ct3_online_window_begin: streams = `online_stream` entries of one pass, qframes [N] int32 (stream time, within
+    +-QUERY_FRAME_LIMIT), qcoords [N,2] fp32 (feature-grid units) -> (valid [N] uint8, entering [N] uint8, rel [N]
+    int32, coords_init [S,N,2], vis_init [S,N], conf_init [S,N])."""
+    _req(qframes, torch.int32, "qframes")
+    _req(qcoords, torch.float32, "qcoords")
+    N = qframes.shape[0]
+    dev = qframes.device
+    if tuple(qcoords.shape) != (N, 2) or qcoords.device != dev:
+        raise EngineError(f"qcoords must be [{N},2] on {dev}")
+    valid = torch.empty(N, dtype=torch.uint8, device=dev)
+    entering = torch.empty(N, dtype=torch.uint8, device=dev)
+    rel = torch.empty(N, dtype=torch.int32, device=dev)
+    coords = torch.empty(S, N, 2, dtype=torch.float32, device=dev)
+    vis = torch.empty(S, N, dtype=torch.float32, device=dev)
+    conf = torch.empty(S, N, dtype=torch.float32, device=dev)
+    table, ws = _online_table(streams, dev)
+    _call("ct3_online_window_begin", dev, table, len(streams), int(S), int(step), int(stride), int(T_pyr),
+          _ptr(qframes), _ptr(qcoords), N, _ptr(valid), _ptr(entering), _ptr(rel), _ptr(coords), _ptr(vis), _ptr(conf),
+          _ptr(ws), ws.numel(), _stream(dev))
+    return valid, entering, rel, coords, vis, conf
+
+
+def online_window_end(streams, S: int, stride: int, coords: torch.Tensor, vis: torch.Tensor, conf: torch.Tensor,
+                      threshold: float = 0.6):
+    """ct3_online_window_end: the loop's coords [S,N,2] / vis / conf [S,N] of one pass into the streams' histories,
+    and each entry's predictor output where it has one (see `online_stream`)."""
+    for t, name in ((coords, "coords"), (vis, "vis"), (conf, "conf")):
+        _req(t, torch.float32, name)
+    N = vis.shape[1]
+    dev = coords.device
+    if tuple(coords.shape) != (S, N, 2) or tuple(vis.shape) != (S, N) or tuple(conf.shape) != (S, N):
+        raise EngineError(f"coords, vis, conf must be [{S},N,2], [{S},N], [{S},N]")
+    table, ws = _online_table(streams, dev)
+    _call("ct3_online_window_end", dev, table, len(streams), int(S), int(stride), _ptr(coords), _ptr(vis), _ptr(conf),
+          N, float(threshold), _ptr(ws), ws.numel(), _stream(dev))
 
 
 def render_prepare(src: torch.Tensor, pad: int, grayscale: bool) -> torch.Tensor:

@@ -130,20 +130,30 @@ def plan_passes(group_sizes: Sequence[int], T: int, H4: int, W4: int, budget_byt
 
 def plan_clip_passes(n_clips: int, group_sizes: Sequence[int], T: int, H4: int, W4: int, budget_bytes: int,
                      frames_fn: Optional[Callable[[int], Optional[int]]] = None) -> List[Tuple[int, int]]:
-    """Split the clips of a batch, in order, into passes [b0, b1): as few as keep a pass within `budget_bytes`, and
-    of even size.  Every clip brings the same groups (`group_sizes`, T frames per update loop), so a pass over n clips
-    costs pass_bytes(T, n * sum(group_sizes), n * len(group_sizes), H4, W4, frames_fn(n)); frames_fn(n): the pyramid
-    frames such a pass reads through its frame map (None: it has none).  A pure host function; a clip that alone
-    exceeds the budget gets a pass of its own.  The library takes any number of groups up to the number of tracks,
-    which a batch of clips with at least one track per group cannot exceed."""
-    N, G = sum(group_sizes), len(group_sizes)
-    fit = 1
-    while fit < n_clips and pass_bytes(T, (fit + 1) * N, (fit + 1) * G, H4, W4,
-                                       frames_fn(fit + 1) if frames_fn else None) <= budget_bytes:
-        fit += 1
-    n_passes = -(-n_clips // fit)
-    per = -(-n_clips // n_passes)
-    return [(b0, min(n_clips, b0 + per)) for b0 in range(0, n_clips, per)]
+    """Split the clips of a batch, in order, into passes [b0, b1): as few as keep a pass within `budget_bytes`.
+    group_sizes: the groups every clip brings, or a list of n_clips such lists when the clips (streams) differ.  A pass
+    over clips [b0, b1) costs pass_bytes(T, their tracks, their groups, H4, W4, frames_fn(b1 - b0)) at T frames per
+    update loop; frames_fn(n): the pyramid frames such a pass reads through its frame map (None: it has none).  When
+    every clip brings the same groups the passes are of even size.  A pure host function; a clip that alone exceeds the
+    budget gets a pass of its own.  The library takes any number of groups up to the number of tracks, which a batch
+    of clips with at least one track per group cannot exceed."""
+    ragged = len(group_sizes) > 0 and isinstance(group_sizes[0], (list, tuple))
+    per_clip = [list(g) for g in group_sizes] if ragged else [list(group_sizes)] * n_clips
+    if len(per_clip) != n_clips:
+        raise ValueError(f"{len(per_clip)} group lists for {n_clips} clips")
+    passes, b0, N, G = [], 0, 0, 0
+    for b, sizes in enumerate(per_clip):
+        if b > b0 and pass_bytes(T, N + sum(sizes), G + len(sizes), H4, W4,
+                                 frames_fn(b + 1 - b0) if frames_fn else None) > budget_bytes:
+            passes.append((b0, b))
+            b0, N, G = b, 0, 0
+        N, G = N + sum(sizes), G + len(sizes)
+    if n_clips > 0:
+        passes.append((b0, n_clips))
+    if not ragged and passes:   # same cost per clip: spread the clips evenly over as many passes
+        per = -(-n_clips // len(passes))
+        passes = [(b0, min(n_clips, b0 + per)) for b0 in range(0, n_clips, per)]
+    return passes
 
 
 class EvaluationPredictor(torch.nn.Module):

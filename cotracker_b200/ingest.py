@@ -69,9 +69,10 @@ def model_device(model: torch.nn.Module) -> torch.device:
     return p.device if p is not None else torch.device("cpu")
 
 
-def prepare_video(video: torch.Tensor, out_hw, device) -> torch.Tensor:
+def prepare_video(video: torch.Tensor, out_hw, device, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """video [B,T,3,H,W] uint8 or float (0..255), host or device, any strides -> [B*T,3,oh,ow] fp32 in [-1,1] on device,
     clip after clip; each clip's frames are bit-identical to the call on that clip alone.
+    out: an optional contiguous fp32 [B*T,3,oh,ow] destination on `device` (e.g. a slice of a larger frame batch).
     Other dtypes (float16, float64, ...) are cast to float32 first and then take the float32 path; for pixel values
     0..255 that cast is exact.  (Before this step existed they were resized in their own dtype, so results for them can
     differ from that in the last bits.)"""
@@ -85,7 +86,11 @@ def prepare_video(video: torch.Tensor, out_hw, device) -> torch.Tensor:
     B, T = video.shape[:2]
     if video.is_cuda and video.device != device:
         video = video.to(device)
-    out = torch.empty(B * T, 3, int(out_hw[0]), int(out_hw[1]), dtype=torch.float32, device=device)
+    shape = (B * T, 3, int(out_hw[0]), int(out_hw[1]))
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=device)
+    elif tuple(out.shape) != shape or out.dtype != torch.float32 or out.device != device or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous fp32 {shape} tensor on {device}")
     staging = None
     for b in range(B):
         if video.is_cuda:

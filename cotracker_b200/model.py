@@ -24,6 +24,7 @@ import torch.nn.functional as F
 
 from . import engine
 from .encoder import BasicEncoder
+from .evaluation import pass_budget_bytes, plan_clip_passes
 
 HID, HEADS, VIRT, XDIM = 384, 8, 64, 1110
 
@@ -144,6 +145,70 @@ def _reversed_flags(reversed_groups, G: int) -> List[bool]:
     if len(flags) != G:
         raise engine.EngineError(f"reversed_groups has {len(flags)} entries for {G} groups")
     return flags
+
+
+# ------------------------------------------------------------------------------------------------------
+# streaming: streams that each hold their own window start (CoTrackerThreeOnline._stream_step)
+class StreamState:
+    """One stream of the streaming model: its window start, the history of its tracks and the encoder features of its
+    last chunk's overlap frames.  Its tracks are rows [first, first + n) of the `StreamPool` it belongs to."""
+
+    def __init__(self, n: int, first: int):
+        self.n, self.first = n, first
+        self.ind = 0              # window start (the reference's online_ind)
+        self.length = 0           # frames of history
+        self.hist = None          # (coords * stride [cap,n,2], vis [cap,n], conf [cap,n] logits); frames >= length unset
+        self.enc = None           # (signatures [S-step,2], frame shape, pyramid) of the last chunk's overlap frames
+
+    def reserve(self, frames: int, device):
+        """Room for `frames` history frames: the buffers at least double when they grow, so a stream reallocates
+        O(log length) times."""
+        cap = 0 if self.hist is None else self.hist[1].shape[0]
+        if frames <= cap:
+            return
+        cap = max(frames, 2 * cap)
+        new = (torch.empty(cap, self.n, 2, device=device), torch.empty(cap, self.n, device=device),
+               torch.empty(cap, self.n, device=device))
+        if self.length:
+            for a, b in zip(new, self.hist):
+                a[:self.length] = b[:self.length]
+        self.hist = new
+
+
+class StreamPool:
+    """The tracks of a set of streams, stream after stream: support features [4,49,N,128] (accumulated as queries enter
+    the window), query frames [N] int32 (stream time) and query coordinates [N,2] (feature-grid units).  `open` appends
+    a stream's tracks; `close` removes them with one copy of what follows."""
+
+    def __init__(self):
+        self.streams: List[StreamState] = []
+        self.support = self.qframes = self.qcoords = None
+
+    def open(self, qframes: torch.Tensor, qcoords: torch.Tensor) -> StreamState:
+        n = qframes.shape[0]
+        state = StreamState(n, 0 if self.qframes is None else self.qframes.shape[0])
+        sup = torch.zeros(4, 49, n, 128, device=qframes.device)
+        if self.support is None:
+            self.support, self.qframes, self.qcoords = sup, qframes.contiguous(), qcoords.contiguous()
+        else:
+            self.support = torch.cat([self.support, sup], 2)
+            self.qframes = torch.cat([self.qframes, qframes])
+            self.qcoords = torch.cat([self.qcoords, qcoords])
+        self.streams.append(state)
+        return state
+
+    def close(self, state: StreamState):
+        a, b = state.first, state.first + state.n
+        self.streams.remove(state)
+        if not self.streams:
+            self.support = self.qframes = self.qcoords = None
+            return
+        self.support = torch.cat([self.support[:, :, :a], self.support[:, :, b:]], 2)
+        self.qframes = torch.cat([self.qframes[:a], self.qframes[b:]])
+        self.qcoords = torch.cat([self.qcoords[:a], self.qcoords[b:]])
+        for s in self.streams:
+            if s.first >= b:
+                s.first -= state.n
 
 
 class CoTrackerThreeBase(nn.Module):
@@ -377,47 +442,165 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
 
     def init_video_online_processing(self):
         self.online_ind = 0
-        # The state of B streams that advance in lockstep holds the tracks clip after clip, as the update loop does:
-        self.online_track_support = None          # [4,49,B*N,128], accumulated as queries enter the window
-        self.online_coords_predicted = None       # [T,B*N,2]
-        self.online_vis_predicted = None          # [T,B*N]
-        self.online_conf_predicted = None         # [T,B*N]
-        self._online_enc_cache = None             # ([B,S,2] per-frame checksums, chunk shape, pyramid) of the last chunk
+        # B streams that advance in lockstep: the pool of their tracks, clip after clip, and one state per stream
+        self._online_pool: Optional[StreamPool] = None
+        self._online_streams: List[StreamState] = []
 
-    def _encode_online(self, frames, chunk, step, H4, W4, B=1):
-        """frames [B*S,3,H,W]: the S-frame chunks of the B streams.  Consecutive online chunks overlap by window_len -
-        step frames and the encoder is strictly per-frame (InstanceNorm statistics are per sample), so the features of
-        the overlap are reused bit-for-bit from the previous call and only the new frames are encoded (SURVEY.md 8(f1):
-        the reference re-encodes all 16).  A stream whose overlap does not match its cache is encoded whole, in the
-        same encoder pass as the other streams' new frames."""
-        S = frames.shape[0] // B
+    def _encode_online(self, frames, chunk, step, H4, W4, streams):
+        """frames [K*S,3,H,W]: the S-frame chunks of the K `streams`.  Consecutive online chunks of a stream overlap by
+        window_len - step frames and the encoder is strictly per-frame (InstanceNorm statistics are per sample), so the
+        features of the overlap are reused bit-for-bit from the stream's previous window and only the new frames are
+        encoded (SURVEY.md 8(f1): the reference re-encodes all 16).  A stream whose overlap does not match its cache is
+        encoded whole, in the same encoder pass as the other streams' new frames.  Each stream then keeps the features
+        of its chunk's last window_len - step frames, and only those."""
+        K = len(streams)
+        S = frames.shape[0] // K
         keep = S - step
-        cache = getattr(self, "_online_enc_cache", None)
-        # [B,S,2] float64: one pass over the chunk, 16 numbers per stream to the host
-        sig = self._frame_signatures(frames).unflatten(0, (B, S))
-        pyr = None
-        if cache is not None and self.online_ind > 0 and keep > 0:
-            prev_sig, prev_shape, prev_pyr = cache
-            same = [False] * B
-            if prev_shape == frames.shape and prev_sig.shape == sig.shape:
-                same = (sig[:, :keep] == prev_sig[:, step:]).flatten(1).all(1).tolist()
-            if any(same):
-                v = frames.unflatten(0, (B, S))
-                fresh = [v[b, keep:] if same[b] else v[b] for b in range(B)]
-                fresh = fresh[0] if B == 1 else torch.cat(fresh, 0)
-                new = self._encode(fresh.contiguous(), chunk)
-                runs, n = [], 0
-                for b in range(B):
-                    if same[b]:
-                        runs.append((prev_pyr, B * S, b * S + step, (b + 1) * S))
-                    k = step if same[b] else S
-                    runs.append((new, fresh.shape[0], n, n + k))
-                    n += k
-                pyr = engine.concat_pyramid_runs(runs, H4, W4)
-        if pyr is None:
+        shape = tuple(frames.shape[1:])
+        # [K,S,2] float64: one pass over the chunks; one flag per stream goes to the host
+        sig = self._frame_signatures(frames).unflatten(0, (K, S))
+        same = [False] * K
+        cand = [k for k, s in enumerate(streams) if keep > 0 and s.ind > 0 and s.enc is not None and s.enc[1] == shape]
+        if cand:
+            prev = torch.stack([streams[k].enc[0] for k in cand])
+            for k, eq in zip(cand, (sig[cand, :keep] == prev).flatten(1).all(1).tolist()):
+                same[k] = eq
+        if any(same):
+            v = frames.unflatten(0, (K, S))
+            fresh = [v[k, keep:] if same[k] else v[k] for k in range(K)]
+            fresh = fresh[0] if K == 1 else torch.cat(fresh, 0)
+            new = self._encode(fresh.contiguous(), chunk)
+            runs, n = [], 0
+            for k in range(K):
+                if same[k]:
+                    runs.append((streams[k].enc[2], keep, 0, keep))
+                m = step if same[k] else S
+                runs.append((new, fresh.shape[0], n, n + m))
+                n += m
+            pyr = engine.concat_pyramid_runs(runs, H4, W4)
+        else:
             pyr = self._encode(frames, chunk)
-        self._online_enc_cache = (sig, frames.shape, pyr)
+        if keep > 0:
+            for k, s in enumerate(streams):
+                s.enc = (sig[k, step:], shape, engine.concat_pyramid_runs([(pyr, K * S, k * S + step, (k + 1) * S)],
+                                                                          H4, W4))
         return pyr
+
+    def stream_advance_error(self, state: "StreamState", T: int) -> Optional[str]:
+        """Why `state` cannot advance by a chunk of T frames (None: it can).  The history of a stream is the window
+        results of its frames so far; a window at `ind` > 0 needs the previous window's overlap and extends the history
+        by min(step, T - step) frames, to ind + T.  After a chunk shorter than the window that no longer holds."""
+        S = self.window_len
+        step = S // 2
+        if not 1 <= T <= S:
+            return f"a chunk must hold 1 to window_len = {S} frames, got {T}"
+        if state.ind > 0 and (state.length != state.ind + S - step or state.length + min(step, T - step) != state.ind + T):
+            return "the stream has ended: its last chunk was shorter than the window"
+        return None
+
+    def _stream_step(self, pool: "StreamPool", streams, frames, Ts, iters, chunk=200, outputs=None):
+        """Advance each of `streams` (states of `pool`, in pool order) by one window, in as few update-loop passes as
+        fit in device memory.  frames [K*S,3,H,W] in [-1,1]: stream k's chunk of Ts[k] frames, padded to S frames with
+        copies of its last frame.  outputs: per stream None, or (n_keep, scale_xy) for the online predictor's output.
+        -> per stream None or (tracks [ind+T,n_keep,2] fp32, visibility [ind+T,n_keep] bool) of all its frames so far.
+        Every stream's result is bit-identical to advancing it alone: streams are independent query groups, each reading
+        its own S frames of one pyramid."""
+        K = len(streams)
+        S = self.window_len
+        step = S // 2
+        _, _, H, W = frames.shape
+        H4, W4 = H // self.stride, W // self.stride
+        dev = frames.device
+        for s, T in zip(streams, Ts):
+            err = self.stream_advance_error(s, T)
+            if err:
+                raise ValueError(err)
+        outputs = outputs or [None] * K
+        pyr = self._encode_online(frames, chunk, step, H4, W4, streams)
+        T_pyr = K * S
+        for s, T in zip(streams, Ts):
+            s.reserve(s.ind + T, dev)
+        passes = [(0, K)]
+        if K > 1:
+            budget = pass_budget_bytes(self, dev, T_pyr, H, W)
+            passes = plan_clip_passes(K, [[s.n] for s in streams], S, H4, W4, budget, lambda n: T_pyr)
+        results = [None] * K
+        for b0, b1 in passes:
+            sub = streams[b0:b1]
+            in_place = sub == pool.streams
+            if in_place:
+                support, qframes, qcoords = pool.support, pool.qframes, pool.qcoords
+            else:   # the support rows of these streams in pass scratch, written back after the pass
+                idx = torch.cat([torch.arange(s.first, s.first + s.n) for s in sub]).to(dev)
+                support = pool.support.index_select(2, idx)
+                qframes, qcoords = pool.qframes[idx], pool.qcoords[idx]
+            entries, first = [], 0
+            for k, s in enumerate(sub, b0):
+                out = None
+                if outputs[k] is not None:
+                    n_keep, scale = outputs[k]
+                    rows = s.ind + Ts[k]
+                    out = (torch.empty(rows, n_keep, 2, device=dev), torch.empty(rows, n_keep, dtype=torch.bool,
+                                                                                 device=dev))
+                    results[k] = out
+                entries.append(engine.online_stream(s.hist, s.length, s.ind, Ts[k], first, k * S, out,
+                                                    *(outputs[k] or (0, (1.0, 1.0)))))
+                first += s.n
+            valid, entering, rel, coords, vis, conf = engine.online_window_begin(entries, S, step, self.stride, T_pyr,
+                                                                                 qframes, qcoords)
+            engine.sample_support(pyr, T_pyr, H4, W4, rel, qcoords, support=support, accumulate_mask=entering)
+            frame_map = None if K == 1 else [[k * S + t for t in range(S)] for k in range(b0, b1)]
+            self._refine(pyr, H4, W4, support, valid, coords, vis, conf, iters, [s.n for s in sub], frame_map)
+            engine.online_window_end(entries, S, self.stride, coords, vis, conf)
+            if not in_place:
+                pool.support.index_copy_(2, idx, support)
+        for s, T in zip(streams, Ts):
+            s.length = s.ind + T
+            s.ind += step
+        return results
+
+    def _lockstep_streams(self, queries):
+        """The pool and states of the B streams of queries [B,N,3] that advance in lockstep (opened at the first chunk
+        after init_video_online_processing); the query points are taken from this call's queries."""
+        B, N = queries.shape[:2]
+        qframes, qcoords = self._stream_queries(queries.reshape(B * N, 3))
+        if self._online_pool is None:
+            self._online_pool = StreamPool()
+            self._online_streams = [self._online_pool.open(qframes[b * N:(b + 1) * N], qcoords[b * N:(b + 1) * N])
+                                    for b in range(B)]
+        pool = self._online_pool
+        if pool.qframes.shape[0] != B * N:
+            raise ValueError(f"the video was started with {pool.qframes.shape[0]} tracks, these queries hold {B * N}")
+        pool.qframes, pool.qcoords = qframes, qcoords
+        return pool, self._online_streams
+
+    def _stream_queries(self, queries):
+        """queries [n,3] (t, x, y) at model resolution -> (query frames [n] int32 within +-QUERY_FRAME_LIMIT, query
+        coordinates [n,2] fp32 in feature-grid units)."""
+        lim = engine.QUERY_FRAME_LIMIT
+        qframes = queries[:, 0].long().clamp(-lim, lim).to(torch.int32).contiguous()
+        return qframes, (queries[:, 1:3].float() / self.stride).contiguous()
+
+    def _track_online(self, frames, queries, iters, chunk=200, predict=None):
+        """One streaming step of the B streams of queries [B,N,3] in lockstep; frames [B*T,3,H,W] in [-1,1], T <=
+        window_len.  -> the model's (coords, vis, conf) [B, frames so far, N, ...], or with predict = (n_keep,
+        scale_xy) the online predictor's (tracks [B,.,n_keep,2], visibility [B,.,n_keep] bool)."""
+        B = queries.shape[0]
+        T = frames.shape[0] // B
+        S = self.window_len
+        assert T <= S, "Online mode: video chunk must be <= window size."
+        assert getattr(self, "online_ind", None) is not None, "Call model.init_video_online_processing() first."
+        if S > T:
+            v = frames.unflatten(0, (B, T))
+            frames = torch.cat([v, v[:, -1:].expand(-1, S - T, -1, -1, -1)], 1).flatten(0, 1)
+        pool, streams = self._lockstep_streams(queries)
+        outs = self._stream_step(pool, streams, frames, [T] * B, iters, chunk, [predict] * B)
+        self.online_ind += S // 2
+        if predict is not None:
+            return tuple(torch.stack([o[i] for o in outs]) for i in range(2))
+        L = streams[0].length
+        coords, vis, conf = (torch.stack([s.hist[i][:L] for s in streams]) for i in range(3))
+        return coords, torch.sigmoid(vis), torch.sigmoid(conf), None
 
     def _frame_signatures(self, frames: torch.Tensor) -> torch.Tensor:
         """Two order-sensitive checksums per frame (plain sum and a position-weighted sum, float64 accumulators):
@@ -458,27 +641,20 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
         B = queries.shape[0]
         BT, _, H, W = frames.shape
         T = BT // B
-        S = self.window_len
-        assert S >= 2
+        assert self.window_len >= 2
         if is_online:
-            assert T <= S, "Online mode: video chunk must be <= window size."
-            assert getattr(self, "online_ind", None) is not None, "Call model.init_video_online_processing() first."
-            H4, W4 = H // self.stride, W // self.stride
-            if S > T:
-                v = frames.unflatten(0, (B, T))
-                frames = torch.cat([v, v[:, -1:].expand(-1, S - T, -1, -1, -1)], 1).flatten(0, 1)
-            pyr_all = self._encode_online(frames, fmaps_chunk_size, S // 2, H4, W4, B)
-        else:
-            pyr_all = self._encode_clip(frames, fmaps_chunk_size, B)
-        return self._track_pyramid(pyr_all, T, H, W, queries, iters, group_sizes, is_online, reversed_groups)
+            if any(_reversed_flags(reversed_groups, len(group_sizes))) or len(group_sizes) != 1:
+                raise NotImplementedError("streaming (is_online=True) tracks one forward group per stream")
+            return self._track_online(frames, queries, iters, fmaps_chunk_size)
+        pyr_all = self._encode_clip(frames, fmaps_chunk_size, B)
+        return self._track_pyramid(pyr_all, T, H, W, queries, iters, group_sizes, reversed_groups=reversed_groups)
 
-    def _track_pyramid(self, pyr_all, T, H, W, queries, iters, group_sizes, is_online=False, reversed_groups=None,
-                       clips=None):
-        """The model after the encoder: pyr_all = the pyramid of the clips, each T frames and the padding
-        (`_encode_clip`).  group_sizes, reversed_groups: the G groups of one clip's N queries (every clip has the same),
-        G flags; a flagged group tracks the clip played backwards (see `forward_groups`).  With reversed groups or more
-        than one clip each window runs on the frames its groups reference (at most 2 S per clip), gathered from
-        pyr_all, through a frame map.
+    def _track_pyramid(self, pyr_all, T, H, W, queries, iters, group_sizes, reversed_groups=None, clips=None):
+        """The model after the encoder, sliding windows over whole clips (streaming is `_stream_step`): pyr_all = the
+        pyramid of the clips, each T frames and the padding (`_encode_clip`).  group_sizes, reversed_groups: the G
+        groups of one clip's N queries (every clip has the same), G flags; a flagged group tracks the clip played
+        backwards (see `forward_groups`).  With reversed groups or more than one clip each window runs on the frames its
+        groups reference (at most 2 S per clip), gathered from pyr_all, through a frame map.
         clips: the clip of the pyramid each of the B rows of `queries` tracks (None: 0 .. B-1, the whole pyramid).
         Below, N counts the tracks of all B clips, clip after clip."""
         dev = pyr_all.device
@@ -487,13 +663,9 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
         S = self.window_len
         step = S // 2
         H4, W4 = H // self.stride, W // self.stride
-        T_pad = T + ((S - T) if is_online else self._clip_pad(T))
+        T_pad = T + self._clip_pad(T)
         flags = _reversed_flags(reversed_groups, len(group_sizes))
-        if is_online and any(flags):
-            raise NotImplementedError("streaming (is_online=True) does not track reversed groups")
         clips, plain = self._pass_clips(B, clips)
-        if is_online and clips != list(range(B)):
-            raise NotImplementedError("streaming (is_online=True) advances every stream of the batch together")
         T_all = T_pad if plain else engine.pyramid_frames(pyr_all, H4, W4)
         clip_off = None if plain else self._clip_offsets(clips, T_pad, queries.shape[1], dev)
         G1 = len(flags)                                   # groups of one clip
@@ -504,40 +676,21 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
         coords_pred = torch.zeros(T, N, 2, device=dev)
         vis_pred = torch.zeros(T, N, device=dev)
         conf_pred = torch.zeros(T, N, device=dev)
-        if is_online and self.online_coords_predicted is not None:
-            grow = min(step, T - step)
-            coords_pred = F.pad(self.online_coords_predicted, (0, 0, 0, 0, 0, grow))
-            vis_pred = F.pad(self.online_vis_predicted, (0, 0, 0, grow))
-            conf_pred = F.pad(self.online_conf_predicted, (0, 0, 0, grow))
 
         # support features of every track at its query frame
-        if is_online:
-            left = 0 if self.online_ind == 0 else self.online_ind + step
-            right = self.online_ind + S
-            entering = ((qframes_l >= left) & (qframes_l < right)).to(torch.uint8).contiguous()
-            if self.online_track_support is None:
-                self.online_track_support = torch.zeros(4, 49, N, 128, device=dev)
-            rel = (qframes_l - self.online_ind).clamp(0, T_pad - 1)
-            if not plain:
-                rel = rel + clip_off
-            engine.sample_support(pyr_all, T_all, H4, W4, rel.to(torch.int32).contiguous(), qcoords,
-                                  support=self.online_track_support, accumulate_mask=entering)
-            support = self.online_track_support
-        else:
-            qf = qframes_l.clamp(0, T_pad - 1)
-            if any(flags):   # frame q of the reversed, padded clip is forward frame max(T-1-q, 0)
-                qf = torch.where(self._track_reversed(group_sizes, flags, dev), (T - 1 - qf).clamp(min=0), qf)
-            if not plain:
-                qf = qf + clip_off
-            support = engine.sample_support(pyr_all, T_all, H4, W4, qf.to(torch.int32).contiguous(), qcoords)
+        qf = qframes_l.clamp(0, T_pad - 1)
+        if any(flags):   # frame q of the reversed, padded clip is forward frame max(T-1-q, 0)
+            qf = torch.where(self._track_reversed(group_sizes, flags, dev), (T - 1 - qf).clamp(min=0), qf)
+        if not plain:
+            qf = qf + clip_off
+        support = engine.sample_support(pyr_all, T_all, H4, W4, qf.to(torch.int32).contiguous(), qcoords)
 
         coords_init = qcoords[None].expand(S, N, 2).contiguous()
         vis_init = torch.zeros(S, N, device=dev)
         conf_init = torch.zeros(S, N, device=dev)
         num_windows = (T - S + step - 1) // step + 1
-        starts = [self.online_ind] if is_online else list(range(0, step * num_windows, step))
 
-        for ind in starts:
+        for ind in range(0, step * num_windows, step):
             if ind > 0:
                 # warm start from the overlap with the previous window (reference :457-482)
                 overlap = S - step
@@ -553,11 +706,7 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
                 conf_init = torch.where(carry, prev_q, conf_init)
             valid = (qframes_l < ind + S).to(torch.uint8).contiguous()                      # reference :484,:493-496
             frame_map = None
-            if is_online:
-                pyr = pyr_all       # the S-frame chunks of the streams, one after another
-                if not plain:
-                    frame_map = batch_frame_map([list(range(S))] * G1, clips, S)
-            elif any(flags) or not plain:
+            if any(flags) or not plain:
                 runs, frame_map = batch_gather_plan(window_frame_map(T, S, ind, flags[:G1]), clips, T_pad)
                 pyr = gather_pyramid(pyr_all, T_all, H4, W4, runs)
             else:
@@ -566,15 +715,10 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
             vis = vis_init.clone().contiguous()
             conf = conf_init.clone().contiguous()
             self._refine(pyr, H4, W4, support, valid, coords, vis, conf, iters, group_sizes, frame_map)
-            S_trim = T if is_online else min(T - ind, S)
+            S_trim = min(T - ind, S)
             coords_pred[ind:ind + S] = (coords * float(self.stride))[:S_trim]
             vis_pred[ind:ind + S] = vis[:S_trim]
             conf_pred[ind:ind + S] = conf[:S_trim]
 
-        if is_online:
-            self.online_ind += step
-            self.online_coords_predicted = coords_pred
-            self.online_vis_predicted = vis_pred
-            self.online_conf_predicted = conf_pred
         return (self._batched(coords_pred, B), self._batched(torch.sigmoid(vis_pred), B),
                 self._batched(torch.sigmoid(conf_pred), B), None)

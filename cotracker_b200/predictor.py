@@ -239,37 +239,45 @@ class CoTrackerOnlinePredictor(torch.nn.Module):
     def forward(self, video_chunk, is_first_step: bool = False, queries: torch.Tensor = None, grid_size: int = 5,
                 grid_query_frame: int = 0, add_support_grid=False):
         B, T, C, H, W = video_chunk.shape
-        ih, iw = self.interp_shape
         dev = ingest.model_device(self.model)
         if is_first_step:
             # (re)start a video: reset the model state and remember the queries (reference :242-274)
             self.model.init_video_online_processing()
-            if queries is not None:
-                B, N, D = queries.shape
-                self.N = N
-                assert D == 3
-                queries = queries.to(dev).clone()
-                queries[:, :, 1:] *= queries.new_tensor([(iw - 1) / (W - 1), (ih - 1) / (H - 1)])
-                if add_support_grid:
-                    sup = get_points_on_a_grid(self.support_grid_size, self.interp_shape, device=dev)
-                    sup = torch.cat([torch.zeros_like(sup[:, :, :1]), sup], dim=2).repeat(B, 1, 1)
-                    queries = torch.cat([queries, sup], dim=1)
-            elif grid_size > 0:
-                grid_pts = get_points_on_a_grid(grid_size, self.interp_shape, device=dev)
-                self.N = grid_size ** 2
-                queries = torch.cat([torch.ones_like(grid_pts[:, :, :1]) * grid_query_frame, grid_pts], dim=2)
-                queries = queries.repeat(B, 1, 1)
-            self.queries = queries
+            self.queries, self.N = self._first_step_queries(B, (H, W), queries, grid_size, grid_query_frame,
+                                                            add_support_grid, dev)
             return (None, None)
 
         if self.queries.shape[0] != B:   # the B streams of the first step advance together
             raise ValueError(f"the video was started with {self.queries.shape[0]} streams, this chunk holds {B}")
         frames = ingest.prepare_video(video_chunk, self.interp_shape, dev)
-        tracks, visibilities, confidence, __ = self.model._track_frames(frames, self.queries, iters=6, is_online=True)
-        if add_support_grid:
-            tracks = tracks[:, :, :self.N]
-            visibilities = visibilities[:, :, :self.N]
-            confidence = confidence[:, :, :self.N]
-        visibilities = visibilities * confidence
-        scale = tracks.new_tensor([(W - 1) / (iw - 1), (H - 1) / (ih - 1)])
-        return tracks * scale, visibilities > 0.6
+        return self.model._track_online(frames, self.queries, 6, predict=self._tail(add_support_grid, (H, W)))
+
+    def _first_step_queries(self, B, frame_hw, queries, grid_size, grid_query_frame, add_support_grid, dev):
+        """The queries [B,N,3] at model resolution a video started with these first-step arguments tracks, and the
+        number of them the output keeps (reference :242-274)."""
+        H, W = frame_hw
+        ih, iw = self.interp_shape
+        N = None
+        if queries is not None:
+            B, N, D = queries.shape
+            assert D == 3
+            queries = queries.to(dev).clone()
+            queries[:, :, 1:] *= queries.new_tensor([(iw - 1) / (W - 1), (ih - 1) / (H - 1)])
+            if add_support_grid:
+                sup = get_points_on_a_grid(self.support_grid_size, self.interp_shape, device=dev)
+                sup = torch.cat([torch.zeros_like(sup[:, :, :1]), sup], dim=2).repeat(B, 1, 1)
+                queries = torch.cat([queries, sup], dim=1)
+        elif grid_size > 0:
+            grid_pts = get_points_on_a_grid(grid_size, self.interp_shape, device=dev)
+            N = grid_size ** 2
+            queries = torch.cat([torch.ones_like(grid_pts[:, :, :1]) * grid_query_frame, grid_pts], dim=2)
+            queries = queries.repeat(B, 1, 1)
+        return queries, N
+
+    def _tail(self, add_support_grid, frame_hw):
+        """(n_keep, scale_xy) of the output of a call on H x W chunks: the support grid dropped when the call asks for
+        it, the tracks scaled from the model's resolution to the chunk's (reference :276-309)."""
+        H, W = frame_hw
+        ih, iw = self.interp_shape
+        n_keep = self.N if add_support_grid else self.queries.shape[1]
+        return n_keep, ((W - 1) / (iw - 1), (H - 1) / (ih - 1))

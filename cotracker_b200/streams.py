@@ -1,0 +1,110 @@
+"""Independent online streams in one update-loop pass.
+
+    hub = OnlineStreams(predictor)                  # a CoTrackerOnlinePredictor; the hub shares its model
+    a = hub.open(frame_size=(720, 1280), grid_size=10)
+    b = hub.open(frame_size=(480, 640), queries=q, add_support_grid=True)
+    hub.push(a, chunk_a)                            # [1,T,3,H,W], T <= window_len, uint8 or float, host or device
+    hub.push(b, chunk_b)
+    out = hub.step()                                # {stream id: (tracks [1,T_so_far,N,2], visibility [1,T_so_far,N])}
+    hub.close(a)
+
+Each stream has its own frame size, queries, start and pace.  `step()` advances every stream with a pushed chunk by one
+window: their chunks are resized into one frame batch, their new frames go through one encoder pass, and their tracks
+run as query groups of one update loop (or of a few, when they do not fit in device memory at once).  For every stream,
+the results of the steps that advanced it are bit-identical to a fresh predictor on the same model called with
+`is_first_step=True` and the `open()` arguments, then with that stream's chunks in order and the same
+`add_support_grid`; whatever the other streams do.
+"""
+from __future__ import annotations
+
+from typing import Dict, Tuple
+
+import torch
+
+from . import ingest
+from .model import StreamPool
+
+
+class OnlineStreams:
+    def __init__(self, predictor):
+        self.predictor = predictor
+        self.model = predictor.model
+        self.pool = StreamPool()
+        self._streams: Dict[int, dict] = {}     # id -> the stream's state, open arguments and output shape
+        self._pending: Dict[int, torch.Tensor] = {}
+        self._next_id = 0
+
+    @torch.no_grad()
+    def open(self, frame_size: Tuple[int, int], queries: torch.Tensor = None, grid_size: int = 5,
+             grid_query_frame: int = 0, add_support_grid: bool = False) -> int:
+        """Start a stream of frames of frame_size = (H, W): the arguments of the predictor's `is_first_step=True` call,
+        with the frame size in place of the first chunk.  -> the stream's id."""
+        H, W = (int(x) for x in frame_size)
+        if H < 2 or W < 2:
+            raise ValueError(f"frame_size must be (H, W) with H, W >= 2, got {tuple(frame_size)}")
+        if queries is None and grid_size <= 0:
+            raise ValueError("open() needs queries or grid_size > 0")
+        if queries is not None and (queries.dim() != 3 or queries.shape[0] != 1 or queries.shape[1] < 1
+                                    or queries.shape[2] != 3):
+            raise ValueError(f"queries must be [1,N,3] with N >= 1, got {tuple(queries.shape)}")
+        dev = ingest.model_device(self.model)
+        if dev.type != "cuda":
+            raise ValueError("the predictor's model must be on a CUDA device")
+        q, n_out = self.predictor._first_step_queries(1, (H, W), queries, grid_size, grid_query_frame,
+                                                      add_support_grid, dev)
+        state = self.pool.open(*self.model._stream_queries(q[0]))
+        sid = self._next_id
+        self._next_id += 1
+        n_keep = n_out if add_support_grid else q.shape[1]
+        ih, iw = self.predictor.interp_shape
+        self._streams[sid] = dict(state=state, hw=(H, W), out=(n_keep, ((W - 1) / (iw - 1), (H - 1) / (ih - 1))))
+        return sid
+
+    def _get(self, sid: int) -> dict:
+        if sid not in self._streams:
+            raise KeyError(f"no open stream {sid}")
+        return self._streams[sid]
+
+    def push(self, sid: int, chunk: torch.Tensor):
+        """Queue the next chunk [1,T,3,H,W] of stream `sid` (T <= window_len) for the next `step()`."""
+        s = self._get(sid)
+        if sid in self._pending:
+            raise ValueError(f"stream {sid} already has a chunk for this step")
+        if chunk.dim() != 5 or chunk.shape[0] != 1 or chunk.shape[2] != 3 or tuple(chunk.shape[3:]) != s["hw"]:
+            raise ValueError(f"stream {sid} takes chunks [1,T,3,{s['hw'][0]},{s['hw'][1]}], got {tuple(chunk.shape)}")
+        err = self.model.stream_advance_error(s["state"], chunk.shape[1])
+        if err:
+            raise ValueError(f"stream {sid}: {err}")
+        self._pending[sid] = chunk
+
+    def close(self, sid: int):
+        """End stream `sid`: its tracks leave the pool and its id is no longer valid."""
+        s = self._get(sid)
+        self._pending.pop(sid, None)
+        self.pool.close(s["state"])
+        del self._streams[sid]
+
+    @torch.no_grad()
+    def step(self) -> Dict[int, Tuple[torch.Tensor, torch.Tensor]]:
+        """Advance every stream with a pushed chunk by one window, in one pass.  -> {id: (tracks [1,T_so_far,n,2] fp32,
+        visibility [1,T_so_far,n] bool)} of the streams it advanced; the others keep their state."""
+        order = {id(s): k for k, s in enumerate(self.pool.streams)}
+        ids = sorted(self._pending, key=lambda i: order[id(self._streams[i]["state"])])
+        if not ids:
+            return {}
+        S = self.model.window_len
+        ih, iw = self.predictor.interp_shape
+        dev = ingest.model_device(self.model)
+        frames = torch.empty(len(ids) * S, 3, ih, iw, dtype=torch.float32, device=dev)
+        Ts = []
+        for k, sid in enumerate(ids):
+            chunk = self._pending[sid]
+            T = chunk.shape[1]
+            ingest.prepare_video(chunk, (ih, iw), dev, out=frames[k * S:k * S + T])
+            if T < S:   # the model pads a short chunk with copies of its last frame
+                frames[k * S + T:(k + 1) * S] = frames[k * S + T - 1]
+            Ts.append(T)
+        self._pending.clear()
+        outs = self.model._stream_step(self.pool, [self._streams[i]["state"] for i in ids], frames, Ts, 6,
+                                       outputs=[self._streams[i]["out"] for i in ids])
+        return {sid: (tr[None], vi[None]) for sid, (tr, vi) in zip(ids, outs)}

@@ -128,6 +128,54 @@ int ct3_finish_tracks(const float* fwd_tracks, const float* fwd_vis, const float
                       const float* queries, int B, int T, int N, int n_keep, float threshold, float scale_x,
                       float scale_y, float* tracks, uint8_t* visibility, ct3_stream_t stream);
 
+/* ---- streaming windows (cotracker3_online.py:457-541, predictor.py:276-309) ------------------------------------
+ * One update-loop pass of the online model advances K streams by one window each.  Stream k holds tracks
+ * [first, first + n) of the pass (streams follow each other: first_0 = 0, first_{k+1} = first_k + n_k, sum n_k = N),
+ * its window starts at frame `ind` of the stream, its chunk has T real frames (window frames T..S-1 are padding) and
+ * its window is pyramid frames [frame0, frame0 + S) of the pass.  Its history (coords * stride at model resolution,
+ * visibility and confidence logits; frame t, track j at t * n + j) has `len` valid frames of `cap` allocated.
+ * `streams_host` is a HOST array of K entries; the library copies it into `workspace` (at least
+ * K * sizeof(ct3_online_stream) bytes, 16-byte aligned) on `stream`, so the host array may be reused on return. */
+typedef struct {
+  float* coords;          /* history [cap, n, 2] fp32                                                           */
+  float* vis;             /* history [cap, n] fp32                                                              */
+  float* conf;            /* history [cap, n] fp32                                                              */
+  int64_t cap;            /* frames the history buffers hold                                                    */
+  int64_t len;            /* valid history frames before the window                                             */
+  float* tracks;          /* window_end: predictor output [ind + T, n_keep, 2] fp32, or NULL                     */
+  uint8_t* visibility;    /* window_end: predictor output [ind + T, n_keep] uint8 (0 | 1)                        */
+  int32_t ind, T, n, first, frame0;
+  int32_t n_keep;         /* window_end: the first n_keep tracks are output (the trailing support grid is dropped) */
+  float scale_x, scale_y; /* window_end: output tracks = history * (scale_x, scale_y), one fp32 multiply each     */
+} ct3_online_stream;
+/* ct3_online_window_begin: the per-window state the update loop starts from, bit-identical to the torch expressions
+ * (qf = qframes[i], the query frame in stream time; overlap = S - step):
+ *   valid[i] = qf < ind + S;   entering[i] = left <= qf < ind + S with left = 0 at ind == 0, else ind + step;
+ *   rel[i] = clamp(qf - ind, 0, S - 1) + frame0 (the frame sample_support reads the query's features from);
+ *   for t in [0, S): where ind > 0 and qf < ind + overlap, the warm start from the history frame
+ *   r = ind + min(t, overlap - 1): coords_init[t,i] = coords[r,j] * (1 / stride), vis_init / conf_init = vis / conf
+ *   [r,j]; elsewhere coords_init[t,i] = qcoords[i], vis_init = conf_init = 0.
+ * qframes [N] int32, qcoords [N,2] fp32 (feature-grid units); valid, entering [N] uint8, rel [N] int32,
+ * coords_init [S,N,2], vis_init, conf_init [S,N] fp32.  Null pointers, K outside [1, 65535], S < 2, step outside
+ * [1, S), stride < 1, a stream whose tracks do not tile [0, N) in order, T outside [1, S], ind < 0 or ind + S > 2^30,
+ * frame0 + S > T_pyr, or (ind > 0) a null history or len < ind + overlap or cap < len return CT3_EINVAL, a small
+ * workspace CT3_ENOSPC, before any launch.  Query frames beyond +-2^30 compare as +-2^30. */
+int ct3_online_window_begin(const ct3_online_stream* streams_host, int K, int S, int step, int stride, int T_pyr,
+                            const int32_t* qframes, const float* qcoords, int N, uint8_t* valid, uint8_t* entering,
+                            int32_t* rel, float* coords_init, float* vis_init, float* conf_init, void* workspace,
+                            size_t workspace_bytes, ct3_stream_t stream);
+/* ct3_online_window_end: the loop's result into the histories and the predictor's output, bit-identical to
+ *   history[ind + t, j] = (coords[t, first + j] * stride, vis[...], conf[...])   for t < T  (frames ind + T.. untouched)
+ *   tracks[t, j] = history_coords[t, j] * (scale_x, scale_y),
+ *   visibility[t, j] = sigmoid(history_vis[t, j]) * sigmoid(history_conf[t, j]) > threshold   for t < ind + T, j < n_keep
+ * with sigmoid(x) = 1 / (1 + expf(-x)) in fp32, as torch.sigmoid evaluates it.  coords [S,N,2], vis, conf [S,N] fp32:
+ * the update loop's state (feature-grid units, logits).  The same argument checks as window_begin (without T_pyr and
+ * the overlap), plus cap < ind + T, len < ind, and a stream with `tracks` whose visibility is NULL or n_keep is outside
+ * [1, n]. */
+int ct3_online_window_end(const ct3_online_stream* streams_host, int K, int S, int stride, const float* coords,
+                          const float* vis, const float* conf, int N, float threshold, void* workspace,
+                          size_t workspace_bytes, ct3_stream_t stream);
+
 /* ---- track visualiser (reference cotracker/utils/visualizer.py) ---------------
  * Frames are uint8 [T,H,W,3] contiguous on the device, drawn in place; every result is bit-identical to the reference's
  * PIL drawing (footprint rules: render.cu).  T <= 65535.
