@@ -1,5 +1,6 @@
 // api_loop.cu -- the update loop of the C ABI (see include/ct3_b200.h): weight packing, workspace carving and the
-// launch sequence of one refinement iteration (cotracker3_offline.py:139-216, cotracker.py:483-531).
+// launch sequence of one refinement iteration (cotracker3_offline.py:139-216, cotracker.py:483-531), whole or in
+// track slabs (ct3_update_loop_slabbed, DESIGN.md §4.4.5).
 #include <math.h>
 
 #include <string>
@@ -101,23 +102,30 @@ const std::vector<std::string>& weight_names() {
 }
 
 // ------------------------------------------------------------------------------------------------
-// workspace
+// workspace.  Without track slabs (slab == N) every buffer covers all rows.  With them (ct3_update_loop_slabbed,
+// slab < N) the scratch of the row-independent stages (vol, h1, xs, hmid, and the first S = slab*T rows of ln / att /
+// qkv) holds one slab of rows; ln / att keep the virtual rows full-size behind it; qkv is also the full-size space-
+// attention operand of the point rows (virtual<-point k|v [N*T, 768], then point<-virtual q [N*T, 384] followed by
+// its split output [N*T, 2*384]), which is never live at the same time as a time block's q|k|v.
 struct Workspace {
-  __nv_bfloat16* vol;     // [N*T*4, 2*2432]
-  __nv_bfloat16* h1;      // [N*T*4, 2*384]
-  __nv_bfloat16* xs;      // [N*T, 2*1152]
+  __nv_bfloat16* vol;     // [S*4, 2*2432]
+  __nv_bfloat16* h1;      // [S*4, 2*384]
+  __nv_bfloat16* xs;      // [S, 2*1152]
   float* tokens;          // [(N+64)*T, 384]
-  __nv_bfloat16* ln;      // [(N+64)*T, 2*384]
-  __nv_bfloat16* att;     // [(N+64)*T, 2*384]
-  float* qkv;             // [(N+64)*T, 1152]   (also point q [N*T,384] / point kv [N*T,768])
+  __nv_bfloat16* ln;      // [S + 64*T, 2*384]  (virtual rows from row S)
+  __nv_bfloat16* att;     // [S + 64*T, 2*384]  (virtual rows from row S)
+  float* qkv;             // [(N+64)*T, 1152]; slabbed: max(S*1152, N*T*768)   (also point q / point kv / p<-v output)
   float* vqkv;            // [64*T, 1152]       (virtual q / kv / qkv)
-  __nv_bfloat16* hmid;    // [(N+64)*T, 2*1536]
+  __nv_bfloat16* hmid;    // [S + 64*T, 2*1536]; slabbed: [S, 2*1536]
   float* row_bias;        // [T, 384]
   float* att_part;        // split-K partials of the virtual<-point attention
   __nv_bfloat16* pyr_split;  // split-bf16 copy of the pyramid (corr_tc2.cu); null when H4 == 0
   int32_t* groups;        // device group table of a grouped call (GroupPlan); null when G == 1
   int32_t* frames;        // device frame map [G, T] of ct3_update_loop_frames; null without one
+  int slab;               // tracks per slab; N: no slabs
   size_t total;
+  bool slabbed() const { return slab_rows < point_rows; }
+  int64_t slab_rows = 0, point_rows = 0;   // S and N*T
 };
 // split-K slots of the virtual<-point partials: a group of n tracks splits at most min(32, ceil(n/64)/2) ways
 // (attention_tc_splits), so G groups of N tracks in all need at most (N + 63 G)/128 slots beyond one group's 32
@@ -129,21 +137,28 @@ int partial_slots(int N, int G) {
 // int32 entries of the group table: offsets [G+1] | all [G] | split [G] | slot [G] | small [G] | tiles [2 * max tiles]
 int64_t group_table_ints(int N, int G) { return G == 1 ? 0 : (int64_t)5 * G + 1 + 2 * ((int64_t)N / 128 + G); }
 
-// T_pyr: frames of the pyramid the correlation reads (sizes the split copy; 0 = T); frames: room for a [G, T] frame map
-Workspace carve(void* base, int T, int N, int H4 = 0, int W4 = 0, int G = 1, int T_pyr = 0, bool frames = false) {
+// T_pyr: frames of the pyramid the correlation reads (sizes the split copy; 0 = T); frames: room for a [G, T] frame map;
+// slab: tracks per slab (0 or >= N: no slabs)
+Workspace carve(void* base, int T, int N, int H4 = 0, int W4 = 0, int G = 1, int T_pyr = 0, bool frames = false,
+                int slab = 0) {
   Workspace w;
   if (T_pyr == 0) T_pyr = T;
-  const size_t R = (size_t)(N + (size_t)kV * G) * T, Rp = (size_t)N * T, Rv = (size_t)kV * G * T, Mc = Rp * kL;
+  w.slab = slab > 0 && slab < N ? slab : N;
+  const size_t R = (size_t)(N + (size_t)kV * G) * T, Rp = (size_t)N * T, Rv = (size_t)kV * G * T;
+  const size_t S = (size_t)w.slab * T, Mc = S * kL;
+  w.slab_rows = (int64_t)S;
+  w.point_rows = (int64_t)Rp;
+  const bool sl = w.slabbed();
   Carver c(base);
   w.vol = (__nv_bfloat16*)c.take(Mc * 2 * kVolPad * 2);
   w.h1 = (__nv_bfloat16*)c.take(Mc * 2 * kCorrHid * 2);
-  w.xs = (__nv_bfloat16*)c.take(Rp * 2 * kXPad * 2);
+  w.xs = (__nv_bfloat16*)c.take(S * 2 * kXPad * 2);
   w.tokens = (float*)c.take(R * kC * 4);
-  w.ln = (__nv_bfloat16*)c.take(R * 2 * kC * 2);
-  w.att = (__nv_bfloat16*)c.take(R * 2 * kC * 2);
-  w.qkv = (float*)c.take(R * 3 * kC * 4);
+  w.ln = (__nv_bfloat16*)c.take((S + Rv) * 2 * kC * 2);
+  w.att = (__nv_bfloat16*)c.take((S + Rv) * 2 * kC * 2);
+  w.qkv = (float*)c.take(sl ? (S * 3 > Rp * 2 ? S * 3 : Rp * 2) * kC * 4 : R * 3 * kC * 4);
   w.vqkv = (float*)c.take(Rv * 3 * kC * 4);
-  w.hmid = (__nv_bfloat16*)c.take(R * 2 * kMlpHid * 2);
+  w.hmid = (__nv_bfloat16*)c.take((sl ? S : R) * 2 * kMlpHid * 2);
   w.row_bias = (float*)c.take((size_t)T * kC * 4);
   w.att_part = (float*)c.take(attention_partial_bytes(T, kV, partial_slots(N, G)));
   w.pyr_split = nullptr;
@@ -334,48 +349,97 @@ int time_attention(Runner& R, const Workspace& W, const Block& b, const __nv_bfl
   return 0;
 }
 
-// x += to_out(attn(...)); x += mlp(LN(x))   for the rows [row0, row0+rows) of the token buffer
-int mlp_half(Runner& R, const Workspace& W, const Block& b, int64_t row0, int rows) {
+// Row `row` of the token buffer in the scratch of the row-independent stages (ln, att, hmid, the time block's qkv):
+// the same row without slabs, relative to the slab's first row with them.
+int64_t scratch_row(const Workspace& W, int64_t row, int64_t slab_row0) { return W.slabbed() ? row - slab_row0 : row; }
+
+// The track ranges [n, n + count) the row-independent stages run on, for tracks [n_begin, n_end) of the N point and
+// kV*G virtual tracks: without slabs the whole range in one piece, so every launch is the unslabbed one; with them,
+// pieces of at most W.slab tracks that never mix point and virtual tracks.  f(n, count) returns 0 or an error code.
+template <class F>
+int for_slabs(const Workspace& W, int N, int n_begin, int n_end, F&& f) {
+  if (!W.slabbed()) return f(n_begin, n_end - n_begin);
+  for (int n = n_begin; n < n_end;) {
+    const int stop = n < N && n_end > N ? N : n_end;
+    const int count = stop - n < W.slab ? stop - n : W.slab;
+    if (int rc = f(n, count)) return rc;
+    n += count;
+  }
+  return 0;
+}
+
+// x += to_out(attn(...)); x += mlp(LN(x))   for the rows [row0, row0+rows) of the token buffer, which lie in the slab
+// whose first row is slab_row0
+int mlp_half(Runner& R, const Workspace& W, const Block& b, int64_t row0, int rows, int64_t slab_row0) {
   float* x = W.tokens + row0 * kC;
-  __nv_bfloat16* ln = W.ln + row0 * 2 * kC;
-  __nv_bfloat16* hm = W.hmid + row0 * 2 * kMlpHid;
+  const int64_t s = scratch_row(W, row0, slab_row0);
+  __nv_bfloat16* ln = W.ln + s * 2 * kC;
+  __nv_bfloat16* hm = W.hmid + s * 2 * kMlpHid;
   RUNC(CAT_LN, launch_layernorm_split(x, rows, nullptr, nullptr, 1e-6f, ln, R.s));
   GEMM(ln, b.fc1, rows, Runner::to_split(hm, 2 * kMlpHid, kMlpHid, /*tanh*/ 2));
   GEMM(hm, b.fc2, rows, Runner::to_f32(x, kC, true));
   return 0;
 }
 
-// EfficientUpdateFormer body on W.tokens (point rows already hold input_transform output) -- cotracker.py:486-524
+// EfficientUpdateFormer body on W.tokens (point rows already hold input_transform output) -- cotracker.py:486-524.
+// With track slabs (DESIGN.md §4.4.5) the row-independent stages run slab by slab (for_slabs); the space attentions
+// always see every track of a group in one launch.
 int transformer_body(Runner& R, const Workspace& W, int T, int N, const GroupPlan& gp) {
   const Layout& L = R.L;
-  const int Rp = N * T, Rv = kV * gp.G * T, Rall = Rp + Rv;
+  const int NV = kV * gp.G, Rp = N * T, Rv = NV * T;
   const uint8_t* pk = R.pk;
   RUNC(CAT_MISC, launch_init_virtual(W.tokens, reinterpret_cast<const float*>(pk + L.virt), T, N, gp.G, R.s));
   float* vtok = W.tokens + (int64_t)Rp * kC;
-  __nv_bfloat16* ln_p = W.ln;
-  __nv_bfloat16* ln_v = W.ln + (int64_t)Rp * 2 * kC;
-  __nv_bfloat16* att_p = W.att;
-  __nv_bfloat16* att_v = W.att + (int64_t)Rp * 2 * kC;
+  __nv_bfloat16* ln_v = W.ln + W.slab_rows * 2 * kC;
+  __nv_bfloat16* att_v = W.att + W.slab_rows * 2 * kC;
+  // point<-virtual's q and output: with slabs both full-size in W.qkv, behind each other
+  float* q_p = W.qkv;
+  __nv_bfloat16* att_p = W.slabbed() ? reinterpret_cast<__nv_bfloat16*>(W.qkv + (int64_t)Rp * kC) : W.att;
+  // LayerNorm (optionally with the context gamma / beta) of point tracks [n, n + count) into the slab scratch, then
+  // the GEMM `lin` of those rows into out (pitch ld) at their own rows
+  auto ln_gemm_points = [&](const Block& b, bool ctx, const Lin& lin, float* out, int ld) {
+    return for_slabs(W, N, 0, N, [&](int n, int count) -> int {
+      const int64_t r0 = (int64_t)n * T;
+      __nv_bfloat16* ln = W.ln + scratch_row(W, r0, r0) * 2 * kC;
+      RUNC(CAT_LN, launch_layernorm_split(W.tokens + r0 * kC, count * T,
+                                          ctx ? reinterpret_cast<const float*>(pk + b.ctx_g) : nullptr,
+                                          ctx ? reinterpret_cast<const float*>(pk + b.ctx_b) : nullptr,
+                                          ctx ? 1e-5f : 1e-6f, ln, R.s));
+      GEMM(ln, lin, count * T, Runner::to_f32(out + r0 * ld, ld, false));
+      return 0;
+    });
+  };
+  // the MLP half of tracks [n_begin, n_end), slab by slab
+  auto mlp_tracks = [&](const Block& b, int n_begin, int n_end) {
+    return for_slabs(W, N, n_begin, n_end, [&](int n, int count) -> int {
+      return mlp_half(R, W, b, (int64_t)n * T, count * T, (int64_t)n * T);
+    });
+  };
 
   for (int i = 0; i < kDepth; ++i) {
     {  // ---- time block over every token row (points + virtual): sequence = track (cotracker.py:494-495)
       const Block& b = L.time[i];
-      RUNC(CAT_LN, launch_layernorm_split(W.tokens, Rall, nullptr, nullptr, 1e-6f, W.ln, R.s));
-      if (int rc = time_attention(R, W, b, W.ln, W.att, Rall, T)) return rc;   // Rall / T = N + kV*G tracks
-      GEMM(W.att, b.out, Rall, Runner::to_f32(W.tokens, kC, true));
-      if (int rc = mlp_half(R, W, b, 0, Rall)) return rc;
+      if (int rc = for_slabs(W, N, 0, N + NV, [&](int n, int count) -> int {
+            const int64_t r0 = (int64_t)n * T;
+            const int rows = count * T;
+            const int64_t s0 = scratch_row(W, r0, r0);
+            float* x = W.tokens + r0 * kC;
+            RUNC(CAT_LN, launch_layernorm_split(x, rows, nullptr, nullptr, 1e-6f, W.ln + s0 * 2 * kC, R.s));
+            if (int rc = time_attention(R, W, b, W.ln + s0 * 2 * kC, W.att + s0 * 2 * kC, rows, T)) return rc;
+            GEMM(W.att + s0 * 2 * kC, b.out, rows, Runner::to_f32(x, kC, true));
+            return mlp_half(R, W, b, r0, rows, r0);
+          }))
+        return rc;
     }
     {  // ---- virtual <- point cross attention (cotracker.py:510-512): x = virtual, context = points
       const Block& b = L.v2p[i];
       RUNC(CAT_LN, launch_layernorm_split(vtok, Rv, nullptr, nullptr, 1e-6f, ln_v, R.s));
-      RUNC(CAT_LN, launch_layernorm_split(W.tokens, Rp, reinterpret_cast<const float*>(pk + b.ctx_g),
-                                 reinterpret_cast<const float*>(pk + b.ctx_b), 1e-5f, ln_p, R.s));
       GEMM(ln_v, b.q, Rv, Runner::to_f32(W.vqkv, kC, false));
-      GEMM(ln_p, b.kv, Rp, Runner::to_f32(W.qkv, 2 * kC, false));
+      if (int rc = ln_gemm_points(b, true, b.kv, W.qkv, 2 * kC)) return rc;
       RUNC(CAT_ATTN, space_attention(R, W, gp, attn_params(W.vqkv, kC, W.qkv, 2 * kC, 0, kC, att_v, kV, N, T), false,
                                      true));
       GEMM(att_v, b.out, Rv, Runner::to_f32(vtok, kC, true));
-      if (int rc = mlp_half(R, W, b, Rp, Rv)) return rc;
+      if (int rc = mlp_tracks(b, N, N + NV)) return rc;
     }
     {  // ---- virtual self attention (cotracker.py:514): sequence = frame over the 64 virtual tokens
       const Block& b = L.vself[i];
@@ -384,19 +448,22 @@ int transformer_body(Runner& R, const Workspace& W, int T, int N, const GroupPla
       RUNC(CAT_ATTN, space_attention(R, W, gp, attn_params(W.vqkv, 3 * kC, W.vqkv, 3 * kC, kC, 2 * kC, att_v, kV, kV,
                                                            T), false, false));
       GEMM(att_v, b.out, Rv, Runner::to_f32(vtok, kC, true));
-      if (int rc = mlp_half(R, W, b, Rp, Rv)) return rc;
+      if (int rc = mlp_tracks(b, N, N + NV)) return rc;
     }
     {  // ---- point <- virtual cross attention (cotracker.py:515-517): x = points, context = virtual
       const Block& b = L.p2v[i];
-      RUNC(CAT_LN, launch_layernorm_split(W.tokens, Rp, nullptr, nullptr, 1e-6f, ln_p, R.s));
+      if (int rc = ln_gemm_points(b, false, b.q, q_p, kC)) return rc;
       RUNC(CAT_LN, launch_layernorm_split(vtok, Rv, reinterpret_cast<const float*>(pk + b.ctx_g),
                                  reinterpret_cast<const float*>(pk + b.ctx_b), 1e-5f, ln_v, R.s));
-      GEMM(ln_p, b.q, Rp, Runner::to_f32(W.qkv, kC, false));
       GEMM(ln_v, b.kv, Rv, Runner::to_f32(W.vqkv, 2 * kC, false));
-      RUNC(CAT_ATTN, space_attention(R, W, gp, attn_params(W.qkv, kC, W.vqkv, 2 * kC, 0, kC, att_p, N, kV, T), true,
+      RUNC(CAT_ATTN, space_attention(R, W, gp, attn_params(q_p, kC, W.vqkv, 2 * kC, 0, kC, att_p, N, kV, T), true,
                                      false));
-      GEMM(att_p, b.out, Rp, Runner::to_f32(W.tokens, kC, true));
-      if (int rc = mlp_half(R, W, b, 0, Rp)) return rc;
+      if (int rc = for_slabs(W, N, 0, N, [&](int n, int count) -> int {
+            const int64_t r0 = (int64_t)n * T;
+            GEMM(att_p + r0 * 2 * kC, b.out, count * T, Runner::to_f32(W.tokens + r0 * kC, kC, true));
+            return mlp_half(R, W, b, r0, count * T, r0);
+          }))
+        return rc;
     }
   }
   return 0;
@@ -418,26 +485,25 @@ Prec effective_prec(bool have_pyr_split, int T, int H4, int W4) {
   return p;
 }
 
-// input_transform of the X rows in W.xs into the point tokens, with the per-frame bias row_bias [T, kC] when given
-int input_transform(Runner& R, const Workspace& W, int T, int N, const float* row_bias) {
-  GemmEpilogue e = Runner::to_f32(W.tokens, kC, false);
+// input_transform of the X rows in W.xs into the point tokens of tracks [n0, n0 + count), with the per-frame bias
+// row_bias [T, kC] when given (a track's rows start at a multiple of T, so row % T is the frame)
+int input_transform(Runner& R, const Workspace& W, int T, int n0, int count, const float* row_bias) {
+  GemmEpilogue e = Runner::to_f32(W.tokens + (int64_t)n0 * T * kC, kC, false);
   if (row_bias) { e.row_bias = row_bias; e.row_mod = T; }
-  GEMM(W.xs, R.L.in_tr, N * T, e);
+  GEMM(W.xs, R.L.in_tr, count * T, e);
   return 0;
 }
 
-// The first half of one update-loop iteration, from the state to the point tokens: the correlation volume (W.vol),
-// corr_mlp into the correlation columns of X and build_x_small into the rest (W.xs), then input_transform with the
-// time-embedding fold W.row_bias into the point rows of W.tokens.  Reads coords / vis / conf, writes none of them.
-// pyr_split: the split pyramid when the patch kernel runs (pr.patch), else null.
-int point_tokens(Runner& R, const Workspace& W, const Prec& pr, const float* pyr, const __nv_bfloat16* pyr_split,
-                 int H4, int W4, const float* support, const uint8_t* track_valid, const float* coords,
-                 const float* vis, const float* conf, int T, int N, int T_pyr, const FrameMap& fm) {
+// point_tokens for the tracks [n0, n0 + count) of the N-track state, from row 0 of the stage's scratch
+int point_tokens_slab(Runner& R, const Workspace& W, const Prec& pr, const float* pyr, const __nv_bfloat16* pyr_split,
+                      int H4, int W4, const float* support, const uint8_t* track_valid, const float* coords,
+                      const float* vis, const float* conf, int T, int N, int T_pyr, const FrameMap& fm, int n0,
+                      int count) {
   const Layout& L = R.L;
-  const int Mc = N * T * kL;
+  const int Mc = count * T * kL;
   // (i)+(ii) sampling + 4-D correlation, all levels -> split volume
-  RUNC(CAT_CORR, launch_corr_sample(pyr, pyr_split, H4, W4, support, track_valid, coords, T, N, W.vol, g_opt_corr,
-                                    pr.corr, pr.vol16() ? 1 : 0, num_sms(), R.s, T_pyr, fm));
+  RUNC(CAT_CORR, launch_corr_sample(pyr, pyr_split, H4, W4, support, track_valid, coords, T, N, n0, count, W.vol,
+                                    g_opt_corr, pr.corr, pr.vol16() ? 1 : 0, num_sms(), R.s, T_pyr, fm));
   // (iii) corr_mlp: 2401 -> 384 (GELU erf) -> 256, written straight into X columns [256*l, 256*l+256)
   if (pr.vol16()) {   // single fp16 volume plane x split fp16 weights: 2 (or 1) tensor-core products per FLOP
     GEMM(W.vol, pr.support_major() ? L.corr_fc1_th : L.corr_fc1_h, Mc,
@@ -452,10 +518,25 @@ int point_tokens(Runner& R, const Workspace& W, const Prec& pr, const float* pyr
     GEMM(W.h1, L.corr_fc2, Mc, e);
   }
   // vis, conf, posenc(rel. motion), zero pad -> X columns [1024,1152)
-  RUNC(CAT_MISC, launch_build_x_small(coords, vis, conf, T, N, W.xs, R.s));
+  RUNC(CAT_MISC, launch_build_x_small(coords, vis, conf, T, N, n0, count, W.xs, R.s));
   // (iv) input_transform (+ folded time embedding) -> point tokens
-  return input_transform(R, W, T, N, W.row_bias);
+  return input_transform(R, W, T, n0, count, W.row_bias);
 }
+
+// The first half of one update-loop iteration, from the state to the point tokens: the correlation volume (W.vol),
+// corr_mlp into the correlation columns of X and build_x_small into the rest (W.xs), then input_transform with the
+// time-embedding fold W.row_bias into the point rows of W.tokens.  Reads coords / vis / conf, writes none of them.
+// pyr_split: the split pyramid when the patch kernel runs (pr.patch), else null.  With track slabs each slab of
+// tracks [n0, n0 + count) runs the whole stage through the slab scratch into its own rows of W.tokens.
+int point_tokens(Runner& R, const Workspace& W, const Prec& pr, const float* pyr, const __nv_bfloat16* pyr_split,
+                 int H4, int W4, const float* support, const uint8_t* track_valid, const float* coords,
+                 const float* vis, const float* conf, int T, int N, int T_pyr, const FrameMap& fm) {
+  return for_slabs(W, N, 0, N, [&](int n0, int count) -> int {
+    return point_tokens_slab(R, W, pr, pyr, pyr_split, H4, W4, support, track_valid, coords, vis, conf, T, N, T_pyr,
+                             fm, n0, count);
+  });
+}
+
 
 // The steps update_loop and updateformer share once the point tokens are in W.tokens: the transformer body, then the
 // heads: the state update of coords / vis / conf, or with delta != nullptr the raw deltas [N,T,4] instead.
@@ -472,6 +553,19 @@ int check_TN(int T, int N, int G = 1) {
   if (T < 1 || N < 1) return fail(CT3_EINVAL, "T and N must be >= 1%s");
   if (G < 1 || G > N) return fail(CT3_EINVAL, "G must be in [1, N]%s");
   if (((int64_t)N + (int64_t)kV * G) * T * 3 * kC >= (int64_t)1 << 40) return fail(CT3_EINVAL, "problem too large%s");
+  return 0;
+}
+
+// The supported size of ct3_update_loop_slabbed: at most 2^21 token rows (N + 64 G)*T.  Track slabs make problems
+// reachable whose full-size buffers (tokens, the point rows' space-attention operands, up to 768 elements per row)
+// no longer fit a full workspace; at this bound every element offset into them stays below 2^31, so no index
+// arithmetic on the slabbed path can overflow 32 bits.  The slab-sized stages run the kernels of a full-workspace
+// call on slab_tracks*T rows.
+constexpr int64_t kSlabbedMaxRows = (int64_t)1 << 21;
+int check_slabbed(int T, int N, int G, int slab_tracks) {
+  if (slab_tracks < 1) return fail(CT3_EINVAL, "slab_tracks must be >= 1%s");
+  if (((int64_t)N + (int64_t)kV * G) * T > kSlabbedMaxRows)
+    return fail(CT3_EINVAL, "problem too large for the slabbed loop: (N + 64 G) * T must be <= 2^21%s");
   return 0;
 }
 
@@ -504,33 +598,39 @@ int check_frames(const int32_t* frames, int G, int T, int T_pyr) {
   return 0;
 }
 
-// ct3_workspace_bytes_groups (frames == false, T_pyr == T: the pyramid shape is checked only when given) and
-// ct3_workspace_bytes_frames
-int loop_workspace_bytes(int T, int T_pyr, int N, int G, int H4, int W4, bool frames, size_t* out_bytes) {
+// ct3_workspace_bytes_groups (frames == false, T_pyr == T: the pyramid shape is checked only when given),
+// ct3_workspace_bytes_frames and, with slab > 0, ct3_workspace_bytes_slabbed
+int loop_workspace_bytes(int T, int T_pyr, int N, int G, int H4, int W4, bool frames, size_t* out_bytes,
+                         int slab = 0) {
   if (!out_bytes) return fail(CT3_EINVAL, "null out_bytes%s");
   if (int rc = check_TN(T, N, G)) return rc;
+  if (slab != 0)
+    if (int rc = check_slabbed(T, N, G, slab)) return rc;
   if (frames)
     if (int rc = check_frames(nullptr, G, T, T_pyr)) return rc;
   if (frames || H4 != 0 || W4 != 0)
     if (int rc = check_pyramid(T_pyr, H4, W4)) return rc;
-  *out_bytes = carve(nullptr, T, N, H4, W4, G, T_pyr, frames).total;
+  *out_bytes = carve(nullptr, T, N, H4, W4, G, T_pyr, frames, slab).total;
   return 0;
 }
 
-// frames: host frame map [G, T] into the T_pyr pyramid frames, or null (frame t, T_pyr == T)
+// frames: host frame map [G, T] into the T_pyr pyramid frames, or null (frame t, T_pyr == T).  slab: tracks per slab
+// of ct3_update_loop_slabbed (its workspace always has room for a frame map), 0 for the other entry points.
 int update_loop(const void* packed, const float* pyr, int H4, int W4, const float* support, const uint8_t* track_valid,
                 float* coords, float* vis, float* conf, const float* time_emb, int T, int N, const int32_t* sizes,
                 int G, int iters, void* workspace, size_t workspace_bytes, cudaStream_t stream, int T_pyr,
-                const int32_t* frames) {
+                const int32_t* frames, int slab = 0) {
   if (!packed || !pyr || !support || !coords || !vis || !conf || !time_emb || !workspace)
     return fail(CT3_EINVAL, "null argument%s");
   int total = 0;
   if (int rc = check_groups(T, N, sizes, G, &total, false)) return rc;
+  if (slab != 0)
+    if (int rc = check_slabbed(T, N, G, slab)) return rc;
   if (iters < 0) return fail(CT3_EINVAL, "iters must be >= 0%s");
   if (int rc = check_frames(frames, G, T, T_pyr)) return rc;
   if (int rc = check_pyramid(T_pyr, H4, W4)) return rc;
   if (int rc = check_aligned(workspace, "workspace")) return rc;
-  const Workspace W = carve(workspace, T, N, H4, W4, G, T_pyr, frames != nullptr);
+  const Workspace W = carve(workspace, T, N, H4, W4, G, T_pyr, frames != nullptr || slab != 0, slab);
   if (int rc = check_space(workspace_bytes, W.total, "workspace")) return rc;
   const Layout& L = layout();
   Runner R{reinterpret_cast<const uint8_t*>(packed), L, stream, g_opt_gemm};
@@ -608,7 +708,7 @@ int updateformer(const void* packed, const float* x, int T, int N, const int32_t
   GroupPlan gp;
   if (int rc = plan_groups(gp, sizes, G, T, N, W.groups, R.s)) return rc;
   RUNC(CAT_MISC, launch_split_rows(x, N * T, kX, kXPad, /*perm_x*/ 1, W.xs, 0, R.s));
-  if (int rc = input_transform(R, W, T, N, nullptr)) return rc;
+  if (int rc = input_transform(R, W, T, 0, N, nullptr)) return rc;
   return transform_and_heads(R, W, T, N, gp, nullptr, nullptr, nullptr, delta);
 }
 
@@ -802,6 +902,11 @@ int ct3_workspace_bytes_frames(int T, int T_pyr, int N, int G, int H4, int W4, s
   return loop_workspace_bytes(T, T_pyr, N, G, H4, W4, true, out_bytes);
 }
 
+int ct3_workspace_bytes_slabbed(int T, int T_pyr, int N, int G, int H4, int W4, int slab_tracks, size_t* out_bytes) {
+  if (slab_tracks < 1) return fail(CT3_EINVAL, "slab_tracks must be >= 1%s");
+  return loop_workspace_bytes(T, T_pyr, N, G, H4, W4, true, out_bytes, slab_tracks);
+}
+
 int ct3_corr_sample(const float* pyr, int H4, int W4, const float* support, const uint8_t* track_valid,
                     const float* coords, int T, int N, void* vol_split, void* scratch, size_t scratch_bytes,
                     ct3_stream_t stream) {
@@ -816,7 +921,7 @@ int ct3_corr_sample(const float* pyr, int H4, int W4, const float* support, cons
     CK(launch_split_pyramid(pyr, T, H4, W4, (__nv_bfloat16*)scratch, pr.corr, (cudaStream_t)stream), "split_pyramid");
     pyr_split = (const __nv_bfloat16*)scratch;
   }
-  CK(launch_corr_sample(pyr, pyr_split, H4, W4, support, track_valid, coords, T, N, (__nv_bfloat16*)vol_split,
+  CK(launch_corr_sample(pyr, pyr_split, H4, W4, support, track_valid, coords, T, N, 0, N, (__nv_bfloat16*)vol_split,
                         g_opt_corr, pr.corr, pr.vol16() ? 1 : 0, num_sms(), (cudaStream_t)stream, T, FrameMap{}),
      "corr_sample");
   return 0;
@@ -903,6 +1008,16 @@ int ct3_update_loop_frames(const void* packed, const float* pyr, int T_pyr, int 
   if (!group_frames_host) return fail(CT3_EINVAL, "null group_frames_host%s");
   return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, group_sizes_host, G,
                      iters, workspace, workspace_bytes, (cudaStream_t)stream, T_pyr, group_frames_host);
+}
+
+int ct3_update_loop_slabbed(const void* packed, const float* pyr, int T_pyr, int H4, int W4, const float* support,
+                            const uint8_t* track_valid, float* coords, float* vis, float* conf, const float* time_emb,
+                            int T, int N, int iters, void* workspace, size_t workspace_bytes, ct3_stream_t stream,
+                            const int32_t* group_sizes_host, int G, const int32_t* group_frames_host, int slab_tracks) {
+  if (slab_tracks < 1) return fail(CT3_EINVAL, "slab_tracks must be >= 1%s");
+  if (!group_frames_host && T_pyr != T) return fail(CT3_EINVAL, "without a frame map T_pyr must equal T%s");
+  return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, group_sizes_host, G,
+                     iters, workspace, workspace_bytes, (cudaStream_t)stream, T_pyr, group_frames_host, slab_tracks);
 }
 
 int ct3_loop_tokens(const void* packed, const float* pyr, int H4, int W4, const float* support,

@@ -128,19 +128,27 @@ bool corr_uses_patch_kernel(int impl, bool have_pyr_split, int T, int H4, int W4
 }
 
 cudaError_t launch_corr_sample(const float* pyr, const __nv_bfloat16* pyr_split, int H4, int W4, const float* support,
-                               const uint8_t* track_valid, const float* coords, int T, int N,
+                               const uint8_t* track_valid, const float* coords, int T, int N, int n0, int count,
                                __nv_bfloat16* vol_split, int impl, int mode, int vol16, int num_sms, cudaStream_t s,
-                               int T_pyr, const FrameMap& fm) {
+                               int T_pyr, const FrameMap& fm_all) {
+  // track n of the launch is track n0 + n of the state: support [4][49, N, 128], track_valid [N] and coords [T, N, 2]
+  // keep pitch N, so moving their base to track n0 is the whole change for the kernels
+  support += (int64_t)n0 * kD;
+  if (track_valid) track_valid += n0;
+  coords += (int64_t)n0 * 2;
+  FrameMap fm = fm_all;
+  fm.n0 = n0;
   if (corr_uses_patch_kernel(impl, pyr_split != nullptr, T_pyr, H4, W4)) {
     if (mode != 3)
-      return launch_corr_patch_t(pyr_split, H4, W4, support, track_valid, coords, T, N, vol_split, vol16, mode == 1,
-                                 num_sms, s, T_pyr, fm);
-    return launch_corr_patch_tc(pyr_split, H4, W4, support, track_valid, coords, T, N, vol_split, vol16, num_sms, s,
-                                T_pyr, fm);
+      return launch_corr_patch_t(pyr_split, H4, W4, support, track_valid, coords, T, N, count, vol_split, vol16,
+                                 mode == 1, num_sms, s, T_pyr, fm);
+    return launch_corr_patch_tc(pyr_split, H4, W4, support, track_valid, coords, T, N, count, vol_split, vol16, num_sms,
+                                s, T_pyr, fm);
   }
   if (vol16) return cudaErrorInvalidValue;   // only the patch kernel writes the single-plane volume
   if (impl != 1)
-    return launch_corr_sample_tc(pyr, H4, W4, support, track_valid, coords, T, N, vol_split, num_sms, s, T_pyr, fm);
+    return launch_corr_sample_tc(pyr, H4, W4, support, track_valid, coords, T, N, count, vol_split, num_sms, s, T_pyr,
+                                 fm);
   CorrArgs g;  // impl 1: exact-fp32 SIMT verification kernel
   g.pyr = pyr;
   g.lay = pyramid_layout(T_pyr, H4, W4);
@@ -159,7 +167,7 @@ cudaError_t launch_corr_sample(const float* pyr, const __nv_bfloat16* pyr_split,
     });
     if (e != cudaSuccess) return e;
   }
-  dim3 grid(N, kL);
+  dim3 grid(count, kL);
   corr_sample_simt_kernel<<<grid, 256, smem, s>>>(g);
   return cudaGetLastError();
 }

@@ -383,7 +383,7 @@ corr_sample_tc_kernel(const __grid_constant__ CorrTcArgs g, const __grid_constan
 }  // namespace
 
 cudaError_t launch_corr_sample_tc(const float* pyr, int H4, int W4, const float* support,
-                                  const uint8_t* track_valid, const float* coords, int T, int N,
+                                  const uint8_t* track_valid, const float* coords, int T, int N, int count,
                                   __nv_bfloat16* vol_split, int num_sms, cudaStream_t s, int T_pyr,
                                   const FrameMap& fm) {
   CorrTcArgs g;
@@ -413,7 +413,7 @@ cudaError_t launch_corr_sample_tc(const float* pyr, int H4, int W4, const float*
     });
     if (e != cudaSuccess) return e;
   }
-  const int num_units = N * kL;
+  const int num_units = count * kL;
   const int grid = num_units < num_sms ? num_units : num_sms;
   corr_sample_tc_kernel<<<grid, THREADS, SMEM_BYTES, s>>>(g, maps, num_units);
   return cudaGetLastError();

@@ -522,7 +522,7 @@ cudaError_t launch_split_pyramid(const float* pyr, int T, int H4, int W4, __nv_b
 }
 
 cudaError_t launch_corr_patch_tc(const __nv_bfloat16* pyr_split, int H4, int W4, const float* support,
-                                 const uint8_t* track_valid, const float* coords, int T, int N,
+                                 const uint8_t* track_valid, const float* coords, int T, int N, int count,
                                  __nv_bfloat16* vol_split, int vol16, int num_sms, cudaStream_t s, int T_pyr,
                                  const FrameMap& fm) {
   Corr2Args g;
@@ -552,7 +552,7 @@ cudaError_t launch_corr_patch_tc(const __nv_bfloat16* pyr_split, int H4, int W4,
                            box, CU_TENSOR_MAP_SWIZZLE_128B))
       return cudaErrorInvalidValue;
   }
-  const int num_units = N * kL;
+  const int num_units = count * kL;
   const cudaError_t le = vol16 ? launch_variant<true>(g, maps, num_units, num_sms, s)
                                : launch_variant<false>(g, maps, num_units, num_sms, s);
   if (le != cudaSuccess) return le;

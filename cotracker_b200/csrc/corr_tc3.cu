@@ -499,7 +499,7 @@ cudaError_t launch_variant(const Corr3Args& g, const Corr3Maps& maps, int num_un
 }  // namespace
 
 cudaError_t launch_corr_patch_t(const __nv_bfloat16* pyr_half, int H4, int W4, const float* support,
-                                const uint8_t* track_valid, const float* coords, int T, int N,
+                                const uint8_t* track_valid, const float* coords, int T, int N, int count,
                                 __nv_bfloat16* vol, int vol16, int one_product, int num_sms, cudaStream_t s, int T_pyr,
                                 const FrameMap& fm) {
   Corr3Args g;
@@ -528,7 +528,7 @@ cudaError_t launch_corr_patch_t(const __nv_bfloat16* pyr_half, int H4, int W4, c
                            box, CU_TENSOR_MAP_SWIZZLE_128B))
       return cudaErrorInvalidValue;
   }
-  const int num_units = N * kL;
+  const int num_units = count * kL;
   if (one_product)
     return vol16 ? launch_variant<true, true>(g, maps, num_units, num_sms, s)
                  : launch_variant<false, true>(g, maps, num_units, num_sms, s);

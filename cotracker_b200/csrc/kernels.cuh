@@ -95,17 +95,20 @@ cudaError_t launch_upsample_concat_split(const float* const src[4], const int c[
 // Frame map of ct3_update_loop_frames: at time step t, track n of group g reads pyramid frame frames[g*T + t] (an index
 // into the T_pyr frames of the pyramid).  frames == nullptr: frame t.  goff: [G+1] first track of every group (nullptr
 // when G == 1).  Every correlation kernel works on units of ONE track, so the lookup is per (track, t): no tile or TMA
-// box ever spans two tracks' frames.
+// box ever spans two tracks' frames.  n0: the global index of the launch's first track (a track slab of
+// ct3_update_loop_slabbed); the group lookup is by global track.
 struct FrameMap {
   const int32_t* frames = nullptr;
   const int32_t* goff = nullptr;
   int G = 1;
+  int n0 = 0;
 };
-// the T-entry frame row of track n (nullptr: identity)
+// the T-entry frame row of track n of the launch (nullptr: identity)
 __device__ __forceinline__ const int32_t* frame_row(const FrameMap& m, int n, int T) {
   if (!m.frames) return nullptr;
   int g = 0;
-  if (m.goff) {   // largest g with goff[g] <= n
+  if (m.goff) {   // largest g with goff[g] <= n0 + n
+    n += m.n0;
     int hi = m.G - 1;
     while (g < hi) {
       const int mid = (g + hi + 1) >> 1;
@@ -124,14 +127,18 @@ __device__ __forceinline__ int map_frame(const int32_t* row, int t) { return row
 // mode / vol16 apply to the correlate-then-interpolate path only (corr_uses_patch_kernel): products per correlation
 // FLOP (3|2|1; pyr_split must have been made with the same mode) and a single-fp16-plane volume [N*T*4, kVolPad]
 // instead of the split one; the other kernels always compute in fp32 / bf16x3 and write the split volume.
+// Track range: the launch covers tracks [n0, n0 + count) of the N-track state and support (N stays their pitch) and
+// writes their volume rows from row 0 of vol_split (a track slab of ct3_update_loop_slabbed; n0 = 0, count = N: all).
+// The dispatcher moves support / track_valid / coords to track n0 and sets fm.n0; the kernels below it see `count`
+// tracks at pitch N.
 bool corr_uses_patch_kernel(int impl, bool have_pyr_split, int T, int H4, int W4);
 cudaError_t launch_corr_sample(const float* pyr, const __nv_bfloat16* pyr_split, int H4, int W4, const float* support,
-                               const uint8_t* track_valid, const float* coords, int T, int N,
+                               const uint8_t* track_valid, const float* coords, int T, int N, int n0, int count,
                                __nv_bfloat16* vol_split, int impl, int mode, int vol16, int num_sms, cudaStream_t s,
                                int T_pyr, const FrameMap& fm);
 
 cudaError_t launch_corr_sample_tc(const float* pyr, int H4, int W4, const float* support,
-                                  const uint8_t* track_valid, const float* coords, int T, int N,
+                                  const uint8_t* track_valid, const float* coords, int T, int N, int count,
                                   __nv_bfloat16* vol_split, int num_sms, cudaStream_t s, int T_pyr, const FrameMap& fm);
 
 // corr_tc2.cu: correlate-then-interpolate on a split-bf16 copy of the pyramid (mode 3)
@@ -141,22 +148,23 @@ bool corr_patch_supported(int T, int H4, int W4);
 cudaError_t launch_split_pyramid(const float* pyr, int T, int H4, int W4, __nv_bfloat16* pyr_split, int mode,
                                  cudaStream_t s);
 cudaError_t launch_corr_patch_tc(const __nv_bfloat16* pyr_split, int H4, int W4, const float* support,
-                                 const uint8_t* track_valid, const float* coords, int T, int N,
+                                 const uint8_t* track_valid, const float* coords, int T, int N, int count,
                                  __nv_bfloat16* vol_split, int vol16, int num_sms, cudaStream_t s, int T_pyr,
                                  const FrameMap& fm);
 
 // corr_tc3.cu: the production kernel -- same algorithm with the MMA transposed (supports = M side), one fp16 texel
 // plane (pyr_split made with mode 1 or 2), supports split fp16 (mode 2) or one fp16 plane (one_product, mode 1)
 cudaError_t launch_corr_patch_t(const __nv_bfloat16* pyr_half, int H4, int W4, const float* support,
-                                const uint8_t* track_valid, const float* coords, int T, int N,
+                                const uint8_t* track_valid, const float* coords, int T, int N, int count,
                                 __nv_bfloat16* vol, int vol16, int one_product, int num_sms, cudaStream_t s, int T_pyr,
                                 const FrameMap& fm);
 
 // ---- tokens.cu : elementwise / row-wise pieces of the transformer ---------------------------------
 cudaError_t launch_layernorm_split(const float* x, int rows, const float* gamma, const float* beta, float eps,
                                    __nv_bfloat16* out_split, cudaStream_t s);
-cudaError_t launch_build_x_small(const float* coords, const float* vis, const float* conf, int T, int N,
-                                 __nv_bfloat16* x_split, cudaStream_t s);
+// the X rows of tracks [n0, n0 + count) of the [T, N] state into x_split from row 0
+cudaError_t launch_build_x_small(const float* coords, const float* vis, const float* conf, int T, int N, int n0,
+                                 int count, __nv_bfloat16* x_split, cudaStream_t s);
 // one copy of the kV virtual tokens per group: rows (N + kV*g + i)*T + t, g < G
 cudaError_t launch_init_virtual(float* tokens, const float* virt, int T, int N, int G, cudaStream_t s);
 // host int32 array -> device, stream-ordered (kernel arguments carry the values: src may be freed on return)

@@ -198,9 +198,10 @@ cudaError_t launch_layernorm_split(const float* x, int rows, const float* gamma,
   layernorm_split_kernel<<<(rows + 7) / 8, 256, 0, s>>>(x, rows, gamma, beta, eps, out_split);
   return cudaGetLastError();
 }
-cudaError_t launch_build_x_small(const float* coords, const float* vis, const float* conf, int T, int N,
-                                 __nv_bfloat16* x_split, cudaStream_t s) {
-  build_x_small_kernel<<<N * T, 128, 0, s>>>(coords, vis, conf, T, N, x_split);
+cudaError_t launch_build_x_small(const float* coords, const float* vis, const float* conf, int T, int N, int n0,
+                                 int count, __nv_bfloat16* x_split, cudaStream_t s) {
+  // the kernel's track n is track n0 + n of the [T, N] state: same pitch, base moved to track n0
+  build_x_small_kernel<<<count * T, 128, 0, s>>>(coords + (int64_t)n0 * 2, vis + n0, conf + n0, T, N, x_split);
   return cudaGetLastError();
 }
 cudaError_t launch_init_virtual(float* tokens, const float* virt, int T, int N, int G, cudaStream_t s) {

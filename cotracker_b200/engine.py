@@ -100,6 +100,12 @@ def _signatures():
         "ct3_update_loop_frames": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p,
                                            ctypes.POINTER(ctypes.c_int32), c_int, ctypes.POINTER(ctypes.c_int32)]),
+        "ct3_workspace_bytes_slabbed": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                                ctypes.POINTER(c_size_t)]),
+        "ct3_update_loop_slabbed": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t,
+                                            c_void_p, ctypes.POINTER(ctypes.c_int32), c_int,
+                                            ctypes.POINTER(ctypes.c_int32), c_int]),
         "ct3_upsample_concat": (c_int, [ctypes.POINTER(c_void_p), intp, intp, intp, c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_enc_tail_packed_bytes": (c_int, [ctypes.POINTER(c_size_t)]),
         "ct3_enc_tail_pack": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
@@ -477,10 +483,15 @@ def sample_support(pyr, T, H4, W4, qframes, qcoords, support=None, accumulate_ma
     return support
 
 
-def workspace_bytes(T: int, N: int, H4: int = 0, W4: int = 0, groups: int = 1, frames: Optional[int] = None) -> int:
+def workspace_bytes(T: int, N: int, H4: int = 0, W4: int = 0, groups: int = 1, frames: Optional[int] = None,
+                    slab_tracks: Optional[int] = None) -> int:
     """Scratch of ct3_update_loop for T frames of H4 x W4 feature maps and N tracks (H4 = W4 = 0: updateformer only),
     split into `groups` track groups (ct3_update_loop_groups).  frames: the T_pyr pyramid frames of a call with a
-    frame map (ct3_update_loop_frames)."""
+    frame map (ct3_update_loop_frames).  slab_tracks: the loop in track slabs of that many tracks
+    (ct3_update_loop_slabbed; frames None = T)."""
+    if slab_tracks is not None:
+        return _size("ct3_workspace_bytes_slabbed", int(T), int(T if frames is None else frames), int(N), int(groups),
+                     int(H4), int(W4), int(slab_tracks))
     if frames is not None:
         return _size("ct3_workspace_bytes_frames", int(T), int(frames), int(N), int(groups), int(H4), int(W4))
     return _size("ct3_workspace_bytes_groups", int(T), int(N), int(groups), int(H4), int(W4))
@@ -512,8 +523,8 @@ class WorkspaceCache:
         self.buf: Optional[torch.Tensor] = None
 
     def get(self, T: int, N: int, device, H4: int = 0, W4: int = 0, groups: int = 1,
-            frames: Optional[int] = None) -> torch.Tensor:
-        need = workspace_bytes(T, N, H4, W4, groups, frames)
+            frames: Optional[int] = None, slab_tracks: Optional[int] = None) -> torch.Tensor:
+        need = workspace_bytes(T, N, H4, W4, groups, frames, slab_tracks)
         if self.buf is None or self.buf.numel() < need or self.buf.device != torch.device(device):
             self.buf = None
             self.buf = torch.empty(need, dtype=torch.uint8, device=device)
@@ -534,13 +545,15 @@ def _frame_array(group_frames, G: int, T: int):
 
 
 def update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, iters, workspace,
-                group_sizes: Optional[Sequence[int]] = None, group_frames=None):
+                group_sizes: Optional[Sequence[int]] = None, group_frames=None, slab_tracks: Optional[int] = None):
     """In-place refinement of coords [T,N,2], vis [T,N], conf [T,N] (fp32, feature-grid units / logits).
     group_sizes: the N tracks as contiguous independent groups (ct3_update_loop_groups); each group's result is
     bit-identical to a call on its tracks alone.  None = one group.
     group_frames: [G, T] frame map (ct3_update_loop_frames): group g reads frame group_frames[g][t] of `pyr` (which may
     hold any number of frames) at time step t; each group's result is bit-identical to a call on a pyramid of exactly
-    those frames.  None = frame t."""
+    those frames.  None = frame t.
+    slab_tracks: run in track slabs of that many tracks (ct3_update_loop_slabbed) in a workspace of
+    workspace_bytes(..., slab_tracks=); bit-identical to the call without.  None = no slabs."""
     _req(coords, torch.float32, "coords"); _req(vis, torch.float32, "vis"); _req(conf, torch.float32, "conf")
     _req(pyr, torch.float32, "pyr"); _req(support, torch.float32, "support"); _req(time_emb, torch.float32, "time_emb")
     T, N, _ = coords.shape
@@ -551,7 +564,12 @@ def update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, ti
     arr, G = _group_array(group_sizes if group_sizes is not None else [N])
     state = (_ptr(support), _ptr(track_valid), _ptr(coords), _ptr(vis), _ptr(conf), _ptr(time_emb), T, N, int(iters),
              _ptr(workspace), workspace.numel(), _stream(coords.device), arr, G)
-    if group_frames is None:
+    if slab_tracks is not None:
+        fr = None if group_frames is None else _frame_array(group_frames, G, T)
+        T_pyr = T if group_frames is None else pyramid_frames(pyr, H4, W4)
+        _call("ct3_update_loop_slabbed", coords.device, _ptr(packed), _ptr(pyr), T_pyr, H4, W4, *state, fr,
+              int(slab_tracks))
+    elif group_frames is None:
         _call("ct3_update_loop_groups", coords.device, _ptr(packed), _ptr(pyr), H4, W4, *state)
     else:
         _call("ct3_update_loop_frames", coords.device, _ptr(packed), _ptr(pyr), pyramid_frames(pyr, H4, W4), H4, W4,

@@ -101,6 +101,24 @@ def pass_budget_bytes(model, device, T: int, ih: int, iw: int) -> int:
     return int(0.9 * max(0, free - reserve))
 
 
+def slab_tracks_for(T: int, N: int, G: int, H4: int, W4: int, frames: Optional[int], budget_bytes: int) -> Optional[int]:
+    """Track slabs of one update-loop pass (ct3_update_loop_slabbed, DESIGN.md §4.4.5): None when the full workspace
+    fits `budget_bytes`, so every pass that fits runs exactly as without slabs; else the largest slab_tracks whose
+    workspace fits (the workspace never shrinks as slab_tracks grows), or 1 when none does.
+    frames: the pyramid frames of a pass with a frame map (engine.workspace_bytes)."""
+    from . import engine
+    if engine.workspace_bytes(T, N, H4, W4, groups=G, frames=frames) <= budget_bytes:
+        return None
+    lo, hi = 1, max(1, N - 1)
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        if engine.workspace_bytes(T, N, H4, W4, groups=G, frames=frames, slab_tracks=mid) <= budget_bytes:
+            lo = mid
+        else:
+            hi = mid - 1
+    return lo
+
+
 def plan_dense_passes(n_offsets: int, n_tracks: int, backward: bool, T: int, H4: int, W4: int, budget_bytes: int,
                       frames: Optional[int] = None) -> Tuple[List[int], List[Tuple[int, int]]]:
     """Groups and passes of the predictor's dense mode: one group of n_tracks per grid offset, followed by that

@@ -24,7 +24,7 @@ import torch.nn.functional as F
 
 from . import engine
 from .encoder import BasicEncoder
-from .evaluation import pass_budget_bytes, plan_clip_passes
+from .evaluation import pass_budget_bytes, plan_clip_passes, slab_tracks_for
 
 HID, HEADS, VIRT, XDIM = 384, 8, 64, 1110
 
@@ -300,15 +300,21 @@ class CoTrackerThreeBase(nn.Module):
             raise engine.EngineError("cotracker_b200 runs on CUDA only; move the module and inputs to a GPU")
 
     def _refine(self, pyr, H4, W4, support, track_valid, coords, vis, conf, iters, group_sizes, group_frames=None):
-        """group_frames: [G, T] frame map into `pyr` (ct3_update_loop_frames), None = frame t."""
+        """group_frames: [G, T] frame map into `pyr` (ct3_update_loop_frames), None = frame t.
+        A pass whose full workspace exceeds the pass budget runs in the largest track slabs that fit
+        (ct3_update_loop_slabbed, bit-identical); every other pass runs as it always did."""
         T, N, _ = coords.shape
         dev = coords.device
         G = len(group_sizes)
-        T_pyr = None if group_frames is None else engine.pyramid_frames(pyr, H4, W4)
+        T_all = engine.pyramid_frames(pyr, H4, W4)
+        T_pyr = None if group_frames is None else T_all
+        budget = pass_budget_bytes(self, dev, T_all, H4 * self.stride, W4 * self.stride)
+        slab = slab_tracks_for(T, N, G, H4, W4, T_pyr, budget)
         engine.update_loop(self.packed_weights(dev), pyr, H4, W4, support, track_valid, coords, vis, conf,
-                           self.interpolate_time_embed(T).to(dev), iters, self._ws.get(T, N, dev, H4, W4, G, T_pyr),
-                           group_sizes=group_sizes if G > 1 or group_frames is not None else None,
-                           group_frames=group_frames)
+                           self.interpolate_time_embed(T).to(dev), iters,
+                           self._ws.get(T, N, dev, H4, W4, G, T_pyr, slab),
+                           group_sizes=group_sizes if G > 1 or group_frames is not None or slab else None,
+                           group_frames=group_frames, slab_tracks=slab)
 
     @staticmethod
     def _track_reversed(group_sizes, flags, device) -> torch.Tensor:

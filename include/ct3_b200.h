@@ -323,6 +323,28 @@ int ct3_update_loop_frames(const void* packed, const float* pyr, int T_pyr, int 
                            size_t workspace_bytes, ct3_stream_t stream, const int32_t* group_sizes_host, int G,
                            const int32_t* group_frames_host);
 
+/* ---- track slabs: the update loop in a bounded workspace ------------------------------------------------------
+ * ct3_update_loop_frames' arguments plus slab_tracks.  A null group_frames_host is the identity map (then T_pyr must
+ * equal T), as in ct3_update_loop_groups.  The stages that are independent per row (correlation, corr_mlp, token
+ * assembly, input_transform, the time blocks, the LayerNorm + projections of the point side of both cross blocks,
+ * out-projections and MLP halves) run on slabs of slab_tracks whole tracks (the 64*G virtual tracks in slabs of
+ * their own), so their scratch is sized by slab_tracks*T rows; the space attentions still see every track of a group
+ * in one launch.  Full-size per point row: the fp32 token (1536 B) and the point side of the space attentions
+ * (3072 B), 4608 B against 65,024 B of ct3_workspace_bytes_frames (DESIGN.md §4.4.5).
+ * Contract: coords/vis/conf are BIT-IDENTICAL to ct3_update_loop_frames (or _groups for a null map) on the same inputs
+ * and options, for every slab_tracks >= 1; slab_tracks >= N is that call's launch sequence and workspace.
+ *   workspace : ct3_workspace_bytes_slabbed(T, T_pyr, N, G, H4, W4, slab_tracks) bytes, non-decreasing in slab_tracks;
+ *               equal to ct3_workspace_bytes_frames for slab_tracks >= N
+ * slab_tracks < 1, (N + 64*G)*T > 2^21 token rows (the supported size: every element offset of a full-size buffer then
+ * stays below 2^31) and every invalid argument of ct3_update_loop_frames return CT3_EINVAL before anything is
+ * enqueued; a workspace smaller than the query returns CT3_ENOSPC. */
+int ct3_workspace_bytes_slabbed(int T, int T_pyr, int N, int G, int H4, int W4, int slab_tracks, size_t* out_bytes);
+int ct3_update_loop_slabbed(const void* packed, const float* pyr, int T_pyr, int H4, int W4, const float* support,
+                            const uint8_t* track_valid, float* coords, float* vis, float* conf,
+                            const float* time_emb, int T, int N, int iters, void* workspace,
+                            size_t workspace_bytes, ct3_stream_t stream, const int32_t* group_sizes_host, int G,
+                            const int32_t* group_frames_host, int slab_tracks);
+
 /* ---- live profiler (bench.py roofline): CUDA events around every launch of the library, summed per
  * kernel category: 0 corr_sample, 1 gemm (wgmma), 2 attention, 3 layernorm, 4 misc.
  * ct3_profile_enable(1) clears and starts recording; ct3_profile_read synchronises and sums. */
