@@ -1,6 +1,6 @@
 // api_loop.cu -- the update loop of the C ABI (see include/ct3_b200.h): weight packing, workspace carving and the
 // launch sequence of one refinement iteration (cotracker3_offline.py:139-216, cotracker.py:483-531), whole or in
-// track slabs (ct3_update_loop_slabbed, DESIGN.md §4.4.5).
+// track slabs (ct3_loop_shape.slab_tracks, DESIGN.md §4.4.5).
 #include <math.h>
 
 #include <string>
@@ -102,11 +102,11 @@ const std::vector<std::string>& weight_names() {
 }
 
 // ------------------------------------------------------------------------------------------------
-// workspace.  Without track slabs (slab == N) every buffer covers all rows.  With them (ct3_update_loop_slabbed,
-// slab < N) the scratch of the row-independent stages (vol, h1, xs, hmid, and the first S = slab*T rows of ln / att /
-// qkv) holds one slab of rows; ln / att keep the virtual rows full-size behind it; qkv is also the full-size space-
-// attention operand of the point rows (virtual<-point k|v [N*T, 768], then point<-virtual q [N*T, 384] followed by
-// its split output [N*T, 2*384]), which is never live at the same time as a time block's q|k|v.
+// workspace.  Without track slabs (slab == N) every buffer covers all rows.  With them (slab_tracks < N) the scratch
+// of the row-independent stages (vol, h1, xs, hmid, and the first S = slab*T rows of ln / att / qkv) holds one slab
+// of rows; ln / att keep the virtual rows full-size behind it; qkv is also the full-size space-attention operand of
+// the point rows (virtual<-point k|v [N*T, 768], then point<-virtual q [N*T, 384] followed by its split output
+// [N*T, 2*384]), which is never live at the same time as a time block's q|k|v.
 struct Workspace {
   __nv_bfloat16* vol;     // [S*4, 2*2432]
   __nv_bfloat16* h1;      // [S*4, 2*384]
@@ -121,7 +121,7 @@ struct Workspace {
   float* att_part;        // split-K partials of the virtual<-point attention
   __nv_bfloat16* pyr_split;  // split-bf16 copy of the pyramid (corr_tc2.cu); null when H4 == 0
   int32_t* groups;        // device group table of a grouped call (GroupPlan); null when G == 1
-  int32_t* frames;        // device frame map [G, T] of ct3_update_loop_frames; null without one
+  int32_t* frames;        // device frame map [G, T] of a pass with T_pyr >= 1; null without one
   int slab;               // tracks per slab; N: no slabs
   size_t total;
   bool slabbed() const { return slab_rows < point_rows; }
@@ -137,13 +137,12 @@ int partial_slots(int N, int G) {
 // int32 entries of the group table: offsets [G+1] | all [G] | split [G] | slot [G] | small [G] | tiles [2 * max tiles]
 int64_t group_table_ints(int N, int G) { return G == 1 ? 0 : (int64_t)5 * G + 1 + 2 * ((int64_t)N / 128 + G); }
 
-// T_pyr: frames of the pyramid the correlation reads (sizes the split copy; 0 = T); frames: room for a [G, T] frame map;
-// slab: tracks per slab (0 or >= N: no slabs)
-Workspace carve(void* base, int T, int N, int H4 = 0, int W4 = 0, int G = 1, int T_pyr = 0, bool frames = false,
-                int slab = 0) {
+// The workspace of pass s (a null base only measures): the split pyramid copy is sized by the T_pyr (0: T) frames the
+// correlation reads, room for the [G, T] frame map iff T_pyr >= 1, slab_tracks 0 or >= N: no slabs
+Workspace carve(void* base, const ct3_loop_shape& s) {
   Workspace w;
-  if (T_pyr == 0) T_pyr = T;
-  w.slab = slab > 0 && slab < N ? slab : N;
+  const int T = s.T, N = s.N, G = s.G, H4 = s.H4, W4 = s.W4, T_pyr = s.T_pyr > 0 ? s.T_pyr : s.T;
+  w.slab = s.slab_tracks > 0 && s.slab_tracks < N ? s.slab_tracks : N;
   const size_t R = (size_t)(N + (size_t)kV * G) * T, Rp = (size_t)N * T, Rv = (size_t)kV * G * T;
   const size_t S = (size_t)w.slab * T, Mc = S * kL;
   w.slab_rows = (int64_t)S;
@@ -165,7 +164,7 @@ Workspace carve(void* base, int T, int N, int H4 = 0, int W4 = 0, int G = 1, int
   if (H4 > 0 && W4 > 0 && corr_patch_supported(T_pyr, H4, W4))
     w.pyr_split = (__nv_bfloat16*)c.take((size_t)pyramid_layout(T_pyr, H4, W4).total * 4);
   w.groups = G > 1 ? (int32_t*)c.take((size_t)group_table_ints(N, G) * 4) : nullptr;
-  w.frames = frames ? (int32_t*)c.take((size_t)G * T * 4) : nullptr;
+  w.frames = s.T_pyr > 0 ? (int32_t*)c.take((size_t)G * T * 4) : nullptr;
   w.total = c.off;
   return w;
 }
@@ -242,8 +241,8 @@ AttnParams attn_params(const float* q, int q_ld, const float* kv, int kv_ld, int
   return a;
 }
 
-// Track groups of a grouped call (ct3_update_loop_groups): G contiguous track ranges, each with its own kV virtual
-// tokens at rows (N + kV*g + i)*T + t.  G == 1 is the plain call (no table; every kernel indexes as it always did).
+// Track groups of a pass (ct3_loop_shape.G): G contiguous track ranges, each with its own kV virtual tokens at rows
+// (N + kV*g + i)*T + t.  G == 1 is one group (no table; every kernel indexes as it always did).
 // For G > 1 the host builds the table below, uploads it into the workspace in stream order, and each space attention
 // runs over (group, frame) sequences, choosing per group what a standalone call on that group's tracks would.
 struct GroupPlan {
@@ -556,89 +555,72 @@ int check_TN(int T, int N, int G = 1) {
   return 0;
 }
 
-// The supported size of ct3_update_loop_slabbed: at most 2^21 token rows (N + 64 G)*T.  Track slabs make problems
+// The supported size of a pass in track slabs: at most 2^21 token rows (N + 64 G)*T.  Track slabs make problems
 // reachable whose full-size buffers (tokens, the point rows' space-attention operands, up to 768 elements per row)
 // no longer fit a full workspace; at this bound every element offset into them stays below 2^31, so no index
 // arithmetic on the slabbed path can overflow 32 bits.  The slab-sized stages run the kernels of a full-workspace
 // call on slab_tracks*T rows.
 constexpr int64_t kSlabbedMaxRows = (int64_t)1 << 21;
-int check_slabbed(int T, int N, int G, int slab_tracks) {
-  if (slab_tracks < 1) return fail(CT3_EINVAL, "slab_tracks must be >= 1%s");
-  if (((int64_t)N + (int64_t)kV * G) * T > kSlabbedMaxRows)
-    return fail(CT3_EINVAL, "problem too large for the slabbed loop: (N + 64 G) * T must be <= 2^21%s");
-  return 0;
-}
 
-// T, N and the track groups of update_loop / updateformer, in this order; *total = the tracks the sizes add up to.
-// n_from_sizes (updateformer with N < 0): the sizes define N, which is then checked after them.
-int check_groups(int T, int N, const int32_t* sizes, int G, int* total, bool n_from_sizes) {
-  if (!n_from_sizes)
-    if (int rc = check_TN(T, N)) return rc;
-  if (!sizes) return fail(CT3_EINVAL, "null group_sizes_host%s");
-  if (G < 1) return fail(CT3_EINVAL, "G must be >= 1%s");
-  int64_t sum = 0;
-  for (int g = 0; g < G; ++g) {
-    if (sizes[g] < 1) return fail(CT3_EINVAL, "every group size must be >= 1%s");
-    sum += sizes[g];
+// What a shape is checked for: the size query (host arrays checked when given; the pyramid unless H4 = W4 = 0 without
+// a frame map or slabs, the transformer alone), a loop run (arrays and pyramid required) or ct3_updateformer (arrays
+// required, no pyramid).
+enum class Use { kSize, kLoop, kFormer };
+
+int check_shape(const ct3_loop_shape* sh, Use use) {
+  if (!sh) return fail(CT3_EINVAL, "null shape%s");
+  const ct3_loop_shape& s = *sh;
+  if (int rc = check_TN(s.T, s.N, s.G)) return rc;
+  if (s.group_sizes) {
+    int64_t sum = 0;
+    for (int g = 0; g < s.G; ++g) {
+      if (s.group_sizes[g] < 1) return fail(CT3_EINVAL, "every group size must be >= 1%s");
+      sum += s.group_sizes[g];
+    }
+    if (sum != s.N) return fail(CT3_EINVAL, "group sizes must sum to N%s");
+  } else if (use != Use::kSize && s.G > 1) {
+    return fail(CT3_EINVAL, "null group_sizes with G > 1%s");
   }
-  if (sum > (int64_t)1 << 30) return fail(CT3_EINVAL, "problem too large%s");
-  if (!n_from_sizes && sum != N) return fail(CT3_EINVAL, "group sizes must sum to N%s");
-  *total = (int)sum;
-  return check_TN(T, *total, G);
+  if (s.slab_tracks < 0) return fail(CT3_EINVAL, "slab_tracks must be >= 0%s");
+  if (s.slab_tracks > 0 && ((int64_t)s.N + (int64_t)kV * s.G) * s.T > kSlabbedMaxRows)
+    return fail(CT3_EINVAL, "problem too large for track slabs: (N + 64 G) * T must be <= 2^21%s");
+  if (s.T_pyr < 0 || (s.T_pyr == 0 && s.group_frames))
+    return fail(CT3_EINVAL, "T_pyr must be >= 1 with a frame map and 0 without one%s");
+  if (s.T_pyr > 0) {
+    if (s.group_frames) {
+      for (int64_t i = 0; i < (int64_t)s.G * s.T; ++i)
+        if (s.group_frames[i] < 0 || s.group_frames[i] >= s.T_pyr)
+          return fail(CT3_EINVAL, "frame index outside [0, T_pyr)%s");
+    } else if (use != Use::kSize) {
+      return fail(CT3_EINVAL, "null group_frames with T_pyr >= 1%s");
+    }
+  }
+  const bool former = s.H4 == 0 && s.W4 == 0 && s.T_pyr == 0 && s.slab_tracks == 0;
+  if (use == Use::kFormer || (use == Use::kSize && former)) return 0;
+  const int T_pyr = s.T_pyr > 0 ? s.T_pyr : s.T;   // a step's frame index stays within int32
+  if ((int64_t)T_pyr * s.T >= (int64_t)1 << 31) return fail(CT3_EINVAL, "problem too large%s");
+  return check_pyramid(T_pyr, s.H4, s.W4);
 }
 
-// frame-map arguments of ct3_update_loop_frames / ct3_workspace_bytes_frames (frames == nullptr: not checked here)
-int check_frames(const int32_t* frames, int G, int T, int T_pyr) {
-  if (T_pyr < 1) return fail(CT3_EINVAL, "T_pyr must be >= 1%s");
-  if ((int64_t)T_pyr * T >= (int64_t)1 << 31 || (int64_t)G * T >= (int64_t)1 << 31)
-    return fail(CT3_EINVAL, "problem too large%s");
-  if (!frames) return 0;
-  for (int64_t i = 0; i < (int64_t)G * T; ++i)
-    if (frames[i] < 0 || frames[i] >= T_pyr) return fail(CT3_EINVAL, "frame index outside [0, T_pyr)%s");
-  return 0;
-}
-
-// ct3_workspace_bytes_groups (frames == false, T_pyr == T: the pyramid shape is checked only when given),
-// ct3_workspace_bytes_frames and, with slab > 0, ct3_workspace_bytes_slabbed
-int loop_workspace_bytes(int T, int T_pyr, int N, int G, int H4, int W4, bool frames, size_t* out_bytes,
-                         int slab = 0) {
-  if (!out_bytes) return fail(CT3_EINVAL, "null out_bytes%s");
-  if (int rc = check_TN(T, N, G)) return rc;
-  if (slab != 0)
-    if (int rc = check_slabbed(T, N, G, slab)) return rc;
-  if (frames)
-    if (int rc = check_frames(nullptr, G, T, T_pyr)) return rc;
-  if (frames || H4 != 0 || W4 != 0)
-    if (int rc = check_pyramid(T_pyr, H4, W4)) return rc;
-  *out_bytes = carve(nullptr, T, N, H4, W4, G, T_pyr, frames, slab).total;
-  return 0;
-}
-
-// frames: host frame map [G, T] into the T_pyr pyramid frames, or null (frame t, T_pyr == T).  slab: tracks per slab
-// of ct3_update_loop_slabbed (its workspace always has room for a frame map), 0 for the other entry points.
-int update_loop(const void* packed, const float* pyr, int H4, int W4, const float* support, const uint8_t* track_valid,
-                float* coords, float* vis, float* conf, const float* time_emb, int T, int N, const int32_t* sizes,
-                int G, int iters, void* workspace, size_t workspace_bytes, cudaStream_t stream, int T_pyr,
-                const int32_t* frames, int slab = 0) {
+int update_loop(const void* packed, const float* pyr, const float* support, const uint8_t* track_valid, float* coords,
+                float* vis, float* conf, const float* time_emb, int iters, const ct3_loop_shape* shape,
+                void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   if (!packed || !pyr || !support || !coords || !vis || !conf || !time_emb || !workspace)
     return fail(CT3_EINVAL, "null argument%s");
-  int total = 0;
-  if (int rc = check_groups(T, N, sizes, G, &total, false)) return rc;
-  if (slab != 0)
-    if (int rc = check_slabbed(T, N, G, slab)) return rc;
+  if (int rc = check_shape(shape, Use::kLoop)) return rc;
   if (iters < 0) return fail(CT3_EINVAL, "iters must be >= 0%s");
-  if (int rc = check_frames(frames, G, T, T_pyr)) return rc;
-  if (int rc = check_pyramid(T_pyr, H4, W4)) return rc;
   if (int rc = check_aligned(workspace, "workspace")) return rc;
-  const Workspace W = carve(workspace, T, N, H4, W4, G, T_pyr, frames != nullptr || slab != 0, slab);
+  const ct3_loop_shape& s = *shape;
+  const int T = s.T, N = s.N, G = s.G, H4 = s.H4, W4 = s.W4, T_pyr = s.T_pyr > 0 ? s.T_pyr : s.T;
+  const Workspace W = carve(workspace, s);
   if (int rc = check_space(workspace_bytes, W.total, "workspace")) return rc;
   const Layout& L = layout();
   Runner R{reinterpret_cast<const uint8_t*>(packed), L, stream, g_opt_gemm};
   GroupPlan gp;
-  if (int rc = plan_groups(gp, sizes, G, T, N, W.groups, R.s)) return rc;
+  if (int rc = plan_groups(gp, s.group_sizes, G, T, N, W.groups, R.s)) return rc;
   FrameMap fm;
-  if (frames) {   // the frame map reaches the device like the group table: in stream order, through kernel arguments
-    CK(launch_upload_i32(W.frames, frames, G * T, R.s), "upload frame map");
+  if (s.T_pyr > 0) {   // the frame map reaches the device like the group table: in stream order, through kernel args
+    CK(launch_upload_i32(W.frames, s.group_frames, G * T, R.s), "upload frame map");
     fm.frames = W.frames;
     fm.goff = G > 1 ? gp.off : nullptr;
     fm.G = G;
@@ -670,13 +652,10 @@ int loop_tokens(const void* packed, const float* pyr, int H4, int W4, const floa
                 size_t workspace_bytes, cudaStream_t stream) {
   if (!packed || !pyr || !support || !coords || !vis || !conf || !time_emb || !workspace)
     return fail(CT3_EINVAL, "null argument%s");
-  const int32_t one = N;
-  int total = 0;
-  if (int rc = check_groups(T, N, &one, 1, &total, false)) return rc;
-  if (int rc = check_frames(nullptr, 1, T, T)) return rc;
-  if (int rc = check_pyramid(T, H4, W4)) return rc;
+  const ct3_loop_shape shape{T, N, H4, W4, 1, nullptr, 0, nullptr, 0};
+  if (int rc = check_shape(&shape, Use::kLoop)) return rc;
   if (int rc = check_aligned(workspace, "workspace")) return rc;
-  const Workspace W = carve(workspace, T, N, H4, W4);
+  const Workspace W = carve(workspace, shape);
   if (int rc = check_space(workspace_bytes, W.total, "workspace")) return rc;
   const Layout& L = layout();
   Runner R{reinterpret_cast<const uint8_t*>(packed), L, stream, g_opt_gemm};
@@ -696,13 +675,13 @@ int loop_tokens(const void* packed, const float* pyr, int H4, int W4, const floa
   return 0;
 }
 
-// N < 0: the group sizes define N (ct3_updateformer_groups)
 int updateformer(const void* packed, const float* x, int T, int N, const int32_t* sizes, int G, float* delta,
                  void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   if (!packed || !x || !delta || !workspace) return fail(CT3_EINVAL, "null argument%s");
-  if (int rc = check_groups(T, N, sizes, G, &N, N < 0)) return rc;
+  const ct3_loop_shape shape{T, N, 0, 0, G, sizes, 0, nullptr, 0};
+  if (int rc = check_shape(&shape, Use::kFormer)) return rc;
   if (int rc = check_aligned(workspace, "workspace")) return rc;
-  const Workspace W = carve(workspace, T, N, 0, 0, G);
+  const Workspace W = carve(workspace, shape);
   if (int rc = check_space(workspace_bytes, W.total, "workspace")) return rc;
   Runner R{reinterpret_cast<const uint8_t*>(packed), layout(), stream, g_opt_gemm};
   GroupPlan gp;
@@ -727,8 +706,9 @@ int attention_stage(int kind, const float* q, const float* kv, int T, int N, con
                     void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   if (!q || !kv || !out || !workspace) return fail(CT3_EINVAL, "null argument%s");
   if (kind < CT3_ATTN_TIME || kind > CT3_ATTN_POINT_FROM_VIRTUAL) return fail(CT3_EINVAL, "unknown attention kind%s");
-  int total = 0;
-  if (int rc = check_groups(T, N, sizes, G, &total, false)) return rc;
+  const ct3_loop_shape shape{T, N, 0, 0, G, sizes, 0, nullptr, 0};
+  if (int rc = check_shape(&shape, Use::kFormer)) return rc;
+  if (!sizes) return fail(CT3_EINVAL, "null group_sizes_host%s");
   if (((uintptr_t)q | (uintptr_t)kv | (uintptr_t)out) & 15) return fail(CT3_EINVAL, "q, kv and out must be 16-byte aligned%s");
   if (int rc = check_aligned(workspace, "workspace")) return rc;
   const Workspace W = carve_attention(workspace, T, N, G);
@@ -890,21 +870,11 @@ int ct3_pack_weights(const float* const* t, int n_tensors, void* packed, size_t 
   return 0;
 }
 
-int ct3_workspace_bytes(int T, int N, int H4, int W4, size_t* out_bytes) {
-  return loop_workspace_bytes(T, T, N, 1, H4, W4, false, out_bytes);
-}
-
-int ct3_workspace_bytes_groups(int T, int N, int G, int H4, int W4, size_t* out_bytes) {
-  return loop_workspace_bytes(T, T, N, G, H4, W4, false, out_bytes);
-}
-
-int ct3_workspace_bytes_frames(int T, int T_pyr, int N, int G, int H4, int W4, size_t* out_bytes) {
-  return loop_workspace_bytes(T, T_pyr, N, G, H4, W4, true, out_bytes);
-}
-
-int ct3_workspace_bytes_slabbed(int T, int T_pyr, int N, int G, int H4, int W4, int slab_tracks, size_t* out_bytes) {
-  if (slab_tracks < 1) return fail(CT3_EINVAL, "slab_tracks must be >= 1%s");
-  return loop_workspace_bytes(T, T_pyr, N, G, H4, W4, true, out_bytes, slab_tracks);
+int ct3_workspace_bytes(const ct3_loop_shape* shape, size_t* out_bytes) {
+  if (!out_bytes) return fail(CT3_EINVAL, "null out_bytes%s");
+  if (int rc = check_shape(shape, Use::kSize)) return rc;
+  *out_bytes = carve(nullptr, *shape).total;
+  return 0;
 }
 
 int ct3_corr_sample(const float* pyr, int H4, int W4, const float* support, const uint8_t* track_valid,
@@ -985,39 +955,11 @@ int ct3_layernorm(const float* x, int rows, const float* gamma, const float* bet
   return 0;
 }
 
-int ct3_update_loop(const void* packed, const float* pyr, int H4, int W4, const float* support,
-                    const uint8_t* track_valid, float* coords, float* vis, float* conf, const float* time_emb,
-                    int T, int N, int iters, void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
-  const int32_t one = N;
-  return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, &one, 1, iters,
-                     workspace, workspace_bytes, (cudaStream_t)stream, T, nullptr);
-}
-
-int ct3_update_loop_groups(const void* packed, const float* pyr, int H4, int W4, const float* support,
-                           const uint8_t* track_valid, float* coords, float* vis, float* conf, const float* time_emb,
-                           int T, int N, int iters, void* workspace, size_t workspace_bytes, ct3_stream_t stream,
-                           const int32_t* group_sizes_host, int G) {
-  return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, group_sizes_host, G,
-                     iters, workspace, workspace_bytes, (cudaStream_t)stream, T, nullptr);
-}
-
-int ct3_update_loop_frames(const void* packed, const float* pyr, int T_pyr, int H4, int W4, const float* support,
-                           const uint8_t* track_valid, float* coords, float* vis, float* conf, const float* time_emb,
-                           int T, int N, int iters, void* workspace, size_t workspace_bytes, ct3_stream_t stream,
-                           const int32_t* group_sizes_host, int G, const int32_t* group_frames_host) {
-  if (!group_frames_host) return fail(CT3_EINVAL, "null group_frames_host%s");
-  return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, group_sizes_host, G,
-                     iters, workspace, workspace_bytes, (cudaStream_t)stream, T_pyr, group_frames_host);
-}
-
-int ct3_update_loop_slabbed(const void* packed, const float* pyr, int T_pyr, int H4, int W4, const float* support,
-                            const uint8_t* track_valid, float* coords, float* vis, float* conf, const float* time_emb,
-                            int T, int N, int iters, void* workspace, size_t workspace_bytes, ct3_stream_t stream,
-                            const int32_t* group_sizes_host, int G, const int32_t* group_frames_host, int slab_tracks) {
-  if (slab_tracks < 1) return fail(CT3_EINVAL, "slab_tracks must be >= 1%s");
-  if (!group_frames_host && T_pyr != T) return fail(CT3_EINVAL, "without a frame map T_pyr must equal T%s");
-  return update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, T, N, group_sizes_host, G,
-                     iters, workspace, workspace_bytes, (cudaStream_t)stream, T_pyr, group_frames_host, slab_tracks);
+int ct3_update_loop(const void* packed, const float* pyr, const float* support, const uint8_t* track_valid,
+                    float* coords, float* vis, float* conf, const float* time_emb, int iters,
+                    const ct3_loop_shape* shape, void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+  return update_loop(packed, pyr, support, track_valid, coords, vis, conf, time_emb, iters, shape, workspace,
+                     workspace_bytes, (cudaStream_t)stream);
 }
 
 int ct3_loop_tokens(const void* packed, const float* pyr, int H4, int W4, const float* support,
@@ -1028,15 +970,9 @@ int ct3_loop_tokens(const void* packed, const float* pyr, int H4, int W4, const 
                      tokens_out, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
-int ct3_updateformer(const void* packed, const float* x, int T, int N, float* delta, void* workspace,
-                     size_t workspace_bytes, ct3_stream_t stream) {
-  const int32_t one = N;
-  return updateformer(packed, x, T, N, &one, 1, delta, workspace, workspace_bytes, (cudaStream_t)stream);
-}
-
-int ct3_updateformer_groups(const void* packed, const float* x, int T, const int32_t* group_sizes_host, int G,
-                            float* delta, void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
-  return updateformer(packed, x, T, -1, group_sizes_host, G, delta, workspace, workspace_bytes, (cudaStream_t)stream);
+int ct3_updateformer(const void* packed, const float* x, int T, int N, const int32_t* group_sizes_host, int G,
+                     float* delta, void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+  return updateformer(packed, x, T, N, group_sizes_host, G, delta, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int ct3_attention_workspace_bytes(int T, int N, int G, size_t* out_bytes) {

@@ -92,11 +92,11 @@ cudaError_t launch_upsample_concat_split(const float* const src[4], const int c[
                                          const int w[4], int T, int Cp, int H, int W, __nv_bfloat16* out, cudaStream_t s);
 
 // ---- corr.cu : correlation sampling ---------------------------------------------------------------
-// Frame map of ct3_update_loop_frames: at time step t, track n of group g reads pyramid frame frames[g*T + t] (an index
+// Frame map of a ct3_update_loop pass: at time step t, track n of group g reads pyramid frame frames[g*T + t] (an index
 // into the T_pyr frames of the pyramid).  frames == nullptr: frame t.  goff: [G+1] first track of every group (nullptr
 // when G == 1).  Every correlation kernel works on units of ONE track, so the lookup is per (track, t): no tile or TMA
 // box ever spans two tracks' frames.  n0: the global index of the launch's first track (a track slab of
-// ct3_update_loop_slabbed); the group lookup is by global track.
+// ct3_loop_shape.slab_tracks); the group lookup is by global track.
 struct FrameMap {
   const int32_t* frames = nullptr;
   const int32_t* goff = nullptr;
@@ -128,7 +128,7 @@ __device__ __forceinline__ int map_frame(const int32_t* row, int t) { return row
 // FLOP (3|2|1; pyr_split must have been made with the same mode) and a single-fp16-plane volume [N*T*4, kVolPad]
 // instead of the split one; the other kernels always compute in fp32 / bf16x3 and write the split volume.
 // Track range: the launch covers tracks [n0, n0 + count) of the N-track state and support (N stays their pitch) and
-// writes their volume rows from row 0 of vol_split (a track slab of ct3_update_loop_slabbed; n0 = 0, count = N: all).
+// writes their volume rows from row 0 of vol_split (a track slab of a ct3_update_loop pass; n0 = 0, count = N: all).
 // The dispatcher moves support / track_valid / coords to track n0 and sets fm.n0; the kernels below it see `count`
 // tracks at pitch N.
 bool corr_uses_patch_kernel(int impl, bool have_pyr_split, int T, int H4, int W4);
@@ -187,7 +187,7 @@ struct AttnParams {
   int64_t q_seq_stride, q_tok_stride;  // q/out row = s*q_seq_stride + i*q_tok_stride
   int64_t k_seq_stride, k_tok_stride;  // k/v row  = s*k_seq_stride + j*k_tok_stride
   float scale;
-  // Grouped space attention (ct3_update_loop_groups): the tracks form contiguous groups, each with its own kV virtual
+  // Grouped space attention (ct3_loop_shape.G > 1): the tracks form contiguous groups, each with its own kV virtual
   // tokens.  gl == nullptr: one group, rows as above.  Otherwise sequence s = (entry s / frames, frame s % frames),
   // entry e covers group gl[e], and Lq / Lk are upper bounds.  A side with grp_stride != 0 is virtual (group g starts
   // at row g * grp_stride, kV tokens); a side with grp_stride == 0 holds points (group g = tracks [goff[g], goff[g+1])).

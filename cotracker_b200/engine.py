@@ -34,6 +34,13 @@ class OnlineStream(ctypes.Structure):
                 ("scale_x", ctypes.c_float), ("scale_y", ctypes.c_float)]
 
 
+class LoopShape(ctypes.Structure):
+    """ct3_loop_shape (include/ct3_b200.h): one update-loop pass."""
+    _fields_ = [("T", ctypes.c_int), ("N", ctypes.c_int), ("H4", ctypes.c_int), ("W4", ctypes.c_int),
+                ("G", ctypes.c_int), ("group_sizes", ctypes.POINTER(ctypes.c_int32)), ("T_pyr", ctypes.c_int),
+                ("group_frames", ctypes.POINTER(ctypes.c_int32)), ("slab_tracks", ctypes.c_int)]
+
+
 def _signatures():
     """name -> (restype, argtypes) of every entry point of include/ct3_b200.h"""
     c_int, c_size_t, c_void_p, c_char_p = ctypes.c_int, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_char_p
@@ -69,9 +76,9 @@ def _signatures():
         "ct3_render_flow_workspace_bytes": (c_int, [c_int, c_int, ctypes.POINTER(c_size_t)]),
         "ct3_render_flow_colors": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
         "ct3_sample_support": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
-        "ct3_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
-        "ct3_update_loop": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                    c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+        "ct3_workspace_bytes": (c_int, [ctypes.POINTER(LoopShape), ctypes.POINTER(c_size_t)]),
+        "ct3_update_loop": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_int, ctypes.POINTER(LoopShape), c_void_p, c_size_t, c_void_p]),
         "ct3_corr_sample": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                     c_size_t, c_void_p]),
         "ct3_loop_tokens": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -86,26 +93,11 @@ def _signatures():
         "ct3_time_block_attention_workspace_bytes": (c_int, [c_int, c_int, ctypes.POINTER(c_size_t)]),
         "ct3_time_block_attention": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t,
                                              c_void_p]),
-        "ct3_updateformer": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
-        "ct3_workspace_bytes_groups": (c_int, [c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
-        "ct3_update_loop_groups": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-                                           c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p,
-                                           ctypes.POINTER(ctypes.c_int32), c_int]),
-        "ct3_updateformer_groups": (c_int, [c_void_p, c_void_p, c_int, ctypes.POINTER(ctypes.c_int32), c_int, c_void_p,
-                                            c_void_p, c_size_t, c_void_p]),
+        "ct3_updateformer": (c_int, [c_void_p, c_void_p, c_int, c_int, ctypes.POINTER(ctypes.c_int32), c_int, c_void_p,
+                                     c_void_p, c_size_t, c_void_p]),
         "ct3_attention_workspace_bytes": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
         "ct3_attention": (c_int, [c_int, c_void_p, c_void_p, c_int, c_int, ctypes.POINTER(ctypes.c_int32), c_int, c_void_p,
                                   c_void_p, c_size_t, c_void_p]),
-        "ct3_workspace_bytes_frames": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
-        "ct3_update_loop_frames": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-                                           c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p,
-                                           ctypes.POINTER(ctypes.c_int32), c_int, ctypes.POINTER(ctypes.c_int32)]),
-        "ct3_workspace_bytes_slabbed": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int,
-                                                ctypes.POINTER(c_size_t)]),
-        "ct3_update_loop_slabbed": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
-                                            c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t,
-                                            c_void_p, ctypes.POINTER(ctypes.c_int32), c_int,
-                                            ctypes.POINTER(ctypes.c_int32), c_int]),
         "ct3_upsample_concat": (c_int, [ctypes.POINTER(c_void_p), intp, intp, intp, c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_enc_tail_packed_bytes": (c_int, [ctypes.POINTER(c_size_t)]),
         "ct3_enc_tail_pack": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
@@ -483,18 +475,18 @@ def sample_support(pyr, T, H4, W4, qframes, qcoords, support=None, accumulate_ma
     return support
 
 
+def _loop_shape(T, N, H4, W4, G=1, sizes=None, T_pyr=None, frames=None, slab_tracks=None) -> LoopShape:
+    """ct3_loop_shape of a pass; None = the field's default (no map, no slabs)."""
+    return LoopShape(int(T), int(N), int(H4), int(W4), int(G), sizes, int(T_pyr or 0), frames, int(slab_tracks or 0))
+
+
 def workspace_bytes(T: int, N: int, H4: int = 0, W4: int = 0, groups: int = 1, frames: Optional[int] = None,
                     slab_tracks: Optional[int] = None) -> int:
     """Scratch of ct3_update_loop for T frames of H4 x W4 feature maps and N tracks (H4 = W4 = 0: updateformer only),
-    split into `groups` track groups (ct3_update_loop_groups).  frames: the T_pyr pyramid frames of a call with a
-    frame map (ct3_update_loop_frames).  slab_tracks: the loop in track slabs of that many tracks
-    (ct3_update_loop_slabbed; frames None = T)."""
-    if slab_tracks is not None:
-        return _size("ct3_workspace_bytes_slabbed", int(T), int(T if frames is None else frames), int(N), int(groups),
-                     int(H4), int(W4), int(slab_tracks))
-    if frames is not None:
-        return _size("ct3_workspace_bytes_frames", int(T), int(frames), int(N), int(groups), int(H4), int(W4))
-    return _size("ct3_workspace_bytes_groups", int(T), int(N), int(groups), int(H4), int(W4))
+    split into `groups` track groups.  frames: the T_pyr pyramid frames of a pass with a frame map.  slab_tracks: the
+    loop in track slabs of that many tracks."""
+    shape = _loop_shape(T, N, H4, W4, groups, None, frames, None, slab_tracks)
+    return _size("ct3_workspace_bytes", ctypes.byref(shape))
 
 
 def pyramid_frames(pyr: torch.Tensor, H4: int, W4: int) -> int:
@@ -506,7 +498,7 @@ def pyramid_frames(pyr: torch.Tensor, H4: int, W4: int) -> int:
 
 
 def _group_array(group_sizes):
-    """Host int32 array of the group sizes (ct3_*_groups); the library validates the values."""
+    """Host int32 array of the group sizes (ct3_loop_shape.group_sizes); the library validates the values."""
     try:
         sizes = [int(g) for g in group_sizes]
     except (TypeError, ValueError) as e:
@@ -547,13 +539,14 @@ def _frame_array(group_frames, G: int, T: int):
 def update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, iters, workspace,
                 group_sizes: Optional[Sequence[int]] = None, group_frames=None, slab_tracks: Optional[int] = None):
     """In-place refinement of coords [T,N,2], vis [T,N], conf [T,N] (fp32, feature-grid units / logits).
-    group_sizes: the N tracks as contiguous independent groups (ct3_update_loop_groups); each group's result is
-    bit-identical to a call on its tracks alone.  None = one group.
-    group_frames: [G, T] frame map (ct3_update_loop_frames): group g reads frame group_frames[g][t] of `pyr` (which may
-    hold any number of frames) at time step t; each group's result is bit-identical to a call on a pyramid of exactly
-    those frames.  None = frame t.
-    slab_tracks: run in track slabs of that many tracks (ct3_update_loop_slabbed) in a workspace of
-    workspace_bytes(..., slab_tracks=); bit-identical to the call without.  None = no slabs."""
+    One ct3_update_loop call with the ct3_loop_shape the arguments describe.
+    group_sizes: the N tracks as contiguous independent groups; each group's result is bit-identical to a call on its
+    tracks alone.  None = one group.
+    group_frames: [G, T] frame map: group g reads frame group_frames[g][t] of `pyr` (which may hold any number of
+    frames) at time step t; each group's result is bit-identical to a call on a pyramid of exactly those frames.
+    None = frame t.
+    slab_tracks: run in track slabs of that many tracks in a workspace of workspace_bytes(..., slab_tracks=);
+    bit-identical to the call without.  None = no slabs."""
     _req(coords, torch.float32, "coords"); _req(vis, torch.float32, "vis"); _req(conf, torch.float32, "conf")
     _req(pyr, torch.float32, "pyr"); _req(support, torch.float32, "support"); _req(time_emb, torch.float32, "time_emb")
     T, N, _ = coords.shape
@@ -562,18 +555,14 @@ def update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, ti
     if track_valid is not None:
         _req(track_valid, torch.uint8, "track_valid")
     arr, G = _group_array(group_sizes if group_sizes is not None else [N])
-    state = (_ptr(support), _ptr(track_valid), _ptr(coords), _ptr(vis), _ptr(conf), _ptr(time_emb), T, N, int(iters),
-             _ptr(workspace), workspace.numel(), _stream(coords.device), arr, G)
-    if slab_tracks is not None:
-        fr = None if group_frames is None else _frame_array(group_frames, G, T)
-        T_pyr = T if group_frames is None else pyramid_frames(pyr, H4, W4)
-        _call("ct3_update_loop_slabbed", coords.device, _ptr(packed), _ptr(pyr), T_pyr, H4, W4, *state, fr,
-              int(slab_tracks))
-    elif group_frames is None:
-        _call("ct3_update_loop_groups", coords.device, _ptr(packed), _ptr(pyr), H4, W4, *state)
+    if group_frames is None:
+        T_pyr, fr = None, None
     else:
-        _call("ct3_update_loop_frames", coords.device, _ptr(packed), _ptr(pyr), pyramid_frames(pyr, H4, W4), H4, W4,
-              *state, _frame_array(group_frames, G, T))
+        T_pyr, fr = pyramid_frames(pyr, H4, W4), _frame_array(group_frames, G, T)
+    shape = _loop_shape(T, N, H4, W4, G, arr, T_pyr, fr, slab_tracks)
+    _call("ct3_update_loop", coords.device, _ptr(packed), _ptr(pyr), _ptr(support), _ptr(track_valid), _ptr(coords),
+          _ptr(vis), _ptr(conf), _ptr(time_emb), int(iters), ctypes.byref(shape), _ptr(workspace), workspace.numel(),
+          _stream(coords.device))
 
 
 # ---- stage-level wrappers (tests, profiles) -----------------------------------------------------------
@@ -762,25 +751,17 @@ def time_block_attention(packed, depth: int, x_split: torch.Tensor, T: int,
 def updateformer(packed, x: torch.Tensor, workspace: Optional[torch.Tensor] = None,
                  group_sizes: Optional[Sequence[int]] = None) -> torch.Tensor:
     """x [N,T,1110] fp32 (reference column order, time embedding added) -> delta [N,T,4].
-    group_sizes: contiguous independent track groups (ct3_updateformer_groups), None = one group."""
+    group_sizes: contiguous independent track groups, None = one group."""
     _req(x, torch.float32, "x")
     N, T, D = x.shape
     if D != XDIM:
         raise EngineError("x must be [N,T,1110]")
     delta = torch.empty(N, T, 4, dtype=torch.float32, device=x.device)
-    if group_sizes is not None:
-        arr, G = _group_array(group_sizes)
-        if sum(arr[:G]) != N:
-            raise EngineError(f"group sizes sum to {sum(arr[:G])}, x has {N} tracks")
-        if workspace is None:
-            workspace = torch.empty(workspace_bytes(T, N, groups=G), dtype=torch.uint8, device=x.device)
-        _call("ct3_updateformer_groups", x.device, _ptr(packed), _ptr(x), T, arr, G, _ptr(delta), _ptr(workspace),
-              workspace.numel(), _stream(x.device))
-        return delta
+    arr, G = _group_array(group_sizes) if group_sizes is not None else (None, 1)
     if workspace is None:
-        workspace = torch.empty(workspace_bytes(T, N), dtype=torch.uint8, device=x.device)
-    _call("ct3_updateformer", x.device, _ptr(packed), _ptr(x), T, N, _ptr(delta), _ptr(workspace), workspace.numel(),
-          _stream(x.device))
+        workspace = torch.empty(workspace_bytes(T, N, groups=G), dtype=torch.uint8, device=x.device)
+    _call("ct3_updateformer", x.device, _ptr(packed), _ptr(x), T, N, arr, G, _ptr(delta), _ptr(workspace),
+          workspace.numel(), _stream(x.device))
     return delta
 
 
@@ -918,18 +899,6 @@ def reverse_pyramid_(pyr: torch.Tensor, T: int, H4: int, W4: int, pad: int = 0, 
         if pad > 0:
             lv[T:].copy_(lv[T - 1:T].expand(pad, -1, -1, -1))
     return pyr
-
-
-def concat_pyramid_frames(pyr_a: torch.Tensor, Ta: int, a0: int, pyr_b: torch.Tensor, Tb: int, H4: int, W4: int):
-    """Flat pyramid holding frames [a0, Ta) of `pyr_a` followed by all Tb frames of `pyr_b` (online feature reuse)."""
-    off_a, h, w, _ = pyramid_layout(Ta, H4, W4)
-    off_b, _, _, _ = pyramid_layout(Tb, H4, W4)
-    parts = []
-    for l in range(LEVELS):
-        per = h[l] * w[l] * LATENT
-        parts.append(pyr_a[off_a[l] + a0 * per: off_a[l] + Ta * per])
-        parts.append(pyr_b[off_b[l]: off_b[l] + Tb * per])
-    return torch.cat(parts)
 
 
 def concat_pyramid_runs(runs, H4: int, W4: int) -> torch.Tensor:

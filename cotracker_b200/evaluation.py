@@ -102,7 +102,7 @@ def pass_budget_bytes(model, device, T: int, ih: int, iw: int) -> int:
 
 
 def slab_tracks_for(T: int, N: int, G: int, H4: int, W4: int, frames: Optional[int], budget_bytes: int) -> Optional[int]:
-    """Track slabs of one update-loop pass (ct3_update_loop_slabbed, DESIGN.md §4.4.5): None when the full workspace
+    """Track slabs of one update-loop pass (ct3_loop_shape.slab_tracks, DESIGN.md §4.4.5): None when the full workspace
     fits `budget_bytes`, so every pass that fits runs exactly as without slabs; else the largest slab_tracks whose
     workspace fits (the workspace never shrinks as slab_tracks grows), or 1 when none does.
     frames: the pyramid frames of a pass with a frame map (engine.workspace_bytes)."""

@@ -91,7 +91,7 @@ def sincos_time_embedding(dim: int, length: int) -> torch.Tensor:
 
 
 # ------------------------------------------------------------------------------------------------------
-# frame maps (ct3_update_loop_frames): which pyramid frame each group reads at each time step
+# frame maps (ct3_loop_shape.group_frames): which pyramid frame each group reads at each time step
 def clip_frame_map(T: int, reversed_groups) -> List[List[int]]:
     """Offline model: a forward group reads frame t, a group on the clip played backwards frame T-1-t."""
     return [list(range(T - 1, -1, -1)) if r else list(range(T)) for r in reversed_groups]
@@ -300,9 +300,9 @@ class CoTrackerThreeBase(nn.Module):
             raise engine.EngineError("cotracker_b200 runs on CUDA only; move the module and inputs to a GPU")
 
     def _refine(self, pyr, H4, W4, support, track_valid, coords, vis, conf, iters, group_sizes, group_frames=None):
-        """group_frames: [G, T] frame map into `pyr` (ct3_update_loop_frames), None = frame t.
+        """group_frames: [G, T] frame map into `pyr` (ct3_loop_shape.group_frames), None = frame t.
         A pass whose full workspace exceeds the pass budget runs in the largest track slabs that fit
-        (ct3_update_loop_slabbed, bit-identical); every other pass runs as it always did."""
+        (ct3_loop_shape.slab_tracks, bit-identical); every other pass runs as it always did."""
         T, N, _ = coords.shape
         dev = coords.device
         G = len(group_sizes)
@@ -313,8 +313,7 @@ class CoTrackerThreeBase(nn.Module):
         engine.update_loop(self.packed_weights(dev), pyr, H4, W4, support, track_valid, coords, vis, conf,
                            self.interpolate_time_embed(T).to(dev), iters,
                            self._ws.get(T, N, dev, H4, W4, G, T_pyr, slab),
-                           group_sizes=group_sizes if G > 1 or group_frames is not None or slab else None,
-                           group_frames=group_frames, slab_tracks=slab)
+                           group_sizes=group_sizes, group_frames=group_frames, slab_tracks=slab)
 
     @staticmethod
     def _track_reversed(group_sizes, flags, device) -> torch.Tensor:
@@ -327,7 +326,7 @@ class CoTrackerThreeBase(nn.Module):
         """Track G independent query sets over one clip in one pass.
 
         queries [1, sum(group_sizes), 3] holds the groups one after another.  The clip is encoded once and the support
-        features are sampled once; each window runs one update loop for all groups together (ct3_update_loop_groups),
+        features are sampled once; each window runs one update loop for all groups together (ct3_loop_shape.G),
         where every group keeps its own virtual tokens.  Returns the 4-tuple of `forward`; the columns of each group
         are bit-identical to `forward(video, that group's queries)`.  Streaming (is_online=True) is not grouped.
         reversed_groups: G flags; a flagged group is tracked on the clip played backwards (its query frames and its

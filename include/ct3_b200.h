@@ -18,7 +18,7 @@
  *     never throws / exits; ct3_last_error() returns a thread-local message;
  *   - all work is enqueued on the given cudaStream_t and is asynchronous w.r.t.
  *     the host; the update loop has no batch dimension (cotracker3_offline.py:135,141): a batch of clips is
- *     more query groups of one ct3_update_loop_frames call, each reading its own frames of one pyramid.
+ *     more query groups of one ct3_update_loop pass with a frame map, each reading its own frames of one pyramid.
  *
  * Symbols (all extern "C"):  see the declarations below; tests/test_host_logic.py checks
  * that the built library exports each of them.
@@ -263,87 +263,68 @@ int ct3_enc_tail(const void* packed, const float* cat, int T, int H4, int W4, fl
                  size_t workspace_bytes, ct3_stream_t stream);
 
 /* ---- the hot loop -----------------------------------------------------------
- * ct3_workspace_bytes: scratch needed by ct3_update_loop for a window of T frames of H4 x W4 feature maps and N
- * tracks (includes the split-bf16 copy of the pyramid the correlation kernel reads through TMA);
- * H4 = W4 = 0 sizes it for ct3_updateformer alone. */
-int ct3_workspace_bytes(int T, int N, int H4, int W4, size_t* out_bytes);
+ * One update-loop pass is described by a ct3_loop_shape.
+ *   groups       : the N tracks form G contiguous groups of group_sizes[0..G-1] tracks.  Each group has its own 64
+ *                  virtual tokens and the space attention stays inside its group; the groups share every other launch
+ *                  (correlation, corr_mlp, GEMMs, LayerNorms, time attention, heads).
+ *   frame map    : with T_pyr >= 1, at time step t group g reads pyramid frame group_frames[g*T + t], an index into
+ *                  the T_pyr frames of `pyr` (ct3_pyramid_layout(T_pyr, H4, W4)).  A group tracking the clip played
+ *                  backwards uses T-1-t; a padded window of the sliding-window model uses clamped indices.  Only
+ *                  correlation sampling reads frames: time attention, the time embedding, tokens and heads work on the
+ *                  group's own time axis.  With T_pyr = 0 step t reads frame t of a T-frame pyramid.
+ *   track slabs  : with slab_tracks >= 1 the stages that are independent per row (correlation, corr_mlp, token
+ *                  assembly, input_transform, the time blocks, the LayerNorm + projections of the point side of both
+ *                  cross blocks, out-projections and MLP halves) run on slabs of slab_tracks whole tracks (the 64*G
+ *                  virtual tracks in slabs of their own), so their scratch is sized by slab_tracks*T rows; the space
+ *                  attentions still see every track of a group in one launch.  Full-size per point row: the fp32 token
+ *                  (1536 B) and the point side of the space attentions (3072 B), 4608 B against 65,024 B without slabs
+ *                  (DESIGN.md §4.4.5).  Supported up to (N + 64*G)*T <= 2^21 token rows: every element offset of a
+ *                  full-size buffer then stays below 2^31.
+ * Contract (default options, same device): group g's coords/vis/conf are BIT-IDENTICAL to a pass over that group's
+ * tracks alone (G = 1, no slabs) on a pyramid holding frames group_frames[g][0..T) in that order (without a map: the
+ * same pyramid), whatever the other groups are; and BIT-IDENTICAL for every slab_tracks: slab_tracks >= N is the
+ * launch sequence and workspace of slab_tracks = 0.
+ * group_sizes and group_frames are HOST arrays and may be freed when the call returns: the device-side group table and
+ * frame map live in the workspace and are filled in stream order (the library still allocates nothing).
+ * Options: the default kernels and the exact-fp32 verification kernels ("gemm" / "corr" / "attn" = 1) support G > 1. */
+typedef struct ct3_loop_shape {
+  int T, N;                       /* loop time steps, tracks (both >= 1)                                              */
+  int H4, W4;                     /* level-0 feature map; 0, 0 = transformer only (ct3_updateformer sizing)           */
+  int G;                          /* track groups, 1 <= G <= N                                                        */
+  const int32_t* group_sizes;     /* HOST [G], each >= 1, sum N; NULL allowed only for G == 1                         */
+  int T_pyr;                      /* 0: no frame map, step t reads frame t of a T-frame pyramid;
+                                     >= 1: a frame map into T_pyr frames is given                                     */
+  const int32_t* group_frames;    /* HOST [G*T] indices into [0, T_pyr) iff T_pyr >= 1, else NULL                     */
+  int slab_tracks;                /* 0: no slabs; >= 1: track slabs, and then (N + 64 G) T <= 2^21                    */
+} ct3_loop_shape;
 
-/* ct3_update_loop: `iters` refinement iterations, in place on the state.
+/* ct3_workspace_bytes: scratch needed by ct3_update_loop for `shape` (it includes the split-bf16 copy of the T_pyr
+ * (0: T) frame pyramid the correlation kernel reads through TMA, sized once per call).  Only the numeric fields are
+ * needed, so a pass can be sized before its arrays exist; the arrays are validated when given.  Grows by 64*T virtual
+ * token rows per group; non-decreasing in slab_tracks.  H4 = W4 = 0 (with T_pyr = slab_tracks = 0) sizes
+ * ct3_updateformer. */
+int ct3_workspace_bytes(const ct3_loop_shape* shape, size_t* out_bytes);
+
+/* ct3_update_loop: `iters` refinement iterations of the pass `shape`, in place on the state.
  *   packed   : ct3_pack_weights output
- *   pyr      : ct3_prepare_pyramid output (T frames of the window)
+ *   pyr      : ct3_prepare_pyramid output (T frames of the window; T_pyr frames with a frame map)
  *   support  : [4][49,N,128] fp32; track_valid (may be NULL) [N] uint8 zeroes the
  *              support of not-yet-queried tracks (cotracker3_online.py:493-496)
  *   coords   : [T,N,2] fp32 stride-4 feature units, in/out
  *   vis,conf : [T,N] fp32 logits, in/out
  *   time_emb : [T,1110] fp32 (buffer already interpolated to T,
  *              cotracker3_online.py:145-156)
+ *   workspace: ct3_workspace_bytes(shape) bytes, 256-byte aligned
  * On return coords/vis/conf hold the state after the last iteration (the caller
- * multiplies coords by the stride and applies sigmoid, cotracker3_offline.py:213-216). */
-int ct3_update_loop(const void* packed, const float* pyr, int H4, int W4, const float* support,
-                    const uint8_t* track_valid, float* coords, float* vis, float* conf,
-                    const float* time_emb, int T, int N, int iters, void* workspace,
-                    size_t workspace_bytes, ct3_stream_t stream);
-
-/* ---- grouped calls: G independent query sets over one clip in one pass ---------------------------------
- * The N tracks form G contiguous groups of group_sizes_host[0..G-1] tracks (sum = N).  Each group has its own 64
- * virtual tokens, and the space attention stays inside its group, so for every group coords/vis/conf (delta) are
- * BIT-IDENTICAL to a standalone call on that group's tracks alone, whatever the other groups are (default options,
- * same device).  The groups share every other launch: correlation, corr_mlp, GEMMs, LayerNorms, time attention, heads.
- * G = 1 is ct3_update_loop / ct3_updateformer.
- *   group_sizes_host : HOST array of G sizes >= 1; it may be freed when the call returns (the device-side group table
- *                      lives in the workspace and is filled in stream order; the library still allocates nothing)
- *   workspace        : ct3_workspace_bytes_groups(T, N, G, H4, W4) bytes (grows by 64*T*G virtual token rows)
- * A null group array, G < 1, a size < 1 or sizes not summing to N return CT3_EINVAL before anything is enqueued.
- * Options: the default kernels and the exact-fp32 verification kernels ("gemm" / "corr" / "attn" = 1) support
- * G > 1. */
-int ct3_workspace_bytes_groups(int T, int N, int G, int H4, int W4, size_t* out_bytes);
-int ct3_update_loop_groups(const void* packed, const float* pyr, int H4, int W4, const float* support,
-                           const uint8_t* track_valid, float* coords, float* vis, float* conf,
-                           const float* time_emb, int T, int N, int iters, void* workspace,
-                           size_t workspace_bytes, ct3_stream_t stream, const int32_t* group_sizes_host, int G);
-
-/* ---- frame maps: groups whose time step t reads a pyramid frame other than t ----------------------------------
- * ct3_update_loop_groups plus one HOST table group_frames_host [G, T]: at time step t, group g reads pyramid frame
- * group_frames_host[g*T + t], an index into the T_pyr frames of `pyr` (ct3_pyramid_layout(T_pyr, H4, W4)).  The identity
- * map (T_pyr = T) is ct3_update_loop_groups; a group tracking the clip played backwards uses T-1-t; a padded window of
- * the sliding-window model uses clamped indices.  Only correlation sampling reads frames: time attention, the time
- * embedding, tokens and heads work on the group's own time axis.
- * Contract: group g's coords/vis/conf are BIT-IDENTICAL to a standalone ct3_update_loop on a pyramid holding frames
- * group_frames_host[g][0..T) in that order (default options, same device).
- *   group_frames_host : may be freed when the call returns (the device copy lives in the workspace, filled in stream
- *                       order like the group table)
- *   workspace         : ct3_workspace_bytes_frames(T, T_pyr, N, G, H4, W4) bytes (the split-bf16 pyramid copy is sized
- *                       by T_pyr and made once per call)
- * A null table, a frame index outside [0, T_pyr), T_pyr < 1 and every invalid argument of ct3_update_loop_groups return
- * CT3_EINVAL before anything is enqueued. */
-int ct3_workspace_bytes_frames(int T, int T_pyr, int N, int G, int H4, int W4, size_t* out_bytes);
-int ct3_update_loop_frames(const void* packed, const float* pyr, int T_pyr, int H4, int W4, const float* support,
-                           const uint8_t* track_valid, float* coords, float* vis, float* conf,
-                           const float* time_emb, int T, int N, int iters, void* workspace,
-                           size_t workspace_bytes, ct3_stream_t stream, const int32_t* group_sizes_host, int G,
-                           const int32_t* group_frames_host);
-
-/* ---- track slabs: the update loop in a bounded workspace ------------------------------------------------------
- * ct3_update_loop_frames' arguments plus slab_tracks.  A null group_frames_host is the identity map (then T_pyr must
- * equal T), as in ct3_update_loop_groups.  The stages that are independent per row (correlation, corr_mlp, token
- * assembly, input_transform, the time blocks, the LayerNorm + projections of the point side of both cross blocks,
- * out-projections and MLP halves) run on slabs of slab_tracks whole tracks (the 64*G virtual tracks in slabs of
- * their own), so their scratch is sized by slab_tracks*T rows; the space attentions still see every track of a group
- * in one launch.  Full-size per point row: the fp32 token (1536 B) and the point side of the space attentions
- * (3072 B), 4608 B against 65,024 B of ct3_workspace_bytes_frames (DESIGN.md §4.4.5).
- * Contract: coords/vis/conf are BIT-IDENTICAL to ct3_update_loop_frames (or _groups for a null map) on the same inputs
- * and options, for every slab_tracks >= 1; slab_tracks >= N is that call's launch sequence and workspace.
- *   workspace : ct3_workspace_bytes_slabbed(T, T_pyr, N, G, H4, W4, slab_tracks) bytes, non-decreasing in slab_tracks;
- *               equal to ct3_workspace_bytes_frames for slab_tracks >= N
- * slab_tracks < 1, (N + 64*G)*T > 2^21 token rows (the supported size: every element offset of a full-size buffer then
- * stays below 2^31) and every invalid argument of ct3_update_loop_frames return CT3_EINVAL before anything is
- * enqueued; a workspace smaller than the query returns CT3_ENOSPC. */
-int ct3_workspace_bytes_slabbed(int T, int T_pyr, int N, int G, int H4, int W4, int slab_tracks, size_t* out_bytes);
-int ct3_update_loop_slabbed(const void* packed, const float* pyr, int T_pyr, int H4, int W4, const float* support,
-                            const uint8_t* track_valid, float* coords, float* vis, float* conf,
-                            const float* time_emb, int T, int N, int iters, void* workspace,
-                            size_t workspace_bytes, ct3_stream_t stream, const int32_t* group_sizes_host, int G,
-                            const int32_t* group_frames_host, int slab_tracks);
+ * multiplies coords by the stride and applies sigmoid, cotracker3_offline.py:213-216).
+ * Every field of the shape is validated: a null pointer or shape, T or N < 1, G outside [1, N], a group size < 1, sizes
+ * not summing to N, a null group_sizes with G > 1, T_pyr < 0, a frame map without T_pyr >= 1 or T_pyr >= 1 without
+ * one, a frame index outside [0, T_pyr), slab_tracks < 0, more than 2^21 token rows with slabs, iters < 0, a bad
+ * pyramid shape or a misaligned workspace return CT3_EINVAL, and a workspace smaller than the query CT3_ENOSPC, before
+ * anything is enqueued. */
+int ct3_update_loop(const void* packed, const float* pyr, const float* support, const uint8_t* track_valid,
+                    float* coords, float* vis, float* conf, const float* time_emb, int iters,
+                    const ct3_loop_shape* shape, void* workspace, size_t workspace_bytes, ct3_stream_t stream);
 
 /* ---- live profiler (bench.py roofline): CUDA events around every launch of the library, summed per
  * kernel category: 0 corr_sample, 1 gemm (wgmma), 2 attention, 3 layernorm, 4 misc.
@@ -378,8 +359,8 @@ int ct3_corr_sample(const float* pyr, int H4, int W4, const float* support,
  *                device column order (DESIGN.md: correlation embeddings 0..1023, vis 1024, conf 1025, posenc
  *                1026..1109, zero 1110..1151), WITHOUT the time embedding
  *   tokens_out : the point tokens fp32 [N*T, 384], row n*T + t
- * workspace: ct3_workspace_bytes(T, N, H4, W4) bytes, 256-byte aligned.  Invalid arguments return CT3_EINVAL and a too
- * small workspace CT3_ENOSPC, with ct3_update_loop's checks and messages, before any launch. */
+ * workspace: ct3_workspace_bytes of the shape {T, N, H4, W4, G = 1} bytes, 256-byte aligned.  Invalid arguments return
+ * CT3_EINVAL and a too small workspace CT3_ENOSPC, with ct3_update_loop's checks and messages, before any launch. */
 int ct3_loop_tokens(const void* packed, const float* pyr, int H4, int W4, const float* support,
                     const uint8_t* track_valid, const float* coords, const float* vis, const float* conf,
                     const float* time_emb, int T, int N, void* vol_out, void* x_out, float* tokens_out,
@@ -443,16 +424,13 @@ int ct3_split_rows_fp16(const float* x, int rows, int K, int Kpad, void* x_split
 
 /* One EfficientUpdateFormer forward (cotracker.py:483-531) on an explicit token
  * input x [N, T, 1110] fp32 (time embedding already added, reference column order);
- * delta out [N, T, 4] fp32. */
-int ct3_updateformer(const void* packed, const float* x, int T, int N, float* delta, void* workspace,
-                     size_t workspace_bytes, ct3_stream_t stream);
-/* The same over G track groups (see ct3_update_loop_groups): N = sum of group_sizes_host; workspace:
- * ct3_workspace_bytes_groups(T, N, G, 0, 0). */
-int ct3_updateformer_groups(const void* packed, const float* x, int T, const int32_t* group_sizes_host, int G,
-                            float* delta, void* workspace, size_t workspace_bytes, ct3_stream_t stream);
+ * delta out [N, T, 4] fp32.  The tracks form G groups as in ct3_loop_shape; a NULL group_sizes_host means G = 1;
+ * workspace: ct3_workspace_bytes of the shape {T, N, 0, 0, G}.  Checks and messages as ct3_update_loop. */
+int ct3_updateformer(const void* packed, const float* x, int T, int N, const int32_t* group_sizes_host, int G,
+                     float* delta, void* workspace, size_t workspace_bytes, ct3_stream_t stream);
 
 /* One attention core  out = softmax(q k^T * 48^-1/2) v  per head (8 x 48; Attention.forward, blocks.py:391-397) of
- * the transformer body, chosen and launched exactly as ct3_updateformer_groups does it under the calling thread's
+ * the transformer body, chosen and launched exactly as ct3_updateformer does it under the calling thread's
  * "attn" option (time attention always takes the unfused path that T > 128 takes in the body).
  * Every buffer holds the body's (N + 64*G)*T token rows: point n at row n*T + t, virtual token i of group g at row
  * (N + 64*g + i)*T + t.
@@ -466,7 +444,7 @@ int ct3_updateformer_groups(const void* packed, const float* x, int T, const int
  *   q, kv          : fp32 device buffers (may alias), 16-byte aligned; only the rows the kind reads are read
  *   out_split      : bf16 [rows, 768] (hi cols 0..383 | lo cols 384..767); the query rows of the kind are written,
  *                    no other row
- *   group_sizes_host, G : as ct3_updateformer_groups (sum = N)
+ *   group_sizes_host, G : the track groups of ct3_loop_shape, sum = N, not NULL
  *   workspace      : ct3_attention_workspace_bytes(T, N, G) bytes, 256-byte aligned (split-K partials, group table)
  * Null pointers, an unknown kind, bad T/N/groups, misalignment return CT3_EINVAL and a too small workspace
  * CT3_ENOSPC, before any launch. */

@@ -1,4 +1,4 @@
-"""Capacity of the offline update loop in track slabs (ct3_update_loop_slabbed, DESIGN.md §4.4.5).
+"""Capacity of the offline update loop in track slabs (ct3_loop_shape.slab_tracks, DESIGN.md §4.4.5).
 
     python scripts/capacity_bench.py [--reps 3] [--frames 16 48 120] [--long 300] [--out DIR]
 

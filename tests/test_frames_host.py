@@ -1,6 +1,6 @@
-"""CPU tests of frame maps (ct3_update_loop_frames): exported symbols, argument validation before any launch, the host
-frame-map builders of both models against a brute-force restatement of the padded / reversed clip, the window gather,
-and the dense-mode pass planner."""
+"""CPU tests of frame maps (ct3_loop_shape.T_pyr, group_frames): exported symbols, argument validation before any
+launch, the host frame-map builders of both models against a brute-force restatement of the padded / reversed clip,
+the window gather, and the dense-mode pass planner."""
 import ctypes
 
 import numpy as np
@@ -12,35 +12,46 @@ from cotracker_b200.build import build_cotracker
 from cotracker_b200.evaluation import pass_bytes, plan_dense_passes, plan_passes
 from cotracker_b200.model import clip_frame_map, gather_plan, gather_pyramid, window_frame_map
 
-FRAME_SYMBOLS = ("ct3_workspace_bytes_frames", "ct3_update_loop_frames")
+FRAME_SYMBOLS = ("ct3_workspace_bytes", "ct3_update_loop")
 
 
 def _i32(*v):
     return (ctypes.c_int32 * max(1, len(v)))(*v)
 
 
-def test_frame_symbols_exported():
+def test_frame_map_is_a_loop_shape_field():
+    """A frame map is a field of the loop shape: the size and loop entry points take it."""
     lib = engine.lib()
     for name in FRAME_SYMBOLS:
         assert hasattr(lib, name) and name in engine.EXPORTED_SYMBOLS, name
 
 
-def test_workspace_bytes_frames():
-    lib = engine.lib()
+def _ws(T, T_pyr, N, G, H4, W4, frames=None):
     n = ctypes.c_size_t(0)
-    assert lib.ct3_workspace_bytes_frames(16, 32, 500, 2, 96, 128, ctypes.byref(n)) == 0
-    assert n.value == engine.workspace_bytes(16, 500, 96, 128, groups=2, frames=32)
+    shape = engine._loop_shape(T, N, H4, W4, G, None, T_pyr, frames)
+    return engine.lib().ct3_workspace_bytes(ctypes.byref(shape), ctypes.byref(n)), n.value
+
+
+def test_workspace_bytes_with_frame_map():
+    lib = engine.lib()
+    rc, n = _ws(16, 32, 500, 2, 96, 128)
+    assert rc == 0 and n == engine.workspace_bytes(16, 500, 96, 128, groups=2, frames=32)
     same = engine.workspace_bytes(16, 500, 96, 128, groups=2, frames=16)
     assert same >= engine.workspace_bytes(16, 500, 96, 128, groups=2)             # + the [G, T] frame map
     *_, per_frame = engine.pyramid_layout(1, 96, 128)
-    assert n.value - same >= 16 * per_frame * 4 - 4096                            # split pyramid copy sized by T_pyr
-    assert lib.ct3_workspace_bytes_frames(16, 0, 500, 2, 96, 128, ctypes.byref(n)) == -1     # T_pyr < 1
-    assert lib.ct3_workspace_bytes_frames(16, 16, 500, 0, 96, 128, ctypes.byref(n)) == -1    # G < 1
+    assert n - same >= 16 * per_frame * 4 - 4096                                  # split pyramid copy sized by T_pyr
+    assert _ws(16, -1, 500, 2, 96, 128)[0] == -1 and b"T_pyr" in lib.ct3_last_error()     # T_pyr < 0
+    assert _ws(16, 16, 500, 0, 96, 128)[0] == -1                                          # G < 1
     with pytest.raises(engine.EngineError):
         engine.workspace_bytes(4, 10, 24, 32, frames=-1)
+    # the size needs no map; one that is given is checked and changes nothing
+    good = _i32(*(list(range(16)) + list(range(31, 15, -1))))
+    assert _ws(16, 32, 500, 2, 96, 128, good) == (0, n)
+    assert _ws(16, 0, 500, 2, 96, 128, good)[0] == -1 and b"T_pyr" in lib.ct3_last_error()   # a map needs T_pyr
+    assert _ws(16, 31, 500, 2, 96, 128, good)[0] == -1 and b"outside" in lib.ct3_last_error()
 
 
-def test_update_loop_frames_rejects_bad_arguments_without_gpu():
+def test_update_loop_rejects_bad_frame_maps_without_gpu():
     """Every invalid frame-map argument returns CT3_EINVAL before anything is enqueued (all pointers are fake and the
     stream is the legacy default: reaching a launch would fail differently)."""
     lib = engine.lib()
@@ -49,8 +60,9 @@ def test_update_loop_frames_rejects_bad_arguments_without_gpu():
     T = 4
 
     def loop(frames, T_pyr=8, sizes=_i32(5, 5), G=2, N=10):
-        return lib.ct3_update_loop_frames(fake, fake, T_pyr, 24, 32, fake, None, fake, fake, fake, fake, T, N, 1, ws,
-                                          1 << 40, None, sizes, G, frames)
+        shape = engine._loop_shape(T, N, 24, 32, G, sizes, T_pyr, frames)
+        return lib.ct3_update_loop(fake, fake, fake, None, fake, fake, fake, fake, 1, ctypes.byref(shape), ws, 1 << 40,
+                                   None)
 
     good = _i32(*([0, 1, 2, 3] + [7, 6, 5, 4]))
     cases = [
@@ -59,8 +71,9 @@ def test_update_loop_frames_rejects_bad_arguments_without_gpu():
         (_i32(0, 1, 2, 8, 7, 6, 5, 4), 8, _i32(5, 5), 2, b"outside"),      # index == T_pyr
         (_i32(0, 1, 2, 3, 7, 6, -1, 4), 8, _i32(5, 5), 2, b"outside"),     # negative index
         (_i32(0, 1, 2, 3), 3, _i32(10), 1, b"outside"),                    # index >= a smaller T_pyr
-        (good, 0, _i32(5, 5), 2, b"T_pyr"),                                # T_pyr < 1
-        (good, -5, _i32(5, 5), 2, b"T_pyr"),
+        (good, 0, _i32(5, 5), 2, b"T_pyr"),                                # a map with T_pyr = 0
+        (good, -5, _i32(5, 5), 2, b"T_pyr"),                               # T_pyr < 0
+        (None, -5, _i32(5, 5), 2, b"T_pyr"),
         (good, 8, _i32(4, 5), 2, b"sum to N"),                             # the group checks still apply
     ]
     for frames, T_pyr, sizes, G, msg in cases:
@@ -115,7 +128,7 @@ def test_window_frame_map_matches_padded_flipped_clip(T, S):
 
 
 def test_gather_pyramid_copies_the_referenced_frames():
-    """gather_pyramid (slice_pyramid + concat_pyramid_frames) on a host pyramid whose every value is its frame id."""
+    """gather_pyramid (concat_pyramid_runs) on a host pyramid whose every value is its frame id."""
     T, H4, W4 = 24, 16, 20
     off, h, w, total = engine.pyramid_layout(T, H4, W4)
     pyr = torch.empty(total)

@@ -1,6 +1,6 @@
-"""Frame maps on the GPU (ct3_update_loop_frames, forward_groups(reversed_groups=), the predictors' grouped backward
-tracking and dense passes).  Every group must be bit-identical to a standalone call on a pyramid holding exactly the
-frames its map names, and the predictors bit-identical to their previous one-pass-at-a-time sequence."""
+"""Frame maps on the GPU (ct3_loop_shape.group_frames, forward_groups(reversed_groups=), the predictors' grouped
+backward tracking and dense passes).  Every group must be bit-identical to a standalone call on a pyramid holding
+exactly the frames its map names, and the predictors bit-identical to their previous one-pass-at-a-time sequence."""
 import numpy as np
 import pytest
 import torch

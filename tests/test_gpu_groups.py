@@ -1,6 +1,6 @@
-"""Grouped calls on the GPU: G independent query sets over one clip in one pass (ct3_update_loop_groups,
-ct3_updateformer_groups, forward_groups, single-point EvaluationPredictor).  Each group's outputs must be bit-identical
-to a standalone call on that group's tracks alone."""
+"""Grouped calls on the GPU: G independent query sets over one clip in one pass (ct3_loop_shape.G,
+ct3_updateformer's groups, forward_groups, single-point EvaluationPredictor).  Each group's outputs must be
+bit-identical to a standalone call on that group's tracks alone."""
 import numpy as np
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""Track slabs on the GPU (ct3_update_loop_slabbed, DESIGN.md §4.4.5): coords / vis / conf bit-identical to the call
+"""Track slabs on the GPU (ct3_loop_shape.slab_tracks, DESIGN.md §4.4.5): coords / vis / conf bit-identical to the call
 without slabs for every slab size, call kind, both time-attention routes and the A/B options; nothing outside the
 queried workspace is written; the offline predictor under a budget that forces slabs returns what it returns without."""
 import pytest
@@ -107,7 +107,7 @@ def test_slabbed_bit_identical_under_options(eng, sd, opt):
 
 @pytest.mark.parametrize("slab", [1, 64])
 def test_slabbed_writes_only_its_workspace(eng, sd, slab):
-    """The pyramid and support are read-only and no byte past ct3_workspace_bytes_slabbed(...) changes."""
+    """The pyramid and support are read-only and no byte past ct3_workspace_bytes(shape) changes."""
     T, H4, W4 = 20, 64, 72
     packed = eng.pack_weights(sd, DEV)
     inp = _inputs(eng, sd, T, H4, W4, seed=4)

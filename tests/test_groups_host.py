@@ -1,4 +1,4 @@
-"""CPU tests of grouped calls (ct3_update_loop_groups / ct3_updateformer_groups): exported symbols, argument
+"""CPU tests of grouped calls (ct3_loop_shape.G / ct3_updateformer's group sizes): exported symbols, argument
 validation before any launch, and the single-point evaluation pass planner."""
 import ctypes
 
@@ -7,34 +7,43 @@ import pytest
 from cotracker_b200 import engine
 from cotracker_b200.evaluation import pass_bytes, plan_passes
 
-GROUP_SYMBOLS = ("ct3_workspace_bytes_groups", "ct3_update_loop_groups", "ct3_updateformer_groups")
+GROUP_SYMBOLS = ("ct3_workspace_bytes", "ct3_update_loop", "ct3_updateformer")
 
 
 def _sizes(*v):
     return (ctypes.c_int32 * max(1, len(v)))(*v)
 
 
-def test_group_symbols_exported():
+def test_groups_are_a_loop_shape_field():
+    """Groups are a field of the loop shape: one entry point each for the size, the loop and the updateformer."""
     lib = engine.lib()
     for name in GROUP_SYMBOLS:
         assert hasattr(lib, name) and name in engine.EXPORTED_SYMBOLS, name
 
 
-def test_workspace_bytes_groups():
-    lib = engine.lib()
+def _ws(T, N, G, H4, W4, sizes=None):
     n = ctypes.c_size_t(0)
-    assert lib.ct3_workspace_bytes_groups(16, 500, 1, 96, 128, ctypes.byref(n)) == 0
-    assert n.value == engine.workspace_bytes(16, 500, 96, 128)          # G = 1 is the plain call
+    rc = engine.lib().ct3_workspace_bytes(ctypes.byref(engine._loop_shape(T, N, H4, W4, G, sizes)), ctypes.byref(n))
+    return rc, n.value
+
+
+def test_workspace_bytes_with_groups():
+    lib = engine.lib()
+    assert _ws(16, 500, 1, 96, 128) == (0, engine.workspace_bytes(16, 500, 96, 128))   # G = 1 is the plain call
     one = engine.workspace_bytes(16, 500, 96, 128, groups=1)
     five = engine.workspace_bytes(16, 500, 96, 128, groups=5)
     assert five > one + 4 * 64 * 16 * 384 * 4                           # 64 virtual token rows per frame per group
-    assert lib.ct3_workspace_bytes_groups(16, 500, 0, 0, 0, ctypes.byref(n)) == -1       # G < 1
-    assert lib.ct3_workspace_bytes_groups(16, 3, 4, 0, 0, ctypes.byref(n)) == -1         # more groups than tracks
+    assert _ws(16, 500, 0, 0, 0)[0] == -1                               # G < 1
+    assert _ws(16, 3, 4, 0, 0)[0] == -1                                 # more groups than tracks
     with pytest.raises(engine.EngineError):
         engine.workspace_bytes(4, 10, groups=0)
+    # the size needs no sizes array; one that is given is checked and changes nothing
+    assert _ws(16, 500, 2, 96, 128, _sizes(100, 400)) == _ws(16, 500, 2, 96, 128)
+    assert _ws(16, 500, 2, 96, 128, _sizes(100, 399))[0] == -1 and b"sum to N" in lib.ct3_last_error()
+    assert _ws(16, 500, 2, 96, 128, _sizes(500, 0))[0] == -1 and b"size must be" in lib.ct3_last_error()
 
 
-def test_grouped_calls_reject_bad_groups_without_gpu():
+def test_loop_and_updateformer_reject_bad_groups_without_gpu():
     """Every invalid group argument returns CT3_EINVAL before anything is enqueued (all pointers are fake and the
     stream is the legacy default: reaching a launch would fail differently)."""
     lib = engine.lib()
@@ -42,11 +51,12 @@ def test_grouped_calls_reject_bad_groups_without_gpu():
     ws = ctypes.c_void_p(1 << 24)
 
     def loop(sizes, G, N=10):
-        return lib.ct3_update_loop_groups(fake, fake, 24, 32, fake, None, fake, fake, fake, fake, 4, N, 1, ws, 1 << 40,
-                                          None, sizes, G)
+        shape = engine._loop_shape(4, N, 24, 32, G, sizes)
+        return lib.ct3_update_loop(fake, fake, fake, None, fake, fake, fake, fake, 1, ctypes.byref(shape), ws, 1 << 40,
+                                   None)
 
-    def former(sizes, G):
-        return lib.ct3_updateformer_groups(fake, fake, 4, sizes, G, fake, ws, 1 << 40, None)
+    def former(sizes, G, N=10):
+        return lib.ct3_updateformer(fake, fake, 4, N, sizes, G, fake, ws, 1 << 40, None)
 
     cases = [
         (None, 2, b"null group"),             # null group array
@@ -60,9 +70,10 @@ def test_grouped_calls_reject_bad_groups_without_gpu():
     for sizes, G, msg in cases:
         assert loop(sizes, G) == -1, (G, msg)
         assert msg in lib.ct3_last_error(), (lib.ct3_last_error(), msg)
-    for sizes, G, msg in cases[:5]:
+    for sizes, G, msg in cases:
         assert former(sizes, G) == -1, (G, msg)
         assert msg in lib.ct3_last_error()
+    assert former(_sizes(5, 5), 2, N=0) == -1 and b"T and N" in lib.ct3_last_error()
     # the Python wrappers raise EngineError for the same arguments
     with pytest.raises(engine.EngineError):
         engine._group_array(["x"])

@@ -24,28 +24,35 @@ def test_library_exports_every_declared_symbol():
     assert lib.ct3_version() >= 100
 
 
-def test_abi_argument_validation_without_gpu():
+def test_abi_argument_validation_with_loop_shapes_without_gpu():
     from cotracker_b200 import engine
     lib = engine.lib()
     n = ctypes.c_size_t(0)
-    assert lib.ct3_workspace_bytes(16, 6400, 96, 128, ctypes.byref(n)) == 0 and n.value > 6e9
-    assert lib.ct3_workspace_bytes(0, 10, 0, 0, ctypes.byref(n)) == -1          # CT3_EINVAL
+
+    def ws(shape, out=ctypes.byref(n)):
+        return lib.ct3_workspace_bytes(None if shape is None else ctypes.byref(shape), out)
+
+    assert ws(engine._loop_shape(16, 6400, 96, 128)) == 0 and n.value > 6e9
+    assert ws(engine._loop_shape(0, 10, 0, 0)) == -1                           # CT3_EINVAL
     assert b"T and N" in lib.ct3_last_error()
-    assert lib.ct3_workspace_bytes(4, 4, 0, 0, None) == -1
+    assert ws(engine._loop_shape(4, 4, 0, 0), None) == -1
+    assert ws(None) == -1 and b"null shape" in lib.ct3_last_error()
     off, h, w, total = engine.pyramid_layout(16, 96, 128)
     assert h == [96, 48, 24, 12] and w == [128, 64, 32, 16] and total == 16 * 16320 * 128
     with pytest.raises(engine.EngineError):
         engine.pyramid_layout(2, 4, 4)                                      # level 3 would be 0x0
     assert lib.ct3_set_option(b"nope", 1) == -1
     assert engine.get_option("gemm") == 0
-    assert lib.ct3_update_loop(None, None, 1, 1, None, None, None, None, None, None, 1, 1, 1, None, 0, None) == -1
+    assert lib.ct3_update_loop(None, None, None, None, None, None, None, None, 1, None, None, 0, None) == -1
+    one = ctypes.c_void_p(256)
+    assert lib.ct3_update_loop(one, one, one, None, one, one, one, one, 1, None, one, 1 << 40, None) == -1
+    assert b"null shape" in lib.ct3_last_error()
     # the split-bf16 pyramid copy of the correlation kernel is part of the workspace iff every level is >= 8x8 texels
     *_, total = engine.pyramid_layout(16, 96, 128)
     assert engine.workspace_bytes(16, 6400, 96, 128) - engine.workspace_bytes(16, 6400) == total * 4
     assert engine.workspace_bytes(4, 10, 24, 32) == engine.workspace_bytes(4, 10)       # level 3 is 3x4
-    assert lib.ct3_workspace_bytes(4, 10, 4, 4, ctypes.byref(n)) == -1                    # level 3 would be 0x0
+    assert ws(engine._loop_shape(4, 10, 4, 4)) == -1                                     # level 3 would be 0x0
     # stage entry: argument checks come before any launch
-    one = ctypes.c_void_p(256)
     assert lib.ct3_corr_sample(None, 96, 128, one, None, one, 2, 5, one, None, 0, None) == -1
     assert lib.ct3_corr_sample(one, 96, 128, one, None, one, 2, 5, one, ctypes.c_void_p(264), 1 << 30, None) == -1
     assert b"256-byte aligned" in lib.ct3_last_error()
@@ -84,7 +91,7 @@ def test_attention_stage_argument_validation_without_gpu():
     assert call(nbytes=need - 1) == -3                                                   # CT3_ENOSPC
 
 
-def test_loop_tokens_argument_validation_without_gpu():
+def test_loop_tokens_and_update_loop_argument_validation_without_gpu():
     """ct3_loop_tokens rejects bad arguments with update_loop's checks and messages (CT3_EINVAL / CT3_ENOSPC) before
     any launch (the pointers below are never dereferenced)."""
     from cotracker_b200 import engine
@@ -107,7 +114,8 @@ def test_loop_tokens_argument_validation_without_gpu():
     assert call(w=ctypes.c_void_p((1 << 21) + 16)) == -1 and b"256-byte" in lib.ct3_last_error()
     assert call(nbytes=need - 1) == -3 and b"workspace too small" in lib.ct3_last_error()   # CT3_ENOSPC
     # the same messages as ct3_update_loop for the same faults
-    assert lib.ct3_update_loop(p, p, H4, W4, p, None, p, p, p, p, T, N, 1, ws, need - 1, None) == -3
+    shape = engine._loop_shape(T, N, H4, W4)
+    assert lib.ct3_update_loop(p, p, p, None, p, p, p, p, 1, ctypes.byref(shape), ws, need - 1, None) == -3
     assert b"workspace too small" in lib.ct3_last_error()
 
 
