@@ -224,7 +224,8 @@ namespace {
 constexpr int kOnlineMaxInd = 1 << 30;   // ind + S and |query frame| stay below this: int32 arithmetic in the kernels
 
 // the checks both ct3_online_window_* share; end = window_end's extra conditions.  max_elems: the largest per-stream
-// element count of the kernel (S * n for begin, (ind + T) * n for end)
+// element count of the kernel (S * n for begin, (ind + T - first frame touched) * n for end).  A ring history (ring =
+// 1) holds frames [len - cap, len): every frame a kernel reads must lie there.
 int check_online(const ct3_online_stream* st, int K, int S, int step, int stride, int N, bool end, int64_t* max_elems,
                  const void* workspace, size_t workspace_bytes) {
   if (!st || !workspace) return fail(CT3_EINVAL, "null argument%s");
@@ -242,7 +243,11 @@ int check_online(const ct3_online_stream* st, int K, int S, int step, int stride
     next += s.n;
     if (s.T < 1 || s.T > S) return fail(CT3_EINVAL, "a stream's T must be in [1, S]%s");
     if (s.ind < 0 || (int64_t)s.ind + S > kOnlineMaxInd) return fail(CT3_EINVAL, "a stream's ind must be in [0, 2^30 - S]%s");
-    if (s.cap < s.len || s.len < 0) return fail(CT3_EINVAL, "a stream's history must have 0 <= len <= cap%s");
+    if (s.ring != 0 && s.ring != 1) return fail(CT3_EINVAL, "a stream's ring must be 0 or 1%s");
+    if (s.len < 0 || (!s.ring && s.cap < s.len))
+      return fail(CT3_EINVAL, "a stream's history must have 0 <= len <= cap%s");
+    if (s.ring && s.cap < S) return fail(CT3_EINVAL, "a ring history must hold at least S frames%s");
+    const int64_t held = s.ring ? s.len - s.cap : 0;   // the first frame the history still holds
     const bool reads = end || s.ind > 0;
     if (reads && (!s.coords || !s.vis || !s.conf)) return fail(CT3_EINVAL, "a stream's history is null%s");
     if (reads && ((uintptr_t)s.coords & 7)) return fail(CT3_EINVAL, "history coords must be 8-byte aligned%s");
@@ -250,13 +255,25 @@ int check_online(const ct3_online_stream* st, int K, int S, int step, int stride
     if (!end) {
       if (s.ind > 0 && s.len < (int64_t)s.ind + (S - step))
         return fail(CT3_EINVAL, "a stream's history must hold the window's overlap frames%s");
+      if (s.ind > 0 && s.ind < held) return fail(CT3_EINVAL, "the ring no longer holds the window's overlap frames%s");
     } else {
-      if (s.cap < (int64_t)s.ind + s.T) return fail(CT3_EINVAL, "a stream's history must hold ind + T frames%s");
+      const int64_t rows = (int64_t)s.ind + s.T;
+      if (!s.ring && s.cap < rows) return fail(CT3_EINVAL, "a stream's history must hold ind + T frames%s");
       if (s.len < s.ind) return fail(CT3_EINVAL, "a stream's history must hold the frames before its window%s");
-      if (s.tracks && (!s.visibility || s.n_keep < 1 || s.n_keep > s.n))
-        return fail(CT3_EINVAL, "a stream's output needs visibility and n_keep in [1, n]%s");
-      if (s.tracks && ((uintptr_t)s.tracks & 7)) return fail(CT3_EINVAL, "output tracks must be 8-byte aligned%s");
-      elems = ((int64_t)s.ind + s.T) * s.n;
+      int64_t lo = s.ind;   // the first frame the kernel touches
+      if (s.tracks) {
+        if (!s.visibility || s.n_keep < 1 || s.n_keep > s.n)
+          return fail(CT3_EINVAL, "a stream's output needs visibility and n_keep in [1, n]%s");
+        if ((uintptr_t)s.tracks & 7) return fail(CT3_EINVAL, "output tracks must be 8-byte aligned%s");
+        if (s.out_first < 0 || s.out_first >= rows)
+          return fail(CT3_EINVAL, "a stream's out_first must be in [0, ind + T)%s");
+        if (s.ring && rows - s.out_first > s.cap)
+          return fail(CT3_EINVAL, "a ring stream's output must fit in the ring (ind + T - out_first <= cap)%s");
+        if (s.out_first < s.ind && s.out_first < held)
+          return fail(CT3_EINVAL, "the ring no longer holds the output's frames before the window%s");
+        if (s.out_first < lo) lo = s.out_first;
+      }
+      elems = (rows - lo) * s.n;
     }
     if (elems > *max_elems) *max_elems = elems;
   }

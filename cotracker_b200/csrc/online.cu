@@ -5,6 +5,8 @@
 // (1 / (1 + expf(-x)), IEEE division, no fast-math), so the results are bit-identical to the ATen expressions they
 // replace (include/ct3_b200.h).  Division by the stride is a multiply by the fp32 reciprocal, as ATen evaluates a
 // division by a scalar.  Block (x, k) strides over the elements of stream k; the grid's y dimension is the stream.
+// A ring history (ring = 1) holds frame f at row f mod cap; the host checks guarantee that every frame a launch reads
+// is still held and that no row is both read and written by one window_end launch.
 #include "../../include/ct3_b200.h"
 #include "kernels.cuh"
 
@@ -13,6 +15,11 @@ namespace {
 
 constexpr int kOnlineThreads = 256;
 constexpr int kOnlineMaxBlocksX = 1024;
+
+// the history row of stream frame f
+__device__ __forceinline__ int64_t history_row(const ct3_online_stream& st, int64_t f) {
+  return st.ring ? f % st.cap : f;
+}
 
 __global__ void __launch_bounds__(kOnlineThreads) online_window_begin_kernel(
     const ct3_online_stream* __restrict__ streams, int S, int step, float inv_stride, const int32_t* __restrict__ qframes,
@@ -39,7 +46,7 @@ __global__ void __launch_bounds__(kOnlineThreads) online_window_begin_kernel(
     float2 c;
     float v = 0.f, q = 0.f;
     if (ind > 0 && qf < ind + overlap) {   // warm start: the previous window's overlap, its last frame repeated
-      const int64_t src = (int64_t)(ind + min(t, overlap - 1)) * n + j;
+      const int64_t src = history_row(st, ind + min(t, overlap - 1)) * n + j;
       const float2 h = hc[src];
       c = make_float2(__fmul_rn(h.x, inv_stride), __fmul_rn(h.y, inv_stride));
       v = hv[src];
@@ -66,12 +73,16 @@ __global__ void __launch_bounds__(kOnlineThreads) online_window_end_kernel(
   float* __restrict__ hq = st.conf;
   float2* __restrict__ tracks = reinterpret_cast<float2*>(st.tracks);
   uint8_t* __restrict__ visibility = st.visibility;
-  const int64_t total = ((int64_t)ind + st.T) * n;
+  // frames [lo, ind + T): the window's frames, and before them those of the output (frames before lo are not touched)
+  const int64_t out_first = st.out_first;
+  const int64_t lo = tracks != nullptr && out_first < ind ? out_first : ind;
+  const int64_t total = ((int64_t)ind + st.T - lo) * n;
   for (int64_t e = (int64_t)blockIdx.x * kOnlineThreads + threadIdx.x; e < total;
        e += (int64_t)gridDim.x * kOnlineThreads) {
-    const int64_t t = e / n;
+    const int64_t t = lo + e / n;
     const int j = (int)(e % n);
-    const bool out = tracks != nullptr && j < n_keep;
+    const bool out = tracks != nullptr && j < n_keep && t >= out_first;
+    const int64_t h = history_row(st, t) * n + j;
     float2 p;
     float v, q;
     if (t >= ind) {   // a frame of this window: the loop's result, written back (frames ind + T.. are padding)
@@ -80,18 +91,18 @@ __global__ void __launch_bounds__(kOnlineThreads) online_window_end_kernel(
       p = make_float2(__fmul_rn(c.x, stride), __fmul_rn(c.y, stride));
       v = __ldg(vis + src);
       q = __ldg(conf + src);
-      hc[e] = p;
-      hv[e] = v;
-      hq[e] = q;
+      hc[h] = p;
+      hv[h] = v;
+      hq[h] = q;
     } else if (out) {   // an earlier frame: the history as it stands
-      p = hc[e];
-      v = hv[e];
-      q = hq[e];
+      p = hc[h];
+      v = hv[h];
+      q = hq[h];
     } else {
       continue;
     }
     if (out) {
-      const int64_t o = t * n_keep + j;
+      const int64_t o = (t - out_first) * n_keep + j;
       tracks[o] = make_float2(__fmul_rn(p.x, st.scale_x), __fmul_rn(p.y, st.scale_y));
       visibility[o] = __fmul_rn(sigmoid_aten(v), sigmoid_aten(q)) > threshold ? 1 : 0;
     }

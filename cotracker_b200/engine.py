@@ -31,7 +31,8 @@ class OnlineStream(ctypes.Structure):
                 ("cap", ctypes.c_int64), ("len", ctypes.c_int64), ("tracks", ctypes.c_void_p),
                 ("visibility", ctypes.c_void_p), ("ind", ctypes.c_int32), ("T", ctypes.c_int32), ("n", ctypes.c_int32),
                 ("first", ctypes.c_int32), ("frame0", ctypes.c_int32), ("n_keep", ctypes.c_int32),
-                ("scale_x", ctypes.c_float), ("scale_y", ctypes.c_float)]
+                ("scale_x", ctypes.c_float), ("scale_y", ctypes.c_float), ("out_first", ctypes.c_int64),
+                ("ring", ctypes.c_int32), ("pad", ctypes.c_int32)]
 
 
 class LoopShape(ctypes.Structure):
@@ -305,14 +306,16 @@ def finish_tracks(fwd, bwd, queries: torch.Tensor, n_keep: int, threshold: float
 
 
 QUERY_FRAME_LIMIT = 1 << 30   # ct3_online_window_begin compares query frames clamped to +-2^30
+STREAM_FRAME_LIMIT = 1 << 30  # ct3_online_window_* take a window at stream frame ind only while ind + S <= 2^30
 
 
 def online_stream(hist, length: int, ind: int, T: int, first: int, frame0: int, out=None, n_keep: int = 0,
-                  scale_xy=(1.0, 1.0)) -> OnlineStream:
+                  scale_xy=(1.0, 1.0), *, out_first: int = 0, ring: bool = False) -> OnlineStream:
     """One entry of a streaming window pass (ct3_online_stream): hist = (coords [cap,n,2], vis [cap,n], conf [cap,n])
-    fp32 histories with `length` valid frames, the window at stream frame `ind` with T real frames, the stream's tracks
-    from `first` in the pass and its window at pyramid frame `frame0`; out = (tracks [ind+T,n_keep,2] fp32,
-    visibility [ind+T,n_keep] bool or uint8) for window_end's predictor output, or None."""
+    fp32 histories with `length` frames written, the window at stream frame `ind` with T real frames, the stream's
+    tracks from `first` in the pass and its window at pyramid frame `frame0`; out = (tracks [ind+T-out_first,n_keep,2]
+    fp32, visibility [ind+T-out_first,n_keep] bool or uint8) for window_end's predictor output of stream frames
+    [out_first, ind+T), or None.  ring: the history holds frame f at row f mod cap (its last cap frames only)."""
     c, v, q = hist
     for t, dtype, name in ((c, torch.float32, "history coords"), (v, torch.float32, "history vis"),
                            (q, torch.float32, "history conf")):
@@ -322,13 +325,13 @@ def online_stream(hist, length: int, ind: int, T: int, first: int, frame0: int, 
         raise EngineError(f"histories must be [cap,n,2], [cap,n], [cap,n], got {tuple(c.shape)}, {tuple(v.shape)}, "
                           f"{tuple(q.shape)}")
     e = OnlineStream(c.data_ptr(), v.data_ptr(), q.data_ptr(), cap, int(length), None, None, int(ind), int(T), n,
-                     int(first), int(frame0), 0, float(scale_xy[0]), float(scale_xy[1]))
+                     int(first), int(frame0), 0, float(scale_xy[0]), float(scale_xy[1]), int(out_first), int(bool(ring)))
     if out is not None:
         tr, vi = out
         _req(tr, torch.float32, "tracks")
         if not vi.is_cuda or vi.dtype not in (torch.bool, torch.uint8) or not vi.is_contiguous():
             raise EngineError("visibility must be a contiguous CUDA bool or uint8 tensor")
-        rows = int(ind) + int(T)
+        rows = int(ind) + int(T) - int(out_first)
         if tuple(tr.shape) != (rows, int(n_keep), 2) or tuple(vi.shape) != (rows, int(n_keep)):
             raise EngineError(f"output must be [{rows},{n_keep},2] and [{rows},{n_keep}], got {tuple(tr.shape)} and "
                               f"{tuple(vi.shape)}")

@@ -151,18 +151,29 @@ def _reversed_flags(reversed_groups, G: int) -> List[bool]:
 # streaming: streams that each hold their own window start (CoTrackerThreeOnline._stream_step)
 class StreamState:
     """One stream of the streaming model: its window start, the history of its tracks and the encoder features of its
-    last chunk's overlap frames.  Its tracks are rows [first, first + n) of the `StreamPool` it belongs to."""
+    last chunk's overlap frames.  Its tracks are rows [first, first + n) of the `StreamPool` it belongs to.
 
-    def __init__(self, n: int, first: int):
+    history=None keeps every frame (frame f at row f).  A bound h keeps the history in a ring that holds frame f at row
+    f mod cap and only the last cap frames; the stream's results then cover its last h frames at most, and its memory
+    does not grow with its length."""
+
+    def __init__(self, n: int, first: int, history: Optional[int] = None):
         self.n, self.first = n, first
+        self.history = history    # None, or the bound on the frames of each result
         self.ind = 0              # window start (the reference's online_ind)
-        self.length = 0           # frames of history
+        self.length = 0           # frames of history (written so far; a ring holds the last cap of them)
         self.hist = None          # (coords * stride [cap,n,2], vis [cap,n], conf [cap,n] logits); frames >= length unset
         self.enc = None           # (signatures [S-step,2], frame shape, pyramid) of the last chunk's overlap frames
 
+    def ring_frames(self, S: int, step: int) -> int:
+        """The ring of a bounded state, in frames.  A window at ind reads frames [ind + T - L, ind) for a result of
+        L <= h frames (T >= 1 real frames) when the history holds frames up to ind + S - step, so h + S - step frames
+        always suffice; the library takes S at least."""
+        return max(S, self.history + S - step)
+
     def reserve(self, frames: int, device):
         """Room for `frames` history frames: the buffers at least double when they grow, so a stream reallocates
-        O(log length) times."""
+        O(log length) times.  A bounded state calls this once, with its `ring_frames`."""
         cap = 0 if self.hist is None else self.hist[1].shape[0]
         if frames <= cap:
             return
@@ -184,9 +195,9 @@ class StreamPool:
         self.streams: List[StreamState] = []
         self.support = self.qframes = self.qcoords = None
 
-    def open(self, qframes: torch.Tensor, qcoords: torch.Tensor) -> StreamState:
+    def open(self, qframes: torch.Tensor, qcoords: torch.Tensor, history: Optional[int] = None) -> StreamState:
         n = qframes.shape[0]
-        state = StreamState(n, 0 if self.qframes is None else self.qframes.shape[0])
+        state = StreamState(n, 0 if self.qframes is None else self.qframes.shape[0], history)
         sup = torch.zeros(4, 49, n, 128, device=qframes.device)
         if self.support is None:
             self.support, self.qframes, self.qcoords = sup, qframes.contiguous(), qcoords.contiguous()
@@ -501,15 +512,18 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
             return f"a chunk must hold 1 to window_len = {S} frames, got {T}"
         if state.ind > 0 and (state.length != state.ind + S - step or state.length + min(step, T - step) != state.ind + T):
             return "the stream has ended: its last chunk was shorter than the window"
+        if state.ind + S > engine.STREAM_FRAME_LIMIT:   # the library's window start limit, checked before any work
+            return "the stream has reached the frame limit: a window must end by frame 2^30"
         return None
 
     def _stream_step(self, pool: "StreamPool", streams, frames, Ts, iters, chunk=200, outputs=None):
         """Advance each of `streams` (states of `pool`, in pool order) by one window, in as few update-loop passes as
         fit in device memory.  frames [K*S,3,H,W] in [-1,1]: stream k's chunk of Ts[k] frames, padded to S frames with
-        copies of its last frame.  outputs: per stream None, or (n_keep, scale_xy) for the online predictor's output.
-        -> per stream None or (tracks [ind+T,n_keep,2] fp32, visibility [ind+T,n_keep] bool) of all its frames so far.
-        Every stream's result is bit-identical to advancing it alone: streams are independent query groups, each reading
-        its own S frames of one pyramid."""
+        copies of its last frame.  outputs: per stream None, or (n_keep, scale_xy) for the online predictor's output
+        of all its frames so far, or (n_keep, scale_xy, L) for that of its last L frames only (L <= ind + T; a bounded
+        state's results need L <= its bound).  -> per stream None or (tracks [L,n_keep,2] fp32, visibility [L,n_keep]
+        bool), L = ind + T without a bound.  Every stream's result is bit-identical to advancing it alone: streams are
+        independent query groups, each reading its own S frames of one pyramid."""
         K = len(streams)
         S = self.window_len
         step = S // 2
@@ -524,7 +538,7 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
         pyr = self._encode_online(frames, chunk, step, H4, W4, streams)
         T_pyr = K * S
         for s, T in zip(streams, Ts):
-            s.reserve(s.ind + T, dev)
+            s.reserve(s.ind + T if s.history is None else s.ring_frames(S, step), dev)
         passes = [(0, K)]
         if K > 1:
             budget = pass_budget_bytes(self, dev, T_pyr, H, W)
@@ -541,15 +555,16 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
                 qframes, qcoords = pool.qframes[idx], pool.qcoords[idx]
             entries, first = [], 0
             for k, s in enumerate(sub, b0):
-                out = None
+                out, n_keep, scale, out_first = None, 0, (1.0, 1.0), 0
                 if outputs[k] is not None:
-                    n_keep, scale = outputs[k]
-                    rows = s.ind + Ts[k]
+                    n_keep, scale = outputs[k][:2]
+                    rows = s.ind + Ts[k] if len(outputs[k]) < 3 else outputs[k][2]
+                    out_first = s.ind + Ts[k] - rows
                     out = (torch.empty(rows, n_keep, 2, device=dev), torch.empty(rows, n_keep, dtype=torch.bool,
                                                                                  device=dev))
                     results[k] = out
-                entries.append(engine.online_stream(s.hist, s.length, s.ind, Ts[k], first, k * S, out,
-                                                    *(outputs[k] or (0, (1.0, 1.0)))))
+                entries.append(engine.online_stream(s.hist, s.length, s.ind, Ts[k], first, k * S, out, n_keep, scale,
+                                                    out_first=out_first, ring=s.history is not None))
                 first += s.n
             valid, entering, rel, coords, vis, conf = engine.online_window_begin(entries, S, step, self.stride, T_pyr,
                                                                                  qframes, qcoords)

@@ -7,6 +7,7 @@
     hub.push(b, chunk_b)
     out = hub.step()                                # {stream id: (tracks [1,T_so_far,N,2], visibility [1,T_so_far,N])}
     hub.close(a)
+    c = hub.open(frame_size=(720, 1280), grid_size=10, history=64)   # bounded: results of the last 64 frames only
 
 Each stream has its own frame size, queries, start and pace.  `step()` advances every stream with a pushed chunk by one
 window: their chunks are resized into one frame batch, their new frames go through one encoder pass, and their tracks
@@ -14,10 +15,16 @@ run as query groups of one update loop (or of a few, when they do not fit in dev
 the results of the steps that advanced it are bit-identical to a fresh predictor on the same model called with
 `is_first_step=True` and the `open()` arguments, then with that stream's chunks in order and the same
 `add_support_grid`; whatever the other streams do.
+
+A stream opened with `history=h` runs in bounded memory: its history is a ring allocated once, each `step()` returns
+its last L = min(h, frames so far) frames only, and a step's work does not grow with the stream's length.  Its result
+is then exactly the last L frames of the unbounded result, `full[:, -L:]`; `length(sid)` gives the stream's frame
+count, so the result covers frames [length - L, length).  A stream can advance until a window would pass frame
+2^30 (about 414 days at 30 fps); `push()` reports that limit.
 """
 from __future__ import annotations
 
-from typing import Dict, Tuple
+from typing import Dict, Optional, Tuple
 
 import torch
 
@@ -36,9 +43,13 @@ class OnlineStreams:
 
     @torch.no_grad()
     def open(self, frame_size: Tuple[int, int], queries: torch.Tensor = None, grid_size: int = 5,
-             grid_query_frame: int = 0, add_support_grid: bool = False) -> int:
+             grid_query_frame: int = 0, add_support_grid: bool = False, history: Optional[int] = None) -> int:
         """Start a stream of frames of frame_size = (H, W): the arguments of the predictor's `is_first_step=True` call,
-        with the frame size in place of the first chunk.  -> the stream's id."""
+        with the frame size in place of the first chunk.  history: None keeps every frame and returns them all at each
+        step; an int h >= 1 keeps the stream in fixed memory and returns its last min(h, frames so far) frames.
+        -> the stream's id."""
+        if history is not None and (isinstance(history, bool) or not isinstance(history, int) or history < 1):
+            raise ValueError(f"history must be None or an int >= 1, got {history!r}")
         H, W = (int(x) for x in frame_size)
         if H < 2 or W < 2:
             raise ValueError(f"frame_size must be (H, W) with H, W >= 2, got {tuple(frame_size)}")
@@ -52,7 +63,7 @@ class OnlineStreams:
             raise ValueError("the predictor's model must be on a CUDA device")
         q, n_out = self.predictor._first_step_queries(1, (H, W), queries, grid_size, grid_query_frame,
                                                       add_support_grid, dev)
-        state = self.pool.open(*self.model._stream_queries(q[0]))
+        state = self.pool.open(*self.model._stream_queries(q[0]), history=history)
         sid = self._next_id
         self._next_id += 1
         n_keep = n_out if add_support_grid else q.shape[1]
@@ -64,6 +75,11 @@ class OnlineStreams:
         if sid not in self._streams:
             raise KeyError(f"no open stream {sid}")
         return self._streams[sid]
+
+    def length(self, sid: int) -> int:
+        """The frames stream `sid` has been advanced by so far: its last result covers frames [length - L, length),
+        with L the result's frame count."""
+        return self._get(sid)["state"].length
 
     def push(self, sid: int, chunk: torch.Tensor):
         """Queue the next chunk [1,T,3,H,W] of stream `sid` (T <= window_len) for the next `step()`."""
@@ -86,8 +102,11 @@ class OnlineStreams:
 
     @torch.no_grad()
     def step(self) -> Dict[int, Tuple[torch.Tensor, torch.Tensor]]:
-        """Advance every stream with a pushed chunk by one window, in one pass.  -> {id: (tracks [1,T_so_far,n,2] fp32,
-        visibility [1,T_so_far,n] bool)} of the streams it advanced; the others keep their state."""
+        """Advance every stream with a pushed chunk by one window, in one pass.  -> {id: (tracks [1,L,n,2] fp32,
+        visibility [1,L,n] bool)} of the streams it advanced, for their frames [length - L, length) with L = length
+        (frames so far), or min(h, length) for a stream opened with history=h; the others keep their state.
+        Frames before length - (window_len - step) (step = window_len // 2) are final: the next window re-tracks the
+        others."""
         order = {id(s): k for k, s in enumerate(self.pool.streams)}
         ids = sorted(self._pending, key=lambda i: order[id(self._streams[i]["state"])])
         if not ids:
@@ -105,6 +124,8 @@ class OnlineStreams:
                 frames[k * S + T:(k + 1) * S] = frames[k * S + T - 1]
             Ts.append(T)
         self._pending.clear()
-        outs = self.model._stream_step(self.pool, [self._streams[i]["state"] for i in ids], frames, Ts, 6,
-                                       outputs=[self._streams[i]["out"] for i in ids])
+        states = [self._streams[i]["state"] for i in ids]
+        outputs = [self._streams[i]["out"] if s.history is None else
+                   (*self._streams[i]["out"], min(s.history, s.ind + T)) for i, s, T in zip(ids, states, Ts)]
+        outs = self.model._stream_step(self.pool, states, frames, Ts, 6, outputs=outputs)
         return {sid: (tr[None], vi[None]) for sid, (tr, vi) in zip(ids, outs)}

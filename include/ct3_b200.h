@@ -133,20 +133,27 @@ int ct3_finish_tracks(const float* fwd_tracks, const float* fwd_vis, const float
  * [first, first + n) of the pass (streams follow each other: first_0 = 0, first_{k+1} = first_k + n_k, sum n_k = N),
  * its window starts at frame `ind` of the stream, its chunk has T real frames (window frames T..S-1 are padding) and
  * its window is pyramid frames [frame0, frame0 + S) of the pass.  Its history (coords * stride at model resolution,
- * visibility and confidence logits; frame t, track j at t * n + j) has `len` valid frames of `cap` allocated.
+ * visibility and confidence logits) has `len` frames written, `cap` frames allocated.  With ring = 0, frame f, track j
+ * is at row f (element f * n + j) and len <= cap.  With ring = 1 the history is a ring: frame f is at row f mod cap,
+ * len may exceed cap and only the last cap frames written, [len - cap, len), are held; a stream then runs in memory
+ * that does not grow with its length.  window_end's output covers stream frames [out_first, ind + T).
  * `streams_host` is a HOST array of K entries; the library copies it into `workspace` (at least
- * K * sizeof(ct3_online_stream) bytes, 16-byte aligned) on `stream`, so the host array may be reused on return. */
+ * K * sizeof(ct3_online_stream) bytes, 16-byte aligned) on `stream`, so the host array may be reused on return.
+ * An entry whose fields after scale_y are zero is a plain history with an output of every frame. */
 typedef struct {
   float* coords;          /* history [cap, n, 2] fp32                                                           */
   float* vis;             /* history [cap, n] fp32                                                              */
   float* conf;            /* history [cap, n] fp32                                                              */
   int64_t cap;            /* frames the history buffers hold                                                    */
-  int64_t len;            /* valid history frames before the window                                             */
-  float* tracks;          /* window_end: predictor output [ind + T, n_keep, 2] fp32, or NULL                     */
-  uint8_t* visibility;    /* window_end: predictor output [ind + T, n_keep] uint8 (0 | 1)                        */
+  int64_t len;            /* history frames written before the window                                           */
+  float* tracks;          /* window_end: predictor output [ind + T - out_first, n_keep, 2] fp32, or NULL         */
+  uint8_t* visibility;    /* window_end: predictor output [ind + T - out_first, n_keep] uint8 (0 | 1)            */
   int32_t ind, T, n, first, frame0;
   int32_t n_keep;         /* window_end: the first n_keep tracks are output (the trailing support grid is dropped) */
   float scale_x, scale_y; /* window_end: output tracks = history * (scale_x, scale_y), one fp32 multiply each     */
+  int64_t out_first;      /* window_end: the first stream frame of the output (0: every frame so far)           */
+  int32_t ring;           /* 0: frame f at history row f; 1: frame f at row f mod cap                          */
+  int32_t pad;            /* keeps the struct a multiple of 8 bytes; set to 0                                    */
 } ct3_online_stream;
 /* ct3_online_window_begin: the per-window state the update loop starts from, bit-identical to the torch expressions
  * (qf = qframes[i], the query frame in stream time; overlap = S - step):
@@ -158,20 +165,27 @@ typedef struct {
  * qframes [N] int32, qcoords [N,2] fp32 (feature-grid units); valid, entering [N] uint8, rel [N] int32,
  * coords_init [S,N,2], vis_init, conf_init [S,N] fp32.  Null pointers, K outside [1, 65535], S < 2, step outside
  * [1, S), stride < 1, a stream whose tracks do not tile [0, N) in order, T outside [1, S], ind < 0 or ind + S > 2^30,
- * frame0 + S > T_pyr, or (ind > 0) a null history or len < ind + overlap or cap < len return CT3_EINVAL, a small
- * workspace CT3_ENOSPC, before any launch.  Query frames beyond +-2^30 compare as +-2^30. */
+ * frame0 + S > T_pyr, or (ind > 0) a null history or len < ind + overlap return CT3_EINVAL, a small workspace
+ * CT3_ENOSPC, before any launch.  So do, with ring = 0, cap < len; with ring = 1, cap < S, ring outside {0, 1}, or
+ * (ind > 0) an overlap frame the ring no longer holds (ind < len - cap).  Query frames beyond +-2^30 compare as
+ * +-2^30. */
 int ct3_online_window_begin(const ct3_online_stream* streams_host, int K, int S, int step, int stride, int T_pyr,
                             const int32_t* qframes, const float* qcoords, int N, uint8_t* valid, uint8_t* entering,
                             int32_t* rel, float* coords_init, float* vis_init, float* conf_init, void* workspace,
                             size_t workspace_bytes, ct3_stream_t stream);
 /* ct3_online_window_end: the loop's result into the histories and the predictor's output, bit-identical to
  *   history[ind + t, j] = (coords[t, first + j] * stride, vis[...], conf[...])   for t < T  (frames ind + T.. untouched)
- *   tracks[t, j] = history_coords[t, j] * (scale_x, scale_y),
- *   visibility[t, j] = sigmoid(history_vis[t, j]) * sigmoid(history_conf[t, j]) > threshold   for t < ind + T, j < n_keep
- * with sigmoid(x) = 1 / (1 + expf(-x)) in fp32, as torch.sigmoid evaluates it.  coords [S,N,2], vis, conf [S,N] fp32:
- * the update loop's state (feature-grid units, logits).  The same argument checks as window_begin (without T_pyr and
- * the overlap), plus cap < ind + T, len < ind, and a stream with `tracks` whose visibility is NULL or n_keep is outside
- * [1, n]. */
+ *   tracks[f - out_first, j] = history_coords[f, j] * (scale_x, scale_y),
+ *   visibility[f - out_first, j] = sigmoid(history_vis[f, j]) * sigmoid(history_conf[f, j]) > threshold
+ *     for out_first <= f < ind + T, j < n_keep
+ * with sigmoid(x) = 1 / (1 + expf(-x)) in fp32, as torch.sigmoid evaluates it, and history frames addressed through
+ * the ring when ring = 1.  coords [S,N,2], vis, conf [S,N] fp32: the update loop's state (feature-grid units, logits).
+ * The work is O((ind + T - out_first) * n) per stream with an output and O(T * n) without.  The same argument checks
+ * as window_begin (without T_pyr and the overlap), plus len < ind, a stream with `tracks` whose visibility is NULL,
+ * n_keep is outside [1, n] or out_first is outside [0, ind + T), and with ring = 0 cap < ind + T.  With ring = 1 also
+ * (`tracks` set) an output frame before the window that the ring no longer holds (out_first < min(ind, len - cap)),
+ * or an output longer than the ring (ind + T - out_first > cap: a frame the launch reads would share its row with one
+ * it writes). */
 int ct3_online_window_end(const ct3_online_stream* streams_host, int K, int S, int stride, const float* coords,
                           const float* vis, const float* conf, int N, float threshold, void* workspace,
                           size_t workspace_bytes, ct3_stream_t stream);
