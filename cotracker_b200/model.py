@@ -185,11 +185,23 @@ class StreamState:
                 a[:self.length] = b[:self.length]
         self.hist = new
 
+    def edit(self, keep: torch.Tensor, at: int, coords: torch.Tensor):
+        """The history side of `StreamPool.edit`: keep columns `keep` [k] (int64, in order) and insert m new columns
+        after the first `at` of them that hold coords [m,2] (model resolution) with vis and conf logits 0 at every row:
+        every frame of the history, and every row a ring holds.  The buffers keep their size."""
+        m = coords.shape[0]
+        if self.hist is not None:
+            cap = self.hist[1].shape[0]
+            new = (coords.expand(cap, m, 2), coords.new_zeros(cap, m), coords.new_zeros(cap, m))
+            self.hist = tuple(torch.cat([h.index_select(1, keep[:at]), x, h.index_select(1, keep[at:])], 1)
+                              for h, x in zip(self.hist, new))
+        self.n = keep.shape[0] + m
+
 
 class StreamPool:
     """The tracks of a set of streams, stream after stream: support features [4,49,N,128] (accumulated as queries enter
     the window), query frames [N] int32 (stream time) and query coordinates [N,2] (feature-grid units).  `open` appends
-    a stream's tracks; `close` removes them with one copy of what follows."""
+    a stream's tracks; `close` removes them and `edit` changes them, each with one copy of the pool."""
 
     def __init__(self):
         self.streams: List[StreamState] = []
@@ -220,6 +232,28 @@ class StreamPool:
         for s in self.streams:
             if s.first >= b:
                 s.first -= state.n
+
+    def edit(self, state: StreamState, keep, at: int, qframes: torch.Tensor, qcoords: torch.Tensor, stride: int):
+        """A column edit of `state`'s tracks, the way the reference's per-track tensors would be edited along their N
+        axis: keep its tracks `keep` (indices into its n, in order), and insert the tracks of qframes [m] / qcoords [m,2]
+        (as `open` takes them) after the first `at` kept ones.  A new track has zero support features and, at every frame
+        of the history, its query point (qcoords * stride) with vis and conf logits 0."""
+        a, b = state.first, state.first + state.n
+        keep = torch.as_tensor(list(keep), dtype=torch.long).to(self.qframes.device)
+        qframes, qcoords = qframes.to(self.qframes), qcoords.to(self.qcoords)
+        head, tail = keep[:at] + a, keep[at:] + a
+
+        def cols(x, dim, new):
+            return torch.cat([x.narrow(dim, 0, a), x.index_select(dim, head), new, x.index_select(dim, tail),
+                              x.narrow(dim, b, x.shape[dim] - b)], dim)
+
+        support = cols(self.support, 2, self.support.new_zeros(4, 49, qframes.shape[0], 128))
+        qf, qc = cols(self.qframes, 0, qframes), cols(self.qcoords, 0, qcoords)
+        state.edit(keep, at, qcoords * float(stride))
+        self.support, self.qframes, self.qcoords = support, qf, qc
+        for s in self.streams:
+            if s.first >= b:
+                s.first += state.n - (b - a)
 
 
 class CoTrackerThreeBase(nn.Module):

@@ -21,10 +21,25 @@ its last L = min(h, frames so far) frames only, and a step's work does not grow 
 is then exactly the last L frames of the unbounded result, `full[:, -L:]`; `length(sid)` gives the stream's frame
 count, so the result covers frames [length - L, length).  A stream can advance until a window would pass frame
 2^30 (about 414 days at 30 fps); `push()` reports that limit.
+
+A stream's tracks can change between steps:
+
+    hub.retire_tracks(c, [3, 7])                    # ids of track_ids(c); the support grid's points have none
+    new = hub.add_tracks(c, q)                      # [1,m,3] (t, x, y), frame pixels, every t >= hub.length(c)
+    hub.track_ids(c)                                # the columns of c's next results: open() gave 0..n-1, adds continue
+
+An edit is the same edit of the reference online model's per-track state between two predictor calls, along its N
+axis: retiring deletes the tracks' columns; adding inserts columns after the stream's own tracks (before its support
+grid) with zero support features and, at every frame so far, the query point with vis and conf logits 0.  So at the
+frames before the next window an added track reads as its query point, not visible, and the other tracks' frames
+there are unchanged.  Edits take effect at the stream's next step and each call copies the track pool once.  A track
+whose query frame lies ahead still takes part in the attention of the other tracks, so adding one mid-stream is not
+the same as having opened the stream with it; before the first step it is, bit for bit.
 """
 from __future__ import annotations
 
-from typing import Dict, Optional, Tuple
+import numbers
+from typing import Dict, List, Optional, Tuple
 
 import torch
 
@@ -68,7 +83,8 @@ class OnlineStreams:
         self._next_id += 1
         n_keep = n_out if add_support_grid else q.shape[1]
         ih, iw = self.predictor.interp_shape
-        self._streams[sid] = dict(state=state, hw=(H, W), out=(n_keep, ((W - 1) / (iw - 1), (H - 1) / (ih - 1))))
+        self._streams[sid] = dict(state=state, hw=(H, W), out=(n_keep, ((W - 1) / (iw - 1), (H - 1) / (ih - 1))),
+                                  ids=list(range(n_keep)), next_id=n_keep)
         return sid
 
     def _get(self, sid: int) -> dict:
@@ -99,6 +115,54 @@ class OnlineStreams:
         self._pending.pop(sid, None)
         self.pool.close(s["state"])
         del self._streams[sid]
+
+    def track_ids(self, sid: int) -> List[int]:
+        """The ids of the tracks of stream `sid`'s results, in column order, from its next step on.  open() numbers
+        its tracks 0..n-1 and each add_tracks() continues upward; a stream never reuses an id."""
+        return list(self._get(sid)["ids"])
+
+    @torch.no_grad()
+    def add_tracks(self, sid: int, queries: torch.Tensor) -> List[int]:
+        """Add the tracks of queries [1,m,3] (t, x, y) to stream `sid` from its next step on: frame pixels and stream
+        time, as open() takes them.  Every t must be >= length(sid): a frame the stream has passed can no longer give
+        a track its features.  The new tracks follow the others in the results (before the support grid).  At the
+        frames before the next window they read as their query point, not visible.  -> their ids."""
+        s = self._get(sid)
+        if queries.dim() != 3 or queries.shape[0] != 1 or queries.shape[1] < 1 or queries.shape[2] != 3:
+            raise ValueError(f"queries must be [1,m,3] with m >= 1, got {tuple(queries.shape)}")
+        state = s["state"]
+        t = queries[0, :, 0]
+        if not bool((t >= state.length).all()):
+            raise ValueError(f"stream {sid} has advanced {state.length} frames: query frames must be >= "
+                             f"{state.length}, got {float(t.min())}")
+        q, _ = self.predictor._first_step_queries(1, s["hw"], queries, 0, 0, False, ingest.model_device(self.model))
+        n_keep, scale = s["out"]
+        self.pool.edit(state, range(state.n), n_keep, *self.model._stream_queries(q[0]), self.model.stride)
+        m = q.shape[1]
+        ids = list(range(s["next_id"], s["next_id"] + m))
+        s.update(ids=s["ids"] + ids, next_id=s["next_id"] + m, out=(n_keep + m, scale))
+        return ids
+
+    def retire_tracks(self, sid: int, ids):
+        """Remove the tracks `ids` (ids of stream `sid`, see track_ids) from its next step on.  The support grid's
+        points have no ids; a stream keeps at least one track of its own: close it instead."""
+        s = self._get(sid)
+        ids = ids.tolist() if torch.is_tensor(ids) else list(ids)
+        col = {i: c for c, i in enumerate(s["ids"])}
+        for i in ids:
+            if isinstance(i, bool) or not isinstance(i, numbers.Integral) or i not in col:
+                raise ValueError(f"stream {sid} has no track {i!r}: its track ids are track_ids({sid})")
+        if len(set(ids)) != len(ids):
+            raise ValueError(f"track ids to retire hold duplicates: {ids}")
+        if len(ids) == len(col):
+            raise ValueError(f"retiring every track of stream {sid} would leave it empty: close it instead")
+        state = s["state"]
+        gone = {col[i] for i in ids}
+        n_keep, scale = s["out"]
+        dev = self.pool.qframes.device
+        self.pool.edit(state, [c for c in range(state.n) if c not in gone], n_keep - len(gone),
+                       torch.empty(0, dtype=torch.int32, device=dev), torch.empty(0, 2, device=dev), self.model.stride)
+        s.update(ids=[i for i in s["ids"] if col[i] not in gone], out=(n_keep - len(gone), scale))
 
     @torch.no_grad()
     def step(self) -> Dict[int, Tuple[torch.Tensor, torch.Tensor]]:
