@@ -15,6 +15,7 @@ the result is bit-identical to the call on `video[b:b+1]`, `queries[b:b+1]` (DES
 """
 from __future__ import annotations
 
+import hashlib
 import math
 from typing import List, Optional
 
@@ -197,20 +198,32 @@ class StreamState:
                               for h, x in zip(self.hist, new))
         self.n = keep.shape[0] + m
 
+    def export_history(self) -> Optional[List[torch.Tensor]]:
+        """Host copies of the history rows a later window can read: the whole ring of a bounded state (frame f stays
+        at row f mod cap), rows [0, length) otherwise; None before the first step."""
+        if self.hist is None:
+            return None
+        rows = self.hist[1].shape[0] if self.history is not None else self.length
+        return [h[:rows].to("cpu", copy=True) for h in self.hist]
+
 
 class StreamPool:
     """The tracks of a set of streams, stream after stream: support features [4,49,N,128] (accumulated as queries enter
     the window), query frames [N] int32 (stream time) and query coordinates [N,2] (feature-grid units).  `open` appends
-    a stream's tracks; `close` removes them and `edit` changes them, each with one copy of the pool."""
+    a stream's tracks; `close` removes them and `edit` changes them, each with one copy of the pool.  `export` copies a
+    stream's state to the host and `restore` appends it back, to this pool or another."""
 
     def __init__(self):
         self.streams: List[StreamState] = []
         self.support = self.qframes = self.qcoords = None
 
-    def open(self, qframes: torch.Tensor, qcoords: torch.Tensor, history: Optional[int] = None) -> StreamState:
+    def open(self, qframes: torch.Tensor, qcoords: torch.Tensor, history: Optional[int] = None,
+             support: Optional[torch.Tensor] = None) -> StreamState:
+        """Append a stream of the tracks qframes [n] / qcoords [n,2], with zero support features or `support`
+        [4,49,n,128]."""
         n = qframes.shape[0]
         state = StreamState(n, 0 if self.qframes is None else self.qframes.shape[0], history)
-        sup = torch.zeros(4, 49, n, 128, device=qframes.device)
+        sup = torch.zeros(4, 49, n, 128, device=qframes.device) if support is None else support.contiguous()
         if self.support is None:
             self.support, self.qframes, self.qcoords = sup, qframes.contiguous(), qcoords.contiguous()
         else:
@@ -255,6 +268,27 @@ class StreamPool:
             if s.first >= b:
                 s.first += state.n - (b - a)
 
+    def export(self, state: StreamState) -> dict:
+        """`state`'s own values as host tensors and ints: its columns of the pool, its window start, length and bound,
+        and its history (`StreamState.export_history`).  The encoder cache is left out: the first window after a
+        `restore` encodes its chunk whole, which gives the same features (the encoder is strictly per frame)."""
+        a, b = state.first, state.first + state.n
+        return dict(n=state.n, ind=state.ind, length=state.length, history=state.history,
+                    support=self.support[:, :, a:b].to("cpu", copy=True),
+                    qframes=self.qframes[a:b].to("cpu", copy=True), qcoords=self.qcoords[a:b].to("cpu", copy=True),
+                    hist=state.export_history())
+
+    def restore(self, snap: dict, device) -> StreamState:
+        """Append the stream of `export`'s `snap` on `device`, as `open` appends one; the state owns copies of the
+        snapshot's tensors, so one snapshot can be restored any number of times."""
+        state = self.open(snap["qframes"].to(device, copy=True), snap["qcoords"].to(device, copy=True),
+                          snap["history"], support=snap["support"].to(device, copy=True))
+        state.ind, state.length = snap["ind"], snap["length"]
+        if snap["hist"] is not None:
+            rows = snap["hist"][1].shape[0] if state.history is not None else state.length
+            state.hist = tuple(h[:rows].to(device, copy=True).contiguous() for h in snap["hist"])
+        return state
+
 
 class CoTrackerThreeBase(nn.Module):
     def __init__(self, window_len=8, stride=4, corr_radius=3, corr_levels=4, num_virtual_tracks=64,
@@ -284,6 +318,8 @@ class CoTrackerThreeBase(nn.Module):
         self._packed_key = None
         self._enc_packed: Optional[torch.Tensor] = None
         self._enc_key = None
+        self._fingerprint: Optional[str] = None
+        self._fingerprint_key = None
         self._ws = engine.WorkspaceCache()
         self._enc_ws: Optional[torch.Tensor] = None
 
@@ -302,6 +338,19 @@ class CoTrackerThreeBase(nn.Module):
             self._packed = engine.pack_weights(sd, device)
             self._packed_key = key
         return self._packed
+
+    def weights_fingerprint(self) -> str:
+        """sha256 over the names, dtypes, shapes and bytes of every parameter and buffer: the same string for the same
+        weights on any device.  Computed once per weights version, like `packed_weights`."""
+        tensors = sorted(self.state_dict(keep_vars=True).items())
+        key = tuple((k, v.data_ptr(), v._version) for k, v in tensors)
+        if self._fingerprint_key != key:
+            h = hashlib.sha256()
+            for k, v in tensors:
+                h.update(f"{k}|{v.dtype}|{tuple(v.shape)};".encode())
+                h.update(v.detach().reshape(-1).to("cpu").contiguous().view(torch.uint8).numpy())
+            self._fingerprint, self._fingerprint_key = h.hexdigest(), key
+        return self._fingerprint
 
     def interpolate_time_embed(self, t: int) -> torch.Tensor:
         """[t, 1110] time embedding (reference cotracker3_online.py:145-156); constant per (buffer, t): cached."""

@@ -35,6 +35,24 @@ frames before the next window an added track reads as its query point, not visib
 there are unchanged.  Edits take effect at the stream's next step and each call copies the track pool once.  A track
 whose query frame lies ahead still takes part in the attention of the other tracks, so adding one mid-stream is not
 the same as having opened the stream with it; before the first step it is, bit for bit.
+
+A stream can be parked on the host and continued on any hub of the same model:
+
+    snap = hub.snapshot(c)                          # CPU tensors and plain values; c runs on unchanged
+    hub.close(c)                                    # frees c's device memory
+    torch.save(snap, f)                             # loads with torch.load(f, weights_only=True)
+    c2 = other_hub.restore(snap)                    # a new id on other_hub's device
+
+From its next step on, a restored stream's results are `torch.equal` to those the snapshotted stream would have given
+without the snapshot, fed the same chunks, whatever the other streams of either hub do.  This needs the same weights
+and the same GPU model: some split-K choices depend on the SM count.  Restoring one snapshot twice gives two
+independent streams.  A snapshot holds the stream's own state and nothing more: its columns of the pool (support
+features, query frames and coordinates), its window start, length and bound, its history (the whole ring of a bounded
+stream, frames [0, length) otherwise), its frame size, output width, track ids and next track id, the format version,
+and the model's window_len, interp_shape, stride and weights fingerprint, which `restore` checks.  It leaves out the
+encoder features of the overlap frames (67 MB at 384x512): the chunk after a restore holds those frames again, and
+the first step encodes the stream's whole chunk, which gives the same features since the encoder is strictly per
+frame.  `restore` validates everything it reads before it changes anything (`check_snapshot`).
 """
 from __future__ import annotations
 
@@ -43,8 +61,91 @@ from typing import Dict, List, Optional, Tuple
 
 import torch
 
-from . import ingest
-from .model import StreamPool
+from . import engine, ingest
+from .model import StreamPool, StreamState
+
+SNAPSHOT_FORMAT = 1
+_SNAPSHOT_FIELDS = ("model", "frame_size", "n_keep", "ids", "next_id", "n", "ind", "length", "history", "support",
+                    "qframes", "qcoords", "hist")
+
+
+def _is_int(x) -> bool:
+    return isinstance(x, numbers.Integral) and not isinstance(x, bool)
+
+
+def _check_tensor(name: str, t, dtype, shape):
+    got = f"{t.dtype} {list(t.shape)}" if torch.is_tensor(t) else type(t).__name__
+    if not torch.is_tensor(t) or t.dtype != dtype or tuple(t.shape) != tuple(shape):
+        raise ValueError(f"snapshot field {name} must be a {dtype} tensor {list(shape)}, got {got}")
+
+
+def check_snapshot(snap, identity: dict):
+    """Raise ValueError unless `snap` is a stream state that `OnlineStreams.restore` can continue on a model of
+    `identity` (`OnlineStreams.model_identity`): a known format, the same model, every field present with its type,
+    dtype and shape, and a window start and length a stream can reach.  A snapshot comes from outside the program (a
+    file), so everything is checked; this reads nothing but its arguments and needs no device."""
+    if not isinstance(snap, dict):
+        raise ValueError(f"a snapshot is a dict, got {type(snap).__name__}")
+    fmt = snap.get("format")
+    if not _is_int(fmt) or fmt != SNAPSHOT_FORMAT:
+        raise ValueError(f"unknown snapshot format {fmt!r}: this version reads format {SNAPSHOT_FORMAT}")
+    missing = [k for k in _SNAPSHOT_FIELDS if k not in snap]
+    if missing:
+        raise ValueError(f"the snapshot misses the fields {missing}")
+    model = snap["model"]
+    if not isinstance(model, dict):
+        raise ValueError(f"snapshot field model must be a dict, got {type(model).__name__}")
+    for k, v in identity.items():
+        if model.get(k) != v:
+            raise ValueError(f"the snapshot was taken on a model with {k} {model.get(k)!r}, this hub's has {v!r}")
+    ints = {k: snap[k] for k in ("n_keep", "next_id", "n", "ind", "length")}
+    for k, v in ints.items():
+        if not _is_int(v):
+            raise ValueError(f"snapshot field {k} must be an int, got {type(v).__name__}")
+    hw, ids, history = snap["frame_size"], snap["ids"], snap["history"]
+    if not isinstance(hw, (list, tuple)) or len(hw) != 2 or not all(_is_int(x) and x >= 2 for x in hw):
+        raise ValueError(f"snapshot field frame_size must be [H, W] with H, W >= 2 ints, got {hw!r}")
+    if history is not None and (not _is_int(history) or history < 1):
+        raise ValueError(f"snapshot field history must be None or an int >= 1, got {history!r}")
+    if not isinstance(ids, (list, tuple)) or not all(_is_int(i) for i in ids):
+        raise ValueError("snapshot field ids must be a list of ints")
+    n, n_keep, next_id, ind, length = (ints[k] for k in ("n", "n_keep", "next_id", "ind", "length"))
+    if n < 1 or not 1 <= n_keep <= n:
+        raise ValueError(f"a snapshot holds 1 <= n_keep <= n tracks, got n_keep {n_keep} of n {n}")
+    if len(ids) != n_keep or len(set(ids)) != n_keep or any(not 0 <= i < next_id for i in ids):
+        raise ValueError(f"snapshot field ids must be n_keep = {n_keep} distinct ids in [0, next_id = {next_id}), "
+                         f"got {len(ids)} ids")
+    _check_tensor("support", snap["support"], torch.float32, (4, 49, n, 128))
+    _check_tensor("qframes", snap["qframes"], torch.int32, (n,))
+    _check_tensor("qcoords", snap["qcoords"], torch.float32, (n, 2))
+    if int(snap["qframes"].abs().max()) > engine.QUERY_FRAME_LIMIT:
+        raise ValueError(f"snapshot field qframes holds query frames past +-{engine.QUERY_FRAME_LIMIT}")
+    S = identity["window_len"]
+    step = S // 2
+    if ind < 0 or length < 0:
+        raise ValueError(f"a stream's window start and length are >= 0, got ind {ind}, length {length}")
+    # after k >= 1 windows of chunks of 1..S frames: ind = k * step, length = ind - step + T
+    if ind % step or (length != 0 if ind == 0 else not ind - step + 1 <= length <= ind - step + S):
+        raise ValueError(f"no stream reaches window start {ind} with length {length} (window_len {S})")
+    if ind and ind - step + S > engine.STREAM_FRAME_LIMIT:
+        raise ValueError(f"window start {ind} lies past the stream frame limit {engine.STREAM_FRAME_LIMIT}")
+    hist = snap["hist"]
+    if length == 0:
+        if hist is not None:
+            raise ValueError("a stream that has not advanced has no history: snapshot field hist must be None")
+        return
+    if not isinstance(hist, (list, tuple)) or len(hist) != 3 or not torch.is_tensor(hist[1]) or hist[1].dim() != 2:
+        raise ValueError("snapshot field hist must be [coords [R,n,2], vis [R,n], conf [R,n]]")
+    rows = hist[1].shape[0]
+    cap = None if history is None else StreamState(n, 0, history).ring_frames(S, step)
+    if history is not None and rows != cap:
+        raise ValueError(f"a stream bounded at history={history} keeps a ring of {cap} frames, the snapshot "
+                         f"holds {rows}")
+    if history is None and rows < length:
+        raise ValueError(f"the history of a stream of length {length} holds {length} frames, the snapshot {rows}")
+    for name, t, shape in (("coords", hist[0], (rows, n, 2)), ("vis", hist[1], (rows, n)),
+                           ("conf", hist[2], (rows, n))):
+        _check_tensor(f"hist {name}", t, torch.float32, shape)
 
 
 class OnlineStreams:
@@ -79,12 +180,17 @@ class OnlineStreams:
         q, n_out = self.predictor._first_step_queries(1, (H, W), queries, grid_size, grid_query_frame,
                                                       add_support_grid, dev)
         state = self.pool.open(*self.model._stream_queries(q[0]), history=history)
+        n_keep = n_out if add_support_grid else q.shape[1]
+        return self._add(state, (H, W), n_keep, list(range(n_keep)), n_keep)
+
+    def _add(self, state, hw, n_keep: int, ids: List[int], next_id: int) -> int:
+        """Register a stream of the pool under a new id: its frame size, output width, track ids and next track id."""
         sid = self._next_id
         self._next_id += 1
-        n_keep = n_out if add_support_grid else q.shape[1]
+        H, W = hw
         ih, iw = self.predictor.interp_shape
         self._streams[sid] = dict(state=state, hw=(H, W), out=(n_keep, ((W - 1) / (iw - 1), (H - 1) / (ih - 1))),
-                                  ids=list(range(n_keep)), next_id=n_keep)
+                                  ids=ids, next_id=next_id)
         return sid
 
     def _get(self, sid: int) -> dict:
@@ -115,6 +221,33 @@ class OnlineStreams:
         self._pending.pop(sid, None)
         self.pool.close(s["state"])
         del self._streams[sid]
+
+    def model_identity(self) -> dict:
+        """What a snapshot must have been taken on to be restored here: window_len, interp_shape, stride and the
+        weights' fingerprint."""
+        return dict(window_len=self.model.window_len, interp_shape=list(self.predictor.interp_shape),
+                    stride=self.model.stride, weights=self.model.weights_fingerprint())
+
+    def snapshot(self, sid: int) -> dict:
+        """Stream `sid`'s state as CPU tensors and plain Python values (`torch.save` it, load it with
+        `weights_only=True`); the stream runs on unchanged.  Taken between steps: a pushed chunk must be stepped first."""
+        s = self._get(sid)
+        if sid in self._pending:
+            raise ValueError(f"stream {sid} has a chunk waiting for step(): take a snapshot between steps")
+        return dict(self.pool.export(s["state"]), format=SNAPSHOT_FORMAT, model=self.model_identity(),
+                    frame_size=list(s["hw"]), n_keep=s["out"][0], ids=list(s["ids"]), next_id=s["next_id"])
+
+    @torch.no_grad()
+    def restore(self, snap: dict) -> int:
+        """Add the stream of `snapshot()`'s `snap` to this hub, on its device, as `open()` adds one.  From its next
+        step on its results are `torch.equal` to those the snapshotted stream would have given, on the same model and
+        device model.  Restoring one snapshot twice gives two independent streams.  -> the new stream's id."""
+        check_snapshot(snap, self.model_identity())
+        dev = ingest.model_device(self.model)
+        if dev.type != "cuda":
+            raise ValueError("the predictor's model must be on a CUDA device")
+        state = self.pool.restore(snap, dev)
+        return self._add(state, tuple(snap["frame_size"]), snap["n_keep"], list(snap["ids"]), snap["next_id"])
 
     def track_ids(self, sid: int) -> List[int]:
         """The ids of the tracks of stream `sid`'s results, in column order, from its next step on.  open() numbers
