@@ -111,7 +111,7 @@ using namespace ct3;
 // ================================================================================================
 extern "C" {
 
-int ct3_version(void) { return 101; }
+int ct3_version(void) { return 102; }
 const char* ct3_last_error(void) { return g_err; }
 
 int ct3_set_option(const char* name, int value) {

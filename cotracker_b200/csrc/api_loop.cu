@@ -117,11 +117,13 @@ struct Workspace {
   float* qkv;             // [(N+64)*T, 1152]; slabbed: max(S*1152, N*T*768)   (also point q / point kv / p<-v output)
   float* vqkv;            // [64*T, 1152]       (virtual q / kv / qkv)
   __nv_bfloat16* hmid;    // [S + 64*T, 2*1536]; slabbed: [S, 2*1536]
-  float* row_bias;        // [T, 384]
+  float* row_bias;        // [T, 384]; with group_T [G*T, 384] (group g's time embedding in rows g*T ..)
   float* att_part;        // split-K partials of the virtual<-point attention
   __nv_bfloat16* pyr_split;  // split-bf16 copy of the pyramid (corr_tc2.cu); null when H4 == 0
   int32_t* groups;        // device group table of a grouped call (GroupPlan); null when G == 1
   int32_t* frames;        // device frame map [G, T] of a pass with T_pyr >= 1; null without one
+  int32_t* track_len;     // [N + 64 G] length of every point and virtual track's group; null without group_T
+  int32_t* track_group;   // [N] group of every point track (its row-bias block); null without group_T
   int slab;               // tracks per slab; N: no slabs
   size_t total;
   bool slabbed() const { return slab_rows < point_rows; }
@@ -135,7 +137,10 @@ int partial_slots(int N, int G) {
   return (int)(s < (int64_t)kAttnMaxSplits * G ? s : (int64_t)kAttnMaxSplits * G);
 }
 // int32 entries of the group table: offsets [G+1] | all [G] | split [G] | slot [G] | small [G] | tiles [2 * max tiles]
-int64_t group_table_ints(int N, int G) { return G == 1 ? 0 : (int64_t)5 * G + 1 + 2 * ((int64_t)N / 128 + G); }
+int64_t group_table_ints(int N, int G) { return (int64_t)5 * G + 1 + 2 * ((int64_t)N / 128 + G); }
+// A pass runs its space attentions through a group table when it has several groups or group lengths (group_T): each
+// group's split-K count is then its own, from its own length
+bool grouped(const ct3_loop_shape& s) { return s.G > 1 || s.group_T; }
 
 // The workspace of pass s (a null base only measures): the split pyramid copy is sized by the T_pyr (0: T) frames the
 // correlation reads, room for the [G, T] frame map iff T_pyr >= 1, slab_tracks 0 or >= N: no slabs
@@ -158,13 +163,15 @@ Workspace carve(void* base, const ct3_loop_shape& s) {
   w.qkv = (float*)c.take(sl ? (S * 3 > Rp * 2 ? S * 3 : Rp * 2) * kC * 4 : R * 3 * kC * 4);
   w.vqkv = (float*)c.take(Rv * 3 * kC * 4);
   w.hmid = (__nv_bfloat16*)c.take((sl ? S : R) * 2 * kMlpHid * 2);
-  w.row_bias = (float*)c.take((size_t)T * kC * 4);
+  w.row_bias = (float*)c.take((size_t)(s.group_T ? G : 1) * T * kC * 4);
   w.att_part = (float*)c.take(attention_partial_bytes(T, kV, partial_slots(N, G)));
   w.pyr_split = nullptr;
   if (H4 > 0 && W4 > 0 && corr_patch_supported(T_pyr, H4, W4))
     w.pyr_split = (__nv_bfloat16*)c.take((size_t)pyramid_layout(T_pyr, H4, W4).total * 4);
-  w.groups = G > 1 ? (int32_t*)c.take((size_t)group_table_ints(N, G) * 4) : nullptr;
+  w.groups = grouped(s) ? (int32_t*)c.take((size_t)group_table_ints(N, G) * 4) : nullptr;
   w.frames = s.T_pyr > 0 ? (int32_t*)c.take((size_t)G * T * 4) : nullptr;
+  w.track_len = s.group_T ? (int32_t*)c.take(((size_t)N + (size_t)kV * G) * 4) : nullptr;
+  w.track_group = s.group_T ? (int32_t*)c.take((size_t)N * 4) : nullptr;
   w.total = c.off;
   return w;
 }
@@ -249,22 +256,26 @@ struct GroupPlan {
   int G = 1, max_n = 0;
   const int32_t *off = nullptr, *all = nullptr, *split = nullptr, *slot = nullptr, *small = nullptr, *tile = nullptr;
   int n_small = 0, n_tiles = 0, split_max = 1, split_slots = 0;
+  // group lengths (ct3_loop_shape.group_T): every point and virtual track's length, on the device and on the host
+  const int32_t *track_len = nullptr, *track_len_host = nullptr;
 };
 
-int plan_groups(GroupPlan& gp, const int32_t* sizes, int G, int T, int N, int32_t* dev, cudaStream_t s) {
+// group_T: null, or the G group lengths; a table is built whenever G > 1 or group_T is given (grouped())
+int plan_groups(GroupPlan& gp, const int32_t* sizes, int G, int T, int N, const int32_t* group_T, int32_t* dev,
+                cudaStream_t s) {
   gp.G = G;
-  if (G == 1) return 0;
+  if (G == 1 && !group_T) return 0;
   std::vector<int32_t> h((size_t)group_table_ints(N, G), 0);
   int32_t* off = h.data();
   int32_t *all = off + G + 1, *split = all + G, *slot = split + G, *small = slot + G, *tile = small + G;
   const int nsm = num_sms();
   for (int g = 0; g < G; ++g) {
-    const int n = sizes[g];
+    const int n = sizes ? sizes[g] : N;
     off[g + 1] = off[g] + n;
     if (n > gp.max_n) gp.max_n = n;
     all[g] = g;
-    // virtual <- point: the split-K count of a standalone call (T sequences of kV queries over n keys)
-    split[g] = attention_tc_splits(T, kV, n, nsm);
+    // virtual <- point: the split-K count of a standalone call (T, or group_T[g], sequences of kV queries over n keys)
+    split[g] = attention_tc_splits(group_T ? group_T[g] : T, kV, n, nsm);
     if (split[g] > 1) {
       slot[g] = gp.split_slots;
       gp.split_slots += split[g];
@@ -294,7 +305,7 @@ int plan_groups(GroupPlan& gp, const int32_t* sizes, int G, int T, int N, int32_
 // One space attention of a block (cotracker.py:510-517) over every group.  `a` describes it for one group of N tracks
 // (sequence = frame); q_pts / k_pts tell which side holds the point tokens.
 int space_attention(Runner& R, const Workspace& W, const GroupPlan& gp, AttnParams a, bool q_pts, bool k_pts) {
-  if (gp.G == 1) return run_attention(R, W, a, false);
+  if (!gp.off) return run_attention(R, W, a, false);
   const int T = a.num_seq, n_all = a.Lq;
   a.goff = gp.off;
   a.frames = T;
@@ -332,19 +343,51 @@ int space_attention(Runner& R, const Workspace& W, const GroupPlan& gp, AttnPara
 // n*T + t) into att (split rows of pitch 2*kC).  With fuse = 1 on the product kernels (gemm 0, attn != 1) and T <= 128
 // both run in ONE kernel, so fp32 q|k|v never reaches HBM; otherwise the b.q GEMM writes q|k|v to W.qkv [rows, 3*kC]
 // and the per-warp attention kernel reads it.
+// len / len_host: null, or the length of each of the rows / T tracks (ct3_loop_shape.group_T) on the device and the
+// host: a track attends over its own frames only.  A track takes the kernel a pass of its own length would take: with
+// T > 128 and fusion on, the runs of tracks of at most 128 frames take the fused kernel (one track per tile, rows
+// t < 128) and the other runs the unfused one, each track once.  The fused kernel leaves rows [128, T) of a short
+// track, all of them padding, unwritten: they are zeroed so that every padded row stays finite.
 int time_attention(Runner& R, const Workspace& W, const Block& b, const __nv_bfloat16* x, __nv_bfloat16* att,
-                   int rows, int T) {
-  if (g_opt[OPT_FUSE] == 1 && R.impl == 0 && g_opt_attn != 1 && qkv_time_attn_supported(T)) {
+                   int rows, int T, const int32_t* len = nullptr, const int32_t* len_host = nullptr) {
+  const bool fuse = g_opt[OPT_FUSE] == 1 && R.impl == 0 && g_opt_attn != 1;
+  // The fused kernel reads keys [0, len) of a track from its 128-row tile: with T > 128 only tracks whose len_host
+  // entry is at most 128 may reach it, which the run split below guarantees (qkv_time_attn_supported).
+  auto fused = [&](int track0, int tracks) -> int {   // tracks [track0, track0 + tracks) of the rows
     ProfScope ps(R.s, CAT_QKVA, 0.0);
     const char* gerr = nullptr;
+    const int64_t r0 = (int64_t)track0 * T;
     const int rc = gemm_qkv_time_attn_launch(
-        x, reinterpret_cast<const __nv_bfloat16*>(R.pk + b.qkv_h.w), reinterpret_cast<const float*>(R.pk + b.qkv_h.b),
-        rows, kC, T, att, 2 * kC, kC, 1.0f / sqrtf((float)kDh), num_sms(), R.s, &gerr);
+        x + r0 * 2 * kC, reinterpret_cast<const __nv_bfloat16*>(R.pk + b.qkv_h.w),
+        reinterpret_cast<const float*>(R.pk + b.qkv_h.b), tracks * T, kC, T, len ? len + track0 : nullptr,
+        att + r0 * 2 * kC, 2 * kC, kC, 1.0f / sqrtf((float)kDh), num_sms(), R.s, &gerr);
     return rc ? fail_launch(rc, "fused qkv + time attention", gerr) : 0;
+  };
+  auto unfused = [&](int track0, int tracks) -> int {
+    const int64_t r0 = (int64_t)track0 * T;
+    GEMM(x + r0 * 2 * kC, b.q, tracks * T, Runner::to_f32(W.qkv, 3 * kC, false));
+    AttnParams a = attn_params(W.qkv, 3 * kC, W.qkv, 3 * kC, kC, 2 * kC, att + r0 * 2 * kC, T, T, T, tracks);
+    a.seq_len = len ? len + track0 : nullptr;
+    RUNC(CAT_ATTN, run_attention(R, W, a, true));
+    return 0;
+  };
+  if (fuse && qkv_time_attn_supported(T)) return fused(0, rows / T);
+  if (!fuse || !len_host) return unfused(0, rows / T);
+  for (int i = 0, n = rows / T; i < n;) {
+    const bool short_run = qkv_time_attn_supported(len_host[i]);
+    int j = i + 1;
+    while (j < n && qkv_time_attn_supported(len_host[j]) == short_run) ++j;
+    if (short_run) {
+      if (int rc = fused(i, j - i)) return rc;
+      const size_t row_bytes = 2 * kC * sizeof(__nv_bfloat16);
+      CK(cudaMemset2DAsync(att + ((int64_t)i * T + 128) * 2 * kC, (size_t)T * row_bytes, 0,
+                           (size_t)(T - 128) * row_bytes, (size_t)(j - i), R.s),
+         "zero padded time-attention rows");
+    } else if (int rc = unfused(i, j - i)) {
+      return rc;
+    }
+    i = j;
   }
-  GEMM(x, b.q, rows, Runner::to_f32(W.qkv, 3 * kC, false));
-  RUNC(CAT_ATTN, run_attention(R, W, attn_params(W.qkv, 3 * kC, W.qkv, 3 * kC, kC, 2 * kC, att, T, T, T, rows / T),
-                               true));
   return 0;
 }
 
@@ -424,7 +467,10 @@ int transformer_body(Runner& R, const Workspace& W, int T, int N, const GroupPla
             const int64_t s0 = scratch_row(W, r0, r0);
             float* x = W.tokens + r0 * kC;
             RUNC(CAT_LN, launch_layernorm_split(x, rows, nullptr, nullptr, 1e-6f, W.ln + s0 * 2 * kC, R.s));
-            if (int rc = time_attention(R, W, b, W.ln + s0 * 2 * kC, W.att + s0 * 2 * kC, rows, T)) return rc;
+            if (int rc = time_attention(R, W, b, W.ln + s0 * 2 * kC, W.att + s0 * 2 * kC, rows, T,
+                                        gp.track_len ? gp.track_len + n : nullptr,
+                                        gp.track_len_host ? gp.track_len_host + n : nullptr))
+              return rc;
             GEMM(W.att + s0 * 2 * kC, b.out, rows, Runner::to_f32(x, kC, true));
             return mlp_half(R, W, b, r0, rows, r0);
           }))
@@ -485,10 +531,12 @@ Prec effective_prec(bool have_pyr_split, int T, int H4, int W4) {
 }
 
 // input_transform of the X rows in W.xs into the point tokens of tracks [n0, n0 + count), with the per-frame bias
-// row_bias [T, kC] when given (a track's rows start at a multiple of T, so row % T is the frame)
+// row_bias [T, kC] when given (a track's rows start at a multiple of T, so row % T is the frame); with W.track_group
+// (group_T) track n adds block track_group[n] of row_bias [G*T, kC], its group's time embedding
 int input_transform(Runner& R, const Workspace& W, int T, int n0, int count, const float* row_bias) {
   GemmEpilogue e = Runner::to_f32(W.tokens + (int64_t)n0 * T * kC, kC, false);
   if (row_bias) { e.row_bias = row_bias; e.row_mod = T; }
+  if (row_bias && W.track_group) e.row_blk = W.track_group + n0;
   GEMM(W.xs, R.L.in_tr, count * T, e);
   return 0;
 }
@@ -517,7 +565,7 @@ int point_tokens_slab(Runner& R, const Workspace& W, const Prec& pr, const float
     GEMM(W.h1, L.corr_fc2, Mc, e);
   }
   // vis, conf, posenc(rel. motion), zero pad -> X columns [1024,1152)
-  RUNC(CAT_MISC, launch_build_x_small(coords, vis, conf, T, N, n0, count, W.xs, R.s));
+  RUNC(CAT_MISC, launch_build_x_small(coords, vis, conf, T, N, n0, count, W.track_len, W.xs, R.s));
   // (iv) input_transform (+ folded time embedding) -> point tokens
   return input_transform(R, W, T, n0, count, W.row_bias);
 }
@@ -571,6 +619,9 @@ int check_shape(const ct3_loop_shape* sh, Use use) {
   if (!sh) return fail(CT3_EINVAL, "null shape%s");
   const ct3_loop_shape& s = *sh;
   if (int rc = check_TN(s.T, s.N, s.G)) return rc;
+  if (s.group_T)
+    for (int g = 0; g < s.G; ++g)
+      if (s.group_T[g] < 1 || s.group_T[g] > s.T) return fail(CT3_EINVAL, "every group_T entry must be in [1, T]%s");
   if (s.group_sizes) {
     int64_t sum = 0;
     for (int g = 0; g < s.G; ++g) {
@@ -617,7 +668,22 @@ int update_loop(const void* packed, const float* pyr, const float* support, cons
   const Layout& L = layout();
   Runner R{reinterpret_cast<const uint8_t*>(packed), L, stream, g_opt_gemm};
   GroupPlan gp;
-  if (int rc = plan_groups(gp, s.group_sizes, G, T, N, W.groups, R.s)) return rc;
+  if (int rc = plan_groups(gp, s.group_sizes, G, T, N, s.group_T, W.groups, R.s)) return rc;
+  std::vector<int32_t> track_len;   // group lengths: every track's, points then virtual tracks, and each point's group
+  if (s.group_T) {
+    track_len.resize((size_t)N + (size_t)kV * G);
+    std::vector<int32_t> track_group((size_t)N);
+    for (int g = 0, n0 = 0; g < G; ++g) {
+      const int n = s.group_sizes ? s.group_sizes[g] : N;
+      for (int i = 0; i < n; ++i) { track_len[n0 + i] = s.group_T[g]; track_group[n0 + i] = g; }
+      for (int i = 0; i < kV; ++i) track_len[(size_t)N + (size_t)kV * g + i] = s.group_T[g];
+      n0 += n;
+    }
+    CK(launch_upload_i32(W.track_len, track_len.data(), (int)track_len.size(), R.s), "upload track lengths");
+    CK(launch_upload_i32(W.track_group, track_group.data(), N, R.s), "upload track groups");
+    gp.track_len = W.track_len;
+    gp.track_len_host = track_len.data();
+  }
   FrameMap fm;
   if (s.T_pyr > 0) {   // the frame map reaches the device like the group table: in stream order, through kernel args
     CK(launch_upload_i32(W.frames, s.group_frames, G * T, R.s), "upload frame map");
@@ -630,8 +696,11 @@ int update_loop(const void* packed, const float* pyr, const float* support, cons
   const __nv_bfloat16* pyr_split = (pr.patch && iters > 0) ? W.pyr_split : nullptr;
   if (pyr_split) RUNC(CAT_MISC, launch_split_pyramid(pyr, T_pyr, H4, W4, W.pyr_split, pr.corr, R.s));
 
-  // W_in * time_emb[t]: x + time_emb is folded into a per-frame bias of input_transform (cotracker3_offline.py:196)
-  RUNC(CAT_MISC, launch_row_bias(time_emb, reinterpret_cast<const float*>(R.pk + L.win_f32), T, W.row_bias, R.s));
+  // W_in * time_emb[t]: x + time_emb is folded into a per-frame bias of input_transform (cotracker3_offline.py:196);
+  // with group_T one [T, kC] block per group.  Each row is computed alone, so a block holds the bits a pass of the
+  // group's own length computes
+  RUNC(CAT_MISC, launch_row_bias(time_emb, reinterpret_cast<const float*>(R.pk + L.win_f32), s.group_T ? G * T : T,
+                                 W.row_bias, R.s));
 
   for (int it = 0; it < iters; ++it) {
     // (i)-(iv) correlation, corr_mlp, X, input_transform -> point tokens
@@ -652,7 +721,7 @@ int loop_tokens(const void* packed, const float* pyr, int H4, int W4, const floa
                 size_t workspace_bytes, cudaStream_t stream) {
   if (!packed || !pyr || !support || !coords || !vis || !conf || !time_emb || !workspace)
     return fail(CT3_EINVAL, "null argument%s");
-  const ct3_loop_shape shape{T, N, H4, W4, 1, nullptr, 0, nullptr, 0};
+  const ct3_loop_shape shape{T, N, H4, W4, 1, nullptr, 0, nullptr, 0, nullptr};
   if (int rc = check_shape(&shape, Use::kLoop)) return rc;
   if (int rc = check_aligned(workspace, "workspace")) return rc;
   const Workspace W = carve(workspace, shape);
@@ -678,14 +747,14 @@ int loop_tokens(const void* packed, const float* pyr, int H4, int W4, const floa
 int updateformer(const void* packed, const float* x, int T, int N, const int32_t* sizes, int G, float* delta,
                  void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   if (!packed || !x || !delta || !workspace) return fail(CT3_EINVAL, "null argument%s");
-  const ct3_loop_shape shape{T, N, 0, 0, G, sizes, 0, nullptr, 0};
+  const ct3_loop_shape shape{T, N, 0, 0, G, sizes, 0, nullptr, 0, nullptr};
   if (int rc = check_shape(&shape, Use::kFormer)) return rc;
   if (int rc = check_aligned(workspace, "workspace")) return rc;
   const Workspace W = carve(workspace, shape);
   if (int rc = check_space(workspace_bytes, W.total, "workspace")) return rc;
   Runner R{reinterpret_cast<const uint8_t*>(packed), layout(), stream, g_opt_gemm};
   GroupPlan gp;
-  if (int rc = plan_groups(gp, sizes, G, T, N, W.groups, R.s)) return rc;
+  if (int rc = plan_groups(gp, sizes, G, T, N, nullptr, W.groups, R.s)) return rc;
   RUNC(CAT_MISC, launch_split_rows(x, N * T, kX, kXPad, /*perm_x*/ 1, W.xs, 0, R.s));
   if (int rc = input_transform(R, W, T, 0, N, nullptr)) return rc;
   return transform_and_heads(R, W, T, N, gp, nullptr, nullptr, nullptr, delta);
@@ -706,7 +775,7 @@ int attention_stage(int kind, const float* q, const float* kv, int T, int N, con
                     void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   if (!q || !kv || !out || !workspace) return fail(CT3_EINVAL, "null argument%s");
   if (kind < CT3_ATTN_TIME || kind > CT3_ATTN_POINT_FROM_VIRTUAL) return fail(CT3_EINVAL, "unknown attention kind%s");
-  const ct3_loop_shape shape{T, N, 0, 0, G, sizes, 0, nullptr, 0};
+  const ct3_loop_shape shape{T, N, 0, 0, G, sizes, 0, nullptr, 0, nullptr};
   if (int rc = check_shape(&shape, Use::kFormer)) return rc;
   if (!sizes) return fail(CT3_EINVAL, "null group_sizes_host%s");
   if (((uintptr_t)q | (uintptr_t)kv | (uintptr_t)out) & 15) return fail(CT3_EINVAL, "q, kv and out must be 16-byte aligned%s");
@@ -721,7 +790,7 @@ int attention_stage(int kind, const float* q, const float* kv, int T, int N, con
     return 0;
   }
   GroupPlan gp;
-  if (int rc = plan_groups(gp, sizes, G, T, N, W.groups, R.s)) return rc;
+  if (int rc = plan_groups(gp, sizes, G, T, N, nullptr, W.groups, R.s)) return rc;
   __nv_bfloat16* att_v = att + Rp * 2 * kC;
   if (kind == CT3_ATTN_VIRTUAL_FROM_POINT)
     RUNC(CAT_ATTN, space_attention(R, W, gp, attn_params(q + Rp * kC, kC, kv, 2 * kC, 0, kC, att_v, kV, N, T), false,

@@ -79,7 +79,9 @@ __device__ __forceinline__ void epilogue_chunk(const GemmEpilogue& e, int M, int
     }
   }
   if (e.row_bias && row < M) {
-    const float4* b4 = reinterpret_cast<const float4*>(e.row_bias + (int64_t)(row % e.row_mod) * N + col0);
+    const int q = row / e.row_mod;
+    const int brow = row - q * e.row_mod + (e.row_blk ? __ldg(e.row_blk + q) * e.row_mod : 0);
+    const float4* b4 = reinterpret_cast<const float4*>(e.row_bias + (int64_t)brow * N + col0);
 #pragma unroll
     for (int i = 0; i < CW / 4; ++i) {
       float4 b = __ldg(b4 + i);
@@ -260,6 +262,9 @@ gemm_split3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
 // so one 128 x 144 output tile holds everything head h needs for the tracks of a row tile.  Token rows are
 // track-major (row = n*T + t): a tile starts at row mt*R with R = floor(128 / T) * T, i.e. it owns whole tracks
 // (the MMA still multiplies 128 rows; the rows past R belong to the next tile and are ignored).
+// With a per-track length table (ct3_loop_shape.group_T) track i attends over its first track_len[i] <= T frames only:
+// the key loop ends there, so a track's result is that of a pass with T = track_len[i].  T > 128 is then allowed for
+// tracks of at most 128 frames: R = T, one track per tile, and only its first 128 rows are computed.
 // Three warpgroups: warps 0..3 MMA (wgmma m64n144k16 on both 64-row halves: 144 fp32 accumulators per thread),
 // warps 4..7 producer (warp 4 issues the TMA loads), warps 8..11 epilogue (thread = row of the tile).  setmaxnreg moves
 // registers from the producer warpgroup (40) to the other two (232 each) so that neither spills and the wgmmas are not
@@ -288,7 +293,8 @@ static_assert(SMEM <= 232448, "shared memory budget");
 
 __global__ void __launch_bounds__(qa::NTHREADS, 1)
 gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, int M,
-                          int Kpad, int T, int R, float scale_log2e, GemmEpilogue epi) {
+                          int Kpad, int T, int R, const int32_t* __restrict__ track_len, float scale_log2e,
+                          GemmEpilogue epi) {
   using namespace qa;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_align1024(smem_raw);
@@ -401,11 +407,14 @@ gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
       }
       named_bar_sync(1, EPIW * 32);                  // K/V of this tile are final in shared memory
       {
+        // the track's own length; a clamped track past M reads the last one (its rows are never stored).  Lengths
+        // are at most min(T, 128) (gemm.cuh); the clamp keeps every key read inside this tile regardless
+        const int Tk = track_len ? min(track_len[min(mt * tracks + jtrack, M / T - 1)], min(T, BM)) : T;
         float m = -INFINITY, l = 0.f;
         float o[kDh];
 #pragma unroll
         for (int i = 0; i < kDh; ++i) o[i] = 0.f;
-        for (int t0 = 0; t0 < T; t0 += 8) {
+        for (int t0 = 0; t0 < Tk; t0 += 8) {
           float sc[8];
 #pragma unroll
           for (int i = 0; i < 8; ++i) sc[i] = 0.f;
@@ -413,7 +422,7 @@ gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
           for (int d4 = 0; d4 < kDh / 4; ++d4) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
-              const float4 kk = *reinterpret_cast<const float4*>(kbase + min(t0 + i, T - 1) * QACC_LD + 4 * d4);
+              const float4 kk = *reinterpret_cast<const float4*>(kbase + min(t0 + i, Tk - 1) * QACC_LD + 4 * d4);
               sc[i] = fmaf(xq[4 * d4 + 0], kk.x, sc[i]);
               sc[i] = fmaf(xq[4 * d4 + 1], kk.y, sc[i]);
               sc[i] = fmaf(xq[4 * d4 + 2], kk.z, sc[i]);
@@ -423,7 +432,7 @@ gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
           float mnew = m;
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
-            sc[i] = (t0 + i < T) ? sc[i] * scale_log2e : -INFINITY;
+            sc[i] = (t0 + i < Tk) ? sc[i] * scale_log2e : -INFINITY;
             mnew = fmaxf(mnew, sc[i]);
           }
           const float corr = exp2f(m - mnew);          // exp2(-inf) = 0 on the first chunk
@@ -434,7 +443,7 @@ gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
           for (int i = 0; i < 8; ++i) {
             const float pi = exp2f(sc[i] - mnew);      // 0 for the masked tail
             l += pi;
-            const float* vr = kbase + min(t0 + i, T - 1) * QACC_LD + kDh;
+            const float* vr = kbase + min(t0 + i, Tk - 1) * QACC_LD + kDh;
 #pragma unroll
             for (int d4 = 0; d4 < kDh / 4; ++d4) {
               const float4 vv = *reinterpret_cast<const float4*>(vr + 4 * d4);
@@ -470,7 +479,11 @@ gemm_qkv_time_attn_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
 // SIMT verification kernel: 64x64 tile, 256 threads, each 4x4 outputs; fp32 FMA on hi+lo.
 __device__ __forceinline__ void epilogue_store1(const GemmEpilogue& e, int N, int row, int col, float v) {
   if (e.bias) v += e.bias[col];
-  if (e.row_bias) v += e.row_bias[(int64_t)(row % e.row_mod) * N + col];
+  if (e.row_bias) {
+    int64_t brow = row % e.row_mod;
+    if (e.row_blk) brow += (int64_t)e.row_blk[row / e.row_mod] * e.row_mod;
+    v += e.row_bias[brow * N + col];
+  }
   v = apply_act(v, e.act);
   if (e.out_f32) {
     float* o = e.out_f32 + (int64_t)row * e.ld_f32 + col;
@@ -597,11 +610,13 @@ cudaError_t launch_tc(const GemmProblem& p, const CUtensorMap& tmX, const CUtens
 bool qkv_time_attn_supported(int T) { return T >= 1 && T <= BM; }
 
 int gemm_qkv_time_attn_launch(const __nv_bfloat16* x_split, const __nv_bfloat16* w_heads, const float* bias_heads,
-                              int M, int Kpad, int T, __nv_bfloat16* att_split, int64_t ld_split, int lo_off,
-                              float scale, int num_sms, cudaStream_t stream, const char** err) {
+                              int M, int Kpad, int T, const int32_t* track_len, __nv_bfloat16* att_split,
+                              int64_t ld_split, int lo_off, float scale, int num_sms, cudaStream_t stream,
+                              const char** err) {
   *err = nullptr;
-  if (M <= 0 || Kpad <= 0 || (Kpad % BK) != 0 || !qkv_time_attn_supported(T) || (M % T) != 0) {
-    *err = "qkv_time_attn: need M > 0, M % T == 0, 1 <= T <= 128, Kpad % 64 == 0";
+  if (M <= 0 || Kpad <= 0 || (Kpad % BK) != 0 || T < 1 || (!track_len && !qkv_time_attn_supported(T)) ||
+      (M % T) != 0) {
+    *err = "qkv_time_attn: need M > 0, M % T == 0, 1 <= T <= 128 (any T with track lengths), Kpad % 64 == 0";
     return (int)cudaErrorInvalidValue;
   }
   if (((reinterpret_cast<uintptr_t>(x_split) | reinterpret_cast<uintptr_t>(w_heads) |
@@ -609,7 +624,7 @@ int gemm_qkv_time_attn_launch(const __nv_bfloat16* x_split, const __nv_bfloat16*
     *err = "qkv_time_attn: operands must be 16-byte aligned";
     return (int)cudaErrorInvalidValue;
   }
-  const int R = (BM / T) * T;
+  const int R = T <= BM ? (BM / T) * T : T;
   CUtensorMap tmX, tmW;
   if (!make_tmap(&tmX, x_split, (uint64_t)M, 2ull * Kpad) ||
       !make_tmap(&tmW, w_heads, (uint64_t)(kHeads * qa::BNQ), 2ull * Kpad, (uint32_t)qa::BNQ)) {
@@ -628,7 +643,7 @@ int gemm_qkv_time_attn_launch(const __nv_bfloat16* x_split, const __nv_bfloat16*
   epi.ld_split = ld_split;
   epi.lo_off = lo_off;
   gemm_qkv_time_attn_kernel<<<num_tiles < num_sms ? num_tiles : num_sms, qa::NTHREADS, qa::SMEM, stream>>>(
-      tmX, tmW, M, Kpad, T, R, scale * 1.44269504088896340736f, epi);
+      tmX, tmW, M, Kpad, T, R, track_len, scale * 1.44269504088896340736f, epi);
   return (int)cudaGetLastError();
 }
 

@@ -14,6 +14,9 @@ struct GemmEpilogue {
   const float* bias = nullptr;      // [N]
   const float* row_bias = nullptr;  // [row_mod, N]; row r adds row_bias[(r % row_mod)]   (time-embedding fold)
   int row_mod = 1;
+  // [M / row_mod] or null: row r adds row_bias[row_blk[r / row_mod] * row_mod + r % row_mod] instead (one bias block of
+  // row_mod rows per track: the time embedding of the track's group, ct3_loop_shape.group_T)
+  const int32_t* row_blk = nullptr;
   int act = 0;                      // 0 none | 1 GELU(erf) | 2 GELU(tanh)
   // fp32 output (optional): out_f32[r*ld_f32 + c] = v   or  += v  when residual
   float* out_f32 = nullptr;
@@ -57,9 +60,13 @@ int gemm_launch(const GemmProblem& p, int impl, int num_sms, cudaStream_t stream
 //   x_split [M, 2*Kpad] (LayerNorm output, rows track-major n*T + t, M % T == 0), w_heads [8*144, 2*Kpad] with the
 //   rows of head h = [q_h | k_h | v_h], bias_heads [8*144] likewise; att_split[row*ld_split + h*48 + c] (hi) and
 //   + lo_off (lo) = softmax(q k^T scale) v.   T <= 128.
+//   track_len [M / T] or null: track i attends over its first track_len[i] frames only (every row of it, its padded
+//   rows too).  With it T may exceed 128 when every track_len is <= 128: each track is then a tile of its own and only
+//   its first 128 rows are written.  The kernel clamps a length to min(T, 128) so that no key is read outside its tile.
 bool qkv_time_attn_supported(int T);
 int gemm_qkv_time_attn_launch(const __nv_bfloat16* x_split, const __nv_bfloat16* w_heads, const float* bias_heads,
-                              int M, int Kpad, int T, __nv_bfloat16* att_split, int64_t ld_split, int lo_off,
-                              float scale, int num_sms, cudaStream_t stream, const char** err);
+                              int M, int Kpad, int T, const int32_t* track_len, __nv_bfloat16* att_split,
+                              int64_t ld_split, int lo_off, float scale, int num_sms, cudaStream_t stream,
+                              const char** err);
 
 }  // namespace ct3

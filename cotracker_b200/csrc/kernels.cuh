@@ -162,9 +162,10 @@ cudaError_t launch_corr_patch_t(const __nv_bfloat16* pyr_half, int H4, int W4, c
 // ---- tokens.cu : elementwise / row-wise pieces of the transformer ---------------------------------
 cudaError_t launch_layernorm_split(const float* x, int rows, const float* gamma, const float* beta, float eps,
                                    __nv_bfloat16* out_split, cudaStream_t s);
-// the X rows of tracks [n0, n0 + count) of the [T, N] state into x_split from row 0
+// the X rows of tracks [n0, n0 + count) of the [T, N] state into x_split from row 0; track_len [N] or null: track n's
+// forward relative motion ends at its own last frame track_len[n] - 1 (ct3_loop_shape.group_T)
 cudaError_t launch_build_x_small(const float* coords, const float* vis, const float* conf, int T, int N, int n0,
-                                 int count, __nv_bfloat16* x_split, cudaStream_t s);
+                                 int count, const int32_t* track_len, __nv_bfloat16* x_split, cudaStream_t s);
 // one copy of the kV virtual tokens per group: rows (N + kV*g + i)*T + t, g < G
 cudaError_t launch_init_virtual(float* tokens, const float* virt, int T, int N, int G, cudaStream_t s);
 // host int32 array -> device, stream-ordered (kernel arguments carry the values: src may be freed on return)
@@ -200,6 +201,9 @@ struct AttnParams {
   // attention_p2v.cu: [tiles] (group, first track) of each 128-track tile; Lq = all tracks, Lk = kV * groups
   const int32_t* gtile;
   int tiles;
+  // Ungrouped calls only: [num_seq] key counts or null (all Lk).  Sequence s attends over its first seq_len[s] <= Lk
+  // keys; every one of its Lq queries is computed (time attention of a pass with ct3_loop_shape.group_T).
+  const int32_t* seq_len;
 };
 // rows and lengths of sequence s (grouped or not)
 struct SeqRows { int64_t q0, k0; int Lq, Lk, e, t; };
@@ -207,7 +211,7 @@ __device__ __forceinline__ SeqRows seq_rows(const AttnParams& p, int s) {
   SeqRows r;
   if (!p.gl) {
     r.q0 = (int64_t)s * p.q_seq_stride; r.k0 = (int64_t)s * p.k_seq_stride;
-    r.Lq = p.Lq; r.Lk = p.Lk; r.e = 0; r.t = s;
+    r.Lq = p.Lq; r.Lk = p.seq_len ? p.seq_len[s] : p.Lk; r.e = 0; r.t = s;
     return r;
   }
   r.e = s / p.frames;

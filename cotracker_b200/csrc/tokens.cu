@@ -53,9 +53,10 @@ layernorm_split_kernel(const float* __restrict__ x, int rows, const float* __res
 // block = one (n,t) row, 128 threads = X columns 1024..1151: [vis, conf, posenc(84), zero pad(42)]
 __global__ void __launch_bounds__(128)
 build_x_small_kernel(const float* __restrict__ coords, const float* __restrict__ vis, const float* __restrict__ conf,
-                     int T, int N, __nv_bfloat16* __restrict__ xs) {
+                     int T, int N, const int32_t* __restrict__ track_len, __nv_bfloat16* __restrict__ xs) {
   const int row = blockIdx.x;  // n*T + t
   const int n = row / T, t = row % T;
+  const int Tn = track_len ? track_len[n] : T;   // the track's own length: its last real frame gets the zero pad
   const int c = threadIdx.x;
   float val = 0.f;
   if (c == 0) {
@@ -74,7 +75,7 @@ build_x_small_kernel(const float* __restrict__ coords, const float* __restrict__
     float u = 0.f;
     const float here = coords[((int64_t)t * N + n) * 2 + axis];
     if (fwd) {
-      if (t + 1 < T) u = here - coords[((int64_t)(t + 1) * N + n) * 2 + axis];
+      if (t + 1 < Tn) u = here - coords[((int64_t)(t + 1) * N + n) * 2 + axis];
     } else {
       if (t > 0) u = here - coords[((int64_t)(t - 1) * N + n) * 2 + axis];
     }
@@ -199,9 +200,10 @@ cudaError_t launch_layernorm_split(const float* x, int rows, const float* gamma,
   return cudaGetLastError();
 }
 cudaError_t launch_build_x_small(const float* coords, const float* vis, const float* conf, int T, int N, int n0,
-                                 int count, __nv_bfloat16* x_split, cudaStream_t s) {
+                                 int count, const int32_t* track_len, __nv_bfloat16* x_split, cudaStream_t s) {
   // the kernel's track n is track n0 + n of the [T, N] state: same pitch, base moved to track n0
-  build_x_small_kernel<<<count * T, 128, 0, s>>>(coords + (int64_t)n0 * 2, vis + n0, conf + n0, T, N, x_split);
+  build_x_small_kernel<<<count * T, 128, 0, s>>>(coords + (int64_t)n0 * 2, vis + n0, conf + n0, T, N,
+                                                 track_len ? track_len + n0 : nullptr, x_split);
   return cudaGetLastError();
 }
 cudaError_t launch_init_virtual(float* tokens, const float* virt, int T, int N, int G, cudaStream_t s) {

@@ -39,7 +39,8 @@ class LoopShape(ctypes.Structure):
     """ct3_loop_shape (include/ct3_b200.h): one update-loop pass."""
     _fields_ = [("T", ctypes.c_int), ("N", ctypes.c_int), ("H4", ctypes.c_int), ("W4", ctypes.c_int),
                 ("G", ctypes.c_int), ("group_sizes", ctypes.POINTER(ctypes.c_int32)), ("T_pyr", ctypes.c_int),
-                ("group_frames", ctypes.POINTER(ctypes.c_int32)), ("slab_tracks", ctypes.c_int)]
+                ("group_frames", ctypes.POINTER(ctypes.c_int32)), ("slab_tracks", ctypes.c_int),
+                ("group_T", ctypes.POINTER(ctypes.c_int32))]
 
 
 def _signatures():
@@ -478,17 +479,24 @@ def sample_support(pyr, T, H4, W4, qframes, qcoords, support=None, accumulate_ma
     return support
 
 
-def _loop_shape(T, N, H4, W4, G=1, sizes=None, T_pyr=None, frames=None, slab_tracks=None) -> LoopShape:
-    """ct3_loop_shape of a pass; None = the field's default (no map, no slabs)."""
-    return LoopShape(int(T), int(N), int(H4), int(W4), int(G), sizes, int(T_pyr or 0), frames, int(slab_tracks or 0))
+def _loop_shape(T, N, H4, W4, G=1, sizes=None, T_pyr=None, frames=None, slab_tracks=None, lengths=None) -> LoopShape:
+    """ct3_loop_shape of a pass; None = the field's default (no map, no slabs, every group of length T)."""
+    return LoopShape(int(T), int(N), int(H4), int(W4), int(G), sizes, int(T_pyr or 0), frames, int(slab_tracks or 0),
+                     lengths)
 
 
 def workspace_bytes(T: int, N: int, H4: int = 0, W4: int = 0, groups: int = 1, frames: Optional[int] = None,
-                    slab_tracks: Optional[int] = None) -> int:
+                    slab_tracks: Optional[int] = None, group_T: Optional[Sequence[int]] = None) -> int:
     """Scratch of ct3_update_loop for T frames of H4 x W4 feature maps and N tracks (H4 = W4 = 0: updateformer only),
     split into `groups` track groups.  frames: the T_pyr pyramid frames of a pass with a frame map.  slab_tracks: the
-    loop in track slabs of that many tracks."""
-    shape = _loop_shape(T, N, H4, W4, groups, None, frames, None, slab_tracks)
+    loop in track slabs of that many tracks.  group_T: the `groups` group lengths of a pass whose groups differ in
+    length (ct3_loop_shape.group_T)."""
+    lengths = None
+    if group_T is not None:
+        lengths, n_len = _group_array(group_T)
+        if n_len != groups:
+            raise EngineError(f"group_T has {n_len} entries for {groups} groups")
+    shape = _loop_shape(T, N, H4, W4, groups, None, frames, None, slab_tracks, lengths)
     return _size("ct3_workspace_bytes", ctypes.byref(shape))
 
 
@@ -518,8 +526,9 @@ class WorkspaceCache:
         self.buf: Optional[torch.Tensor] = None
 
     def get(self, T: int, N: int, device, H4: int = 0, W4: int = 0, groups: int = 1,
-            frames: Optional[int] = None, slab_tracks: Optional[int] = None) -> torch.Tensor:
-        need = workspace_bytes(T, N, H4, W4, groups, frames, slab_tracks)
+            frames: Optional[int] = None, slab_tracks: Optional[int] = None,
+            group_T: Optional[Sequence[int]] = None) -> torch.Tensor:
+        need = workspace_bytes(T, N, H4, W4, groups, frames, slab_tracks, group_T)
         if self.buf is None or self.buf.numel() < need or self.buf.device != torch.device(device):
             self.buf = None
             self.buf = torch.empty(need, dtype=torch.uint8, device=device)
@@ -540,7 +549,8 @@ def _frame_array(group_frames, G: int, T: int):
 
 
 def update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, time_emb, iters, workspace,
-                group_sizes: Optional[Sequence[int]] = None, group_frames=None, slab_tracks: Optional[int] = None):
+                group_sizes: Optional[Sequence[int]] = None, group_frames=None, slab_tracks: Optional[int] = None,
+                group_T: Optional[Sequence[int]] = None):
     """In-place refinement of coords [T,N,2], vis [T,N], conf [T,N] (fp32, feature-grid units / logits).
     One ct3_update_loop call with the ct3_loop_shape the arguments describe.
     group_sizes: the N tracks as contiguous independent groups; each group's result is bit-identical to a call on its
@@ -549,20 +559,29 @@ def update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, ti
     frames) at time step t; each group's result is bit-identical to a call on a pyramid of exactly those frames.
     None = frame t.
     slab_tracks: run in track slabs of that many tracks in a workspace of workspace_bytes(..., slab_tracks=);
-    bit-identical to the call without.  None = no slabs."""
+    bit-identical to the call without.  None = no slabs.
+    group_T: G group lengths in [1, T]: group g tracks a clip of group_T[g] frames padded to T, and its rows t < group_T[g]
+    are bit-identical to a call on its tracks alone with T = group_T[g]; time_emb is then [G, T, 1110], group g's time
+    embedding in rows [0, group_T[g]).  None = every group has length T."""
     _req(coords, torch.float32, "coords"); _req(vis, torch.float32, "vis"); _req(conf, torch.float32, "conf")
     _req(pyr, torch.float32, "pyr"); _req(support, torch.float32, "support"); _req(time_emb, torch.float32, "time_emb")
     T, N, _ = coords.shape
-    if time_emb.shape != (T, XDIM):
-        raise EngineError(f"time_emb must be [{T},{XDIM}]")
+    arr, G = _group_array(group_sizes if group_sizes is not None else [N])
+    lengths = None
+    if group_T is not None:
+        lengths, n_len = _group_array(group_T)
+        if n_len != G:
+            raise EngineError(f"group_T has {n_len} entries for {G} groups")
+    want = (T, XDIM) if group_T is None else (G, T, XDIM)
+    if tuple(time_emb.shape) != want:
+        raise EngineError(f"time_emb must be [{','.join(map(str, want))}]")
     if track_valid is not None:
         _req(track_valid, torch.uint8, "track_valid")
-    arr, G = _group_array(group_sizes if group_sizes is not None else [N])
     if group_frames is None:
         T_pyr, fr = None, None
     else:
         T_pyr, fr = pyramid_frames(pyr, H4, W4), _frame_array(group_frames, G, T)
-    shape = _loop_shape(T, N, H4, W4, G, arr, T_pyr, fr, slab_tracks)
+    shape = _loop_shape(T, N, H4, W4, G, arr, T_pyr, fr, slab_tracks, lengths)
     _call("ct3_update_loop", coords.device, _ptr(packed), _ptr(pyr), _ptr(support), _ptr(track_valid), _ptr(coords),
           _ptr(vis), _ptr(conf), _ptr(time_emb), int(iters), ctypes.byref(shape), _ptr(workspace), workspace.numel(),
           _stream(coords.device))

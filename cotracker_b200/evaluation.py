@@ -78,12 +78,14 @@ def points_on_a_grid(size: int, extent, center=None, device="cpu") -> torch.Tens
     return torch.stack([gx, gy], dim=-1).reshape(1, -1, 2)
 
 
-def pass_bytes(T: int, N: int, G: int, H4: int, W4: int, frames: Optional[int] = None) -> int:
+def pass_bytes(T: int, N: int, G: int, H4: int, W4: int, frames: Optional[int] = None, ragged: bool = False) -> int:
     """Device memory of one grouped update-loop pass over N tracks in G groups and T frames: the library workspace
     plus the per-track support features [4,49,N,128] and the per-frame state and outputs (about 16 floats).
-    frames: the pyramid frames of a pass with a frame map (engine.workspace_bytes)."""
+    frames: the pyramid frames of a pass with a frame map (engine.workspace_bytes).  ragged: the groups have lengths of
+    their own (ct3_loop_shape.group_T), which adds a time embedding per group."""
     from . import engine
-    return engine.workspace_bytes(T, N, H4, W4, groups=G, frames=frames) + N * (4 * 49 * 128 * 4 + T * 16 * 4)
+    ws = engine.workspace_bytes(T, N, H4, W4, groups=G, frames=frames, group_T=[T] * G if ragged else None)
+    return ws + N * (4 * 49 * 128 * 4 + T * 16 * 4) + (G * T * 1110 * 4 if ragged else 0)
 
 
 def pass_budget_bytes(model, device, T: int, ih: int, iw: int) -> int:
@@ -101,18 +103,20 @@ def pass_budget_bytes(model, device, T: int, ih: int, iw: int) -> int:
     return int(0.9 * max(0, free - reserve))
 
 
-def slab_tracks_for(T: int, N: int, G: int, H4: int, W4: int, frames: Optional[int], budget_bytes: int) -> Optional[int]:
+def slab_tracks_for(T: int, N: int, G: int, H4: int, W4: int, frames: Optional[int], budget_bytes: int,
+                    group_T: Optional[Sequence[int]] = None) -> Optional[int]:
     """Track slabs of one update-loop pass (ct3_loop_shape.slab_tracks, DESIGN.md §4.4.5): None when the full workspace
     fits `budget_bytes`, so every pass that fits runs exactly as without slabs; else the largest slab_tracks whose
     workspace fits (the workspace never shrinks as slab_tracks grows), or 1 when none does.
-    frames: the pyramid frames of a pass with a frame map (engine.workspace_bytes)."""
+    frames: the pyramid frames of a pass with a frame map; group_T: its group lengths (engine.workspace_bytes)."""
     from . import engine
-    if engine.workspace_bytes(T, N, H4, W4, groups=G, frames=frames) <= budget_bytes:
+    if engine.workspace_bytes(T, N, H4, W4, groups=G, frames=frames, group_T=group_T) <= budget_bytes:
         return None
     lo, hi = 1, max(1, N - 1)
     while lo < hi:
         mid = (lo + hi + 1) // 2
-        if engine.workspace_bytes(T, N, H4, W4, groups=G, frames=frames, slab_tracks=mid) <= budget_bytes:
+        if engine.workspace_bytes(T, N, H4, W4, groups=G, frames=frames, slab_tracks=mid,
+                                  group_T=group_T) <= budget_bytes:
             lo = mid
         else:
             hi = mid - 1
@@ -171,6 +175,36 @@ def plan_clip_passes(n_clips: int, group_sizes: Sequence[int], T: int, H4: int, 
     if not ragged and passes:   # same cost per clip: spread the clips evenly over as many passes
         per = -(-n_clips // len(passes))
         passes = [(b0, min(n_clips, b0 + per)) for b0 in range(0, n_clips, per)]
+    return passes
+
+
+def plan_ragged_passes(lengths: Sequence[int], tracks: Sequence[int], groups: Sequence[int], H4: int, W4: int,
+                       budget_bytes: int, pad_fraction: float, frames: int, pad_rows: int = 0) -> List[List[int]]:
+    """Passes of clips of different lengths (`CoTrackerPredictor` on a list): clip b has lengths[b] frames, tracks[b]
+    tracks in all and groups[b] query groups.  The clips are taken shortest first; a pass pads every clip to its
+    longest one.  Padding is counted in token rows: each clip's point tracks and the 64 virtual tracks of each of its
+    groups, times the frames it is padded by.  A new pass starts when the next clip would take the pass past
+    `budget_bytes` (`pass_bytes` with group lengths, `frames` pyramid frames), or its padded token rows past
+    pad_fraction times its real ones plus pad_rows.  A pure host function: -> the clips of each pass (indices into
+    `lengths`), shortest first; a clip that alone exceeds the budget gets a pass of its own.  Groups are independent,
+    so the split changes no result."""
+    if not (len(lengths) == len(tracks) == len(groups)):
+        raise ValueError(f"{len(lengths)} lengths, {len(tracks)} track counts and {len(groups)} group counts")
+    rows = [tracks[b] + 64 * groups[b] for b in range(len(lengths))]   # token rows per frame
+    order = sorted(range(len(lengths)), key=lambda b: (lengths[b], b))
+    passes: List[List[int]] = []
+    cur: List[int] = []
+    for b in order:
+        if cur:
+            T, N, G = lengths[b], sum(tracks[c] for c in cur) + tracks[b], sum(groups[c] for c in cur) + groups[b]
+            real = sum(rows[c] * lengths[c] for c in cur + [b])
+            padded = sum(rows[c] for c in cur + [b]) * T - real
+            if pass_bytes(T, N, G, H4, W4, frames, ragged=True) > budget_bytes or padded > pad_fraction * real + pad_rows:
+                passes.append(cur)
+                cur = []
+        cur.append(b)
+    if cur:
+        passes.append(cur)
     return passes
 
 

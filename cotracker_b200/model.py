@@ -105,6 +105,17 @@ def window_frame_map(T: int, S: int, ind: int, reversed_groups) -> List[List[int
     return [[max(T - 1 - ind - t, 0) for t in range(S)] if r else [ind + t for t in range(S)] for r in reversed_groups]
 
 
+def ragged_frame_map(T: int, groups) -> List[List[int]]:
+    """Pass of clips of different lengths in one pyramid: groups = (first pyramid frame f0 of the clip, its length T_g,
+    reversed) per group.  A group reads f0 + t (f0 + T_g-1-t reversed) and, at its padded steps t >= T_g, the frame of
+    its last real step, as the sliding-window model clamps its padded window."""
+    rows = []
+    for f0, T_g, rev in groups:
+        row = [f0 + (T_g - 1 - t if rev else t) for t in range(T_g)]
+        rows.append(row + [row[-1]] * (T - T_g))
+    return rows
+
+
 def gather_plan(frame_map):
     """The runs [a, b) of consecutive frames a frame map references, in order, and the map remapped into the pyramid
     that concatenates those runs (each referenced frame once)."""
@@ -352,15 +363,24 @@ class CoTrackerThreeBase(nn.Module):
             self._fingerprint, self._fingerprint_key = h.hexdigest(), key
         return self._fingerprint
 
+    TIME_EMBED_CACHE = 64   # lengths whose interpolated time embedding is kept (a list call needs one per length)
+
     def interpolate_time_embed(self, t: int) -> torch.Tensor:
-        """[t, 1110] time embedding (reference cotracker3_online.py:145-156); constant per (buffer, t): cached."""
-        key = (t, self.time_emb.data_ptr(), self.time_emb._version, str(self.time_emb.device))
-        if getattr(self, "_te_key", None) != key:
+        """[t, 1110] time embedding (reference cotracker3_online.py:145-156); constant per (buffer, t): cached per
+        length, for the last TIME_EMBED_CACHE lengths."""
+        buf = (self.time_emb.data_ptr(), self.time_emb._version, str(self.time_emb.device))
+        cache = getattr(self, "_te_cache", None)
+        if not isinstance(cache, dict) or getattr(self, "_te_key", None) != buf:
+            cache, self._te_key = {}, buf
+            self._te_cache = cache
+        if t not in cache:
             te = self.time_emb.float()
             if t != te.shape[1]:
                 te = F.interpolate(te.permute(0, 2, 1), size=t, mode="linear").permute(0, 2, 1)
-            self._te_cache, self._te_key = te[0].contiguous(), key
-        return self._te_cache
+            if len(cache) >= self.TIME_EMBED_CACHE:
+                del cache[next(iter(cache))]
+            cache[t] = te[0].contiguous()
+        return cache[t]
 
     def _encode(self, video: torch.Tensor, chunk: int) -> torch.Tensor:
         """video [T,3,H,W] already scaled to [-1,1] -> L2-normalised channels-last 4-level pyramid (flat fp32).
@@ -393,8 +413,10 @@ class CoTrackerThreeBase(nn.Module):
         if not video.is_cuda:
             raise engine.EngineError("cotracker_b200 runs on CUDA only; move the module and inputs to a GPU")
 
-    def _refine(self, pyr, H4, W4, support, track_valid, coords, vis, conf, iters, group_sizes, group_frames=None):
+    def _refine(self, pyr, H4, W4, support, track_valid, coords, vis, conf, iters, group_sizes, group_frames=None,
+                group_T=None):
         """group_frames: [G, T] frame map into `pyr` (ct3_loop_shape.group_frames), None = frame t.
+        group_T: G group lengths (ct3_loop_shape.group_T), None = every group has T frames.
         A pass whose full workspace exceeds the pass budget runs in the largest track slabs that fit
         (ct3_loop_shape.slab_tracks, bit-identical); every other pass runs as it always did."""
         T, N, _ = coords.shape
@@ -403,11 +425,18 @@ class CoTrackerThreeBase(nn.Module):
         T_all = engine.pyramid_frames(pyr, H4, W4)
         T_pyr = None if group_frames is None else T_all
         budget = pass_budget_bytes(self, dev, T_all, H4 * self.stride, W4 * self.stride)
-        slab = slab_tracks_for(T, N, G, H4, W4, T_pyr, budget)
+        slab = slab_tracks_for(T, N, G, H4, W4, T_pyr, budget, group_T)
+        if group_T is None:
+            time_emb = self.interpolate_time_embed(T).to(dev)
+        else:   # each group's own embedding, zero rows past its length
+            time_emb = torch.zeros(G, T, XDIM, device=dev)
+            for g, t in enumerate(group_T):
+                time_emb[g, :t] = self.interpolate_time_embed(t).to(dev)
+        ws = (self._ws.get(T, N, dev, H4, W4, G, T_pyr, slab) if group_T is None
+              else self._ws.get(T, N, dev, H4, W4, G, T_pyr, slab, group_T))
         engine.update_loop(self.packed_weights(dev), pyr, H4, W4, support, track_valid, coords, vis, conf,
-                           self.interpolate_time_embed(T).to(dev), iters,
-                           self._ws.get(T, N, dev, H4, W4, G, T_pyr, slab),
-                           group_sizes=group_sizes, group_frames=group_frames, slab_tracks=slab)
+                           time_emb, iters, ws,
+                           group_sizes=group_sizes, group_frames=group_frames, slab_tracks=slab, group_T=group_T)
 
     @staticmethod
     def _track_reversed(group_sizes, flags, device) -> torch.Tensor:
@@ -534,6 +563,39 @@ class CoTrackerThreeOffline(CoTrackerThreeBase):
         self._refine(pyr, H4, W4, support, None, coords, vis, conf, iters, group_sizes * B, frame_map)
         return (self._batched(coords * float(self.stride), B), self._batched(torch.sigmoid(vis), B),
                 self._batched(torch.sigmoid(conf), B), None)
+
+
+    def _track_ragged(self, pyr, H, W, groups, iters):
+        """One update-loop pass over query groups of clips of different lengths in one pyramid (`_encode_clip` of
+        the clips one after another, H x W frames).  groups: (queries [1,n,3] at model resolution in the group's own
+        clip time, first pyramid frame f0 of its clip, clip length T_g, reversed) per group; a reversed group tracks its
+        clip played backwards and reads the forward pyramid through its frame map.  The pass pads every group to the
+        longest T_g (ct3_loop_shape.group_T); a padded step reads its group's last frame.
+        -> [(tracks [1,T_g,n,2] at model resolution, visibility [1,T_g,n])] per group, each bit-identical to the
+        one-clip pass on that group (`_track_pyramid`)."""
+        dev = pyr.device
+        H4, W4 = H // self.stride, W // self.stride
+        T = max(g[2] for g in groups)
+        sizes = [q.shape[1] for q, *_ in groups]
+        lengths = [int(T_g) for _, _, T_g, _ in groups]
+        qframes = []
+        for q, f0, T_g, rev in groups:
+            qf = q[0, :, 0].long()
+            qframes.append((T_g - 1 - qf if rev else qf) + f0)
+        frame_map = ragged_frame_map(T, [(f0, T_g, rev) for _, f0, T_g, rev in groups])
+        qframes = torch.cat(qframes).to(torch.int32).contiguous()
+        qcoords = (torch.cat([q[0, :, 1:3] for q, *_ in groups]).float() / self.stride).contiguous()
+        support = engine.sample_support(pyr, engine.pyramid_frames(pyr, H4, W4), H4, W4, qframes, qcoords)
+        N = qcoords.shape[0]
+        coords = qcoords[None].expand(T, N, 2).contiguous()
+        vis = torch.zeros(T, N, device=dev)
+        conf = torch.zeros(T, N, device=dev)
+        self._refine(pyr, H4, W4, support, None, coords, vis, conf, iters, sizes, frame_map, lengths)
+        out, a = [], 0
+        for n, T_g in zip(sizes, lengths):
+            out.append(((coords[:T_g, a:a + n] * float(self.stride))[None], torch.sigmoid(vis[:T_g, a:a + n])[None]))
+            a += n
+        return out
 
 
 class CoTrackerThreeOnline(CoTrackerThreeBase):

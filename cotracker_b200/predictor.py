@@ -10,6 +10,8 @@ machine.  The model behind it is `cotracker_b200.model` whose update loop runs i
 B clips of one length and size are tracked together (the reference fails for B > 1): one resize, one encoder pass and,
 memory permitting, one update-loop pass for the whole batch; slot b of the result is bit-identical to the call on
 `video[b:b+1]` (and `queries[b:b+1]`).  `segm_mask` keeps a different number of points per clip and is for B = 1 only.
+A list of [1,T_b,3,H_b,W_b] clips of any lengths and sizes (offline model, sparse queries) is tracked the same way, with
+per-clip `queries` / `segm_mask` lists; it returns lists, and entry b is bit-identical to the call on clip b alone.
 """
 from __future__ import annotations
 
@@ -18,13 +20,27 @@ import torch.nn.functional as F
 
 from . import engine, ingest
 from .build import build_cotracker
-from .evaluation import pass_budget_bytes, plan_clip_passes, plan_dense_passes
+from .evaluation import pass_budget_bytes, plan_clip_passes, plan_dense_passes, plan_ragged_passes
 
 # Backward tracking runs the forward and the reversed queries as two groups of one update-loop pass while one direction
 # has at most this many tracks x loop frames, and as two passes above it.  Measured on an H100 (DESIGN.md 4.4.2): one
 # pass is faster at 136 x 50 (-10 %) and 6436 x 16 (-2 %); at 6436 x 50 the loop is throughput-bound, one pass is not
 # faster (+0.3 %) and needs twice the update-loop workspace (45.8 instead of 24.6 GiB).
 BACKWARD_GROUP_TRACK_FRAMES = 1 << 17
+
+# A list call pads the clips of one update-loop pass to its longest clip, and starts a new pass before its padded token
+# rows (points and virtual tracks) exceed RAGGED_PAD_FRACTION times the real ones plus RAGGED_PAD_ROWS
+# (`plan_ragged_passes`).  Set by a sweep on an H100 (DESIGN.md 5.1, scripts/ragged_bench.py), 512x512 clips of 16-64
+# frames, clips/s against one call per clip:
+#   fraction       0      0.1    0.25   0.5    1     | rows 2^14  2^16
+#   8 clips, grid 10   -2 %   +4 %   +7 %   +7 %   -2 %  |   +6 %    -2 %
+#   32 clips, grid 10  -4 %   +8 %   +8 %   +7 %   -1 %  |   +8 %    +4 %
+#   8 clips, grid 30   -1 %   -1 %   -5 %   -9 %  -26 %  |   -4 %    -9 %
+# Padding pays where the loop is launch-bound (grid 10) and costs where it is throughput-bound (grid 30); 0.1 keeps
+# most of the gain at grid 10 for the smallest loss at grid 30.  A fixed row allowance (which favours small passes)
+# did no better than a fraction, so it is 0.
+RAGGED_PAD_FRACTION = 0.1
+RAGGED_PAD_ROWS = 0
 
 
 def get_points_on_a_grid(size: int, extent, device="cpu") -> torch.Tensor:
@@ -49,10 +65,13 @@ class CoTrackerPredictor(torch.nn.Module):
         self.interp_shape = model.model_resolution
         self.model = model
         self.model.eval()
+        self._list_budget_bytes = None   # device memory of one pass of a list call (None: from free device memory)
 
     @torch.no_grad()
     def forward(self, video, queries: torch.Tensor = None, segm_mask: torch.Tensor = None, grid_size: int = 0,
                 grid_query_frame: int = 0, backward_tracking: bool = False):
+        if isinstance(video, (list, tuple)):
+            return self._track_list(list(video), queries, segm_mask, grid_size, grid_query_frame, backward_tracking)
         if segm_mask is not None and video.shape[0] != 1:
             raise ValueError("segm_mask keeps a different number of grid points per clip: it needs B == 1")
         if queries is None and grid_size == 0:
@@ -61,6 +80,51 @@ class CoTrackerPredictor(torch.nn.Module):
         return self._compute_sparse_tracks(video, queries, segm_mask, grid_size,
                                            add_support_grid=(grid_size == 0 or segm_mask is not None),
                                            grid_query_frame=grid_query_frame, backward_tracking=backward_tracking)
+
+    def _track_list(self, clips, queries, segm_mask, grid_size, grid_query_frame, backward_tracking):
+        """Clips [1,T_b,3,H_b,W_b] of any lengths and sizes: one resize per clip into one frame buffer, one encoder
+        pass, and as few update-loop passes as the memory budget and RAGGED_PAD_FRACTION allow, each clip's groups
+        padded to the longest clip of their pass (ct3_loop_shape.group_T).  -> (tracks, visibility), lists in input
+        order, entry b bit-identical to the call on clip b with its own queries / segm_mask."""
+        B = len(clips)
+        _check_list_call(self.model, clips, queries, segm_mask, grid_size, grid_query_frame)
+        qs = [None] * B if queries is None else list(queries)
+        masks = [None] * B if segm_mask is None else list(segm_mask)
+        lengths = [int(c.shape[1]) for c in clips]
+        ih, iw = self.interp_shape
+        dev = ingest.model_device(self.model)
+        first = [sum(lengths[:b]) for b in range(B)]
+        frames = torch.empty(sum(lengths), 3, ih, iw, device=dev)
+        for b, clip in enumerate(clips):
+            ingest.prepare_video(clip, (ih, iw), dev, out=frames[first[b]:first[b] + lengths[b]])
+        pyr = self.model._encode_clip(frames)
+        del frames
+        at = _Device(dev)
+        add = [grid_size == 0 or m is not None for m in masks]
+        mq = [self._model_queries(at, c.shape, q, m, grid_size, a, grid_query_frame)
+              for c, q, m, a in zip(clips, qs, masks, add)]
+        groups = [[(q, first[b], lengths[b], False)] + ([(_reversed_queries(q, lengths[b]), first[b], lengths[b], True)]
+                                                         if backward_tracking else [])
+                  for b, q in enumerate(mq)]
+        s = self.model.stride
+        budget = self._list_budget_bytes
+        if budget is None:
+            budget = pass_budget_bytes(self.model, dev, sum(lengths), ih, iw)
+        passes = plan_ragged_passes(lengths, [sum(g[0].shape[1] for g in gs) for gs in groups],
+                                    [len(gs) for gs in groups], ih // s, iw // s, budget, RAGGED_PAD_FRACTION,
+                                    sum(lengths), RAGGED_PAD_ROWS)
+        outs = [None] * B
+        for p in passes:
+            res = self.model._track_ragged(pyr, ih, iw, [g for b in p for g in groups[b]], _EncodedClip.ITERS)
+            for b in p:
+                outs[b], res = res[:len(groups[b])], res[len(groups[b]):]
+        tracks, visibility = [], []
+        for b in range(B):
+            bwd = outs[b][1] if backward_tracking else None
+            tr, vi = self._finish(mq[b], outs[b][0], bwd, clips[b].shape, add[b])
+            tracks.append(tr)
+            visibility.append(vi)
+        return tracks, visibility
 
     def _compute_dense_tracks(self, video, grid_query_frame, grid_size=80, backward_tracking=False):
         """grid_step^2 shifted grids, one query group per offset (and one reversed group per offset with backward
@@ -152,6 +216,44 @@ class CoTrackerPredictor(torch.nn.Module):
         fwd, bwd = [None if p is None else (p[0].contiguous(), p[1].contiguous()) for p in (fwd, bwd)]
         return engine.finish_tracks(fwd, bwd, queries.float().contiguous(), n_keep, 0.9,
                                     ((W - 1) / (iw - 1), (H - 1) / (ih - 1)))
+
+
+class _Device:
+    """The device of a list call's clips, where `_model_queries` takes an `_EncodedClip`."""
+
+    def __init__(self, device):
+        self.device = device
+
+
+def _check_list_call(model, clips, queries, segm_mask, grid_size, grid_query_frame):
+    """The ValueErrors of a list call, raised before any work."""
+    if hasattr(model, "init_video_online_processing"):
+        raise ValueError("a list of clips needs the offline model (offline=True)")
+    B = len(clips)
+    if B == 0:
+        raise ValueError("the list of clips is empty")
+    for name, lst in (("queries", queries), ("segm_mask", segm_mask)):
+        if lst is not None and (not isinstance(lst, (list, tuple)) or len(lst) != B):
+            raise ValueError(f"{name} must be a list of {B} entries, one per clip")
+    for b, c in enumerate(clips):
+        if not torch.is_tensor(c) or c.dim() != 5 or c.shape[0] != 1 or c.shape[1] < 1 or c.shape[2] != 3:
+            raise ValueError(f"clip {b} must be a [1,T,3,H,W] tensor, got "
+                             f"{tuple(c.shape) if torch.is_tensor(c) else type(c).__name__}")
+    for b, c in enumerate(clips):
+        T = c.shape[1]
+        q = None if queries is None else queries[b]
+        if q is None:
+            if grid_size <= 0:
+                raise ValueError("a list of clips needs queries for every clip or grid_size > 0 "
+                                 "(dense mode takes one clip)")
+            if not 0 <= grid_query_frame < T:
+                raise ValueError(f"clip {b}: grid_query_frame {grid_query_frame} lies outside its {T} frames")
+            continue
+        if not torch.is_tensor(q) or q.dim() != 3 or q.shape[0] != 1 or q.shape[2] != 3:
+            raise ValueError(f"queries[{b}] must be a [1,N,3] tensor")
+        t = q[0, :, 0].long()
+        if t.numel() and (int(t.min()) < 0 or int(t.max()) >= T):
+            raise ValueError(f"clip {b}: a query frame lies outside its {T} frames")
 
 
 def _reversed_queries(queries, T: int):

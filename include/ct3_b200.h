@@ -298,9 +298,20 @@ int ct3_enc_tail(const void* packed, const float* cat, int T, int H4, int W4, fl
  * tracks alone (G = 1, no slabs) on a pyramid holding frames group_frames[g][0..T) in that order (without a map: the
  * same pyramid), whatever the other groups are; and BIT-IDENTICAL for every slab_tracks: slab_tracks >= N is the
  * launch sequence and workspace of slab_tracks = 0.
- * group_sizes and group_frames are HOST arrays and may be freed when the call returns: the device-side group table and
- * frame map live in the workspace and are filled in stream order (the library still allocates nothing).
- * Options: the default kernels and the exact-fp32 verification kernels ("gemm" / "corr" / "attn" = 1) support G > 1. */
+ *   group lengths: with group_T set, group g is a clip of group_T[g] steps padded to the pass's T.  Its steps
+ *                  [group_T[g], T) are padding: computed, with unspecified state.  Its time attention runs over its own
+ *                  steps only, its relative-motion posenc ends at its own last step, its time embedding is time_emb[g]
+ *                  and its space attention splits K as a pass of group_T[g] steps does.  Map its padded steps to real
+ *                  frames of its clip (e.g. the last one) in group_frames.  NULL is the launch sequence without the field.
+ * Contract with group_T: group g's coords/vis/conf at steps t < group_T[g] are BIT-IDENTICAL to a pass over that group
+ * alone with T = group_T[g], time embedding time_emb[g][0..group_T[g]) and frames group_frames[g][0..group_T[g]), with
+ * or without slabs.  A group of at most 128 steps takes the fused time attention whenever a pass of its own length
+ * would, also in a pass with T > 128.
+ * group_sizes, group_frames and group_T are HOST arrays and may be freed when the call returns: the device-side group
+ * table, frame map and per-track lengths live in the workspace and are filled in stream order (the library still
+ * allocates nothing).
+ * Options: the default kernels and the exact-fp32 verification kernels ("gemm" / "corr" / "attn" = 1) support G > 1
+ * and group_T, as does "fuse" = 0. */
 typedef struct ct3_loop_shape {
   int T, N;                       /* loop time steps, tracks (both >= 1)                                              */
   int H4, W4;                     /* level-0 feature map; 0, 0 = transformer only (ct3_updateformer sizing)           */
@@ -310,6 +321,7 @@ typedef struct ct3_loop_shape {
                                      >= 1: a frame map into T_pyr frames is given                                     */
   const int32_t* group_frames;    /* HOST [G*T] indices into [0, T_pyr) iff T_pyr >= 1, else NULL                     */
   int slab_tracks;                /* 0: no slabs; >= 1: track slabs, and then (N + 64 G) T <= 2^21                    */
+  const int32_t* group_T;         /* HOST [G] group lengths, each in [1, T], or NULL: every group has length T (102)  */
 } ct3_loop_shape;
 
 /* ct3_workspace_bytes: scratch needed by ct3_update_loop for `shape` (it includes the split-bf16 copy of the T_pyr
@@ -327,13 +339,15 @@ int ct3_workspace_bytes(const ct3_loop_shape* shape, size_t* out_bytes);
  *   coords   : [T,N,2] fp32 stride-4 feature units, in/out
  *   vis,conf : [T,N] fp32 logits, in/out
  *   time_emb : [T,1110] fp32 (buffer already interpolated to T,
- *              cotracker3_online.py:145-156)
+ *              cotracker3_online.py:145-156); with group_T [G,T,1110], group g's
+ *              interpolated to group_T[g] in rows [0, group_T[g])
  *   workspace: ct3_workspace_bytes(shape) bytes, 256-byte aligned
  * On return coords/vis/conf hold the state after the last iteration (the caller
  * multiplies coords by the stride and applies sigmoid, cotracker3_offline.py:213-216).
  * Every field of the shape is validated: a null pointer or shape, T or N < 1, G outside [1, N], a group size < 1, sizes
  * not summing to N, a null group_sizes with G > 1, T_pyr < 0, a frame map without T_pyr >= 1 or T_pyr >= 1 without
- * one, a frame index outside [0, T_pyr), slab_tracks < 0, more than 2^21 token rows with slabs, iters < 0, a bad
+ * one, a frame index outside [0, T_pyr), slab_tracks < 0, more than 2^21 token rows with slabs, a group_T entry outside
+ * [1, T] (ct3_workspace_bytes checks it too, and sizes the per-group tables when it is set), iters < 0, a bad
  * pyramid shape or a misaligned workspace return CT3_EINVAL, and a workspace smaller than the query CT3_ENOSPC, before
  * anything is enqueued. */
 int ct3_update_loop(const void* packed, const float* pyr, const float* support, const uint8_t* track_valid,
