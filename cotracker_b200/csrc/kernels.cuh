@@ -25,6 +25,10 @@ cudaError_t launch_pyramid_pools(int T, int H4, int W4, float* pyr, cudaStream_t
 // = 2 * (bilinear(align_corners=True) / 255) - 1, bit-identical to the ATen expression (see ingest.cu)
 cudaError_t launch_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t st, int64_t sc, int64_t sh,
                                   int64_t sw, int oh, int ow, float* out, cudaStream_t s);
+// the same of uint8 YUV frames (layout CT3_YUV_*, frame / row byte strides st, sr), converted to RGB as
+// cv2.cvtColor does: bit-identical to launch_prepare_frames on that uint8 RGB clip
+cudaError_t launch_prepare_frames_yuv(const uint8_t* src, int layout, int T, int H, int W, int64_t st, int64_t sr,
+                                      int oh, int ow, float* out, cudaStream_t s);
 
 // ---- finish.cu : the predictor's tail (arguments validated by ct3_finish_tracks) --------------------
 // forward (+ optional backward, reversed-clip time) tracks [B,T,N,2] / visibility probabilities [B,T,N], queries

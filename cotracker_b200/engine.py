@@ -63,6 +63,8 @@ def _signatures():
         "ct3_prepare_pyramid": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_prepare_frames": (c_int, [c_void_p, c_int, c_int, c_int, c_int, i64, i64, i64, i64, c_int, c_int, c_void_p,
                                        c_void_p]),
+        "ct3_prepare_frames_yuv": (c_int, [c_void_p, c_int, c_int, c_int, c_int, i64, i64, c_int, c_int, c_void_p,
+                                           c_void_p]),
         "ct3_finish_tracks": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                       ctypes.c_float, ctypes.c_float, ctypes.c_float, c_void_p, c_void_p, c_void_p]),
         "ct3_online_window_begin": (c_int, [ctypes.POINTER(OnlineStream), c_int, c_int, c_int, c_int, c_int, c_void_p,
@@ -275,6 +277,51 @@ def prepare_frames(src: torch.Tensor, out_hw, out: Optional[torch.Tensor] = None
         raise EngineError(f"out must be [{T},3,{oh},{ow}] on {src.device}")
     _call("ct3_prepare_frames", src.device, _ptr(src), FRAME_DTYPES[src.dtype], T, H, W, *src.stride(), oh, ow, _ptr(out),
           _stream(src.device))
+    return out
+
+
+YUV_LAYOUTS = {"nv12": 0, "i420": 1, "yuyv": 2}   # CT3_YUV_NV12, CT3_YUV_I420, CT3_YUV_YUYV
+
+
+def yuv_frame_hw(layout: str, shape) -> tuple:
+    """(H, W) of the frames of a YUV tensor whose last dimensions are one frame: [H*3/2, W] (nv12, i420) or [H, W, 2]
+    (yuyv); None when the shape is not one of those."""
+    if layout == "yuyv":
+        return (shape[-3], shape[-2]) if len(shape) >= 3 and shape[-1] == 2 else None
+    return (shape[-2] // 3 * 2, shape[-1]) if len(shape) >= 2 and shape[-2] % 3 == 0 else None
+
+
+def prepare_frames_yuv(src: torch.Tensor, layout: str, out_hw, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """src: T uint8 YUV frames on the device, [T,H*3/2,W] ("nv12", "i420") or [T,H,W,2] ("yuyv") -> [T,3,oh,ow] fp32,
+    bit-identical to prepare_frames on the uint8 RGB clip cv2.cvtColor(COLOR_YUV2RGB_*) makes of them
+    (ct3_prepare_frames_yuv in include/ct3_b200.h).  Any frame stride; NV12 and YUYV rows at any row stride (pitched surfaces), I420 frames
+    dense.  out: optional contiguous fp32 destination of that shape."""
+    if src.dtype != torch.uint8:
+        raise EngineError(f"YUV frames must be uint8, got {src.dtype}")
+    if layout not in YUV_LAYOUTS:
+        raise EngineError(f"unknown YUV layout {layout!r}: one of {sorted(YUV_LAYOUTS)}")
+    rank = 4 if layout == "yuyv" else 3
+    hw = yuv_frame_hw(layout, src.shape) if src.dim() == rank else None
+    if hw is None or src.shape[0] < 1 or hw[0] < 1 or hw[1] < 1:
+        want = "[T,H,W,2]" if layout == "yuyv" else "[T,H*3/2,W]"
+        raise EngineError(f"{layout} frames must be {want}, got {tuple(src.shape)}")
+    T, (H, W) = src.shape[0], hw
+    # the bytes of a row must be contiguous; a row stride only matters when there is more than one row
+    inner = (2, 1) if layout == "yuyv" else (1,)
+    if tuple(src.stride()[-len(inner):]) != inner:
+        raise EngineError(f"the bytes of a {layout} row must be contiguous, got strides {src.stride()}")
+    if not src.is_cuda:
+        raise EngineError("src must be a CUDA tensor (no CPU fallback)")
+    rows = src.shape[1]
+    stride_row = src.stride(1) if rows > 1 else (2 * W if layout == "yuyv" else W)
+    oh, ow = int(out_hw[0]), int(out_hw[1])
+    if out is None:
+        out = torch.empty(T, 3, oh, ow, dtype=torch.float32, device=src.device)
+    _req(out, torch.float32, "out")
+    if tuple(out.shape) != (T, 3, oh, ow) or out.device != src.device:
+        raise EngineError(f"out must be [{T},3,{oh},{ow}] on {src.device}")
+    _call("ct3_prepare_frames_yuv", src.device, _ptr(src), YUV_LAYOUTS[layout], T, H, W, src.stride(0), stride_row, oh,
+          ow, _ptr(out), _stream(src.device))
     return out
 
 

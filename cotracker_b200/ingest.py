@@ -15,6 +15,11 @@ device never holds more than two raw chunks.  Staging memory is bounded: 2 * k *
 the same on the device, with k = max(1, min(T, STAGING_SLOT_BYTES // frame_bytes)) -- at most
 2 * max(STAGING_SLOT_BYTES, frame_bytes) each (`staging_bytes`).  The clips of a host batch go through the same two
 slots one after another, so the bound does not grow with B.
+
+A `YUVClip` holds the clip as decoders and cameras emit it (NV12, I420, YUYV) and goes in wherever an RGB clip does.
+Its frames are converted, resized and normalised by one library kernel (ct3_prepare_frames_yuv), bit-identical to the
+RGB path on the uint8 clip cv2.cvtColor(COLOR_YUV2RGB_*) makes of it, and a host clip is uploaded as YUV bytes (1.5
+bytes per pixel for 4:2:0 instead of RGB's 3) through the same two staging slots.
 """
 from __future__ import annotations
 
@@ -64,14 +69,57 @@ def _dense_strides(shape, strides):
     return tuple(st if n != 1 else 0 for n, st in zip(shape, strides))
 
 
+class YUVClip:
+    """A clip of uint8 YUV frames: data [B,T,H*3/2,W] for layout "nv12" (H luma rows, then H/2 rows of interleaved U,V)
+    or "i420" (the Y, U and V planes packed, as PyAV's `to_ndarray()` gives yuv420p), or [B,T,H,W,2] for "yuyv"
+    (Y0 U Y1 V per pixel pair); on the host or the device.  H and W must be even (W only, for yuyv).
+
+    It stands for the RGB clip [B,T,3,H,W] whose frames are cv2.cvtColor(frame, COLOR_YUV2RGB_{NV12|I420|YUYV}): every
+    predictor and `OnlineStreams.push` take it where they take that clip and give results `torch.equal` to it.  `shape`
+    is that clip's logical (B, T, 3, H, W); `data` is read by `prepare_video` only."""
+
+    def __init__(self, data: torch.Tensor, layout: str):
+        if layout not in engine.YUV_LAYOUTS:
+            raise ValueError(f"unknown YUV layout {layout!r}: one of {sorted(engine.YUV_LAYOUTS)}")
+        want = "[B,T,H,W,2]" if layout == "yuyv" else "[B,T,H*3/2,W]"
+        if not torch.is_tensor(data) or data.dtype != torch.uint8:
+            raise ValueError(f"{layout} data must be a uint8 tensor {want}, got "
+                             f"{data.dtype if torch.is_tensor(data) else type(data).__name__}")
+        hw = engine.yuv_frame_hw(layout, data.shape) if data.dim() == (5 if layout == "yuyv" else 4) else None
+        if hw is None or min(data.shape[:2]) < 1 or min(hw) < 1:
+            raise ValueError(f"{layout} data must be {want} with B, T, H, W >= 1, got {tuple(data.shape)}")
+        if hw[1] % 2 or (layout != "yuyv" and hw[0] % 2):
+            raise ValueError(f"{layout} frames must have an even {'width' if layout == 'yuyv' else 'width and height'}"
+                             f", got H x W = {hw[0]} x {hw[1]}")
+        self.data, self.layout = data, layout
+        self.shape = torch.Size((data.shape[0], data.shape[1], 3) + tuple(hw))
+
+    def dim(self) -> int:
+        return 5
+
+    @property
+    def device(self) -> torch.device:
+        return self.data.device
+
+    @property
+    def is_cuda(self) -> bool:
+        return self.data.is_cuda
+
+    def to(self, device) -> "YUVClip":
+        return YUVClip(self.data.to(device), self.layout)
+
+    def __repr__(self) -> str:
+        return f"YUVClip({self.layout}, shape={tuple(self.shape)}, device={self.device})"
+
+
 def model_device(model: torch.nn.Module) -> torch.device:
     p = next(model.parameters(), None)
     return p.device if p is not None else torch.device("cpu")
 
 
-def prepare_video(video: torch.Tensor, out_hw, device, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """video [B,T,3,H,W] uint8 or float (0..255), host or device, any strides -> [B*T,3,oh,ow] fp32 in [-1,1] on device,
-    clip after clip; each clip's frames are bit-identical to the call on that clip alone.
+def prepare_video(video, out_hw, device, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """video [B,T,3,H,W] uint8 or float (0..255), host or device, any strides, or a `YUVClip` -> [B*T,3,oh,ow] fp32 in
+    [-1,1] on device, clip after clip; each clip's frames are bit-identical to the call on that clip alone.
     out: an optional contiguous fp32 [B*T,3,oh,ow] destination on `device` (e.g. a slice of a larger frame batch).
     Other dtypes (float16, float64, ...) are cast to float32 first and then take the float32 path; for pixel values
     0..255 that cast is exact.  (Before this step existed they were resized in their own dtype, so results for them can
@@ -81,7 +129,8 @@ def prepare_video(video: torch.Tensor, out_hw, device, out: Optional[torch.Tenso
         raise engine.EngineError("cotracker_b200 runs on CUDA only; move the module to a GPU")
     if video.dim() != 5 or video.shape[0] < 1 or video.shape[1] < 1 or video.shape[2] != 3:
         raise ValueError(f"video must be [B,T,3,H,W] with B, T >= 1, got {tuple(video.shape)}")
-    if video.dtype not in engine.FRAME_DTYPES:
+    yuv = isinstance(video, YUVClip)
+    if not yuv and video.dtype not in engine.FRAME_DTYPES:
         video = video.float()
     B, T = video.shape[:2]
     if video.is_cuda and video.device != device:
@@ -92,26 +141,33 @@ def prepare_video(video: torch.Tensor, out_hw, device, out: Optional[torch.Tenso
     elif tuple(out.shape) != shape or out.dtype != torch.float32 or out.device != device or not out.is_contiguous():
         raise ValueError(f"out must be a contiguous fp32 {shape} tensor on {device}")
     staging = None
+    layout = video.layout if yuv else None
     for b in range(B):
-        if video.is_cuda:
-            engine.prepare_frames(video[b], out_hw, out=out[b * T:(b + 1) * T])
+        clip = video.data[b] if yuv else video[b]
+        if video.is_cuda and yuv:
+            engine.prepare_frames_yuv(clip, layout, out_hw, out=out[b * T:(b + 1) * T])
+        elif video.is_cuda:
+            engine.prepare_frames(clip, out_hw, out=out[b * T:(b + 1) * T])
         else:
-            staging = _prepare_host(video[b], out_hw, out[b * T:(b + 1) * T], staging)
+            staging = _prepare_host(clip, out_hw, out[b * T:(b + 1) * T], staging, layout)
     return out
 
 
-def _prepare_host(v: torch.Tensor, out_hw, out: torch.Tensor, staging=None):
-    """One host clip [T,3,H,W] -> out [T,3,oh,ow] on the device.  Returns its staging buffers (pinned slots, device
-    slots), which the next clip of a batch takes as `staging`."""
-    T, C, H, W = v.shape
+def _prepare_host(v: torch.Tensor, out_hw, out: torch.Tensor, staging=None, layout: Optional[str] = None):
+    """One host clip -> out [T,3,oh,ow] on the device: v [T,3,H,W], or with a YUV `layout` the clip's YUV frames (a
+    `YUVClip`'s data[b]), which are uploaded as they are and converted on the device.  Returns its staging buffers
+    (pinned slots, device slots), which the next clip of a batch takes as `staging`."""
+    T, fshape = v.shape[0], tuple(v.shape[1:])
     oh, ow = int(out_hw[0]), int(out_hw[1])
     device = out.device
-    fe = C * H * W                                  # elements per frame
+    fe = v[0].numel()                               # elements per frame
     esize = v.element_size()
     chunks = plan_chunks(T, fe * esize)
     k = chunks[0][1] - chunks[0][0]
-    dense = frame_is_dense(v.shape[1:], v.stride()[1:]) and all(s >= 0 for s in v.stride())
-    fstrides = _dense_strides(v.shape[1:], v.stride()[1:]) if dense else (H * W, W, 1)
+    dense = frame_is_dense(fshape, v.stride()[1:]) and all(s >= 0 for s in v.stride())
+    if layout is not None:   # the YUV kernel reads rows in their own order: a dense frame must be row-major
+        dense = dense and v[0].is_contiguous()
+    fstrides = _dense_strides(fshape, v.stride()[1:]) if dense else torch.empty(fshape, device="meta").stride()
 
     main = torch.cuda.current_stream(device)
     side = torch.cuda.Stream(device)
@@ -143,8 +199,11 @@ def _prepare_host(v: torch.Tensor, out_hw, out: torch.Tensor, staging=None):
             raw[slot][:n * fe].copy_(pinned[slot][:n * fe], non_blocking=True)
             copied[slot].record(side)
         main.wait_event(copied[slot])
-        src_dev = torch.as_strided(raw[slot], (n, C, H, W), (fe,) + tuple(fstrides))
-        engine.prepare_frames(src_dev, (oh, ow), out=out[t0:t1])
+        src_dev = torch.as_strided(raw[slot], (n,) + fshape, (fe,) + tuple(fstrides))
+        if layout is None:
+            engine.prepare_frames(src_dev, (oh, ow), out=out[t0:t1])
+        else:
+            engine.prepare_frames_yuv(src_dev, layout, (oh, ow), out=out[t0:t1])
         consumed[slot].record(main)
         used[slot] = True
     # the staging buffers go back to PyTorch's caches when this returns: uploads must be done with the pinned memory

@@ -12,6 +12,8 @@ memory permitting, one update-loop pass for the whole batch; slot b of the resul
 `video[b:b+1]` (and `queries[b:b+1]`).  `segm_mask` keeps a different number of points per clip and is for B = 1 only.
 A list of [1,T_b,3,H_b,W_b] clips of any lengths and sizes (offline model, sparse queries) is tracked the same way, with
 per-clip `queries` / `segm_mask` lists; it returns lists, and entry b is bit-identical to the call on clip b alone.
+A clip, or an entry of such a list, may be a `YUVClip` (NV12, I420 or YUYV frames): results are `torch.equal` to the
+call on its RGB conversion by cv2.cvtColor.
 """
 from __future__ import annotations
 
@@ -236,9 +238,10 @@ def _check_list_call(model, clips, queries, segm_mask, grid_size, grid_query_fra
         if lst is not None and (not isinstance(lst, (list, tuple)) or len(lst) != B):
             raise ValueError(f"{name} must be a list of {B} entries, one per clip")
     for b, c in enumerate(clips):
-        if not torch.is_tensor(c) or c.dim() != 5 or c.shape[0] != 1 or c.shape[1] < 1 or c.shape[2] != 3:
+        clip = torch.is_tensor(c) or isinstance(c, ingest.YUVClip)
+        if not clip or c.dim() != 5 or c.shape[0] != 1 or c.shape[1] < 1 or c.shape[2] != 3:
             raise ValueError(f"clip {b} must be a [1,T,3,H,W] tensor, got "
-                             f"{tuple(c.shape) if torch.is_tensor(c) else type(c).__name__}")
+                             f"{tuple(c.shape) if clip else type(c).__name__}")
     for b, c in enumerate(clips):
         T = c.shape[1]
         q = None if queries is None else queries[b]

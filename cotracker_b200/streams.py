@@ -204,7 +204,8 @@ class OnlineStreams:
         return self._get(sid)["state"].length
 
     def push(self, sid: int, chunk: torch.Tensor):
-        """Queue the next chunk [1,T,3,H,W] of stream `sid` (T <= window_len) for the next `step()`."""
+        """Queue the next chunk [1,T,3,H,W] of stream `sid` (T <= window_len), or a `YUVClip` of it, for the next
+        `step()`."""
         s = self._get(sid)
         if sid in self._pending:
             raise ValueError(f"stream {sid} already has a chunk for this step")

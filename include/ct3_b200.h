@@ -109,6 +109,24 @@ int ct3_pack_weights(const float* const* tensors_host_array_of_device_ptrs, int 
 enum { CT3_FRAMES_U8 = 0, CT3_FRAMES_F32 = 1 };
 int ct3_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c,
                        int64_t stride_h, int64_t stride_w, int out_h, int out_w, float* out, ct3_stream_t stream);
+/* ct3_prepare_frames_yuv: the same from T uint8 YUV frames, as decoders and cameras emit them.  The output is
+ * bit-identical to ct3_prepare_frames on the uint8 RGB clip cv2.cvtColor(frame, COLOR_YUV2RGB_{NV12|I420|YUYV}) gives:
+ * BT.601 limited range, each chroma sample shared by its 2x2 block (4:2:0) or its horizontal pair (YUYV), in Q20
+ * integers (>> is a floor shift; every term fits int32):
+ *     y = max(Y - 16, 0) * 1220542        u = U - 128        v = V - 128
+ *     R = clamp((y + 1673527 v            + 2^19) >> 20, 0, 255)
+ *     G = clamp((y -  852492 v - 409993 u + 2^19) >> 20, 0, 255)
+ *     B = clamp((y + 2116026 u            + 2^19) >> 20, 0, 255)
+ * One frame, at byte strides stride_t (frame, any sign) and stride_row (row):
+ *     CT3_YUV_NV12  H luma rows, then H/2 rows of interleaved U,V; W bytes each, stride_row >= W (pitched surfaces)
+ *     CT3_YUV_I420  the Y plane, the (H/2)x(W/2) U plane, the V plane, packed: stride_row == W
+ *     CT3_YUV_YUYV  H rows of W/2 pixel pairs Y0 U Y1 V; stride_row >= 2W
+ * H and W must be even (W only, for YUYV).  Null pointers, an unknown layout, T/H/W/out_h/out_w < 1, odd dimensions,
+ * a row stride below those bounds, a stride extent beyond int64 or an output plane above INT32_MAX pixels return
+ * CT3_EINVAL before any launch. */
+enum { CT3_YUV_NV12 = 0, CT3_YUV_I420 = 1, CT3_YUV_YUYV = 2 };
+int ct3_prepare_frames_yuv(const uint8_t* src, int layout, int T, int H, int W, int64_t stride_t, int64_t stride_row,
+                           int out_h, int out_w, float* out, ct3_stream_t stream);
 
 /* ---- the predictor's tail ---------------------------------------------------
  * ct3_finish_tracks: what CoTrackerPredictor does with the model's output (predictor.py:161-209), for B clips in one
