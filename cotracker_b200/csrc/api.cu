@@ -4,7 +4,9 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
 #include <atomic>
+#include <cmath>
 #include <vector>
 
 #include "abi.cuh"
@@ -407,6 +409,86 @@ int ct3_render_flow_colors(const float* pts, int T, int N, int query_frame, uint
   if (query_frame < 0 || query_frame >= T) return fail(CT3_EINVAL, "query_frame must be in [0, T)%s");
   if (workspace_bytes < need) return fail(CT3_EINVAL, "workspace too small%s");
   CK(launch_render_flow_colors(pts, T, N, query_frame, colors, workspace, (cudaStream_t)stream), "render_flow_colors");
+  return 0;
+}
+
+// ---- Shi-Tomasi corners (corners.cu) -----------------------------------------------------------------------------
+namespace {
+// the workspace's buffers (lam first: ct3_detect_corners documents it); a null base only measures
+CornerWorkspace corner_workspace(void* base, int K, int64_t HW, CornerFrame** fp, size_t* total) {
+  Carver c(base);
+  CornerWorkspace w;
+  w.lam = static_cast<double*>(c.take((size_t)K * HW * sizeof(double)));
+  w.cand = static_cast<uint8_t*>(c.take((size_t)K * HW * 16));
+  w.sorted = static_cast<int*>(c.take((size_t)K * HW * sizeof(int)));
+  w.maxkey = static_cast<unsigned long long*>(c.take((size_t)K * (sizeof(unsigned long long) + sizeof(int))));
+  *fp = static_cast<CornerFrame*>(c.take((size_t)K * sizeof(CornerFrame)));
+  *total = c.off;
+  return w;
+}
+int check_corner_shape(int K, int H, int W) {
+  if (K < 1 || K > 65535) return fail(CT3_EINVAL, "K must be in [1, 65535]%s");
+  if (H < 1 || W < 1) return fail(CT3_EINVAL, "H and W must be >= 1%s");
+  if ((int64_t)H * W > INT32_MAX) return fail(CT3_EINVAL, "frame plane too large%s");
+  if (H > 65535 * 16) return fail(CT3_EINVAL, "H must be <= 1048560%s");
+  return 0;
+}
+}  // namespace
+
+int ct3_corners_workspace_bytes(int K, int H, int W, size_t* bytes) {
+  if (!bytes) return fail(CT3_EINVAL, "null argument%s");
+  if (int rc = check_corner_shape(K, H, W)) return rc;
+  CornerFrame* fp = nullptr;
+  corner_workspace(nullptr, K, (int64_t)H * W, &fp, bytes);
+  return 0;
+}
+
+int ct3_detect_corners(const float* frames, int64_t frame_stride, int K, int H, int W, const ct3_corner_params* params,
+                       const float* exclude, const int32_t* exclude_counts, int E_max, float* corners, int32_t* counts,
+                       void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+  if (!frames || !params || !corners || !counts || !workspace) return fail(CT3_EINVAL, "null argument%s");
+  if (int rc = check_corner_shape(K, H, W)) return rc;
+  if (int rc = check_aligned(workspace, "workspace")) return rc;
+  const int64_t HW = (int64_t)H * W;
+  if (frame_stride < 0) return fail(CT3_EINVAL, "frame_stride must be >= 0%s");
+  if (K > 1 && frame_stride > (INT64_MAX / 4 - 3 * HW) / (K - 1)) return fail(CT3_EINVAL, "stride extent overflows int64%s");
+  if (E_max < 0 || E_max > INT32_MAX / 2) return fail(CT3_EINVAL, "E_max must be in [0, 2^30)%s");
+  std::vector<CornerFrame> fp(K);
+  int M = 0;
+  for (int k = 0; k < K; ++k) {
+    const ct3_corner_params& p = params[k];
+    if (p.block_size != 3 && p.block_size != 5 && p.block_size != 7) return fail(CT3_EINVAL, "block_size must be 3, 5 or 7%s");
+    if (H < p.block_size || W < p.block_size) return fail(CT3_EINVAL, "H and W must be >= block_size%s");
+    if (!(p.quality_level > 0.0 && p.quality_level <= 1.0)) return fail(CT3_EINVAL, "quality_level must be in (0, 1]%s");
+    if (p.max_corners < 1) return fail(CT3_EINVAL, "max_corners must be >= 1%s");
+    if (!(p.min_distance >= 0.0 && p.min_distance < 1e300)) return fail(CT3_EINVAL, "min_distance must be finite and >= 0%s");
+    if (!(p.exclude_radius >= 0.0 && p.exclude_radius < 1e300))
+      return fail(CT3_EINVAL, "exclude_radius must be finite and >= 0%s");
+    const int E = exclude_counts ? exclude_counts[k] : 0;
+    if (E < 0 || E > E_max) return fail(CT3_EINVAL, "exclude_counts must be in [0, E_max]%s");
+    if (E > 0 && !exclude) return fail(CT3_EINVAL, "exclusion points given without the exclude buffer%s");
+    CornerFrame& f = fp[k];
+    f.max_corners = p.max_corners;
+    f.block = p.block_size;
+    f.E = p.exclude_radius > 0.0 ? E : 0;
+    f.quality = p.quality_level;
+    f.md2 = p.min_distance * p.min_distance;
+    f.r2 = p.exclude_radius * p.exclude_radius;
+    const double side = std::floor(p.min_distance);
+    f.cs = side < 1.0 ? 1 : side > (double)std::max(H, W) ? std::max(H, W) : (int)side;
+    f.gw = (W + f.cs - 1) / f.cs;
+    f.gh = (H + f.cs - 1) / f.cs;
+    M = std::max(M, p.max_corners);
+  }
+  if ((int64_t)K * M > INT32_MAX) return fail(CT3_EINVAL, "K * max(max_corners) too large%s");
+  CornerFrame* fp_dev = nullptr;
+  size_t need = 0;
+  const CornerWorkspace ws = corner_workspace(workspace, K, HW, &fp_dev, &need);
+  if (int rc = check_space(workspace_bytes, need, "workspace")) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  CK(cudaMemcpyAsync(fp_dev, fp.data(), (size_t)K * sizeof(CornerFrame), cudaMemcpyHostToDevice, s), "detect_corners");
+  CK(launch_detect_corners(frames, frame_stride, K, H, W, fp_dev, exclude, E_max, M, corners, counts, ws, num_sms(), s),
+     "detect_corners");
   return 0;
 }
 

@@ -183,6 +183,21 @@ cudaError_t launch_row_bias(const float* time_emb, const float* w_in, int T, flo
 cudaError_t launch_split_rows(const float* x, int rows, int K, int Kpad, int perm_x, __nv_bfloat16* out,
                               int64_t dst_row_off, cudaStream_t s, int fp16 = 0);
 
+// ---- corners.cu : Shi-Tomasi corners of K prepared frames (ct3_detect_corners) --------------------------------
+struct CornerFrame {        // one frame's parameters as the kernels read them (derived on the host)
+  int max_corners, block, E, cs, gw, gh;   // E exclusion points; cs: grid cell side floor(min_distance), gw x gh cells
+  double quality, md2, r2;                 // quality_level, min_distance^2, exclude_radius^2
+};
+struct CornerWorkspace {
+  double* lam;                  // [K, H, W] responses
+  unsigned long long* maxkey;   // [K] order keys of the frames' max response, then [K] int candidate counts
+  uint8_t* cand;                // [K, H*W, 16 bytes] candidates (u64 key, i32 index, i32 rank), then the cell grid
+  int* sorted;                  // [K, H*W] candidate pixel indices in rank order
+};
+cudaError_t launch_detect_corners(const float* frames, int64_t frame_stride, int K, int H, int W,
+                                  const CornerFrame* fp_dev, const float* exclude, int E_max, int M, float* corners,
+                                  int32_t* counts, const CornerWorkspace& ws, int num_sms, cudaStream_t s);
+
 // ---- attention.cu -------------------------------------------------------------------------------
 struct AttnParams {
   const float* q;  int64_t q_ld;  int q_col;

@@ -43,6 +43,12 @@ class LoopShape(ctypes.Structure):
                 ("group_T", ctypes.POINTER(ctypes.c_int32))]
 
 
+class CornerParams(ctypes.Structure):
+    """ct3_corner_params (include/ct3_b200.h): one frame's detector parameters."""
+    _fields_ = [("max_corners", ctypes.c_int32), ("block_size", ctypes.c_int32), ("quality_level", ctypes.c_double),
+                ("min_distance", ctypes.c_double), ("exclude_radius", ctypes.c_double)]
+
+
 def _signatures():
     """name -> (restype, argtypes) of every entry point of include/ct3_b200.h"""
     c_int, c_size_t, c_void_p, c_char_p = ctypes.c_int, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_char_p
@@ -113,6 +119,10 @@ def _signatures():
         "ct3_encoder_pack": (c_int, [ctypes.POINTER(c_void_p), c_int, c_void_p, c_size_t, c_void_p]),
         "ct3_encoder_workspace_bytes": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
         "ct3_encoder": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+        "ct3_corners_workspace_bytes": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+        "ct3_detect_corners": (c_int, [c_void_p, i64, c_int, c_int, c_int, ctypes.POINTER(CornerParams), c_void_p,
+                                       ctypes.POINTER(ctypes.c_int32), c_int, c_void_p, c_void_p, c_void_p, c_size_t,
+                                       c_void_p]),
         "ct3_profile_enable": (c_int, [c_int]),
         "ct3_profile_read": (c_int, [ctypes.POINTER(ctypes.c_double), intp, ctypes.POINTER(ctypes.c_double)]),
     }
@@ -503,6 +513,56 @@ def render_flow_colors(pts: torch.Tensor, query_frame: int) -> torch.Tensor:
     _call("ct3_render_flow_colors", dev, _ptr(pts), T, N, int(query_frame), _ptr(colors), _ptr(workspace),
           workspace.numel(), _stream(dev))
     return colors
+
+
+def corners_workspace_bytes(K: int, H: int, W: int) -> int:
+    return _size("ct3_corners_workspace_bytes", int(K), int(H), int(W))
+
+
+def detect_corners(frames: torch.Tensor, params, exclude=None, workspace: Optional[torch.Tensor] = None):
+    """Shi-Tomasi corners of K frames in one library call (ct3_detect_corners in include/ct3_b200.h).
+    frames [K,3,H,W] fp32 CUDA, each frame contiguous, any frame stride >= 0 (e.g. prepared model-resolution frames).
+    params: one CornerParams for every frame, or a sequence of K.  exclude: None, or (points [K,E,2] fp32 CUDA
+    contiguous, counts: K ints) -- frame k excludes discs of its params' exclude_radius around its first counts[k]
+    points.  workspace: optional scratch of corners_workspace_bytes(K, H, W) bytes; it starts with the responses,
+    fp64 [K,H,W].  -> (corners [K,M,2] fp32 (x, y) in selection order, zero past counts[k]; counts [K] int32), both on
+    the frames' device, M = the largest max_corners."""
+    if not frames.is_cuda:
+        raise EngineError("frames must be a CUDA tensor (no CPU fallback)")
+    if frames.dtype != torch.float32:
+        raise EngineError(f"frames must be float32, got {frames.dtype}")
+    if frames.dim() != 4 or frames.shape[1] != 3 or frames.shape[0] < 1:
+        raise EngineError(f"frames must be [K,3,H,W] with K >= 1, got {tuple(frames.shape)}")
+    K, _, H, W = frames.shape
+    if not frames[0].is_contiguous():
+        raise EngineError(f"each frame must be contiguous, got strides {frames.stride()}")
+    if frames.stride(0) < 0:
+        raise EngineError("the frame stride must be >= 0")
+    params = [params] * K if isinstance(params, CornerParams) else list(params)
+    if len(params) != K or not all(isinstance(p, CornerParams) for p in params):
+        raise EngineError(f"params must be a CornerParams or a sequence of {K} of them")
+    dev = frames.device
+    points, counts, E = None, None, 0
+    if exclude is not None:
+        points, counts = exclude
+        _req(points, torch.float32, "exclude points")
+        if points.dim() != 3 or points.shape[0] != K or points.shape[2] != 2 or points.device != dev:
+            raise EngineError(f"exclude points must be [{K},E,2] on {dev}, got {tuple(points.shape)} on {points.device}")
+        E = points.shape[1]
+        counts = [int(c) for c in counts]
+        if len(counts) != K:
+            raise EngineError(f"exclude counts must hold {K} entries, got {len(counts)}")
+        counts = (ctypes.c_int32 * K)(*counts)
+    table = (CornerParams * K)(*params)
+    M = max(p.max_corners for p in params)
+    corners = torch.empty(K, max(M, 0), 2, dtype=torch.float32, device=dev)
+    found = torch.empty(K, dtype=torch.int32, device=dev)
+    nbytes = corners_workspace_bytes(K, H, W)
+    if workspace is None:
+        workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    _call("ct3_detect_corners", dev, _ptr(frames), frames.stride(0), K, H, W, table, _ptr(points), counts, E,
+          _ptr(corners), _ptr(found), _ptr(workspace), workspace.numel(), _stream(dev))
+    return corners, found
 
 
 def pyramid_levels(pyr: torch.Tensor, T: int, H4: int, W4: int) -> List[torch.Tensor]:

@@ -61,7 +61,7 @@ from typing import Dict, List, Optional, Tuple
 
 import torch
 
-from . import engine, ingest
+from . import corners, engine, ingest
 from .model import StreamPool, StreamState
 
 SNAPSHOT_FORMAT = 1
@@ -269,6 +269,11 @@ class OnlineStreams:
         if not bool((t >= state.length).all()):
             raise ValueError(f"stream {sid} has advanced {state.length} frames: query frames must be >= "
                              f"{state.length}, got {float(t.min())}")
+        return self._insert_tracks(s, queries)
+
+    def _insert_tracks(self, s: dict, queries: torch.Tensor) -> List[int]:
+        """add_tracks on the stream entry `s` once its queries are checked."""
+        state = s["state"]
         q, _ = self.predictor._first_step_queries(1, s["hw"], queries, 0, 0, False, ingest.model_device(self.model))
         n_keep, scale = s["out"]
         self.pool.edit(state, range(state.n), n_keep, *self.model._stream_queries(q[0]), self.model.stride)
@@ -276,6 +281,39 @@ class OnlineStreams:
         ids = list(range(s["next_id"], s["next_id"] + m))
         s.update(ids=s["ids"] + ids, next_id=s["next_id"] + m, out=(n_keep + m, scale))
         return ids
+
+    @torch.no_grad()
+    def seed_corners(self, sid: int, max_tracks: int, *, quality_level: float = 0.01, min_distance: float = 10,
+                     block_size: int = 3, exclude_radius: Optional[float] = None) -> List[int]:
+        """Add up to max_tracks tracks at the Shi-Tomasi corners (`detect_corners`) of stream frame length(sid), the
+        first frame the pending chunk adds: call it after push(sid, chunk) and before step().  Corners closer than
+        exclude_radius (default min_distance; both model-resolution pixels) to one of the stream's own tracks at frame
+        length(sid) - 1 are left out.  The new tracks start at frame length(sid), as add_tracks adds them.  -> their
+        ids; [] when no corner qualifies, and the stream is unchanged.  Only the corner count reaches the host."""
+        s = self._get(sid)
+        radius = min_distance if exclude_radius is None else exclude_radius
+        par = corners.params(max_tracks, quality_level, min_distance, block_size, radius)
+        if sid not in self._pending:
+            raise ValueError(f"stream {sid} has no pending chunk: push() the chunk to seed before step()")
+        state, chunk = s["state"], self._pending[sid]
+        t = state.length - state.ind      # the chunk's first new frame: 0 before the first step
+        if not 0 <= t < chunk.shape[1]:
+            raise ValueError(f"stream {sid}'s pending chunk of {chunk.shape[1]} frames adds no frame after frame "
+                             f"{state.length - 1}")
+        dev = ingest.model_device(self.model)
+        frame = ingest.prepare_video(corners.clip_frame(chunk, t), self.predictor.interp_shape, dev)
+        n_keep, scale = s["out"]
+        exclude = None
+        if state.length:   # the history holds coords * stride: model-resolution pixels
+            coords = state.hist[0]
+            row = (state.length - 1) % coords.shape[0] if state.history is not None else state.length - 1
+            exclude = (coords[row, :n_keep][None].contiguous(), [n_keep])
+        found, counts = engine.detect_corners(frame, par, exclude)
+        n = int(counts[0])
+        if n == 0:
+            return []
+        xy = (found[0, :n] * found.new_tensor(scale)).double()
+        return self._insert_tracks(s, torch.cat([xy.new_full((n, 1), float(state.length)), xy], 1)[None])
 
     def retire_tracks(self, sid: int, ids):
         """Remove the tracks `ids` (ids of stream `sid`, see track_ids) from its next step on.  The support grid's

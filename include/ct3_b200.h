@@ -128,6 +128,47 @@ enum { CT3_YUV_NV12 = 0, CT3_YUV_I420 = 1, CT3_YUV_YUYV = 2 };
 int ct3_prepare_frames_yuv(const uint8_t* src, int layout, int T, int H, int W, int64_t stride_t, int64_t stride_row,
                            int out_h, int out_w, float* out, ct3_stream_t stream);
 
+/* ---- Shi-Tomasi corners: where to seed new tracks ----------------------------------------------------------------
+ * ct3_detect_corners: the corners cv2.goodFeaturesToTrack(gray, max_corners, quality_level, min_distance, mask,
+ * block_size, useHarrisDetector=False) selects, in K frames at once, bit-identical to this float64 restatement:
+ *   1. g = 0.299 R + 0.587 G + 0.114 B in fp32, in that order, without contraction;
+ *   2. 3x3 Sobel in fp64 with reflect-101 borders: dx = ((g[y-1][x+1] - g[y-1][x-1]) + 2 (g[y][x+1] - g[y][x-1]))
+ *      + (g[y+1][x+1] - g[y+1][x-1]), dy likewise with rows and columns swapped;
+ *   3. Sxx, Sxy, Syy: sums of dx^2, dx dy, dy^2 over the block_size x block_size window (reflect-101), accumulated in
+ *      row-major order from 0 in fp64;
+ *   4. lambda = (a + c) - sqrt((a - c)^2 + b^2) with a = Sxx / 2, b = Sxy, c = Syy / 2, in fp64, without contraction;
+ *   5. candidates: pixels with 1 <= x < W-1, 1 <= y < H-1, lambda > quality_level * (the frame's max lambda), lambda
+ *      equal to the max of its 3x3 neighbourhood, and (x - ex)^2 + (y - ey)^2 >= exclude_radius^2 (fp64) for every
+ *      exclusion point (ex, ey) of the frame;
+ *   6. sorted by lambda descending, ties by raster index y * W + x descending;
+ *   7. walked in that order: a candidate is kept unless a kept corner lies at dx^2 + dy^2 < min_distance^2, until
+ *      max_corners are kept.
+ * frames: K fp32 frames [3,H,W] (contiguous inside a frame) at element stride frame_stride >= 0, e.g. the prepared
+ * model-resolution frames.  params: HOST array of K entries.  exclude: device [K, E_max, 2] fp32 (x, y) of which frame k
+ * uses its first exclude_counts[k] (HOST array of K, or NULL: none), or NULL when there are none; a frame with
+ * exclude_radius 0 excludes nothing.  corners: [K, M, 2] fp32 (x, y) with M = the largest max_corners; frame k fills
+ * rows [0, counts[k]) in selection order and zeroes the rest; counts: [K] int32.  Both are written in stream order,
+ * without host synchronisation.  The workspace (ct3_corners_workspace_bytes, 256-byte aligned) starts with the
+ * frames' responses lambda, fp64 [K,H,W], which stay there after the call.  Null pointers, K outside [1, 65535],
+ * H * W above INT32_MAX, H or W below a frame's block_size, block_size outside {3,5,7}, quality_level outside (0, 1],
+ * max_corners < 1, a negative or non-finite min_distance or exclude_radius, frame_stride < 0 or a frame extent beyond
+ * int64, E_max < 0, an exclusion count outside [0, E_max] or without `exclude` return CT3_EINVAL, a small workspace
+ * CT3_ENOSPC, before any launch.  The sort compares every pair of a frame's candidates: microseconds for the few
+ * thousand of a textured frame, far slower (but exact) when a plateau makes most pixels candidates. */
+typedef struct {
+  int32_t max_corners;     /* >= 1: corners kept at most                                                         */
+  int32_t block_size;      /* 3, 5 or 7                                                                          */
+  double quality_level;    /* (0, 1]: a candidate's lambda exceeds quality_level * the frame's max lambda         */
+  double min_distance;     /* >= 0, pixels: kept corners are at least this far apart                             */
+  double exclude_radius;   /* >= 0, pixels: no corner closer than this to an exclusion point                     */
+} ct3_corner_params;
+/* Scratch of ct3_detect_corners for K frames of H x W: 28 bytes per pixel and 60 per frame, each buffer aligned.
+ * CT3_EINVAL unless K in [1, 65535], H, W >= 1, H <= 1048560 and H * W <= INT32_MAX. */
+int ct3_corners_workspace_bytes(int K, int H, int W, size_t* bytes);
+int ct3_detect_corners(const float* frames, int64_t frame_stride, int K, int H, int W, const ct3_corner_params* params,
+                       const float* exclude, const int32_t* exclude_counts, int E_max, float* corners, int32_t* counts,
+                       void* workspace, size_t workspace_bytes, ct3_stream_t stream);
+
 /* ---- the predictor's tail ---------------------------------------------------
  * ct3_finish_tracks: what CoTrackerPredictor does with the model's output (predictor.py:161-209), for B clips in one
  * kernel.  fwd_tracks [B,T,N,2] fp32 at model resolution and fwd_vis [B,T,N] fp32 visibility probabilities of the
