@@ -228,9 +228,10 @@ int ct3_prepare_frames_yuv(const uint8_t* src, int layout, int T, int H, int W, 
 }
 
 // ---- the predictor's tail (finish.cu) ----------------------------------------------------------------------------
-int ct3_finish_tracks(const float* fwd_tracks, const float* fwd_vis, const float* bwd_tracks, const float* bwd_vis,
-                      const float* queries, int B, int T, int N, int n_keep, float threshold, float scale_x,
-                      float scale_y, float* tracks, uint8_t* visibility, ct3_stream_t stream) {
+namespace {
+// the checks ct3_finish_tracks and ct3_finish_tracks_scores share
+int check_finish(const float* fwd_tracks, const float* fwd_vis, const float* bwd_tracks, const float* bwd_vis,
+                 const float* queries, int B, int T, int N, int n_keep, const float* tracks, const uint8_t* visibility) {
   if (!fwd_tracks || !fwd_vis || !queries || !tracks || !visibility) return fail(CT3_EINVAL, "null argument%s");
   if ((bwd_tracks == nullptr) != (bwd_vis == nullptr))
     return fail(CT3_EINVAL, "bwd_tracks and bwd_vis must be given together%s");
@@ -241,8 +242,34 @@ int ct3_finish_tracks(const float* fwd_tracks, const float* fwd_vis, const float
   // one thread per output element, one-dimensional grid
   if ((int64_t)B * T > (INT64_MAX >> 12) / N || (int64_t)B * T * N > (int64_t)INT32_MAX * 256)
     return fail(CT3_EINVAL, "problem too large%s");
+  return 0;
+}
+}  // namespace
+
+int ct3_finish_tracks(const float* fwd_tracks, const float* fwd_vis, const float* bwd_tracks, const float* bwd_vis,
+                      const float* queries, int B, int T, int N, int n_keep, float threshold, float scale_x,
+                      float scale_y, float* tracks, uint8_t* visibility, ct3_stream_t stream) {
+  if (int rc = check_finish(fwd_tracks, fwd_vis, bwd_tracks, bwd_vis, queries, B, T, N, n_keep, tracks, visibility))
+    return rc;
   CK(launch_finish_tracks(fwd_tracks, fwd_vis, bwd_tracks, bwd_vis, queries, B, T, N, n_keep, threshold, scale_x,
                           scale_y, tracks, visibility, (cudaStream_t)stream), "finish_tracks");
+  return 0;
+}
+
+int ct3_finish_tracks_scores(const float* fwd_tracks, const float* fwd_vis, const float* fwd_conf,
+                             const float* bwd_tracks, const float* bwd_vis, const float* bwd_conf, const float* queries,
+                             int B, int T, int N, int n_keep, float threshold, float scale_x, float scale_y,
+                             float* tracks, uint8_t* visibility, float* score_vis, float* score_conf,
+                             ct3_stream_t stream) {
+  if (int rc = check_finish(fwd_tracks, fwd_vis, bwd_tracks, bwd_vis, queries, B, T, N, n_keep, tracks, visibility))
+    return rc;
+  if (!fwd_conf || !score_vis || !score_conf) return fail(CT3_EINVAL, "null argument%s");
+  if ((bwd_conf == nullptr) != (bwd_vis == nullptr))
+    return fail(CT3_EINVAL, "bwd_conf must be given with the backward pair, and only with it%s");
+  CK(launch_finish_tracks_scores(fwd_tracks, fwd_vis, fwd_conf, bwd_tracks, bwd_vis, bwd_conf, queries, B, T, N, n_keep,
+                                 threshold, scale_x, scale_y, tracks, visibility, score_vis, score_conf,
+                                 (cudaStream_t)stream),
+     "finish_tracks_scores");
   return 0;
 }
 
@@ -343,6 +370,37 @@ int ct3_online_window_end(const ct3_online_stream* streams_host, int K, int S, i
   CK(cudaMemcpyAsync(dev, streams_host, (size_t)K * sizeof(ct3_online_stream), cudaMemcpyHostToDevice, s),
      "online_window_end");
   CK(launch_online_window_end(dev, K, max_elems, (float)stride, coords, vis, conf, N, threshold, s), "online_window_end");
+  return 0;
+}
+
+int ct3_online_window_end_scores(const ct3_online_stream* streams_host, int K, int S, int stride, const float* coords,
+                                 const float* vis, const float* conf, int N, float threshold,
+                                 const ct3_online_scores* scores_host, void* workspace, size_t workspace_bytes,
+                                 ct3_stream_t stream) {
+  if (!coords || !vis || !conf || !scores_host) return fail(CT3_EINVAL, "null argument%s");
+  if ((uintptr_t)coords & 7) return fail(CT3_EINVAL, "coords must be 8-byte aligned%s");
+  int64_t max_elems = 0;
+  if (int rc = check_online(streams_host, K, S, 1, stride, N, true, &max_elems, workspace, workspace_bytes)) return rc;
+  // the scores follow the streams in the workspace
+  static_assert(sizeof(ct3_online_stream) % alignof(ct3_online_scores) == 0, "scores table misaligned");
+  const size_t table = (size_t)K * sizeof(ct3_online_stream);
+  if (workspace_bytes < table + (size_t)K * sizeof(ct3_online_scores)) return fail(CT3_ENOSPC, "workspace too small%s");
+  for (int k = 0; k < K; ++k) {
+    const ct3_online_scores& sc = scores_host[k];
+    if ((sc.vis == nullptr) != (sc.conf == nullptr))
+      return fail(CT3_EINVAL, "a stream's scores need both vis and conf, or neither%s");
+    if (sc.vis && !streams_host[k].tracks)
+      return fail(CT3_EINVAL, "a stream's scores need its output (tracks and visibility)%s");
+    if (((uintptr_t)sc.vis | (uintptr_t)sc.conf) & 3) return fail(CT3_EINVAL, "scores must be 4-byte aligned%s");
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  auto* dev = reinterpret_cast<ct3_online_stream*>(workspace);
+  auto* dev_scores = reinterpret_cast<ct3_online_scores*>(static_cast<char*>(workspace) + table);
+  CK(cudaMemcpyAsync(dev, streams_host, table, cudaMemcpyHostToDevice, s), "online_window_end_scores");
+  CK(cudaMemcpyAsync(dev_scores, scores_host, (size_t)K * sizeof(ct3_online_scores), cudaMemcpyHostToDevice, s),
+     "online_window_end_scores");
+  CK(launch_online_window_end_scores(dev, dev_scores, K, max_elems, (float)stride, coords, vis, conf, N, threshold, s),
+     "online_window_end_scores");
   return 0;
 }
 

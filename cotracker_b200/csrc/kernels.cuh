@@ -5,6 +5,10 @@
 
 namespace ct3 {
 
+// torch.sigmoid of fp32 as ATen evaluates it: 1 / (1 + expf(-x)), IEEE division, no fast-math.  Every probability the
+// library derives from a logit goes through this one function, so they all agree bit for bit with torch.sigmoid.
+__device__ __forceinline__ float sigmoid_aten(float x) { return 1.0f / (1.0f + expf(-x)); }
+
 // ---- prep.cu : per-clip preparation -------------------------------------------------------------
 struct PyramidLayout {
   int64_t off[kL];  // float offset of each level inside the pyramid buffer
@@ -37,6 +41,12 @@ cudaError_t launch_finish_tracks(const float* fwd_tracks, const float* fwd_vis, 
                                  const float* bwd_vis, const float* queries, int B, int T, int N, int n_keep,
                                  float threshold, float scale_x, float scale_y, float* tracks, uint8_t* visibility,
                                  cudaStream_t s);
+// the same, also copying the merged visibility / confidence probabilities into score_vis / score_conf [B,T,n_keep]
+cudaError_t launch_finish_tracks_scores(const float* fwd_tracks, const float* fwd_vis, const float* fwd_conf,
+                                        const float* bwd_tracks, const float* bwd_vis, const float* bwd_conf,
+                                        const float* queries, int B, int T, int N, int n_keep, float threshold,
+                                        float scale_x, float scale_y, float* tracks, uint8_t* visibility,
+                                        float* score_vis, float* score_conf, cudaStream_t s);
 
 // ---- online.cu : per-window state of K streams (arguments validated by ct3_online_window_*) -------------------
 // streams: the device copy of the K entries; max_elems: the largest per-stream element count (S * n or (ind + T) * n)
@@ -47,6 +57,10 @@ cudaError_t launch_online_window_begin(const ct3_online_stream* streams, int K, 
 cudaError_t launch_online_window_end(const ct3_online_stream* streams, int K, int64_t max_elems, float stride,
                                      const float* coords, const float* vis, const float* conf, int N, float threshold,
                                      cudaStream_t s);
+// the same, also writing sigmoid(vis) and sigmoid(conf) of each output element where scores[k] is set (device copy)
+cudaError_t launch_online_window_end_scores(const ct3_online_stream* streams, const ct3_online_scores* scores, int K,
+                                            int64_t max_elems, float stride, const float* coords, const float* vis,
+                                            const float* conf, int N, float threshold, cudaStream_t s);
 
 // ---- render.cu : the track visualiser on uint8 frames [T,H,W,3] (arguments validated by ct3_render_*) ----------
 constexpr int kRenderMaxRadius = 255;   // largest point radius (int(linewidth * 2)) the footprint table holds

@@ -5,6 +5,7 @@
 // (1 / (1 + expf(-x)), IEEE division, no fast-math), so the results are bit-identical to the ATen expressions they
 // replace (include/ct3_b200.h).  Division by the stride is a multiply by the fp32 reciprocal, as ATen evaluates a
 // division by a scalar.  Block (x, k) strides over the elements of stream k; the grid's y dimension is the stream.
+// With scores (ct3_online_window_end_scores) the two sigmoids of the visibility compare are stored as well.
 // A ring history (ring = 1) holds frame f at row f mod cap; the host checks guarantee that every frame a launch reads
 // is still held and that no row is both read and written by one window_end launch.
 #include "../../include/ct3_b200.h"
@@ -61,12 +62,15 @@ __global__ void __launch_bounds__(kOnlineThreads) online_window_begin_kernel(
   }
 }
 
-__device__ __forceinline__ float sigmoid_aten(float x) { return 1.0f / (1.0f + expf(-x)); }
-
+// kScores: also write the two probabilities of each output element where the stream's scores entry is set
+template <bool kScores>
 __global__ void __launch_bounds__(kOnlineThreads) online_window_end_kernel(
-    const ct3_online_stream* __restrict__ streams, float stride, const float2* __restrict__ coords,
-    const float* __restrict__ vis, const float* __restrict__ conf, int N, float threshold) {
+    const ct3_online_stream* __restrict__ streams, const ct3_online_scores* __restrict__ scores, float stride,
+    const float2* __restrict__ coords, const float* __restrict__ vis, const float* __restrict__ conf, int N,
+    float threshold) {
   const ct3_online_stream& st = streams[blockIdx.y];
+  float* __restrict__ score_vis = kScores ? scores[blockIdx.y].vis : nullptr;
+  float* __restrict__ score_conf = kScores ? scores[blockIdx.y].conf : nullptr;
   const int n = st.n, first = st.first, ind = st.ind, n_keep = st.n_keep;
   float2* __restrict__ hc = reinterpret_cast<float2*>(st.coords);
   float* __restrict__ hv = st.vis;
@@ -104,7 +108,14 @@ __global__ void __launch_bounds__(kOnlineThreads) online_window_end_kernel(
     if (out) {
       const int64_t o = (t - out_first) * n_keep + j;
       tracks[o] = make_float2(__fmul_rn(p.x, st.scale_x), __fmul_rn(p.y, st.scale_y));
-      visibility[o] = __fmul_rn(sigmoid_aten(v), sigmoid_aten(q)) > threshold ? 1 : 0;
+      const float pv = sigmoid_aten(v), pq = sigmoid_aten(q);
+      visibility[o] = __fmul_rn(pv, pq) > threshold ? 1 : 0;
+      if constexpr (kScores) {
+        if (score_vis != nullptr) {
+          score_vis[o] = pv;
+          score_conf[o] = pq;
+        }
+      }
     }
   }
 }
@@ -129,8 +140,16 @@ cudaError_t launch_online_window_begin(const ct3_online_stream* streams, int K, 
 cudaError_t launch_online_window_end(const ct3_online_stream* streams, int K, int64_t max_elems, float stride,
                                      const float* coords, const float* vis, const float* conf, int N, float threshold,
                                      cudaStream_t s) {
-  online_window_end_kernel<<<online_grid(K, max_elems), kOnlineThreads, 0, s>>>(
-      streams, stride, reinterpret_cast<const float2*>(coords), vis, conf, N, threshold);
+  online_window_end_kernel<false><<<online_grid(K, max_elems), kOnlineThreads, 0, s>>>(
+      streams, nullptr, stride, reinterpret_cast<const float2*>(coords), vis, conf, N, threshold);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_online_window_end_scores(const ct3_online_stream* streams, const ct3_online_scores* scores, int K,
+                                            int64_t max_elems, float stride, const float* coords, const float* vis,
+                                            const float* conf, int N, float threshold, cudaStream_t s) {
+  online_window_end_kernel<true><<<online_grid(K, max_elems), kOnlineThreads, 0, s>>>(
+      streams, scores, stride, reinterpret_cast<const float2*>(coords), vis, conf, N, threshold);
   return cudaGetLastError();
 }
 

@@ -35,6 +35,11 @@ class OnlineStream(ctypes.Structure):
                 ("ring", ctypes.c_int32), ("pad", ctypes.c_int32)]
 
 
+class OnlineScores(ctypes.Structure):
+    """ct3_online_scores (include/ct3_b200.h): one stream's probability outputs of ct3_online_window_end_scores."""
+    _fields_ = [("vis", ctypes.c_void_p), ("conf", ctypes.c_void_p)]
+
+
 class LoopShape(ctypes.Structure):
     """ct3_loop_shape (include/ct3_b200.h): one update-loop pass."""
     _fields_ = [("T", ctypes.c_int), ("N", ctypes.c_int), ("H4", ctypes.c_int), ("W4", ctypes.c_int),
@@ -73,11 +78,17 @@ def _signatures():
                                            c_void_p]),
         "ct3_finish_tracks": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                       ctypes.c_float, ctypes.c_float, ctypes.c_float, c_void_p, c_void_p, c_void_p]),
+        "ct3_finish_tracks_scores": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                             c_int, c_int, c_int, ctypes.c_float, ctypes.c_float, ctypes.c_float,
+                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
         "ct3_online_window_begin": (c_int, [ctypes.POINTER(OnlineStream), c_int, c_int, c_int, c_int, c_int, c_void_p,
                                             c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_void_p, c_size_t, c_void_p]),
         "ct3_online_window_end": (c_int, [ctypes.POINTER(OnlineStream), c_int, c_int, c_int, c_void_p, c_void_p,
                                           c_void_p, c_int, ctypes.c_float, c_void_p, c_size_t, c_void_p]),
+        "ct3_online_window_end_scores": (c_int, [ctypes.POINTER(OnlineStream), c_int, c_int, c_int, c_void_p, c_void_p,
+                                                 c_void_p, c_int, ctypes.c_float, ctypes.POINTER(OnlineScores),
+                                                 c_void_p, c_size_t, c_void_p]),
         "ct3_render_prepare": (c_int, [c_void_p, c_int, c_int, c_int, c_int, i64, i64, i64, i64, c_int, c_int, c_void_p,
                                        c_void_p]),
         "ct3_render_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
@@ -335,14 +346,23 @@ def prepare_frames_yuv(src: torch.Tensor, layout: str, out_hw, out: Optional[tor
     return out
 
 
-def finish_tracks(fwd, bwd, queries: torch.Tensor, n_keep: int, threshold: float, scale_xy):
+def finish_tracks(fwd, bwd, queries: torch.Tensor, n_keep: int, threshold: float, scale_xy, scores: bool = False):
     """The predictor's tail in one kernel (ct3_finish_tracks in include/ct3_b200.h).  fwd = (tracks [B,T,N,2],
     visibility probabilities [B,T,N]) of the forward pass, bwd = the same of the pass on the clip played backwards (in
     reversed-clip time) or None, queries [B,N,3] at model resolution; all fp32 on one device.
-    -> (tracks [B,T,n_keep,2] fp32 scaled by scale_xy, visibility [B,T,n_keep] bool)."""
+    -> (tracks [B,T,n_keep,2] fp32 scaled by scale_xy, visibility [B,T,n_keep] bool).
+    scores=True: fwd and bwd also carry the confidence probabilities [B,T,N] third, and the result also holds the
+    merged, sliced vis and conf probabilities [B,T,n_keep] fp32, not pinned at the query points
+    (ct3_finish_tracks_scores, the same single pass)."""
+    width = 3 if scores else 2
     tensors = [("fwd tracks", fwd[0]), ("fwd visibility", fwd[1]), ("queries", queries)]
     if bwd is not None:
         tensors += [("bwd tracks", bwd[0]), ("bwd visibility", bwd[1])]
+    for name, pair in (("fwd", fwd), ("bwd", bwd)):
+        if pair is not None and len(pair) < width:
+            raise EngineError(f"{name} must hold (tracks, visibility{', confidence' if scores else ''})")
+        if pair is not None and scores:
+            tensors.append((f"{name} confidence", pair[2]))
     for name, t in tensors:
         _req(t, torch.float32, name)
     if queries.dim() != 3 or queries.shape[2] != 3:
@@ -357,10 +377,17 @@ def finish_tracks(fwd, bwd, queries: torch.Tensor, n_keep: int, threshold: float
     n_keep = int(n_keep)
     tracks = torch.empty(B, T, max(n_keep, 0), 2, dtype=torch.float32, device=dev)
     visibility = torch.empty(B, T, max(n_keep, 0), dtype=torch.bool, device=dev)
-    _call("ct3_finish_tracks", dev, _ptr(fwd[0]), _ptr(fwd[1]), _ptr(None if bwd is None else bwd[0]),
-          _ptr(None if bwd is None else bwd[1]), _ptr(queries), B, T, N, n_keep, float(threshold), float(scale_xy[0]),
-          float(scale_xy[1]), _ptr(tracks), _ptr(visibility), _stream(dev))
-    return tracks, visibility
+    tail = (float(threshold), float(scale_xy[0]), float(scale_xy[1]), _ptr(tracks), _ptr(visibility))
+    if not scores:
+        _call("ct3_finish_tracks", dev, _ptr(fwd[0]), _ptr(fwd[1]), _ptr(None if bwd is None else bwd[0]),
+              _ptr(None if bwd is None else bwd[1]), _ptr(queries), B, T, N, n_keep, *tail, _stream(dev))
+        return tracks, visibility
+    score_vis = torch.empty(B, T, max(n_keep, 0), dtype=torch.float32, device=dev)
+    score_conf = torch.empty_like(score_vis)
+    b = (None, None, None) if bwd is None else bwd
+    _call("ct3_finish_tracks_scores", dev, _ptr(fwd[0]), _ptr(fwd[1]), _ptr(fwd[2]), _ptr(b[0]), _ptr(b[1]),
+          _ptr(b[2]), _ptr(queries), B, T, N, n_keep, *tail, _ptr(score_vis), _ptr(score_conf), _stream(dev))
+    return tracks, visibility, score_vis, score_conf
 
 
 QUERY_FRAME_LIMIT = 1 << 30   # ct3_online_window_begin compares query frames clamped to +-2^30
@@ -429,18 +456,42 @@ def online_window_begin(streams, S: int, step: int, stride: int, T_pyr: int, qfr
 
 
 def online_window_end(streams, S: int, stride: int, coords: torch.Tensor, vis: torch.Tensor, conf: torch.Tensor,
-                      threshold: float = 0.6):
+                      threshold: float = 0.6, scores=None):
     """ct3_online_window_end: the loop's coords [S,N,2] / vis / conf [S,N] of one pass into the streams' histories,
-    and each entry's predictor output where it has one (see `online_stream`)."""
+    and each entry's predictor output where it has one (see `online_stream`).  scores: None, or per entry None or
+    (vis, conf) fp32 [rows, n_keep] tensors shaped as its output, which receive the sigmoids of its output's
+    visibility compare in the same launch (ct3_online_window_end_scores)."""
     for t, name in ((coords, "coords"), (vis, "vis"), (conf, "conf")):
         _req(t, torch.float32, name)
     N = vis.shape[1]
     dev = coords.device
     if tuple(coords.shape) != (S, N, 2) or tuple(vis.shape) != (S, N) or tuple(conf.shape) != (S, N):
         raise EngineError(f"coords, vis, conf must be [{S},N,2], [{S},N], [{S},N]")
-    table, ws = _online_table(streams, dev)
-    _call("ct3_online_window_end", dev, table, len(streams), int(S), int(stride), _ptr(coords), _ptr(vis), _ptr(conf),
-          N, float(threshold), _ptr(ws), ws.numel(), _stream(dev))
+    if scores is None:
+        table, ws = _online_table(streams, dev)
+        _call("ct3_online_window_end", dev, table, len(streams), int(S), int(stride), _ptr(coords), _ptr(vis),
+              _ptr(conf), N, float(threshold), _ptr(ws), ws.numel(), _stream(dev))
+        return
+    if len(scores) != len(streams):
+        raise EngineError(f"scores must hold one entry per stream ({len(streams)}), got {len(scores)}")
+    entries = []
+    for e, sc in zip(streams, scores):
+        if sc is None:
+            entries.append(OnlineScores(None, None))
+            continue
+        rows = int(e.ind) + int(e.T) - int(e.out_first)
+        if not e.tracks:
+            raise EngineError("a stream's scores need its output (online_stream(out=...))")
+        for t, name in ((sc[0], "score vis"), (sc[1], "score conf")):
+            _req(t, torch.float32, name)
+            if tuple(t.shape) != (rows, int(e.n_keep)) or t.device != dev:
+                raise EngineError(f"{name} must be [{rows},{int(e.n_keep)}] on {dev}, got {tuple(t.shape)}")
+        entries.append(OnlineScores(sc[0].data_ptr(), sc[1].data_ptr()))
+    table = (OnlineStream * max(1, len(streams)))(*streams)
+    sc_table = (OnlineScores * max(1, len(entries)))(*entries)
+    ws = torch.empty(ctypes.sizeof(table) + ctypes.sizeof(sc_table), dtype=torch.uint8, device=dev)
+    _call("ct3_online_window_end_scores", dev, table, len(streams), int(S), int(stride), _ptr(coords), _ptr(vis),
+          _ptr(conf), N, float(threshold), sc_table, _ptr(ws), ws.numel(), _stream(dev))
 
 
 def render_prepare(src: torch.Tensor, pad: int, grayscale: bool) -> torch.Tensor:

@@ -565,14 +565,14 @@ class CoTrackerThreeOffline(CoTrackerThreeBase):
                 self._batched(torch.sigmoid(conf), B), None)
 
 
-    def _track_ragged(self, pyr, H, W, groups, iters):
+    def _track_ragged(self, pyr, H, W, groups, iters, scores=False):
         """One update-loop pass over query groups of clips of different lengths in one pyramid (`_encode_clip` of
         the clips one after another, H x W frames).  groups: (queries [1,n,3] at model resolution in the group's own
         clip time, first pyramid frame f0 of its clip, clip length T_g, reversed) per group; a reversed group tracks its
         clip played backwards and reads the forward pyramid through its frame map.  The pass pads every group to the
         longest T_g (ct3_loop_shape.group_T); a padded step reads its group's last frame.
         -> [(tracks [1,T_g,n,2] at model resolution, visibility [1,T_g,n])] per group, each bit-identical to the
-        one-clip pass on that group (`_track_pyramid`)."""
+        one-clip pass on that group (`_track_pyramid`); scores=True appends the confidence [1,T_g,n] to each."""
         dev = pyr.device
         H4, W4 = H // self.stride, W // self.stride
         T = max(g[2] for g in groups)
@@ -593,7 +593,8 @@ class CoTrackerThreeOffline(CoTrackerThreeBase):
         self._refine(pyr, H4, W4, support, None, coords, vis, conf, iters, sizes, frame_map, lengths)
         out, a = [], 0
         for n, T_g in zip(sizes, lengths):
-            out.append(((coords[:T_g, a:a + n] * float(self.stride))[None], torch.sigmoid(vis[:T_g, a:a + n])[None]))
+            out.append(((coords[:T_g, a:a + n] * float(self.stride))[None], torch.sigmoid(vis[:T_g, a:a + n])[None])
+                       + ((torch.sigmoid(conf[:T_g, a:a + n])[None],) if scores else ()))
             a += n
         return out
 
@@ -661,14 +662,16 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
             return "the stream has reached the frame limit: a window must end by frame 2^30"
         return None
 
-    def _stream_step(self, pool: "StreamPool", streams, frames, Ts, iters, chunk=200, outputs=None):
+    def _stream_step(self, pool: "StreamPool", streams, frames, Ts, iters, chunk=200, outputs=None, scores=False):
         """Advance each of `streams` (states of `pool`, in pool order) by one window, in as few update-loop passes as
         fit in device memory.  frames [K*S,3,H,W] in [-1,1]: stream k's chunk of Ts[k] frames, padded to S frames with
         copies of its last frame.  outputs: per stream None, or (n_keep, scale_xy) for the online predictor's output
         of all its frames so far, or (n_keep, scale_xy, L) for that of its last L frames only (L <= ind + T; a bounded
         state's results need L <= its bound).  -> per stream None or (tracks [L,n_keep,2] fp32, visibility [L,n_keep]
-        bool), L = ind + T without a bound.  Every stream's result is bit-identical to advancing it alone: streams are
-        independent query groups, each reading its own S frames of one pyramid."""
+        bool), L = ind + T without a bound.  scores=True appends to each result its visibility and confidence
+        probabilities [L,n_keep] fp32, sigmoid(vis) and sigmoid(conf) of the history, written by the same launch
+        as the visibility.  Every stream's result is bit-identical to advancing it alone: streams are independent query
+        groups, each reading its own S frames of one pyramid."""
         K = len(streams)
         S = self.window_len
         step = S // 2
@@ -698,7 +701,7 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
                 idx = torch.cat([torch.arange(s.first, s.first + s.n) for s in sub]).to(dev)
                 support = pool.support.index_select(2, idx)
                 qframes, qcoords = pool.qframes[idx], pool.qcoords[idx]
-            entries, first = [], 0
+            entries, probs, first = [], [], 0
             for k, s in enumerate(sub, b0):
                 out, n_keep, scale, out_first = None, 0, (1.0, 1.0), 0
                 if outputs[k] is not None:
@@ -708,6 +711,11 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
                     out = (torch.empty(rows, n_keep, 2, device=dev), torch.empty(rows, n_keep, dtype=torch.bool,
                                                                                  device=dev))
                     results[k] = out
+                    if scores:
+                        probs.append((torch.empty(rows, n_keep, device=dev), torch.empty(rows, n_keep, device=dev)))
+                        results[k] = out + probs[-1]
+                if scores and out is None:
+                    probs.append(None)
                 entries.append(engine.online_stream(s.hist, s.length, s.ind, Ts[k], first, k * S, out, n_keep, scale,
                                                     out_first=out_first, ring=s.history is not None))
                 first += s.n
@@ -716,7 +724,7 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
             engine.sample_support(pyr, T_pyr, H4, W4, rel, qcoords, support=support, accumulate_mask=entering)
             frame_map = None if K == 1 else [[k * S + t for t in range(S)] for k in range(b0, b1)]
             self._refine(pyr, H4, W4, support, valid, coords, vis, conf, iters, [s.n for s in sub], frame_map)
-            engine.online_window_end(entries, S, self.stride, coords, vis, conf)
+            engine.online_window_end(entries, S, self.stride, coords, vis, conf, scores=probs if scores else None)
             if not in_place:
                 pool.support.index_copy_(2, idx, support)
         for s, T in zip(streams, Ts):
@@ -746,10 +754,11 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
         qframes = queries[:, 0].long().clamp(-lim, lim).to(torch.int32).contiguous()
         return qframes, (queries[:, 1:3].float() / self.stride).contiguous()
 
-    def _track_online(self, frames, queries, iters, chunk=200, predict=None):
+    def _track_online(self, frames, queries, iters, chunk=200, predict=None, scores=False):
         """One streaming step of the B streams of queries [B,N,3] in lockstep; frames [B*T,3,H,W] in [-1,1], T <=
         window_len.  -> the model's (coords, vis, conf) [B, frames so far, N, ...], or with predict = (n_keep,
-        scale_xy) the online predictor's (tracks [B,.,n_keep,2], visibility [B,.,n_keep] bool)."""
+        scale_xy) the online predictor's (tracks [B,.,n_keep,2], visibility [B,.,n_keep] bool), and with scores=True
+        also its visibility and confidence probabilities [B,.,n_keep] fp32."""
         B = queries.shape[0]
         T = frames.shape[0] // B
         S = self.window_len
@@ -759,10 +768,11 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
             v = frames.unflatten(0, (B, T))
             frames = torch.cat([v, v[:, -1:].expand(-1, S - T, -1, -1, -1)], 1).flatten(0, 1)
         pool, streams = self._lockstep_streams(queries)
-        outs = self._stream_step(pool, streams, frames, [T] * B, iters, chunk, [predict] * B)
+        outs = self._stream_step(pool, streams, frames, [T] * B, iters, chunk, [predict] * B,
+                                 scores=scores and predict is not None)
         self.online_ind += S // 2
         if predict is not None:
-            return tuple(torch.stack([o[i] for o in outs]) for i in range(2))
+            return tuple(torch.stack([o[i] for o in outs]) for i in range(len(outs[0])))
         L = streams[0].length
         coords, vis, conf = (torch.stack([s.hist[i][:L] for s in streams]) for i in range(3))
         return coords, torch.sigmoid(vis), torch.sigmoid(conf), None

@@ -14,8 +14,17 @@ A list of [1,T_b,3,H_b,W_b] clips of any lengths and sizes (offline model, spars
 per-clip `queries` / `segm_mask` lists; it returns lists, and entry b is bit-identical to the call on clip b alone.
 A clip, or an entry of such a list, may be a `YUVClip` (NV12, I420 or YUYV frames): results are `torch.equal` to the
 call on its RGB conversion by cv2.cvtColor.
+
+`return_scores=True` (both predictors) adds a third output, `TrackScores(visibility, confidence)`: the model's
+probabilities sigmoid(vis) and sigmoid(conf), fp32 on the device, of the visibility output's shape (a list of them for a
+list call).  They pass the same backward merge, support-grid drop and frame selection as the visibility.  The offline
+predictor's visibility is `scores.visibility > 0.9` except at the query points, which it pins to True while the scores
+keep the model's values there; the online predictor's is `scores.visibility * scores.confidence > 0.6`, bit for bit.
+Tracks and visibility are the same with and without the flag.
 """
 from __future__ import annotations
+
+from typing import NamedTuple
 
 import torch
 import torch.nn.functional as F
@@ -45,6 +54,18 @@ RAGGED_PAD_FRACTION = 0.1
 RAGGED_PAD_ROWS = 0
 
 
+class TrackScores(NamedTuple):
+    """Per-track, per-frame probabilities of the model, fp32 [B,T,N] on the device: `visibility` = sigmoid(vis),
+    `confidence` = sigmoid(conf) (reference cotracker3_offline.py:215-216, cotracker3_online.py:524-525)."""
+    visibility: torch.Tensor
+    confidence: torch.Tensor
+
+
+def _check_return_scores(return_scores):
+    if not isinstance(return_scores, bool):
+        raise ValueError(f"return_scores must be True or False, got {type(return_scores).__name__}")
+
+
 def get_points_on_a_grid(size: int, extent, device="cpu") -> torch.Tensor:
     """size x size query grid (x, y) over an (H, W) extent with a W/64 margin, row-major, shape [1, size^2, 2]
     (contract of reference model_utils.py:83-139 with the default centre)."""
@@ -71,23 +92,29 @@ class CoTrackerPredictor(torch.nn.Module):
 
     @torch.no_grad()
     def forward(self, video, queries: torch.Tensor = None, segm_mask: torch.Tensor = None, grid_size: int = 0,
-                grid_query_frame: int = 0, backward_tracking: bool = False):
+                grid_query_frame: int = 0, backward_tracking: bool = False, return_scores: bool = False):
+        """-> (tracks, visibility), or with return_scores=True (tracks, visibility, TrackScores) (module docstring)."""
+        _check_return_scores(return_scores)
         if isinstance(video, (list, tuple)):
-            return self._track_list(list(video), queries, segm_mask, grid_size, grid_query_frame, backward_tracking)
+            return self._track_list(list(video), queries, segm_mask, grid_size, grid_query_frame, backward_tracking,
+                                    return_scores)
         if segm_mask is not None and video.shape[0] != 1:
             raise ValueError("segm_mask keeps a different number of grid points per clip: it needs B == 1")
         if queries is None and grid_size == 0:
             return self._compute_dense_tracks(video, grid_query_frame=grid_query_frame,
-                                              backward_tracking=backward_tracking)
+                                              backward_tracking=backward_tracking, return_scores=return_scores)
         return self._compute_sparse_tracks(video, queries, segm_mask, grid_size,
                                            add_support_grid=(grid_size == 0 or segm_mask is not None),
-                                           grid_query_frame=grid_query_frame, backward_tracking=backward_tracking)
+                                           grid_query_frame=grid_query_frame, backward_tracking=backward_tracking,
+                                           return_scores=return_scores)
 
-    def _track_list(self, clips, queries, segm_mask, grid_size, grid_query_frame, backward_tracking):
+    def _track_list(self, clips, queries, segm_mask, grid_size, grid_query_frame, backward_tracking,
+                    return_scores=False):
         """Clips [1,T_b,3,H_b,W_b] of any lengths and sizes: one resize per clip into one frame buffer, one encoder
         pass, and as few update-loop passes as the memory budget and RAGGED_PAD_FRACTION allow, each clip's groups
         padded to the longest clip of their pass (ct3_loop_shape.group_T).  -> (tracks, visibility), lists in input
-        order, entry b bit-identical to the call on clip b with its own queries / segm_mask."""
+        order, entry b bit-identical to the call on clip b with its own queries / segm_mask; return_scores=True adds
+        a list of TrackScores."""
         B = len(clips)
         _check_list_call(self.model, clips, queries, segm_mask, grid_size, grid_query_frame)
         qs = [None] * B if queries is None else list(queries)
@@ -117,18 +144,16 @@ class CoTrackerPredictor(torch.nn.Module):
                                     sum(lengths), RAGGED_PAD_ROWS)
         outs = [None] * B
         for p in passes:
-            res = self.model._track_ragged(pyr, ih, iw, [g for b in p for g in groups[b]], _EncodedClip.ITERS)
+            res = self.model._track_ragged(pyr, ih, iw, [g for b in p for g in groups[b]], _EncodedClip.ITERS,
+                                           scores=return_scores)
             for b in p:
                 outs[b], res = res[:len(groups[b])], res[len(groups[b]):]
-        tracks, visibility = [], []
-        for b in range(B):
-            bwd = outs[b][1] if backward_tracking else None
-            tr, vi = self._finish(mq[b], outs[b][0], bwd, clips[b].shape, add[b])
-            tracks.append(tr)
-            visibility.append(vi)
-        return tracks, visibility
+        res = [self._finish(mq[b], outs[b][0], outs[b][1] if backward_tracking else None, clips[b].shape, add[b],
+                            return_scores) for b in range(B)]
+        return tuple(list(r) for r in zip(*res))
 
-    def _compute_dense_tracks(self, video, grid_query_frame, grid_size=80, backward_tracking=False):
+    def _compute_dense_tracks(self, video, grid_query_frame, grid_size=80, backward_tracking=False,
+                              return_scores=False):
         """grid_step^2 shifted grids, one query group per offset (and one reversed group per offset with backward
         tracking), tracked in as few grouped passes over one encoded clip as fit in device memory."""
         *_, H, W = video.shape
@@ -154,34 +179,39 @@ class CoTrackerPredictor(torch.nn.Module):
             for g in range(g0, g1):
                 if g % per == 0:
                     print(f"step {g // per} / {n_off}")
-            outs += clip.track_groups(groups[g0:g1], [g % per == 1 for g in range(g0, g1)])
-        tracks = visibilities = None
+            outs += clip.track_groups(groups[g0:g1], [g % per == 1 for g in range(g0, g1)], return_scores)
+        tracks = visibilities = probs = None
         for i in range(n_off):
-            t_step, v_step = self._finish(queries[i], outs[per * i], outs[per * i + 1] if backward_tracking else None,
-                                          video.shape)
+            step = self._finish(queries[i], outs[per * i], outs[per * i + 1] if backward_tracking else None,
+                                video.shape, scores=return_scores)
+            t_step, v_step = step[:2]
             tracks = t_step if tracks is None else torch.cat([tracks, t_step], dim=2)
             visibilities = v_step if visibilities is None else torch.cat([visibilities, v_step], dim=2)
-        return tracks, visibilities
+            if return_scores:
+                probs = step[2] if probs is None else TrackScores(*(torch.cat([a, b], dim=2)
+                                                                    for a, b in zip(probs, step[2])))
+        return (tracks, visibilities, probs) if return_scores else (tracks, visibilities)
 
     def _compute_sparse_tracks(self, video, queries, segm_mask=None, grid_size=0, add_support_grid=False,
-                               grid_query_frame=0, backward_tracking=False):
+                               grid_query_frame=0, backward_tracking=False, return_scores=False):
         clip = _EncodedClip(self.model, video, self.interp_shape)
         return self._sparse_tracks(clip, video.shape, queries, segm_mask, grid_size, add_support_grid,
-                                   grid_query_frame, backward_tracking)
+                                   grid_query_frame, backward_tracking, return_scores)
 
     def _sparse_tracks(self, clip, video_shape, queries, segm_mask=None, grid_size=0, add_support_grid=False,
-                       grid_query_frame=0, backward_tracking=False):
+                       grid_query_frame=0, backward_tracking=False, return_scores=False):
         queries = self._model_queries(clip, video_shape, queries, segm_mask, grid_size, add_support_grid,
                                       grid_query_frame)
         if backward_tracking:   # the clip played backwards (reference :187-209) is a reversed group
             inv = _reversed_queries(queries, clip.T)
             if queries.shape[1] * clip.loop_frames() <= BACKWARD_GROUP_TRACK_FRAMES:
-                fwd, bwd = clip.track_groups([queries, inv], [False, True])
+                fwd, bwd = clip.track_groups([queries, inv], [False, True], return_scores)
             else:
-                (fwd,), (bwd,) = clip.track_groups([queries], [False]), clip.track_groups([inv], [True])
+                (fwd,), (bwd,) = (clip.track_groups([queries], [False], return_scores),
+                                  clip.track_groups([inv], [True], return_scores))
         else:
-            (fwd,), bwd = clip.track_groups([queries], [False]), None
-        return self._finish(queries, fwd, bwd, video_shape, add_support_grid)
+            (fwd,), bwd = clip.track_groups([queries], [False], return_scores), None
+        return self._finish(queries, fwd, bwd, video_shape, add_support_grid, return_scores)
 
     def _model_queries(self, clip, video_shape, queries, segm_mask=None, grid_size=0, add_support_grid=False,
                        grid_query_frame=0):
@@ -208,16 +238,19 @@ class CoTrackerPredictor(torch.nn.Module):
             queries = torch.cat([queries, sup], dim=1)
         return queries
 
-    def _finish(self, queries, fwd, bwd, video_shape, add_support_grid=False):
+    def _finish(self, queries, fwd, bwd, video_shape, add_support_grid=False, scores=False):
         """(tracks, visibility) of the forward pass, merged with the backward pass's before each query frame
-        (reference :187-209), support grid dropped, query points pinned, scaled to the input (reference :161-190)."""
+        (reference :187-209), support grid dropped, query points pinned, scaled to the input (reference :161-190).
+        scores=True: fwd / bwd also hold the confidence third, and the result gains the TrackScores of the same merge
+        and columns, not pinned at the query points (one kernel still)."""
         B, T, C, H, W = video_shape
         ih, iw = self.interp_shape
         n_keep = queries.shape[1] - (self.support_grid_size ** 2 if add_support_grid else 0)
         # query points are, by definition, where they were asked for and visible (reference :173-185); one kernel
-        fwd, bwd = [None if p is None else (p[0].contiguous(), p[1].contiguous()) for p in (fwd, bwd)]
-        return engine.finish_tracks(fwd, bwd, queries.float().contiguous(), n_keep, 0.9,
-                                    ((W - 1) / (iw - 1), (H - 1) / (ih - 1)))
+        fwd, bwd = [None if p is None else tuple(x.contiguous() for x in p[:3 if scores else 2]) for p in (fwd, bwd)]
+        out = engine.finish_tracks(fwd, bwd, queries.float().contiguous(), n_keep, 0.9,
+                                   ((W - 1) / (iw - 1), (H - 1) / (ih - 1)), scores=scores)
+        return (out[0], out[1], TrackScores(out[2], out[3])) if scores else out
 
 
 class _Device:
@@ -283,11 +316,12 @@ class _EncodedClip:
         self.T = BT // self.B
         self.pyr = model._encode_clip(frames, B=self.B)
 
-    def track_groups(self, groups, reversed_groups):
+    def track_groups(self, groups, reversed_groups, scores=False):
         """Query groups [B,n_g,3] (model resolution) of every clip in one pass, or, when the batch does not fit in
         device memory, in one pass per sub-batch of clips (`plan_clip_passes`; groups are independent, so the split
         does not change a bit).  A flagged group tracks the clip played backwards, with query frames in reversed-clip
-        time.  -> [(tracks [B,T,n_g,2], visibility [B,T,n_g])] per group."""
+        time.  -> [(tracks [B,T,n_g,2], visibility [B,T,n_g])] per group, with the confidence [B,T,n_g] third when
+        `scores` (otherwise it is dropped at once)."""
         if any(q.shape[0] != self.B for q in groups):
             raise ValueError(f"every query group must hold the batch's {self.B} clips")
         sizes = [q.shape[1] for q in groups]
@@ -297,13 +331,14 @@ class _EncodedClip:
         if self.B > 1:
             T_loop, H4, W4, budget, _ = self.pass_shape(any(flags))
             passes = plan_clip_passes(self.B, sizes, T_loop, H4, W4, budget, lambda n: self.pass_frames(any(flags), n))
+        keep = 3 if scores else 2
         outs = [self.model._track_pyramid(self.pyr, self.T, self.H, self.W, queries[b0:b1], self.ITERS, sizes,
-                                          reversed_groups=flags, clips=None if len(passes) == 1 else range(b0, b1))[:2]
+                                          reversed_groups=flags, clips=None if len(passes) == 1 else range(b0, b1))[:keep]
                 for b0, b1 in passes]
-        tr, vi = outs[0] if len(outs) == 1 else (torch.cat([o[i] for o in outs], dim=0) for i in range(2))
+        res = outs[0] if len(outs) == 1 else tuple(torch.cat([o[i] for o in outs], dim=0) for i in range(len(outs[0])))
         out, a = [], 0
         for n in sizes:
-            out.append((tr[:, :, a:a + n], vi[:, :, a:a + n]))
+            out.append(tuple(x[:, :, a:a + n] for x in res))
             a += n
         return out
 
@@ -342,7 +377,10 @@ class CoTrackerOnlinePredictor(torch.nn.Module):
 
     @torch.no_grad()
     def forward(self, video_chunk, is_first_step: bool = False, queries: torch.Tensor = None, grid_size: int = 5,
-                grid_query_frame: int = 0, add_support_grid=False):
+                grid_query_frame: int = 0, add_support_grid=False, return_scores: bool = False):
+        """-> (tracks, visibility), or with return_scores=True (tracks, visibility, TrackScores) of the frames so far
+        (module docstring); (None, None[, None]) at the first step."""
+        _check_return_scores(return_scores)
         B, T, C, H, W = video_chunk.shape
         dev = ingest.model_device(self.model)
         if is_first_step:
@@ -350,12 +388,14 @@ class CoTrackerOnlinePredictor(torch.nn.Module):
             self.model.init_video_online_processing()
             self.queries, self.N = self._first_step_queries(B, (H, W), queries, grid_size, grid_query_frame,
                                                             add_support_grid, dev)
-            return (None, None)
+            return (None, None, None) if return_scores else (None, None)
 
         if self.queries.shape[0] != B:   # the B streams of the first step advance together
             raise ValueError(f"the video was started with {self.queries.shape[0]} streams, this chunk holds {B}")
         frames = ingest.prepare_video(video_chunk, self.interp_shape, dev)
-        return self.model._track_online(frames, self.queries, 6, predict=self._tail(add_support_grid, (H, W)))
+        out = self.model._track_online(frames, self.queries, 6, predict=self._tail(add_support_grid, (H, W)),
+                                       scores=return_scores)
+        return (out[0], out[1], TrackScores(out[2], out[3])) if return_scores else out
 
     def _first_step_queries(self, B, frame_hw, queries, grid_size, grid_query_frame, add_support_grid, dev):
         """The queries [B,N,3] at model resolution a video started with these first-step arguments tracks, and the

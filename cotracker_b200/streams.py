@@ -6,6 +6,7 @@
     hub.push(a, chunk_a)                            # [1,T,3,H,W], T <= window_len, uint8 or float, host or device
     hub.push(b, chunk_b)
     out = hub.step()                                # {stream id: (tracks [1,T_so_far,N,2], visibility [1,T_so_far,N])}
+    out = hub.step(return_scores=True)              # {stream id: (tracks, visibility, TrackScores(vis, conf))}
     hub.close(a)
     c = hub.open(frame_size=(720, 1280), grid_size=10, history=64)   # bounded: results of the last 64 frames only
 
@@ -21,6 +22,11 @@ its last L = min(h, frames so far) frames only, and a step's work does not grow 
 is then exactly the last L frames of the unbounded result, `full[:, -L:]`; `length(sid)` gives the stream's frame
 count, so the result covers frames [length - L, length).  A stream can advance until a window would pass frame
 2^30 (about 414 days at 30 fps); `push()` reports that limit.
+
+`step(return_scores=True)` adds each stream's `TrackScores`: sigmoid(vis) and sigmoid(conf) of its history, fp32
+[1,L,n] on the device, for the same frames and columns as its visibility, which is exactly their fp32 product > 0.6.
+All streams of a pass get them from the launch that writes their visibility.  They come from the history's logits, so
+a restored stream's scores continue bit for bit as well.
 
 A stream's tracks can change between steps:
 
@@ -63,6 +69,7 @@ import torch
 
 from . import corners, engine, ingest
 from .model import StreamPool, StreamState
+from .predictor import TrackScores, _check_return_scores
 
 SNAPSHOT_FORMAT = 1
 _SNAPSHOT_FIELDS = ("model", "frame_size", "n_keep", "ids", "next_id", "n", "ind", "length", "history", "support",
@@ -337,12 +344,15 @@ class OnlineStreams:
         s.update(ids=[i for i in s["ids"] if col[i] not in gone], out=(n_keep - len(gone), scale))
 
     @torch.no_grad()
-    def step(self) -> Dict[int, Tuple[torch.Tensor, torch.Tensor]]:
+    def step(self, return_scores: bool = False) -> Dict[int, tuple]:
         """Advance every stream with a pushed chunk by one window, in one pass.  -> {id: (tracks [1,L,n,2] fp32,
         visibility [1,L,n] bool)} of the streams it advanced, for their frames [length - L, length) with L = length
         (frames so far), or min(h, length) for a stream opened with history=h; the others keep their state.
         Frames before length - (window_len - step) (step = window_len // 2) are final: the next window re-tracks the
-        others."""
+        others.  return_scores=True adds a third value, TrackScores(visibility, confidence) [1,L,n] fp32: the model's
+        probabilities, with visibility == (scores.visibility * scores.confidence > 0.6).  An added track reads 0.5 for
+        both at the frames before its first window (logits 0)."""
+        _check_return_scores(return_scores)
         order = {id(s): k for k, s in enumerate(self.pool.streams)}
         ids = sorted(self._pending, key=lambda i: order[id(self._streams[i]["state"])])
         if not ids:
@@ -363,5 +373,7 @@ class OnlineStreams:
         states = [self._streams[i]["state"] for i in ids]
         outputs = [self._streams[i]["out"] if s.history is None else
                    (*self._streams[i]["out"], min(s.history, s.ind + T)) for i, s, T in zip(ids, states, Ts)]
-        outs = self.model._stream_step(self.pool, states, frames, Ts, 6, outputs=outputs)
+        outs = self.model._stream_step(self.pool, states, frames, Ts, 6, outputs=outputs, scores=return_scores)
+        if return_scores:
+            return {sid: (o[0][None], o[1][None], TrackScores(o[2][None], o[3][None])) for sid, o in zip(ids, outs)}
         return {sid: (tr[None], vi[None]) for sid, (tr, vi) in zip(ids, outs)}

@@ -186,6 +186,19 @@ int ct3_detect_corners(const float* frames, int64_t frame_stride, int K, int H, 
 int ct3_finish_tracks(const float* fwd_tracks, const float* fwd_vis, const float* bwd_tracks, const float* bwd_vis,
                       const float* queries, int B, int T, int N, int n_keep, float threshold, float scale_x,
                       float scale_y, float* tracks, uint8_t* visibility, ct3_stream_t stream);
+/* ct3_finish_tracks_scores: ct3_finish_tracks that also writes the model's probabilities of the output elements, in
+ * the same pass.  fwd_conf [B,T,N] (and bwd_conf with the backward pair) are the confidence probabilities next to
+ * fwd_vis (bwd_vis).  Output element (b, t, i) of score_vis / score_conf [B,T,n_keep] fp32 is the vis / conf value
+ * the merge selects, copied:  bwd_*[b, T-1-t, i] where the backward pass is given and (float)t < queries[b,i,0],
+ * fwd_*[b, t, i] elsewhere.  The query point is not pinned: at t == (int64)queries[b,i,0] it is the model's value
+ * while visibility there is 1.  tracks and visibility are bit-identical to ct3_finish_tracks.  The same checks as
+ * ct3_finish_tracks, plus a null fwd_conf, score_vis or score_conf, or bwd_conf given without the backward pair (or
+ * missing with it), return CT3_EINVAL before any launch. */
+int ct3_finish_tracks_scores(const float* fwd_tracks, const float* fwd_vis, const float* fwd_conf,
+                             const float* bwd_tracks, const float* bwd_vis, const float* bwd_conf, const float* queries,
+                             int B, int T, int N, int n_keep, float threshold, float scale_x, float scale_y,
+                             float* tracks, uint8_t* visibility, float* score_vis, float* score_conf,
+                             ct3_stream_t stream);
 
 /* ---- streaming windows (cotracker3_online.py:457-541, predictor.py:276-309) ------------------------------------
  * One update-loop pass of the online model advances K streams by one window each.  Stream k holds tracks
@@ -248,6 +261,25 @@ int ct3_online_window_begin(const ct3_online_stream* streams_host, int K, int S,
 int ct3_online_window_end(const ct3_online_stream* streams_host, int K, int S, int stride, const float* coords,
                           const float* vis, const float* conf, int N, float threshold, void* workspace,
                           size_t workspace_bytes, ct3_stream_t stream);
+/* The probabilities of one stream's output (ct3_online_window_end_scores): [ind + T - out_first, n_keep] fp32 each,
+ * rows and columns as the stream's tracks / visibility; both NULL for a stream without them. */
+typedef struct {
+  float* vis;             /* sigmoid(history_vis[f, j])                                                          */
+  float* conf;            /* sigmoid(history_conf[f, j])                                                         */
+} ct3_online_scores;
+/* ct3_online_window_end_scores: ct3_online_window_end in the same launch, and for every stream k whose scores_host[k]
+ * is set also
+ *   scores.vis[f - out_first, j] = sigmoid(history_vis[f, j]),  scores.conf[...] = sigmoid(history_conf[f, j])
+ *     for out_first <= f < ind + T, j < n_keep,
+ * the two factors of its visibility compare (so visibility == (vis * conf > threshold) element for element, fp32
+ * product).  scores_host is a HOST array of K entries, copied into `workspace` after the streams: the workspace holds
+ * at least K * (sizeof(ct3_online_stream) + sizeof(ct3_online_scores)) bytes.  Histories, tracks and visibility are
+ * bit-identical to ct3_online_window_end.  Its checks, plus a null scores_host, an entry with one pointer of the pair,
+ * or an entry set on a stream without `tracks` return CT3_EINVAL, a small workspace CT3_ENOSPC, before any launch. */
+int ct3_online_window_end_scores(const ct3_online_stream* streams_host, int K, int S, int stride, const float* coords,
+                                 const float* vis, const float* conf, int N, float threshold,
+                                 const ct3_online_scores* scores_host, void* workspace, size_t workspace_bytes,
+                                 ct3_stream_t stream);
 
 /* ---- track visualiser (reference cotracker/utils/visualizer.py) ---------------
  * Frames are uint8 [T,H,W,3] contiguous on the device, drawn in place; every result is bit-identical to the reference's
