@@ -302,7 +302,12 @@ int check_online(const ct3_online_stream* st, int K, int S, int step, int stride
       return fail(CT3_EINVAL, "a stream's history must have 0 <= len <= cap%s");
     if (s.ring && s.cap < S) return fail(CT3_EINVAL, "a ring history must hold at least S frames%s");
     const int64_t held = s.ring ? s.len - s.cap : 0;   // the first frame the history still holds
-    const bool reads = end || s.ind > 0;
+    // a preview (window_end only) writes no history: at ind = 0 it reads none either, so it may have none
+    const bool preview = end && s.preview;
+    if (end && s.preview != 0 && s.preview != 1) return fail(CT3_EINVAL, "a stream's preview must be 0 or 1%s");
+    if (preview && !s.tracks) return fail(CT3_EINVAL, "a preview entry needs an output (tracks)%s");
+    const bool no_history = !s.coords && !s.vis && !s.conf && s.cap == 0 && s.len == 0 && !s.ring;
+    const bool reads = (end || s.ind > 0) && !(preview && s.ind == 0 && no_history);
     if (reads && (!s.coords || !s.vis || !s.conf)) return fail(CT3_EINVAL, "a stream's history is null%s");
     if (reads && ((uintptr_t)s.coords & 7)) return fail(CT3_EINVAL, "history coords must be 8-byte aligned%s");
     int64_t elems = (int64_t)S * s.n;
@@ -312,7 +317,7 @@ int check_online(const ct3_online_stream* st, int K, int S, int step, int stride
       if (s.ind > 0 && s.ind < held) return fail(CT3_EINVAL, "the ring no longer holds the window's overlap frames%s");
     } else {
       const int64_t rows = (int64_t)s.ind + s.T;
-      if (!s.ring && s.cap < rows) return fail(CT3_EINVAL, "a stream's history must hold ind + T frames%s");
+      if (!s.ring && !preview && s.cap < rows) return fail(CT3_EINVAL, "a stream's history must hold ind + T frames%s");
       if (s.len < s.ind) return fail(CT3_EINVAL, "a stream's history must hold the frames before its window%s");
       int64_t lo = s.ind;   // the first frame the kernel touches
       if (s.tracks) {

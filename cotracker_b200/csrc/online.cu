@@ -7,7 +7,9 @@
 // division by a scalar.  Block (x, k) strides over the elements of stream k; the grid's y dimension is the stream.
 // With scores (ct3_online_window_end_scores) the two sigmoids of the visibility compare are stored as well.
 // A ring history (ring = 1) holds frame f at row f mod cap; the host checks guarantee that every frame a launch reads
-// is still held and that no row is both read and written by one window_end launch.
+// is still held and that no row is both read and written by one window_end launch.  A preview entry (preview = 1)
+// takes the same loads and arithmetic and skips the three history stores, so its output is that of the same entry
+// with preview = 0 and its history is left as it was.
 #include "../../include/ct3_b200.h"
 #include "kernels.cuh"
 
@@ -62,9 +64,11 @@ __global__ void __launch_bounds__(kOnlineThreads) online_window_begin_kernel(
   }
 }
 
-// kScores: also write the two probabilities of each output element where the stream's scores entry is set
+// kScores: also write the two probabilities of each output element where the stream's scores entry is set.
+// 8 blocks per SM: with the preview branch the kScores instantiation would otherwise take 40 registers (6 blocks);
+// with the bound both take 32 with no spills, as before the branch.
 template <bool kScores>
-__global__ void __launch_bounds__(kOnlineThreads) online_window_end_kernel(
+__global__ void __launch_bounds__(kOnlineThreads, 8) online_window_end_kernel(
     const ct3_online_stream* __restrict__ streams, const ct3_online_scores* __restrict__ scores, float stride,
     const float2* __restrict__ coords, const float* __restrict__ vis, const float* __restrict__ conf, int N,
     float threshold) {
@@ -72,6 +76,7 @@ __global__ void __launch_bounds__(kOnlineThreads) online_window_end_kernel(
   float* __restrict__ score_vis = kScores ? scores[blockIdx.y].vis : nullptr;
   float* __restrict__ score_conf = kScores ? scores[blockIdx.y].conf : nullptr;
   const int n = st.n, first = st.first, ind = st.ind, n_keep = st.n_keep;
+  const bool preview = st.preview != 0;   // read the history, never write it
   float2* __restrict__ hc = reinterpret_cast<float2*>(st.coords);
   float* __restrict__ hv = st.vis;
   float* __restrict__ hq = st.conf;
@@ -95,9 +100,11 @@ __global__ void __launch_bounds__(kOnlineThreads) online_window_end_kernel(
       p = make_float2(__fmul_rn(c.x, stride), __fmul_rn(c.y, stride));
       v = __ldg(vis + src);
       q = __ldg(conf + src);
-      hc[h] = p;
-      hv[h] = v;
-      hq[h] = q;
+      if (!preview) {
+        hc[h] = p;
+        hv[h] = v;
+        hq[h] = q;
+      }
     } else if (out) {   // an earlier frame: the history as it stands
       p = hc[h];
       v = hv[h];

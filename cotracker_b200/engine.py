@@ -34,6 +34,16 @@ class OnlineStream(ctypes.Structure):
                 ("scale_x", ctypes.c_float), ("scale_y", ctypes.c_float), ("out_first", ctypes.c_int64),
                 ("ring", ctypes.c_int32), ("pad", ctypes.c_int32)]
 
+    # The last field is ct3_online_stream.preview.  Its ctypes name stays `pad`, the C field's earlier name, so code
+    # written against the earlier binding keeps working; `preview` reads and writes the same field.
+    @property
+    def preview(self) -> int:
+        return self.pad
+
+    @preview.setter
+    def preview(self, value: int):
+        self.pad = value
+
 
 class OnlineScores(ctypes.Structure):
     """ct3_online_scores (include/ct3_b200.h): one stream's probability outputs of ct3_online_window_end_scores."""
@@ -395,22 +405,31 @@ STREAM_FRAME_LIMIT = 1 << 30  # ct3_online_window_* take a window at stream fram
 
 
 def online_stream(hist, length: int, ind: int, T: int, first: int, frame0: int, out=None, n_keep: int = 0,
-                  scale_xy=(1.0, 1.0), *, out_first: int = 0, ring: bool = False) -> OnlineStream:
+                  scale_xy=(1.0, 1.0), *, out_first: int = 0, ring: bool = False, preview: bool = False,
+                  n: Optional[int] = None) -> OnlineStream:
     """One entry of a streaming window pass (ct3_online_stream): hist = (coords [cap,n,2], vis [cap,n], conf [cap,n])
     fp32 histories with `length` frames written, the window at stream frame `ind` with T real frames, the stream's
     tracks from `first` in the pass and its window at pyramid frame `frame0`; out = (tracks [ind+T-out_first,n_keep,2]
     fp32, visibility [ind+T-out_first,n_keep] bool or uint8) for window_end's predictor output of stream frames
-    [out_first, ind+T), or None.  ring: the history holds frame f at row f mod cap (its last cap frames only)."""
-    c, v, q = hist
-    for t, dtype, name in ((c, torch.float32, "history coords"), (v, torch.float32, "history vis"),
-                           (q, torch.float32, "history conf")):
-        _req(t, dtype, name)
-    cap, n = v.shape
-    if tuple(c.shape) != (cap, n, 2) or tuple(q.shape) != (cap, n):
-        raise EngineError(f"histories must be [cap,n,2], [cap,n], [cap,n], got {tuple(c.shape)}, {tuple(v.shape)}, "
-                          f"{tuple(q.shape)}")
-    e = OnlineStream(c.data_ptr(), v.data_ptr(), q.data_ptr(), cap, int(length), None, None, int(ind), int(T), n,
-                     int(first), int(frame0), 0, float(scale_xy[0]), float(scale_xy[1]), int(out_first), int(bool(ring)))
+    [out_first, ind+T), or None.  ring: the history holds frame f at row f mod cap (its last cap frames only).
+    preview: window_end reads the history and writes none of it.  hist=None (with the stream's track count n): no
+    history, which only a preview at ind = 0 may have."""
+    if hist is None:
+        if n is None:
+            raise EngineError("an entry without a history needs its track count n")
+        ptrs, cap, n, ring = (None, None, None), 0, int(n), False
+    else:
+        c, v, q = hist
+        for t, dtype, name in ((c, torch.float32, "history coords"), (v, torch.float32, "history vis"),
+                               (q, torch.float32, "history conf")):
+            _req(t, dtype, name)
+        cap, n = v.shape
+        if tuple(c.shape) != (cap, n, 2) or tuple(q.shape) != (cap, n):
+            raise EngineError(f"histories must be [cap,n,2], [cap,n], [cap,n], got {tuple(c.shape)}, "
+                              f"{tuple(v.shape)}, {tuple(q.shape)}")
+        ptrs = (c.data_ptr(), v.data_ptr(), q.data_ptr())
+    e = OnlineStream(*ptrs, cap, int(length), None, None, int(ind), int(T), n, int(first), int(frame0), 0,
+                     float(scale_xy[0]), float(scale_xy[1]), int(out_first), int(bool(ring)), int(bool(preview)))
     if out is not None:
         tr, vi = out
         _req(tr, torch.float32, "tracks")

@@ -176,6 +176,9 @@ class StreamState:
         self.length = 0           # frames of history (written so far; a ring holds the last cap of them)
         self.hist = None          # (coords * stride [cap,n,2], vis [cap,n], conf [cap,n] logits); frames >= length unset
         self.enc = None           # (signatures [S-step,2], frame shape, pyramid) of the last chunk's overlap frames
+        # window position p -> (signature [2], frame shape, (pyramid, its frames, index)): the frames of the current
+        # window that previews encoded, for later previews and the step that commits the window
+        self.preview_enc = {}
 
     def ring_frames(self, S: int, step: int) -> int:
         """The ring of a bounded state, in frames.  A window at ind reads frames [ind + T - L, ind) for a result of
@@ -608,16 +611,23 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
         self._online_pool: Optional[StreamPool] = None
         self._online_streams: List[StreamState] = []
 
-    def _encode_online(self, frames, chunk, step, H4, W4, streams):
-        """frames [K*S,3,H,W]: the S-frame chunks of the K `streams`.  Consecutive online chunks of a stream overlap by
-        window_len - step frames and the encoder is strictly per-frame (InstanceNorm statistics are per sample), so the
-        features of the overlap are reused bit-for-bit from the stream's previous window and only the new frames are
-        encoded (SURVEY.md 8(f1): the reference re-encodes all 16).  A stream whose overlap does not match its cache is
-        encoded whole, in the same encoder pass as the other streams' new frames.  Each stream then keeps the features
-        of its chunk's last window_len - step frames, and only those."""
+    def _encode_online(self, frames, chunk, step, H4, W4, streams, Ts=None, previews=None):
+        """frames [K*S,3,H,W]: the S-frame chunks of the K `streams`, stream k's of Ts[k] real frames (default S).
+        Consecutive online chunks of a stream overlap by window_len - step frames and the encoder is strictly per-frame
+        (InstanceNorm statistics are per sample), so the features of the overlap are reused bit-for-bit from the
+        stream's previous window and only the new frames are encoded (SURVEY.md 8(f1): the reference re-encodes all
+        16).  A stream whose overlap does not match its cache is encoded whole, in the same encoder pass as the other
+        streams' new frames.  Each stream then keeps the features of its chunk's last window_len - step frames, and
+        only those.
+        previews[k]: stream k's chunk is a preview.  Its real frames whose signature matches a frame that an earlier
+        preview of the window encoded at the same position are reused (for a committing chunk as well), its padding
+        frames take the features of its last real frame, the frames it encodes join the stream's `preview_enc`, and
+        its `enc` is left as it is.  A committing chunk empties `preview_enc`: the window moves on."""
         K = len(streams)
         S = frames.shape[0] // K
         keep = S - step
+        Ts = Ts or [S] * K
+        previews = previews or [False] * K
         shape = tuple(frames.shape[1:])
         # [K,S,2] float64: one pass over the chunks; one flag per stream goes to the host
         sig = self._frame_signatures(frames).unflatten(0, (K, S))
@@ -627,26 +637,64 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
             prev = torch.stack([streams[k].enc[0] for k in cand])
             for k, eq in zip(cand, (sig[cand, :keep] == prev).flatten(1).all(1).tolist()):
                 same[k] = eq
-        if any(same):
-            v = frames.unflatten(0, (K, S))
-            fresh = [v[k, keep:] if same[k] else v[k] for k in range(K)]
-            fresh = fresh[0] if K == 1 else torch.cat(fresh, 0)
-            new = self._encode(fresh.contiguous(), chunk)
-            runs, n = [], 0
-            for k in range(K):
-                if same[k]:
-                    runs.append((streams[k].enc[2], keep, 0, keep))
-                m = step if same[k] else S
-                runs.append((new, fresh.shape[0], n, n + m))
-                n += m
-            pyr = engine.concat_pyramid_runs(runs, H4, W4)
+        hits = [{} for _ in range(K)]   # position -> (pyramid, frames, index) of a frame a preview encoded
+        look = [(k, p) for k, s in enumerate(streams) for p, (_, shp, _) in s.preview_enc.items()
+                if p < Ts[k] and not (same[k] and p < keep) and shp == shape]
+        if look:
+            prev = torch.stack([streams[k].preview_enc[p][0] for k, p in look])
+            at = torch.tensor([k * S + p for k, p in look], device=sig.device)
+            for (k, p), eq in zip(look, (sig.flatten(0, 1)[at] == prev).all(1).tolist()):
+                if eq:
+                    hits[k][p] = streams[k].preview_enc[p][2]
+        # the source of each window frame: (pyramid, its frames, index), pyramid None = the j-th frame encoded here
+        src, fresh = [], []
+        for k, s in enumerate(streams):
+            for p in range(S):
+                if same[k] and p < keep:
+                    src.append((s.enc[2], keep, p))
+                elif p in hits[k]:
+                    src.append(hits[k][p])
+                elif previews[k] and p >= Ts[k]:   # padding: a copy of the last real frame
+                    src.append(src[k * S + Ts[k] - 1])
+                else:
+                    src.append((None, 0, len(fresh)))
+                    fresh.append(k * S + p)
+        if len(fresh) == K * S:
+            pyr = new = self._encode(frames, chunk)
         else:
-            pyr = self._encode(frames, chunk)
-        if keep > 0:
-            for k, s in enumerate(streams):
-                s.enc = (sig[k, step:], shape, engine.concat_pyramid_runs([(pyr, K * S, k * S + step, (k + 1) * S)],
-                                                                          H4, W4))
+            new = None
+            if fresh:
+                at = torch.tensor(fresh, device=frames.device)
+                new = self._encode(frames.index_select(0, at), chunk)
+            pyr = engine.concat_pyramid_runs(self._frame_runs(src, new, len(fresh)), H4, W4)
+        for k, s in enumerate(streams):
+            if not previews[k]:
+                s.preview_enc = {}
+                if keep > 0:
+                    s.enc = (sig[k, step:], shape, engine.concat_pyramid_runs(
+                        [(pyr, K * S, k * S + step, (k + 1) * S)], H4, W4))
+                continue
+            mine = [p for p in range(Ts[k]) if src[k * S + p][0] is None]
+            if mine:
+                own = engine.concat_pyramid_runs(self._frame_runs([src[k * S + p] for p in mine], new, len(fresh)),
+                                                 H4, W4)
+                for i, p in enumerate(mine):
+                    s.preview_enc[p] = (sig[k, p].clone(), shape, (own, len(mine), i))
         return pyr
+
+    @staticmethod
+    def _frame_runs(src, new, n_new):
+        """`concat_pyramid_runs` runs of the frame sources (pyramid, frames, index), consecutive frames of one pyramid
+        merged into one run; pyramid None = frame `index` of `new`, the n_new frames encoded in this call."""
+        runs = []
+        for pyr, T, i in src:
+            if pyr is None:
+                pyr, T = new, n_new
+            if runs and runs[-1][0] is pyr and runs[-1][3] == i:
+                runs[-1][3] = i + 1
+            else:
+                runs.append([pyr, T, i, i + 1])
+        return [tuple(r) for r in runs]
 
     def stream_advance_error(self, state: "StreamState", T: int) -> Optional[str]:
         """Why `state` cannot advance by a chunk of T frames (None: it can).  The history of a stream is the window
@@ -662,7 +710,16 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
             return "the stream has reached the frame limit: a window must end by frame 2^30"
         return None
 
-    def _stream_step(self, pool: "StreamPool", streams, frames, Ts, iters, chunk=200, outputs=None, scores=False):
+    def stream_preview_error(self, state: "StreamState", T: int) -> Optional[str]:
+        """Why a chunk of T frames cannot preview `state` (None: it can), on top of `stream_advance_error`: a preview
+        holds frames [ind, ind + T) and must add at least one frame after the stream's last, T > length - ind."""
+        if T <= state.length - state.ind:
+            return (f"a preview chunk holds frames [{state.ind}, f] and must add a frame after frame {state.length - 1}:"
+                    f" T must be > {state.length - state.ind}, got {T}")
+        return None
+
+    def _stream_step(self, pool: "StreamPool", streams, frames, Ts, iters, chunk=200, outputs=None, scores=False,
+                     previews=None):
         """Advance each of `streams` (states of `pool`, in pool order) by one window, in as few update-loop passes as
         fit in device memory.  frames [K*S,3,H,W] in [-1,1]: stream k's chunk of Ts[k] frames, padded to S frames with
         copies of its last frame.  outputs: per stream None, or (n_keep, scale_xy) for the online predictor's output
@@ -671,22 +728,30 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
         bool), L = ind + T without a bound.  scores=True appends to each result its visibility and confidence
         probabilities [L,n_keep] fp32, sigmoid(vis) and sigmoid(conf) of the history, written by the same launch
         as the visibility.  Every stream's result is bit-identical to advancing it alone: streams are independent query
-        groups, each reading its own S frames of one pyramid."""
+        groups, each reading its own S frames of one pyramid.
+        previews[k] (default False): stream k's chunk is a preview, which needs an output.  Its result is the one the
+        chunk would give, and the stream is left as it was: its support features are accumulated in pass scratch and
+        not written back, its history is read and not written, and its window start, length and overlap features stay
+        (`_encode_online` keeps the frames it encodes for the window's later chunks)."""
         K = len(streams)
         S = self.window_len
         step = S // 2
         _, _, H, W = frames.shape
         H4, W4 = H // self.stride, W // self.stride
         dev = frames.device
-        for s, T in zip(streams, Ts):
-            err = self.stream_advance_error(s, T)
+        outputs = outputs or [None] * K
+        previews = previews or [False] * K
+        for s, T, pv, out in zip(streams, Ts, previews, outputs):
+            err = self.stream_advance_error(s, T) or (pv and self.stream_preview_error(s, T))
             if err:
                 raise ValueError(err)
-        outputs = outputs or [None] * K
-        pyr = self._encode_online(frames, chunk, step, H4, W4, streams)
+            if pv and out is None:
+                raise ValueError("a preview needs an output")
+        pyr = self._encode_online(frames, chunk, step, H4, W4, streams, Ts, previews)
         T_pyr = K * S
-        for s, T in zip(streams, Ts):
-            s.reserve(s.ind + T if s.history is None else s.ring_frames(S, step), dev)
+        for s, T, pv in zip(streams, Ts, previews):
+            if not pv:
+                s.reserve(s.ind + T if s.history is None else s.ring_frames(S, step), dev)
         passes = [(0, K)]
         if K > 1:
             budget = pass_budget_bytes(self, dev, T_pyr, H, W)
@@ -694,10 +759,11 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
         results = [None] * K
         for b0, b1 in passes:
             sub = streams[b0:b1]
-            in_place = sub == pool.streams
+            commits = [not pv for pv in previews[b0:b1]]
+            in_place = sub == pool.streams and all(commits)
             if in_place:
                 support, qframes, qcoords = pool.support, pool.qframes, pool.qcoords
-            else:   # the support rows of these streams in pass scratch, written back after the pass
+            else:   # the support rows of these streams in pass scratch, those of committing streams written back
                 idx = torch.cat([torch.arange(s.first, s.first + s.n) for s in sub]).to(dev)
                 support = pool.support.index_select(2, idx)
                 qframes, qcoords = pool.qframes[idx], pool.qcoords[idx]
@@ -717,7 +783,8 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
                 if scores and out is None:
                     probs.append(None)
                 entries.append(engine.online_stream(s.hist, s.length, s.ind, Ts[k], first, k * S, out, n_keep, scale,
-                                                    out_first=out_first, ring=s.history is not None))
+                                                    out_first=out_first, ring=s.history is not None,
+                                                    preview=previews[k], n=s.n))
                 first += s.n
             valid, entering, rel, coords, vis, conf = engine.online_window_begin(entries, S, step, self.stride, T_pyr,
                                                                                  qframes, qcoords)
@@ -725,11 +792,20 @@ class CoTrackerThreeOnline(CoTrackerThreeBase):
             frame_map = None if K == 1 else [[k * S + t for t in range(S)] for k in range(b0, b1)]
             self._refine(pyr, H4, W4, support, valid, coords, vis, conf, iters, [s.n for s in sub], frame_map)
             engine.online_window_end(entries, S, self.stride, coords, vis, conf, scores=probs if scores else None)
-            if not in_place:
+            if in_place:
+                continue
+            if all(commits):
                 pool.support.index_copy_(2, idx, support)
-        for s, T in zip(streams, Ts):
-            s.length = s.ind + T
-            s.ind += step
+            elif any(commits):
+                offs = [0]
+                for s in sub:
+                    offs.append(offs[-1] + s.n)
+                cols = torch.cat([torch.arange(offs[i], offs[i + 1]) for i, c in enumerate(commits) if c]).to(dev)
+                pool.support.index_copy_(2, idx[cols], support.index_select(2, cols))
+        for s, T, pv in zip(streams, Ts, previews):
+            if not pv:
+                s.length = s.ind + T
+                s.ind += step
         return results
 
     def _lockstep_streams(self, queries):

@@ -28,6 +28,18 @@ count, so the result covers frames [length - L, length).  A stream can advance u
 All streams of a pass get them from the launch that writes their visibility.  They come from the history's logits, so
 a restored stream's scores continue bit for bit as well.
 
+A stream gives results at every frame with previews:
+
+    w = max(0, hub.length(a) - (window_len - window_len // 2))   # the current window start
+    hub.push(a, frames[:, w:f + 1], preview=True)   # any f >= hub.length(a): frames [w, f]
+    out = hub.step()                                # a's result as if its video ended at frame f; a is not advanced
+
+A preview is the reference's last chunk (the window from its start to frame f, padded with copies of frame f) without
+ending the stream: `step()` returns what the chunk pushed without the flag would return, in the same pass as the other
+streams, and leaves the stream exactly as it was before the push (its snapshot is unchanged).  Frames before
+length - (window_len - step) are final; later ones are provisional, a preview's newest frames the most.  The frames a
+preview encodes are kept for the window's later previews and its committing step, so each camera frame is encoded once.
+
 A stream's tracks can change between steps:
 
     hub.retire_tracks(c, [3, 7])                    # ids of track_ids(c); the support grid's points have none
@@ -162,6 +174,7 @@ class OnlineStreams:
         self.pool = StreamPool()
         self._streams: Dict[int, dict] = {}     # id -> the stream's state, open arguments and output shape
         self._pending: Dict[int, torch.Tensor] = {}
+        self._previews = set()                  # ids of the pending chunks pushed with preview=True
         self._next_id = 0
 
     @torch.no_grad()
@@ -210,23 +223,35 @@ class OnlineStreams:
         with L the result's frame count."""
         return self._get(sid)["state"].length
 
-    def push(self, sid: int, chunk: torch.Tensor):
+    def push(self, sid: int, chunk: torch.Tensor, preview: bool = False):
         """Queue the next chunk [1,T,3,H,W] of stream `sid` (T <= window_len), or a `YUVClip` of it, for the next
-        `step()`."""
+        `step()`.  preview=True: the chunk holds frames [w, f] of the stream, w = max(0, length - (window_len - step))
+        the current window start and f > length - 1 the newest frame, of any T allowed; `step()` returns for `sid`
+        exactly what it would return for the chunk pushed without the flag (a result ending at frame f) and leaves the
+        stream as it was before this push: length, window start, track ids, history and support are unchanged, a short
+        chunk does not end the stream, and no chunk stays pending.  Track edits made before the step are seen by it and
+        stay.  A preview's frames after length - (window_len - step) are provisional, its newest ones the most."""
         s = self._get(sid)
+        if not isinstance(preview, bool):
+            raise ValueError(f"preview must be a bool, got {preview!r}")
         if sid in self._pending:
             raise ValueError(f"stream {sid} already has a chunk for this step")
         if chunk.dim() != 5 or chunk.shape[0] != 1 or chunk.shape[2] != 3 or tuple(chunk.shape[3:]) != s["hw"]:
             raise ValueError(f"stream {sid} takes chunks [1,T,3,{s['hw'][0]},{s['hw'][1]}], got {tuple(chunk.shape)}")
         err = self.model.stream_advance_error(s["state"], chunk.shape[1])
+        if not err and preview:
+            err = self.model.stream_preview_error(s["state"], chunk.shape[1])
         if err:
             raise ValueError(f"stream {sid}: {err}")
         self._pending[sid] = chunk
+        if preview:
+            self._previews.add(sid)
 
     def close(self, sid: int):
         """End stream `sid`: its tracks leave the pool and its id is no longer valid."""
         s = self._get(sid)
         self._pending.pop(sid, None)
+        self._previews.discard(sid)
         self.pool.close(s["state"])
         del self._streams[sid]
 
@@ -351,7 +376,9 @@ class OnlineStreams:
         Frames before length - (window_len - step) (step = window_len // 2) are final: the next window re-tracks the
         others.  return_scores=True adds a third value, TrackScores(visibility, confidence) [1,L,n] fp32: the model's
         probabilities, with visibility == (scores.visibility * scores.confidence > 0.6).  An added track reads 0.5 for
-        both at the frames before its first window (logits 0)."""
+        both at the frames before its first window (logits 0).  A stream pushed with preview=True gets the same result
+        for its frames [ind + T - L, ind + T) and is not advanced (see `push`); previews and committing chunks share the
+        pass."""
         _check_return_scores(return_scores)
         order = {id(s): k for k, s in enumerate(self.pool.streams)}
         ids = sorted(self._pending, key=lambda i: order[id(self._streams[i]["state"])])
@@ -369,11 +396,14 @@ class OnlineStreams:
             if T < S:   # the model pads a short chunk with copies of its last frame
                 frames[k * S + T:(k + 1) * S] = frames[k * S + T - 1]
             Ts.append(T)
+        previews = [sid in self._previews for sid in ids]
         self._pending.clear()
+        self._previews.clear()
         states = [self._streams[i]["state"] for i in ids]
         outputs = [self._streams[i]["out"] if s.history is None else
                    (*self._streams[i]["out"], min(s.history, s.ind + T)) for i, s, T in zip(ids, states, Ts)]
-        outs = self.model._stream_step(self.pool, states, frames, Ts, 6, outputs=outputs, scores=return_scores)
+        outs = self.model._stream_step(self.pool, states, frames, Ts, 6, outputs=outputs, scores=return_scores,
+                                       previews=previews)
         if return_scores:
             return {sid: (o[0][None], o[1][None], TrackScores(o[2][None], o[3][None])) for sid, o in zip(ids, outs)}
         return {sid: (tr[None], vi[None]) for sid, (tr, vi) in zip(ids, outs)}

@@ -225,8 +225,15 @@ typedef struct {
   float scale_x, scale_y; /* window_end: output tracks = history * (scale_x, scale_y), one fp32 multiply each     */
   int64_t out_first;      /* window_end: the first stream frame of the output (0: every frame so far)           */
   int32_t ring;           /* 0: frame f at history row f; 1: frame f at row f mod cap                          */
-  int32_t pad;            /* keeps the struct a multiple of 8 bytes; set to 0                                    */
+  int32_t preview;        /* window_end: 0 writes the window into the history; 1 (a preview) reads it only       */
 } ct3_online_stream;
+/* A preview entry (preview = 1) gives window_end's output of the same entry with preview = 0, bit for bit, and leaves
+ * its history untouched: output frames [ind, ind + T) come straight from the loop's result, earlier ones from the
+ * history as it stands.  So a stream can show the result it would give if its video ended at frame ind + T - 1
+ * without ending.  A preview needs an output (`tracks`) and no history room for its window: with ring = 0, cap >= len
+ * suffices.  At ind = 0 neither kernel reads the history, so a preview entry there may have null history pointers
+ * with cap = len = 0 and ring = 0: a stream that has not taken its first step needs no history for a preview.
+ * window_begin ignores the field. */
 /* ct3_online_window_begin: the per-window state the update loop starts from, bit-identical to the torch expressions
  * (qf = qframes[i], the query frame in stream time; overlap = S - step):
  *   valid[i] = qf < ind + S;   entering[i] = left <= qf < ind + S with left = 0 at ind == 0, else ind + step;
@@ -257,7 +264,8 @@ int ct3_online_window_begin(const ct3_online_stream* streams_host, int K, int S,
  * n_keep is outside [1, n] or out_first is outside [0, ind + T), and with ring = 0 cap < ind + T.  With ring = 1 also
  * (`tracks` set) an output frame before the window that the ring no longer holds (out_first < min(ind, len - cap)),
  * or an output longer than the ring (ind + T - out_first > cap: a frame the launch reads would share its row with one
- * it writes). */
+ * it writes).  So does preview outside {0, 1} or a preview entry without `tracks`; a preview entry is exempt from
+ * cap >= ind + T, and at ind = 0 from the null-history check when its history is null with cap = len = ring = 0. */
 int ct3_online_window_end(const ct3_online_stream* streams_host, int K, int S, int stride, const float* coords,
                           const float* vis, const float* conf, int N, float threshold, void* workspace,
                           size_t workspace_bytes, ct3_stream_t stream);
