@@ -765,15 +765,30 @@ def update_loop(packed, pyr, H4, W4, support, track_valid, coords, vis, conf, ti
 
 
 # ---- stage-level wrappers (tests, profiles) -----------------------------------------------------------
-def corr_sample(pyr, H4, W4, support, track_valid, coords, scratch: bool = True) -> torch.Tensor:
+def corr_sample(pyr, H4, W4, support, track_valid, coords, scratch=True,
+                vol: Optional[torch.Tensor] = None) -> torch.Tensor:
     """-> fp32 correlation volume [N, T, 4, 2401] reconstructed from the split-bf16 device layout.
-    scratch=False withholds the split-pyramid scratch, i.e. selects the sample-then-correlate kernel."""
+    scratch=False withholds the split-pyramid scratch, i.e. selects the sample-then-correlate kernel; a uint8 tensor is
+    used as that scratch (the pyramid copy the correlate-then-interpolate kernels read stays in it).
+    vol: a caller-owned bf16 buffer of at least N*T*4 rows of 2*2432; the volume is written to its first rows and the
+    buffer is returned undecoded (volume_planes decodes it)."""
     T, N, _ = coords.shape
-    vol = torch.zeros(N * T * LEVELS, 2 * VOL_PAD, dtype=torch.bfloat16, device=coords.device)
-    scr = torch.empty(pyr.numel() * 4, dtype=torch.uint8, device=coords.device) if scratch else None
+    rows = N * T * LEVELS
+    if vol is None:
+        out = torch.zeros(rows, 2 * VOL_PAD, dtype=torch.bfloat16, device=coords.device)
+    else:
+        out = _req(vol, torch.bfloat16, "vol")
+        if out.dim() != 2 or out.shape[1] != 2 * VOL_PAD or out.shape[0] < rows:
+            raise EngineError(f"vol must be [>= {rows}, {2 * VOL_PAD}], got {tuple(out.shape)}")
+    if isinstance(scratch, torch.Tensor):
+        scr = _req(scratch, torch.uint8, "scratch")
+    else:
+        scr = torch.empty(pyr.numel() * 4, dtype=torch.uint8, device=coords.device) if scratch else None
     _call("ct3_corr_sample", coords.device, _ptr(pyr), H4, W4, _ptr(support), _ptr(track_valid), _ptr(coords), T, N,
-          _ptr(vol), _ptr(scr), scr.numel() if scratch else 0, _stream(coords.device))
-    return volume_planes(vol, T, N, H4, W4, scratch).sum(0).reshape(N, T, LEVELS, VOL)
+          _ptr(out), _ptr(scr), 0 if scr is None else scr.numel(), _stream(coords.device))
+    if vol is not None:
+        return out
+    return volume_planes(out, T, N, H4, W4, scr is not None).sum(0).reshape(N, T, LEVELS, VOL)
 
 
 def volume_planes(vol: torch.Tensor, T: int, N: int, H4: int, W4: int, patch: bool = True) -> torch.Tensor:

@@ -308,14 +308,16 @@ def test_options_are_validated_and_thread_local():
 
 
 def test_corr_shift_pattern_covers_every_sample():
-    """fp32 restatement of box_origin8 / tap_weights (csrc/corr_tc3.cu).  The transposed correlation kernel blends the
-    8x8 raw correlations with STATIC register indices: per frame and axis the two taps of sample a are box entries
-    clamp07(a + d) and clamp07(a + d + 1) for one shift d = clamp(floor(clamp(c)) - 3 - origin, -7, 7).  This test
-    brute-forces, for every map size >= 8 and every coordinate class (far outside, on texel centres, a few ulps either
-    side), that the border-clamped bilinear taps of all 7 samples -- computed exactly as grid_sample does -- ARE that
-    pattern with weights (1 - w, w), or (0, 1) when c + offset rounded up to an integer; and that the blend value equals
-    the straightforward two-tap evaluation.  The kernel traps otherwise; this is the proof that it never does."""
+    """fp32 restatement of box_origin8 / tap_weights (csrc/corr_tc3.cu; tests/corr_cases.py).  The transposed
+    correlation kernel blends the 8x8 raw correlations with STATIC register indices: per frame and axis the two taps of
+    sample a are box entries clamp07(a + d) and clamp07(a + d + 1) for one shift d = clamp(floor(clamp(c)) - 3 - origin,
+    -7, 7).  This test brute-forces, for every map size >= 8 and every coordinate class (far outside, on texel centres,
+    a few ulps either side), that the border-clamped bilinear taps of all 7 samples -- computed exactly as grid_sample
+    does -- ARE that pattern with weights (1 - w, w), or (0, 1) when c + offset rounded up to an integer; and that the
+    blend value equals the straightforward two-tap evaluation.  The kernel traps otherwise; this is the proof that it
+    never does."""
     import numpy as np
+    from corr_cases import box_origin8, tap_weights
     f32 = np.float32
     rng = np.random.default_rng(1)
     for size in (8, 9, 12, 16, 24, 48, 96, 128, 1000):
@@ -326,25 +328,12 @@ def test_corr_shift_pattern_covers_every_sample():
             lo, hi = np.nextafter(lo, f32(-1e9)), np.nextafter(hi, f32(1e9))
             near += [lo.copy(), hi.copy()]
         c = np.concatenate([rng.uniform(-40, size + 40, 200000).astype(f32), np.array([-1e9, 1e9, 0.5, size - 0.5], dtype=f32)] + near)
-        cc = np.minimum(np.maximum(c, f32(-16)), f32(size + 16)).astype(f32)
-        base = np.floor(cc).astype(np.int64) - 3
-        origin = np.clip(base, 0, size - 8)
-        d = np.clip(base - origin, -7, 7)
+        origin, d = box_origin8(c, size)
         box = rng.standard_normal((len(c), 8)).astype(f32)            # the 8 box entries along this axis
         rows = np.arange(len(c))
         for a in range(7):
-            x = np.minimum(np.maximum((c + f32(a - 3)).astype(f32), f32(0)), f32(size - 1)).astype(f32)
-            xf = np.floor(x)
-            x0 = xf.astype(np.int64)
-            fr = (x - xf).astype(f32)
-            s0 = np.clip(x0 - origin, 0, 7)
-            s1 = np.where(fr > 0, np.clip(np.minimum(x0 + 1, size - 1) - origin, 0, 7), s0)
-            i0, i1 = np.clip(a + d, 0, 7), np.clip(a + d + 1, 0, 7)
-            direct = (s0 == i0) & ((fr == 0) | (s1 == i1))
-            rounded = (~direct) & (fr == 0) & (s0 == i1)
-            assert bool((direct | rounded).all()), (size, a, c[~(direct | rounded)][:5])
-            u = np.where(direct, f32(1) - fr, f32(0)).astype(f32)
-            w = np.where(direct, fr, f32(1)).astype(f32)
+            branch, u, w, s0, s1, i0, i1, fr = tap_weights(c, a, size, origin, d)
+            assert bool((branch != 0).all()), (size, a, c[branch == 0][:5])
             want = (f32(1) - fr) * box[rows, s0] + fr * box[rows, s1]
             got = u * box[rows, i0] + w * box[rows, i1]
             assert np.array_equal(want.astype(f32), got.astype(f32)), (size, a)
