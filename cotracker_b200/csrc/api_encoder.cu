@@ -41,13 +41,19 @@ EncWs enc_carve(void* base, int T, int H4, int W4) {
 // The end of both encoders for frames [t0, t0+tc) of T: conv3 (1x1, 256 -> 128) of the split rows ys straight into
 // level 0 of the pyramid (its rows (t,y,x) are the channels-last texels), L2-normalised; after the last chunk, the
 // pools of levels 1..3.
+// A trace sink (ct3_encoder_trace) takes a copy of conv3's output between the GEMM and the in-place L2 norm.
+struct EncTrace;
+int trace_put(EncTrace* tr, const void* src, size_t bytes, cudaStream_t s);
+
 int pyramid_tail(const uint8_t* pk, const Lin& conv3, const __nv_bfloat16* ys, int T, int t0, int tc, int H4, int W4,
-                 float* pyr, cudaStream_t s) {
+                 float* pyr, cudaStream_t s, EncTrace* tr = nullptr) {
   const int64_t Mc = (int64_t)tc * H4 * W4;
   float* f0 = pyr + pyramid_layout(T, H4, W4).off[0] + (int64_t)t0 * H4 * W4 * kD;
   if (int rc = run_gemm(linear_problem(ys, pk + conv3.w, pk + conv3.b, Mc, kD, conv3.Kpad, f0), g_opt_gemm, s,
                         "encoder conv3 gemm"))
     return rc;
+  if (tr)
+    if (int rc = trace_put(tr, f0, (size_t)Mc * kD * 4, s)) return rc;
   CK(launch_l2norm_rows(f0, Mc, f0, s), "l2norm rows");
   if (t0 + tc == T) CK(launch_pyramid_pools(T, H4, W4, pyr, s), "pyramid pools");
   return 0;
@@ -241,6 +247,170 @@ EncFullWs enc_full_carve(void* base, int T, int H, int W) {
   return w;
 }
 
+
+// ct3_encoder / ct3_encoder_workspace_bytes: T >= 1, H, W >= 16 and a 4-level pyramid at H/4 x W/4, which makes the
+// smallest frame 32 x 32 (include/ct3_b200.h)
+int check_encoder_shape(int T, int H, int W) {
+  if (T < 1 || H < 16 || W < 16) return fail(CT3_EINVAL, "encoder: need T >= 1 and H, W >= 16%s");
+  return check_pyramid(T, H / 4, W / 4);
+}
+
+// ---- ct3_encoder_trace: the links of one chunk, each 256-byte aligned in the caller's buffer, in launch order
+struct EncTrace {
+  uint8_t* base = nullptr;
+  size_t off[CT3_ENCODER_TRACE_LINKS] = {}, bytes[CT3_ENCODER_TRACE_LINKS] = {};
+  int n = 0;   // links copied so far
+};
+// fills tr.off / tr.bytes for T (<= 16) frames of H x W; returns the total bytes
+size_t trace_layout(EncTrace& tr, int T, int H, int W) {
+  const EncGeom g = enc_geom(H, W);
+  int n = 0;
+  size_t off = 0;
+  auto link = [&](int64_t rows, int C, int esz) {
+    tr.off[n] = off;
+    tr.bytes[n] = (size_t)rows * C * esz;
+    off = align_up(off + tr.bytes[n]);
+    ++n;
+  };
+  auto unit1 = [&](int64_t rows, int Cp) {   // a stride-1 residual unit
+    link(rows, Cp, 4); link(T, 2 * Cp, 4); link(rows, 2 * Cp, 2);
+    link(rows, Cp, 4); link(T, 2 * Cp, 4); link(rows, Cp, 4); link(rows, 2 * Cp, 2);
+  };
+  int64_t rows = (int64_t)T * g.h[0] * g.w[0];
+  link(rows, 64, 4); link(T, 2 * 64, 4); link(rows, 64, 4); link(rows, 2 * 64, 2);
+  for (int st = 0; st < 4; ++st) {
+    const int Cp = kStageCp[st];
+    rows = (int64_t)T * g.h[st] * g.w[st];
+    if (st > 0) {
+      const int Cin = kStageCp[st - 1];
+      link(rows, 2 * 9 * Cin, 2); link(rows, 2 * Cin, 2);
+      link(rows, Cp, 4); link(T, 2 * Cp, 4); link(rows, 2 * Cp, 2);
+      link(rows, Cp, 4); link(T, 2 * Cp, 4);
+      link(rows, Cp, 4); link(T, 2 * Cp, 4);
+      link(rows, Cp, 4); link(rows, 2 * Cp, 2);
+    }
+    for (int u = (st > 0 ? 1 : 0); u < 2; ++u) unit1(rows, Cp);
+  }
+  const int64_t rows4 = (int64_t)T * g.H4 * g.W4;
+  link(rows4, 2 * kCatCp, 2); link(rows4, kEncMid, 4); link(T, 2 * kEncMid, 4); link(rows4, 2 * kEncMid, 2);
+  link(rows4, kD, 4);
+  return off;
+}
+
+// the next link of the trace: its size must be the layout's
+int trace_put(EncTrace* tr, const void* src, size_t bytes, cudaStream_t s) {
+  if (tr->n >= CT3_ENCODER_TRACE_LINKS || bytes != tr->bytes[tr->n])
+    return fail(CT3_EINVAL, "encoder trace: links out of step with the layout%s");
+  CK(cudaMemcpyAsync(tr->base + tr->off[tr->n], src, bytes, cudaMemcpyDeviceToDevice, s), "encoder trace copy");
+  ++tr->n;
+  return 0;
+}
+
+// ct3_encoder with an optional trace sink: tr == nullptr launches exactly what ct3_encoder launches; otherwise each
+// link's output is also copied into the trace buffer (trace_layout's order) right after the launch that writes it.
+int encoder_run(const void* packed, const float* frames, int T, int H, int W, float* pyr, void* workspace,
+                size_t workspace_bytes, cudaStream_t s, EncTrace* tr) {
+  if (!packed || !frames || !pyr || !workspace) return fail(CT3_EINVAL, "null argument%s");
+  if (int rc = check_encoder_shape(T, H, W)) return rc;
+  const EncGeom g = enc_geom(H, W);
+  if (int rc = check_aligned(workspace, "workspace")) return rc;
+  const EncFullWs Wk = enc_full_carve(workspace, T, H, W);
+  if (int rc = check_space(workspace_bytes, Wk.total, "workspace")) return rc;
+  const EncFull& E = enc_full();
+  const uint8_t* pk = reinterpret_cast<const uint8_t*>(packed);
+  const int nsm = num_sms();
+  auto W16 = [&](const ConvW& c) { return reinterpret_cast<const __nv_bfloat16*>(pk + c.w); };
+  auto B32 = [&](const ConvW& c) { return reinterpret_cast<const float*>(pk + c.b); };
+  // y = GEMM(gathered rows, conv weights): the stride-2 convolutions
+  auto gemm_rows = [&](const __nv_bfloat16* rows, const ConvW& c, int64_t M, float* y) {
+    return run_gemm(linear_problem(rows, W16(c), B32(c), M, c.cout_pad, c.taps * c.cp, y), g_opt_gemm, s,
+                    "encoder gemm");
+  };
+  // TAP(p, rows, C, element bytes): the trace copy of the [rows, C] output p of the launch just made
+#define TAP(p, rows, C, esz) \
+  if (tr)                    \
+    if (int rc = trace_put(tr, p, (size_t)(rows) * (C) * (esz), s)) return rc
+  const int chunks = (T + Wk.tc - 1) / Wk.tc;
+  ProfScope ps_all(s, CAT_ENC, 0.0, chunks * 90 + 3);   // kernels launched per 16-frame chunk + the 3 pyramid pools
+  for (int t0 = 0; t0 < T; t0 += Wk.tc) {
+    const int tc = (T - t0) < Wk.tc ? (T - t0) : Wk.tc;
+    // ---- stem: conv1 7x7/2 -> IN -> ReLU
+    int h = g.h[0], w = g.w[0], C = 64;
+    int64_t rows = (int64_t)tc * h * w;
+    CK(launch_conv_stem(frames + (int64_t)t0 * 3 * H * W, reinterpret_cast<const float*>(pk + E.stem_w),
+                        reinterpret_cast<const float*>(pk + E.stem_b), tc, H, W, Wk.fy, s), "conv1");
+    TAP(Wk.fy, rows, C, 4);
+    CK(launch_instnorm_stats(Wk.fy, tc, h * w, C, 1e-5f, Wk.stats, Wk.stat_scratch, s), "stem stats");
+    TAP(Wk.stats, tc, 2 * C, 4);
+    CK(launch_norm_act(Wk.fy, Wk.stats, nullptr, nullptr, 0, rows, h * w, C, Wk.fx[0], Wk.sx, s), "stem norm");
+    TAP(Wk.fx[0], rows, C, 4);
+    TAP(Wk.sx, rows, 2 * C, 2);
+    // ---- four stages of two residual units
+    for (int st = 0; st < 4; ++st) {
+      float* X = Wk.fx[st];
+      const int Cp = kStageCp[st];
+      if (st > 0) {
+        // unit 0 of a strided stage: y = conv3x3/2(x); x' = IN(conv1x1/2(x)); out = relu(x' + relu(IN(conv3x3(relu(IN(y))))))
+        const int Cin = kStageCp[st - 1];
+        const int ho = g.h[st], wo = g.w[st];
+        const int64_t orows = (int64_t)tc * ho * wo;
+        CK(launch_gather_s2(Wk.sx, tc, h, w, Cin, 9, Wk.gat, s), "gather 3x3/2");
+        TAP(Wk.gat, orows, 2 * 9 * Cin, 2);
+        CK(launch_gather_s2(Wk.sx, tc, h, w, Cin, 1, Wk.gat_d, s), "gather 1x1/2");
+        TAP(Wk.gat_d, orows, 2 * Cin, 2);
+        if (int rc = gemm_rows(Wk.gat, E.unit[st][0][0], orows, Wk.fy)) return rc;
+        TAP(Wk.fy, orows, Cp, 4);
+        CK(launch_instnorm_stats(Wk.fy, tc, ho * wo, Cp, 1e-5f, Wk.stats, Wk.stat_scratch, s), "stats");
+        TAP(Wk.stats, tc, 2 * Cp, 4);
+        CK(launch_norm_act(Wk.fy, Wk.stats, nullptr, nullptr, 0, orows, ho * wo, Cp, nullptr, Wk.sy, s), "norm");
+        TAP(Wk.sy, orows, 2 * Cp, 2);
+        CK(launch_conv3x3_tc(Wk.sy, W16(E.unit[st][0][1]), B32(E.unit[st][0][1]), tc, ho, wo, Cp, Cp, Wk.fy, nsm, s), "conv");
+        TAP(Wk.fy, orows, Cp, 4);
+        CK(launch_instnorm_stats(Wk.fy, tc, ho * wo, Cp, 1e-5f, Wk.stats, Wk.stat_scratch, s), "stats");
+        TAP(Wk.stats, tc, 2 * Cp, 4);
+        if (int rc = gemm_rows(Wk.gat_d, E.down[st], orows, Wk.fyd)) return rc;
+        TAP(Wk.fyd, orows, Cp, 4);
+        CK(launch_instnorm_stats(Wk.fyd, tc, ho * wo, Cp, 1e-5f, Wk.stats_d, Wk.stat_scratch, s), "stats");
+        TAP(Wk.stats_d, tc, 2 * Cp, 4);
+        CK(launch_norm_act(Wk.fy, Wk.stats, Wk.fyd, Wk.stats_d, 2, orows, ho * wo, Cp, X, Wk.sx, s), "norm");
+        TAP(X, orows, Cp, 4);
+        TAP(Wk.sx, orows, 2 * Cp, 2);
+        h = ho; w = wo; rows = orows;
+      }
+      for (int u = (st > 0 ? 1 : 0); u < 2; ++u) {
+        // stride-1 unit: out = relu(x + relu(IN(conv(relu(IN(conv(x)))))))
+        CK(launch_conv3x3_tc(Wk.sx, W16(E.unit[st][u][0]), B32(E.unit[st][u][0]), tc, h, w, Cp, Cp, Wk.fy, nsm, s), "conv");
+        TAP(Wk.fy, rows, Cp, 4);
+        CK(launch_instnorm_stats(Wk.fy, tc, h * w, Cp, 1e-5f, Wk.stats, Wk.stat_scratch, s), "stats");
+        TAP(Wk.stats, tc, 2 * Cp, 4);
+        CK(launch_norm_act(Wk.fy, Wk.stats, nullptr, nullptr, 0, rows, h * w, Cp, nullptr, Wk.sy, s), "norm");
+        TAP(Wk.sy, rows, 2 * Cp, 2);
+        CK(launch_conv3x3_tc(Wk.sy, W16(E.unit[st][u][1]), B32(E.unit[st][u][1]), tc, h, w, Cp, Cp, Wk.fy, nsm, s), "conv");
+        TAP(Wk.fy, rows, Cp, 4);
+        CK(launch_instnorm_stats(Wk.fy, tc, h * w, Cp, 1e-5f, Wk.stats, Wk.stat_scratch, s), "stats");
+        TAP(Wk.stats, tc, 2 * Cp, 4);
+        CK(launch_norm_act(Wk.fy, Wk.stats, X, nullptr, 1, rows, h * w, Cp, X, Wk.sx, s), "norm");
+        TAP(X, rows, Cp, 4);
+        TAP(Wk.sx, rows, 2 * Cp, 2);
+      }
+    }
+    // ---- resize + concat -> conv2 3x3 -> IN -> ReLU -> conv3 1x1 -> L2-normalise (rows = level-0 texels)
+    const int HW4 = g.H4 * g.W4;
+    const float* srcs[4] = {Wk.fx[0], Wk.fx[1], Wk.fx[2], Wk.fx[3]};
+    const int64_t rows4 = (int64_t)tc * HW4;
+    CK(launch_upsample_concat_split(srcs, kStageC, kStageCp, g.h, g.w, tc, kCatCp, g.H4, g.W4, Wk.cat, s), "upsample concat");
+    TAP(Wk.cat, rows4, 2 * kCatCp, 2);
+    CK(launch_conv3x3_tc(Wk.cat, W16(E.conv2), B32(E.conv2), tc, g.H4, g.W4, kCatCp, kEncMid, Wk.fy, nsm, s), "conv2");
+    TAP(Wk.fy, rows4, kEncMid, 4);
+    CK(launch_instnorm_stats(Wk.fy, tc, HW4, kEncMid, 1e-5f, Wk.stats, Wk.stat_scratch, s), "instnorm stats");
+    TAP(Wk.stats, tc, 2 * kEncMid, 4);
+    CK(launch_instnorm_relu_split(Wk.fy, Wk.stats, rows4, HW4, kEncMid, Wk.sy, s), "instnorm relu split");
+    TAP(Wk.sy, rows4, 2 * kEncMid, 2);
+    if (int rc = pyramid_tail(pk, E.conv3, Wk.sy, T, t0, tc, g.H4, g.W4, pyr, s, tr)) return rc;
+  }
+#undef TAP
+  return 0;
+}
 }  // namespace
 
 extern "C" {
@@ -289,84 +459,41 @@ int ct3_encoder_pack(const float* const* t, int n_tensors, void* packed, size_t 
 
 int ct3_encoder_workspace_bytes(int T, int H, int W, size_t* out_bytes) {
   if (!out_bytes) return fail(CT3_EINVAL, "null out_bytes%s");
-  if (T < 1 || H < 16 || W < 16) return fail(CT3_EINVAL, "encoder: need T >= 1 and H, W >= 16%s");
-  if (int rc = check_pyramid(T, H / 4, W / 4)) return rc;
+  if (int rc = check_encoder_shape(T, H, W)) return rc;
   *out_bytes = enc_full_carve(nullptr, T, H, W).total;
   return 0;
 }
 
 int ct3_encoder(const void* packed, const float* frames, int T, int H, int W, float* pyr, void* workspace,
                 size_t workspace_bytes, ct3_stream_t stream) {
-  if (!packed || !frames || !pyr || !workspace) return fail(CT3_EINVAL, "null argument%s");
-  if (T < 1 || H < 16 || W < 16) return fail(CT3_EINVAL, "encoder: need T >= 1 and H, W >= 16%s");
-  const EncGeom g = enc_geom(H, W);
-  if (int rc = check_pyramid(T, g.H4, g.W4)) return rc;
-  if (int rc = check_aligned(workspace, "workspace")) return rc;
-  const EncFullWs Wk = enc_full_carve(workspace, T, H, W);
-  if (int rc = check_space(workspace_bytes, Wk.total, "workspace")) return rc;
-  const EncFull& E = enc_full();
-  const uint8_t* pk = reinterpret_cast<const uint8_t*>(packed);
-  cudaStream_t s = (cudaStream_t)stream;
-  const int nsm = num_sms();
-  auto W16 = [&](const ConvW& c) { return reinterpret_cast<const __nv_bfloat16*>(pk + c.w); };
-  auto B32 = [&](const ConvW& c) { return reinterpret_cast<const float*>(pk + c.b); };
-  // y = GEMM(gathered rows, conv weights): the stride-2 convolutions
-  auto gemm_rows = [&](const __nv_bfloat16* rows, const ConvW& c, int64_t M, float* y) {
-    return run_gemm(linear_problem(rows, W16(c), B32(c), M, c.cout_pad, c.taps * c.cp, y), g_opt_gemm, s,
-                    "encoder gemm");
-  };
-  const int chunks = (T + Wk.tc - 1) / Wk.tc;
-  ProfScope ps_all(s, CAT_ENC, 0.0, chunks * 90 + 3);   // kernels launched per 16-frame chunk + the 3 pyramid pools
-  for (int t0 = 0; t0 < T; t0 += Wk.tc) {
-    const int tc = (T - t0) < Wk.tc ? (T - t0) : Wk.tc;
-    // ---- stem: conv1 7x7/2 -> IN -> ReLU
-    int h = g.h[0], w = g.w[0], C = 64;
-    int64_t rows = (int64_t)tc * h * w;
-    CK(launch_conv_stem(frames + (int64_t)t0 * 3 * H * W, reinterpret_cast<const float*>(pk + E.stem_w),
-                        reinterpret_cast<const float*>(pk + E.stem_b), tc, H, W, Wk.fy, s), "conv1");
-    CK(launch_instnorm_stats(Wk.fy, tc, h * w, C, 1e-5f, Wk.stats, Wk.stat_scratch, s), "stem stats");
-    CK(launch_norm_act(Wk.fy, Wk.stats, nullptr, nullptr, 0, rows, h * w, C, Wk.fx[0], Wk.sx, s), "stem norm");
-    // ---- four stages of two residual units
-    for (int st = 0; st < 4; ++st) {
-      float* X = Wk.fx[st];
-      const int Cp = kStageCp[st];
-      if (st > 0) {
-        // unit 0 of a strided stage: y = conv3x3/2(x); x' = IN(conv1x1/2(x)); out = relu(x' + relu(IN(conv3x3(relu(IN(y))))))
-        const int Cin = kStageCp[st - 1];
-        const int ho = g.h[st], wo = g.w[st];
-        const int64_t orows = (int64_t)tc * ho * wo;
-        CK(launch_gather_s2(Wk.sx, tc, h, w, Cin, 9, Wk.gat, s), "gather 3x3/2");
-        CK(launch_gather_s2(Wk.sx, tc, h, w, Cin, 1, Wk.gat_d, s), "gather 1x1/2");
-        if (int rc = gemm_rows(Wk.gat, E.unit[st][0][0], orows, Wk.fy)) return rc;
-        CK(launch_instnorm_stats(Wk.fy, tc, ho * wo, Cp, 1e-5f, Wk.stats, Wk.stat_scratch, s), "stats");
-        CK(launch_norm_act(Wk.fy, Wk.stats, nullptr, nullptr, 0, orows, ho * wo, Cp, nullptr, Wk.sy, s), "norm");
-        CK(launch_conv3x3_tc(Wk.sy, W16(E.unit[st][0][1]), B32(E.unit[st][0][1]), tc, ho, wo, Cp, Cp, Wk.fy, nsm, s), "conv");
-        CK(launch_instnorm_stats(Wk.fy, tc, ho * wo, Cp, 1e-5f, Wk.stats, Wk.stat_scratch, s), "stats");
-        if (int rc = gemm_rows(Wk.gat_d, E.down[st], orows, Wk.fyd)) return rc;
-        CK(launch_instnorm_stats(Wk.fyd, tc, ho * wo, Cp, 1e-5f, Wk.stats_d, Wk.stat_scratch, s), "stats");
-        CK(launch_norm_act(Wk.fy, Wk.stats, Wk.fyd, Wk.stats_d, 2, orows, ho * wo, Cp, X, Wk.sx, s), "norm");
-        h = ho; w = wo; rows = orows;
-      }
-      for (int u = (st > 0 ? 1 : 0); u < 2; ++u) {
-        // stride-1 unit: out = relu(x + relu(IN(conv(relu(IN(conv(x)))))))
-        CK(launch_conv3x3_tc(Wk.sx, W16(E.unit[st][u][0]), B32(E.unit[st][u][0]), tc, h, w, Cp, Cp, Wk.fy, nsm, s), "conv");
-        CK(launch_instnorm_stats(Wk.fy, tc, h * w, Cp, 1e-5f, Wk.stats, Wk.stat_scratch, s), "stats");
-        CK(launch_norm_act(Wk.fy, Wk.stats, nullptr, nullptr, 0, rows, h * w, Cp, nullptr, Wk.sy, s), "norm");
-        CK(launch_conv3x3_tc(Wk.sy, W16(E.unit[st][u][1]), B32(E.unit[st][u][1]), tc, h, w, Cp, Cp, Wk.fy, nsm, s), "conv");
-        CK(launch_instnorm_stats(Wk.fy, tc, h * w, Cp, 1e-5f, Wk.stats, Wk.stat_scratch, s), "stats");
-        CK(launch_norm_act(Wk.fy, Wk.stats, X, nullptr, 1, rows, h * w, Cp, X, Wk.sx, s), "norm");
-      }
-    }
-    // ---- resize + concat -> conv2 3x3 -> IN -> ReLU -> conv3 1x1 -> L2-normalise (rows = level-0 texels)
-    const int HW4 = g.H4 * g.W4;
-    const float* srcs[4] = {Wk.fx[0], Wk.fx[1], Wk.fx[2], Wk.fx[3]};
-    CK(launch_upsample_concat_split(srcs, kStageC, kStageCp, g.h, g.w, tc, kCatCp, g.H4, g.W4, Wk.cat, s), "upsample concat");
-    CK(launch_conv3x3_tc(Wk.cat, W16(E.conv2), B32(E.conv2), tc, g.H4, g.W4, kCatCp, kEncMid, Wk.fy, nsm, s), "conv2");
-    CK(launch_instnorm_stats(Wk.fy, tc, HW4, kEncMid, 1e-5f, Wk.stats, Wk.stat_scratch, s), "instnorm stats");
-    CK(launch_instnorm_relu_split(Wk.fy, Wk.stats, (int64_t)tc * HW4, HW4, kEncMid, Wk.sy, s), "instnorm relu split");
-    if (int rc = pyramid_tail(pk, E.conv3, Wk.sy, T, t0, tc, g.H4, g.W4, pyr, s)) return rc;
+  return encoder_run(packed, frames, T, H, W, pyr, workspace, workspace_bytes, (cudaStream_t)stream, nullptr);
+}
+
+int ct3_encoder_trace_layout(int T, int H, int W, int64_t* offsets, int64_t* bytes, size_t* total_bytes) {
+  if (!total_bytes) return fail(CT3_EINVAL, "null total_bytes%s");
+  if (int rc = check_encoder_shape(T, H, W)) return rc;
+  if (T > 16) return fail(CT3_EINVAL, "encoder trace: one chunk, T <= 16%s");
+  EncTrace tr;
+  *total_bytes = trace_layout(tr, T, H, W);
+  for (int i = 0; i < CT3_ENCODER_TRACE_LINKS; ++i) {
+    if (offsets) offsets[i] = (int64_t)tr.off[i];
+    if (bytes) bytes[i] = (int64_t)tr.bytes[i];
   }
   return 0;
+}
+
+int ct3_encoder_trace(const void* packed, const float* frames, int T, int H, int W, float* pyr, void* trace,
+                      size_t trace_bytes, void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+  if (!trace) return fail(CT3_EINVAL, "null argument%s");
+  if (int rc = check_encoder_shape(T, H, W)) return rc;
+  if (T > 16) return fail(CT3_EINVAL, "encoder trace: one chunk, T <= 16%s");
+  if (int rc = check_aligned(trace, "trace")) return rc;
+  EncTrace tr;
+  tr.base = reinterpret_cast<uint8_t*>(trace);
+  if (int rc = check_space(trace_bytes, trace_layout(tr, T, H, W), "trace buffer")) return rc;
+  if (int rc = encoder_run(packed, frames, T, H, W, pyr, workspace, workspace_bytes, (cudaStream_t)stream, &tr))
+    return rc;
+  return tr.n == CT3_ENCODER_TRACE_LINKS ? 0 : fail(CT3_EINVAL, "encoder trace: links out of step with the layout%s");
 }
 
 }  // extern "C"

@@ -7,6 +7,7 @@ fails, a RuntimeError is raised (the product path never routes through the oracl
 from __future__ import annotations
 
 import ctypes
+import math
 import os
 from typing import List, Optional, Sequence
 
@@ -140,6 +141,9 @@ def _signatures():
         "ct3_encoder_pack": (c_int, [ctypes.POINTER(c_void_p), c_int, c_void_p, c_size_t, c_void_p]),
         "ct3_encoder_workspace_bytes": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
         "ct3_encoder": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+        "ct3_encoder_trace_layout": (c_int, [c_int, c_int, c_int, i64p, i64p, ctypes.POINTER(c_size_t)]),
+        "ct3_encoder_trace": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p,
+                                      c_size_t, c_void_p]),
         "ct3_corners_workspace_bytes": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
         "ct3_detect_corners": (c_int, [c_void_p, i64, c_int, c_int, c_int, ctypes.POINTER(CornerParams), c_void_p,
                                        ctypes.POINTER(ctypes.c_int32), c_int, c_void_p, c_void_p, c_void_p, c_size_t,
@@ -1084,6 +1088,93 @@ def encoder(packed: torch.Tensor, frames: torch.Tensor, workspace: torch.Tensor)
     _call("ct3_encoder", frames.device, _ptr(packed), _ptr(frames), T, H, W, _ptr(pyr), _ptr(workspace), workspace.numel(),
           _stream(frames.device))
     return pyr
+
+
+ENCODER_TRACE_LINKS = 77
+ENCODER_STAGE_C = (64, 128, 128, 128)     # channels each stage carries (stage 1: 96 real + 32 zero)
+
+
+def encoder_stage_hw(H: int, W: int) -> List[tuple]:
+    """(h, w) of the four stage maps of an H x W frame: the 7x7/2 stem, then three stride-2 stages"""
+    hw = [((H - 1) // 2 + 1, (W - 1) // 2 + 1)]
+    for _ in range(3):
+        hw.append(((hw[-1][0] - 1) // 2 + 1, (hw[-1][1] - 1) // 2 + 1))
+    return hw
+
+
+def encoder_trace_links(T: int, H: int, W: int) -> List[tuple]:
+    """The links of ct3_encoder_trace in buffer order (include/ct3_b200.h) -> [(name, dtype, shape)]: "f32" links
+    are [T, h, w, C] channels-last, "split" links [T*h*w, 2*C] bf16 (hi | lo), "stats" links [T, C, 2] (mean, rstd)."""
+    links = []
+    hw = encoder_stage_hw(H, W)
+
+    def f32(name, s, C):
+        links.append((name, torch.float32, (T, hw[s][0], hw[s][1], C)))
+
+    def split(name, s, C):
+        links.append((name, torch.bfloat16, (T * hw[s][0] * hw[s][1], 2 * C)))
+
+    def stats(name, C):
+        links.append((name, torch.float32, (T, C, 2)))
+
+    f32("stem.conv", 0, 64), stats("stem.stats", 64), f32("stem.out", 0, 64), split("stem.out_split", 0, 64)
+    for s in range(4):
+        C, p = ENCODER_STAGE_C[s], f"layer{s + 1}"
+        if s > 0:
+            split(f"{p}.0.gather", s, 9 * ENCODER_STAGE_C[s - 1])
+            split(f"{p}.0.gather_d", s, ENCODER_STAGE_C[s - 1])
+            f32(f"{p}.0.conv1", s, C), stats(f"{p}.0.conv1.stats", C), split(f"{p}.0.norm1_split", s, C)
+            f32(f"{p}.0.conv2", s, C), stats(f"{p}.0.conv2.stats", C)
+            f32(f"{p}.0.downsample", s, C), stats(f"{p}.0.downsample.stats", C)
+            f32(f"{p}.0.out", s, C), split(f"{p}.0.out_split", s, C)
+        for u in range(1 if s > 0 else 0, 2):
+            q = f"{p}.{u}"
+            f32(f"{q}.conv1", s, C), stats(f"{q}.conv1.stats", C), split(f"{q}.norm1_split", s, C)
+            f32(f"{q}.conv2", s, C), stats(f"{q}.conv2.stats", C), f32(f"{q}.out", s, C), split(f"{q}.out_split", s, C)
+    H4, W4 = H // 4, W // 4
+    links.append(("cat_split", torch.bfloat16, (T * H4 * W4, 2 * 448)))
+    links.append(("conv2", torch.float32, (T, H4, W4, 256)))
+    links.append(("conv2.stats", torch.float32, (T, 256, 2)))
+    links.append(("conv2.out_split", torch.bfloat16, (T * H4 * W4, 512)))
+    links.append(("conv3", torch.float32, (T, H4, W4, LATENT)))
+    assert len(links) == ENCODER_TRACE_LINKS
+    return links
+
+
+def encoder_trace_layout(T: int, H: int, W: int):
+    """ct3_encoder_trace_layout -> (offsets [77], bytes [77], total bytes)"""
+    off = (ctypes.c_int64 * ENCODER_TRACE_LINKS)()
+    nb = (ctypes.c_int64 * ENCODER_TRACE_LINKS)()
+    tot = ctypes.c_size_t(0)
+    _check(lib().ct3_encoder_trace_layout(T, H, W, off, nb, ctypes.byref(tot)), "ct3_encoder_trace_layout")
+    return list(off), list(nb), tot.value
+
+
+def encoder_trace(packed: torch.Tensor, frames: torch.Tensor, workspace: Optional[torch.Tensor] = None) -> dict:
+    """ct3_encoder_trace: frames [T,3,H,W] fp32 (T <= 16) through ct3_encoder's own code -> {link name: tensor} with
+    the links of encoder_trace_links plus "pyramid", the flat pyramid ct3_encoder writes."""
+    _req(frames, torch.float32, "frames")
+    T, C, H, W = frames.shape
+    if C != 3:
+        raise EngineError("frames must be [T,3,H,W]")
+    dev = frames.device
+    offs, nbytes, total = encoder_trace_layout(T, H, W)
+    links = encoder_trace_links(T, H, W)
+    if workspace is None:
+        workspace = torch.empty(encoder_workspace_bytes(T, H, W), dtype=torch.uint8, device=dev)
+    *_, ptotal = pyramid_layout(T, H // 4, W // 4)
+    pyr = torch.empty(ptotal, dtype=torch.float32, device=dev)
+    buf = torch.empty(total, dtype=torch.uint8, device=dev)
+    _call("ct3_encoder_trace", dev, _ptr(packed), _ptr(frames), T, H, W, _ptr(pyr), _ptr(buf), total, _ptr(workspace),
+          workspace.numel(), _stream(dev))
+    out = {}
+    for (name, dtype, shape), o, n in zip(links, offs, nbytes):
+        numel = math.prod(shape)
+        if numel * dtype.itemsize != n:
+            raise EngineError(f"encoder trace link {name}: {n} bytes, expected {shape} {dtype}")
+        out[name] = buf[o:o + n].view(dtype).reshape(shape)
+    out["pyramid"] = pyr
+    return out
 
 
 def slice_pyramid(pyr: torch.Tensor, T: int, H4: int, W4: int, t0: int, S: int) -> torch.Tensor:

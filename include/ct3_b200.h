@@ -585,7 +585,9 @@ int ct3_attention(int kind, const float* q, const float* kv, int T, int N, const
  * frames [T,3,H,W] fp32 already scaled to [-1,1] (cotracker3_offline.py:63) -> pyr (ct3_pyramid_layout(T, H/4, W/4)).
  * conv1 7x7/2 runs as fp32 SIMT, every other convolution as split-bf16x3 wgmma GEMMs (3x3 stride-1: implicit GEMM
  * over TMA-shifted NHWC boxes; strided ones: gather + GEMM); InstanceNorm statistics in fp64.
- * Weight tensors in the order of ct3_encoder_weight_name() (state-dict keys below `fnet.`). */
+ * Weight tensors in the order of ct3_encoder_weight_name() (state-dict keys below `fnet.`).
+ * Frames are at least 32 x 32: H, W >= 16 and a 4-level pyramid at H/4 x W/4 (ct3_pyramid_layout); anything smaller,
+ * or T < 1, returns CT3_EINVAL from ct3_encoder and ct3_encoder_workspace_bytes before any launch. */
 int ct3_encoder_num_weight_tensors(void);
 const char* ct3_encoder_weight_name(int index);
 int ct3_encoder_packed_bytes(size_t* out_bytes);
@@ -594,6 +596,29 @@ int ct3_encoder_pack(const float* const* tensors_host_array_of_device_ptrs, int 
 int ct3_encoder_workspace_bytes(int T, int H, int W, size_t* out_bytes);
 int ct3_encoder(const void* packed, const float* frames, int T, int H, int W, float* pyr, void* workspace,
                 size_t workspace_bytes, ct3_stream_t stream);
+
+/* ct3_encoder run by its own code on one chunk (1 <= T <= 16), with a copy of every link's output taken right after
+ * the launch that writes it, for testing each link on its own input.  Arguments, checks and pyr as ct3_encoder;
+ * workspace: ct3_encoder_workspace_bytes(T, H, W).  trace: a 256-byte aligned device buffer of at least the
+ * total_bytes of ct3_encoder_trace_layout(T, H, W), which also gives each link's byte offset and size
+ * (CT3_ENCODER_TRACE_LINKS of each; offsets and bytes may be NULL).  Null pointers, T > 16 or a bad shape return
+ * CT3_EINVAL and a too small trace or workspace CT3_ENOSPC, before any launch.
+ * Shapes: h_s x w_s the stage maps (h_0 = (H-1)/2 + 1, h_s = (h_{s-1}-1)/2 + 1), H4 = H/4, C_s = 64, 128, 128, 128
+ * the carried channels (stage 1 holds 96 real ones and 32 zero ones), rows = T*h*w of the map named, "split" a
+ * bf16 [rows, 2*C] operand (hi C | lo C), "f32" fp32 [rows, C] channels-last, "stats" fp32 [T, C, 2] (mean, rstd).
+ *   stem           : conv1 f32 (C 64) | stats | relu(IN) f32 | split
+ *   stride-1 unit  : conv1 f32 | stats | relu(IN) split | conv2 f32 | stats | relu(x + relu(IN)) f32 | split
+ *                    (stage 0: units 0 and 1; stages 1..3: unit 1)
+ *   stride-2 unit  : 3x3/2 gather split [rows, 2*9*C_{s-1}] | 1x1/2 gather split [rows, 2*C_{s-1}] | conv1 f32 |
+ *   (stages 1..3,     stats | relu(IN) split | conv2 f32 | stats | downsample f32 | stats |
+ *    unit 0)          relu(IN_d(downsample) + relu(IN(conv2))) f32 | split
+ *   tail           : resize + concat split [T*H4*W4, 2*448] (416 real channels) | conv2 f32 (C 256) | stats |
+ *                    relu(IN) split | conv3 f32 (C 128) before the L2 norm
+ * in the order stem, stage 0 .. 3 (unit 0 then unit 1), tail: 77 links. */
+#define CT3_ENCODER_TRACE_LINKS 77
+int ct3_encoder_trace_layout(int T, int H, int W, int64_t* offsets, int64_t* bytes, size_t* total_bytes);
+int ct3_encoder_trace(const void* packed, const float* frames, int T, int H, int W, float* pyr, void* trace,
+                      size_t trace_bytes, void* workspace, size_t workspace_bytes, ct3_stream_t stream);
 
 #ifdef __cplusplus
 }
