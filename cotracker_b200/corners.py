@@ -51,7 +51,7 @@ def params(max_corners, quality_level=0.01, min_distance=10, block_size=3, exclu
 def clip_frame(video, t: int):
     """Frame t of every clip of `video` ([B,T,3,H,W] or a YUVClip), as a one-frame clip of the same kind."""
     if isinstance(video, ingest.YUVClip):
-        return ingest.YUVClip(video.data[:, t:t + 1], video.layout)
+        return video.with_data(video.data[:, t:t + 1])
     return video[:, t:t + 1]
 
 

@@ -207,22 +207,39 @@ int ct3_prepare_frames_yuv(const uint8_t* src, int layout, int T, int H, int W, 
   if (!src || !out) return fail(CT3_EINVAL, "null argument%s");
   if (layout != CT3_YUV_NV12 && layout != CT3_YUV_I420 && layout != CT3_YUV_YUYV)
     return fail(CT3_EINVAL, "unknown YUV layout%s");
+  return ct3_prepare_frames_yuv_fmt(src, layout, CT3_MATRIX_BT601, 0, T, H, W, stride_t, stride_row, out_h, out_w, out,
+                                    stream);
+}
+
+int ct3_prepare_frames_yuv_fmt(const void* src, int layout, int matrix, int full_range, int T, int H, int W,
+                               int64_t stride_t, int64_t stride_row, int out_h, int out_w, float* out,
+                               ct3_stream_t stream) {
+  if (!src || !out) return fail(CT3_EINVAL, "null argument%s");
+  const YuvFormat* f = yuv_format(layout);
+  if (!f) return fail(CT3_EINVAL, "unknown YUV layout%s");
+  if (matrix != CT3_MATRIX_BT601 && matrix != CT3_MATRIX_BT709 && matrix != CT3_MATRIX_BT2020)
+    return fail(CT3_EINVAL, "unknown colour matrix%s");
+  if (full_range != 0 && full_range != 1) return fail(CT3_EINVAL, "full_range must be 0 or 1%s");
   if (T < 1 || H < 1 || W < 1 || out_h < 1 || out_w < 1) return fail(CT3_EINVAL, "T, H, W, out_h and out_w must be >= 1%s");
-  if ((W & 1) || (layout != CT3_YUV_YUYV && (H & 1)))
-    return fail(CT3_EINVAL, "%s frames must have an even width and height (YUYV: an even width)",
-                layout == CT3_YUV_YUYV ? "YUYV" : layout == CT3_YUV_NV12 ? "NV12" : "I420");
-  const int64_t row_bytes = layout == CT3_YUV_YUYV ? 2 * (int64_t)W : W;
+  if ((f->ys && (H & 1)) || (f->xs && (W & 1)))
+    return fail(CT3_EINVAL, f->ys ? "%s frames must have an even width and height" : "%s frames must have an even width",
+                f->name);
+  if (f->bytes == 2 && ((stride_t | stride_row) & 1))
+    return fail(CT3_EINVAL, "%s strides must be even (16-bit samples)", f->name);
+  const int64_t row_bytes = (int64_t)W * f->bytes * (f->family == YuvFormat::kPacked ? 2 : 1);
   if (stride_row < row_bytes) return fail(CT3_EINVAL, "the row stride is below the bytes of a row%s");
-  if (layout == CT3_YUV_I420 && stride_row != W) return fail(CT3_EINVAL, "I420 rows must be dense (stride_row == W)%s");
+  if (f->family == YuvFormat::kPlanar && stride_row != row_bytes)
+    return fail(CT3_EINVAL, "%s rows must be dense (stride_row == W * sample bytes)", f->name);
   // the last byte of the last frame: |stride_t| * (T - 1) + stride_row * (rows - 1) + row_bytes - 1 fits int64
-  const int64_t rows = layout == CT3_YUV_YUYV ? H : (int64_t)H / 2 * 3;
+  const int64_t rows = yuv_rows(*f, H);
   if (stride_t == INT64_MIN || stride_row > (INT64_MAX - row_bytes) / rows)
     return fail(CT3_EINVAL, "stride extent overflows int64%s");
   const int64_t frame = stride_row * (rows - 1) + row_bytes, at = stride_t < 0 ? -stride_t : stride_t;
   if (T > 1 && at > (INT64_MAX - frame) / (T - 1)) return fail(CT3_EINVAL, "stride extent overflows int64%s");
   if ((int64_t)out_h * out_w > INT32_MAX) return fail(CT3_EINVAL, "output plane too large%s");
   if ((int64_t)out_h * out_w > INT64_MAX / 12 / T) return fail(CT3_EINVAL, "output too large%s");
-  CK(launch_prepare_frames_yuv(src, layout, T, H, W, stride_t, stride_row, out_h, out_w, out, (cudaStream_t)stream),
+  CK(launch_prepare_frames_yuv(src, layout, matrix, full_range, T, H, W, stride_t, stride_row, out_h, out_w, out,
+                               (cudaStream_t)stream),
      "prepare_frames_yuv");
   return 0;
 }

@@ -15,9 +15,10 @@
 //     reciprocal), then * 2 (exact) and - 1.
 //
 // The kernel is templated on how it reads one source pixel's three channels (a "fetch"): the strided RGB read, or a
-// YUV read (NV12, I420, YUYV) that loads the pixel's Y and its shared chroma and applies cv2's integer BT.601
-// conversion (ct3_prepare_frames_yuv).  The resize, copy and normalisation are this one piece of code for both, so a
-// YUV clip gives exactly the floats its uint8 RGB conversion would.
+// YUV read that loads the pixel's Y and its shared chroma (semi-planar, planar or packed, 8- or 16-bit samples) and
+// applies the integer conversion of ct3_prepare_frames_yuv_fmt (cv2's BT.601 constants by default).  The resize, copy
+// and normalisation are this one piece of code for all of them, so a YUV clip gives exactly the floats its uint8 RGB
+// conversion would.
 #include "../../include/ct3_b200.h"
 #include "kernels.cuh"
 
@@ -56,43 +57,97 @@ struct RgbFetch {
   }
 };
 
-// YuvFetch<L>: uint8 YUV frames of layout L (CT3_YUV_*) at byte strides st (frame) and sr (row), converted to RGB as
-// cv2.cvtColor(COLOR_YUV2RGB_*) does (BT.601 limited range, Q20 integers; the formula is in include/ct3_b200.h).
-// uv: the byte offset of the chroma in a frame (NV12: H rows; I420: the U plane at H*W, V a quarter plane further).
-template <int L>
-struct YuvFetch {
-  using Src = uint8_t;
-  int64_t sr, uv, quarter;
+// A YUV fetch is a read family (how a pixel's Y and its shared U, V are found in a frame) and a colour (how they
+// become RGB).  Strides and offsets are in samples of the family's type S (uint8_t or uint16_t).
+//
+// SemiPlanarRead: NV12, P010, P016: H luma rows, then H/2 rows of interleaved U,V, at row stride sr; uv = H * sr.
+template <typename S>
+struct SemiPlanarRead {
+  using Src = S;
+  int64_t sr, uv;
+  __device__ __forceinline__ void load(const S* f, int y, int x, int& Y, int& U, int& V) const {
+    Y = __ldg(f + y * sr + x);
+    const S* c = f + uv + (y >> 1) * sr + (x & ~1);
+    U = __ldg(c);
+    V = __ldg(c + 1);
+  }
+};
 
-  __device__ __forceinline__ void pixel(const uint8_t* f, int y, int x, float (&v)[3]) const {
-    int Y, U, V;
-    if (L == CT3_YUV_NV12) {
-      Y = __ldg(f + y * sr + x);
-      const uint8_t* c = f + uv + (y >> 1) * sr + (x & ~1);
-      U = __ldg(c);
-      V = __ldg(c + 1);
-    } else if (L == CT3_YUV_I420) {   // rows are dense: sr == W
-      Y = __ldg(f + y * sr + x);
-      const int64_t c = uv + (y >> 1) * (sr >> 1) + (x >> 1);
-      U = __ldg(f + c);
-      V = __ldg(f + c + quarter);
-    } else {   // YUYV: Y0 U Y1 V per pixel pair
-      const uint8_t* p = f + y * sr + 2 * (x & ~1);
-      Y = __ldg(p + 2 * (x & 1));
-      U = __ldg(p + 1);
-      V = __ldg(p + 3);
-    }
+// PlanarRead<S, XS, YS>: I420 (1, 1), YUV422P (1, 0), YUV444P (0, 0) and their 10-bit forms: the Y plane (rows dense,
+// sr == W), then the U plane at uv = H * W and the V plane cplane further, chroma rows of W >> XS samples; a chroma
+// sample covers 2^XS x 2^YS pixels.  The shifts are compile-time, so I420 makes the loads and index arithmetic of the
+// I420 read this replaced.
+template <typename S, int XS, int YS>
+struct PlanarRead {
+  using Src = S;
+  int64_t sr, uv, cplane;
+  __device__ __forceinline__ void load(const S* f, int y, int x, int& Y, int& U, int& V) const {
+    Y = __ldg(f + y * sr + x);
+    const int64_t c = uv + (y >> YS) * (sr >> XS) + (x >> XS);
+    U = __ldg(f + c);
+    V = __ldg(f + c + cplane);
+  }
+};
+
+// PackedRead: YUYV, H rows of W/2 pixel pairs Y0 U Y1 V at row stride sr.
+template <typename S>
+struct PackedRead {
+  using Src = S;
+  int64_t sr;
+  __device__ __forceinline__ void load(const S* f, int y, int x, int& Y, int& U, int& V) const {
+    const S* p = f + y * sr + 2 * (x & ~1);
+    Y = __ldg(p + 2 * (x & 1));
+    U = __ldg(p + 1);
+    V = __ldg(p + 3);
+  }
+};
+
+__device__ __forceinline__ float clamp255(long long x) { return (float)(int)min(max(x, 0ll), 255ll); }
+
+// Cv2Bt601: cv2's BT.601 limited-range conversion of 8-bit samples, the default colour, with its Q20 constants
+// compiled in (every term fits int32).
+struct Cv2Bt601 {
+  __device__ __forceinline__ void rgb(int Y, int U, int V, float (&v)[3]) const {
     const int yy = max(Y - 16, 0) * 1220542, u = U - 128, w = V - 128;
     v[0] = (float)min(max((yy + 1673527 * w + (1 << 19)) >> 20, 0), 255);
     v[1] = (float)min(max((yy - 852492 * w - 409993 * u + (1 << 19)) >> 20, 0), 255);
     v[2] = (float)min(max((yy + 2116026 * u + (1 << 19)) >> 20, 0), 255);
+  }
+};
+
+// YuvCoeffs: any layout and colour, the formula of ct3_prepare_frames_yuv_fmt in int64 (yuv_coeffs() below).  A
+// container value c holds the sample (c >> rshift) & mask.
+struct YuvCoeffs {
+  int rshift, mask, yoff, ylo, coff, shift;
+  long long cy, crv, cgv, cgu, cbu;
+  __device__ __forceinline__ void rgb(int Y, int U, int V, float (&v)[3]) const {
+    Y = (Y >> rshift) & mask;
+    U = (U >> rshift) & mask;
+    V = (V >> rshift) & mask;
+    const long long yy = max(Y - yoff, ylo) * cy, u = U - coff, w = V - coff, h = 1ll << (shift - 1);
+    v[0] = clamp255((yy + crv * w + h) >> shift);
+    v[1] = clamp255((yy - cgv * w - cgu * u + h) >> shift);
+    v[2] = clamp255((yy + cbu * u + h) >> shift);
+  }
+};
+
+template <class Read, class Color>
+struct YuvFetch {
+  using Src = typename Read::Src;
+  Read read;
+  Color color;
+
+  __device__ __forceinline__ void pixel(const Src* f, int y, int x, float (&v)[3]) const {
+    int Y, U, V;
+    read.load(f, y, x, Y, U, V);
+    color.rgb(Y, U, V, v);
   }
   // the 2x2 neighbourhood, converted up front: a pixel's three channels come from the same loads
   struct Quad {
     float p[4][3];
     __device__ __forceinline__ float at(int c, int k) const { return p[k][c]; }
   };
-  __device__ __forceinline__ Quad quad(const uint8_t* f, int y, int x, int dy, int dx) const {
+  __device__ __forceinline__ Quad quad(const Src* f, int y, int x, int dy, int dx) const {
     Quad q;
     pixel(f, y, x, q.p[0]);
     pixel(f, y, x + dx, q.p[1]);
@@ -168,15 +223,84 @@ cudaError_t launch_prepare_frames(const void* src, int dtype, int T, int H, int 
   return launch_fetch(static_cast<const float*>(src), st, RgbFetch<float>{sc, sh, sw}, T, H, W, oh, ow, out, s);
 }
 
-cudaError_t launch_prepare_frames_yuv(const uint8_t* src, int layout, int T, int H, int W, int64_t st, int64_t sr,
-                                      int oh, int ow, float* out, cudaStream_t s) {
-  if (layout == CT3_YUV_NV12)
-    return launch_fetch(src, st, YuvFetch<CT3_YUV_NV12>{sr, (int64_t)H * sr, 0}, T, H, W, oh, ow, out, s);
-  if (layout == CT3_YUV_I420) {
-    const int64_t quarter = (int64_t)(H / 2) * (W / 2);
-    return launch_fetch(src, st, YuvFetch<CT3_YUV_I420>{sr, (int64_t)H * W, quarter}, T, H, W, oh, ow, out, s);
+namespace {
+
+// The coefficients of ct3_prepare_frames_yuv_fmt (include/ct3_b200.h) for one layout and colour: cv2's constants for
+// BT.601 limited range, otherwise each derived exactly from Kr, Kb (in 1e-4) and rounded half up at Q = 48.
+YuvCoeffs yuv_coeffs(const YuvFormat& f, int matrix, int full_range) {
+  constexpr int kQ = 48;
+  const int n = f.bits, s = 1 << (n - 8);
+  YuvCoeffs k;
+  k.rshift = f.msb ? 16 - n : 0;
+  k.mask = (1 << n) - 1;
+  if (matrix == CT3_MATRIX_BT601 && !full_range) {
+    k.yoff = 16 * s, k.ylo = 0, k.coff = 128 * s, k.shift = 20 + n - 8;
+    k.cy = 1220542, k.crv = 1673527, k.cgv = 852492, k.cgu = 409993, k.cbu = 2116026;
+    return k;
   }
-  return launch_fetch(src, st, YuvFetch<CT3_YUV_YUYV>{sr, 0, 0}, T, H, W, oh, ow, out, s);
+  static const long long kKrKb[3][2] = {{2990, 1140}, {2126, 722}, {2627, 593}};
+  const long long kr = kKrKb[matrix][0], kb = kKrKb[matrix][1], kg = 10000 - kr - kb;
+  long long dy, dc;
+  if (full_range) {
+    k.yoff = 0, k.coff = 1 << (n - 1), dy = dc = (1ll << n) - 1;
+  } else {
+    k.yoff = 16 * s, k.coff = 128 * s, dy = 219ll * s, dc = 224ll * s;
+  }
+  k.ylo = -k.yoff, k.shift = kQ;
+  // num / den * 2^Q rounded half up: num < 2^37 and den < 2^47, so num * 2^(Q+1) + den fits 128 bits
+  auto q = [](long long num, long long den) {
+    using u128 = unsigned __int128;
+    return (long long)((((u128)num << (kQ + 1)) + (u128)den) / (2 * (u128)den));
+  };
+  k.cy = q(255, dy);
+  k.crv = q(510 * (10000 - kr), 10000 * dc);
+  k.cgv = q(510 * kr * (10000 - kr), 10000 * kg * dc);
+  k.cgu = q(510 * kb * (10000 - kb), 10000 * kg * dc);
+  k.cbu = q(510 * (10000 - kb), 10000 * dc);
+  return k;
+}
+
+// Launch the fetch of one read family: 8-bit samples in cv2's BT.601 limited range take the compiled-in constants,
+// everything else the runtime coefficients.
+template <class Read>
+cudaError_t launch_read(const void* src, int64_t st, const Read& read, const YuvFormat& f, int matrix, int full_range,
+                        int T, int H, int W, int oh, int ow, float* out, cudaStream_t s) {
+  using S = typename Read::Src;
+  const S* p = static_cast<const S*>(src);
+  if constexpr (sizeof(S) == 1) {
+    if (matrix == CT3_MATRIX_BT601 && !full_range)
+      return launch_fetch(p, st, YuvFetch<Read, Cv2Bt601>{read, {}}, T, H, W, oh, ow, out, s);
+  }
+  return launch_fetch(p, st, YuvFetch<Read, YuvCoeffs>{read, yuv_coeffs(f, matrix, full_range)}, T, H, W, oh, ow, out,
+                      s);
+}
+
+template <typename S>
+cudaError_t launch_family(const void* src, const YuvFormat& f, int matrix, int full_range, int T, int H, int W,
+                          int64_t st, int64_t sr, int oh, int ow, float* out, cudaStream_t s) {
+  st /= (int64_t)sizeof(S), sr /= (int64_t)sizeof(S);   // byte strides -> sample strides (validated multiples)
+  if (f.family == YuvFormat::kSemiPlanar)
+    return launch_read(src, st, SemiPlanarRead<S>{sr, (int64_t)H * sr}, f, matrix, full_range, T, H, W, oh, ow, out, s);
+  if (f.family == YuvFormat::kPlanar) {
+    const int64_t uv = (int64_t)H * W, cplane = (int64_t)(H >> f.ys) * (W >> f.xs);
+    if (f.ys)
+      return launch_read(src, st, PlanarRead<S, 1, 1>{sr, uv, cplane}, f, matrix, full_range, T, H, W, oh, ow, out, s);
+    if (f.xs)
+      return launch_read(src, st, PlanarRead<S, 1, 0>{sr, uv, cplane}, f, matrix, full_range, T, H, W, oh, ow, out, s);
+    return launch_read(src, st, PlanarRead<S, 0, 0>{sr, uv, cplane}, f, matrix, full_range, T, H, W, oh, ow, out, s);
+  }
+  if constexpr (sizeof(S) == 1)   // YUYV is the only packed layout
+    return launch_read(src, st, PackedRead<S>{sr}, f, matrix, full_range, T, H, W, oh, ow, out, s);
+  return cudaErrorInvalidValue;
+}
+
+}  // namespace
+
+cudaError_t launch_prepare_frames_yuv(const void* src, int layout, int matrix, int full_range, int T, int H, int W,
+                                      int64_t st, int64_t sr, int oh, int ow, float* out, cudaStream_t s) {
+  const YuvFormat& f = *yuv_format(layout);
+  if (f.bytes == 1) return launch_family<uint8_t>(src, f, matrix, full_range, T, H, W, st, sr, oh, ow, out, s);
+  return launch_family<uint16_t>(src, f, matrix, full_range, T, H, W, st, sr, oh, ow, out, s);
 }
 
 }  // namespace ct3

@@ -29,10 +29,30 @@ cudaError_t launch_pyramid_pools(int T, int H4, int W4, float* pyr, cudaStream_t
 // = 2 * (bilinear(align_corners=True) / 255) - 1, bit-identical to the ATen expression (see ingest.cu)
 cudaError_t launch_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t st, int64_t sc, int64_t sh,
                                   int64_t sw, int oh, int ow, float* out, cudaStream_t s);
-// the same of uint8 YUV frames (layout CT3_YUV_*, frame / row byte strides st, sr), converted to RGB as
-// cv2.cvtColor does: bit-identical to launch_prepare_frames on that uint8 RGB clip
-cudaError_t launch_prepare_frames_yuv(const uint8_t* src, int layout, int T, int H, int W, int64_t st, int64_t sr,
-                                      int oh, int ow, float* out, cudaStream_t s);
+// A YUV layout (CT3_YUV_*): its sample size, significant bits, alignment, read family and chroma subsampling.
+struct YuvFormat {
+  enum Family { kSemiPlanar, kPlanar, kPacked };
+  const char* name;
+  int bytes, bits, msb, family, xs, ys;   // chroma covers 2^xs x 2^ys pixels
+};
+inline const YuvFormat* yuv_format(int layout) {
+  static const YuvFormat k[] = {
+      {"NV12", 1, 8, 0, YuvFormat::kSemiPlanar, 1, 1},  {"I420", 1, 8, 0, YuvFormat::kPlanar, 1, 1},
+      {"YUYV", 1, 8, 0, YuvFormat::kPacked, 1, 0},      {"YUV422P", 1, 8, 0, YuvFormat::kPlanar, 1, 0},
+      {"YUV444P", 1, 8, 0, YuvFormat::kPlanar, 0, 0},   {"P010", 2, 10, 1, YuvFormat::kSemiPlanar, 1, 1},
+      {"P016", 2, 16, 1, YuvFormat::kSemiPlanar, 1, 1}, {"YUV420P10", 2, 10, 0, YuvFormat::kPlanar, 1, 1},
+      {"YUV422P10", 2, 10, 0, YuvFormat::kPlanar, 1, 0}, {"YUV444P10", 2, 10, 0, YuvFormat::kPlanar, 0, 0}};
+  return layout >= 0 && layout < (int)(sizeof(k) / sizeof(k[0])) ? &k[layout] : nullptr;
+}
+// rows of one frame seen as [rows, W] samples (YUYV: [H, W, 2])
+inline int64_t yuv_rows(const YuvFormat& f, int H) {
+  if (f.family == YuvFormat::kPacked) return H;
+  return H + (f.xs ? 1 : 2) * (int64_t)(H >> f.ys);
+}
+// the same of YUV frames (layout CT3_YUV_*, CT3_MATRIX_*, full_range 0 | 1; frame / row byte strides st, sr), converted
+// to uint8 RGB by the integer formula of ct3_b200.h: bit-identical to launch_prepare_frames on that uint8 RGB clip
+cudaError_t launch_prepare_frames_yuv(const void* src, int layout, int matrix, int full_range, int T, int H, int W,
+                                      int64_t st, int64_t sr, int oh, int ow, float* out, cudaStream_t s);
 
 // ---- finish.cu : the predictor's tail (arguments validated by ct3_finish_tracks) --------------------
 // forward (+ optional backward, reversed-clip time) tracks [B,T,N,2] / visibility probabilities [B,T,N], queries

@@ -87,6 +87,8 @@ def _signatures():
                                        c_void_p]),
         "ct3_prepare_frames_yuv": (c_int, [c_void_p, c_int, c_int, c_int, c_int, i64, i64, c_int, c_int, c_void_p,
                                            c_void_p]),
+        "ct3_prepare_frames_yuv_fmt": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, i64, i64, c_int, c_int,
+                                               c_void_p, c_void_p]),
         "ct3_finish_tracks": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                       ctypes.c_float, ctypes.c_float, ctypes.c_float, c_void_p, c_void_p, c_void_p]),
         "ct3_finish_tracks_scores": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
@@ -315,39 +317,78 @@ def prepare_frames(src: torch.Tensor, out_hw, out: Optional[torch.Tensor] = None
     return out
 
 
-YUV_LAYOUTS = {"nv12": 0, "i420": 1, "yuyv": 2}   # CT3_YUV_NV12, CT3_YUV_I420, CT3_YUV_YUYV
+YUV_LAYOUTS = {"nv12": 0, "i420": 1, "yuyv": 2}   # CT3_YUV_NV12, CT3_YUV_I420, CT3_YUV_YUYV: ct3_prepare_frames_yuv
+# every layout of ct3_prepare_frames_yuv_fmt (CT3_YUV_*), named as FFmpeg's pix_fmt
+YUV_FORMATS = dict(YUV_LAYOUTS, yuv422p=3, yuv444p=4, p010=5, p016=6, yuv420p10=7, yuv422p10=8, yuv444p10=9)
+YUV_MATRICES = {"bt601": 0, "bt709": 1, "bt2020": 2}   # CT3_MATRIX_*
+_YUV_WIDE = ("p010", "p016", "yuv420p10", "yuv422p10", "yuv444p10")   # 16-bit containers
+# rows of a planar or semi-planar frame per two luma rows: 4:2:0, 4:2:2, 4:4:4
+_YUV_ROWS = {"nv12": 3, "i420": 3, "p010": 3, "p016": 3, "yuv420p10": 3, "yuv422p": 4, "yuv422p10": 4, "yuv444p": 6,
+             "yuv444p10": 6}
+
+
+def yuv_dtype(layout: str) -> torch.dtype:
+    """The sample container of a YUV layout: torch.uint16 for p010, p016 and yuv4xxp10, else torch.uint8."""
+    return torch.uint16 if layout in _YUV_WIDE else torch.uint8
+
+
+def yuv_subsampling(layout: str) -> tuple:
+    """(xs, ys): a chroma sample of a YUV layout covers 2^xs x 2^ys pixels."""
+    return (1, 0) if layout == "yuyv" else {3: (1, 1), 4: (1, 0), 6: (0, 0)}[_YUV_ROWS[layout]]
+
+
+def yuv_frame_shape(layout: str) -> str:
+    """One frame's shape, for messages: [H,W,2] (yuyv) or [rows,W] with rows = H*3/2, 2H or 3H."""
+    return "[H,W,2]" if layout == "yuyv" else {3: "[H*3/2,W]", 4: "[2H,W]", 6: "[3H,W]"}[_YUV_ROWS[layout]]
 
 
 def yuv_frame_hw(layout: str, shape) -> tuple:
-    """(H, W) of the frames of a YUV tensor whose last dimensions are one frame: [H*3/2, W] (nv12, i420) or [H, W, 2]
-    (yuyv); None when the shape is not one of those."""
+    """(H, W) of the frames of a YUV tensor whose last dimensions are one frame: [H*3/2, W] (4:2:0), [2H, W] (4:2:2
+    planar), [3H, W] (4:4:4) or [H, W, 2] (yuyv); None when the shape is not one of those."""
     if layout == "yuyv":
         return (shape[-3], shape[-2]) if len(shape) >= 3 and shape[-1] == 2 else None
-    return (shape[-2] // 3 * 2, shape[-1]) if len(shape) >= 2 and shape[-2] % 3 == 0 else None
+    per = _YUV_ROWS[layout]
+    return (shape[-2] * 2 // per, shape[-1]) if len(shape) >= 2 and shape[-2] * 2 % per == 0 else None
 
 
-def prepare_frames_yuv(src: torch.Tensor, layout: str, out_hw, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """src: T uint8 YUV frames on the device, [T,H*3/2,W] ("nv12", "i420") or [T,H,W,2] ("yuyv") -> [T,3,oh,ow] fp32,
-    bit-identical to prepare_frames on the uint8 RGB clip cv2.cvtColor(COLOR_YUV2RGB_*) makes of them
-    (ct3_prepare_frames_yuv in include/ct3_b200.h).  Any frame stride; NV12 and YUYV rows at any row stride (pitched surfaces), I420 frames
-    dense.  out: optional contiguous fp32 destination of that shape."""
-    if src.dtype != torch.uint8:
-        raise EngineError(f"YUV frames must be uint8, got {src.dtype}")
-    if layout not in YUV_LAYOUTS:
-        raise EngineError(f"unknown YUV layout {layout!r}: one of {sorted(YUV_LAYOUTS)}")
+def check_yuv_colour(matrix: str, full_range) -> None:
+    """Raise ValueError unless matrix is one of YUV_MATRICES and full_range a bool."""
+    if matrix not in YUV_MATRICES:
+        raise ValueError(f"unknown YUV matrix {matrix!r}: one of {sorted(YUV_MATRICES)}")
+    if not isinstance(full_range, bool):
+        raise ValueError(f"full_range must be a bool, got {full_range!r}")
+
+
+def prepare_frames_yuv(src: torch.Tensor, layout: str, out_hw, out: Optional[torch.Tensor] = None, *,
+                       matrix: str = "bt601", full_range: bool = False) -> torch.Tensor:
+    """src: T YUV frames on the device, [T,<one frame>] as `yuv_frame_shape(layout)` gives it, uint8 or (p010, p016,
+    yuv4xxp10) uint16 -> [T,3,oh,ow] fp32, bit-identical to prepare_frames on the uint8 RGB clip the integer formula of
+    include/ct3_b200.h makes of them: with the defaults (BT.601 limited range), the RGB cv2.cvtColor(COLOR_YUV2RGB_*)
+    gives.  Any frame stride; semi-planar and yuyv rows at any row stride (pitched surfaces), planar frames dense.
+    out: optional contiguous fp32 destination of that shape.  The three original layouts in the default colour call
+    ct3_prepare_frames_yuv, everything else ct3_prepare_frames_yuv_fmt."""
+    if src.dtype not in (torch.uint8, torch.uint16):
+        raise EngineError(f"YUV frames must be uint8 or uint16, got {src.dtype}")
+    if layout not in YUV_FORMATS:
+        raise EngineError(f"unknown YUV layout {layout!r}: one of {sorted(YUV_FORMATS)}")
+    if src.dtype != yuv_dtype(layout):
+        raise EngineError(f"{layout} frames must be {yuv_dtype(layout)}, got {src.dtype}")
+    try:
+        check_yuv_colour(matrix, full_range)
+    except ValueError as e:
+        raise EngineError(str(e)) from None
     rank = 4 if layout == "yuyv" else 3
     hw = yuv_frame_hw(layout, src.shape) if src.dim() == rank else None
     if hw is None or src.shape[0] < 1 or hw[0] < 1 or hw[1] < 1:
-        want = "[T,H,W,2]" if layout == "yuyv" else "[T,H*3/2,W]"
-        raise EngineError(f"{layout} frames must be {want}, got {tuple(src.shape)}")
+        raise EngineError(f"{layout} frames must be [T,{yuv_frame_shape(layout)[1:]}, got {tuple(src.shape)}")
     T, (H, W) = src.shape[0], hw
-    # the bytes of a row must be contiguous; a row stride only matters when there is more than one row
+    # the samples of a row must be contiguous; a row stride only matters when there is more than one row
     inner = (2, 1) if layout == "yuyv" else (1,)
     if tuple(src.stride()[-len(inner):]) != inner:
-        raise EngineError(f"the bytes of a {layout} row must be contiguous, got strides {src.stride()}")
+        raise EngineError(f"the samples of a {layout} row must be contiguous, got strides {src.stride()}")
     if not src.is_cuda:
         raise EngineError("src must be a CUDA tensor (no CPU fallback)")
-    rows = src.shape[1]
+    rows, es = src.shape[1], src.element_size()
     stride_row = src.stride(1) if rows > 1 else (2 * W if layout == "yuyv" else W)
     oh, ow = int(out_hw[0]), int(out_hw[1])
     if out is None:
@@ -355,8 +396,12 @@ def prepare_frames_yuv(src: torch.Tensor, layout: str, out_hw, out: Optional[tor
     _req(out, torch.float32, "out")
     if tuple(out.shape) != (T, 3, oh, ow) or out.device != src.device:
         raise EngineError(f"out must be [{T},3,{oh},{ow}] on {src.device}")
-    _call("ct3_prepare_frames_yuv", src.device, _ptr(src), YUV_LAYOUTS[layout], T, H, W, src.stride(0), stride_row, oh,
-          ow, _ptr(out), _stream(src.device))
+    args = (T, H, W, src.stride(0) * es, stride_row * es, oh, ow, _ptr(out), _stream(src.device))
+    if layout in YUV_LAYOUTS and matrix == "bt601" and not full_range:
+        _call("ct3_prepare_frames_yuv", src.device, _ptr(src), YUV_LAYOUTS[layout], *args)
+    else:
+        _call("ct3_prepare_frames_yuv_fmt", src.device, _ptr(src), YUV_FORMATS[layout], YUV_MATRICES[matrix],
+              int(full_range), *args)
     return out
 
 

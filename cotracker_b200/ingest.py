@@ -16,10 +16,12 @@ the same on the device, with k = max(1, min(T, STAGING_SLOT_BYTES // frame_bytes
 2 * max(STAGING_SLOT_BYTES, frame_bytes) each (`staging_bytes`).  The clips of a host batch go through the same two
 slots one after another, so the bound does not grow with B.
 
-A `YUVClip` holds the clip as decoders and cameras emit it (NV12, I420, YUYV) and goes in wherever an RGB clip does.
-Its frames are converted, resized and normalised by one library kernel (ct3_prepare_frames_yuv), bit-identical to the
-RGB path on the uint8 clip cv2.cvtColor(COLOR_YUV2RGB_*) makes of it, and a host clip is uploaded as YUV bytes (1.5
-bytes per pixel for 4:2:0 instead of RGB's 3) through the same two staging slots.
+A `YUVClip` holds the clip as decoders and cameras emit it (NV12, I420, YUYV, 4:2:2 / 4:4:4 planar, and P010 / P016
+/ 10-bit planar in 16-bit containers), with its colour matrix and range, and goes in wherever an RGB clip does.  Its
+frames are converted, resized and normalised by one library kernel (ct3_prepare_frames_yuv[_fmt]), bit-identical to
+the RGB path on the uint8 clip the header's integer formula makes of it (cv2.cvtColor(COLOR_YUV2RGB_*) for 8-bit
+BT.601 limited range), and a host clip is uploaded as YUV bytes (1.5 bytes per pixel for 8-bit 4:2:0 instead of RGB's
+3; a 16-bit 4:2:0 frame is 3) through the same two staging slots.
 """
 from __future__ import annotations
 
@@ -70,28 +72,43 @@ def _dense_strides(shape, strides):
 
 
 class YUVClip:
-    """A clip of uint8 YUV frames: data [B,T,H*3/2,W] for layout "nv12" (H luma rows, then H/2 rows of interleaved U,V)
-    or "i420" (the Y, U and V planes packed, as PyAV's `to_ndarray()` gives yuv420p), or [B,T,H,W,2] for "yuyv"
-    (Y0 U Y1 V per pixel pair); on the host or the device.  H and W must be even (W only, for yuyv).
+    """A clip of YUV frames as decoders and cameras emit them, on the host or the device.  `layout` (FFmpeg's pix_fmt
+    names) and `data`:
+        "nv12"       uint8 [B,T,H*3/2,W]: H luma rows, then H/2 rows of interleaved U,V
+        "i420"       uint8 [B,T,H*3/2,W]: the Y, U and V planes packed, as PyAV's `to_ndarray()` gives yuv420p
+        "yuyv"       uint8 [B,T,H,W,2]: Y0 U Y1 V per pixel pair
+        "yuv422p"    uint8 [B,T,2H,W]: the Y plane, then the H x W/2 U and V planes, packed
+        "yuv444p"    uint8 [B,T,3H,W]: the Y, U and V planes of H x W, packed
+        "p010", "p016"                          torch.uint16 [B,T,H*3/2,W]: nv12 with 16-bit samples, MSB-aligned (10
+                                                or 16 significant bits; the low bits are ignored)
+        "yuv420p10", "yuv422p10", "yuv444p10"   torch.uint16, planar as i420 / yuv422p / yuv444p, 10-bit LSB-aligned
+                                                (the bits above bit 9 are ignored)
+    H must be even for 4:2:0 and W for 4:2:0 / 4:2:2 (yuyv included).
 
-    It stands for the RGB clip [B,T,3,H,W] whose frames are cv2.cvtColor(frame, COLOR_YUV2RGB_{NV12|I420|YUYV}): every
-    predictor and `OnlineStreams.push` take it where they take that clip and give results `torch.equal` to it.  `shape`
-    is that clip's logical (B, T, 3, H, W); `data` is read by `prepare_video` only."""
+    `matrix` ("bt601", "bt709" or "bt2020") and `full_range` describe the colour.  The clip stands for the uint8 RGB
+    clip [B,T,3,H,W] that the integer formula of include/ct3_b200.h gives (a 10- or 16-bit frame rounded to 8 bits, as
+    an rgb24 conversion rounds it).  With the defaults, BT.601 limited range, that is cv2.cvtColor(frame,
+    COLOR_YUV2RGB_*) at 8 bits.  Only the matrix is applied: there is no PQ / HLG transfer function and no tone mapping.
+    Every predictor and `OnlineStreams.push` take a YUVClip where they take that clip and give results `torch.equal` to
+    it.  `shape` is that clip's logical (B, T, 3, H, W); `data` is read by `prepare_video` only."""
 
-    def __init__(self, data: torch.Tensor, layout: str):
-        if layout not in engine.YUV_LAYOUTS:
-            raise ValueError(f"unknown YUV layout {layout!r}: one of {sorted(engine.YUV_LAYOUTS)}")
-        want = "[B,T,H,W,2]" if layout == "yuyv" else "[B,T,H*3/2,W]"
-        if not torch.is_tensor(data) or data.dtype != torch.uint8:
-            raise ValueError(f"{layout} data must be a uint8 tensor {want}, got "
+    def __init__(self, data: torch.Tensor, layout: str, *, matrix: str = "bt601", full_range: bool = False):
+        if layout not in engine.YUV_FORMATS:
+            raise ValueError(f"unknown YUV layout {layout!r}: one of {sorted(engine.YUV_FORMATS)}")
+        engine.check_yuv_colour(matrix, full_range)
+        want = f"[B,T,{engine.yuv_frame_shape(layout)[1:]}"
+        dtype = engine.yuv_dtype(layout)
+        if not torch.is_tensor(data) or data.dtype != dtype:
+            raise ValueError(f"{layout} data must be a {dtype} tensor {want}, got "
                              f"{data.dtype if torch.is_tensor(data) else type(data).__name__}")
         hw = engine.yuv_frame_hw(layout, data.shape) if data.dim() == (5 if layout == "yuyv" else 4) else None
         if hw is None or min(data.shape[:2]) < 1 or min(hw) < 1:
             raise ValueError(f"{layout} data must be {want} with B, T, H, W >= 1, got {tuple(data.shape)}")
-        if hw[1] % 2 or (layout != "yuyv" and hw[0] % 2):
-            raise ValueError(f"{layout} frames must have an even {'width' if layout == 'yuyv' else 'width and height'}"
+        xs, ys = engine.yuv_subsampling(layout)
+        if (ys and hw[0] % 2) or (xs and hw[1] % 2):
+            raise ValueError(f"{layout} frames must have an even {'width and height' if ys else 'width'}"
                              f", got H x W = {hw[0]} x {hw[1]}")
-        self.data, self.layout = data, layout
+        self.data, self.layout, self.matrix, self.full_range = data, layout, matrix, full_range
         self.shape = torch.Size((data.shape[0], data.shape[1], 3) + tuple(hw))
 
     def dim(self) -> int:
@@ -105,11 +122,17 @@ class YUVClip:
     def is_cuda(self) -> bool:
         return self.data.is_cuda
 
+    def with_data(self, data: torch.Tensor) -> "YUVClip":
+        """A clip of the same layout and colour over other frames (e.g. a slice of `data`)."""
+        return YUVClip(data, self.layout, matrix=self.matrix, full_range=self.full_range)
+
     def to(self, device) -> "YUVClip":
-        return YUVClip(self.data.to(device), self.layout)
+        return self.with_data(self.data.to(device))
 
     def __repr__(self) -> str:
-        return f"YUVClip({self.layout}, shape={tuple(self.shape)}, device={self.device})"
+        colour = "" if (self.matrix, self.full_range) == ("bt601", False) else \
+            f", {self.matrix}{' full range' if self.full_range else ''}"
+        return f"YUVClip({self.layout}{colour}, shape={tuple(self.shape)}, device={self.device})"
 
 
 def model_device(model: torch.nn.Module) -> torch.device:
@@ -141,22 +164,24 @@ def prepare_video(video, out_hw, device, out: Optional[torch.Tensor] = None) -> 
     elif tuple(out.shape) != shape or out.dtype != torch.float32 or out.device != device or not out.is_contiguous():
         raise ValueError(f"out must be a contiguous fp32 {shape} tensor on {device}")
     staging = None
-    layout = video.layout if yuv else None
     for b in range(B):
         clip = video.data[b] if yuv else video[b]
         if video.is_cuda and yuv:
-            engine.prepare_frames_yuv(clip, layout, out_hw, out=out[b * T:(b + 1) * T])
+            engine.prepare_frames_yuv(clip, video.layout, out_hw, out=out[b * T:(b + 1) * T], matrix=video.matrix,
+                                      full_range=video.full_range)
         elif video.is_cuda:
             engine.prepare_frames(clip, out_hw, out=out[b * T:(b + 1) * T])
         else:
-            staging = _prepare_host(clip, out_hw, out[b * T:(b + 1) * T], staging, layout)
+            staging = _prepare_host(clip, out_hw, out[b * T:(b + 1) * T], staging, video if yuv else None)
     return out
 
 
-def _prepare_host(v: torch.Tensor, out_hw, out: torch.Tensor, staging=None, layout: Optional[str] = None):
-    """One host clip -> out [T,3,oh,ow] on the device: v [T,3,H,W], or with a YUV `layout` the clip's YUV frames (a
-    `YUVClip`'s data[b]), which are uploaded as they are and converted on the device.  Returns its staging buffers
-    (pinned slots, device slots), which the next clip of a batch takes as `staging`."""
+def _prepare_host(v: torch.Tensor, out_hw, out: torch.Tensor, staging=None, yuv: Optional[YUVClip] = None):
+    """One host clip -> out [T,3,oh,ow] on the device: v [T,3,H,W], or the YUV frames of clip b of `yuv` (its
+    data[b]), which are uploaded as they are, 1 or 2 bytes a sample, and converted on the device in its layout and
+    colour.  Returns its staging buffers (pinned slots, device slots), which the next clip of a batch takes as
+    `staging`."""
+    layout = None if yuv is None else yuv.layout
     T, fshape = v.shape[0], tuple(v.shape[1:])
     oh, ow = int(out_hw[0]), int(out_hw[1])
     device = out.device
@@ -203,7 +228,8 @@ def _prepare_host(v: torch.Tensor, out_hw, out: torch.Tensor, staging=None, layo
         if layout is None:
             engine.prepare_frames(src_dev, (oh, ow), out=out[t0:t1])
         else:
-            engine.prepare_frames_yuv(src_dev, layout, (oh, ow), out=out[t0:t1])
+            engine.prepare_frames_yuv(src_dev, layout, (oh, ow), out=out[t0:t1], matrix=yuv.matrix,
+                                      full_range=yuv.full_range)
         consumed[slot].record(main)
         used[slot] = True
     # the staging buffers go back to PyTorch's caches when this returns: uploads must be done with the pinned memory

@@ -127,6 +127,50 @@ int ct3_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t 
 enum { CT3_YUV_NV12 = 0, CT3_YUV_I420 = 1, CT3_YUV_YUYV = 2 };
 int ct3_prepare_frames_yuv(const uint8_t* src, int layout, int T, int H, int W, int64_t stride_t, int64_t stride_row,
                            int out_h, int out_w, float* out, ct3_stream_t stream);
+/* ct3_prepare_frames_yuv_fmt: the same for more layouts, 10- and 16-bit samples, and a colour description (`matrix`,
+ * `full_range` 0 | 1).  CT3_YUV_NV12 | I420 | YUYV with CT3_MATRIX_BT601 and full_range 0 give exactly what
+ * ct3_prepare_frames_yuv gives.  The layouts (FFmpeg pix_fmt names), at byte strides stride_t and stride_row:
+ *     CT3_YUV_NV12, P010, P016  H luma rows, then H/2 rows of interleaved U,V; stride_row >= W * sample bytes
+ *     CT3_YUV_I420, YUV422P, YUV444P, YUV420P10, YUV422P10, YUV444P10   the Y plane, then the U and V planes of
+ *                               (H/2 | H) x (W/2 | W) samples, packed: stride_row == W * sample bytes
+ *     CT3_YUV_YUYV              H rows of W/2 pixel pairs Y0 U Y1 V; stride_row >= 2W
+ * Samples are uint8, or uint16 for P010 / P016 / *P10 (n = 10, 16, 10 significant bits).  A 16-bit container v holds
+ * the sample v >> (16 - n) when MSB-aligned (P010, P016) and v & (2^n - 1) when LSB-aligned (*P10): the other bits are
+ * ignored.  Chroma is shared by its 2x2 block (4:2:0), its horizontal pair (4:2:2, YUYV) or not at all (4:4:4).
+ *
+ * Each pixel's samples become uint8 RGB by one integer formula (>> is a floor shift), with s = 2^(n-8):
+ *     y = max(Y - yoff, ylo) * cy        u = U - coff        v = V - coff        h = 2^(shift-1)
+ *     R = clamp((y + crv v           + h) >> shift, 0, 255)
+ *     G = clamp((y - cgv v - cgu u   + h) >> shift, 0, 255)
+ *     B = clamp((y + cbu u           + h) >> shift, 0, 255)
+ * - BT.601 limited range keeps cv2's constants at every depth: yoff = 16s, ylo = 0, coff = 128s, shift = 20 + log2 s,
+ *   (cy, crv, cgv, cgu, cbu) = (1220542, 1673527, 852492, 409993, 2116026).  At n = 8 this is the formula above.
+ * - Every other (matrix, range) is derived from Kr, Kb (BT.601 0.299 / 0.114, BT.709 0.2126 / 0.0722, BT.2020
+ *   0.2627 / 0.0593; BT.2020 non-constant luminance) with Kg = 1 - Kr - Kb.  Limited range: yoff = 16s, coff = 128s,
+ *   dy = 219s, dc = 224s.  Full range: yoff = 0, coff = 2^(n-1), dy = dc = 2^n - 1.  Then ylo = -yoff (no floor),
+ *   shift = Q = 48 and each coefficient is its exact rational value times 2^48, rounded half up (computed in 128-bit
+ *   integers from Kr, Kb in units of 1e-4):
+ *     cy = 255 / dy      crv = 255 * 2(1-Kr) / dc      cbu = 255 * 2(1-Kb) / dc
+ *     cgv = 255 * 2Kr(1-Kr) / (Kg dc)      cgu = 255 * 2Kb(1-Kb) / (Kg dc)
+ *   so that R = clamp(floor(255 (Y' + 2(1-Kr) Cr') + 0.5), 0, 255) and likewise G and B, with Y' = (Y - yoff) / dy
+ *   and C' = (C - coff) / dc.  The integers differ from that real value by at most 2^-49 * (|y| + |u| + |v|) <=
+ *   2^(n-48), so they give its rounding wherever it lies farther than that from a tie k + 1/2.  Over all 2^24 8-bit
+ *   triples that is every triple except exact ties, all BT.601 full range: B at U = 3 or 253 (1.772 * 125 = 221.5)
+ *   and G at (U, V) = (78, 178) or (178, 78) (0.37 * 50 = 18.5), for any Y.
+ * - Every term fits int64: |255 Y'| < 280 and |255 * 2(1-K) C'| < 275, so with Q = 48 each product is below 2^57 and
+ *   each sum below 2^59; the cv2 constants at n = 16 stay below 2^38.  (Q20 products overflow int32 from n = 10 on.)
+ * Transfer functions are not applied: no PQ / HLG linearisation and no tone mapping (a BT.2020 frame is converted by
+ * its matrix only, as swscale's default conversion does).
+ *
+ * H must be even for 4:2:0 and W for 4:2:x.  Null pointers, an unknown layout or matrix, full_range outside {0, 1},
+ * T/H/W/out_h/out_w < 1, odd dimensions, an odd stride of a 16-bit layout, a row stride below those bounds, a stride
+ * extent beyond int64 or an output plane above INT32_MAX pixels return CT3_EINVAL before any launch. */
+enum { CT3_YUV_YUV422P = 3, CT3_YUV_YUV444P = 4, CT3_YUV_P010 = 5, CT3_YUV_P016 = 6, CT3_YUV_YUV420P10 = 7,
+       CT3_YUV_YUV422P10 = 8, CT3_YUV_YUV444P10 = 9 };
+enum { CT3_MATRIX_BT601 = 0, CT3_MATRIX_BT709 = 1, CT3_MATRIX_BT2020 = 2 };
+int ct3_prepare_frames_yuv_fmt(const void* src, int layout, int matrix, int full_range, int T, int H, int W,
+                               int64_t stride_t, int64_t stride_row, int out_h, int out_w, float* out,
+                               ct3_stream_t stream);
 
 /* ---- Shi-Tomasi corners: where to seed new tracks ----------------------------------------------------------------
  * ct3_detect_corners: the corners cv2.goodFeaturesToTrack(gray, max_corners, quality_level, min_distance, mask,
