@@ -9,6 +9,14 @@ model-resolution frame (interp_shape, values in [-1, 1]) the predictors track on
 min_distance and exclude_radius are model-resolution pixels.  The points come back in frame pixels, scaled by
 (W-1)/(iw-1), (H-1)/(ih-1) as the predictors scale tracks, so they go straight back in as queries.
 `OnlineStreams.seed_corners` adds such corners to a running stream, away from its own tracks.
+
+A region mask keeps the corners on one object (cv2's `mask` argument, ct3_detect_corners_masked):
+
+    queries = detect_corners(video, 300, mask=object_mask)   # object_mask [1,1,H,W] at frame size, nonzero = inside
+
+Masks are resized to the model resolution on the device (ct3_prepare_masks), exactly as the offline predictor resizes
+`segm_mask`: F.interpolate(mask.float(), interp_shape, mode="nearest") != 0.  `grid_in_mask` is the predictor's rule
+for which grid points a mask keeps.
 """
 from __future__ import annotations
 
@@ -72,16 +80,45 @@ def _exclusion_list(exclude, B: int):
     return exclude
 
 
+def check_mask(mask, B: int, frame_hw, name: str = "mask") -> None:
+    """Raise ValueError unless `mask` is a real or bool tensor [B,1,H,W] or [1,1,H,W] at frame size (H, W)."""
+    H, W = frame_hw
+    if not torch.is_tensor(mask) or mask.dim() != 4 or mask.shape[0] not in (1, B) or mask.shape[1] != 1 \
+            or tuple(mask.shape[2:]) != (H, W) or mask.is_complex():
+        got = tuple(mask.shape) if torch.is_tensor(mask) else type(mask).__name__
+        raise ValueError(f"{name} must be a real or bool tensor [{B},1,{H},{W}] or [1,1,{H},{W}] at frame size, "
+                         f"got {got}")
+
+
+def model_masks(mask: torch.Tensor, interp_shape, device) -> torch.Tensor:
+    """Frame-size masks [B,1,H,W] (any real dtype or bool, host or device) -> [B,ih,iw] uint8 on `device`, 1 where
+    F.interpolate(mask.float(), interp_shape, mode="nearest") != 0: the offline predictor's resize of segm_mask,
+    computed by ct3_prepare_masks."""
+    m = mask[:, 0].to(device)
+    if m.dtype not in engine.MASK_DTYPES:   # nonzero-ness commutes with the nearest resize
+        m = m != 0
+    return engine.prepare_masks(m, interp_shape)
+
+
+def grid_in_mask(grid_pts: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
+    """Grid points [1,n,2] (x, y) at model resolution -> those inside mask [ih,iw] (`model_masks`), read at
+    (round(y), round(x)) as the offline predictor selects them for segm_mask: [1,m,2], m may be 0."""
+    keep = mask[grid_pts[0, :, 1].round().long(), grid_pts[0, :, 0].round().long()] != 0
+    return grid_pts[:, keep]
+
+
 @torch.no_grad()
 def detect_corners(video, max_corners: int, *, frame: int = 0, quality_level: float = 0.01, min_distance: float = 10,
-                   block_size: int = 3, exclude=None, exclude_radius: float = 0, interp_shape=(384, 512)):
+                   block_size: int = 3, exclude=None, exclude_radius: float = 0, interp_shape=(384, 512), mask=None):
     """Shi-Tomasi corners of frame `frame` of each clip of `video`, as queries for the predictors.
 
     video: anything `prepare_video` takes, [B,T,3,H,W] uint8 or float, host or device, or a `YUVClip`; only frame
     `frame` of each clip is prepared (at interp_shape) and searched.  max_corners, quality_level, min_distance and
     block_size are goodFeaturesToTrack's; min_distance is in model-resolution pixels.  exclude: points [B,E,2] or a
     list of B [E_b,2], (x, y) in frame pixels like queries; no corner lies closer than exclude_radius
-    (model-resolution pixels) to one of its clip's points.
+    (model-resolution pixels) to one of its clip's points.  mask: None, or a region per clip [B,1,H,W] or one for
+    every clip [1,1,H,W], at frame size, host or device, nonzero = inside: corners lie inside it, with cv2's `mask`
+    semantics (the quality threshold is relative to the best response inside the mask; an empty mask gives none).
     -> queries [1,n,3] (frame, x, y) in frame pixels, best corner first, for B = 1; a list of B of them otherwise (the
     list-of-queries form CoTrackerPredictor takes).  Runs on the video's device, or the current CUDA device for a host
     video; only the B corner counts are copied to the host."""
@@ -96,6 +133,8 @@ def detect_corners(video, max_corners: int, *, frame: int = 0, quality_level: fl
     if len(interp_shape) != 2 or not all(_is_int(x) and x >= block_size for x in interp_shape):
         raise ValueError(f"interp_shape must be (ih, iw) ints >= block_size = {block_size}, got {interp_shape!r}")
     excl = _exclusion_list(exclude, B)
+    if mask is not None:
+        check_mask(mask, B, (H, W))
     ih, iw = interp_shape
     dev = video.device if video.is_cuda else torch.device("cuda", torch.cuda.current_device())
     frames = ingest.prepare_video(clip_frame(video, frame), (ih, iw), dev)
@@ -106,8 +145,9 @@ def detect_corners(video, max_corners: int, *, frame: int = 0, quality_level: fl
             e = e.to(dev, torch.float32)
             pts[b, :e.shape[0]] = e * e.new_tensor([(iw - 1) / (W - 1), (ih - 1) / (H - 1)])
         points = (pts, [e.shape[0] for e in excl])
+    region = None if mask is None else model_masks(mask, (ih, iw), dev).expand(B, ih, iw)
     found, counts = engine.detect_corners(frames, params(max_corners, quality_level, min_distance, block_size,
-                                                         exclude_radius), points)
+                                                         exclude_radius), points, mask=region)
     scale = found.new_tensor([(W - 1) / (iw - 1), (H - 1) / (ih - 1)])
     out = []
     for b, n in enumerate(counts.tolist()):

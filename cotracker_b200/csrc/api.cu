@@ -523,15 +523,22 @@ int ct3_corners_workspace_bytes(int K, int H, int W, size_t* bytes) {
   return 0;
 }
 
-int ct3_detect_corners(const float* frames, int64_t frame_stride, int K, int H, int W, const ct3_corner_params* params,
-                       const float* exclude, const int32_t* exclude_counts, int E_max, float* corners, int32_t* counts,
-                       void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+namespace {
+// ct3_detect_corners and ct3_detect_corners_masked: mask null runs the kernels without a mask
+int detect_corners(const float* frames, int64_t frame_stride, int K, int H, int W, const ct3_corner_params* params,
+                   const float* exclude, const int32_t* exclude_counts, int E_max, const uint8_t* mask,
+                   int64_t mask_stride, float* corners, int32_t* counts, void* workspace, size_t workspace_bytes,
+                   ct3_stream_t stream) {
   if (!frames || !params || !corners || !counts || !workspace) return fail(CT3_EINVAL, "null argument%s");
   if (int rc = check_corner_shape(K, H, W)) return rc;
   if (int rc = check_aligned(workspace, "workspace")) return rc;
   const int64_t HW = (int64_t)H * W;
   if (frame_stride < 0) return fail(CT3_EINVAL, "frame_stride must be >= 0%s");
   if (K > 1 && frame_stride > (INT64_MAX / 4 - 3 * HW) / (K - 1)) return fail(CT3_EINVAL, "stride extent overflows int64%s");
+  if (mask) {
+    if (mask_stride < 0) return fail(CT3_EINVAL, "mask_stride must be >= 0%s");
+    if (K > 1 && mask_stride > (INT64_MAX - HW) / (K - 1)) return fail(CT3_EINVAL, "mask stride extent overflows int64%s");
+  }
   if (E_max < 0 || E_max > INT32_MAX / 2) return fail(CT3_EINVAL, "E_max must be in [0, 2^30)%s");
   std::vector<CornerFrame> fp(K);
   int M = 0;
@@ -567,8 +574,41 @@ int ct3_detect_corners(const float* frames, int64_t frame_stride, int K, int H, 
   if (int rc = check_space(workspace_bytes, need, "workspace")) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaMemcpyAsync(fp_dev, fp.data(), (size_t)K * sizeof(CornerFrame), cudaMemcpyHostToDevice, s), "detect_corners");
-  CK(launch_detect_corners(frames, frame_stride, K, H, W, fp_dev, exclude, E_max, M, corners, counts, ws, num_sms(), s),
-     "detect_corners");
+  CK(launch_detect_corners(frames, frame_stride, K, H, W, fp_dev, exclude, E_max, mask, mask_stride, M, corners, counts,
+                           ws, num_sms(), s),
+     mask ? "detect_corners_masked" : "detect_corners");
+  return 0;
+}
+}  // namespace
+
+int ct3_detect_corners(const float* frames, int64_t frame_stride, int K, int H, int W, const ct3_corner_params* params,
+                       const float* exclude, const int32_t* exclude_counts, int E_max, float* corners, int32_t* counts,
+                       void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+  return detect_corners(frames, frame_stride, K, H, W, params, exclude, exclude_counts, E_max, nullptr, 0, corners,
+                        counts, workspace, workspace_bytes, stream);
+}
+
+int ct3_detect_corners_masked(const float* frames, int64_t frame_stride, int K, int H, int W,
+                              const ct3_corner_params* params, const float* exclude, const int32_t* exclude_counts,
+                              int E_max, const uint8_t* mask, int64_t mask_stride, float* corners, int32_t* counts,
+                              void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+  if (!mask) return fail(CT3_EINVAL, "null argument%s");
+  return detect_corners(frames, frame_stride, K, H, W, params, exclude, exclude_counts, E_max, mask, mask_stride,
+                        corners, counts, workspace, workspace_bytes, stream);
+}
+
+int ct3_prepare_masks(const void* src, int dtype, int K, int H, int W, int64_t stride_k, int64_t stride_h,
+                      int64_t stride_w, int out_h, int out_w, uint8_t* out, ct3_stream_t stream) {
+  if (!src || !out) return fail(CT3_EINVAL, "null argument%s");
+  if (dtype != CT3_MASK_U8 && dtype != CT3_MASK_BOOL && dtype != CT3_MASK_F32) return fail(CT3_EINVAL, "unknown mask dtype%s");
+  if (K < 1 || K > 65535) return fail(CT3_EINVAL, "K must be in [1, 65535]%s");
+  if (H < 1 || W < 1 || out_h < 1 || out_w < 1) return fail(CT3_EINVAL, "H, W, out_h and out_w must be >= 1%s");
+  // a [K,H,W] source is a [K,3,H,W] frame tensor whose channel stride is 0
+  if (!frame_extent_fits(dtype == CT3_MASK_F32 ? CT3_FRAMES_F32 : CT3_FRAMES_U8, K, H, W, stride_k, 0, stride_h, stride_w))
+    return fail(CT3_EINVAL, "stride extent overflows int64%s");
+  if ((int64_t)out_h * out_w > INT32_MAX) return fail(CT3_EINVAL, "output plane too large%s");
+  CK(launch_prepare_masks(src, dtype == CT3_MASK_F32, K, H, W, stride_k, stride_h, stride_w, out_h, out_w, out,
+                          (cudaStream_t)stream), "prepare_masks");
   return 0;
 }
 

@@ -15,6 +15,10 @@
 //      dx^2 + dy^2 < min_distance^2, up to max_corners.  Kept corners live in a grid of floor(min_distance)-pixel cells
 //      (at most 4 per cell, and a conflict is never more than one cell away); the conflicts inside a batch of 32 are
 //      resolved in rank order with warp shuffles, so the result is the sequential walk's.
+// With a region mask (ct3_detect_corners_masked; kMasked = true) step 1 takes the maximum over the mask's pixels only
+// and step 2 also drops candidates outside the mask; the 3x3 maximum still reads every pixel, as cv2 dilates the whole
+// thresholded map.  ct3_detect_corners runs the kMasked = false instantiations, which are the kernels without the mask.
+// ct3_prepare_masks resizes masks to the detector's frames: ATen's nearest rule, one thread per output pixel.
 #include <math.h>
 
 #include "../../include/ct3_b200.h"
@@ -42,9 +46,11 @@ __device__ __forceinline__ double order_value(unsigned long long k) {
   return __longlong_as_double((long long)((k & 0x8000000000000000ull) ? (k & 0x7fffffffffffffffull) : ~k));
 }
 
+template <bool kMasked>
 __global__ void __launch_bounds__(kTX * kTY)
 corner_response_kernel(const float* __restrict__ frames, int64_t frame_stride, int H, int W,
-                       const CornerFrame* __restrict__ fp, double* __restrict__ lam, unsigned long long* __restrict__ maxkey) {
+                       const CornerFrame* __restrict__ fp, const uint8_t* __restrict__ mask, int64_t mask_stride,
+                       double* __restrict__ lam, unsigned long long* __restrict__ maxkey) {
   __shared__ float g[kTY + 2 * kMaxR][kTX + 2 * kMaxR];
   __shared__ double sdx[kTY + 2 * kMaxR - 2][kTX + 2 * kMaxR - 2];
   __shared__ double sdy[kTY + 2 * kMaxR - 2][kTX + 2 * kMaxR - 2];
@@ -100,7 +106,11 @@ corner_response_kernel(const float* __restrict__ frames, int64_t frame_stride, i
     const double a = __dmul_rn(sxx, 0.5), c = __dmul_rn(syy, 0.5), d = __dsub_rn(a, c);
     const double l = __dsub_rn(__dadd_rn(a, c), __dsqrt_rn(__dadd_rn(__dmul_rn(d, d), __dmul_rn(sxy, sxy))));
     lam[(int64_t)k * HW + (int64_t)y * W + x] = l;
-    key = order_key(l);
+    if constexpr (kMasked) {
+      if (mask[(int64_t)k * mask_stride + (int64_t)y * W + x]) key = order_key(l);   // minMaxLoc(eig, ..., mask)
+    } else {
+      key = order_key(l);
+    }
   }
   for (int o = 16; o; o >>= 1) key = max(key, __shfl_xor_sync(0xffffffffu, key, o));
   if ((tid & 31) == 0 && key) atomicMax(maxkey + k, key);
@@ -112,16 +122,21 @@ __device__ __forceinline__ unsigned long long* cand_keys(uint8_t* cand, int k, i
   return reinterpret_cast<unsigned long long*>(cand + (size_t)k * HW * 16);
 }
 
+template <bool kMasked>
 __global__ void __launch_bounds__(kThreads)
 corner_candidates_kernel(int H, int W, const CornerFrame* __restrict__ fp, const double* __restrict__ lam,
                          const unsigned long long* __restrict__ maxkey, const float* __restrict__ exclude, int E_max,
-                         int* __restrict__ count, uint8_t* __restrict__ cand) {
+                         const uint8_t* __restrict__ mask, int64_t mask_stride, int* __restrict__ count,
+                         uint8_t* __restrict__ cand) {
   const int k = blockIdx.y;
   const int64_t HW = (int64_t)H * W;
   const int64_t p = (int64_t)blockIdx.x * kThreads + threadIdx.x;
   if (p >= HW) return;
   const int y = (int)(p / W), x = (int)(p - (int64_t)y * W);
   if (x < 1 || x >= W - 1 || y < 1 || y >= H - 1) return;
+  if constexpr (kMasked) {
+    if (!mask[(int64_t)k * mask_stride + p]) return;
+  }
   const double* L = lam + (size_t)k * HW;
   const double l = L[p];
   const CornerFrame P = fp[k];
@@ -250,19 +265,57 @@ corner_greedy_kernel(int H, int W, const CornerFrame* __restrict__ fp, const int
   }
 }
 
+// out[k][y][x] = src[k][sy][sx] != 0 with s = min(floor(d * (in / out)), in - 1) in fp32, ATen's nearest index
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+prepare_masks_kernel(const T* __restrict__ src, int H, int W, int64_t stride_k, int64_t stride_h, int64_t stride_w,
+                     int oh, int ow, float scale_h, float scale_w, uint8_t* __restrict__ out) {
+  const int k = blockIdx.y;
+  const int64_t p = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+  if (p >= (int64_t)oh * ow) return;
+  const int y = (int)(p / ow), x = (int)(p - (int64_t)y * ow);
+  const int sy = min((int)floorf(__fmul_rn((float)y, scale_h)), H - 1);
+  const int sx = min((int)floorf(__fmul_rn((float)x, scale_w)), W - 1);
+  const T v = src[(int64_t)k * stride_k + (int64_t)sy * stride_h + (int64_t)sx * stride_w];
+  out[(int64_t)k * oh * ow + p] = v != T(0) ? 1 : 0;
+}
+
 }  // namespace
 
+cudaError_t launch_prepare_masks(const void* src, bool f32, int K, int H, int W, int64_t stride_k, int64_t stride_h,
+                                 int64_t stride_w, int oh, int ow, uint8_t* out, cudaStream_t s) {
+  const dim3 grid((unsigned)(((int64_t)oh * ow + kThreads - 1) / kThreads), K);
+  // area_pixel_compute_scale without align_corners or a scale factor: (float)in / out
+  const float sh = (float)H / (float)oh, sw = (float)W / (float)ow;
+  if (f32)
+    prepare_masks_kernel<float><<<grid, kThreads, 0, s>>>(static_cast<const float*>(src), H, W, stride_k, stride_h,
+                                                          stride_w, oh, ow, sh, sw, out);
+  else
+    prepare_masks_kernel<uint8_t><<<grid, kThreads, 0, s>>>(static_cast<const uint8_t*>(src), H, W, stride_k, stride_h,
+                                                            stride_w, oh, ow, sh, sw, out);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_detect_corners(const float* frames, int64_t frame_stride, int K, int H, int W,
-                                  const CornerFrame* fp_dev, const float* exclude, int E_max, int M, float* corners,
-                                  int32_t* counts, const CornerWorkspace& ws, int num_sms, cudaStream_t s) {
+                                  const CornerFrame* fp_dev, const float* exclude, int E_max, const uint8_t* mask,
+                                  int64_t mask_stride, int M, float* corners, int32_t* counts,
+                                  const CornerWorkspace& ws, int num_sms, cudaStream_t s) {
   const int64_t HW = (int64_t)H * W;
   cudaError_t e = cudaMemsetAsync(ws.maxkey, 0, (size_t)K * (sizeof(unsigned long long) + sizeof(int)), s);
   if (e != cudaSuccess) return e;
   int* count = reinterpret_cast<int*>(ws.maxkey + K);
-  corner_response_kernel<<<dim3((W + kTX - 1) / kTX, (H + kTY - 1) / kTY, K), dim3(kTX, kTY), 0, s>>>(
-      frames, frame_stride, H, W, fp_dev, ws.lam, ws.maxkey);
-  corner_candidates_kernel<<<dim3((unsigned)((HW + kThreads - 1) / kThreads), K), kThreads, 0, s>>>(
-      H, W, fp_dev, ws.lam, ws.maxkey, exclude, E_max, count, ws.cand);
+  const dim3 rgrid((W + kTX - 1) / kTX, (H + kTY - 1) / kTY, K), cgrid((unsigned)((HW + kThreads - 1) / kThreads), K);
+  if (mask) {
+    corner_response_kernel<true><<<rgrid, dim3(kTX, kTY), 0, s>>>(frames, frame_stride, H, W, fp_dev, mask, mask_stride,
+                                                                  ws.lam, ws.maxkey);
+    corner_candidates_kernel<true><<<cgrid, kThreads, 0, s>>>(H, W, fp_dev, ws.lam, ws.maxkey, exclude, E_max, mask,
+                                                              mask_stride, count, ws.cand);
+  } else {
+    corner_response_kernel<false><<<rgrid, dim3(kTX, kTY), 0, s>>>(frames, frame_stride, H, W, fp_dev, nullptr, 0,
+                                                                   ws.lam, ws.maxkey);
+    corner_candidates_kernel<false><<<cgrid, kThreads, 0, s>>>(H, W, fp_dev, ws.lam, ws.maxkey, exclude, E_max,
+                                                               nullptr, 0, count, ws.cand);
+  }
   const int per_frame = max(1, min(4096, (4 * num_sms + K - 1) / K));
   corner_rank_kernel<<<dim3(per_frame, K), kThreads, 0, s>>>(H, W, count, ws.cand);
   corner_greedy_kernel<<<K, kThreads, 0, s>>>(H, W, fp_dev, count, ws.cand, ws.sorted, M, corners, counts);

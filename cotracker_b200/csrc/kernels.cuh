@@ -228,9 +228,14 @@ struct CornerWorkspace {
   uint8_t* cand;                // [K, H*W, 16 bytes] candidates (u64 key, i32 index, i32 rank), then the cell grid
   int* sorted;                  // [K, H*W] candidate pixel indices in rank order
 };
+// mask: null (every pixel), or [K] region masks of H x W bytes at element stride mask_stride (nonzero = inside)
 cudaError_t launch_detect_corners(const float* frames, int64_t frame_stride, int K, int H, int W,
-                                  const CornerFrame* fp_dev, const float* exclude, int E_max, int M, float* corners,
-                                  int32_t* counts, const CornerWorkspace& ws, int num_sms, cudaStream_t s);
+                                  const CornerFrame* fp_dev, const float* exclude, int E_max, const uint8_t* mask,
+                                  int64_t mask_stride, int M, float* corners, int32_t* counts,
+                                  const CornerWorkspace& ws, int num_sms, cudaStream_t s);
+// K masks [H,W] of bytes (uint8 / bool) or fp32 at element strides -> [K,oh,ow] uint8 (ct3_prepare_masks)
+cudaError_t launch_prepare_masks(const void* src, bool f32, int K, int H, int W, int64_t stride_k, int64_t stride_h,
+                                 int64_t stride_w, int oh, int ow, uint8_t* out, cudaStream_t s);
 
 // ---- attention.cu -------------------------------------------------------------------------------
 struct AttnParams {

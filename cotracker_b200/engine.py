@@ -150,6 +150,11 @@ def _signatures():
         "ct3_detect_corners": (c_int, [c_void_p, i64, c_int, c_int, c_int, ctypes.POINTER(CornerParams), c_void_p,
                                        ctypes.POINTER(ctypes.c_int32), c_int, c_void_p, c_void_p, c_void_p, c_size_t,
                                        c_void_p]),
+        "ct3_detect_corners_masked": (c_int, [c_void_p, i64, c_int, c_int, c_int, ctypes.POINTER(CornerParams), c_void_p,
+                                              ctypes.POINTER(ctypes.c_int32), c_int, c_void_p, i64, c_void_p, c_void_p,
+                                              c_void_p, c_size_t, c_void_p]),
+        "ct3_prepare_masks": (c_int, [c_void_p, c_int, c_int, c_int, c_int, i64, i64, i64, c_int, c_int, c_void_p,
+                                      c_void_p]),
         "ct3_profile_enable": (c_int, [c_int]),
         "ct3_profile_read": (c_int, [ctypes.POINTER(ctypes.c_double), intp, ctypes.POINTER(ctypes.c_double)]),
     }
@@ -638,14 +643,17 @@ def corners_workspace_bytes(K: int, H: int, W: int) -> int:
     return _size("ct3_corners_workspace_bytes", int(K), int(H), int(W))
 
 
-def detect_corners(frames: torch.Tensor, params, exclude=None, workspace: Optional[torch.Tensor] = None):
+def detect_corners(frames: torch.Tensor, params, exclude=None, workspace: Optional[torch.Tensor] = None,
+                   mask: Optional[torch.Tensor] = None):
     """Shi-Tomasi corners of K frames in one library call (ct3_detect_corners in include/ct3_b200.h).
     frames [K,3,H,W] fp32 CUDA, each frame contiguous, any frame stride >= 0 (e.g. prepared model-resolution frames).
     params: one CornerParams for every frame, or a sequence of K.  exclude: None, or (points [K,E,2] fp32 CUDA
     contiguous, counts: K ints) -- frame k excludes discs of its params' exclude_radius around its first counts[k]
     points.  workspace: optional scratch of corners_workspace_bytes(K, H, W) bytes; it starts with the responses,
-    fp64 [K,H,W].  -> (corners [K,M,2] fp32 (x, y) in selection order, zero past counts[k]; counts [K] int32), both on
-    the frames' device, M = the largest max_corners."""
+    fp64 [K,H,W].  mask: None, or region masks [K,H,W] uint8 CUDA (nonzero = inside; each mask contiguous, any
+    mask stride >= 0, e.g. `prepare_masks`' output or one mask expanded): cv2's `mask` argument, through
+    ct3_detect_corners_masked.  -> (corners [K,M,2] fp32 (x, y) in selection order, zero past counts[k]; counts [K]
+    int32), both on the frames' device, M = the largest max_corners."""
     if not frames.is_cuda:
         raise EngineError("frames must be a CUDA tensor (no CPU fallback)")
     if frames.dtype != torch.float32:
@@ -672,6 +680,12 @@ def detect_corners(frames: torch.Tensor, params, exclude=None, workspace: Option
         if len(counts) != K:
             raise EngineError(f"exclude counts must hold {K} entries, got {len(counts)}")
         counts = (ctypes.c_int32 * K)(*counts)
+    if mask is not None:
+        if not mask.is_cuda or mask.dtype != torch.uint8 or mask.device != dev:
+            raise EngineError(f"mask must be a uint8 tensor on {dev}, got {mask.dtype} on {mask.device}")
+        if tuple(mask.shape) != (K, H, W) or not mask[0].is_contiguous() or mask.stride(0) < 0:
+            raise EngineError(f"mask must be [{K},{H},{W}] with each mask contiguous, got {tuple(mask.shape)} "
+                              f"strides {mask.stride()}")
     table = (CornerParams * K)(*params)
     M = max(p.max_corners for p in params)
     corners = torch.empty(K, max(M, 0), 2, dtype=torch.float32, device=dev)
@@ -679,9 +693,38 @@ def detect_corners(frames: torch.Tensor, params, exclude=None, workspace: Option
     nbytes = corners_workspace_bytes(K, H, W)
     if workspace is None:
         workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    _call("ct3_detect_corners", dev, _ptr(frames), frames.stride(0), K, H, W, table, _ptr(points), counts, E,
-          _ptr(corners), _ptr(found), _ptr(workspace), workspace.numel(), _stream(dev))
+    if mask is None:
+        _call("ct3_detect_corners", dev, _ptr(frames), frames.stride(0), K, H, W, table, _ptr(points), counts, E,
+              _ptr(corners), _ptr(found), _ptr(workspace), workspace.numel(), _stream(dev))
+    else:
+        _call("ct3_detect_corners_masked", dev, _ptr(frames), frames.stride(0), K, H, W, table, _ptr(points), counts, E,
+              _ptr(mask), mask.stride(0), _ptr(corners), _ptr(found), _ptr(workspace), workspace.numel(), _stream(dev))
     return corners, found
+
+
+MASK_DTYPES = {torch.uint8: 0, torch.bool: 1, torch.float32: 2}   # CT3_MASK_U8, CT3_MASK_BOOL, CT3_MASK_F32
+
+
+def prepare_masks(src: torch.Tensor, out_hw, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """src [K,H,W] uint8, bool or float32 CUDA tensor with any strides -> [K,oh,ow] uint8, 1 where
+    F.interpolate(src[:, None].float(), out_hw, mode="nearest") != 0 and 0 elsewhere, bit-identical to that ATen
+    expression (ct3_prepare_masks).  out: optional contiguous uint8 destination of that shape."""
+    if not src.is_cuda:
+        raise EngineError("src must be a CUDA tensor (no CPU fallback)")
+    if src.dtype not in MASK_DTYPES:
+        raise EngineError(f"src must be uint8, bool or float32, got {src.dtype}")
+    if src.dim() != 3:
+        raise EngineError(f"src must be [K,H,W], got {tuple(src.shape)}")
+    K, H, W = src.shape
+    oh, ow = int(out_hw[0]), int(out_hw[1])
+    if out is None:
+        out = torch.empty(K, oh, ow, dtype=torch.uint8, device=src.device)
+    _req(out, torch.uint8, "out")
+    if tuple(out.shape) != (K, oh, ow) or out.device != src.device:
+        raise EngineError(f"out must be [{K},{oh},{ow}] on {src.device}")
+    _call("ct3_prepare_masks", src.device, _ptr(src), MASK_DTYPES[src.dtype], K, H, W, *src.stride(), oh, ow, _ptr(out),
+          _stream(src.device))
+    return out
 
 
 def pyramid_levels(pyr: torch.Tensor, T: int, H4: int, W4: int) -> List[torch.Tensor]:

@@ -29,7 +29,7 @@ from typing import NamedTuple
 import torch
 import torch.nn.functional as F
 
-from . import engine, ingest
+from . import corners, engine, ingest
 from .build import build_cotracker
 from .evaluation import pass_budget_bytes, plan_clip_passes, plan_dense_passes, plan_ragged_passes
 
@@ -377,17 +377,21 @@ class CoTrackerOnlinePredictor(torch.nn.Module):
 
     @torch.no_grad()
     def forward(self, video_chunk, is_first_step: bool = False, queries: torch.Tensor = None, grid_size: int = 5,
-                grid_query_frame: int = 0, add_support_grid=False, return_scores: bool = False):
+                grid_query_frame: int = 0, add_support_grid=False, return_scores: bool = False,
+                segm_mask: torch.Tensor = None):
         """-> (tracks, visibility), or with return_scores=True (tracks, visibility, TrackScores) of the frames so far
-        (module docstring); (None, None[, None]) at the first step."""
+        (module docstring); (None, None[, None]) at the first step.  segm_mask ([1,1,H,W] at the chunk's frame size,
+        first step, with grid_size): track only the grid points inside it, selected as the offline predictor selects
+        them; add_support_grid then appends the support grid as it does to queries."""
         _check_return_scores(return_scores)
         B, T, C, H, W = video_chunk.shape
         dev = ingest.model_device(self.model)
         if is_first_step:
             # (re)start a video: reset the model state and remember the queries (reference :242-274)
+            queries, self.N = self._first_step_queries(B, (H, W), queries, grid_size, grid_query_frame,
+                                                       add_support_grid, dev, segm_mask)
             self.model.init_video_online_processing()
-            self.queries, self.N = self._first_step_queries(B, (H, W), queries, grid_size, grid_query_frame,
-                                                            add_support_grid, dev)
+            self.queries = queries
             return (None, None, None) if return_scores else (None, None)
 
         if self.queries.shape[0] != B:   # the B streams of the first step advance together
@@ -397,26 +401,40 @@ class CoTrackerOnlinePredictor(torch.nn.Module):
                                        scores=return_scores)
         return (out[0], out[1], TrackScores(out[2], out[3])) if return_scores else out
 
-    def _first_step_queries(self, B, frame_hw, queries, grid_size, grid_query_frame, add_support_grid, dev):
+    def _first_step_queries(self, B, frame_hw, queries, grid_size, grid_query_frame, add_support_grid, dev,
+                            segm_mask=None):
         """The queries [B,N,3] at model resolution a video started with these first-step arguments tracks, and the
-        number of them the output keeps (reference :242-274)."""
+        number of them the output keeps (reference :242-274).  segm_mask keeps the grid points inside it (ValueError
+        when none is) and then treats them as queries: add_support_grid appends the support grid."""
         H, W = frame_hw
         ih, iw = self.interp_shape
         N = None
-        if queries is not None:
+        as_queries = queries is not None or segm_mask is not None
+        if segm_mask is not None:
+            if queries is not None or grid_size <= 0:
+                raise ValueError("segm_mask selects grid points: it needs grid_size > 0 and no queries")
+            corners.check_mask(segm_mask, 1, (H, W), "segm_mask")
+            grid_pts = get_points_on_a_grid(grid_size, self.interp_shape, device=dev)
+            grid_pts = corners.grid_in_mask(grid_pts, corners.model_masks(segm_mask, self.interp_shape, dev)[0])
+            if grid_pts.shape[1] == 0:
+                raise ValueError(f"segm_mask keeps none of the {grid_size}x{grid_size} grid points")
+            N = grid_pts.shape[1]
+            queries = torch.cat([torch.ones_like(grid_pts[:, :, :1]) * grid_query_frame, grid_pts], dim=2)
+            queries = queries.repeat(B, 1, 1)
+        elif queries is not None:
             B, N, D = queries.shape
             assert D == 3
             queries = queries.to(dev).clone()
             queries[:, :, 1:] *= queries.new_tensor([(iw - 1) / (W - 1), (ih - 1) / (H - 1)])
-            if add_support_grid:
-                sup = get_points_on_a_grid(self.support_grid_size, self.interp_shape, device=dev)
-                sup = torch.cat([torch.zeros_like(sup[:, :, :1]), sup], dim=2).repeat(B, 1, 1)
-                queries = torch.cat([queries, sup], dim=1)
         elif grid_size > 0:
             grid_pts = get_points_on_a_grid(grid_size, self.interp_shape, device=dev)
             N = grid_size ** 2
             queries = torch.cat([torch.ones_like(grid_pts[:, :, :1]) * grid_query_frame, grid_pts], dim=2)
             queries = queries.repeat(B, 1, 1)
+        if as_queries and add_support_grid:   # the reference appends no support grid to a plain grid
+            sup = get_points_on_a_grid(self.support_grid_size, self.interp_shape, device=dev)
+            sup = torch.cat([torch.zeros_like(sup[:, :, :1]), sup], dim=2).repeat(B, 1, 1)
+            queries = torch.cat([queries, sup], dim=1)
         return queries, N
 
     def _tail(self, add_support_grid, frame_hw):

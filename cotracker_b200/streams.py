@@ -44,6 +44,7 @@ A stream's tracks can change between steps:
 
     hub.retire_tracks(c, [3, 7])                    # ids of track_ids(c); the support grid's points have none
     new = hub.add_tracks(c, q)                      # [1,m,3] (t, x, y), frame pixels, every t >= hub.length(c)
+    new = hub.seed_grid(c, 20, segm_mask=m)         # the points of a 20x20 grid inside an object's mask [1,1,H,W]
     hub.track_ids(c)                                # the columns of c's next results: open() gave 0..n-1, adds continue
 
 An edit is the same edit of the reference online model's per-track state between two predictor calls, along its N
@@ -81,7 +82,7 @@ import torch
 
 from . import corners, engine, ingest
 from .model import StreamPool, StreamState
-from .predictor import TrackScores, _check_return_scores
+from .predictor import TrackScores, _check_return_scores, get_points_on_a_grid
 
 SNAPSHOT_FORMAT = 1
 _SNAPSHOT_FIELDS = ("model", "frame_size", "n_keep", "ids", "next_id", "n", "ind", "length", "history", "support",
@@ -179,11 +180,14 @@ class OnlineStreams:
 
     @torch.no_grad()
     def open(self, frame_size: Tuple[int, int], queries: torch.Tensor = None, grid_size: int = 5,
-             grid_query_frame: int = 0, add_support_grid: bool = False, history: Optional[int] = None) -> int:
+             grid_query_frame: int = 0, add_support_grid: bool = False, history: Optional[int] = None,
+             segm_mask: Optional[torch.Tensor] = None) -> int:
         """Start a stream of frames of frame_size = (H, W): the arguments of the predictor's `is_first_step=True` call,
         with the frame size in place of the first chunk.  history: None keeps every frame and returns them all at each
         step; an int h >= 1 keeps the stream in fixed memory and returns its last min(h, frames so far) frames.
-        -> the stream's id."""
+        segm_mask: [1,1,H,W] at frame size (host or device, nonzero = inside) of frame grid_query_frame, with
+        grid_size: the stream tracks the grid points inside it, selected as the offline predictor selects them
+        (ValueError when none is), exactly as if they had been passed as queries.  -> the stream's id."""
         if history is not None and (isinstance(history, bool) or not isinstance(history, int) or history < 1):
             raise ValueError(f"history must be None or an int >= 1, got {history!r}")
         H, W = (int(x) for x in frame_size)
@@ -198,7 +202,7 @@ class OnlineStreams:
         if dev.type != "cuda":
             raise ValueError("the predictor's model must be on a CUDA device")
         q, n_out = self.predictor._first_step_queries(1, (H, W), queries, grid_size, grid_query_frame,
-                                                      add_support_grid, dev)
+                                                      add_support_grid, dev, segm_mask)
         state = self.pool.open(*self.model._stream_queries(q[0]), history=history)
         n_keep = n_out if add_support_grid else q.shape[1]
         return self._add(state, (H, W), n_keep, list(range(n_keep)), n_keep)
@@ -305,26 +309,35 @@ class OnlineStreams:
 
     def _insert_tracks(self, s: dict, queries: torch.Tensor) -> List[int]:
         """add_tracks on the stream entry `s` once its queries are checked."""
-        state = s["state"]
         q, _ = self.predictor._first_step_queries(1, s["hw"], queries, 0, 0, False, ingest.model_device(self.model))
+        return self._insert_model_tracks(s, q[0])
+
+    def _insert_model_tracks(self, s: dict, q: torch.Tensor) -> List[int]:
+        """Insert the tracks of queries q [m,3] (t, x, y) at model resolution into the stream entry `s`."""
+        state = s["state"]
         n_keep, scale = s["out"]
-        self.pool.edit(state, range(state.n), n_keep, *self.model._stream_queries(q[0]), self.model.stride)
-        m = q.shape[1]
+        self.pool.edit(state, range(state.n), n_keep, *self.model._stream_queries(q), self.model.stride)
+        m = q.shape[0]
         ids = list(range(s["next_id"], s["next_id"] + m))
         s.update(ids=s["ids"] + ids, next_id=s["next_id"] + m, out=(n_keep + m, scale))
         return ids
 
     @torch.no_grad()
     def seed_corners(self, sid: int, max_tracks: int, *, quality_level: float = 0.01, min_distance: float = 10,
-                     block_size: int = 3, exclude_radius: Optional[float] = None) -> List[int]:
+                     block_size: int = 3, exclude_radius: Optional[float] = None,
+                     mask: Optional[torch.Tensor] = None) -> List[int]:
         """Add up to max_tracks tracks at the Shi-Tomasi corners (`detect_corners`) of stream frame length(sid), the
         first frame the pending chunk adds: call it after push(sid, chunk) and before step().  Corners closer than
         exclude_radius (default min_distance; both model-resolution pixels) to one of the stream's own tracks at frame
-        length(sid) - 1 are left out.  The new tracks start at frame length(sid), as add_tracks adds them.  -> their
-        ids; [] when no corner qualifies, and the stream is unchanged.  Only the corner count reaches the host."""
+        length(sid) - 1 are left out.  mask: None, or [1,1,H,W] at frame size (host or device, nonzero = inside) of
+        frame length(sid): only corners inside it, with cv2's `mask` semantics (`detect_corners`).  The new tracks
+        start at frame length(sid), as add_tracks adds them.  -> their ids; [] when no corner qualifies, and the stream
+        is unchanged.  Only the corner count reaches the host."""
         s = self._get(sid)
         radius = min_distance if exclude_radius is None else exclude_radius
         par = corners.params(max_tracks, quality_level, min_distance, block_size, radius)
+        if mask is not None:
+            corners.check_mask(mask, 1, s["hw"])
         if sid not in self._pending:
             raise ValueError(f"stream {sid} has no pending chunk: push() the chunk to seed before step()")
         state, chunk = s["state"], self._pending[sid]
@@ -340,12 +353,35 @@ class OnlineStreams:
             coords = state.hist[0]
             row = (state.length - 1) % coords.shape[0] if state.history is not None else state.length - 1
             exclude = (coords[row, :n_keep][None].contiguous(), [n_keep])
-        found, counts = engine.detect_corners(frame, par, exclude)
+        region = None if mask is None else corners.model_masks(mask, self.predictor.interp_shape, dev)
+        found, counts = engine.detect_corners(frame, par, exclude, mask=region)
         n = int(counts[0])
         if n == 0:
             return []
         xy = (found[0, :n] * found.new_tensor(scale)).double()
         return self._insert_tracks(s, torch.cat([xy.new_full((n, 1), float(state.length)), xy], 1)[None])
+
+    @torch.no_grad()
+    def seed_grid(self, sid: int, grid_size: int, segm_mask: Optional[torch.Tensor] = None) -> List[int]:
+        """Add tracks at the points of a grid_size x grid_size grid (the grid `open(grid_size=)` tracks) that lie inside
+        segm_mask ([1,1,H,W] at frame size, host or device, nonzero = inside; None: every point), selected as the
+        offline predictor selects them, with query frame length(sid): how an object that appears mid-stream gets
+        tracks.  The tracks are added as add_tracks adds them, with the grid's model-resolution coordinates (so for a
+        frame size equal to the model resolution the result is `torch.equal` to add_tracks with the same points).
+        -> their ids; [] when the mask keeps no point, and the stream is unchanged."""
+        s = self._get(sid)
+        if not _is_int(grid_size) or grid_size < 1:
+            raise ValueError(f"grid_size must be an int >= 1, got {grid_size!r}")
+        if segm_mask is not None:
+            corners.check_mask(segm_mask, 1, s["hw"], "segm_mask")
+        dev = ingest.model_device(self.model)
+        pts = get_points_on_a_grid(grid_size, self.predictor.interp_shape, device=dev)
+        if segm_mask is not None:
+            pts = corners.grid_in_mask(pts, corners.model_masks(segm_mask, self.predictor.interp_shape, dev)[0])
+        if pts.shape[1] == 0:
+            return []
+        pts = pts[0].double()   # fp64 query frames: an fp32 frame index is exact only below 2^24
+        return self._insert_model_tracks(s, torch.cat([pts.new_full((pts.shape[0], 1), float(s["state"].length)), pts], 1))
 
     def retire_tracks(self, sid: int, ids):
         """Remove the tracks `ids` (ids of stream `sid`, see track_ids) from its next step on.  The support grid's

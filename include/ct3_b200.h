@@ -212,6 +212,34 @@ int ct3_corners_workspace_bytes(int K, int H, int W, size_t* bytes);
 int ct3_detect_corners(const float* frames, int64_t frame_stride, int K, int H, int W, const ct3_corner_params* params,
                        const float* exclude, const int32_t* exclude_counts, int E_max, float* corners, int32_t* counts,
                        void* workspace, size_t workspace_bytes, ct3_stream_t stream);
+/* ct3_detect_corners_masked: the same with cv2's `mask` argument, a region per frame, as OpenCV 4's
+ * goodFeaturesToTrack applies it.  Steps 1-4, 6 and 7 are those above; with M the frame's mask (nonzero = inside):
+ *   5a. the threshold's maximum is the max lambda over the pixels inside M only (minMaxLoc(eig, ..., mask)), so corners
+ *       weaker than quality_level times the frame's global maximum can be returned;
+ *   5b. the threshold and the 3x3 maximum test still read every pixel: a neighbour outside M suppresses a candidate
+ *       inside it (cv2 dilates the whole thresholded map);
+ *   5c. a candidate lies inside M (besides the border and the exclusion discs of step 5);
+ *   5d. a frame whose mask is all zero yields 0 corners.
+ * mask: device [K,H,W] bytes at element stride mask_stride >= 0 between frames (0: one mask for every frame), rows
+ * contiguous.  Every other argument, the workspace and the outputs are ct3_detect_corners's.  A null mask, a negative
+ * mask_stride or a mask extent beyond int64 return CT3_EINVAL before any launch, besides every rejection of
+ * ct3_detect_corners.  ct3_detect_corners itself runs the kernels without a mask. */
+int ct3_detect_corners_masked(const float* frames, int64_t frame_stride, int K, int H, int W,
+                              const ct3_corner_params* params, const float* exclude, const int32_t* exclude_counts,
+                              int E_max, const uint8_t* mask, int64_t mask_stride, float* corners, int32_t* counts,
+                              void* workspace, size_t workspace_bytes, ct3_stream_t stream);
+/* ct3_prepare_masks: K region masks resized to the detector's frames by nearest-neighbour sampling, bit-identical to
+ *     F.interpolate(mask.float(), (out_h, out_w), mode="nearest") != 0
+ * as ATen evaluates it: out[k][y][x] = src[k][sy][sx] != 0 with sy = min(floor(y * s_h), H - 1), s_h = (float)H / out_h,
+ * the product and the quotient rounded to fp32 (likewise x).  That is not always floor(y * H / out_h): the rounded
+ * quotient can put the product on the other side of an integer.  src: device [K,H,W] of element type `dtype`
+ * (CT3_MASK_*: uint8 and bool are bytes, nonzero = inside; fp32 is inside unless it equals 0, so NaN is inside and -0 is
+ * not) at any int64 ELEMENT strides.  out: [K,out_h,out_w] uint8 contiguous, 1 inside, 0 outside.  Null pointers, an
+ * unknown dtype, K outside [1, 65535], H/W/out_h/out_w < 1, a stride extent beyond int64 or an output plane above
+ * INT32_MAX pixels return CT3_EINVAL before any launch. */
+enum { CT3_MASK_U8 = 0, CT3_MASK_BOOL = 1, CT3_MASK_F32 = 2 };
+int ct3_prepare_masks(const void* src, int dtype, int K, int H, int W, int64_t stride_k, int64_t stride_h,
+                      int64_t stride_w, int out_h, int out_w, uint8_t* out, ct3_stream_t stream);
 
 /* ---- the predictor's tail ---------------------------------------------------
  * ct3_finish_tracks: what CoTrackerPredictor does with the model's output (predictor.py:161-209), for B clips in one
