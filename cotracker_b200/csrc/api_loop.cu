@@ -339,6 +339,49 @@ int space_attention(Runner& R, const Workspace& W, const GroupPlan& gp, AttnPara
   return 0;
 }
 
+// ---- ct3_body_trace: the links of transformer_body, each 256-byte aligned in the caller's buffer, in launch order
+struct BodyTrace {
+  uint8_t* base = nullptr;
+  size_t off[CT3_BODY_TRACE_LINKS] = {}, bytes[CT3_BODY_TRACE_LINKS] = {};
+  int n = 0;   // links taken so far
+};
+// fills tr.off / tr.bytes for a G = 1 pass of T frames and N tracks; returns the total bytes
+size_t body_trace_layout(BodyTrace& tr, int T, int N) {
+  const int64_t Rp = (int64_t)N * T, Rv = (int64_t)kV * T, R = Rp + Rv;
+  int n = 0;
+  size_t off = 0;
+  auto link = [&](int64_t rows, int cols, int esz) {
+    tr.off[n] = off;
+    tr.bytes[n] = (size_t)rows * cols * esz;
+    off = align_up(off + tr.bytes[n]);
+    ++n;
+  };
+  auto mlp = [&](int64_t rows) { link(rows, 2 * kC, 2); link(rows, 2 * kMlpHid, 2); link(rows, kC, 4); };
+  link(Rv, kC, 4);                                                                      // virtual init
+  for (int i = 0; i < kDepth; ++i) {
+    link(R, 2 * kC, 2); link(R, 3 * kC, 4); link(R, 2 * kC, 2); link(R, kC, 4); mlp(R);  // time
+    link(Rv, 2 * kC, 2); link(Rv, kC, 4); link(Rp, 2 * kC, 2); link(Rp, 2 * kC, 4);      // virtual <- point
+    link(Rv, 2 * kC, 2); link(Rv, kC, 4); mlp(Rv);
+    link(Rv, 2 * kC, 2); link(Rv, 3 * kC, 4); link(Rv, 2 * kC, 2); link(Rv, kC, 4); mlp(Rv);   // virtual self
+    link(Rp, 2 * kC, 2); link(Rp, kC, 4); link(Rv, 2 * kC, 2); link(Rv, 2 * kC, 4);      // point <- virtual
+    link(Rp, 2 * kC, 2); link(Rp, kC, 4); mlp(Rp);
+  }
+  return off;
+}
+// the next link of the trace: a copy of src, whose size must be the layout's; src == nullptr leaves the link as it is
+// (the time block's q|k|v when the fused kernel keeps it on chip).  tr == nullptr: nothing.
+int body_tap(BodyTrace* tr, const void* src, int64_t rows, int cols, int esz, cudaStream_t s) {
+  if (!tr) return 0;
+  const size_t bytes = (size_t)rows * cols * esz;
+  if (tr->n >= CT3_BODY_TRACE_LINKS || bytes != tr->bytes[tr->n])
+    return fail(CT3_EINVAL, "body trace: links out of step with the layout%s");
+  if (src) CK(cudaMemcpyAsync(tr->base + tr->off[tr->n], src, bytes, cudaMemcpyDeviceToDevice, s), "body trace copy");
+  ++tr->n;
+  return 0;
+}
+#define TAP(...) \
+  if (int rc__ = body_tap(__VA_ARGS__)) return rc__
+
 // q|k|v projection and the per-track T x T attention of time block b on the LayerNorm output x [rows, 2*kC] (rows
 // n*T + t) into att (split rows of pitch 2*kC).  With fuse = 1 on the product kernels (gemm 0, attn != 1) and T <= 128
 // both run in ONE kernel, so fp32 q|k|v never reaches HBM; otherwise the b.q GEMM writes q|k|v to W.qkv [rows, 3*kC]
@@ -348,8 +391,10 @@ int space_attention(Runner& R, const Workspace& W, const GroupPlan& gp, AttnPara
 // T > 128 and fusion on, the runs of tracks of at most 128 frames take the fused kernel (one track per tile, rows
 // t < 128) and the other runs the unfused one, each track once.  The fused kernel leaves rows [128, T) of a short
 // track, all of them padding, unwritten: they are zeroed so that every padded row stays finite.
+// tr: a trace sink (G = 1 only), which takes the unfused route's fp32 q|k|v or notes that the fused kernel ran.
 int time_attention(Runner& R, const Workspace& W, const Block& b, const __nv_bfloat16* x, __nv_bfloat16* att,
-                   int rows, int T, const int32_t* len = nullptr, const int32_t* len_host = nullptr) {
+                   int rows, int T, const int32_t* len = nullptr, const int32_t* len_host = nullptr,
+                   BodyTrace* tr = nullptr) {
   const bool fuse = g_opt[OPT_FUSE] == 1 && R.impl == 0 && g_opt_attn != 1;
   // The fused kernel reads keys [0, len) of a track from its 128-row tile: with T > 128 only tracks whose len_host
   // entry is at most 128 may reach it, which the run split below guarantees (qkv_time_attn_supported).
@@ -361,11 +406,14 @@ int time_attention(Runner& R, const Workspace& W, const Block& b, const __nv_bfl
         x + r0 * 2 * kC, reinterpret_cast<const __nv_bfloat16*>(R.pk + b.qkv_h.w),
         reinterpret_cast<const float*>(R.pk + b.qkv_h.b), tracks * T, kC, T, len ? len + track0 : nullptr,
         att + r0 * 2 * kC, 2 * kC, kC, 1.0f / sqrtf((float)kDh), num_sms(), R.s, &gerr);
-    return rc ? fail_launch(rc, "fused qkv + time attention", gerr) : 0;
+    if (rc) return fail_launch(rc, "fused qkv + time attention", gerr);
+    TAP(tr, nullptr, (int64_t)tracks * T, 3 * kC, 4, R.s);
+    return 0;
   };
   auto unfused = [&](int track0, int tracks) -> int {
     const int64_t r0 = (int64_t)track0 * T;
     GEMM(x + r0 * 2 * kC, b.q, tracks * T, Runner::to_f32(W.qkv, 3 * kC, false));
+    TAP(tr, W.qkv, (int64_t)tracks * T, 3 * kC, 4, R.s);
     AttnParams a = attn_params(W.qkv, 3 * kC, W.qkv, 3 * kC, kC, 2 * kC, att + r0 * 2 * kC, T, T, T, tracks);
     a.seq_len = len ? len + track0 : nullptr;
     RUNC(CAT_ATTN, run_attention(R, W, a, true));
@@ -412,26 +460,33 @@ int for_slabs(const Workspace& W, int N, int n_begin, int n_end, F&& f) {
 
 // x += to_out(attn(...)); x += mlp(LN(x))   for the rows [row0, row0+rows) of the token buffer, which lie in the slab
 // whose first row is slab_row0
-int mlp_half(Runner& R, const Workspace& W, const Block& b, int64_t row0, int rows, int64_t slab_row0) {
+int mlp_half(Runner& R, const Workspace& W, const Block& b, int64_t row0, int rows, int64_t slab_row0,
+             BodyTrace* tr = nullptr) {
   float* x = W.tokens + row0 * kC;
   const int64_t s = scratch_row(W, row0, slab_row0);
   __nv_bfloat16* ln = W.ln + s * 2 * kC;
   __nv_bfloat16* hm = W.hmid + s * 2 * kMlpHid;
   RUNC(CAT_LN, launch_layernorm_split(x, rows, nullptr, nullptr, 1e-6f, ln, R.s));
+  TAP(tr, ln, rows, 2 * kC, 2, R.s);
   GEMM(ln, b.fc1, rows, Runner::to_split(hm, 2 * kMlpHid, kMlpHid, /*tanh*/ 2));
+  TAP(tr, hm, rows, 2 * kMlpHid, 2, R.s);
   GEMM(hm, b.fc2, rows, Runner::to_f32(x, kC, true));
+  TAP(tr, x, rows, kC, 4, R.s);
   return 0;
 }
 
 // EfficientUpdateFormer body on W.tokens (point rows already hold input_transform output) -- cotracker.py:486-524.
 // With track slabs (DESIGN.md §4.4.5) the row-independent stages run slab by slab (for_slabs); the space attentions
-// always see every track of a group in one launch.
-int transformer_body(Runner& R, const Workspace& W, int T, int N, const GroupPlan& gp) {
+// always see every track of a group in one launch.  tr: an optional trace sink (G = 1, no slabs), which takes a copy of
+// every link's output right after the launch that writes it (body_trace_layout's order); without one the launches are
+// the same.
+int transformer_body(Runner& R, const Workspace& W, int T, int N, const GroupPlan& gp, BodyTrace* tr = nullptr) {
   const Layout& L = R.L;
   const int NV = kV * gp.G, Rp = N * T, Rv = NV * T;
   const uint8_t* pk = R.pk;
   RUNC(CAT_MISC, launch_init_virtual(W.tokens, reinterpret_cast<const float*>(pk + L.virt), T, N, gp.G, R.s));
   float* vtok = W.tokens + (int64_t)Rp * kC;
+  TAP(tr, vtok, Rv, kC, 4, R.s);
   __nv_bfloat16* ln_v = W.ln + W.slab_rows * 2 * kC;
   __nv_bfloat16* att_v = W.att + W.slab_rows * 2 * kC;
   // point<-virtual's q and output: with slabs both full-size in W.qkv, behind each other
@@ -447,14 +502,16 @@ int transformer_body(Runner& R, const Workspace& W, int T, int N, const GroupPla
                                           ctx ? reinterpret_cast<const float*>(pk + b.ctx_g) : nullptr,
                                           ctx ? reinterpret_cast<const float*>(pk + b.ctx_b) : nullptr,
                                           ctx ? 1e-5f : 1e-6f, ln, R.s));
+      TAP(tr, ln, (int64_t)count * T, 2 * kC, 2, R.s);
       GEMM(ln, lin, count * T, Runner::to_f32(out + r0 * ld, ld, false));
+      TAP(tr, out + r0 * ld, (int64_t)count * T, ld, 4, R.s);
       return 0;
     });
   };
   // the MLP half of tracks [n_begin, n_end), slab by slab
   auto mlp_tracks = [&](const Block& b, int n_begin, int n_end) {
     return for_slabs(W, N, n_begin, n_end, [&](int n, int count) -> int {
-      return mlp_half(R, W, b, (int64_t)n * T, count * T, (int64_t)n * T);
+      return mlp_half(R, W, b, (int64_t)n * T, count * T, (int64_t)n * T, tr);
     });
   };
 
@@ -467,32 +524,43 @@ int transformer_body(Runner& R, const Workspace& W, int T, int N, const GroupPla
             const int64_t s0 = scratch_row(W, r0, r0);
             float* x = W.tokens + r0 * kC;
             RUNC(CAT_LN, launch_layernorm_split(x, rows, nullptr, nullptr, 1e-6f, W.ln + s0 * 2 * kC, R.s));
+            TAP(tr, W.ln + s0 * 2 * kC, rows, 2 * kC, 2, R.s);
             if (int rc = time_attention(R, W, b, W.ln + s0 * 2 * kC, W.att + s0 * 2 * kC, rows, T,
                                         gp.track_len ? gp.track_len + n : nullptr,
-                                        gp.track_len_host ? gp.track_len_host + n : nullptr))
+                                        gp.track_len_host ? gp.track_len_host + n : nullptr, tr))
               return rc;
+            TAP(tr, W.att + s0 * 2 * kC, rows, 2 * kC, 2, R.s);
             GEMM(W.att + s0 * 2 * kC, b.out, rows, Runner::to_f32(x, kC, true));
-            return mlp_half(R, W, b, r0, rows, r0);
+            TAP(tr, x, rows, kC, 4, R.s);
+            return mlp_half(R, W, b, r0, rows, r0, tr);
           }))
         return rc;
     }
     {  // ---- virtual <- point cross attention (cotracker.py:510-512): x = virtual, context = points
       const Block& b = L.v2p[i];
       RUNC(CAT_LN, launch_layernorm_split(vtok, Rv, nullptr, nullptr, 1e-6f, ln_v, R.s));
+      TAP(tr, ln_v, Rv, 2 * kC, 2, R.s);
       GEMM(ln_v, b.q, Rv, Runner::to_f32(W.vqkv, kC, false));
+      TAP(tr, W.vqkv, Rv, kC, 4, R.s);
       if (int rc = ln_gemm_points(b, true, b.kv, W.qkv, 2 * kC)) return rc;
       RUNC(CAT_ATTN, space_attention(R, W, gp, attn_params(W.vqkv, kC, W.qkv, 2 * kC, 0, kC, att_v, kV, N, T), false,
                                      true));
+      TAP(tr, att_v, Rv, 2 * kC, 2, R.s);
       GEMM(att_v, b.out, Rv, Runner::to_f32(vtok, kC, true));
+      TAP(tr, vtok, Rv, kC, 4, R.s);
       if (int rc = mlp_tracks(b, N, N + NV)) return rc;
     }
     {  // ---- virtual self attention (cotracker.py:514): sequence = frame over the 64 virtual tokens
       const Block& b = L.vself[i];
       RUNC(CAT_LN, launch_layernorm_split(vtok, Rv, nullptr, nullptr, 1e-6f, ln_v, R.s));
+      TAP(tr, ln_v, Rv, 2 * kC, 2, R.s);
       GEMM(ln_v, b.q, Rv, Runner::to_f32(W.vqkv, 3 * kC, false));
+      TAP(tr, W.vqkv, Rv, 3 * kC, 4, R.s);
       RUNC(CAT_ATTN, space_attention(R, W, gp, attn_params(W.vqkv, 3 * kC, W.vqkv, 3 * kC, kC, 2 * kC, att_v, kV, kV,
                                                            T), false, false));
+      TAP(tr, att_v, Rv, 2 * kC, 2, R.s);
       GEMM(att_v, b.out, Rv, Runner::to_f32(vtok, kC, true));
+      TAP(tr, vtok, Rv, kC, 4, R.s);
       if (int rc = mlp_tracks(b, N, N + NV)) return rc;
     }
     {  // ---- point <- virtual cross attention (cotracker.py:515-517): x = points, context = virtual
@@ -500,13 +568,17 @@ int transformer_body(Runner& R, const Workspace& W, int T, int N, const GroupPla
       if (int rc = ln_gemm_points(b, false, b.q, q_p, kC)) return rc;
       RUNC(CAT_LN, launch_layernorm_split(vtok, Rv, reinterpret_cast<const float*>(pk + b.ctx_g),
                                  reinterpret_cast<const float*>(pk + b.ctx_b), 1e-5f, ln_v, R.s));
+      TAP(tr, ln_v, Rv, 2 * kC, 2, R.s);
       GEMM(ln_v, b.kv, Rv, Runner::to_f32(W.vqkv, 2 * kC, false));
+      TAP(tr, W.vqkv, Rv, 2 * kC, 4, R.s);
       RUNC(CAT_ATTN, space_attention(R, W, gp, attn_params(q_p, kC, W.vqkv, 2 * kC, 0, kC, att_p, N, kV, T), true,
                                      false));
+      TAP(tr, att_p, Rp, 2 * kC, 2, R.s);
       if (int rc = for_slabs(W, N, 0, N, [&](int n, int count) -> int {
             const int64_t r0 = (int64_t)n * T;
             GEMM(att_p + r0 * 2 * kC, b.out, count * T, Runner::to_f32(W.tokens + r0 * kC, kC, true));
-            return mlp_half(R, W, b, r0, count * T, r0);
+            TAP(tr, W.tokens + r0 * kC, (int64_t)count * T, kC, 4, R.s);
+            return mlp_half(R, W, b, r0, count * T, r0, tr);
           }))
         return rc;
     }
@@ -588,9 +660,9 @@ int point_tokens(Runner& R, const Workspace& W, const Prec& pr, const float* pyr
 // The steps update_loop and updateformer share once the point tokens are in W.tokens: the transformer body, then the
 // heads: the state update of coords / vis / conf, or with delta != nullptr the raw deltas [N,T,4] instead.
 int transform_and_heads(Runner& R, const Workspace& W, int T, int N, const GroupPlan& gp, float* coords, float* vis,
-                        float* conf, float* delta) {
+                        float* conf, float* delta, BodyTrace* tr = nullptr) {
   const Layout& L = R.L;
-  if (int rc = transformer_body(R, W, T, N, gp)) return rc;
+  if (int rc = transformer_body(R, W, T, N, gp, tr)) return rc;
   RUNC(CAT_MISC, launch_heads(W.tokens, reinterpret_cast<const float*>(R.pk + L.heads_w),
                               reinterpret_cast<const float*>(R.pk + L.heads_b), coords, vis, conf, delta, T, N, R.s));
   return 0;
@@ -758,6 +830,27 @@ int updateformer(const void* packed, const float* x, int T, int N, const int32_t
   RUNC(CAT_MISC, launch_split_rows(x, N * T, kX, kXPad, /*perm_x*/ 1, W.xs, 0, R.s));
   if (int rc = input_transform(R, W, T, 0, N, nullptr)) return rc;
   return transform_and_heads(R, W, T, N, gp, nullptr, nullptr, nullptr, delta);
+}
+
+// ct3_body_trace: the point tokens into W.tokens, then transform_and_heads with a trace sink (G = 1, no slabs, no frame
+// map or group lengths).  Checks as ct3_updateformer.
+int body_trace(const void* packed, const float* tokens, int T, int N, float* coords, float* vis, float* conf,
+               void* trace, size_t trace_bytes, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (!packed || !tokens || !coords || !vis || !conf || !trace || !workspace) return fail(CT3_EINVAL, "null argument%s");
+  const ct3_loop_shape shape{T, N, 0, 0, 1, nullptr, 0, nullptr, 0, nullptr};
+  if (int rc = check_shape(&shape, Use::kFormer)) return rc;
+  if (int rc = check_aligned(workspace, "workspace")) return rc;
+  if (int rc = check_aligned(trace, "trace")) return rc;
+  const Workspace W = carve(workspace, shape);
+  if (int rc = check_space(workspace_bytes, W.total, "workspace")) return rc;
+  BodyTrace tr;
+  tr.base = reinterpret_cast<uint8_t*>(trace);
+  if (int rc = check_space(trace_bytes, body_trace_layout(tr, T, N), "trace buffer")) return rc;
+  Runner R{reinterpret_cast<const uint8_t*>(packed), layout(), stream, g_opt_gemm};
+  const GroupPlan gp;
+  CK(cudaMemcpyAsync(W.tokens, tokens, (size_t)N * T * kC * 4, cudaMemcpyDeviceToDevice, R.s), "copy point tokens");
+  if (int rc = transform_and_heads(R, W, T, N, gp, coords, vis, conf, nullptr, &tr)) return rc;
+  return tr.n == CT3_BODY_TRACE_LINKS ? 0 : fail(CT3_EINVAL, "body trace: links out of step with the layout%s");
 }
 
 // ct3_attention: the split-K partials and the group table, the attention parts of carve()
@@ -1042,6 +1135,24 @@ int ct3_loop_tokens(const void* packed, const float* pyr, int H4, int W4, const 
 int ct3_updateformer(const void* packed, const float* x, int T, int N, const int32_t* group_sizes_host, int G,
                      float* delta, void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
   return updateformer(packed, x, T, N, group_sizes_host, G, delta, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int ct3_body_trace_layout(int T, int N, int64_t* offsets, int64_t* bytes, size_t* total_bytes) {
+  if (!total_bytes) return fail(CT3_EINVAL, "null total_bytes%s");
+  if (int rc = check_TN(T, N)) return rc;
+  BodyTrace tr;
+  *total_bytes = body_trace_layout(tr, T, N);
+  for (int i = 0; i < CT3_BODY_TRACE_LINKS; ++i) {
+    if (offsets) offsets[i] = (int64_t)tr.off[i];
+    if (bytes) bytes[i] = (int64_t)tr.bytes[i];
+  }
+  return 0;
+}
+
+int ct3_body_trace(const void* packed, const float* tokens, int T, int N, float* coords, float* vis, float* conf,
+                   void* trace, size_t trace_bytes, void* workspace, size_t workspace_bytes, ct3_stream_t stream) {
+  return body_trace(packed, tokens, T, N, coords, vis, conf, trace, trace_bytes, workspace, workspace_bytes,
+                    (cudaStream_t)stream);
 }
 
 int ct3_attention_workspace_bytes(int T, int N, int G, size_t* out_bytes) {

@@ -146,6 +146,9 @@ def _signatures():
         "ct3_encoder_trace_layout": (c_int, [c_int, c_int, c_int, i64p, i64p, ctypes.POINTER(c_size_t)]),
         "ct3_encoder_trace": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p,
                                       c_size_t, c_void_p]),
+        "ct3_body_trace_layout": (c_int, [c_int, c_int, i64p, i64p, ctypes.POINTER(c_size_t)]),
+        "ct3_body_trace": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                                   c_void_p, c_size_t, c_void_p]),
         "ct3_corners_workspace_bytes": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
         "ct3_detect_corners": (c_int, [c_void_p, i64, c_int, c_int, c_int, ctypes.POINTER(CornerParams), c_void_p,
                                        ctypes.POINTER(ctypes.c_int32), c_int, c_void_p, c_void_p, c_void_p, c_size_t,
@@ -1262,6 +1265,88 @@ def encoder_trace(packed: torch.Tensor, frames: torch.Tensor, workspace: Optiona
             raise EngineError(f"encoder trace link {name}: {n} bytes, expected {shape} {dtype}")
         out[name] = buf[o:o + n].view(dtype).reshape(shape)
     out["pyramid"] = pyr
+    return out
+
+
+BODY_TRACE_LINKS = 97
+BODY_DEPTH = 3
+
+
+def body_trace_links(T: int, N: int) -> List[tuple]:
+    """The links of ct3_body_trace in buffer order (include/ct3_b200.h) -> [(name, dtype, shape)]: bf16 links are split
+    rows [rows, 2*C] (hi | lo), fp32 links [rows, C].  Names are "virtual_init" and "<block>.<kind>.<link>" with kind
+    time, v2p (virtual <- point), vself (virtual self) or p2v (point <- virtual)."""
+    Rp, Rv = N * T, 64 * T
+    R = Rp + Rv
+    links = [("virtual_init", torch.float32, (Rv, HID))]
+
+    def add(p, name, rows, cols, dtype):
+        links.append((f"{p}.{name}", dtype, (rows, cols)))
+
+    def mlp(p, rows):
+        add(p, "mlp_ln", rows, 2 * HID, torch.bfloat16)
+        add(p, "fc1", rows, 2 * 4 * HID, torch.bfloat16)
+        add(p, "fc2", rows, HID, torch.float32)
+
+    for i in range(BODY_DEPTH):
+        p = f"{i}.time"
+        add(p, "ln", R, 2 * HID, torch.bfloat16), add(p, "qkv", R, 3 * HID, torch.float32)
+        add(p, "attn", R, 2 * HID, torch.bfloat16), add(p, "out", R, HID, torch.float32), mlp(p, R)
+        p = f"{i}.v2p"
+        add(p, "ln", Rv, 2 * HID, torch.bfloat16), add(p, "q", Rv, HID, torch.float32)
+        add(p, "ctx_ln", Rp, 2 * HID, torch.bfloat16), add(p, "kv", Rp, 2 * HID, torch.float32)
+        add(p, "attn", Rv, 2 * HID, torch.bfloat16), add(p, "out", Rv, HID, torch.float32), mlp(p, Rv)
+        p = f"{i}.vself"
+        add(p, "ln", Rv, 2 * HID, torch.bfloat16), add(p, "qkv", Rv, 3 * HID, torch.float32)
+        add(p, "attn", Rv, 2 * HID, torch.bfloat16), add(p, "out", Rv, HID, torch.float32), mlp(p, Rv)
+        p = f"{i}.p2v"
+        add(p, "ln", Rp, 2 * HID, torch.bfloat16), add(p, "q", Rp, HID, torch.float32)
+        add(p, "ctx_ln", Rv, 2 * HID, torch.bfloat16), add(p, "kv", Rv, 2 * HID, torch.float32)
+        add(p, "attn", Rp, 2 * HID, torch.bfloat16), add(p, "out", Rp, HID, torch.float32), mlp(p, Rp)
+    assert len(links) == BODY_TRACE_LINKS
+    return links
+
+
+def body_trace_layout(T: int, N: int):
+    """ct3_body_trace_layout -> (offsets [97], bytes [97], total bytes)"""
+    off = (ctypes.c_int64 * BODY_TRACE_LINKS)()
+    nb = (ctypes.c_int64 * BODY_TRACE_LINKS)()
+    tot = ctypes.c_size_t(0)
+    _check(lib().ct3_body_trace_layout(T, N, off, nb, ctypes.byref(tot)), "ct3_body_trace_layout")
+    return list(off), list(nb), tot.value
+
+
+def body_trace(packed: torch.Tensor, tokens: torch.Tensor, coords: torch.Tensor, vis: torch.Tensor, conf: torch.Tensor,
+               workspace: Optional[torch.Tensor] = None, trace: Optional[torch.Tensor] = None) -> dict:
+    """ct3_body_trace: the point tokens [N*T, 384] fp32 through the update loop's transformer body and heads under this
+    thread's options; coords [T,N,2], vis and conf [T,N] are updated in place -> {link name: tensor} (body_trace_links),
+    views into the trace buffer.  trace: a uint8 buffer of at least the layout's total bytes (a caller may prefill it;
+    bytes no link owns keep their value), None = a new one."""
+    for t, name in ((tokens, "tokens"), (coords, "coords"), (vis, "vis"), (conf, "conf")):
+        _req(t, torch.float32, name)
+    if coords.dim() != 3 or coords.shape[2] != 2:
+        raise EngineError(f"coords must be [T, N, 2], got {tuple(coords.shape)}")
+    T, N, _ = coords.shape
+    for t, name in ((vis, "vis"), (conf, "conf")):
+        if tuple(t.shape) != (T, N):
+            raise EngineError(f"{name} must be [{T}, {N}] like coords, got {tuple(t.shape)}")
+    if tokens.numel() != N * T * HID:
+        raise EngineError(f"tokens must be [{N * T}, {HID}]")
+    dev = coords.device
+    offs, nbytes, total = body_trace_layout(T, N)
+    if workspace is None:
+        workspace = torch.empty(workspace_bytes(T, N), dtype=torch.uint8, device=dev)
+    _req(workspace, torch.uint8, "workspace")
+    if trace is None:
+        trace = torch.empty(total, dtype=torch.uint8, device=dev)
+    _req(trace, torch.uint8, "trace")
+    _call("ct3_body_trace", dev, _ptr(packed), _ptr(tokens), T, N, _ptr(coords), _ptr(vis), _ptr(conf), _ptr(trace),
+          trace.numel(), _ptr(workspace), workspace.numel(), _stream(dev))
+    out = {}
+    for (name, dtype, shape), o, n in zip(body_trace_links(T, N), offs, nbytes):
+        if math.prod(shape) * dtype.itemsize != n:
+            raise EngineError(f"body trace link {name}: {n} bytes, expected {shape} {dtype}")
+        out[name] = trace[o:o + n].view(dtype).reshape(shape)
     return out
 
 

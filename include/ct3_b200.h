@@ -628,6 +628,32 @@ int ct3_split_rows_fp16(const float* x, int rows, int K, int Kpad, void* x_split
 int ct3_updateformer(const void* packed, const float* x, int T, int N, const int32_t* group_sizes_host, int G,
                      float* delta, void* workspace, size_t workspace_bytes, ct3_stream_t stream);
 
+/* The second half of one ct3_update_loop iteration (G = 1), run by the loop's own code under the thread's options,
+ * with a copy of every link's output taken right after the launch that writes it, for testing each link on its own
+ * input: the point tokens `tokens` fp32 [N*T, 384] (row n*T + t, as ct3_loop_tokens writes tokens_out) go through the
+ * transformer body, and the heads add their deltas to coords [T, N, 2], vis and conf [T, N] in place.
+ * workspace: ct3_workspace_bytes of the shape {T, N, 0, 0, G = 1}, 256-byte aligned.  trace: a 256-byte aligned device
+ * buffer of at least the total_bytes of ct3_body_trace_layout(T, N), which also gives each link's byte offset and
+ * size (CT3_BODY_TRACE_LINKS of each; offsets and bytes may be NULL).  Null pointers or a bad T / N return CT3_EINVAL
+ * (ct3_update_loop's messages) and a too small trace or workspace CT3_ENOSPC, before any launch.
+ * Rows: Rp = N*T point rows, Rv = 64*T virtual rows, R = Rp + Rv all of them (points first, then virtual token i at
+ * i*T + t).  "split" is bf16 [rows, 2*C] (hi C | lo C), "f32" fp32 [rows, C]; "tokens" the fp32 token rows [rows, 384]
+ * after the launch named.
+ *   virtual init     : tokens Rv
+ *   time block       : LayerNorm split R | q|k|v f32 R x 1152 (written by the unfused route only: with the fused
+ *                      kernel the link is left as it is) | attention split R | tokens after to_out R | MLP(R)
+ *   virtual <- point : LayerNorm split Rv | q f32 Rv x 384 | norm_context split Rp | k|v f32 Rp x 768 |
+ *                      attention split Rv | tokens after to_out Rv | MLP(Rv)
+ *   virtual self     : LayerNorm split Rv | q|k|v f32 Rv x 1152 | attention split Rv | tokens after to_out Rv | MLP(Rv)
+ *   point <- virtual : LayerNorm split Rp | q f32 Rp x 384 | norm_context split Rv | k|v f32 Rv x 768 |
+ *                      attention split Rp | tokens after to_out Rp | MLP(Rp)
+ *   MLP(rows)        : LayerNorm split | fc1 + GELU split rows x 2*1536 | tokens after fc2
+ * in the order virtual init, then per block 0 .. 2: time, virtual <- point, virtual self, point <- virtual: 97 links. */
+#define CT3_BODY_TRACE_LINKS 97
+int ct3_body_trace_layout(int T, int N, int64_t* offsets, int64_t* bytes, size_t* total_bytes);
+int ct3_body_trace(const void* packed, const float* tokens, int T, int N, float* coords, float* vis, float* conf,
+                   void* trace, size_t trace_bytes, void* workspace, size_t workspace_bytes, ct3_stream_t stream);
+
 /* One attention core  out = softmax(q k^T * 48^-1/2) v  per head (8 x 48; Attention.forward, blocks.py:391-397) of
  * the transformer body, chosen and launched exactly as ct3_updateformer does it under the calling thread's
  * "attn" option (time attention always takes the unfused path that T > 128 takes in the body).

@@ -2,7 +2,7 @@
 dispatch matrix of the transformer body and at sharp logits; and the whole EfficientUpdateFormer at sharp attention
 against the float64 oracle.
 
-The branch map at the top restates, in Python, how the host picks a kernel (attention_tc.cu: attention_tc_splits and
+The branch map (tests/body_cases.py) restates, in Python, how the host picks a kernel (attention_tc.cu: attention_tc_splits and
 launch_attention_tc; api_loop.cu: run_attention, space_attention, plan_groups).  A CPU test pins it to values computed by
 the C++; the GPU test prints the branch of every case and asserts that the case list reaches every branch on the
 device it runs on, so a change to the heuristics cannot silently drop one from coverage.
@@ -24,74 +24,11 @@ import zlib
 import pytest
 import torch
 
+from body_cases import C, DH, HEADS, KV, P_FROM_V, TIME, V_FROM_P, V_SELF, bound, branch, describe, tc_qtw, tc_splits
 from cases import O
 
 DEV = "cuda:0"
-WARPS, KV, HEADS, DH, C = 4, 64, 8, 48, 384
-MAX_SPLITS = 32
-TIME, V_FROM_P, V_SELF, P_FROM_V = 0, 1, 2, 3
 KIND_NAMES = {TIME: "time", V_FROM_P: "virtual<-point", V_SELF: "virtual self", P_FROM_V: "point<-virtual"}
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# branch map
-def tc_splits(num_seq, Lq, Lk, sms):
-    """attention_tc_splits: split-K count of a shared-K/V launch (mma.sync kernel)."""
-    q_tiles = (Lq + 15) // 16
-    ctas = num_seq * HEADS * ((q_tiles + WARPS - 1) // WARPS)
-    chunks = (Lk + 63) // 64
-    splits = 1
-    if ctas < 2 * sms and chunks >= 8:
-        slots, best = 4 * sms, -1
-        for sp in range(1, min(MAX_SPLITS, chunks // 2) + 1):
-            cost = ((ctas * sp + slots - 1) // slots) * ((chunks + sp - 1) // sp)
-            if best < 0 or cost < best:
-                best, splits = cost, sp
-    return splits
-
-
-def tc_qtw(num_seq, Lq, Lk, sms):
-    """launch_attention_tc without split-K: query tiles per warp when K/V fit one chunk."""
-    q_tiles = (Lq + 15) // 16
-    qtw = 1
-    if (Lk + 63) // 64 == 1:
-        while qtw < 8 and num_seq * HEADS * ((q_tiles + WARPS * 2 * qtw - 1) // (WARPS * 2 * qtw)) >= 4 * sms:
-            qtw *= 2
-    return qtw
-
-
-def branch(kind, T, N, sizes, attn, sms):
-    """What ct3_attention runs for this call: a dict of the branch's features."""
-    sizes = list(sizes) if sizes is not None else [N]
-    G = len(sizes)
-    if attn == 1:
-        return {"path": "simt"}
-    if kind == TIME:   # run_attention(per_warp): every track, KB by the key count
-        return {"path": "per_warp", "kb": 16 if T <= 16 else 32 if T <= 32 else 64, "T": T}
-    if G == 1:
-        if kind == P_FROM_V and N > KV:
-            return {"path": "wgmma"}
-        Lq, Lk = {V_FROM_P: (KV, N), V_SELF: (KV, KV), P_FROM_V: (N, KV)}[kind]
-        s = tc_splits(T, Lq, Lk, sms)
-        if s > 1:
-            return {"path": "split_k", "splits": s}
-        return {"path": "shared", "qtw": tc_qtw(T, Lq, Lk, sms)}
-    if kind == V_FROM_P:   # per-group split-K counts (plan_groups), one launch
-        splits = [tc_splits(T, KV, n, sms) for n in sizes]
-        if max(splits) > 1:
-            return {"path": "grouped_split_k", "group_splits": splits}
-        return {"path": "grouped", "qtw": tc_qtw(T * G, KV, max(sizes), sms)}
-    if kind == V_SELF:
-        return {"path": "grouped", "qtw": tc_qtw(T * G, KV, KV, sms)}
-    small = [n for n in sizes if n <= KV]   # point <- virtual: groups of > 64 tracks on wgmma tiles, the rest mma.sync
-    out = {"path": "grouped_p2v", "wgmma_groups": G - len(small), "mma_groups": len(small)}
-    if small:
-        out["qtw"] = tc_qtw(T * len(small), KV, KV, sms)
-    return out
-
-
-def describe(b):
-    return " ".join(f"{k}={v}" for k, v in b.items())
 
 
 def coverage(branches):
@@ -203,12 +140,6 @@ def reference(kind, q, kv, T, N, sizes):
         stats.append((qr, labs, float(V.abs().max()), K.shape[1], float(logits.abs().max())))
         del logits
     return want, stats
-
-
-def bound(attn, labs, vmax, lk):
-    if attn == 1:
-        return (2.0 ** -17 + 4 * 2.0 ** -24 * (math.sqrt(DH) * (1 + labs) + math.sqrt(lk))) * vmax
-    return 2 * (1 + labs) * 2.0 ** -16 * vmax
 
 
 # ---------------------------------------------------------------------------------------------------------------------

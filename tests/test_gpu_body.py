@@ -50,9 +50,9 @@ import zlib
 import pytest
 import torch
 
+from body_cases import C, DH, HEADS, acc_bound, ln_ref, planes, qkv64, round16, time_reference
+
 DEV = "cuda:0"
-C, HEADS, DH, KV = 384, 8, 48, 64
-U = 2.0 ** -24
 BF16_SENTINEL = 0x7FA5                 # a bf16 NaN: no kernel writes it
 F32_SENTINEL = 0x7FC0ABCD              # an fp32 NaN
 
@@ -61,32 +61,12 @@ def pad64(k):
     return (k + 63) // 64 * 64
 
 
-def round16(w):
-    """w rounded to 16 significant bits: exactly bf16 hi + bf16 lo, so that packing it adds no error"""
-    m, e = torch.frexp(w.double())
-    return torch.ldexp(torch.round(m * 65536.0) / 65536.0, e)
-
-
-def planes(v, fp16=False):
-    """float64 values -> (hi, lo) 16-bit planes (bf16 or fp16)"""
-    dt = torch.float16 if fp16 else torch.bfloat16
-    hi = v.to(dt)
-    return hi, (v - hi.double()).to(dt)
-
-
 def assert_well_formed(hi, lo, what):
     """|lo| <= ulp_bf16(hi) / 2 elementwise (hi = m 2^e with m in [0.5, 1): ulp = 2^(e-8)); lo = 0 where hi = 0"""
     h, l = hi.double(), lo.double()
     _, e = torch.frexp(h)
     ok = torch.where(h == 0, l == 0, l.abs() <= torch.ldexp(torch.ones_like(h), e - 9))
     assert bool(ok.all()), f"{what}: {int((~ok).sum())} split elements with |lo| > ulp(hi) / 2"
-
-
-def acc_bound(impl, products, Kpad):
-    """accumulation error per unit of S (module docstring)"""
-    if impl == 1:
-        return 2 * Kpad * U
-    return (products * Kpad // 16 + 1) * 2 * U
 
 
 def sms():
@@ -365,13 +345,6 @@ def base_state():
     return seeded_state_dict(17, offline=True, window_len=60)
 
 
-def qkv64(x, wq, bq, wkv, bkv):
-    """float64 q, k, v [rows, 384] and their elementwise magnitudes S = |x| |w|^T"""
-    q, kv = x @ wq.t() + bq, x @ wkv.t() + bkv
-    sq, skv = x.abs() @ wq.abs().t(), x.abs() @ wkv.abs().t()
-    return q, kv[:, :C], kv[:, C:], sq, skv[:, :C], skv[:, C:]
-
-
 def time_inputs(T, n, regime, g):
     """-> the crafted split operand x_split [rows, 768] and float64 weights exact to 16 bits (wq [384, 384], bq,
     wkv [768, 384], bkv) of the regime"""
@@ -409,43 +382,6 @@ def time_inputs(T, n, regime, g):
         wq, bq = wq * s, bq * s
     wq, bq, wkv, bkv = (round16(w).float().double() for w in (wq, bq, wkv, bkv))
     return torch.cat([xh, xl], 1).contiguous(), wq, bq, wkv, bkv
-
-
-def time_reference(x_split, wq, bq, wkv, bkv, T, n, fused, impl, chunk=256):
-    """-> (want [rows, 384] float64, bound [rows, 384], max |logit|)"""
-    x = x_split[:, :C].double() + x_split[:, C:].double()
-    q, k, v, sq, sk, sv = qkv64(x, wq, bq, wkv, bkv)
-    if impl == 0:   # the dropped lo*lo products, from the planes (the weights split exactly, see round16)
-        xl = x_split[:, C:].double().abs()
-        lq, lkv = xl @ planes(wq)[1].double().abs().t(), xl @ planes(wkv)[1].double().abs().t()
-    else:
-        lq, lkv = torch.zeros_like(q), torch.zeros(q.shape[0], 2 * C, device=q.device, dtype=q.dtype)
-    c_acc = acc_bound(impl, 3, C)
-
-    def gemm_err(val, lolo, s, b):
-        return lolo + c_acc * s + 2 * U * (val.abs() + b.abs())
-    dq, dk, dv = (gemm_err(q, lq, sq, bq), gemm_err(k, lkv[:, :C], sk, bkv[:C]),
-                  gemm_err(v, lkv[:, C:], sv, bkv[C:]))
-    want = torch.empty_like(q)
-    bound = torch.empty_like(q)
-    lmax = 0.0
-    for n0 in range(0, n, chunk):
-        r = slice(n0 * T, min(n, n0 + chunk) * T)
-        Q, K, V, DQ, DK, DV = (t[r].view(-1, T, HEADS, DH) for t in (q, k, v, dq, dk, dv))
-        s = torch.einsum("nihd,njhd->nhij", Q, K) / math.sqrt(DH)
-        qk = torch.einsum("nihd,njhd->nhij", Q.abs(), K.abs()) / math.sqrt(DH)
-        ds = (torch.einsum("nihd,njhd->nhij", DQ, K.abs()) + torch.einsum("nihd,njhd->nhij", Q.abs(), DK)
-              + torch.einsum("nihd,njhd->nhij", DQ, DK)) / math.sqrt(DH) + 48 * U * qk + 2.0 ** -22 * s.abs()
-        o = torch.einsum("nhij,njhd->nihd", torch.softmax(s, dim=-1), V)
-        D = ds.amax(dim=(2, 3))                                        # [n, h]
-        vmax = V.abs().amax(dim=(1, 3))
-        b = torch.expm1(2 * D) * vmax + DV.amax(dim=(1, 3)) + (T + 16) * 2 * U * vmax
-        if not fused:
-            b = b + 2 * (1 + qk.amax(dim=(2, 3))) * 2.0 ** -16 * vmax
-        want[r] = o.reshape(-1, C)
-        bound[r] = (b[:, None, :, None] + 2.0 ** -17 * o.abs()).reshape(-1, C)
-        lmax = max(lmax, float(s.abs().max()))
-    return want, bound, lmax
 
 
 @pytest.mark.gpu
@@ -508,16 +444,7 @@ def test_layernorm_matches_fp64(eng, rows, eps, affine):
     hi, lo = out[:, :C], out[:, C:]
     assert_well_formed(hi, lo, "layernorm")
     got = hi.double() + lo.double()
-    x64 = x.double()
-    mean = x64.mean(1, keepdim=True)
-    eps32 = float(torch.tensor(eps, dtype=torch.float32))   # the eps the kernel adds
-    sigma = (x64.var(1, unbiased=False, keepdim=True) + eps32).sqrt()
-    z = (x64 - mean) / sigma
-    gm = gamma.double() if affine else torch.ones(C, device=DEV, dtype=torch.float64)
-    bt = beta.double() if affine else torch.zeros(C, device=DEV, dtype=torch.float64)
-    want = z * gm + bt
-    A = x64.abs().mean(1, keepdim=True)
-    bd = gm.abs() * 2.0 ** -19 * (z.abs() + A / sigma) + 2.0 ** -22 * bt.abs() + 2.0 ** -17 * want.abs()
+    want, bd = ln_ref(x.double(), eps, gamma.double() if affine else None, beta.double() if affine else None)
     err = (got - want).abs()
     ratio = err / bd
     kind = torch.arange(rows, device=DEV) % len(ROW_KINDS)
