@@ -3,7 +3,7 @@ reference's `cotracker.predictor` API.  See DESIGN.md and include/ct3_b200.h."""
 from .build import build_cotracker  # noqa: F401
 from .corners import detect_corners  # noqa: F401
 from .ingest import YUVClip  # noqa: F401
-from .predictor import CoTrackerOnlinePredictor, CoTrackerPredictor, TrackScores  # noqa: F401
+from .predictor import CoTrackerOnlinePredictor, CoTrackerPredictor, EncodedClip, TrackScores  # noqa: F401
 from .streams import OnlineStreams  # noqa: F401
 
 __version__ = "0.1.0"

@@ -123,6 +123,7 @@ def detect_corners(video, max_corners: int, *, frame: int = 0, quality_level: fl
     list-of-queries form CoTrackerPredictor takes).  Runs on the video's device, or the current CUDA device for a host
     video; only the B corner counts are copied to the host."""
     check_params(max_corners, quality_level, min_distance, block_size, exclude_radius)
+    ingest.reject_encoded_clip(video, "detect_corners")
     if not (isinstance(video, ingest.YUVClip) or torch.is_tensor(video)) or video.dim() != 5 or video.shape[2] != 3:
         raise ValueError(f"video must be [B,T,3,H,W] or a YUVClip, got {getattr(video, 'shape', type(video))}")
     B, T, _, H, W = video.shape

@@ -176,6 +176,13 @@ int ct3_prepare_pyramid(const float* fmaps, int T, int H4, int W4, float* pyr, c
   return 0;
 }
 
+int ct3_pyramid_pools(int T, int H4, int W4, float* pyr, ct3_stream_t stream) {
+  if (!pyr) return fail(CT3_EINVAL, "null argument%s");
+  if (int rc = check_pyramid(T, H4, W4)) return rc;
+  CK(launch_pyramid_pools(T, H4, W4, pyr, (cudaStream_t)stream), "pyramid_pools");
+  return 0;
+}
+
 int ct3_sample_support(const float* pyr, int T, int H4, int W4, const int32_t* queried_frames,
                        const float* queried_coords, int N, const uint8_t* accumulate_mask, float* support,
                        ct3_stream_t stream) {

@@ -83,6 +83,7 @@ def _signatures():
         "ct3_pack_weights": (c_int, [ctypes.POINTER(c_void_p), c_int, c_void_p, c_size_t, c_void_p]),
         "ct3_pyramid_layout": (c_int, [c_int, c_int, c_int, i64p, intp, intp, i64p]),
         "ct3_prepare_pyramid": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+        "ct3_pyramid_pools": (c_int, [c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_prepare_frames": (c_int, [c_void_p, c_int, c_int, c_int, c_int, i64, i64, i64, i64, c_int, c_int, c_void_p,
                                        c_void_p]),
         "ct3_prepare_frames_yuv": (c_int, [c_void_p, c_int, c_int, c_int, c_int, i64, i64, c_int, c_int, c_void_p,
@@ -297,6 +298,17 @@ def prepare_pyramid(fmaps: torch.Tensor) -> torch.Tensor:
     *_, total = pyramid_layout(T, H4, W4)
     pyr = torch.empty(total, dtype=torch.float32, device=fmaps.device)
     _call("ct3_prepare_pyramid", fmaps.device, _ptr(fmaps), T, H4, W4, _ptr(pyr), _stream(fmaps.device))
+    return pyr
+
+
+def pyramid_pools(pyr: torch.Tensor, T: int, H4: int, W4: int) -> torch.Tensor:
+    """In place: levels 1-3 of the flat T-frame pyramid `pyr` recomputed from its level 0 with the encoder's own
+    average pools (ct3_pyramid_pools), bit-identical to the levels the encoder wrote.  -> pyr"""
+    _req(pyr, torch.float32, "pyr")
+    *_, total = pyramid_layout(T, H4, W4)
+    if pyr.numel() != total:
+        raise EngineError(f"pyr holds {pyr.numel()} floats, a {T}-frame {H4}x{W4} pyramid {total}")
+    _call("ct3_pyramid_pools", pyr.device, T, H4, W4, _ptr(pyr), _stream(pyr.device))
     return pyr
 
 

@@ -255,6 +255,7 @@ class EvaluationPredictor(torch.nn.Module):
     @torch.no_grad()
     def forward(self, video, queries):
         from . import ingest
+        ingest.reject_encoded_clip(video, "EvaluationPredictor")
         B, T, C, H, W = video.shape
         assert queries.shape[0] == 1 and queries.shape[2] == 3 and B == 1
         N = queries.shape[1]

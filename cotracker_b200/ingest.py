@@ -135,6 +135,15 @@ class YUVClip:
         return f"YUVClip({self.layout}{colour}, shape={tuple(self.shape)}, device={self.device})"
 
 
+def reject_encoded_clip(video, where: str):
+    """TypeError when `video` is an `EncodedClip`: `where` takes pixels, and only CoTrackerPredictor takes a clip
+    encoded already."""
+    from .predictor import EncodedClip   # predictor imports this module
+    if isinstance(video, EncodedClip):
+        raise TypeError(f"{where} takes the video's pixels, not an EncodedClip (only CoTrackerPredictor calls take an "
+                        "encoded clip)")
+
+
 def model_device(model: torch.nn.Module) -> torch.device:
     p = next(model.parameters(), None)
     return p.device if p is not None else torch.device("cpu")

@@ -21,10 +21,17 @@ list call).  They pass the same backward merge, support-grid drop and frame sele
 predictor's visibility is `scores.visibility > 0.9` except at the query points, which it pins to True while the scores
 keep the model's values there; the online predictor's is `scores.visibility * scores.confidence > 0.6`, bit for bit.
 Tracks and visibility are the same with and without the flag.
+
+`CoTrackerPredictor.encode(video)` resizes and encodes a clip once and returns an `EncodedClip`, which the offline
+predictor takes wherever it takes a video, in every mode and any number of times: `predictor(predictor.encode(video),
+**kw)` is `torch.equal` to `predictor(video, **kw)`, because a direct call is that same encode followed by the same
+tracking path.  `clip.to("cpu")` parks an idle clip in pinned host memory and `clip.to(device)` brings it back
+bit-identical.
 """
 from __future__ import annotations
 
-from typing import NamedTuple
+import copy
+from typing import NamedTuple, Optional
 
 import torch
 import torch.nn.functional as F
@@ -93,20 +100,61 @@ class CoTrackerPredictor(torch.nn.Module):
     @torch.no_grad()
     def forward(self, video, queries: torch.Tensor = None, segm_mask: torch.Tensor = None, grid_size: int = 0,
                 grid_query_frame: int = 0, backward_tracking: bool = False, return_scores: bool = False):
-        """-> (tracks, visibility), or with return_scores=True (tracks, visibility, TrackScores) (module docstring)."""
+        """-> (tracks, visibility), or with return_scores=True (tracks, visibility, TrackScores) (module docstring).
+        video may be an `EncodedClip` of `encode`; the call then neither uploads nor encodes, and leaves the clip as it
+        was."""
         _check_return_scores(return_scores)
         if isinstance(video, (list, tuple)):
             return self._track_list(list(video), queries, segm_mask, grid_size, grid_query_frame, backward_tracking,
                                     return_scores)
-        if segm_mask is not None and video.shape[0] != 1:
+        encoded = isinstance(video, EncodedClip)
+        if encoded:
+            video = self._check_clip(video)
+        if segm_mask is not None and (video.B if encoded else video.shape[0]) != 1:
             raise ValueError("segm_mask keeps a different number of grid points per clip: it needs B == 1")
+        # a direct call is `encode` without the weights' fingerprint, which only a clip that outlives the call needs
+        clip = video if encoded else EncodedClip(self.model, video, self.interp_shape)
         if queries is None and grid_size == 0:
-            return self._compute_dense_tracks(video, grid_query_frame=grid_query_frame,
+            return self._compute_dense_tracks(clip, grid_query_frame=grid_query_frame,
                                               backward_tracking=backward_tracking, return_scores=return_scores)
-        return self._compute_sparse_tracks(video, queries, segm_mask, grid_size,
+        return self._compute_sparse_tracks(clip, queries, segm_mask, grid_size,
                                            add_support_grid=(grid_size == 0 or segm_mask is not None),
                                            grid_query_frame=grid_query_frame, backward_tracking=backward_tracking,
                                            return_scores=return_scores)
+
+    @torch.no_grad()
+    def encode(self, video) -> "EncodedClip":
+        """video ([B,T,3,H,W] uint8 or float, host or device, any strides, or a `YUVClip`: anything one call takes)
+        -> its `EncodedClip`: resized, normalised and encoded once, on the model's device, for any number of calls."""
+        if isinstance(video, (list, tuple, EncodedClip)):
+            raise TypeError(f"encode takes one clip [B,T,3,H,W] or a YUVClip, got {type(video).__name__} (list calls "
+                            "take pixels; an EncodedClip is encoded already)")
+        return EncodedClip(self.model, video, self.interp_shape, weights=self.model.weights_fingerprint())
+
+    def _check_clip(self, clip: "EncodedClip") -> "EncodedClip":
+        """The ValueErrors of an EncodedClip this predictor cannot track, raised before any work.  -> the clip, bound
+        to this predictor's model (a shallow copy sharing the pyramid when another predictor's model encoded it)."""
+        if clip.parked:
+            raise ValueError("the EncodedClip is parked on the host: bring it back with clip.to(device) first")
+        if tuple(clip.interp_shape) != tuple(self.interp_shape):
+            raise ValueError(f"the EncodedClip was encoded at interp_shape {tuple(clip.interp_shape)}, this predictor "
+                             f"tracks at {tuple(self.interp_shape)}")
+        if clip.stride != self.model.stride:
+            raise ValueError(f"the EncodedClip was encoded at stride {clip.stride}, this predictor's model has stride "
+                             f"{self.model.stride}")
+        if clip.loop != _loop(self.model):
+            raise ValueError(f"the EncodedClip was encoded for the {clip.loop} model, this predictor runs the "
+                             f"{_loop(self.model)} model")
+        dev = ingest.model_device(self.model)
+        if clip.device != dev:
+            raise ValueError(f"the EncodedClip is on {clip.device}, the predictor's model on {dev}: move one of them")
+        if clip.weights != self.model.weights_fingerprint():
+            raise ValueError("the EncodedClip was encoded with other weights than the predictor's model has now "
+                             "(weights_fingerprint differs): encode the video again")
+        if clip.model is not self.model:
+            clip = copy.copy(clip)
+            clip.model = self.model
+        return clip
 
     def _track_list(self, clips, queries, segm_mask, grid_size, grid_query_frame, backward_tracking,
                     return_scores=False):
@@ -144,7 +192,7 @@ class CoTrackerPredictor(torch.nn.Module):
                                     sum(lengths), RAGGED_PAD_ROWS)
         outs = [None] * B
         for p in passes:
-            res = self.model._track_ragged(pyr, ih, iw, [g for b in p for g in groups[b]], _EncodedClip.ITERS,
+            res = self.model._track_ragged(pyr, ih, iw, [g for b in p for g in groups[b]], EncodedClip.ITERS,
                                            scores=return_scores)
             for b in p:
                 outs[b], res = res[:len(groups[b])], res[len(groups[b]):]
@@ -152,25 +200,24 @@ class CoTrackerPredictor(torch.nn.Module):
                             return_scores) for b in range(B)]
         return tuple(list(r) for r in zip(*res))
 
-    def _compute_dense_tracks(self, video, grid_query_frame, grid_size=80, backward_tracking=False,
+    def _compute_dense_tracks(self, clip, grid_query_frame, grid_size=80, backward_tracking=False,
                               return_scores=False):
         """grid_step^2 shifted grids, one query group per offset (and one reversed group per offset with backward
-        tracking), tracked in as few grouped passes over one encoded clip as fit in device memory."""
-        *_, H, W = video.shape
+        tracking), tracked in as few grouped passes over the one EncodedClip as fit in device memory."""
+        H, W = clip.input_hw
         grid_step = W // grid_size
         gw, gh = W // grid_step, H // grid_step
-        clip = _EncodedClip(self.model, video, self.interp_shape)   # one resize + encoder pass for every offset
         dev = clip.device
         n_off = grid_step * grid_step
         base_x = (torch.arange(gw, device=dev).repeat(gh) * grid_step).float()
         base_y = (torch.arange(gh, device=dev).repeat_interleave(gw) * grid_step).float()
         queries = []
         for offset in range(n_off):
-            pts = torch.zeros((video.shape[0], gw * gh, 3), device=dev)
+            pts = torch.zeros((clip.B, gw * gh, 3), device=dev)
             pts[:, :, 0] = grid_query_frame
             pts[:, :, 1] = base_x + offset % grid_step
             pts[:, :, 2] = base_y + offset // grid_step
-            queries.append(self._model_queries(clip, video.shape, pts))
+            queries.append(self._model_queries(clip, clip.video_shape, pts))
         per = 2 if backward_tracking else 1
         groups = [g for q in queries for g in ([q, _reversed_queries(q, clip.T)] if backward_tracking else [q])]
         _, passes = plan_dense_passes(n_off, gw * gh, backward_tracking, *clip.pass_shape(backward_tracking))
@@ -183,7 +230,7 @@ class CoTrackerPredictor(torch.nn.Module):
         tracks = visibilities = probs = None
         for i in range(n_off):
             step = self._finish(queries[i], outs[per * i], outs[per * i + 1] if backward_tracking else None,
-                                video.shape, scores=return_scores)
+                                clip.video_shape, scores=return_scores)
             t_step, v_step = step[:2]
             tracks = t_step if tracks is None else torch.cat([tracks, t_step], dim=2)
             visibilities = v_step if visibilities is None else torch.cat([visibilities, v_step], dim=2)
@@ -192,10 +239,9 @@ class CoTrackerPredictor(torch.nn.Module):
                                                                     for a, b in zip(probs, step[2])))
         return (tracks, visibilities, probs) if return_scores else (tracks, visibilities)
 
-    def _compute_sparse_tracks(self, video, queries, segm_mask=None, grid_size=0, add_support_grid=False,
+    def _compute_sparse_tracks(self, clip, queries, segm_mask=None, grid_size=0, add_support_grid=False,
                                grid_query_frame=0, backward_tracking=False, return_scores=False):
-        clip = _EncodedClip(self.model, video, self.interp_shape)
-        return self._sparse_tracks(clip, video.shape, queries, segm_mask, grid_size, add_support_grid,
+        return self._sparse_tracks(clip, clip.video_shape, queries, segm_mask, grid_size, add_support_grid,
                                    grid_query_frame, backward_tracking, return_scores)
 
     def _sparse_tracks(self, clip, video_shape, queries, segm_mask=None, grid_size=0, add_support_grid=False,
@@ -254,7 +300,7 @@ class CoTrackerPredictor(torch.nn.Module):
 
 
 class _Device:
-    """The device of a list call's clips, where `_model_queries` takes an `_EncodedClip`."""
+    """The device of a list call's clips, where `_model_queries` takes an `EncodedClip`."""
 
     def __init__(self, device):
         self.device = device
@@ -271,6 +317,7 @@ def _check_list_call(model, clips, queries, segm_mask, grid_size, grid_query_fra
         if lst is not None and (not isinstance(lst, (list, tuple)) or len(lst) != B):
             raise ValueError(f"{name} must be a list of {B} entries, one per clip")
     for b, c in enumerate(clips):
+        ingest.reject_encoded_clip(c, f"entry {b} of a list call")
         clip = torch.is_tensor(c) or isinstance(c, ingest.YUVClip)
         if not clip or c.dim() != 5 or c.shape[0] != 1 or c.shape[1] < 1 or c.shape[2] != 3:
             raise ValueError(f"clip {b} must be a [1,T,3,H,W] tensor, got "
@@ -299,22 +346,111 @@ def _reversed_queries(queries, T: int):
     return inv
 
 
-class _EncodedClip:
-    """One predictor call's clips (a batch of B), resized + normalised (cotracker_b200.ingest) and encoded once into
-    one pyramid; every model pass of the call (dense offsets, backward tracking, the sub-batches of a batch that does
-    not fit in device memory at once) runs on this one pyramid.  A pass on the clip played backwards is a
-    reversed query group (model `reversed_groups`): it reads the forward pyramid through a frame map, so device memory
-    never holds a second pyramid and the pyramid is never reversed."""
+def _loop(model) -> str:
+    """How a model runs the update loop over a clip, which decides the padding frames its pyramid holds."""
+    if hasattr(model, "init_video_online_processing"):
+        return f"sliding-window (window_len {model.window_len})"
+    return "one-window"
+
+
+class EncodedClip:
+    """Clips (a batch of B) resized + normalised (cotracker_b200.ingest) and encoded once into one pyramid, made by
+    `CoTrackerPredictor.encode` (and by every direct predictor call, for that call).  Every model pass of a call
+    (dense offsets, backward tracking, the sub-batches of a batch that does not fit in device memory at once) runs on
+    this one pyramid, and no pass writes to it, so one clip serves any number of calls.  A pass on the clip played
+    backwards is a reversed query group (model `reversed_groups`): it reads the forward pyramid through a frame map, so
+    device memory never holds a second pyramid and the pyramid is never reversed.
+
+    It records what a call needs to scale queries and results and to check that a predictor may track it: `B`, `T`,
+    the input frame size `input_hw` (`video_shape` = (B, T, 3, H, W)), the model resolution `interp_shape` (= `H`,
+    `W`), the model's `stride` and update `loop`, its `device` and `weights`, the `weights_fingerprint()` of the model
+    that encoded it.  `nbytes` is the device memory it holds.
+
+    `to("cpu")` parks it in pinned host memory and frees its device memory; `to(device)` brings it back.  Levels 1-3 of
+    the pyramid are 2x2 average pools of level 0, so only level 0 is parked (`host`, [B, T', H/s, W/s, 128] fp32, 6.3 of
+    the 8.4 MB of a 384x512 frame), and the sliding-window model's padding frames are left out when they are copies of
+    each clip's last frame.  On return the padding is copied again and `ct3_pyramid_pools` recomputes levels 1-3 with
+    the kernel the encoder ran, so the pyramid is bit-identical to the one parked.  Each direction is one DMA per clip
+    straight between the device pyramid and the pinned park: no staging buffer, and no pinned memory beyond the parked
+    level 0 itself."""
 
     ITERS = 6
 
-    def __init__(self, model, video, interp_shape):
+    def __init__(self, model, video, interp_shape, weights: Optional[str] = None):
         frames = ingest.prepare_video(video, interp_shape, ingest.model_device(model))
-        self.model, self.device = model, frames.device
+        self.model, self.device, self.weights = model, frames.device, weights
+        self.video_shape = torch.Size(video.shape)
         self.B = video.shape[0]
         BT, _, self.H, self.W = frames.shape
         self.T = BT // self.B
+        self.interp_shape = (self.H, self.W)
+        self.stride, self.loop, self.pad = model.stride, _loop(model), model._clip_pad(self.T)
+        self.host = None
         self.pyr = model._encode_clip(frames, B=self.B)
+
+    @property
+    def input_hw(self):
+        return tuple(self.video_shape[3:])
+
+    @property
+    def parked(self) -> bool:
+        return self.pyr is None
+
+    @property
+    def nbytes(self) -> int:
+        return 0 if self.pyr is None else self.pyr.numel() * self.pyr.element_size()
+
+    def __repr__(self) -> str:
+        where = "parked on the host" if self.parked else f"device={self.device}"
+        return f"EncodedClip(video_shape={tuple(self.video_shape)}, interp_shape={self.interp_shape}, {where})"
+
+    def to(self, device) -> "EncodedClip":
+        """In place: park the clip on the host ("cpu") or bring it (back) to a CUDA device.  -> the clip."""
+        device = torch.device(device)
+        if device.type == "cuda" and device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        if device.type == "cpu":
+            if not self.parked:
+                self._park()
+        elif device.type != "cuda":
+            raise ValueError(f"an EncodedClip lives on a CUDA device or parked on the host (\"cpu\"), not {device}")
+        elif self.parked:
+            self._unpark(device)
+        elif device != self.device:
+            self.pyr, self.device = self.pyr.to(device), device
+        return self
+
+    def _level0(self, pyr) -> torch.Tensor:
+        """[B, T + pad, H/s * W/s * 128] view of level 0 of `pyr`, the first level of the flat layout."""
+        s = self.stride
+        n = (self.H // s) * (self.W // s) * engine.LATENT
+        return pyr[:self.B * (self.T + self.pad) * n].view(self.B, self.T + self.pad, n)
+
+    def _park(self):
+        lv0 = self._level0(self.pyr)
+        keep = self.T + self.pad
+        if self.pad and torch.equal(lv0[:, self.T:], lv0[:, self.T - 1:self.T].expand(-1, self.pad, -1)):
+            keep = self.T   # the padding is copies of each clip's last frame: remade on return
+        s = self.stride
+        host = torch.empty((self.B, keep, self.H // s, self.W // s, engine.LATENT), dtype=lv0.dtype, pin_memory=True)
+        with torch.cuda.device(self.device):
+            for b in range(self.B):
+                host[b].view(keep, -1).copy_(lv0[b, :keep], non_blocking=True)
+            torch.cuda.current_stream().synchronize()
+        self.host, self.pyr, self.device = host, None, torch.device("cpu")
+
+    def _unpark(self, device):
+        s, Tp, keep = self.stride, self.T + self.pad, self.host.shape[1]
+        H4, W4 = self.H // s, self.W // s
+        with torch.cuda.device(device):
+            pyr = torch.empty(engine.pyramid_layout(self.B * Tp, H4, W4)[3], dtype=self.host.dtype, device=device)
+            lv0 = self._level0(pyr)
+            for b in range(self.B):
+                lv0[b, :keep].copy_(self.host[b].view(keep, -1), non_blocking=True)
+            if keep < Tp:
+                lv0[:, keep:].copy_(lv0[:, keep - 1:keep].expand(-1, Tp - keep, -1))
+            engine.pyramid_pools(pyr, self.B * Tp, H4, W4)
+        self.pyr, self.host, self.device = pyr, None, device
 
     def track_groups(self, groups, reversed_groups, scores=False):
         """Query groups [B,n_g,3] (model resolution) of every clip in one pass, or, when the batch does not fit in
@@ -364,6 +500,9 @@ class _EncodedClip:
         return self.loop_frames(), self.H // s, self.W // s, budget, self.pass_frames(backward)
 
 
+_EncodedClip = EncodedClip   # its name while it lived inside one call, kept for code that imports it
+
+
 class CoTrackerOnlinePredictor(torch.nn.Module):
     def __init__(self, checkpoint="./checkpoints/scaled_online.pth", offline=False, v2=False, window_len=16):
         super().__init__()
@@ -384,6 +523,7 @@ class CoTrackerOnlinePredictor(torch.nn.Module):
         first step, with grid_size): track only the grid points inside it, selected as the offline predictor selects
         them; add_support_grid then appends the support grid as it does to queries."""
         _check_return_scores(return_scores)
+        ingest.reject_encoded_clip(video_chunk, "CoTrackerOnlinePredictor")
         B, T, C, H, W = video_chunk.shape
         dev = ingest.model_device(self.model)
         if is_first_step:

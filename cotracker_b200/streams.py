@@ -235,6 +235,7 @@ class OnlineStreams:
         stream as it was before this push: length, window start, track ids, history and support are unchanged, a short
         chunk does not end the stream, and no chunk stays pending.  Track edits made before the step are seen by it and
         stay.  A preview's frames after length - (window_len - step) are provisional, its newest ones the most."""
+        ingest.reject_encoded_clip(chunk, "OnlineStreams.push")
         s = self._get(sid)
         if not isinstance(preview, bool):
             raise ValueError(f"preview must be a bool, got {preview!r}")

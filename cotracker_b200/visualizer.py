@@ -25,7 +25,7 @@ from typing import Optional
 import numpy as np
 import torch
 
-from . import engine
+from . import engine, ingest
 
 
 def _get_cmap(name: str):
@@ -150,6 +150,7 @@ class Visualizer:
         compensate_for_camera_motion: bool = False,
         opacity: float = 1.0,
     ):
+        ingest.reject_encoded_clip(video, "Visualizer.visualize")
         if gt_tracks is not None:
             raise NotImplementedError("gt_tracks is not provided (the reference cannot draw more than one of them)")
         if compensate_for_camera_motion:
@@ -196,6 +197,7 @@ class Visualizer:
         color_alpha: int = 255,
     ):
         """video (B,T,3,H,W) as drawn on (already padded), tracks (B,T,N,2) in its pixel coordinates, segm_mask [N]."""
+        ingest.reject_encoded_clip(video, "Visualizer.draw_tracks_on_video")
         if gt_tracks is not None:
             raise NotImplementedError("gt_tracks is not provided (the reference cannot draw more than one of them)")
         B, T, C, H, W = video.shape

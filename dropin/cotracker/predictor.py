@@ -1,1 +1,1 @@
-from cotracker_b200.predictor import CoTrackerOnlinePredictor, CoTrackerPredictor, TrackScores  # noqa: F401
+from cotracker_b200.predictor import CoTrackerOnlinePredictor, CoTrackerPredictor, EncodedClip, TrackScores  # noqa: F401

@@ -419,6 +419,12 @@ int ct3_pyramid_layout(int T, int H4, int W4, int64_t level_off[4], int level_h[
                        int64_t* total_floats);
 int ct3_prepare_pyramid(const float* fmaps, int T, int H4, int W4, float* pyr, ct3_stream_t stream);
 
+/* ct3_pyramid_pools: in place, levels 1-3 of the T-frame pyramid `pyr` (ct3_pyramid_layout(T, H4, W4)) recomputed
+ * from its level 0 by the 2x2 average pools that ct3_encoder and ct3_prepare_pyramid end with (the same kernel and
+ * launches), so a pyramid whose level 0 was kept alone (e.g. parked on the host) comes back bit-identical.  Level 0
+ * is read only.  A null pyr or a bad pyramid shape returns CT3_EINVAL before any launch. */
+int ct3_pyramid_pools(int T, int H4, int W4, float* pyr, ct3_stream_t stream);
+
 /* ct3_sample_support: get_track_feat / sample_features5d
  * (cotracker3_online.py:113-128, model_utils.py:293-323) for all 4 levels.
  * queried_frames [N] int32 (already relative to the window, clamped into [0,T-1]),
