@@ -57,7 +57,7 @@ def params(max_corners, quality_level=0.01, min_distance=10, block_size=3, exclu
 
 
 def clip_frame(video, t: int):
-    """Frame t of every clip of `video` ([B,T,3,H,W] or a YUVClip), as a one-frame clip of the same kind."""
+    """Frame t of every clip of `video` ([B,T,3,H,W], a YUVClip or a Crop), as a one-frame clip of the same kind."""
     if isinstance(video, ingest.YUVClip):
         return video.with_data(video.data[:, t:t + 1])
     return video[:, t:t + 1]
@@ -112,8 +112,8 @@ def detect_corners(video, max_corners: int, *, frame: int = 0, quality_level: fl
                    block_size: int = 3, exclude=None, exclude_radius: float = 0, interp_shape=(384, 512), mask=None):
     """Shi-Tomasi corners of frame `frame` of each clip of `video`, as queries for the predictors.
 
-    video: anything `prepare_video` takes, [B,T,3,H,W] uint8 or float, host or device, or a `YUVClip`; only frame
-    `frame` of each clip is prepared (at interp_shape) and searched.  max_corners, quality_level, min_distance and
+    video: anything `prepare_video` takes, [B,T,3,H,W] uint8 or float, host or device, a `YUVClip` or a `Crop`; only
+    frame `frame` of each clip is prepared (at interp_shape) and searched.  max_corners, quality_level, min_distance and
     block_size are goodFeaturesToTrack's; min_distance is in model-resolution pixels.  exclude: points [B,E,2] or a
     list of B [E_b,2], (x, y) in frame pixels like queries; no corner lies closer than exclude_radius
     (model-resolution pixels) to one of its clip's points.  mask: None, or a region per clip [B,1,H,W] or one for
@@ -124,8 +124,9 @@ def detect_corners(video, max_corners: int, *, frame: int = 0, quality_level: fl
     video; only the B corner counts are copied to the host."""
     check_params(max_corners, quality_level, min_distance, block_size, exclude_radius)
     ingest.reject_encoded_clip(video, "detect_corners")
-    if not (isinstance(video, ingest.YUVClip) or torch.is_tensor(video)) or video.dim() != 5 or video.shape[2] != 3:
-        raise ValueError(f"video must be [B,T,3,H,W] or a YUVClip, got {getattr(video, 'shape', type(video))}")
+    if not (isinstance(video, (ingest.YUVClip, ingest.Crop)) or torch.is_tensor(video)) or video.dim() != 5 \
+            or video.shape[2] != 3:
+        raise ValueError(f"video must be [B,T,3,H,W], a YUVClip or a Crop, got {getattr(video, 'shape', type(video))}")
     B, T, _, H, W = video.shape
     if B < 1 or T < 1 or H < 2 or W < 2:
         raise ValueError(f"video must have B, T >= 1 and H, W >= 2, got {tuple(video.shape)}")

@@ -194,8 +194,10 @@ int ct3_sample_support(const float* pyr, int T, int H4, int W4, const int32_t* q
   return 0;
 }
 
-int ct3_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c,
-                       int64_t stride_h, int64_t stride_w, int out_h, int out_w, float* out, ct3_stream_t stream) {
+namespace {
+// the checks of ct3_prepare_frames and ct3_prepare_frames_crop
+int check_frames(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c, int64_t stride_h,
+                 int64_t stride_w, int out_h, int out_w, const float* out) {
   if (!src || !out) return fail(CT3_EINVAL, "null argument%s");
   if (T < 1 || H < 1 || W < 1 || out_h < 1 || out_w < 1) return fail(CT3_EINVAL, "T, H, W, out_h and out_w must be >= 1%s");
   if (dtype != CT3_FRAMES_U8 && dtype != CT3_FRAMES_F32) return fail(CT3_EINVAL, "unknown frame dtype%s");
@@ -204,8 +206,34 @@ int ct3_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t 
   // the kernel indexes the pixels of one output plane with int
   if ((int64_t)out_h * out_w > INT32_MAX) return fail(CT3_EINVAL, "output plane too large%s");
   if ((int64_t)out_h * out_w > INT64_MAX / 12 / T) return fail(CT3_EINVAL, "output too large%s");
-  CK(launch_prepare_frames(src, dtype, T, H, W, stride_t, stride_c, stride_h, stride_w, out_h, out_w, out,
-                           (cudaStream_t)stream), "prepare_frames");
+  return 0;
+}
+
+int check_window(const int32_t* offsets, int H, int W, int crop_h, int crop_w) {
+  if (!offsets) return fail(CT3_EINVAL, "null offsets%s");
+  if (crop_h < 1 || crop_h > H || crop_w < 1 || crop_w > W)
+    return fail(CT3_EINVAL, "crop_h and crop_w must lie in [1, H] and [1, W]%s");
+  return 0;
+}
+}  // namespace
+
+int ct3_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c,
+                       int64_t stride_h, int64_t stride_w, int out_h, int out_w, float* out, ct3_stream_t stream) {
+  if (int rc = check_frames(src, dtype, T, H, W, stride_t, stride_c, stride_h, stride_w, out_h, out_w, out)) return rc;
+  CK(launch_prepare_frames(src, dtype, T, H, W, stride_t, stride_c, stride_h, stride_w, nullptr, H, W, out_h, out_w,
+                           out, (cudaStream_t)stream),
+     "prepare_frames");
+  return 0;
+}
+
+int ct3_prepare_frames_crop(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c,
+                            int64_t stride_h, int64_t stride_w, const int32_t* offsets, int crop_h, int crop_w,
+                            int out_h, int out_w, float* out, ct3_stream_t stream) {
+  if (int rc = check_frames(src, dtype, T, H, W, stride_t, stride_c, stride_h, stride_w, out_h, out_w, out)) return rc;
+  if (int rc = check_window(offsets, H, W, crop_h, crop_w)) return rc;
+  CK(launch_prepare_frames(src, dtype, T, H, W, stride_t, stride_c, stride_h, stride_w, offsets, crop_h, crop_w, out_h,
+                           out_w, out, (cudaStream_t)stream),
+     "prepare_frames_crop");
   return 0;
 }
 
@@ -218,9 +246,10 @@ int ct3_prepare_frames_yuv(const uint8_t* src, int layout, int T, int H, int W, 
                                     stream);
 }
 
-int ct3_prepare_frames_yuv_fmt(const void* src, int layout, int matrix, int full_range, int T, int H, int W,
-                               int64_t stride_t, int64_t stride_row, int out_h, int out_w, float* out,
-                               ct3_stream_t stream) {
+namespace {
+// the checks of ct3_prepare_frames_yuv_fmt and ct3_prepare_frames_yuv_crop
+int check_frames_yuv(const void* src, int layout, int matrix, int full_range, int T, int H, int W, int64_t stride_t,
+                     int64_t stride_row, int out_h, int out_w, const float* out) {
   if (!src || !out) return fail(CT3_EINVAL, "null argument%s");
   const YuvFormat* f = yuv_format(layout);
   if (!f) return fail(CT3_EINVAL, "unknown YUV layout%s");
@@ -245,9 +274,30 @@ int ct3_prepare_frames_yuv_fmt(const void* src, int layout, int matrix, int full
   if (T > 1 && at > (INT64_MAX - frame) / (T - 1)) return fail(CT3_EINVAL, "stride extent overflows int64%s");
   if ((int64_t)out_h * out_w > INT32_MAX) return fail(CT3_EINVAL, "output plane too large%s");
   if ((int64_t)out_h * out_w > INT64_MAX / 12 / T) return fail(CT3_EINVAL, "output too large%s");
-  CK(launch_prepare_frames_yuv(src, layout, matrix, full_range, T, H, W, stride_t, stride_row, out_h, out_w, out,
-                               (cudaStream_t)stream),
+  return 0;
+}
+}  // namespace
+
+int ct3_prepare_frames_yuv_fmt(const void* src, int layout, int matrix, int full_range, int T, int H, int W,
+                               int64_t stride_t, int64_t stride_row, int out_h, int out_w, float* out,
+                               ct3_stream_t stream) {
+  if (int rc = check_frames_yuv(src, layout, matrix, full_range, T, H, W, stride_t, stride_row, out_h, out_w, out))
+    return rc;
+  CK(launch_prepare_frames_yuv(src, layout, matrix, full_range, T, H, W, stride_t, stride_row, nullptr, H, W, out_h,
+                               out_w, out, (cudaStream_t)stream),
      "prepare_frames_yuv");
+  return 0;
+}
+
+int ct3_prepare_frames_yuv_crop(const void* src, int layout, int matrix, int full_range, int T, int H, int W,
+                                int64_t stride_t, int64_t stride_row, const int32_t* offsets, int crop_h, int crop_w,
+                                int out_h, int out_w, float* out, ct3_stream_t stream) {
+  if (int rc = check_frames_yuv(src, layout, matrix, full_range, T, H, W, stride_t, stride_row, out_h, out_w, out))
+    return rc;
+  if (int rc = check_window(offsets, H, W, crop_h, crop_w)) return rc;
+  CK(launch_prepare_frames_yuv(src, layout, matrix, full_range, T, H, W, stride_t, stride_row, offsets, crop_h, crop_w,
+                               out_h, out_w, out, (cudaStream_t)stream),
+     "prepare_frames_yuv_crop");
   return 0;
 }
 

@@ -19,6 +19,11 @@
 // applies the integer conversion of ct3_prepare_frames_yuv_fmt (cv2's BT.601 constants by default).  The resize, copy
 // and normalisation are this one piece of code for all of them, so a YUV clip gives exactly the floats its uint8 RGB
 // conversion would.
+//
+// The kernel optionally reads a crop_h x crop_w window of each frame at a per-frame (top, left) from the device
+// (kCrop, ct3_prepare_frames_crop / ct3_prepare_frames_yuv_crop): the resize is that of a crop_h x crop_w frame and the
+// offset moves only the integer sample indices, so the output is the un-cropped kernel's on the materialised window.
+// Without kCrop the template makes exactly the code it made before windows existed.
 #include "../../include/ct3_b200.h"
 #include "kernels.cuh"
 
@@ -157,32 +162,62 @@ struct YuvFetch {
   }
 };
 
-template <class Fetch>
+// The window of a launch: frames H x W, resized from a window ch x cw whose top-left corner in frame t is
+// (offsets[2t], offsets[2t + 1]) (kCrop), or from the whole frame (ch = H, cw = W, no offsets).
+struct Geom {
+  int T, H, W, ch, cw, oh, ow;
+  const int32_t* offsets;   // device [T,2] (top, left), or null for the whole frame
+};
+
+// A window sample index: r + o, clamped into [0, n - 1] so that an offset the host did not check never reads outside
+// the frame (int64: o is any int32).
+__device__ __forceinline__ int clamp_index(int r, int o, int n) {
+  return (int)min(max((long long)r + o, 0ll), (long long)n - 1);
+}
+
+template <class Fetch, bool kCrop>
 __global__ void __launch_bounds__(kPrepThreads) prepare_frames_kernel(const typename Fetch::Src* __restrict__ src,
-                                                                      int64_t st, const Fetch fetch, int H, int W,
-                                                                      int oh, int ow, float rh, float rw, int copy,
-                                                                      float inv255, float* __restrict__ out) {
+                                                                      int64_t st, const Fetch fetch,
+                                                                      const int32_t* __restrict__ offsets, int H, int W,
+                                                                      int ch, int cw, int oh, int ow, float rh,
+                                                                      float rw, int copy, float inv255,
+                                                                      float* __restrict__ out) {
   const int64_t p = (int64_t)blockIdx.x * kPrepThreads + threadIdx.x;
   const int64_t plane = (int64_t)oh * ow;   // <= INT32_MAX (ct3_prepare_frames*), so y and x fit in int
   if (p >= plane) return;
   const int t = blockIdx.y;
   const int y = (int)(p / ow), x = (int)(p - (int64_t)y * ow);
   const typename Fetch::Src* f = src + (int64_t)t * st;
+  int top = 0, left = 0;
+  if constexpr (kCrop) {
+    top = __ldg(offsets + 2 * t);
+    left = __ldg(offsets + 2 * t + 1);
+  }
   float v[3];
   if (copy) {
-    fetch.pixel(f, y, x, v);
+    if constexpr (kCrop)
+      fetch.pixel(f, clamp_index(y, top, H), clamp_index(x, left, W), v);
+    else
+      fetch.pixel(f, y, x, v);
   } else {
+    // ATen's source indices of a ch x cw frame; the window's offset moves the integer samples only
     const float h1r = __fmul_rn(rh, (float)y);
     const int h1 = (int)h1r;
-    const int h1p = h1 < H - 1 ? 1 : 0;
+    const int h1p = h1 < ch - 1 ? 1 : 0;
     const float h1l = __fsub_rn(h1r, (float)h1);
     const float h0l = __fsub_rn(1.0f, h1l);
     const float w1r = __fmul_rn(rw, (float)x);
     const int w1 = (int)w1r;
-    const int w1p = w1 < W - 1 ? 1 : 0;
+    const int w1p = w1 < cw - 1 ? 1 : 0;
     const float w1l = __fsub_rn(w1r, (float)w1);
     const float w0l = __fsub_rn(1.0f, w1l);
-    const auto q = fetch.quad(f, h1, w1, h1p, w1p);
+    typename Fetch::Quad q;
+    if constexpr (kCrop) {
+      const int y0 = clamp_index(h1, top, H), x0 = clamp_index(w1, left, W);
+      q = fetch.quad(f, y0, x0, clamp_index(h1 + h1p, top, H) - y0, clamp_index(w1 + w1p, left, W) - x0);
+    } else {
+      q = fetch.quad(f, h1, w1, h1p, w1p);
+    }
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const float row0 = __fmaf_rn(w0l, q.at(c, 0), __fmul_rn(w1l, q.at(c, 1)));
@@ -196,20 +231,27 @@ __global__ void __launch_bounds__(kPrepThreads) prepare_frames_kernel(const type
 }
 
 template <class Fetch>
-cudaError_t launch_fetch(const typename Fetch::Src* src, int64_t st, const Fetch& fetch, int T, int H, int W, int oh,
-                         int ow, float* out, cudaStream_t s) {
-  // area_pixel_compute_scale<float>(in, out, align_corners=true): float / int in float
-  const float rh = oh > 1 ? (float)(H - 1) / (oh - 1) : 0.0f;
-  const float rw = ow > 1 ? (float)(W - 1) / (ow - 1) : 0.0f;
-  const int copy = (H == oh && W == ow) ? 1 : 0;
+cudaError_t launch_fetch(const typename Fetch::Src* src, int64_t st, const Fetch& fetch, const Geom& g, float* out,
+                         cudaStream_t s) {
+  // area_pixel_compute_scale<float>(in, out, align_corners=true): float / int in float, in = the window
+  const float rh = g.oh > 1 ? (float)(g.ch - 1) / (g.oh - 1) : 0.0f;
+  const float rw = g.ow > 1 ? (float)(g.cw - 1) / (g.ow - 1) : 0.0f;
+  const int copy = (g.ch == g.oh && g.cw == g.ow) ? 1 : 0;
   const float inv255 = 1.0f / 255.0f;
-  const int64_t plane = (int64_t)oh * ow;
+  const int64_t plane = (int64_t)g.oh * g.ow;
   const unsigned gx = (unsigned)((plane + kPrepThreads - 1) / kPrepThreads);
-  for (int t0 = 0; t0 < T; t0 += kMaxGridY) {
-    const int tc = (T - t0) < kMaxGridY ? (T - t0) : kMaxGridY;
-    prepare_frames_kernel<Fetch><<<dim3(gx, tc), kPrepThreads, 0, s>>>(src + (int64_t)t0 * st, st, fetch, H, W, oh, ow,
-                                                                      rh, rw, copy, inv255,
-                                                                      out + (int64_t)t0 * 3 * plane);
+  for (int t0 = 0; t0 < g.T; t0 += kMaxGridY) {
+    const int tc = (g.T - t0) < kMaxGridY ? (g.T - t0) : kMaxGridY;
+    const dim3 grid(gx, tc);
+    const auto* s0 = src + (int64_t)t0 * st;
+    float* o0 = out + (int64_t)t0 * 3 * plane;
+    if (g.offsets)
+      prepare_frames_kernel<Fetch, true><<<grid, kPrepThreads, 0, s>>>(s0, st, fetch, g.offsets + 2 * (int64_t)t0, g.H,
+                                                                       g.W, g.ch, g.cw, g.oh, g.ow, rh, rw, copy,
+                                                                       inv255, o0);
+    else
+      prepare_frames_kernel<Fetch, false><<<grid, kPrepThreads, 0, s>>>(s0, st, fetch, nullptr, g.H, g.W, g.ch, g.cw,
+                                                                        g.oh, g.ow, rh, rw, copy, inv255, o0);
   }
   return cudaGetLastError();
 }
@@ -217,10 +259,12 @@ cudaError_t launch_fetch(const typename Fetch::Src* src, int64_t st, const Fetch
 }  // namespace
 
 cudaError_t launch_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t st, int64_t sc, int64_t sh,
-                                  int64_t sw, int oh, int ow, float* out, cudaStream_t s) {
+                                  int64_t sw, const int32_t* offsets, int ch, int cw, int oh, int ow, float* out,
+                                  cudaStream_t s) {
+  const Geom g{T, H, W, ch, cw, oh, ow, offsets};
   if (dtype == CT3_FRAMES_U8)
-    return launch_fetch(static_cast<const uint8_t*>(src), st, RgbFetch<uint8_t>{sc, sh, sw}, T, H, W, oh, ow, out, s);
-  return launch_fetch(static_cast<const float*>(src), st, RgbFetch<float>{sc, sh, sw}, T, H, W, oh, ow, out, s);
+    return launch_fetch(static_cast<const uint8_t*>(src), st, RgbFetch<uint8_t>{sc, sh, sw}, g, out, s);
+  return launch_fetch(static_cast<const float*>(src), st, RgbFetch<float>{sc, sh, sw}, g, out, s);
 }
 
 namespace {
@@ -264,43 +308,42 @@ YuvCoeffs yuv_coeffs(const YuvFormat& f, int matrix, int full_range) {
 // everything else the runtime coefficients.
 template <class Read>
 cudaError_t launch_read(const void* src, int64_t st, const Read& read, const YuvFormat& f, int matrix, int full_range,
-                        int T, int H, int W, int oh, int ow, float* out, cudaStream_t s) {
+                        const Geom& g, float* out, cudaStream_t s) {
   using S = typename Read::Src;
   const S* p = static_cast<const S*>(src);
   if constexpr (sizeof(S) == 1) {
     if (matrix == CT3_MATRIX_BT601 && !full_range)
-      return launch_fetch(p, st, YuvFetch<Read, Cv2Bt601>{read, {}}, T, H, W, oh, ow, out, s);
+      return launch_fetch(p, st, YuvFetch<Read, Cv2Bt601>{read, {}}, g, out, s);
   }
-  return launch_fetch(p, st, YuvFetch<Read, YuvCoeffs>{read, yuv_coeffs(f, matrix, full_range)}, T, H, W, oh, ow, out,
-                      s);
+  return launch_fetch(p, st, YuvFetch<Read, YuvCoeffs>{read, yuv_coeffs(f, matrix, full_range)}, g, out, s);
 }
 
 template <typename S>
-cudaError_t launch_family(const void* src, const YuvFormat& f, int matrix, int full_range, int T, int H, int W,
-                          int64_t st, int64_t sr, int oh, int ow, float* out, cudaStream_t s) {
+cudaError_t launch_family(const void* src, const YuvFormat& f, int matrix, int full_range, const Geom& g, int64_t st,
+                          int64_t sr, float* out, cudaStream_t s) {
   st /= (int64_t)sizeof(S), sr /= (int64_t)sizeof(S);   // byte strides -> sample strides (validated multiples)
   if (f.family == YuvFormat::kSemiPlanar)
-    return launch_read(src, st, SemiPlanarRead<S>{sr, (int64_t)H * sr}, f, matrix, full_range, T, H, W, oh, ow, out, s);
+    return launch_read(src, st, SemiPlanarRead<S>{sr, (int64_t)g.H * sr}, f, matrix, full_range, g, out, s);
   if (f.family == YuvFormat::kPlanar) {
-    const int64_t uv = (int64_t)H * W, cplane = (int64_t)(H >> f.ys) * (W >> f.xs);
-    if (f.ys)
-      return launch_read(src, st, PlanarRead<S, 1, 1>{sr, uv, cplane}, f, matrix, full_range, T, H, W, oh, ow, out, s);
-    if (f.xs)
-      return launch_read(src, st, PlanarRead<S, 1, 0>{sr, uv, cplane}, f, matrix, full_range, T, H, W, oh, ow, out, s);
-    return launch_read(src, st, PlanarRead<S, 0, 0>{sr, uv, cplane}, f, matrix, full_range, T, H, W, oh, ow, out, s);
+    const int64_t uv = (int64_t)g.H * g.W, cplane = (int64_t)(g.H >> f.ys) * (g.W >> f.xs);
+    if (f.ys) return launch_read(src, st, PlanarRead<S, 1, 1>{sr, uv, cplane}, f, matrix, full_range, g, out, s);
+    if (f.xs) return launch_read(src, st, PlanarRead<S, 1, 0>{sr, uv, cplane}, f, matrix, full_range, g, out, s);
+    return launch_read(src, st, PlanarRead<S, 0, 0>{sr, uv, cplane}, f, matrix, full_range, g, out, s);
   }
   if constexpr (sizeof(S) == 1)   // YUYV is the only packed layout
-    return launch_read(src, st, PackedRead<S>{sr}, f, matrix, full_range, T, H, W, oh, ow, out, s);
+    return launch_read(src, st, PackedRead<S>{sr}, f, matrix, full_range, g, out, s);
   return cudaErrorInvalidValue;
 }
 
 }  // namespace
 
 cudaError_t launch_prepare_frames_yuv(const void* src, int layout, int matrix, int full_range, int T, int H, int W,
-                                      int64_t st, int64_t sr, int oh, int ow, float* out, cudaStream_t s) {
+                                      int64_t st, int64_t sr, const int32_t* offsets, int ch, int cw, int oh, int ow,
+                                      float* out, cudaStream_t s) {
   const YuvFormat& f = *yuv_format(layout);
-  if (f.bytes == 1) return launch_family<uint8_t>(src, f, matrix, full_range, T, H, W, st, sr, oh, ow, out, s);
-  return launch_family<uint16_t>(src, f, matrix, full_range, T, H, W, st, sr, oh, ow, out, s);
+  const Geom g{T, H, W, ch, cw, oh, ow, offsets};
+  if (f.bytes == 1) return launch_family<uint8_t>(src, f, matrix, full_range, g, st, sr, out, s);
+  return launch_family<uint16_t>(src, f, matrix, full_range, g, st, sr, out, s);
 }
 
 }  // namespace ct3

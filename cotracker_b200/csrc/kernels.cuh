@@ -26,9 +26,12 @@ cudaError_t launch_pyramid_pools(int T, int H4, int W4, float* pyr, cudaStream_t
 
 // ---- ingest.cu : raw frames -> encoder input ------------------------------------------------------
 // src [T,3,H,W] (element strides st, sc, sh, sw; dtype CT3_FRAMES_U8 | CT3_FRAMES_F32) -> out [T,3,oh,ow] fp32 contiguous
-// = 2 * (bilinear(align_corners=True) / 255) - 1, bit-identical to the ATen expression (see ingest.cu)
+// = 2 * (bilinear(align_corners=True) / 255) - 1, bit-identical to the ATen expression (see ingest.cu).  The source is
+// the ch x cw window of each frame whose (top, left) is device offsets[2t], offsets[2t + 1] (sample indices clamped
+// into the frame), or the whole frame when offsets is null (ch = H, cw = W).
 cudaError_t launch_prepare_frames(const void* src, int dtype, int T, int H, int W, int64_t st, int64_t sc, int64_t sh,
-                                  int64_t sw, int oh, int ow, float* out, cudaStream_t s);
+                                  int64_t sw, const int32_t* offsets, int ch, int cw, int oh, int ow, float* out,
+                                  cudaStream_t s);
 // A YUV layout (CT3_YUV_*): its sample size, significant bits, alignment, read family and chroma subsampling.
 struct YuvFormat {
   enum Family { kSemiPlanar, kPlanar, kPacked };
@@ -51,8 +54,10 @@ inline int64_t yuv_rows(const YuvFormat& f, int H) {
 }
 // the same of YUV frames (layout CT3_YUV_*, CT3_MATRIX_*, full_range 0 | 1; frame / row byte strides st, sr), converted
 // to uint8 RGB by the integer formula of ct3_b200.h: bit-identical to launch_prepare_frames on that uint8 RGB clip
+// (chroma read at each pixel's position in the whole frame, whatever the window)
 cudaError_t launch_prepare_frames_yuv(const void* src, int layout, int matrix, int full_range, int T, int H, int W,
-                                      int64_t st, int64_t sr, int oh, int ow, float* out, cudaStream_t s);
+                                      int64_t st, int64_t sr, const int32_t* offsets, int ch, int cw, int oh, int ow,
+                                      float* out, cudaStream_t s);
 
 // ---- finish.cu : the predictor's tail (arguments validated by ct3_finish_tracks) --------------------
 // forward (+ optional backward, reversed-clip time) tracks [B,T,N,2] / visibility probabilities [B,T,N], queries

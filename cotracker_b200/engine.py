@@ -90,6 +90,10 @@ def _signatures():
                                            c_void_p]),
         "ct3_prepare_frames_yuv_fmt": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, i64, i64, c_int, c_int,
                                                c_void_p, c_void_p]),
+        "ct3_prepare_frames_crop": (c_int, [c_void_p, c_int, c_int, c_int, c_int, i64, i64, i64, i64, c_void_p, c_int,
+                                            c_int, c_int, c_int, c_void_p, c_void_p]),
+        "ct3_prepare_frames_yuv_crop": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, i64, i64, c_void_p,
+                                                c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
         "ct3_finish_tracks": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                       ctypes.c_float, ctypes.c_float, ctypes.c_float, c_void_p, c_void_p, c_void_p]),
         "ct3_finish_tracks_scores": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
@@ -315,10 +319,21 @@ def pyramid_pools(pyr: torch.Tensor, T: int, H4: int, W4: int) -> torch.Tensor:
 FRAME_DTYPES = {torch.uint8: 0, torch.float32: 1}   # CT3_FRAMES_U8, CT3_FRAMES_F32
 
 
-def prepare_frames(src: torch.Tensor, out_hw, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+def _window(crop, T: int, device):
+    """crop = (offsets, (h, w)) of a prepare_frames* call -> (offsets, h, w), offsets an int32 [T,2] device tensor."""
+    offsets, (h, w) = crop
+    _req(offsets, torch.int32, "crop offsets")
+    if tuple(offsets.shape) != (T, 2) or offsets.device != device:
+        raise EngineError(f"crop offsets must be [{T},2] (top, left) on {device}, got {tuple(offsets.shape)}")
+    return offsets, int(h), int(w)
+
+
+def prepare_frames(src: torch.Tensor, out_hw, out: Optional[torch.Tensor] = None, *, crop=None) -> torch.Tensor:
     """src [T,3,H,W] uint8 or float32 CUDA tensor with any strides (e.g. a permuted [T,H,W,3] decoder buffer) ->
     [T,3,oh,ow] fp32 = 2 * (bilinear(align_corners=True) resize / 255) - 1, bit-identical to the ATen expression.
-    out: optional contiguous fp32 destination of that shape."""
+    out: optional contiguous fp32 destination of that shape.  crop = (offsets, (h, w)): resize the h x w window of
+    each frame whose (top, left) is row t of offsets (int32 [T,2] on the device; ct3_prepare_frames_crop, which
+    does not check them: the caller does), bit-identical to the call on the materialised windows."""
     if not src.is_cuda:
         raise EngineError("src must be a CUDA tensor (no CPU fallback)")
     if src.dtype not in FRAME_DTYPES:
@@ -332,8 +347,13 @@ def prepare_frames(src: torch.Tensor, out_hw, out: Optional[torch.Tensor] = None
     _req(out, torch.float32, "out")
     if tuple(out.shape) != (T, 3, oh, ow) or out.device != src.device:
         raise EngineError(f"out must be [{T},3,{oh},{ow}] on {src.device}")
-    _call("ct3_prepare_frames", src.device, _ptr(src), FRAME_DTYPES[src.dtype], T, H, W, *src.stride(), oh, ow, _ptr(out),
-          _stream(src.device))
+    head = (_ptr(src), FRAME_DTYPES[src.dtype], T, H, W, *src.stride())
+    tail = (oh, ow, _ptr(out), _stream(src.device))
+    if crop is None:
+        _call("ct3_prepare_frames", src.device, *head, *tail)
+    else:
+        offsets, h, w = _window(crop, T, src.device)
+        _call("ct3_prepare_frames_crop", src.device, *head, _ptr(offsets), h, w, *tail)
     return out
 
 
@@ -380,13 +400,15 @@ def check_yuv_colour(matrix: str, full_range) -> None:
 
 
 def prepare_frames_yuv(src: torch.Tensor, layout: str, out_hw, out: Optional[torch.Tensor] = None, *,
-                       matrix: str = "bt601", full_range: bool = False) -> torch.Tensor:
+                       matrix: str = "bt601", full_range: bool = False, crop=None) -> torch.Tensor:
     """src: T YUV frames on the device, [T,<one frame>] as `yuv_frame_shape(layout)` gives it, uint8 or (p010, p016,
     yuv4xxp10) uint16 -> [T,3,oh,ow] fp32, bit-identical to prepare_frames on the uint8 RGB clip the integer formula of
     include/ct3_b200.h makes of them: with the defaults (BT.601 limited range), the RGB cv2.cvtColor(COLOR_YUV2RGB_*)
     gives.  Any frame stride; semi-planar and yuyv rows at any row stride (pitched surfaces), planar frames dense.
     out: optional contiguous fp32 destination of that shape.  The three original layouts in the default colour call
-    ct3_prepare_frames_yuv, everything else ct3_prepare_frames_yuv_fmt."""
+    ct3_prepare_frames_yuv, everything else ct3_prepare_frames_yuv_fmt.  crop = (offsets, (h, w)) as for
+    prepare_frames (ct3_prepare_frames_yuv_crop): the windows of that RGB clip, chroma read at each pixel's position in
+    the whole frame."""
     if src.dtype not in (torch.uint8, torch.uint16):
         raise EngineError(f"YUV frames must be uint8 or uint16, got {src.dtype}")
     if layout not in YUV_FORMATS:
@@ -417,7 +439,11 @@ def prepare_frames_yuv(src: torch.Tensor, layout: str, out_hw, out: Optional[tor
     if tuple(out.shape) != (T, 3, oh, ow) or out.device != src.device:
         raise EngineError(f"out must be [{T},3,{oh},{ow}] on {src.device}")
     args = (T, H, W, src.stride(0) * es, stride_row * es, oh, ow, _ptr(out), _stream(src.device))
-    if layout in YUV_LAYOUTS and matrix == "bt601" and not full_range:
+    if crop is not None:
+        offsets, h, w = _window(crop, T, src.device)
+        _call("ct3_prepare_frames_yuv_crop", src.device, _ptr(src), YUV_FORMATS[layout], YUV_MATRICES[matrix],
+              int(full_range), *args[:5], _ptr(offsets), h, w, *args[5:])
+    elif layout in YUV_LAYOUTS and matrix == "bt601" and not full_range:
         _call("ct3_prepare_frames_yuv", src.device, _ptr(src), YUV_LAYOUTS[layout], *args)
     else:
         _call("ct3_prepare_frames_yuv_fmt", src.device, _ptr(src), YUV_FORMATS[layout], YUV_MATRICES[matrix],

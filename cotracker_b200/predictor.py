@@ -13,7 +13,8 @@ memory permitting, one update-loop pass for the whole batch; slot b of the resul
 A list of [1,T_b,3,H_b,W_b] clips of any lengths and sizes (offline model, sparse queries) is tracked the same way, with
 per-clip `queries` / `segm_mask` lists; it returns lists, and entry b is bit-identical to the call on clip b alone.
 A clip, or an entry of such a list, may be a `YUVClip` (NV12, I420 or YUYV frames): results are `torch.equal` to the
-call on its RGB conversion by cv2.cvtColor.
+call on its RGB conversion by cv2.cvtColor.  It may also be a `Crop`, a window of each frame of a clip or a YUVClip:
+results are `torch.equal` to the call on the materialised window, in window pixels.
 
 `return_scores=True` (both predictors) adds a third output, `TrackScores(visibility, confidence)`: the model's
 probabilities sigmoid(vis) and sigmoid(conf), fp32 on the device, of the visibility output's shape (a list of them for a
@@ -124,7 +125,8 @@ class CoTrackerPredictor(torch.nn.Module):
 
     @torch.no_grad()
     def encode(self, video) -> "EncodedClip":
-        """video ([B,T,3,H,W] uint8 or float, host or device, any strides, or a `YUVClip`: anything one call takes)
+        """video ([B,T,3,H,W] uint8 or float, host or device, any strides, a `YUVClip` or a `Crop`: anything one call
+        takes)
         -> its `EncodedClip`: resized, normalised and encoded once, on the model's device, for any number of calls."""
         if isinstance(video, (list, tuple, EncodedClip)):
             raise TypeError(f"encode takes one clip [B,T,3,H,W] or a YUVClip, got {type(video).__name__} (list calls "
@@ -318,7 +320,7 @@ def _check_list_call(model, clips, queries, segm_mask, grid_size, grid_query_fra
             raise ValueError(f"{name} must be a list of {B} entries, one per clip")
     for b, c in enumerate(clips):
         ingest.reject_encoded_clip(c, f"entry {b} of a list call")
-        clip = torch.is_tensor(c) or isinstance(c, ingest.YUVClip)
+        clip = torch.is_tensor(c) or isinstance(c, (ingest.YUVClip, ingest.Crop))
         if not clip or c.dim() != 5 or c.shape[0] != 1 or c.shape[1] < 1 or c.shape[2] != 3:
             raise ValueError(f"clip {b} must be a [1,T,3,H,W] tensor, got "
                              f"{tuple(c.shape) if clip else type(c).__name__}")

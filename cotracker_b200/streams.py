@@ -228,7 +228,7 @@ class OnlineStreams:
         return self._get(sid)["state"].length
 
     def push(self, sid: int, chunk: torch.Tensor, preview: bool = False):
-        """Queue the next chunk [1,T,3,H,W] of stream `sid` (T <= window_len), or a `YUVClip` of it, for the next
+        """Queue the next chunk [1,T,3,H,W] of stream `sid` (T <= window_len), or a `YUVClip` or `Crop` of it, for the next
         `step()`.  preview=True: the chunk holds frames [w, f] of the stream, w = max(0, length - (window_len - step))
         the current window start and f > length - 1 the newest frame, of any T allowed; `step()` returns for `sid`
         exactly what it would return for the chunk pushed without the flag (a result ending at frame f) and leaves the

@@ -99,6 +99,12 @@ def _device_for(*tensors) -> torch.device:
     return torch.device("cuda", torch.cuda.current_device())
 
 
+def _reject_crop(video, where: str):
+    """TypeError for a `Crop`: drawing draws on whole frames; draw on the frame with `crop.to_frame(tracks)`."""
+    if isinstance(video, ingest.Crop):
+        raise TypeError(f"{where} draws on whole frames, not a Crop: pass the video and crop.to_frame(tracks)")
+
+
 class Visualizer:
     def __init__(
         self,
@@ -151,6 +157,7 @@ class Visualizer:
         opacity: float = 1.0,
     ):
         ingest.reject_encoded_clip(video, "Visualizer.visualize")
+        _reject_crop(video, "Visualizer.visualize")
         if gt_tracks is not None:
             raise NotImplementedError("gt_tracks is not provided (the reference cannot draw more than one of them)")
         if compensate_for_camera_motion:
@@ -198,6 +205,7 @@ class Visualizer:
     ):
         """video (B,T,3,H,W) as drawn on (already padded), tracks (B,T,N,2) in its pixel coordinates, segm_mask [N]."""
         ingest.reject_encoded_clip(video, "Visualizer.draw_tracks_on_video")
+        _reject_crop(video, "Visualizer.draw_tracks_on_video")
         if gt_tracks is not None:
             raise NotImplementedError("gt_tracks is not provided (the reference cannot draw more than one of them)")
         B, T, C, H, W = video.shape

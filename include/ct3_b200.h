@@ -171,6 +171,26 @@ enum { CT3_MATRIX_BT601 = 0, CT3_MATRIX_BT709 = 1, CT3_MATRIX_BT2020 = 2 };
 int ct3_prepare_frames_yuv_fmt(const void* src, int layout, int matrix, int full_range, int T, int H, int W,
                                int64_t stride_t, int64_t stride_row, int out_h, int out_w, float* out,
                                ct3_stream_t stream);
+/* ct3_prepare_frames_crop, ct3_prepare_frames_yuv_crop: ct3_prepare_frames and ct3_prepare_frames_yuv_fmt on a
+ * crop_h x crop_w window of each frame, which may move from frame to frame.  offsets: a DEVICE array [T,2] of int32
+ * (top, left), the window's top-left corner in frame t.  The output is bit-identical to ct3_prepare_frames on the
+ * materialised window [T,3,crop_h,crop_w] (frame t's rows top..top+crop_h-1, columns left..left+crop_w-1); for YUV, on
+ * that window of the uint8 RGB the integer formula above gives of the whole frame:
+ * - the align_corners=True source coordinates are those of a crop_h x crop_w frame; the offset is added to the integer
+ *   sample indices only, and a window of out_h x out_w is copied as ct3_prepare_frames copies a frame of that size;
+ * - chroma is read at the pixel's absolute position in the frame (its 2x2 block or its horizontal pair), so an odd top
+ *   or left on a 4:2:0 / 4:2:2 layout converts exactly as the whole frame does.
+ * The offsets are not read on the host, so the kernel clamps every sample index into [0,H-1] x [0,W-1]: a window
+ * reaching outside the frame gives unspecified values but never reads outside it.  Callers check the offsets
+ * (0 <= top <= H - crop_h, 0 <= left <= W - crop_w) before the call.  Every argument check of the un-cropped entry
+ * point applies, and a null `offsets`, or crop_h outside [1,H] or crop_w outside [1,W], also return CT3_EINVAL before
+ * any launch. */
+int ct3_prepare_frames_crop(const void* src, int dtype, int T, int H, int W, int64_t stride_t, int64_t stride_c,
+                            int64_t stride_h, int64_t stride_w, const int32_t* offsets, int crop_h, int crop_w,
+                            int out_h, int out_w, float* out, ct3_stream_t stream);
+int ct3_prepare_frames_yuv_crop(const void* src, int layout, int matrix, int full_range, int T, int H, int W,
+                                int64_t stride_t, int64_t stride_row, const int32_t* offsets, int crop_h, int crop_w,
+                                int out_h, int out_w, float* out, ct3_stream_t stream);
 
 /* ---- Shi-Tomasi corners: where to seed new tracks ----------------------------------------------------------------
  * ct3_detect_corners: the corners cv2.goodFeaturesToTrack(gray, max_corners, quality_level, min_distance, mask,
